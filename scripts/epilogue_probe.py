@@ -44,8 +44,8 @@ def case(name, M, N, K, a_mn, b_mn, out_bf16, tf32, splitk):
         C = torch.zeros(M, N, device=dev, dtype=torch.bfloat16 if out_bf16 else torch.float32)
 
         def f():
-            L.gemm_bf16(A.data_ptr(), B.data_ptr(), C.data_ptr(), 0, M, N, K, A.shape[1], B.shape[1], N, int(a_mn), int(b_mn), int(out_bf16),
-                        0, 0, 1.0, 0, splitk, S(), int(tf32))
+            L.gemm(A.data_ptr(), B.data_ptr(), C.data_ptr(), 0, M, N, K, A.shape[1], B.shape[1], N, int(a_mn), int(b_mn), int(out_bf16),
+                   0, 0, 1.0, 0, splitk, int(tf32), S())
         times.append(timeit(f))
         f(); torch.cuda.synchronize()
         outs.append(C.float().clone())

@@ -50,10 +50,10 @@ def conv_case(name, N, H, W, C, O, K, s, p):
     flops = 2.0 * N * Ho * Ho * O * K * K * C
 
     def f():
-        L.conv_fprop(x.data_ptr(), w.data_ptr(), y.data_ptr(), b.data_ptr(), N, H, W, C, 0, C, K, K, Ho, Ho, s, p, O, O, 1, 1, 0, S())
+        L.conv_fprop(x.data_ptr(), w.data_ptr(), y.data_ptr(), b.data_ptr(), N, H, W, C, 0, C, K, K, Ho, Ho, s, p, O, O, 1, 0, 0, S())
 
     def g():
-        L.conv_wgrad(dy.data_ptr(), x.data_ptr(), dw.data_ptr(), N, H, W, C, 0, C, K, K, Ho, Ho, s, p, O, O, S())
+        L.conv_wgrad(dy.data_ptr(), x.data_ptr(), dw.data_ptr(), N, H, W, C, 0, C, K, K, Ho, Ho, s, p, O, O, 0, S())
 
     return [(name + " fprop", f, flops), (name + " wgrad", g, flops)]
 
@@ -64,8 +64,8 @@ def gemm_case(name, M, Nn, K, a_mn, b_mn, out_bf16):
     Cc = torch.empty(M, Nn, device=dev, dtype=BF if out_bf16 else torch.float32)
 
     def f():
-        L.gemm_bf16(A.data_ptr(), B.data_ptr(), Cc.data_ptr(), 0, M, Nn, K, A.shape[1], B.shape[1], Nn, int(a_mn), int(b_mn),
-                    int(out_bf16), 0, 0, 1.0, 0, 0, S())
+        L.gemm(A.data_ptr(), B.data_ptr(), Cc.data_ptr(), 0, M, Nn, K, A.shape[1], B.shape[1], Nn, int(a_mn), int(b_mn),
+               int(out_bf16), 0, 0, 1.0, 0, 0, 0, S())
 
     return [(name, f, 2.0 * M * Nn * K)]
 

@@ -58,67 +58,49 @@ void gemm_rs_add_range(const void* c_lo, const void* c_hi, long long blo, long l
 void gemm_rs_clear();
 int gemm_plan_splits(int tiles, int num_kb, int sms);          // split-K factor the launcher would pick
 int gemm_plan_tall(long long M, int nt, int out_bf16, int sms);   // 1 = 256-row CTA tiles   // bottleneck probe knobs of the wgmma GEMM (see Params::dbg)
-void gemm_bf16(const void* A, const void* B, void* C, const float* bias, int M, int N, int K, long long lda, long long ldb,
-               long long ldc, int a_mn, int b_mn, int out_bf16, int bias_mode, int relu, float alpha, int bn_hint, int splitk,
-               cudaStream_t st, int tf32 = 0);     // tf32 = 1: fp32 operands / fp32 output through wgmma tf32
+// f32 = 1: fp32 operands through wgmma tf32 (fp32 output), else bf16 operands
+void gemm(const void* A, const void* B, void* C, const float* bias, int M, int N, int K, long long lda, long long ldb, long long ldc,
+          int a_mn, int b_mn, int out_bf16, int bias_mode, int relu, float alpha, int bn_hint, int splitk, int f32, cudaStream_t st);
 
-void conv_fprop_bf16(const void* x, const void* w, void* y, const float* bias, int N, int H, int W, int Ctot, int c_off, int Cg, int KH,
-                     int KW, int Ho, int Wo, int S, int P, int O, long long ldc, int relu, int out_bf16, int dgrad, cudaStream_t st, int tf32 = 0);
-void conv_wgrad_bf16(const void* dy, const void* x, void* dw, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho,
-                     int Wo, int S, int P, int O, long long ldy, cudaStream_t st, int tf32 = 0);
+void conv_fprop(const void* x, const void* w, void* y, const float* bias, int N, int H, int W, int Ctot, int c_off, int Cg, int KH,
+                int KW, int Ho, int Wo, int S, int P, int O, long long ldc, int relu, int dgrad, int f32, cudaStream_t st);
+void conv_wgrad(const void* dy, const void* x, void* dw, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho,
+                int Wo, int S, int P, int O, long long ldy, int f32, cudaStream_t st);
 // both groups of a 2-group convolution in one persistent launch (see gemm_wgmma.cu)
-void conv_fprop2_bf16(const void* x, const void* w0, const void* w1, void* y0, void* y1, const float* bias0, const float* bias1, int N, int H,
-                      int W, int Ctot, int c_off0, int c_off1, int Cg, int KH, int KW, int Ho, int Wo, int S, int P, int O, long long ldc,
-                      int relu, int out_bf16, int dgrad, cudaStream_t st, int tf32 = 0);
-void conv_wgrad2_bf16(const void* dy0, const void* dy1, const void* x, void* dw0, void* dw1, int N, int H, int W, int Ctot, int c_off0,
-                      int c_off1, int Cg, int KH, int KW, int Ho, int Wo, int S, int P, int O, long long ldy, cudaStream_t st, int tf32 = 0);
+void conv_fprop2(const void* x, const void* w0, const void* w1, void* y0, void* y1, const float* bias0, const float* bias1, int N, int H,
+                 int W, int Ctot, int c_off0, int c_off1, int Cg, int KH, int KW, int Ho, int Wo, int S, int P, int O, long long ldc,
+                 int relu, int dgrad, int f32, cudaStream_t st);
+void conv_wgrad2(const void* dy0, const void* dy1, const void* x, void* dw0, void* dw1, int N, int H, int W, int Ctot, int c_off0,
+                 int c_off1, int Cg, int KH, int KW, int Ho, int Wo, int S, int P, int O, long long ldy, int f32, cudaStream_t st);
 
-// ---- nn_kernels.cu
-void space_to_depth(const void* x, void* y, int N, int H, int W, int C, int S, int Hs, int Ws, int Cp, int P, cudaStream_t st);
-void s2d_filter(const void* src, void* dst, int O, int KH, int KW, int C, int S, int KHs, int KWs, int Cp, int dir, cudaStream_t st);
-void conv_weight_flip(const void* w, void* wt, int O, int KH, int KW, int Cg, cudaStream_t st);
-void lrn_fwd(const void* x, void* y, long long rows, int C, int n, float k, float alpha, float beta, cudaStream_t st);
-void lrn_bwd(const void* x, const void* dy, void* dx, long long rows, int C, int n, float k, float alpha, float beta, cudaStream_t st);
-void pool_fwd(const void* x, void* y, void* arg, int N, int H, int W, int C, int Ho, int Wo, int k, int s, int p, int is_max, cudaStream_t st);
-void pool_bwd(const void* dy, const void* arg, void* dx, int N, int H, int W, int C, int Ho, int Wo, int k, int s, int p, int is_max, cudaStream_t st);
-void dropout_fwd(const void* x, void* y, void* mask, long long n, float p_drop, unsigned long long seed, int layer, const void* step, cudaStream_t st);
-void dropout_bwd(const void* dy, const void* mask, void* dx, long long n, cudaStream_t st);
+// ---- nn_kernels.cu  (f32: fp32 activations, C % 4 == 0; else bf16, C % 8 == 0)
+void space_to_depth(const void* x, void* y, int N, int H, int W, int C, int S, int Hs, int Ws, int Cp, int P, int f32, cudaStream_t st);
+void s2d_filter(const void* src, void* dst, int O, int KH, int KW, int C, int S, int KHs, int KWs, int Cp, int dir, int f32, cudaStream_t st);
+void lrn_fwd(const void* x, void* y, long long rows, int C, int n, float k, float alpha, float beta, int f32, cudaStream_t st);
+void lrn_bwd(const void* x, const void* dy, void* dx, long long rows, int C, int n, float k, float alpha, float beta, int f32, cudaStream_t st);
+void pool_fwd(const void* x, void* y, void* arg, int N, int H, int W, int C, int Ho, int Wo, int k, int s, int p, int is_max, int f32,
+              cudaStream_t st);
+void pool_bwd(const void* dy, const void* arg, void* dx, int N, int H, int W, int C, int Ho, int Wo, int k, int s, int p, int is_max, int f32,
+              cudaStream_t st);
+void dropout_fwd(const void* x, void* y, void* mask, long long n, float p_drop, unsigned long long seed, int layer, const void* step, int f32,
+                 cudaStream_t st);
+void dropout_bwd(const void* dy, const void* mask, void* dx, long long n, int f32, cudaStream_t st);
 void advance_step(void* step, cudaStream_t st);
-void softmax_xent(const void* logits, const void* labels, void* dlogits, void* rowstat, void* out3, int B, int C, float weight, cudaStream_t st);
-void relu_bias_bwd(const void* dy, const void* y, void* dym, void* db, long long R, int C, long long ld, int relu, cudaStream_t st);
-void relu_bias_bwd2(const void* dy, const void* y, void* dym, void* db, void* db1, int c_split, long long R, int C, long long ld, int relu,
-                    cudaStream_t st);
+void softmax_xent(const void* logits, const void* labels, void* dlogits, void* rowstat, void* out3, int B, int C, float weight, int f32,
+                  cudaStream_t st);
+void relu_bias_bwd(const void* dy, const void* y, void* dym, void* db, void* db1, int c_split, long long R, int C, long long ld, int relu,
+                   int f32, cudaStream_t st);
+void bias_act(const void* acc, const void* bias, void* y, int R, int C, int relu, int f32, cudaStream_t st);
+// bf16 only (packed-bf16 compares)
 void maxpool_relu_bias_bwd(const void* dyp, const void* arg, const void* y, void* dym, void* db0, void* db1, int c_split, int N, int H,
                            int W, int C, int Ho, int Wo, int k, int s, int p, cudaStream_t st);
 void im2col(const void* x, void* col, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho, int Wo, int s, int p,
-            long long ldcol, cudaStream_t st);
+            long long ldcol, int f32, cudaStream_t st);
 void col2im(const void* dcol, void* dx, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho, int Wo, int s, int p,
-            long long ldcol, cudaStream_t st);
-void pad_rows(const void* src, void* dst, long long rows, int cols, long long src_ld, long long dst_ld, cudaStream_t st);
-void transpose_bf16(const void* src, void* dst, int R, int C, cudaStream_t st);
+            long long ldcol, int f32, cudaStream_t st);
+void pad_rows(const void* src, void* dst, long long rows, int cols, long long src_ld, long long dst_ld, int f32, cudaStream_t st);
 void crop_mirror_norm(const void* x, int in_kind, const void* mean, int mean_mode, float scale, const void* cscale, void* out, int out_bf16, const void* offs,
                       const void* flips, int N, int H, int W, int C, int ch, int cw, int Cout, cudaStream_t st);
-
-// ---- nn_kernels_f32.cu: fp32-storage variants for the tf32 precision mode (same semantics, C % 4 == 0)
-void lrn_fwd_f32(const void* x, void* y, long long rows, int C, int n, float k, float alpha, float beta, cudaStream_t st);
-void lrn_bwd_f32(const void* x, const void* dy, void* dx, long long rows, int C, int n, float k, float alpha, float beta, cudaStream_t st);
-void pool_fwd_f32(const void* x, void* y, void* arg, int N, int H, int W, int C, int Ho, int Wo, int k, int s, int p, int is_max, cudaStream_t st);
-void pool_bwd_f32(const void* dy, const void* arg, void* dx, int N, int H, int W, int C, int Ho, int Wo, int k, int s, int p, int is_max,
-                  cudaStream_t st);
-void dropout_fwd_f32(const void* x, void* y, void* mask, long long n, float p_drop, unsigned long long seed, int layer, const void* step,
-                     cudaStream_t st);
-void dropout_bwd_f32(const void* dy, const void* mask, void* dx, long long n, cudaStream_t st);
-void softmax_xent_f32(const void* logits, const void* labels, void* dlogits, void* rowstat, void* out3, int B, int C, float weight, cudaStream_t st);
-void relu_bias_bwd2_f32(const void* dy, const void* y, void* dym, void* db, void* db1, int c_split, long long R, int C, long long ld, int relu,
-                        cudaStream_t st);
-void bias_act_f32(const void* acc, const void* bias, void* y, int R, int C, int relu, cudaStream_t st);
-void im2col_f32(const void* x, void* col, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho, int Wo, int s, int p,
-                long long ldcol, cudaStream_t st);
-void col2im_f32(const void* dcol, void* dx, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho, int Wo, int s, int p,
-                long long ldcol, cudaStream_t st);
-void pad_rows_f32(const void* src, void* dst, long long rows, int cols, long long src_ld, long long dst_ld, cudaStream_t st);
-void space_to_depth_f32(const void* x, void* y, int N, int H, int W, int C, int S, int Hs, int Ws, int Cp, int P, cudaStream_t st);
-void s2d_filter_pack_f32(const void* src, void* dst, int O, int KH, int KW, int C, int S, int KHs, int KWs, int Cp, cudaStream_t st);
 
 // ---- bn_kernels.cu: batch norm (+ residual)(+ ReLU) forward / backward, residual add  (f32: fp32 activations, else bf16)
 void bn_forward(const void* x, const void* res, void* y, const void* gamma, const void* beta, void* mean, void* rstd, void* run_mean,
@@ -158,7 +140,6 @@ void gosgd_push(const CommCtx& c, void* state, int dest, long long w_off, long l
 void gosgd_poll_merge(const CommCtx& c, void* state, long long w_off, long long h_off, long long snap_off, long long n, int max_blocks,
                       cudaStream_t st);
 void gosgd_merge(void* w, void* h, const void* b, float a_self, float a_src, long long n, int max_blocks, cudaStream_t st);
-void bias_act_cast(const void* acc, const void* bias, void* y, int R, int C, int relu, cudaStream_t st);
 void cast_flat(const void* src, void* dst, long long n, int kind, cudaStream_t st);
 void sum_chunks(const void* src, void* dst, long long chunk, int nchunks, int is_half, cudaStream_t st);
 void vecadd(void* cur, const void* tmp, long long n, int is_half, cudaStream_t st);

@@ -17,7 +17,6 @@ typedef uintptr_t ptr_t;
 
 static inline void* P(ptr_t p) { return reinterpret_cast<void*>(p); }
 static inline cudaStream_t S(ptr_t s) { return reinterpret_cast<cudaStream_t>(s); }
-static inline cudaStream_t S_(ptr_t s) { return reinterpret_cast<cudaStream_t>(s); }
 
 static GroupTable make_table(const std::vector<float>& lr_mult, const std::vector<float>& wd, const std::vector<int>& exch) {
   GroupTable t;
@@ -53,108 +52,64 @@ PYBIND11_MODULE(_tmpi_native, m) {
   m.def("gemm_rs_clear", &gemm_rs_clear);
   m.def("gemm_plan_splits", &gemm_plan_splits);
   m.def("gemm_plan_tall", &gemm_plan_tall);
-  m.def("gemm_bf16", [](ptr_t A, ptr_t B, ptr_t C, ptr_t bias, int M, int N, int K, long long lda, long long ldb, long long ldc,
-                        int a_mn, int b_mn, int out_bf16, int bias_mode, int relu, float alpha, int bn_hint, int splitk, ptr_t st, int tf32) {
-    gemm_bf16(P(A), P(B), P(C), (const float*)P(bias), M, N, K, lda, ldb, ldc, a_mn, b_mn, out_bf16, bias_mode, relu, alpha, bn_hint,
-              splitk, S(st), tf32);
+  m.def("gemm", [](ptr_t A, ptr_t B, ptr_t C, ptr_t bias, int M, int N, int K, long long lda, long long ldb, long long ldc, int a_mn, int b_mn,
+                   int out_bf16, int bias_mode, int relu, float alpha, int bn_hint, int splitk, int f32, ptr_t st) {
+    gemm(P(A), P(B), P(C), (const float*)P(bias), M, N, K, lda, ldb, ldc, a_mn, b_mn, out_bf16, bias_mode, relu, alpha, bn_hint, splitk, f32,
+         S(st));
   }, py::arg("A"), py::arg("B"), py::arg("C"), py::arg("bias"), py::arg("M"), py::arg("N"), py::arg("K"), py::arg("lda"), py::arg("ldb"),
      py::arg("ldc"), py::arg("a_mn"), py::arg("b_mn"), py::arg("out_bf16"), py::arg("bias_mode"), py::arg("relu"), py::arg("alpha"),
-     py::arg("bn_hint"), py::arg("splitk"), py::arg("st"), py::arg("tf32") = 0);
+     py::arg("bn_hint"), py::arg("splitk"), py::arg("f32"), py::arg("st"));
 
+  // convolution strides are named Sd (S is the stream cast)
   m.def("conv_fprop", [](ptr_t x, ptr_t w, ptr_t y, ptr_t bias, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho, int Wo,
-                         int S, int Pd, int O, long long ldc, int relu, int out_bf16, int dgrad, ptr_t st, int tf32) {
-    conv_fprop_bf16(P(x), P(w), P(y), (const float*)P(bias), N, H, W, Ctot, c_off, Cg, KH, KW, Ho, Wo, S, Pd, O, ldc, relu, out_bf16, dgrad,
-                    S_(st), tf32);
-  }, py::arg("x"), py::arg("w"), py::arg("y"), py::arg("bias"), py::arg("N"), py::arg("H"), py::arg("W"), py::arg("Ctot"), py::arg("c_off"),
-     py::arg("Cg"), py::arg("KH"), py::arg("KW"), py::arg("Ho"), py::arg("Wo"), py::arg("S"), py::arg("P"), py::arg("O"), py::arg("ldc"),
-     py::arg("relu"), py::arg("out_bf16"), py::arg("dgrad"), py::arg("st"), py::arg("tf32") = 0);
-  m.def("conv_wgrad", [](ptr_t dy, ptr_t x, ptr_t dw, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho, int Wo, int S,
-                         int Pd, int O, long long ldy, ptr_t st, int tf32) {
-    conv_wgrad_bf16(P(dy), P(x), P(dw), N, H, W, Ctot, c_off, Cg, KH, KW, Ho, Wo, S, Pd, O, ldy, S_(st), tf32);
-  }, py::arg("dy"), py::arg("x"), py::arg("dw"), py::arg("N"), py::arg("H"), py::arg("W"), py::arg("Ctot"), py::arg("c_off"), py::arg("Cg"),
-     py::arg("KH"), py::arg("KW"), py::arg("Ho"), py::arg("Wo"), py::arg("S"), py::arg("P"), py::arg("O"), py::arg("ldy"), py::arg("st"),
-     py::arg("tf32") = 0);
+                         int Sd, int Pd, int O, long long ldc, int relu, int dgrad, int f32, ptr_t st) {
+    conv_fprop(P(x), P(w), P(y), (const float*)P(bias), N, H, W, Ctot, c_off, Cg, KH, KW, Ho, Wo, Sd, Pd, O, ldc, relu, dgrad, f32, S(st)); });
+  m.def("conv_wgrad", [](ptr_t dy, ptr_t x, ptr_t dw, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho, int Wo, int Sd,
+                         int Pd, int O, long long ldy, int f32, ptr_t st) {
+    conv_wgrad(P(dy), P(x), P(dw), N, H, W, Ctot, c_off, Cg, KH, KW, Ho, Wo, Sd, Pd, O, ldy, f32, S(st)); });
   m.def("conv_fprop2", [](ptr_t x, ptr_t w0, ptr_t w1, ptr_t y0, ptr_t y1, ptr_t b0, ptr_t b1, int N, int H, int W, int Ctot, int c_off0, int c_off1,
-                          int Cg, int KH, int KW, int Ho, int Wo, int S, int Pd, int O, long long ldc, int relu, int out_bf16, int dgrad, ptr_t st,
-                          int tf32) {
-    conv_fprop2_bf16(P(x), P(w0), P(w1), P(y0), P(y1), (const float*)P(b0), (const float*)P(b1), N, H, W, Ctot, c_off0, c_off1, Cg, KH, KW, Ho,
-                     Wo, S, Pd, O, ldc, relu, out_bf16, dgrad, S_(st), tf32);
-  }, py::arg("x"), py::arg("w0"), py::arg("w1"), py::arg("y0"), py::arg("y1"), py::arg("b0"), py::arg("b1"), py::arg("N"), py::arg("H"),
-     py::arg("W"), py::arg("Ctot"), py::arg("c_off0"), py::arg("c_off1"), py::arg("Cg"), py::arg("KH"), py::arg("KW"), py::arg("Ho"),
-     py::arg("Wo"), py::arg("S"), py::arg("P"), py::arg("O"), py::arg("ldc"), py::arg("relu"), py::arg("out_bf16"), py::arg("dgrad"),
-     py::arg("st"), py::arg("tf32") = 0);
+                          int Cg, int KH, int KW, int Ho, int Wo, int Sd, int Pd, int O, long long ldc, int relu, int dgrad, int f32, ptr_t st) {
+    conv_fprop2(P(x), P(w0), P(w1), P(y0), P(y1), (const float*)P(b0), (const float*)P(b1), N, H, W, Ctot, c_off0, c_off1, Cg, KH, KW, Ho, Wo,
+                Sd, Pd, O, ldc, relu, dgrad, f32, S(st)); });
   m.def("conv_wgrad2", [](ptr_t dy0, ptr_t dy1, ptr_t x, ptr_t dw0, ptr_t dw1, int N, int H, int W, int Ctot, int c_off0, int c_off1, int Cg,
-                          int KH, int KW, int Ho, int Wo, int S, int Pd, int O, long long ldy, ptr_t st, int tf32) {
-    conv_wgrad2_bf16(P(dy0), P(dy1), P(x), P(dw0), P(dw1), N, H, W, Ctot, c_off0, c_off1, Cg, KH, KW, Ho, Wo, S, Pd, O, ldy, S_(st), tf32);
-  }, py::arg("dy0"), py::arg("dy1"), py::arg("x"), py::arg("dw0"), py::arg("dw1"), py::arg("N"), py::arg("H"), py::arg("W"), py::arg("Ctot"),
-     py::arg("c_off0"), py::arg("c_off1"), py::arg("Cg"), py::arg("KH"), py::arg("KW"), py::arg("Ho"), py::arg("Wo"), py::arg("S"),
-     py::arg("P"), py::arg("O"), py::arg("ldy"), py::arg("st"), py::arg("tf32") = 0);
-  m.def("space_to_depth", [](ptr_t x, ptr_t y, int N, int H, int W, int C, int S, int Hs, int Ws, int Cp, int Pd, ptr_t st) {
-    space_to_depth(P(x), P(y), N, H, W, C, S, Hs, Ws, Cp, Pd, S_(st)); });
-  m.def("s2d_filter", [](ptr_t src, ptr_t dst, int O, int KH, int KW, int C, int S, int KHs, int KWs, int Cp, int dir, ptr_t st) {
-    s2d_filter(P(src), P(dst), O, KH, KW, C, S, KHs, KWs, Cp, dir, S_(st)); });
-  m.def("conv_weight_flip", [](ptr_t w, ptr_t wt, int O, int KH, int KW, int Cg, ptr_t st) { conv_weight_flip(P(w), P(wt), O, KH, KW, Cg, S_(st)); });
+                          int KH, int KW, int Ho, int Wo, int Sd, int Pd, int O, long long ldy, int f32, ptr_t st) {
+    conv_wgrad2(P(dy0), P(dy1), P(x), P(dw0), P(dw1), N, H, W, Ctot, c_off0, c_off1, Cg, KH, KW, Ho, Wo, Sd, Pd, O, ldy, f32, S(st)); });
+  m.def("space_to_depth", [](ptr_t x, ptr_t y, int N, int H, int W, int C, int Sd, int Hs, int Ws, int Cp, int Pd, int f32, ptr_t st) {
+    space_to_depth(P(x), P(y), N, H, W, C, Sd, Hs, Ws, Cp, Pd, f32, S(st)); });
+  m.def("s2d_filter", [](ptr_t src, ptr_t dst, int O, int KH, int KW, int C, int Sd, int KHs, int KWs, int Cp, int dir, int f32, ptr_t st) {
+    s2d_filter(P(src), P(dst), O, KH, KW, C, Sd, KHs, KWs, Cp, dir, f32, S(st)); });
 
-  // ---------------------------------------------------------------- layer kernels
-  m.def("lrn_fwd", [](ptr_t x, ptr_t y, long long rows, int C, int n, float k, float alpha, float beta, ptr_t st) {
-    lrn_fwd(P(x), P(y), rows, C, n, k, alpha, beta, S(st)); });
-  m.def("lrn_bwd", [](ptr_t x, ptr_t dy, ptr_t dx, long long rows, int C, int n, float k, float alpha, float beta, ptr_t st) {
-    lrn_bwd(P(x), P(dy), P(dx), rows, C, n, k, alpha, beta, S(st)); });
-  m.def("pool_fwd", [](ptr_t x, ptr_t y, ptr_t arg, int N, int H, int W, int C, int Ho, int Wo, int k, int s, int p, int is_max, ptr_t st) {
-    pool_fwd(P(x), P(y), P(arg), N, H, W, C, Ho, Wo, k, s, p, is_max, S(st)); });
-  m.def("pool_bwd", [](ptr_t dy, ptr_t arg, ptr_t dx, int N, int H, int W, int C, int Ho, int Wo, int k, int s, int p, int is_max, ptr_t st) {
-    pool_bwd(P(dy), P(arg), P(dx), N, H, W, C, Ho, Wo, k, s, p, is_max, S(st)); });
-  m.def("dropout_fwd", [](ptr_t x, ptr_t y, ptr_t mask, long long n, float p, unsigned long long seed, int layer, ptr_t step, ptr_t st) {
-    dropout_fwd(P(x), P(y), P(mask), n, p, seed, layer, P(step), S(st)); });
-  m.def("dropout_bwd", [](ptr_t dy, ptr_t mask, ptr_t dx, long long n, ptr_t st) { dropout_bwd(P(dy), P(mask), P(dx), n, S(st)); });
+  // ---------------------------------------------------------------- layer kernels (f32: fp32 activations, else bf16)
+  m.def("lrn_fwd", [](ptr_t x, ptr_t y, long long rows, int C, int n, float k, float alpha, float beta, int f32, ptr_t st) {
+    lrn_fwd(P(x), P(y), rows, C, n, k, alpha, beta, f32, S(st)); });
+  m.def("lrn_bwd", [](ptr_t x, ptr_t dy, ptr_t dx, long long rows, int C, int n, float k, float alpha, float beta, int f32, ptr_t st) {
+    lrn_bwd(P(x), P(dy), P(dx), rows, C, n, k, alpha, beta, f32, S(st)); });
+  m.def("pool_fwd", [](ptr_t x, ptr_t y, ptr_t arg, int N, int H, int W, int C, int Ho, int Wo, int k, int s, int p, int is_max, int f32, ptr_t st) {
+    pool_fwd(P(x), P(y), P(arg), N, H, W, C, Ho, Wo, k, s, p, is_max, f32, S(st)); });
+  m.def("pool_bwd", [](ptr_t dy, ptr_t arg, ptr_t dx, int N, int H, int W, int C, int Ho, int Wo, int k, int s, int p, int is_max, int f32, ptr_t st) {
+    pool_bwd(P(dy), P(arg), P(dx), N, H, W, C, Ho, Wo, k, s, p, is_max, f32, S(st)); });
+  m.def("dropout_fwd", [](ptr_t x, ptr_t y, ptr_t mask, long long n, float p, unsigned long long seed, int layer, ptr_t step, int f32, ptr_t st) {
+    dropout_fwd(P(x), P(y), P(mask), n, p, seed, layer, P(step), f32, S(st)); });
+  m.def("dropout_bwd", [](ptr_t dy, ptr_t mask, ptr_t dx, long long n, int f32, ptr_t st) { dropout_bwd(P(dy), P(mask), P(dx), n, f32, S(st)); });
   m.def("advance_step", [](ptr_t step, ptr_t st) { advance_step(P(step), S(st)); });
-  m.def("softmax_xent", [](ptr_t logits, ptr_t labels, ptr_t dlogits, ptr_t rowstat, ptr_t out3, int B, int C, float weight, ptr_t st) {
-    softmax_xent(P(logits), P(labels), P(dlogits), P(rowstat), P(out3), B, C, weight, S(st)); });
+  m.def("softmax_xent", [](ptr_t logits, ptr_t labels, ptr_t dlogits, ptr_t rowstat, ptr_t out3, int B, int C, float weight, int f32, ptr_t st) {
+    softmax_xent(P(logits), P(labels), P(dlogits), P(rowstat), P(out3), B, C, weight, f32, S(st)); });
   m.def("maxpool_relu_bias_bwd", [](ptr_t dyp, ptr_t arg, ptr_t y, ptr_t dym, ptr_t db0, ptr_t db1, int c_split, int N, int H, int W, int C,
                                     int Ho, int Wo, int k, int s, int p, ptr_t st) {
     maxpool_relu_bias_bwd(P(dyp), P(arg), P(y), P(dym), P(db0), P(db1), c_split, N, H, W, C, Ho, Wo, k, s, p, S(st)); });
-  m.def("relu_bias_bwd2", [](ptr_t dy, ptr_t y, ptr_t dym, ptr_t db, ptr_t db1, int c_split, long long R, int C, long long ld, int relu, ptr_t st) {
-    relu_bias_bwd2(P(dy), P(y), P(dym), P(db), P(db1), c_split, R, C, ld, relu, S(st)); });
-  m.def("relu_bias_bwd", [](ptr_t dy, ptr_t y, ptr_t dym, ptr_t db, long long R, int C, long long ld, int relu, ptr_t st) {
-    relu_bias_bwd(P(dy), P(y), P(dym), P(db), R, C, ld, relu, S(st)); });
+  m.def("relu_bias_bwd", [](ptr_t dy, ptr_t y, ptr_t dym, ptr_t db, ptr_t db1, int c_split, long long R, int C, long long ld, int relu, int f32,
+                            ptr_t st) { relu_bias_bwd(P(dy), P(y), P(dym), P(db), P(db1), c_split, R, C, ld, relu, f32, S(st)); });
+  m.def("bias_act", [](ptr_t acc, ptr_t bias, ptr_t y, int R, int C, int relu, int f32, ptr_t st) {
+    bias_act(P(acc), P(bias), P(y), R, C, relu, f32, S(st)); });
   m.def("im2col", [](ptr_t x, ptr_t col, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho, int Wo, int s, int p,
-                     long long ldcol, ptr_t st) { im2col(P(x), P(col), N, H, W, Ctot, c_off, Cg, KH, KW, Ho, Wo, s, p, ldcol, S(st)); });
+                     long long ldcol, int f32, ptr_t st) { im2col(P(x), P(col), N, H, W, Ctot, c_off, Cg, KH, KW, Ho, Wo, s, p, ldcol, f32, S(st)); });
   m.def("col2im", [](ptr_t dcol, ptr_t dx, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho, int Wo, int s, int p,
-                     long long ldcol, ptr_t st) { col2im(P(dcol), P(dx), N, H, W, Ctot, c_off, Cg, KH, KW, Ho, Wo, s, p, ldcol, S(st)); });
-  m.def("pad_rows", [](ptr_t src, ptr_t dst, long long rows, int cols, long long src_ld, long long dst_ld, ptr_t st) {
-    pad_rows(P(src), P(dst), rows, cols, src_ld, dst_ld, S(st)); });
-  m.def("transpose_bf16", [](ptr_t src, ptr_t dst, int R, int C, ptr_t st) { transpose_bf16(P(src), P(dst), R, C, S(st)); });
+                     long long ldcol, int f32, ptr_t st) { col2im(P(dcol), P(dx), N, H, W, Ctot, c_off, Cg, KH, KW, Ho, Wo, s, p, ldcol, f32, S(st)); });
+  m.def("pad_rows", [](ptr_t src, ptr_t dst, long long rows, int cols, long long src_ld, long long dst_ld, int f32, ptr_t st) {
+    pad_rows(P(src), P(dst), rows, cols, src_ld, dst_ld, f32, S(st)); });
   m.def("crop_mirror_norm", [](ptr_t x, int in_kind, ptr_t mean, int mean_mode, float scale, ptr_t cscale, ptr_t out, int out_bf16, ptr_t offs,
                                ptr_t flips, int N, int H, int W, int C, int ch, int cw, int Cout, ptr_t st) {
     crop_mirror_norm(P(x), in_kind, P(mean), mean_mode, scale, P(cscale), P(out), out_bf16, P(offs), P(flips), N, H, W, C, ch, cw, Cout, S(st)); });
-
-  // ---------------------------------------------------------------- fp32-storage layer kernels (tf32 precision mode)
-  m.def("lrn_fwd_f32", [](ptr_t x, ptr_t y, long long rows, int C, int n, float k, float alpha, float beta, ptr_t st) {
-    lrn_fwd_f32(P(x), P(y), rows, C, n, k, alpha, beta, S(st)); });
-  m.def("lrn_bwd_f32", [](ptr_t x, ptr_t dy, ptr_t dx, long long rows, int C, int n, float k, float alpha, float beta, ptr_t st) {
-    lrn_bwd_f32(P(x), P(dy), P(dx), rows, C, n, k, alpha, beta, S(st)); });
-  m.def("pool_fwd_f32", [](ptr_t x, ptr_t y, ptr_t arg, int N, int H, int W, int C, int Ho, int Wo, int k, int s, int p, int is_max, ptr_t st) {
-    pool_fwd_f32(P(x), P(y), P(arg), N, H, W, C, Ho, Wo, k, s, p, is_max, S(st)); });
-  m.def("pool_bwd_f32", [](ptr_t dy, ptr_t arg, ptr_t dx, int N, int H, int W, int C, int Ho, int Wo, int k, int s, int p, int is_max, ptr_t st) {
-    pool_bwd_f32(P(dy), P(arg), P(dx), N, H, W, C, Ho, Wo, k, s, p, is_max, S(st)); });
-  m.def("dropout_fwd_f32", [](ptr_t x, ptr_t y, ptr_t mask, long long n, float p, unsigned long long seed, int layer, ptr_t step, ptr_t st) {
-    dropout_fwd_f32(P(x), P(y), P(mask), n, p, seed, layer, P(step), S(st)); });
-  m.def("dropout_bwd_f32", [](ptr_t dy, ptr_t mask, ptr_t dx, long long n, ptr_t st) { dropout_bwd_f32(P(dy), P(mask), P(dx), n, S(st)); });
-  m.def("softmax_xent_f32", [](ptr_t logits, ptr_t labels, ptr_t dlogits, ptr_t rowstat, ptr_t out3, int B, int C, float weight, ptr_t st) {
-    softmax_xent_f32(P(logits), P(labels), P(dlogits), P(rowstat), P(out3), B, C, weight, S(st)); });
-  m.def("relu_bias_bwd2_f32", [](ptr_t dy, ptr_t y, ptr_t dym, ptr_t db, ptr_t db1, int c_split, long long R, int C, long long ld, int relu, ptr_t st) {
-    relu_bias_bwd2_f32(P(dy), P(y), P(dym), P(db), P(db1), c_split, R, C, ld, relu, S(st)); });
-  m.def("bias_act_f32", [](ptr_t acc, ptr_t bias, ptr_t y, int R, int C, int relu, ptr_t st) { bias_act_f32(P(acc), P(bias), P(y), R, C, relu, S(st)); });
-  m.def("im2col_f32", [](ptr_t x, ptr_t col, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho, int Wo, int s, int p,
-                         long long ldcol, ptr_t st) { im2col_f32(P(x), P(col), N, H, W, Ctot, c_off, Cg, KH, KW, Ho, Wo, s, p, ldcol, S(st)); });
-  m.def("col2im_f32", [](ptr_t dcol, ptr_t dx, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho, int Wo, int s, int p,
-                         long long ldcol, ptr_t st) { col2im_f32(P(dcol), P(dx), N, H, W, Ctot, c_off, Cg, KH, KW, Ho, Wo, s, p, ldcol, S(st)); });
-  m.def("pad_rows_f32", [](ptr_t src, ptr_t dst, long long rows, int cols, long long src_ld, long long dst_ld, ptr_t st) {
-    pad_rows_f32(P(src), P(dst), rows, cols, src_ld, dst_ld, S(st)); });
-  m.def("space_to_depth_f32", [](ptr_t x, ptr_t y, int N, int H, int W, int C, int S, int Hs, int Ws, int Cp, int Pd, ptr_t st) {
-    space_to_depth_f32(P(x), P(y), N, H, W, C, S, Hs, Ws, Cp, Pd, S_(st)); });
-  m.def("s2d_filter_pack_f32", [](ptr_t src, ptr_t dst, int O, int KH, int KW, int C, int S, int KHs, int KWs, int Cp, ptr_t st) {
-    s2d_filter_pack_f32(P(src), P(dst), O, KH, KW, C, S, KHs, KWs, Cp, S_(st)); });
 
   // ---------------------------------------------------------------- batch norm / residual
   m.def("bn_forward", [](ptr_t x, ptr_t res, ptr_t y, ptr_t gamma, ptr_t beta, ptr_t mean, ptr_t rstd, ptr_t run_mean, ptr_t run_var, ptr_t scratch,
@@ -195,7 +150,6 @@ PYBIND11_MODULE(_tmpi_native, m) {
     copy_flat(P(dst), P(dst_h), P(src), n, max_blocks, nullptr, S(st)); });
   m.def("gosgd_merge", [](ptr_t w, ptr_t h, ptr_t b, float a_self, float a_src, long long n, int max_blocks, ptr_t st) {
     gosgd_merge(P(w), P(h), P(b), a_self, a_src, n, max_blocks, S(st)); });
-  m.def("bias_act_cast", [](ptr_t acc, ptr_t bias, ptr_t y, int R, int C, int relu, ptr_t st) { bias_act_cast(P(acc), P(bias), P(y), R, C, relu, S(st)); });
   m.def("cast_flat", [](ptr_t src, ptr_t dst, long long n, int kind, ptr_t st) { cast_flat(P(src), P(dst), n, kind, S(st)); });
   m.def("sum_chunks", [](ptr_t src, ptr_t dst, long long chunk, int nchunks, int is_half, ptr_t st) {
     sum_chunks(P(src), P(dst), chunk, nchunks, is_half, S(st)); });

@@ -15,20 +15,6 @@
 
 namespace tmpi {
 
-template <typename T> struct VecIO;
-template <> struct VecIO<__nv_bfloat16> {
-  static constexpr int N = 8;
-  static __device__ __forceinline__ void ld(const __nv_bfloat16* p, float* f) { unpack8(*reinterpret_cast<const bf16x8*>(p), f); }
-  static __device__ __forceinline__ void st(__nv_bfloat16* p, const float* f) { *reinterpret_cast<bf16x8*>(p) = pack8(f); }
-};
-template <> struct VecIO<float> {
-  static constexpr int N = 4;
-  static __device__ __forceinline__ void ld(const float* p, float* f) {
-    const float4 v = *reinterpret_cast<const float4*>(p); f[0] = v.x; f[1] = v.y; f[2] = v.z; f[3] = v.w;
-  }
-  static __device__ __forceinline__ void st(float* p, const float* f) { *reinterpret_cast<float4*>(p) = make_float4(f[0], f[1], f[2], f[3]); }
-};
-
 static inline int grid1(long long n, int block) { return (int)((n + block - 1) / block); }
 
 // ---------------------------------------------------------------- column reductions over row slabs

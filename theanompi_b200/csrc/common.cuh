@@ -63,6 +63,40 @@ __device__ __forceinline__ bf16x8 pack8(const float* f) {
   return p;
 }
 
+// 16-byte vectors of bf16 (8) or fp32 (4) activations, unpacked to / packed from fp32 registers: the kernels that run in both
+// precision modes are templates on the storage type T
+template <typename T> struct VecIO;
+// (Raw: the 16-byte register type, for kernels that keep vectors packed between load and store; LOG2N: C >> LOG2N vectors per row)
+template <> struct VecIO<__nv_bfloat16> {
+  static constexpr int N = 8, LOG2N = 3;
+  using Raw = bf16x8;
+  static __device__ __forceinline__ void unpack(const Raw& r, float* f) { unpack8(r, f); }
+  static __device__ __forceinline__ Raw pack(const float* f) { return pack8(f); }
+  static __device__ __forceinline__ void ld(const __nv_bfloat16* p, float* f) { unpack8(*reinterpret_cast<const bf16x8*>(p), f); }
+  static __device__ __forceinline__ void st(__nv_bfloat16* p, const float* f) { *reinterpret_cast<bf16x8*>(p) = pack8(f); }
+};
+template <> struct VecIO<float> {
+  static constexpr int N = 4, LOG2N = 2;
+  using Raw = float4;
+  static __device__ __forceinline__ void unpack(const Raw& v, float* f) { f[0] = v.x; f[1] = v.y; f[2] = v.z; f[3] = v.w; }
+  static __device__ __forceinline__ Raw pack(const float* f) { return make_float4(f[0], f[1], f[2], f[3]); }
+  static __device__ __forceinline__ void ld(const float* p, float* f) {
+    const float4 v = *reinterpret_cast<const float4*>(p); f[0] = v.x; f[1] = v.y; f[2] = v.z; f[3] = v.w;
+  }
+  static __device__ __forceinline__ void st(float* p, const float* f) { *reinterpret_cast<float4*>(p) = make_float4(f[0], f[1], f[2], f[3]); }
+};
+// N one-byte flags (argmax window indices, dropout keep bits) with one 8- or 4-byte load; .y is 0 for N = 4
+template <int N> __device__ __forceinline__ uint2 ld_flags(const uint8_t* p) {
+  if (N == 8) return *reinterpret_cast<const uint2*>(p);
+  return make_uint2(*reinterpret_cast<const uint32_t*>(p), 0u);
+}
+// scalar conversions between the storage type and fp32
+__device__ __forceinline__ float to_f(__nv_bfloat16 v) { return bf16_to_f(v); }
+__device__ __forceinline__ float to_f(float v) { return v; }
+template <typename T> __device__ __forceinline__ T from_f(float v);
+template <> __device__ __forceinline__ __nv_bfloat16 from_f<__nv_bfloat16>(float v) { return f_to_bf16(v); }
+template <> __device__ __forceinline__ float from_f<float>(float v) { return v; }
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -27,7 +27,7 @@
 namespace tmpi {
 std::atomic<unsigned long long> g_launch_count{0};
 
-namespace gemm {
+namespace wgmma {
 
 constexpr int BM = 128;
 constexpr int NUM_THREADS = 384;       // warpgroup 0 TMA producer, warpgroups 1..2 wgmma consumers + epilogue
@@ -813,13 +813,13 @@ static bool use_tall_tiles(long long M, int nt, int eligible, int sms) {
   return w2 * 17 <= w1 * 10;
 }
 
-}  // namespace gemm
+}  // namespace wgmma
 
-void gemm_set_debug(int flags) { gemm::g_dbg = flags; }
-void gemm_set_bulk(int mask) { gemm::g_bulk = mask; }
+void gemm_set_debug(int flags) { wgmma::g_dbg = flags; }
+void gemm_set_bulk(int mask) { wgmma::g_bulk = mask; }
 
 // ---- reduce-scatter epilogue registry (see api.h)
-namespace gemm {
+namespace wgmma {
 struct RsRange { const char* lo; const char* hi; long long blo, per; };
 static int g_rs_world = 0, g_rs_rank = 0;
 static float* g_rs_peer[kMaxRanks] = {};
@@ -842,39 +842,39 @@ static bool rs_lookup(const void* C, Params& p) {
   }
   return false;
 }
-}  // namespace gemm
+}  // namespace wgmma
 
 void gemm_rs_configure(int world, const void* const* peer_g, const void* local_g) {
-  std::lock_guard<std::mutex> lk(gemm::g_rs_mu);
+  std::lock_guard<std::mutex> lk(wgmma::g_rs_mu);
   if (world > kMaxRanks) throw std::runtime_error("gemm_rs_configure: too many ranks");
-  gemm::g_rs_world = world;
-  gemm::g_rs_local = reinterpret_cast<const char*>(local_g);
-  gemm::g_rs_rank = 0;
+  wgmma::g_rs_world = world;
+  wgmma::g_rs_local = reinterpret_cast<const char*>(local_g);
+  wgmma::g_rs_rank = 0;
   for (int q = 0; q < world; ++q) {
-    gemm::g_rs_peer[q] = reinterpret_cast<float*>(const_cast<void*>(peer_g[q]));
-    if (peer_g[q] == local_g) gemm::g_rs_rank = q;
+    wgmma::g_rs_peer[q] = reinterpret_cast<float*>(const_cast<void*>(peer_g[q]));
+    if (peer_g[q] == local_g) wgmma::g_rs_rank = q;
   }
-  gemm::g_rs_ranges.clear();
+  wgmma::g_rs_ranges.clear();
 }
 void gemm_rs_add_range(const void* c_lo, const void* c_hi, long long blo, long long per) {
-  std::lock_guard<std::mutex> lk(gemm::g_rs_mu);
-  gemm::g_rs_ranges.push_back({reinterpret_cast<const char*>(c_lo), reinterpret_cast<const char*>(c_hi), blo, per});
+  std::lock_guard<std::mutex> lk(wgmma::g_rs_mu);
+  wgmma::g_rs_ranges.push_back({reinterpret_cast<const char*>(c_lo), reinterpret_cast<const char*>(c_hi), blo, per});
 }
 void gemm_rs_clear() {
-  std::lock_guard<std::mutex> lk(gemm::g_rs_mu);
-  gemm::g_rs_world = 0; gemm::g_rs_ranges.clear();
+  std::lock_guard<std::mutex> lk(wgmma::g_rs_mu);
+  wgmma::g_rs_world = 0; wgmma::g_rs_ranges.clear();
 }
 
 // host-side planning helpers, exported so the wave arithmetic can be unit-tested without a GPU
-int gemm_plan_splits(int tiles, int num_kb, int sms) { return gemm::choose_splits(tiles, num_kb, sms); }
-int gemm_plan_tall(long long M, int nt, int out_bf16, int sms) { return gemm::use_tall_tiles(M, nt, out_bf16, sms) ? 1 : 0; }
+int gemm_plan_splits(int tiles, int num_kb, int sms) { return wgmma::choose_splits(tiles, num_kb, sms); }
+int gemm_plan_tall(long long M, int nt, int out_bf16, int sms) { return wgmma::use_tall_tiles(M, nt, out_bf16, sms) ? 1 : 0; }
 
 // C[M,N] (ldc) = alpha * op(A) op(B) + bias, optional ReLU.
 //   a_mn == 0: A is [M, K] with row pitch lda (elements);  a_mn == 1: A is [K, M] with row pitch lda.
 //   b_mn == 0: B is [N, K] with row pitch ldb;             b_mn == 1: B is [K, N] with row pitch ldb.
 //   bn_hint: 0 = auto, else 32/64/128.  splitk: 0 = auto, 1 = none, >1 = forced (fp32 output only, no bias/relu).
 //   T = __nv_bfloat16: bf16 operands (wgmma bf16), bf16 or fp32 output.  T = float: fp32 operands (wgmma tf32), fp32 output.
-namespace gemm {
+namespace wgmma {
 template <typename T>
 static void gemm_host(const void* A, const void* B, void* C, const float* bias, int M, int N, int K, long long lda, long long ldb,
                       long long ldc, int a_mn, int b_mn, int out_bf16, int bias_mode, int relu, float alpha, int bn_hint, int splitk,
@@ -935,17 +935,17 @@ static void gemm_host(const void* A, const void* B, void* C, const float* bias, 
   else if (BN == 64) launch<T, 64, 1>(ta, tb, p, splits, st);
   else launch<T, 32, 1>(ta, tb, p, splits, st);
 }
-}  // namespace gemm
+}  // namespace wgmma
 
-void gemm_bf16(const void* A, const void* B, void* C, const float* bias, int M, int N, int K, long long lda, long long ldb,
-               long long ldc, int a_mn, int b_mn, int out_bf16, int bias_mode, int relu, float alpha, int bn_hint, int splitk,
-               cudaStream_t st, int tf32) {
-  if (tf32) gemm::gemm_host<float>(A, B, C, bias, M, N, K, lda, ldb, ldc, a_mn, b_mn, 0, bias_mode, relu, alpha, bn_hint, splitk, st);
-  else gemm::gemm_host<__nv_bfloat16>(A, B, C, bias, M, N, K, lda, ldb, ldc, a_mn, b_mn, out_bf16, bias_mode, relu, alpha, bn_hint, splitk, st);
+void gemm(const void* A, const void* B, void* C, const float* bias, int M, int N, int K, long long lda, long long ldb,
+          long long ldc, int a_mn, int b_mn, int out_bf16, int bias_mode, int relu, float alpha, int bn_hint, int splitk, int f32,
+          cudaStream_t st) {
+  if (f32) wgmma::gemm_host<float>(A, B, C, bias, M, N, K, lda, ldb, ldc, a_mn, b_mn, 0, bias_mode, relu, alpha, bn_hint, splitk, st);
+  else wgmma::gemm_host<__nv_bfloat16>(A, B, C, bias, M, N, K, lda, ldb, ldc, a_mn, b_mn, out_bf16, bias_mode, relu, alpha, bn_hint, splitk, st);
 }
 
 // ------------------------------------------------------------------ implicit-GEMM convolution (TMA im2col)
-namespace gemm {
+namespace wgmma {
 typedef CUresult (*PFN_encodeIm2col)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const int*,
                                      const int*, cuuint32_t, cuuint32_t, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                      CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -1091,35 +1091,36 @@ static void conv_wgrad_groups(int ngroups, const void* const* dy, const void* x,
   }
   launch<T, 128, 1>(ta[0], tb[0], p, splits, st, ngroups > 1 ? &ta[1] : nullptr, ngroups > 1 ? &tb[1] : nullptr);
 }
-}  // namespace gemm
+}  // namespace wgmma
 
-void conv_fprop_bf16(const void* x, const void* w, void* y, const float* bias, int N, int H, int W, int Ctot, int c_off, int Cg, int KH,
-                     int KW, int Ho, int Wo, int S, int P, int O, long long ldc, int relu, int out_bf16, int dgrad, cudaStream_t st, int tf32) {
+// the output has the activation dtype: bf16, or fp32 on the tf32 path
+void conv_fprop(const void* x, const void* w, void* y, const float* bias, int N, int H, int W, int Ctot, int c_off, int Cg, int KH,
+                int KW, int Ho, int Wo, int S, int P, int O, long long ldc, int relu, int dgrad, int f32, cudaStream_t st) {
   const void* ws[1] = {w}; void* ys[1] = {y}; const float* bs[1] = {bias};
-  if (tf32) gemm::conv_fprop_groups<float>(1, x, &c_off, ws, ys, bs, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldc, relu, 0, dgrad, st);
-  else gemm::conv_fprop_groups<__nv_bfloat16>(1, x, &c_off, ws, ys, bs, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldc, relu, out_bf16, dgrad, st);
+  if (f32) wgmma::conv_fprop_groups<float>(1, x, &c_off, ws, ys, bs, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldc, relu, 0, dgrad, st);
+  else wgmma::conv_fprop_groups<__nv_bfloat16>(1, x, &c_off, ws, ys, bs, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldc, relu, 1, dgrad, st);
 }
 
-void conv_fprop2_bf16(const void* x, const void* w0, const void* w1, void* y0, void* y1, const float* bias0, const float* bias1, int N, int H,
-                      int W, int Ctot, int c_off0, int c_off1, int Cg, int KH, int KW, int Ho, int Wo, int S, int P, int O, long long ldc,
-                      int relu, int out_bf16, int dgrad, cudaStream_t st, int tf32) {
+void conv_fprop2(const void* x, const void* w0, const void* w1, void* y0, void* y1, const float* bias0, const float* bias1, int N, int H,
+                 int W, int Ctot, int c_off0, int c_off1, int Cg, int KH, int KW, int Ho, int Wo, int S, int P, int O, long long ldc,
+                 int relu, int dgrad, int f32, cudaStream_t st) {
   const int co[2] = {c_off0, c_off1}; const void* ws[2] = {w0, w1}; void* ys[2] = {y0, y1}; const float* bs[2] = {bias0, bias1};
-  if (tf32) gemm::conv_fprop_groups<float>(2, x, co, ws, ys, bs, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldc, relu, 0, dgrad, st);
-  else gemm::conv_fprop_groups<__nv_bfloat16>(2, x, co, ws, ys, bs, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldc, relu, out_bf16, dgrad, st);
+  if (f32) wgmma::conv_fprop_groups<float>(2, x, co, ws, ys, bs, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldc, relu, 0, dgrad, st);
+  else wgmma::conv_fprop_groups<__nv_bfloat16>(2, x, co, ws, ys, bs, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldc, relu, 1, dgrad, st);
 }
 
-void conv_wgrad_bf16(const void* dy, const void* x, void* dw, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho,
-                     int Wo, int S, int P, int O, long long ldy, cudaStream_t st, int tf32) {
+void conv_wgrad(const void* dy, const void* x, void* dw, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho,
+                int Wo, int S, int P, int O, long long ldy, int f32, cudaStream_t st) {
   const void* dys[1] = {dy}; void* dws[1] = {dw};
-  if (tf32) gemm::conv_wgrad_groups<float>(1, dys, x, dws, &c_off, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldy, st);
-  else gemm::conv_wgrad_groups<__nv_bfloat16>(1, dys, x, dws, &c_off, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldy, st);
+  if (f32) wgmma::conv_wgrad_groups<float>(1, dys, x, dws, &c_off, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldy, st);
+  else wgmma::conv_wgrad_groups<__nv_bfloat16>(1, dys, x, dws, &c_off, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldy, st);
 }
 
-void conv_wgrad2_bf16(const void* dy0, const void* dy1, const void* x, void* dw0, void* dw1, int N, int H, int W, int Ctot, int c_off0,
-                      int c_off1, int Cg, int KH, int KW, int Ho, int Wo, int S, int P, int O, long long ldy, cudaStream_t st, int tf32) {
+void conv_wgrad2(const void* dy0, const void* dy1, const void* x, void* dw0, void* dw1, int N, int H, int W, int Ctot, int c_off0,
+                 int c_off1, int Cg, int KH, int KW, int Ho, int Wo, int S, int P, int O, long long ldy, int f32, cudaStream_t st) {
   const void* dys[2] = {dy0, dy1}; void* dws[2] = {dw0, dw1}; const int co[2] = {c_off0, c_off1};
-  if (tf32) gemm::conv_wgrad_groups<float>(2, dys, x, dws, co, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldy, st);
-  else gemm::conv_wgrad_groups<__nv_bfloat16>(2, dys, x, dws, co, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldy, st);
+  if (f32) wgmma::conv_wgrad_groups<float>(2, dys, x, dws, co, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldy, st);
+  else wgmma::conv_wgrad_groups<__nv_bfloat16>(2, dys, x, dws, co, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldy, st);
 }
 
 }  // namespace tmpi

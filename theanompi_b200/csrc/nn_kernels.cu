@@ -1,7 +1,9 @@
 // Fused non-GEMM layer kernels for sm_90a: LRN fwd/bwd, max/avg pooling fwd/bwd, dropout (Philox),
 // softmax + NLL + top-1/top-5 error (+ dlogits), ReLU-mask + bias-gradient reduction, NHWC im2col /
 // col2im-gather for the implicit-GEMM convolutions, normalise+crop+mirror for the loader.
-// All activations are NHWC bf16 with C % 8 == 0 (16-byte vectors) unless noted; math is fp32.
+// Activations are NHWC bf16 (C % 8 == 0) or, in the tf32 precision mode, fp32 (C % 4 == 0): 16-byte vectors unless noted;
+// math is fp32.  Each op has one entry point taking `f32`; kernels that do the same arithmetic for both storage types are
+// templates on VecIO<T>, the packed-bf16 tricks (max-pool forward, fused conv→max-pool backward) are bf16-only.
 // Reference ops: theanompi/models/layers2.py (LRN :753-809, Pool :402-428, Dropout :864-908,
 // Softmax :937-997, Crop/Subtract :223-347) and data/utils.py:42-129 (crop_and_mirror).
 #include "common.cuh"
@@ -89,7 +91,42 @@ __global__ void lrn_bwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_b
   *reinterpret_cast<bf16x8*>(dx + r * C + cv * 8) = pack8(out);
 }
 
-void lrn_fwd(const void* x, void* y, long long rows, int C, int n, float k, float alpha, float beta, cudaStream_t st) {
+// fp32: one thread per element, any C and any window (the vector kernels above need C % 8 == 0 and n <= 9)
+__global__ void lrn_fwd_f32_kernel(const float* __restrict__ x, float* __restrict__ y, long long rows, int C, int half, float k,
+                                   float alpha, float beta) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= rows * C) return;
+  const long long r = idx / C; const int c = (int)(idx - r * C);
+  const float* row = x + r * C;
+  float s = 0.f;
+  for (int j = max(0, c - half); j <= min(C - 1, c + half); ++j) s += row[j] * row[j];
+  y[idx] = row[c] * exp2f(-beta * __log2f(k + alpha * s));
+}
+__global__ void lrn_bwd_f32_kernel(const float* __restrict__ x, const float* __restrict__ dy, float* __restrict__ dx, long long rows, int C,
+                                   int half, float k, float alpha, float beta) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= rows * C) return;
+  const long long r = idx / C; const int c = (int)(idx - r * C);
+  const float* xr = x + r * C; const float* dr = dy + r * C;
+  // dx_c = dy_c * s_c^-beta - 2 alpha beta x_c * sum_{i : |i - c| <= half} dy_i x_i s_i^(-beta-1)
+  float acc = 0.f, pc = 0.f;
+  for (int i = max(0, c - half); i <= min(C - 1, c + half); ++i) {
+    float s = 0.f;
+    for (int j = max(0, i - half); j <= min(C - 1, i + half); ++j) s += xr[j] * xr[j];
+    const float scale = k + alpha * s;
+    const float p = exp2f(-beta * __log2f(scale));
+    acc += dr[i] * xr[i] * p / scale;
+    if (i == c) pc = p;
+  }
+  dx[idx] = dr[c] * pc - 2.f * alpha * beta * xr[c] * acc;
+}
+
+void lrn_fwd(const void* x, void* y, long long rows, int C, int n, float k, float alpha, float beta, int f32, cudaStream_t st) {
+  if (f32) {
+    lrn_fwd_f32_kernel<<<grid_for(rows * C, 256), 256, 0, st>>>((const float*)x, (float*)y, rows, C, n / 2, k, alpha, beta);
+    count_launch(); TMPI_CHECK_LAUNCH("lrn_fwd"); ::tmpi::check_capture(st, "lrn_fwd");
+    return;
+  }
   if (C % 8) throw std::runtime_error("lrn: C must be a multiple of 8");
   const int half = n / 2;
   long long total = rows * (C / 8);
@@ -106,7 +143,12 @@ void lrn_fwd(const void* x, void* y, long long rows, int C, int n, float k, floa
   count_launch(); TMPI_CHECK_LAUNCH("lrn_fwd"); ::tmpi::check_capture(st, "lrn_fwd");
 }
 
-void lrn_bwd(const void* x, const void* dy, void* dx, long long rows, int C, int n, float k, float alpha, float beta, cudaStream_t st) {
+void lrn_bwd(const void* x, const void* dy, void* dx, long long rows, int C, int n, float k, float alpha, float beta, int f32, cudaStream_t st) {
+  if (f32) {
+    lrn_bwd_f32_kernel<<<grid_for(rows * C, 256), 256, 0, st>>>((const float*)x, (const float*)dy, (float*)dx, rows, C, n / 2, k, alpha, beta);
+    count_launch(); TMPI_CHECK_LAUNCH("lrn_bwd"); ::tmpi::check_capture(st, "lrn_bwd");
+    return;
+  }
   if (C % 8) throw std::runtime_error("lrn: C must be a multiple of 8");
   const int half = n / 2;
   long long total = rows * (C / 8);
@@ -184,18 +226,48 @@ __global__ void __launch_bounds__(256) maxpool_fwd_kernel(const __nv_bfloat16* _
   }
 }
 
-__global__ void maxpool_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const uint8_t* __restrict__ arg,
-                                   __nv_bfloat16* __restrict__ dx, PoolGeom g) {
-  const int nvec = g.C >> 3;
+// fp32 max pooling: one thread per output vector with plain compares (the packed-bf16 compare above has no fp32 counterpart)
+__global__ void maxpool_fwd_f32_kernel(const float* __restrict__ x, float* __restrict__ y, uint8_t* __restrict__ arg, PoolGeom g) {
+  const int nvec = g.C >> 2;
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long total = (long long)g.N * g.Ho * g.Wo * nvec;
+  if (idx >= total) return;
+  const int cv = (int)(idx % nvec); long long t = idx / nvec;
+  const int wo = (int)(t % g.Wo); t /= g.Wo;
+  const int ho = (int)(t % g.Ho); const int n = (int)(t / g.Ho);
+  float best[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
+  uint32_t bi[4] = {0u, 0u, 0u, 0u};
+  for (int kh = 0; kh < g.k; ++kh) {
+    const int h = ho * g.s - g.p + kh;
+    if (h < 0 || h >= g.H) continue;
+    for (int kw = 0; kw < g.k; ++kw) {
+      const int w = wo * g.s - g.p + kw;
+      if (w < 0 || w >= g.W) continue;
+      float v[4];
+      VecIO<float>::ld(x + (((long long)n * g.H + h) * g.W + w) * g.C + cv * 4, v);
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+        if (v[i] > best[i]) { best[i] = v[i]; bi[i] = (uint32_t)(kh * g.k + kw); }
+    }
+  }
+  const long long o = (((long long)n * g.Ho + ho) * g.Wo + wo) * g.C + cv * 4;
+  VecIO<float>::st(y + o, best);
+  *reinterpret_cast<uint32_t*>(arg + o) = bi[0] | (bi[1] << 8) | (bi[2] << 16) | (bi[3] << 24);
+}
+
+template <typename T>
+__global__ void maxpool_bwd_kernel(const T* __restrict__ dy, const uint8_t* __restrict__ arg, T* __restrict__ dx, PoolGeom g) {
+  constexpr int N = VecIO<T>::N;
+  const int nvec = g.C >> VecIO<T>::LOG2N;
   const unsigned idx = blockIdx.x * blockDim.x + threadIdx.x;             // host guarantees total < 2^32
   const unsigned total = (unsigned)g.N * g.H * g.W * nvec;
   if (idx >= total) return;
   const int cv = (int)(idx % (unsigned)nvec); unsigned t = idx / (unsigned)nvec;
   const int w = (int)(t % g.W); t /= g.W;
   const int h = (int)(t % g.H); const int n = (int)(t / g.H);
-  float acc[8];
+  float acc[N];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+  for (int i = 0; i < N; ++i) acc[i] = 0.f;
   // outputs whose window covers (h, w): ho*s - p <= h < ho*s - p + k
   int ho_lo = (h + g.p - g.k + g.s) / g.s; if (h + g.p - g.k + 1 <= 0) ho_lo = 0;
   int wo_lo = (w + g.p - g.k + g.s) / g.s; if (w + g.p - g.k + 1 <= 0) wo_lo = 0;
@@ -207,19 +279,19 @@ __global__ void maxpool_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const u
     for (int wo = wo_lo; wo <= wo_hi; ++wo) {
       const int kw = w + g.p - wo * g.s;
       if (kw < 0 || kw >= g.k) continue;
-      const long long o = (((long long)n * g.Ho + ho) * g.Wo + wo) * g.C + cv * 8;
-      const uint2 a = *reinterpret_cast<const uint2*>(arg + o);
-      float d[8];
-      unpack8(*reinterpret_cast<const bf16x8*>(dy + o), d);
+      const long long o = (((long long)n * g.Ho + ho) * g.Wo + wo) * g.C + cv * N;
+      const uint2 a = ld_flags<N>(arg + o);
+      float d[N];
+      VecIO<T>::ld(dy + o, d);
       const uint32_t me = (uint32_t)(kh * g.k + kw);
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
+      for (int i = 0; i < N; ++i) {
         const uint32_t ai = ((i < 4 ? a.x : a.y) >> (8 * (i & 3))) & 0xFFu;
         if (ai == me) acc[i] += d[i];
       }
     }
   }
-  *reinterpret_cast<bf16x8*>(dx + (((long long)n * g.H + h) * g.W + w) * g.C + cv * 8) = pack8(acc);
+  VecIO<T>::st(dx + (((long long)n * g.H + h) * g.W + w) * g.C + cv * N, acc);
 }
 
 __device__ __forceinline__ int avg_count(const PoolGeom& g, int ho, int wo) {
@@ -228,46 +300,50 @@ __device__ __forceinline__ int avg_count(const PoolGeom& g, int ho, int wo) {
   return max(1, (h1 - h0) * (w1 - w0));
 }
 
-__global__ void avgpool_fwd_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y, PoolGeom g) {
-  const int nvec = g.C >> 3;
+template <typename T>
+__global__ void avgpool_fwd_kernel(const T* __restrict__ x, T* __restrict__ y, PoolGeom g) {
+  constexpr int N = VecIO<T>::N;
+  const int nvec = g.C >> VecIO<T>::LOG2N;
   const unsigned idx = blockIdx.x * blockDim.x + threadIdx.x;             // host guarantees total < 2^32
   const unsigned total = (unsigned)g.N * g.Ho * g.Wo * nvec;
   if (idx >= total) return;
   const int cv = (int)(idx % (unsigned)nvec); unsigned t = idx / (unsigned)nvec;
   const int wo = (int)(t % g.Wo); t /= g.Wo;
   const int ho = (int)(t % g.Ho); const int n = (int)(t / g.Ho);
-  float acc[8];
+  float acc[N];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+  for (int i = 0; i < N; ++i) acc[i] = 0.f;
   for (int kh = 0; kh < g.k; ++kh) {
     const int h = ho * g.s - g.p + kh;
     if (h < 0 || h >= g.H) continue;
     for (int kw = 0; kw < g.k; ++kw) {
       const int w = wo * g.s - g.p + kw;
       if (w < 0 || w >= g.W) continue;
-      float v[8];
-      unpack8(*reinterpret_cast<const bf16x8*>(x + (((long long)n * g.H + h) * g.W + w) * g.C + cv * 8), v);
+      float v[N];
+      VecIO<T>::ld(x + (((long long)n * g.H + h) * g.W + w) * g.C + cv * N, v);
 #pragma unroll
-      for (int i = 0; i < 8; ++i) acc[i] += v[i];
+      for (int i = 0; i < N; ++i) acc[i] += v[i];
     }
   }
   const float inv = 1.f / (float)avg_count(g, ho, wo);
 #pragma unroll
-  for (int i = 0; i < 8; ++i) acc[i] *= inv;
-  *reinterpret_cast<bf16x8*>(y + (((long long)n * g.Ho + ho) * g.Wo + wo) * g.C + cv * 8) = pack8(acc);
+  for (int i = 0; i < N; ++i) acc[i] *= inv;
+  VecIO<T>::st(y + (((long long)n * g.Ho + ho) * g.Wo + wo) * g.C + cv * N, acc);
 }
 
-__global__ void avgpool_bwd_kernel(const __nv_bfloat16* __restrict__ dy, __nv_bfloat16* __restrict__ dx, PoolGeom g) {
-  const int nvec = g.C >> 3;
+template <typename T>
+__global__ void avgpool_bwd_kernel(const T* __restrict__ dy, T* __restrict__ dx, PoolGeom g) {
+  constexpr int N = VecIO<T>::N;
+  const int nvec = g.C >> VecIO<T>::LOG2N;
   const unsigned idx = blockIdx.x * blockDim.x + threadIdx.x;             // host guarantees total < 2^32
   const unsigned total = (unsigned)g.N * g.H * g.W * nvec;
   if (idx >= total) return;
   const int cv = (int)(idx % (unsigned)nvec); unsigned t = idx / (unsigned)nvec;
   const int w = (int)(t % g.W); t /= g.W;
   const int h = (int)(t % g.H); const int n = (int)(t / g.H);
-  float acc[8];
+  float acc[N];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+  for (int i = 0; i < N; ++i) acc[i] = 0.f;
   const int ho_hi = min(g.Ho - 1, (h + g.p) / g.s);
   const int wo_hi = min(g.Wo - 1, (w + g.p) / g.s);
   for (int ho = 0; ho <= ho_hi; ++ho) {
@@ -276,47 +352,68 @@ __global__ void avgpool_bwd_kernel(const __nv_bfloat16* __restrict__ dy, __nv_bf
     for (int wo = 0; wo <= wo_hi; ++wo) {
       const int kw = w + g.p - wo * g.s;
       if (kw < 0 || kw >= g.k) continue;
-      float d[8];
-      unpack8(*reinterpret_cast<const bf16x8*>(dy + (((long long)n * g.Ho + ho) * g.Wo + wo) * g.C + cv * 8), d);
+      float d[N];
+      VecIO<T>::ld(dy + (((long long)n * g.Ho + ho) * g.Wo + wo) * g.C + cv * N, d);
       const float inv = 1.f / (float)avg_count(g, ho, wo);
 #pragma unroll
-      for (int i = 0; i < 8; ++i) acc[i] += d[i] * inv;
+      for (int i = 0; i < N; ++i) acc[i] += d[i] * inv;
     }
   }
-  *reinterpret_cast<bf16x8*>(dx + (((long long)n * g.H + h) * g.W + w) * g.C + cv * 8) = pack8(acc);
+  VecIO<T>::st(dx + (((long long)n * g.H + h) * g.W + w) * g.C + cv * N, acc);
 }
 
-void pool_fwd(const void* x, void* y, void* arg, int N, int H, int W, int C, int Ho, int Wo, int k, int s, int p, int is_max, cudaStream_t st) {
-  if (C % 8) throw std::runtime_error("pool: C must be a multiple of 8");
+static void need_vec(int C, int f32, const char* what) {
+  if (C % (f32 ? 4 : 8)) throw std::runtime_error(std::string(what) + (f32 ? ": C must be a multiple of 4" : ": C must be a multiple of 8"));
+}
+
+void pool_fwd(const void* x, void* y, void* arg, int N, int H, int W, int C, int Ho, int Wo, int k, int s, int p, int is_max, int f32,
+              cudaStream_t st) {
+  need_vec(C, f32, "pool");
   PoolGeom g{N, H, W, C, Ho, Wo, k, s, p};
-  long long total = (long long)N * Ho * Wo * (C / 8);
-  if ((long long)N * H * W * (C / 8) >= (1LL << 32)) throw std::runtime_error("pool: tensor too large for 32-bit indexing");
-  if ((long long)H * W * C >= (1LL << 31)) throw std::runtime_error("pool: image too large for 32-bit in-image offsets");
-  if (is_max) {
+  const int nvec = f32 ? C / 4 : C / 8;
+  const long long total = (long long)N * Ho * Wo * nvec;
+  if ((long long)N * H * W * nvec >= (1LL << 32)) throw std::runtime_error("pool: tensor too large for 32-bit indexing");
+  if (!f32 && (long long)H * W * C >= (1LL << 31)) throw std::runtime_error("pool: image too large for 32-bit in-image offsets");
+  if (is_max && f32) {
+    maxpool_fwd_f32_kernel<<<grid_for(total, 256), 256, 0, st>>>((const float*)x, (float*)y, (uint8_t*)arg, g);
+  } else if (is_max) {
     const unsigned rows = (unsigned)N * Ho;
     auto X = (const __nv_bfloat16*)x; auto Y = (__nv_bfloat16*)y; auto A = (uint8_t*)arg;
     if (k == 3) maxpool_fwd_kernel<3><<<rows, 256, 0, st>>>(X, Y, A, g);
     else if (k == 2) maxpool_fwd_kernel<2><<<rows, 256, 0, st>>>(X, Y, A, g);
     else maxpool_fwd_kernel<0><<<rows, 256, 0, st>>>(X, Y, A, g);
-  } else avgpool_fwd_kernel<<<grid_for(total, 256), 256, 0, st>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, g);
+  } else if (f32) {
+    avgpool_fwd_kernel<float><<<grid_for(total, 256), 256, 0, st>>>((const float*)x, (float*)y, g);
+  } else {
+    avgpool_fwd_kernel<__nv_bfloat16><<<grid_for(total, 256), 256, 0, st>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, g);
+  }
   count_launch(); TMPI_CHECK_LAUNCH("pool_fwd"); ::tmpi::check_capture(st, "pool_fwd");
 }
 
-void pool_bwd(const void* dy, const void* arg, void* dx, int N, int H, int W, int C, int Ho, int Wo, int k, int s, int p, int is_max, cudaStream_t st) {
+void pool_bwd(const void* dy, const void* arg, void* dx, int N, int H, int W, int C, int Ho, int Wo, int k, int s, int p, int is_max, int f32,
+              cudaStream_t st) {
+  need_vec(C, f32, "pool");
   PoolGeom g{N, H, W, C, Ho, Wo, k, s, p};
-  long long total = (long long)N * H * W * (C / 8);
+  const long long total = (long long)N * H * W * (f32 ? C / 4 : C / 8);
   const int maxw = (k + s - 1) / s;
-  if (is_max && maxw <= 3 && (long long)H * W * C < (1LL << 31)) {
+  const auto A = (const uint8_t*)arg;
+  if (f32) {
+    if (is_max) maxpool_bwd_kernel<float><<<grid_for(total, 256), 256, 0, st>>>((const float*)dy, A, (float*)dx, g);
+    else avgpool_bwd_kernel<float><<<grid_for(total, 256), 256, 0, st>>>((const float*)dy, (float*)dx, g);
+  } else if (is_max && maxw <= 3 && (long long)H * W * C < (1LL << 31)) {
     // row-per-CTA kernel shared with the fused conv→pool backward (all candidate windows in flight at once)
     const int nvec = C / 8;
     const int VT = nvec < 32 ? nvec : 32;
     dim3 grid((unsigned)N * H, (unsigned)((nvec + VT - 1) / VT));
-    auto DY = (const __nv_bfloat16*)dy; auto A = (const uint8_t*)arg; auto DX = (__nv_bfloat16*)dx;
+    auto DY = (const __nv_bfloat16*)dy; auto DX = (__nv_bfloat16*)dx;
     if (maxw == 1) maxpool_relu_bias_bwd_kernel<1, false><<<grid, 256, 0, st>>>(DY, A, nullptr, DX, nullptr, nullptr, C, g, VT);
     else if (maxw == 2) maxpool_relu_bias_bwd_kernel<2, false><<<grid, 256, 0, st>>>(DY, A, nullptr, DX, nullptr, nullptr, C, g, VT);
     else maxpool_relu_bias_bwd_kernel<3, false><<<grid, 256, 0, st>>>(DY, A, nullptr, DX, nullptr, nullptr, C, g, VT);
-  } else if (is_max) maxpool_bwd_kernel<<<grid_for(total, 256), 256, 0, st>>>((const __nv_bfloat16*)dy, (const uint8_t*)arg, (__nv_bfloat16*)dx, g);
-  else avgpool_bwd_kernel<<<grid_for(total, 256), 256, 0, st>>>((const __nv_bfloat16*)dy, (__nv_bfloat16*)dx, g);
+  } else if (is_max) {
+    maxpool_bwd_kernel<__nv_bfloat16><<<grid_for(total, 256), 256, 0, st>>>((const __nv_bfloat16*)dy, A, (__nv_bfloat16*)dx, g);
+  } else {
+    avgpool_bwd_kernel<__nv_bfloat16><<<grid_for(total, 256), 256, 0, st>>>((const __nv_bfloat16*)dy, (__nv_bfloat16*)dx, g);
+  }
   count_launch(); TMPI_CHECK_LAUNCH("pool_bwd"); ::tmpi::check_capture(st, "pool_bwd");
 }
 
@@ -333,10 +430,13 @@ __device__ __forceinline__ void philox4x32(uint32_t c0, uint32_t c1, uint32_t c2
   out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
 }
 
-// y = x * keep; keep drawn with P(keep) = 1 - p_drop from Philox keyed by (seed, layer) and counter (idx, *step)
-__global__ void dropout_fwd_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y, uint8_t* __restrict__ mask,
+// y = x * keep; keep drawn with P(keep) = 1 - p_drop from Philox keyed by (seed, layer) and counter (idx, *step).  One counter
+// draws 8 keep bits, so a thread handles 8 elements in both storage types (one bf16 vector or two fp32 vectors).
+template <typename T>
+__global__ void dropout_fwd_kernel(const T* __restrict__ x, T* __restrict__ y, uint8_t* __restrict__ mask,
                                    long long n8, float p_drop, unsigned long long seed, uint32_t layer,
                                    const unsigned long long* __restrict__ step) {
+  constexpr int N = VecIO<T>::N;
   long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= n8) return;
   const unsigned long long stp = *step;
@@ -345,7 +445,8 @@ __global__ void dropout_fwd_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfl
              (uint32_t)(seed >> 32) ^ (layer * 0x9E3779B9u), r);
   const uint32_t thr = (uint32_t)(p_drop * 65536.f);
   float v[8];
-  unpack8(*reinterpret_cast<const bf16x8*>(x + idx * 8), v);
+#pragma unroll
+  for (int j = 0; j < 8; j += N) VecIO<T>::ld(x + idx * 8 + j, v + j);
   uint32_t mlo = 0, mhi = 0;
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
@@ -354,32 +455,39 @@ __global__ void dropout_fwd_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfl
     v[i] = keep ? v[i] : 0.f;
     if (i < 4) mlo |= keep << (8 * i); else mhi |= keep << (8 * (i - 4));
   }
-  *reinterpret_cast<bf16x8*>(y + idx * 8) = pack8(v);
+#pragma unroll
+  for (int j = 0; j < 8; j += N) VecIO<T>::st(y + idx * 8 + j, v + j);
   *reinterpret_cast<uint2*>(mask + idx * 8) = make_uint2(mlo, mhi);
 }
 
-__global__ void dropout_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const uint8_t* __restrict__ mask,
-                                   __nv_bfloat16* __restrict__ dx, long long n8) {
+template <typename T>
+__global__ void dropout_bwd_kernel(const T* __restrict__ dy, const uint8_t* __restrict__ mask, T* __restrict__ dx, long long nv) {
+  constexpr int N = VecIO<T>::N;
   long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= n8) return;
-  float v[8];
-  unpack8(*reinterpret_cast<const bf16x8*>(dy + idx * 8), v);
-  const uint2 m = *reinterpret_cast<const uint2*>(mask + idx * 8);
+  if (idx >= nv) return;
+  float v[N];
+  VecIO<T>::ld(dy + idx * N, v);
+  const uint2 m = ld_flags<N>(mask + idx * N);
 #pragma unroll
-  for (int i = 0; i < 8; ++i) { const uint32_t k = ((i < 4 ? m.x : m.y) >> (8 * (i & 3))) & 0xFFu; if (!k) v[i] = 0.f; }
-  *reinterpret_cast<bf16x8*>(dx + idx * 8) = pack8(v);
+  for (int i = 0; i < N; ++i) { const uint32_t k = ((i < 4 ? m.x : m.y) >> (8 * (i & 3))) & 0xFFu; if (!k) v[i] = 0.f; }
+  VecIO<T>::st(dx + idx * N, v);
 }
 
 __global__ void advance_step_kernel(unsigned long long* step) { if (threadIdx.x == 0 && blockIdx.x == 0) *step += 1ull; }
 
-void dropout_fwd(const void* x, void* y, void* mask, long long n, float p_drop, unsigned long long seed, int layer, const void* step, cudaStream_t st) {
+void dropout_fwd(const void* x, void* y, void* mask, long long n, float p_drop, unsigned long long seed, int layer, const void* step, int f32,
+                 cudaStream_t st) {
   if (n % 8) throw std::runtime_error("dropout: numel must be a multiple of 8");
-  dropout_fwd_kernel<<<grid_for(n / 8, 256), 256, 0, st>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, (uint8_t*)mask, n / 8, p_drop, seed,
-                                                           (uint32_t)layer, (const unsigned long long*)step);
+  auto M = (uint8_t*)mask; auto S = (const unsigned long long*)step;
+  if (f32) dropout_fwd_kernel<float><<<grid_for(n / 8, 256), 256, 0, st>>>((const float*)x, (float*)y, M, n / 8, p_drop, seed, (uint32_t)layer, S);
+  else dropout_fwd_kernel<__nv_bfloat16><<<grid_for(n / 8, 256), 256, 0, st>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, M, n / 8, p_drop,
+                                                                                 seed, (uint32_t)layer, S);
   count_launch(); TMPI_CHECK_LAUNCH("dropout_fwd"); ::tmpi::check_capture(st, "dropout_fwd");
 }
-void dropout_bwd(const void* dy, const void* mask, void* dx, long long n, cudaStream_t st) {
-  dropout_bwd_kernel<<<grid_for(n / 8, 256), 256, 0, st>>>((const __nv_bfloat16*)dy, (const uint8_t*)mask, (__nv_bfloat16*)dx, n / 8);
+void dropout_bwd(const void* dy, const void* mask, void* dx, long long n, int f32, cudaStream_t st) {
+  auto M = (const uint8_t*)mask;
+  if (f32) dropout_bwd_kernel<float><<<grid_for(n / 4, 256), 256, 0, st>>>((const float*)dy, M, (float*)dx, n / 4);
+  else dropout_bwd_kernel<__nv_bfloat16><<<grid_for(n / 8, 256), 256, 0, st>>>((const __nv_bfloat16*)dy, M, (__nv_bfloat16*)dx, n / 8);
   count_launch(); TMPI_CHECK_LAUNCH("dropout_bwd"); ::tmpi::check_capture(st, "dropout_bwd");
 }
 void advance_step(void* step, cudaStream_t st) {
@@ -389,16 +497,17 @@ void advance_step(void* step, cudaStream_t st) {
 
 // ============================================================================ softmax + NLL + errors + dlogits
 // one CTA per row; rowstat[b] = {nll, err1, err5}; dlogits = (softmax - onehot) * scale
-__global__ void softmax_xent_kernel(const __nv_bfloat16* __restrict__ logits, const long long* __restrict__ labels,
-                                    __nv_bfloat16* __restrict__ dlogits, float* __restrict__ rowstat, int C, float scale) {
+template <typename T>
+__global__ void softmax_xent_kernel(const T* __restrict__ logits, const long long* __restrict__ labels,
+                                    T* __restrict__ dlogits, float* __restrict__ rowstat, int C, float scale) {
   const int b = blockIdx.x;
-  const __nv_bfloat16* row = logits + (long long)b * C;
+  const T* row = logits + (long long)b * C;
   const int label = (int)labels[b];
   __shared__ float red[32];
   __shared__ float bcast;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
   float mx = -INFINITY;
-  for (int c = threadIdx.x; c < C; c += blockDim.x) mx = fmaxf(mx, bf16_to_f(row[c]));
+  for (int c = threadIdx.x; c < C; c += blockDim.x) mx = fmaxf(mx, to_f(row[c]));
   mx = warp_max(mx);
   if (lane == 0) red[warp] = mx;
   __syncthreads();
@@ -406,10 +515,10 @@ __global__ void softmax_xent_kernel(const __nv_bfloat16* __restrict__ logits, co
   __syncthreads();
   mx = bcast;
   __syncthreads();
-  const float lab = bf16_to_f(row[label]);
+  const float lab = to_f(row[label]);
   float se = 0.f, gt = 0.f;
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    const float v = bf16_to_f(row[c]);
+    const float v = to_f(row[c]);
     se += __expf(v - mx);
     gt += (v > lab || (v == lab && c < label)) ? 1.f : 0.f;     // rank of the label's logit
   }
@@ -427,9 +536,9 @@ __global__ void softmax_xent_kernel(const __nv_bfloat16* __restrict__ logits, co
   gt = bcast;
   const float inv = 1.f / se;
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    float pr = __expf(bf16_to_f(row[c]) - mx) * inv;
+    float pr = __expf(to_f(row[c]) - mx) * inv;
     if (c == label) pr -= 1.f;
-    dlogits[(long long)b * C + c] = f_to_bf16(pr * scale);
+    dlogits[(long long)b * C + c] = from_f<T>(pr * scale);
   }
   if (threadIdx.x == 0) {
     rowstat[3 * b + 0] = -(lab - mx - __logf(se));
@@ -453,57 +562,62 @@ __global__ void rowstat_mean_kernel(const float* __restrict__ rowstat, float* __
   }
 }
 
-void softmax_xent(const void* logits, const void* labels, void* dlogits, void* rowstat, void* out3, int B, int C, float weight, cudaStream_t st) {
-  softmax_xent_kernel<<<B, 256, 0, st>>>((const __nv_bfloat16*)logits, (const long long*)labels, (__nv_bfloat16*)dlogits, (float*)rowstat, C, weight / (float)B);
+void softmax_xent(const void* logits, const void* labels, void* dlogits, void* rowstat, void* out3, int B, int C, float weight, int f32,
+                  cudaStream_t st) {
+  auto LB = (const long long*)labels; auto RS = (float*)rowstat;
+  if (f32) softmax_xent_kernel<float><<<B, 256, 0, st>>>((const float*)logits, LB, (float*)dlogits, RS, C, weight / (float)B);
+  else softmax_xent_kernel<__nv_bfloat16><<<B, 256, 0, st>>>((const __nv_bfloat16*)logits, LB, (__nv_bfloat16*)dlogits, RS, C, weight / (float)B);
   count_launch(); TMPI_CHECK_LAUNCH("softmax_xent"); ::tmpi::check_capture(st, "softmax_xent");
   rowstat_mean_kernel<<<1, 256, 0, st>>>((const float*)rowstat, (float*)out3, B, weight);
   count_launch(); TMPI_CHECK_LAUNCH("rowstat_mean"); ::tmpi::check_capture(st, "rowstat_mean");
 }
 
 // ============================================================================ ReLU mask + bias gradient
-// dym = dy * (y > 0) (bf16, contiguous [R, C]);  db[c] += sum_r dym[r, c]   (db pre-zeroed by the launcher)
+// dym = dy * (y > 0) (contiguous [R, C]);  db[c] += sum_r dym[r, c]   (db pre-zeroed by the launcher)
 // dy / y have row pitch ld (elements) so channel slices of a wider tensor work (grouped conv).
-template <bool RELU, bool WRITE>
-__global__ void relu_bias_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ y,
-                                     __nv_bfloat16* __restrict__ dym, float* __restrict__ db, float* __restrict__ db1, int c_split,
+template <typename T, bool RELU, bool WRITE>
+__global__ void relu_bias_bwd_kernel(const T* __restrict__ dy, const T* __restrict__ y,
+                                     T* __restrict__ dym, float* __restrict__ db, float* __restrict__ db1, int c_split,
                                      long long R, int C, long long ld, int VT, int rows_per_cta) {
-  extern __shared__ float sm[];                       // [RL][VT*8]
-  const int nvec = C >> 3;
+  using V = VecIO<T>;
+  constexpr int N = V::N;
+  extern __shared__ float sm[];                       // [RL][VT*N]
+  const int nvec = C >> V::LOG2N;
   const int RL = blockDim.x / VT;
   const int tv = threadIdx.x % VT, tr = threadIdx.x / VT;
   const int cv = blockIdx.y * VT + tv;
   const long long r0 = (long long)blockIdx.x * rows_per_cta;
-  float acc[8];
+  float acc[N];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+  for (int i = 0; i < N; ++i) acc[i] = 0.f;
   if (tr < RL && cv < nvec) {
     const long long rend = min(R, r0 + rows_per_cta);
     for (long long r = r0 + tr; r < rend; r += 4 * RL) {
       // 4 rows per trip, all loads issued before any use (memory-level parallelism: this kernel is pure streaming)
-      bf16x8 dv[4], yv[4];
+      typename V::Raw dv[4], yv[4];
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
         const long long rr = r + (long long)u * RL;
         if (rr < rend) {
-          dv[u] = *reinterpret_cast<const bf16x8*>(dy + rr * ld + cv * 8);
-          if (RELU) yv[u] = *reinterpret_cast<const bf16x8*>(y + rr * ld + cv * 8);
+          dv[u] = *reinterpret_cast<const typename V::Raw*>(dy + rr * ld + cv * N);
+          if (RELU) yv[u] = *reinterpret_cast<const typename V::Raw*>(y + rr * ld + cv * N);
         }
       }
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
         const long long rr = r + (long long)u * RL;
         if (rr < rend) {
-          float d[8];
-          unpack8(dv[u], d);
+          float d[N];
+          V::unpack(dv[u], d);
           if (RELU) {
-            float v[8];
-            unpack8(yv[u], v);
+            float v[N];
+            V::unpack(yv[u], v);
 #pragma unroll
-            for (int i = 0; i < 8; ++i) if (!(v[i] > 0.f)) d[i] = 0.f;
+            for (int i = 0; i < N; ++i) if (!(v[i] > 0.f)) d[i] = 0.f;
           }
-          if (WRITE) *reinterpret_cast<bf16x8*>(dym + rr * C + cv * 8) = pack8(d);
+          if (WRITE) *reinterpret_cast<typename V::Raw*>(dym + rr * C + cv * N) = V::pack(d);
 #pragma unroll
-          for (int i = 0; i < 8; ++i) acc[i] += d[i];
+          for (int i = 0; i < N; ++i) acc[i] += d[i];
         }
       }
     }
@@ -511,15 +625,15 @@ __global__ void relu_bias_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const
   if (db == nullptr) return;
   if (tr < RL) {
 #pragma unroll
-    for (int i = 0; i < 8; ++i) sm[(tr * VT + tv) * 8 + i] = acc[i];
+    for (int i = 0; i < N; ++i) sm[(tr * VT + tv) * N + i] = acc[i];
   }
   __syncthreads();
-  if (threadIdx.x < VT * 8) {
-    const int v = threadIdx.x / 8, i = threadIdx.x % 8;
-    const int c = (blockIdx.y * VT + v) * 8 + i;
+  if (threadIdx.x < VT * N) {
+    const int v = threadIdx.x / N, i = threadIdx.x % N;
+    const int c = (blockIdx.y * VT + v) * N + i;
     if (c < C) {
       float s = 0.f;
-      for (int t = 0; t < RL; ++t) s += sm[(t * VT + v) * 8 + i];
+      for (int t = 0; t < RL; ++t) s += sm[(t * VT + v) * N + i];
       atomicAdd(c < c_split ? db + c : db1 + (c - c_split), s);
     }
   }
@@ -527,10 +641,11 @@ __global__ void relu_bias_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const
 
 // db: bias gradient for channels [0, c_split), db1: for channels [c_split, C) (the two parameter sets of a 2-group block);
 // pass db1 = nullptr / c_split = C for a single bias vector.
-void relu_bias_bwd2(const void* dy, const void* y, void* dym, void* db, void* db1, int c_split, long long R, int C, long long ld, int relu,
-                    cudaStream_t st) {
-  if (C % 8) throw std::runtime_error("relu_bias_bwd: C must be a multiple of 8");
-  const int nvec = C / 8;
+template <typename T>
+static void relu_bias_bwd_t(const void* dy, const void* y, void* dym, void* db, void* db1, int c_split, long long R, int C, long long ld,
+                            int relu, cudaStream_t st) {
+  constexpr int N = VecIO<T>::N;
+  const int nvec = C / N;
   const int VT = nvec < 32 ? nvec : 32;
   const int RL = 256 / VT;
   // deterministic mode: one CTA per channel group sums ALL rows (fixed order) instead of row slabs + atomics
@@ -538,48 +653,59 @@ void relu_bias_bwd2(const void* dy, const void* y, void* dym, void* db, void* db
   if (rows_per_cta_ll >= (1LL << 31)) throw std::runtime_error("relu_bias_bwd: too many rows for the deterministic mode");
   const int rows_per_cta = (int)rows_per_cta_ll;
   dim3 grid((unsigned)((R + rows_per_cta - 1) / rows_per_cta), (unsigned)((nvec + VT - 1) / VT));
-  const size_t smem = (size_t)RL * VT * 8 * sizeof(float);
+  const size_t smem = (size_t)RL * VT * N * sizeof(float);
   if (!db1 || c_split > C) c_split = C;
   if (db) check_cuda(cudaMemsetAsync(db, 0, (size_t)c_split * 4, st), "relu_bias_bwd memset");
   if (db && c_split < C) check_cuda(cudaMemsetAsync(db1, 0, (size_t)(C - c_split) * 4, st), "relu_bias_bwd memset");
   const bool write = dym != nullptr;
-  auto DY = (const __nv_bfloat16*)dy; auto Y = (const __nv_bfloat16*)y; auto DM = (__nv_bfloat16*)dym; auto DB = (float*)db; auto DB1 = (float*)db1;
-  if (relu && write) relu_bias_bwd_kernel<true, true><<<grid, 256, smem, st>>>(DY, Y, DM, DB, DB1, c_split, R, C, ld, VT, rows_per_cta);
-  else if (relu) relu_bias_bwd_kernel<true, false><<<grid, 256, smem, st>>>(DY, Y, DM, DB, DB1, c_split, R, C, ld, VT, rows_per_cta);
-  else if (write) relu_bias_bwd_kernel<false, true><<<grid, 256, smem, st>>>(DY, Y, DM, DB, DB1, c_split, R, C, ld, VT, rows_per_cta);
-  else relu_bias_bwd_kernel<false, false><<<grid, 256, smem, st>>>(DY, Y, DM, DB, DB1, c_split, R, C, ld, VT, rows_per_cta);
+  auto DY = (const T*)dy; auto Y = (const T*)y; auto DM = (T*)dym; auto DB = (float*)db; auto DB1 = (float*)db1;
+  if (relu && write) relu_bias_bwd_kernel<T, true, true><<<grid, 256, smem, st>>>(DY, Y, DM, DB, DB1, c_split, R, C, ld, VT, rows_per_cta);
+  else if (relu) relu_bias_bwd_kernel<T, true, false><<<grid, 256, smem, st>>>(DY, Y, DM, DB, DB1, c_split, R, C, ld, VT, rows_per_cta);
+  else if (write) relu_bias_bwd_kernel<T, false, true><<<grid, 256, smem, st>>>(DY, Y, DM, DB, DB1, c_split, R, C, ld, VT, rows_per_cta);
+  else relu_bias_bwd_kernel<T, false, false><<<grid, 256, smem, st>>>(DY, Y, DM, DB, DB1, c_split, R, C, ld, VT, rows_per_cta);
   count_launch(); TMPI_CHECK_LAUNCH("relu_bias_bwd"); ::tmpi::check_capture(st, "relu_bias_bwd");
 }
-void relu_bias_bwd(const void* dy, const void* y, void* dym, void* db, long long R, int C, long long ld, int relu, cudaStream_t st) {
-  relu_bias_bwd2(dy, y, dym, db, nullptr, C, R, C, ld, relu, st);
+void relu_bias_bwd(const void* dy, const void* y, void* dym, void* db, void* db1, int c_split, long long R, int C, long long ld, int relu,
+                   int f32, cudaStream_t st) {
+  need_vec(C, f32, "relu_bias_bwd");
+  if (f32) relu_bias_bwd_t<float>(dy, y, dym, db, db1, c_split, R, C, ld, relu, st);
+  else relu_bias_bwd_t<__nv_bfloat16>(dy, y, dym, db, db1, c_split, R, C, ld, relu, st);
 }
 
-// y[r, c] (bf16) = act(acc[r, c] (fp32) + bias[c]) — finishing pass of a split-K forward GEMM (small-batch FC layers: the
-// parallelism has to come from splitting K, and split-K accumulates in fp32 with reductions, so bias / ReLU / cast run here)
-__global__ void bias_act_cast_kernel(const float* __restrict__ acc, const float* __restrict__ bias, __nv_bfloat16* __restrict__ y,
-                                     int R, int C, int relu) {
-  const int nvec = C >> 3;
-  const unsigned idx = blockIdx.x * blockDim.x + threadIdx.x;
+// y[r, c] = act(acc[r, c] (fp32) + bias[c]), stored as T — finishing pass of a split-K forward GEMM (small-batch FC layers: the
+// parallelism has to come from splitting K, and split-K accumulates in fp32 with reductions, so bias / ReLU / cast run here).
+// The fp32 output may alias acc (in place).
+template <typename T>
+__global__ void bias_act_kernel(const float* __restrict__ acc, const float* __restrict__ bias, T* __restrict__ y, int R, int C, int relu) {
+  constexpr int N = VecIO<T>::N;
+  const int nvec = C >> VecIO<T>::LOG2N;
+  const unsigned idx = blockIdx.x * blockDim.x + threadIdx.x;            // host guarantees R * nvec < 2^32
   if (idx >= (unsigned)R * (unsigned)nvec) return;
   const unsigned r = idx / (unsigned)nvec; const int cv = (int)(idx - r * (unsigned)nvec);
-  const float4 a0 = *reinterpret_cast<const float4*>(acc + (size_t)r * C + cv * 8);
-  const float4 a1 = *reinterpret_cast<const float4*>(acc + (size_t)r * C + cv * 8 + 4);
-  float v[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+  float v[N];
+#pragma unroll
+  for (int j = 0; j < N; j += 4) VecIO<float>::ld(acc + (size_t)r * C + cv * N + j, v + j);
   if (bias) {
-    const float4 b0 = *reinterpret_cast<const float4*>(bias + cv * 8), b1 = *reinterpret_cast<const float4*>(bias + cv * 8 + 4);
-    v[0] += b0.x; v[1] += b0.y; v[2] += b0.z; v[3] += b0.w; v[4] += b1.x; v[5] += b1.y; v[6] += b1.z; v[7] += b1.w;
+#pragma unroll
+    for (int j = 0; j < N; j += 4) {
+      const float4 b = *reinterpret_cast<const float4*>(bias + cv * N + j);
+      v[j] += b.x; v[j + 1] += b.y; v[j + 2] += b.z; v[j + 3] += b.w;
+    }
   }
   if (relu) {
 #pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = fmaxf(v[i], 0.f);
+    for (int i = 0; i < N; ++i) v[i] = fmaxf(v[i], 0.f);
   }
-  *reinterpret_cast<bf16x8*>(y + (size_t)r * C + cv * 8) = pack8(v);
+  VecIO<T>::st(y + (size_t)r * C + cv * N, v);
 }
-void bias_act_cast(const void* acc, const void* bias, void* y, int R, int C, int relu, cudaStream_t st) {
-  if (C % 8) throw std::runtime_error("bias_act_cast: C must be a multiple of 8");
-  const long long total = (long long)R * (C / 8);
-  bias_act_cast_kernel<<<grid_for(total, 256), 256, 0, st>>>((const float*)acc, (const float*)bias, (__nv_bfloat16*)y, R, C, relu);
-  count_launch(); TMPI_CHECK_LAUNCH("bias_act_cast"); ::tmpi::check_capture(st, "bias_act_cast");
+void bias_act(const void* acc, const void* bias, void* y, int R, int C, int relu, int f32, cudaStream_t st) {
+  need_vec(C, f32, "bias_act");
+  const long long total = (long long)R * (f32 ? C / 4 : C / 8);
+  if (total >= (1LL << 32)) throw std::runtime_error("bias_act: tensor too large for 32-bit indexing");
+  auto A = (const float*)acc; auto B = (const float*)bias;
+  if (f32) bias_act_kernel<float><<<grid_for(total, 256), 256, 0, st>>>(A, B, (float*)y, R, C, relu);
+  else bias_act_kernel<__nv_bfloat16><<<grid_for(total, 256), 256, 0, st>>>(A, B, (__nv_bfloat16*)y, R, C, relu);
+  count_launch(); TMPI_CHECK_LAUNCH("bias_act"); ::tmpi::check_capture(st, "bias_act");
 }
 
 // Fused backward of  conv(+bias+ReLU) -> max-pool : one pass over the conv output instead of three.
@@ -707,15 +833,17 @@ void maxpool_relu_bias_bwd(const void* dyp, const void* arg, const void* y, void
   count_launch(); TMPI_CHECK_LAUNCH("maxpool_relu_bias_bwd"); ::tmpi::check_capture(st, "maxpool_relu_bias_bwd");
 }
 
-// ============================================================================ im2col / col2im (NHWC, bf16)
+// ============================================================================ im2col / col2im (NHWC)
 struct ConvGeom { int N, H, W, Ctot, c_off, Cg, KH, KW, Ho, Wo, s, p; long long ldcol; int K; };
 
 // col[m, (kh*KW+kw)*Cg + c] = x[n, ho*s-p+kh, wo*s-p+kw, c_off+c]   (zero outside the image)
-__global__ void __launch_bounds__(256) im2col_vec8_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ col, ConvGeom g) {
+template <typename T>
+__global__ void __launch_bounds__(256) im2col_vec_kernel(const T* __restrict__ x, T* __restrict__ col, ConvGeom g) {
   // one CTA per IM2COL_ROWS consecutive output pixels; (n, ho, wo) is decoded once per row, the threads sweep the
-  // row's KH*KW*(Cg/8) 16-byte vectors with 32-bit index math only.
+  // row's KH*KW*(Cg/N) 16-byte vectors with 32-bit index math only.
   constexpr int IM2COL_ROWS = 8;
-  const int cvn = g.Cg >> 3;
+  constexpr int N = VecIO<T>::N;
+  const int cvn = g.Cg >> VecIO<T>::LOG2N;
   const int per_m = g.KH * g.KW * cvn;
   const long long M = (long long)g.N * g.Ho * g.Wo;
   const long long m_base = (long long)blockIdx.x * IM2COL_ROWS;
@@ -725,76 +853,80 @@ __global__ void __launch_bounds__(256) im2col_vec8_kernel(const __nv_bfloat16* _
     const int wo = (int)(m % g.Wo); const long long t = m / g.Wo;
     const int ho = (int)(t % g.Ho); const int n = (int)(t / g.Ho);
     const int h0 = ho * g.s - g.p, w0 = wo * g.s - g.p;
-    const __nv_bfloat16* xin = x + (long long)n * g.H * g.W * g.Ctot + g.c_off;
-    __nv_bfloat16* dst = col + m * g.ldcol;
+    const T* xin = x + (long long)n * g.H * g.W * g.Ctot + g.c_off;
+    T* dst = col + m * g.ldcol;
     for (int v = threadIdx.x; v < per_m; v += blockDim.x) {
       const int kk = v / cvn, cv = v - kk * cvn;
       const int kh = kk / g.KW, kw = kk - kh * g.KW;
       const int h = h0 + kh, w = w0 + kw;
-      bf16x8 val;
+      typename VecIO<T>::Raw val;
       if (h >= 0 && h < g.H && w >= 0 && w < g.W)
-        val = *reinterpret_cast<const bf16x8*>(xin + ((long long)h * g.W + w) * g.Ctot + cv * 8);
+        val = *reinterpret_cast<const typename VecIO<T>::Raw*>(xin + ((long long)h * g.W + w) * g.Ctot + cv * N);
       else {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) val.v[i] = __floats2bfloat162_rn(0.f, 0.f);
+        const float zero[N] = {};
+        val = VecIO<T>::pack(zero);
       }
-      *reinterpret_cast<bf16x8*>(dst + kk * g.Cg + cv * 8) = val;
+      *reinterpret_cast<typename VecIO<T>::Raw*>(dst + kk * g.Cg + cv * N) = val;
     }
   }
 }
 
 // generic (any Cg): one thread per (m, kh*KW+kw); the extra index KH*KW zero-fills the K..ldcol padding
-__global__ void im2col_scalar_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ col, ConvGeom g) {
+template <typename T>
+__global__ void im2col_scalar_kernel(const T* __restrict__ x, T* __restrict__ col, ConvGeom g) {
   const int per_m = g.KH * g.KW + 1;
   long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   long long M = (long long)g.N * g.Ho * g.Wo;
   if (idx >= M * per_m) return;
   const long long m = idx / per_m; const int kk = (int)(idx % per_m);
-  __nv_bfloat16* dst = col + m * g.ldcol;
-  if (kk == g.KH * g.KW) { for (int c = g.K; c < g.ldcol; ++c) dst[c] = f_to_bf16(0.f); return; }
+  T* dst = col + m * g.ldcol;
+  if (kk == g.KH * g.KW) { for (int c = g.K; c < g.ldcol; ++c) dst[c] = from_f<T>(0.f); return; }
   const int kh = kk / g.KW, kw = kk % g.KW;
   const int wo = (int)(m % g.Wo); long long t = m / g.Wo;
   const int ho = (int)(t % g.Ho); const int n = (int)(t / g.Ho);
   const int h = ho * g.s - g.p + kh, w = wo * g.s - g.p + kw;
   const bool ok = (h >= 0 && h < g.H && w >= 0 && w < g.W);
-  const __nv_bfloat16* src = x + (((long long)n * g.H + h) * g.W + w) * g.Ctot + g.c_off;
+  const T* src = x + (((long long)n * g.H + h) * g.W + w) * g.Ctot + g.c_off;
   dst += (long long)kk * g.Cg;
-  for (int c = 0; c < g.Cg; ++c) dst[c] = ok ? src[c] : f_to_bf16(0.f);
+  for (int c = 0; c < g.Cg; ++c) dst[c] = ok ? src[c] : from_f<T>(0.f);
 }
 
 // small-C path (conv1: C = 3): one CTA per (image, output row).  The KH input rows the output row needs are staged in
 // shared memory with coalesced loads; the CTA then emits its Wo consecutive col rows (one contiguous Wo*ldcol span)
 // as 16-byte vectors — each col row is KH runs of KW*Cg contiguous input elements.
-__global__ void __launch_bounds__(256) im2col_rows_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ col, ConvGeom g) {
-  extern __shared__ __nv_bfloat16 rows[];                  // [KH][W*Cg]
+template <typename T>
+__global__ void __launch_bounds__(256) im2col_rows_kernel(const T* __restrict__ x, T* __restrict__ col, ConvGeom g) {
+  constexpr int N = VecIO<T>::N;
+  extern __shared__ __align__(16) unsigned char im2col_smem[];
+  T* rows = reinterpret_cast<T*>(im2col_smem);             // [KH][W*Cg]
   const int n = blockIdx.x / g.Ho, ho = blockIdx.x % g.Ho;
   const int rowlen = g.W * g.Cg;
   const bool dense = (g.Cg == g.Ctot);                     // all channels used: an input row is one contiguous span
   for (int kh = 0; kh < g.KH; ++kh) {
     const int h = ho * g.s - g.p + kh;
-    __nv_bfloat16* dst = rows + kh * rowlen;
+    T* dst = rows + kh * rowlen;
     if (h < 0 || h >= g.H) {
-      for (int e = threadIdx.x; e < rowlen; e += blockDim.x) dst[e] = f_to_bf16(0.f);
+      for (int e = threadIdx.x; e < rowlen; e += blockDim.x) dst[e] = from_f<T>(0.f);
     } else if (dense) {
-      const __nv_bfloat16* src = x + ((long long)n * g.H + h) * g.W * g.Ctot;
+      const T* src = x + ((long long)n * g.H + h) * g.W * g.Ctot;
       for (int e = threadIdx.x; e < rowlen; e += blockDim.x) dst[e] = src[e];
     } else {
-      const __nv_bfloat16* src = x + ((long long)n * g.H + h) * g.W * g.Ctot + g.c_off;
+      const T* src = x + ((long long)n * g.H + h) * g.W * g.Ctot + g.c_off;
       for (int e = threadIdx.x; e < rowlen; e += blockDim.x) { const int w = e / g.Cg; dst[e] = src[(long long)w * g.Ctot + (e - w * g.Cg)]; }
     }
   }
   __syncthreads();
   const int run = g.KW * g.Cg;                             // contiguous elements per (kh)
-  const int vec_per_row = (int)(g.ldcol >> 3);
-  __nv_bfloat16* out = col + ((long long)n * g.Ho + ho) * g.Wo * g.ldcol;
+  const int vec_per_row = (int)(g.ldcol >> VecIO<T>::LOG2N);
+  T* out = col + ((long long)n * g.Ho + ho) * g.Wo * g.ldcol;
   for (int i = threadIdx.x; i < g.Wo * vec_per_row; i += blockDim.x) {
-    const int wo = i / vec_per_row, e0 = (i - wo * vec_per_row) * 8;
+    const int wo = i / vec_per_row, e0 = (i - wo * vec_per_row) * N;
     const int xbase = (wo * g.s - g.p) * g.Cg;              // may be negative with padding
     int kh = e0 / run, r = e0 - kh * run;
-    __align__(16) __nv_bfloat16 v[8];
+    __align__(16) T v[N];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      __nv_bfloat16 t = f_to_bf16(0.f);
+    for (int j = 0; j < N; ++j) {
+      T t = from_f<T>(0.f);
       if (e0 + j < g.K) {
         const int xi = xbase + r;
         if (xi >= 0 && xi < rowlen) t = rows[kh * rowlen + xi];
@@ -807,17 +939,19 @@ __global__ void __launch_bounds__(256) im2col_rows_kernel(const __nv_bfloat16* _
 }
 
 // dx[n,h,w,c_off+c] = sum over (kh,kw) with (h+p-kh)%s==0, (w+p-kw)%s==0 of dcol[m(n,ho,wo), (kh*KW+kw)*Cg + c]
-__global__ void col2im_vec8_kernel(const __nv_bfloat16* __restrict__ dcol, __nv_bfloat16* __restrict__ dx, ConvGeom g) {
-  const unsigned cvn = (unsigned)(g.Cg >> 3);
+template <typename T>
+__global__ void col2im_vec_kernel(const T* __restrict__ dcol, T* __restrict__ dx, ConvGeom g) {
+  constexpr int N = VecIO<T>::N;
+  const unsigned cvn = (unsigned)(g.Cg >> VecIO<T>::LOG2N);
   const unsigned idx = blockIdx.x * blockDim.x + threadIdx.x;           // host guarantees total < 2^32
   const unsigned total = (unsigned)g.N * g.H * g.W * cvn;
   if (idx >= total) return;
   const int cv = (int)(idx % cvn); unsigned t = idx / cvn;
   const int w = (int)(t % g.W); t /= g.W;
   const int h = (int)(t % g.H); const int n = (int)(t / g.H);
-  float acc[8];
+  float acc[N];
 #pragma unroll
-  for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+  for (int i = 0; i < N; ++i) acc[i] = 0.f;
   for (int kh = 0; kh < g.KH; ++kh) {
     const int th = h + g.p - kh;
     if (th < 0 || th % g.s) continue;
@@ -829,83 +963,65 @@ __global__ void col2im_vec8_kernel(const __nv_bfloat16* __restrict__ dcol, __nv_
       const int wo = tw / g.s;
       if (wo >= g.Wo) continue;
       const long long m = ((long long)n * g.Ho + ho) * g.Wo + wo;
-      float v[8];
-      unpack8(*reinterpret_cast<const bf16x8*>(dcol + m * g.ldcol + (long long)(kh * g.KW + kw) * g.Cg + cv * 8), v);
+      float v[N];
+      VecIO<T>::ld(dcol + m * g.ldcol + (long long)(kh * g.KW + kw) * g.Cg + cv * N, v);
 #pragma unroll
-      for (int i = 0; i < 8; ++i) acc[i] += v[i];
+      for (int i = 0; i < N; ++i) acc[i] += v[i];
     }
   }
-  *reinterpret_cast<bf16x8*>(dx + (((long long)n * g.H + h) * g.W + w) * g.Ctot + g.c_off + cv * 8) = pack8(acc);
+  VecIO<T>::st(dx + (((long long)n * g.H + h) * g.W + w) * g.Ctot + g.c_off + cv * N, acc);
+}
+
+template <typename T>
+static void im2col_t(const void* x, void* col, const ConvGeom& g, cudaStream_t st) {
+  constexpr int N = VecIO<T>::N;
+  const long long M = (long long)g.N * g.Ho * g.Wo;
+  // the vector kernel writes the K columns only: it needs rows without padding
+  if (g.Cg % N == 0 && g.c_off % N == 0 && g.Ctot % N == 0 && g.ldcol == g.K) {
+    im2col_vec_kernel<T><<<grid_for(M, 8), 256, 0, st>>>((const T*)x, (T*)col, g);
+  } else if (g.ldcol % N == 0 && (size_t)g.KH * g.W * g.Cg * sizeof(T) <= 48 * 1024) {
+    im2col_rows_kernel<T><<<g.N * g.Ho, 256, (size_t)g.KH * g.W * g.Cg * sizeof(T), st>>>((const T*)x, (T*)col, g);
+  } else {
+    const long long total = M * (g.KH * g.KW + 1);
+    im2col_scalar_kernel<T><<<grid_for(total, 256), 256, 0, st>>>((const T*)x, (T*)col, g);
+  }
 }
 
 void im2col(const void* x, void* col, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho, int Wo, int s, int p,
-            long long ldcol, cudaStream_t st) {
+            long long ldcol, int f32, cudaStream_t st) {
   ConvGeom g{N, H, W, Ctot, c_off, Cg, KH, KW, Ho, Wo, s, p, ldcol, KH * KW * Cg};
-  long long M = (long long)N * Ho * Wo;
-  if (Cg % 8 == 0 && c_off % 8 == 0 && Ctot % 8 == 0 && ldcol % 8 == 0) {
-    im2col_vec8_kernel<<<grid_for(M, 8), 256, 0, st>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)col, g);
-  } else if (ldcol % 8 == 0 && (size_t)KH * W * Cg * 2 <= 48 * 1024) {
-    im2col_rows_kernel<<<N * Ho, 256, (size_t)KH * W * Cg * 2, st>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)col, g);
-  } else {
-    long long total = M * (KH * KW + 1);
-    im2col_scalar_kernel<<<grid_for(total, 256), 256, 0, st>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)col, g);
-  }
+  if (f32) im2col_t<float>(x, col, g, st);
+  else im2col_t<__nv_bfloat16>(x, col, g, st);
   count_launch(); TMPI_CHECK_LAUNCH("im2col"); ::tmpi::check_capture(st, "im2col");
 }
 
 void col2im(const void* dcol, void* dx, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho, int Wo, int s, int p,
-            long long ldcol, cudaStream_t st) {
-  if (Cg % 8 || c_off % 8 || Ctot % 8 || ldcol % 8) throw std::runtime_error("col2im: channel counts must be multiples of 8");
+            long long ldcol, int f32, cudaStream_t st) {
+  const int V = f32 ? 4 : 8;
+  if (Cg % V || c_off % V || Ctot % V || ldcol % V)
+    throw std::runtime_error(f32 ? "col2im: channel counts must be multiples of 4" : "col2im: channel counts must be multiples of 8");
   ConvGeom g{N, H, W, Ctot, c_off, Cg, KH, KW, Ho, Wo, s, p, ldcol, KH * KW * Cg};
-  long long total = (long long)N * H * W * (Cg / 8);
+  long long total = (long long)N * H * W * (Cg / V);
   if (total >= (1LL << 32)) throw std::runtime_error("col2im: tensor too large for 32-bit indexing");
-  col2im_vec8_kernel<<<grid_for(total, 256), 256, 0, st>>>((const __nv_bfloat16*)dcol, (__nv_bfloat16*)dx, g);
+  if (f32) col2im_vec_kernel<float><<<grid_for(total, 256), 256, 0, st>>>((const float*)dcol, (float*)dx, g);
+  else col2im_vec_kernel<__nv_bfloat16><<<grid_for(total, 256), 256, 0, st>>>((const __nv_bfloat16*)dcol, (__nv_bfloat16*)dx, g);
   count_launch(); TMPI_CHECK_LAUNCH("col2im"); ::tmpi::check_capture(st, "col2im");
 }
 
 // ============================================================================ small utility kernels
 // rows x cols (pitch src_ld) → rows x dst_ld with zero padding (K-padding of conv1 weights for TMA pitch rules)
-__global__ void pad_rows_kernel(const __nv_bfloat16* __restrict__ src, __nv_bfloat16* __restrict__ dst, long long rows, int cols,
-                                long long src_ld, long long dst_ld) {
+template <typename T>
+__global__ void pad_rows_kernel(const T* __restrict__ src, T* __restrict__ dst, long long rows, int cols, long long src_ld, long long dst_ld) {
   long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= rows * dst_ld) return;
   const long long r = idx / dst_ld; const int c = (int)(idx % dst_ld);
-  dst[idx] = c < cols ? src[r * src_ld + c] : f_to_bf16(0.f);
+  dst[idx] = c < cols ? src[r * src_ld + c] : from_f<T>(0.f);
 }
-void pad_rows(const void* src, void* dst, long long rows, int cols, long long src_ld, long long dst_ld, cudaStream_t st) {
-  pad_rows_kernel<<<grid_for(rows * dst_ld, 256), 256, 0, st>>>((const __nv_bfloat16*)src, (__nv_bfloat16*)dst, rows, cols, src_ld, dst_ld);
+void pad_rows(const void* src, void* dst, long long rows, int cols, long long src_ld, long long dst_ld, int f32, cudaStream_t st) {
+  if (f32) pad_rows_kernel<float><<<grid_for(rows * dst_ld, 256), 256, 0, st>>>((const float*)src, (float*)dst, rows, cols, src_ld, dst_ld);
+  else pad_rows_kernel<__nv_bfloat16><<<grid_for(rows * dst_ld, 256), 256, 0, st>>>((const __nv_bfloat16*)src, (__nv_bfloat16*)dst, rows, cols,
+                                                                                      src_ld, dst_ld);
   count_launch(); TMPI_CHECK_LAUNCH("pad_rows"); ::tmpi::check_capture(st, "pad_rows");
-}
-
-__global__ void transpose_bf16_kernel(const __nv_bfloat16* __restrict__ src, __nv_bfloat16* __restrict__ dst, int R, int C) {
-  __shared__ __nv_bfloat16 tile[32][33];
-  int c = blockIdx.x * 32 + threadIdx.x, r = blockIdx.y * 32 + threadIdx.y;
-  for (int j = 0; j < 32; j += 8) if (c < C && r + j < R) tile[threadIdx.y + j][threadIdx.x] = src[(long long)(r + j) * C + c];
-  __syncthreads();
-  int oc = blockIdx.y * 32 + threadIdx.x, orow = blockIdx.x * 32 + threadIdx.y;
-  for (int j = 0; j < 32; j += 8) if (oc < R && orow + j < C) dst[(long long)(orow + j) * R + oc] = tile[threadIdx.x][threadIdx.y + j];
-}
-void transpose_bf16(const void* src, void* dst, int R, int C, cudaStream_t st) {
-  dim3 grid((C + 31) / 32, (R + 31) / 32), block(32, 8);
-  transpose_bf16_kernel<<<grid, block, 0, st>>>((const __nv_bfloat16*)src, (__nv_bfloat16*)dst, R, C);
-  count_launch(); TMPI_CHECK_LAUNCH("transpose_bf16"); ::tmpi::check_capture(st, "transpose_bf16");
-}
-
-// dgrad of a stride-1 convolution is a forward convolution of dy with the spatially flipped, channel-transposed filter:
-// wt[c][KH-1-r][KW-1-s][o] = w[o][r][s][c]     (tiny: runs once per layer per step)
-__global__ void conv_weight_flip_kernel(const __nv_bfloat16* __restrict__ w, __nv_bfloat16* __restrict__ wt, int O, int KH, int KW, int Cg) {
-  const int total = O * KH * KW * Cg;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-    const int o = i % O; int t = i / O;                      // iterate over the OUTPUT layout [c][r'][s'][o] (coalesced writes)
-    const int s2 = t % KW; t /= KW;
-    const int r2 = t % KH; const int c = t / KH;
-    wt[i] = w[(((long long)o * KH + (KH - 1 - r2)) * KW + (KW - 1 - s2)) * Cg + c];
-  }
-}
-void conv_weight_flip(const void* w, void* wt, int O, int KH, int KW, int Cg, cudaStream_t st) {
-  const int total = O * KH * KW * Cg;
-  conv_weight_flip_kernel<<<std::min(grid_for(total, 256), sm_count() * 8), 256, 0, st>>>((const __nv_bfloat16*)w, (__nv_bfloat16*)wt, O, KH, KW, Cg);
-  count_launch(); TMPI_CHECK_LAUNCH("conv_weight_flip"); ::tmpi::check_capture(st, "conv_weight_flip");
 }
 
 // ============================================================================ space-to-depth for strided few-channel convs
@@ -938,7 +1054,30 @@ __global__ void __launch_bounds__(256) space_to_depth_kernel(const __nv_bfloat16
     orow[(unsigned)(j * Cp)] = (chan_ok && col >= 0 && col < WC) ? irow[col] : zero;
   }
 }
-void space_to_depth(const void* x, void* y, int N, int H, int W, int C, int S, int Hs, int Ws, int Cp, int P, cudaStream_t st) {
+// fp32: one thread per output element (the row kernel above is limited to 256 packed channels)
+__global__ void space_to_depth_f32_kernel(const float* __restrict__ x, float* __restrict__ y, int N, int H, int W, int C, int S, int Hs, int Ws,
+                                          int Cp, int P) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long total = (long long)N * Hs * Ws * Cp;
+  if (idx >= total) return;
+  const int cp = (int)(idx % Cp); long long t = idx / Cp;
+  const int j = (int)(t % Ws); t /= Ws;
+  const int i = (int)(t % Hs); const int n = (int)(t / Hs);
+  float v = 0.f;
+  if (cp < S * S * C) {
+    const int c = cp % C, d = cp / C, dy = d / S, dx = d % S;
+    const int h = i * S + dy - P, w = j * S + dx - P;
+    if (h >= 0 && h < H && w >= 0 && w < W) v = x[(((long long)n * H + h) * W + w) * C + c];
+  }
+  y[idx] = v;
+}
+
+void space_to_depth(const void* x, void* y, int N, int H, int W, int C, int S, int Hs, int Ws, int Cp, int P, int f32, cudaStream_t st) {
+  if (f32) {
+    space_to_depth_f32_kernel<<<grid_for((long long)N * Hs * Ws * Cp, 256), 256, 0, st>>>((const float*)x, (float*)y, N, H, W, C, S, Hs, Ws, Cp, P);
+    count_launch(); TMPI_CHECK_LAUNCH("space_to_depth"); ::tmpi::check_capture(st, "space_to_depth");
+    return;
+  }
   if (Cp > 256) throw std::runtime_error("space_to_depth: more than 256 packed channels");
   const dim3 blk((unsigned)Cp, (unsigned)std::max(1, 256 / Cp));
   auto X = (const __nv_bfloat16*)x; auto Y = (__nv_bfloat16*)y;
@@ -948,7 +1087,8 @@ void space_to_depth(const void* x, void* y, int N, int H, int W, int C, int S, i
 }
 
 // w [O][KH][KW][C]  <->  ws [O][KHs][KWs][Cp]   with  ws[o, a, b, (dy*S+dx)*C + c] = w[o, S*a+dy, S*b+dx, c]  (0 outside the filter)
-// dir 0: pack bf16 filter (w -> ws);  dir 1: unpack fp32 gradient (gs -> g)
+// dir 0: pack the filter of storage type T (w -> ws);  dir 1: unpack the fp32 gradient (gs -> g)
+template <typename T>
 __global__ void s2d_filter_kernel(const void* __restrict__ src, void* __restrict__ dst, int O, int KH, int KW, int C, int S, int KHs, int KWs,
                                   int Cp, int dir) {
   if (dir == 0) {
@@ -957,13 +1097,13 @@ __global__ void s2d_filter_kernel(const void* __restrict__ src, void* __restrict
       const int cp = i % Cp; int t = i / Cp;
       const int b = t % KWs; t /= KWs;
       const int a = t % KHs; const int o = t / KHs;
-      __nv_bfloat16 v = f_to_bf16(0.f);
+      T v = from_f<T>(0.f);
       if (cp < S * S * C) {
         const int c = cp % C, d = cp / C, dy = d / S, dx = d % S;
         const int kh = a * S + dy, kw = b * S + dx;
-        if (kh < KH && kw < KW) v = reinterpret_cast<const __nv_bfloat16*>(src)[(((long long)o * KH + kh) * KW + kw) * C + c];
+        if (kh < KH && kw < KW) v = reinterpret_cast<const T*>(src)[(((long long)o * KH + kh) * KW + kw) * C + c];
       }
-      reinterpret_cast<__nv_bfloat16*>(dst)[i] = v;
+      reinterpret_cast<T*>(dst)[i] = v;
     }
   } else {
     const int total = O * KH * KW * C;
@@ -977,9 +1117,11 @@ __global__ void s2d_filter_kernel(const void* __restrict__ src, void* __restrict
     }
   }
 }
-void s2d_filter(const void* src, void* dst, int O, int KH, int KW, int C, int S, int KHs, int KWs, int Cp, int dir, cudaStream_t st) {
+void s2d_filter(const void* src, void* dst, int O, int KH, int KW, int C, int S, int KHs, int KWs, int Cp, int dir, int f32, cudaStream_t st) {
   const int total = dir == 0 ? O * KHs * KWs * Cp : O * KH * KW * C;
-  s2d_filter_kernel<<<std::min(grid_for(total, 256), sm_count() * 8), 256, 0, st>>>(src, dst, O, KH, KW, C, S, KHs, KWs, Cp, dir);
+  const int grid = std::min(grid_for(total, 256), sm_count() * 8);
+  if (f32) s2d_filter_kernel<float><<<grid, 256, 0, st>>>(src, dst, O, KH, KW, C, S, KHs, KWs, Cp, dir);
+  else s2d_filter_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(src, dst, O, KH, KW, C, S, KHs, KWs, Cp, dir);
   count_launch(); TMPI_CHECK_LAUNCH("s2d_filter"); ::tmpi::check_capture(st, "s2d_filter");
 }
 

@@ -2,7 +2,7 @@
 device pointers of torch tensors to the hand-written sm_90a kernels in ``csrc/``.
 
 GEMM-shaped work (FC forward/dgrad/wgrad; conv forward/dgrad/wgrad through an NHWC
-im2col gather) runs on ONE kernel, ``gemm_bf16`` (TMA → smem → ``wgmma`` →
+im2col gather) runs on ONE kernel, ``gemm`` (TMA → smem → ``wgmma`` →
 registers → fused epilogue, see ``csrc/gemm_wgmma.cu``).  Operand-major flags make
 transposed copies unnecessary:
 
@@ -99,9 +99,9 @@ def gemm(a, b, M, N, K, a_mn=False, b_mn=False, out=None, out_dtype=None, bias=N
         ldc = out.stride(0) if out.dim() == 2 else N
     if bias is not None:
         assert bias.dtype == torch.float32
-    L().gemm_bf16(a.data_ptr(), b.data_ptr(), out.data_ptr(), _p(bias), int(M), int(N), int(K), int(lda), int(ldb),
-                  int(ldc), int(bool(a_mn)), int(bool(b_mn)), int(out.dtype == BF16), int(bias_mode), int(bool(relu)),
-                  float(alpha), int(bn), int(splitk), _st(a), int(tf32))
+    L().gemm(a.data_ptr(), b.data_ptr(), out.data_ptr(), _p(bias), int(M), int(N), int(K), int(lda), int(ldb),
+             int(ldc), int(bool(a_mn)), int(bool(b_mn)), int(out.dtype == BF16), int(bias_mode), int(bool(relu)),
+             float(alpha), int(bn), int(splitk), int(tf32), _st(a))
     return out
 
 
@@ -113,17 +113,15 @@ def linear_bias_act(x, w, b, relu=True):
     xa, lda = _rows8(x2)
     wa, ldb = _rows8(_bf(w))
     bias = b.float() if b is not None and b.dtype != torch.float32 else b
-    if FC_SPLITK and B_ <= 128 and I >= 1024 and O % 8 == 0 and _is32(x2):
-        acc = gemm(xa, wa, B_, O, I, lda=lda, ldb=ldb)                    # fp32 split-K accumulation, finished in place
-        L().bias_act_f32(acc.data_ptr(), _p(bias), acc.data_ptr(), int(B_), int(O), int(bool(relu)), _st(x2))
-        return acc
     if FC_SPLITK and B_ <= 128 and I >= 1024 and O % 8 == 0:
         # small-batch FC forward is a weight stream: one m-tile, so the parallelism comes from n-tiles x split-K (fp32
-        # reductions into a scratch tile), followed by a tiny bias + ReLU + bf16 pass.  (The fused-epilogue kernel needs
-        # 32-wide tiles to fill the machine and then re-reads the activations 128 times through L2: 37 us vs 13 us for fc6.)
+        # reductions into a scratch tile), followed by a tiny bias + ReLU (+ bf16 cast) pass; fp32 output is finished in
+        # place.  (The fused-epilogue kernel needs 32-wide tiles to fill the machine and then re-reads the activations 128
+        # times through L2: 37 us vs 13 us for fc6.)
+        f32 = _is32(x2)
         acc = gemm(xa, wa, B_, O, I, out_dtype=torch.float32, lda=lda, ldb=ldb)
-        y = torch.empty((B_, O), dtype=BF16, device=x2.device)
-        L().bias_act_cast(acc.data_ptr(), _p(bias), y.data_ptr(), int(B_), int(O), int(bool(relu)), _st(x2))
+        y = acc if f32 else torch.empty((B_, O), dtype=BF16, device=x2.device)
+        L().bias_act(acc.data_ptr(), _p(bias), y.data_ptr(), int(B_), int(O), int(bool(relu)), int(f32), _st(x2))
         return y
     return gemm(xa, wa, B_, O, I, bias=bias, bias_mode=1 if b is not None else 0, relu=relu, lda=lda, ldb=ldb)
 
@@ -134,21 +132,13 @@ def _mask_and_bias_grad(dy, y, relu, db_out, R, C, ld, need_db=True):
     if not need_db and not relu and ld == C:
         return dy, None                                    # bias-free linear conv (a BatchNormal follows): nothing to do
     db = db_out if db_out is not None else torch.empty(C, dtype=torch.float32, device=dev)
-    contiguous = (ld == C)
-    if _is32(dy):
-        if relu or not contiguous:
-            dym = torch.empty((R, C), dtype=F32, device=dev)
-            L().relu_bias_bwd2_f32(dy.data_ptr(), _p(y), dym.data_ptr(), db.data_ptr(), 0, int(C), int(R), int(C), int(ld), int(bool(relu)), _st(dy))
-        else:
-            dym = dy
-            L().relu_bias_bwd2_f32(dy.data_ptr(), 0, 0, db.data_ptr(), 0, int(C), int(R), int(C), int(ld), 0, _st(dy))
-        return dym, db
-    if relu or not contiguous:
-        dym = torch.empty((R, C), dtype=BF16, device=dev)
-        L().relu_bias_bwd(dy.data_ptr(), _p(y), dym.data_ptr(), db.data_ptr(), int(R), int(C), int(ld), int(bool(relu)), _st(dy))
+    if relu or ld != C:
+        dym = torch.empty((R, C), dtype=dy.dtype, device=dev)
+        L().relu_bias_bwd(dy.data_ptr(), _p(y), dym.data_ptr(), db.data_ptr(), 0, int(C), int(R), int(C), int(ld), int(bool(relu)),
+                          int(_is32(dy)), _st(dy))
     else:
         dym = dy
-        L().relu_bias_bwd(dy.data_ptr(), 0, 0, db.data_ptr(), int(R), int(C), int(ld), 0, _st(dy))
+        L().relu_bias_bwd(dy.data_ptr(), 0, 0, db.data_ptr(), 0, int(C), int(R), int(C), int(ld), 0, int(_is32(dy)), _st(dy))
     return dym, db
 
 
@@ -222,8 +212,7 @@ def _im2col(x, c_off, Cg, KH, KW, Ho, Wo, s, p):
         return x.view(N * H * W, Ct), Ct, K                     # 1x1 conv: the activation IS the matrix
     Kp = (K + 7) // 8 * 8
     col = torch.empty((N * Ho * Wo, Kp), dtype=x.dtype, device=x.device)
-    fn = L().im2col_f32 if _is32(x) else L().im2col
-    fn(x.data_ptr(), col.data_ptr(), N, H, W, Ct, int(c_off), int(Cg), KH, KW, Ho, Wo, int(s), int(p), Kp, _st(x))
+    L().im2col(x.data_ptr(), col.data_ptr(), N, H, W, Ct, int(c_off), int(Cg), KH, KW, Ho, Wo, int(s), int(p), Kp, int(_is32(x)), _st(x))
     return col, Kp, K
 
 
@@ -234,7 +223,7 @@ def _w2d(w, K, Kp):
     if Kp == K and w2.data_ptr() % 16 == 0:
         return w2
     wp = torch.empty((O, Kp), dtype=w2.dtype, device=w.device)
-    (L().pad_rows_f32 if _is32(w2) else L().pad_rows)(w2.data_ptr(), wp.data_ptr(), O, K, K, Kp, _st(w))
+    L().pad_rows(w2.data_ptr(), wp.data_ptr(), O, K, K, Kp, int(_is32(w2)), _st(w))
     return wp
 
 
@@ -261,7 +250,7 @@ def _conv_fwd_group(x, w, b, y, o_off, c_off, Cg, s, p, relu):
         # implicit GEMM: the activation tile is gathered by TMA im2col loads inside the kernel — no col matrix
         yp = y.data_ptr() + o_off * y.element_size()
         L().conv_fprop(x.data_ptr(), wb.data_ptr(), yp, _p(b), N, H, W, Ct, int(c_off), int(Cg), KH, KW, Ho, Wo, int(s), int(p),
-                       Og, Ot, int(bool(relu)), int(not _is32(x)), 0, _st(x), int(_is32(x)))
+                       Og, Ot, int(bool(relu)), 0, int(_is32(x)), _st(x))
         return None
     col, Kp, K = _im2col(x, c_off, Cg, KH, KW, Ho, Wo, s, p)
     w2 = _w2d(w, K, Kp)
@@ -293,18 +282,14 @@ def _conv_s2d_fwd(x, w, b, relu, g):
     N, H, W, C = x.shape
     O, KH, KW, _ = w.shape
     dev = x.device
-    f32 = _is32(x)
+    f32 = int(_is32(x))
     xs = torch.empty((N, Hs, Ws, Cp), dtype=x.dtype, device=dev)
     ws = torch.empty((O, KHs, KWs, Cp), dtype=x.dtype, device=dev)
-    if f32:
-        L().space_to_depth_f32(x.data_ptr(), xs.data_ptr(), N, H, W, C, S, Hs, Ws, Cp, P0, _st(x))
-        L().s2d_filter_pack_f32(_bf(w).contiguous().data_ptr(), ws.data_ptr(), O, KH, KW, C, S, KHs, KWs, Cp, _st(x))
-    else:
-        L().space_to_depth(x.data_ptr(), xs.data_ptr(), N, H, W, C, S, Hs, Ws, Cp, P0, _st(x))
-        L().s2d_filter(_bf(w).contiguous().data_ptr(), ws.data_ptr(), O, KH, KW, C, S, KHs, KWs, Cp, 0, _st(x))
+    L().space_to_depth(x.data_ptr(), xs.data_ptr(), N, H, W, C, S, Hs, Ws, Cp, P0, f32, _st(x))
+    L().s2d_filter(_bf(w).contiguous().data_ptr(), ws.data_ptr(), O, KH, KW, C, S, KHs, KWs, Cp, 0, f32, _st(x))
     y = torch.empty((N, Ho, Wo, O), dtype=x.dtype, device=dev)
     L().conv_fprop(xs.data_ptr(), ws.data_ptr(), y.data_ptr(), _p(b), N, Hs, Ws, Cp, 0, Cp, KHs, KWs, Ho, Wo, 1, 0, O, O,
-                   int(bool(relu)), int(not f32), 0, _st(x), int(f32))
+                   int(bool(relu)), 0, f32, _st(x))
     return y, xs
 
 
@@ -319,9 +304,10 @@ def _conv_s2d_bwd(xs, w, y, dy, relu, g, dw_out, db_out, pre_masked=False):
     else:
         dym, db = _mask_and_bias_grad(dy.view(M, O), y.view(M, O), relu, db_out.view(-1) if db_out is not None else None, M, O, O)
     dws = torch.empty((O, KHs, KWs, Cp), dtype=torch.float32, device=dev)
-    L().conv_wgrad(dym.data_ptr(), xs.data_ptr(), dws.data_ptr(), N, Hs, Ws, Cp, 0, Cp, KHs, KWs, Ho, Wo, 1, 0, O, O, _st(xs), int(_is32(xs)))
+    f32 = int(_is32(xs))
+    L().conv_wgrad(dym.data_ptr(), xs.data_ptr(), dws.data_ptr(), N, Hs, Ws, Cp, 0, Cp, KHs, KWs, Ho, Wo, 1, 0, O, O, f32, _st(xs))
     dw = dw_out if dw_out is not None else torch.empty((O, KH, KW, C), dtype=torch.float32, device=dev)
-    L().s2d_filter(dws.data_ptr(), dw.data_ptr(), O, KH, KW, C, S, KHs, KWs, Cp, 1, _st(xs))
+    L().s2d_filter(dws.data_ptr(), dw.data_ptr(), O, KH, KW, C, S, KHs, KWs, Cp, 1, f32, _st(xs))
     return dw, db
 
 
@@ -351,12 +337,11 @@ def conv2d_group2_bias_act(x, w0, b0, w1, b1, stride, pad, relu, return_cols=Fal
     Ho, Wo = _out_hw(H, W, KH, KW, stride, pad)
     y = torch.empty((N, Ho, Wo, 2 * Og), dtype=x.dtype, device=x.device)
     wb0, wb1 = _bf(w0), _bf(w1)
-    es, f32 = x.element_size(), _is32(x)
+    es, f32 = x.element_size(), int(_is32(x))
     if GROUP2_FUSED and _implicit_ok(x, wb0, 0, Cg, 2 * Og, 0) and _implicit_ok(x, wb1, Cg, Cg, 2 * Og, Og) and (b0 is None) == (b1 is None):
         # both groups in ONE persistent launch: their tiles fill the SMs together instead of two under-filled waves
         L().conv_fprop2(x.data_ptr(), wb0.data_ptr(), wb1.data_ptr(), y.data_ptr(), y.data_ptr() + Og * es, _p(b0), _p(b1), N, H, W, C, 0,
-                        int(Cg), int(Cg), KH, KW, Ho, Wo, int(stride), int(pad), Og, 2 * Og, int(bool(relu)), int(not f32), 0, _st(x),
-                        int(f32))
+                        int(Cg), int(Cg), KH, KW, Ho, Wo, int(stride), int(pad), Og, 2 * Og, int(bool(relu)), 0, f32, _st(x))
         return (y, [None, None]) if return_cols else y
     cols = [_conv_fwd_group(x, w0, b0, y, 0, 0, Cg, stride, pad, relu),
             _conv_fwd_group(x, w1, b1, y, Og, Cg, Cg, stride, pad, relu)]
@@ -383,21 +368,20 @@ def _conv_bwd_group(x, w, y, dy, dx, o_off, c_off, Cg, s, p, relu, need_dx, dw_o
         # ---- implicit GEMM backward: wgrad gathers im2col(x) by TMA; dgrad (stride 1) is a forward conv of dy with the
         # flipped / transposed filter, written straight into dx's channel slice.
         dw = dw_out if dw_out is not None else torch.empty((Og, KH, KW, Cg), dtype=torch.float32, device=dev)
-        es, f32 = x.element_size(), _is32(x)
+        es, f32 = x.element_size(), int(_is32(x))
         L().conv_wgrad(dym.data_ptr(), x.data_ptr(), dw.data_ptr(), N, H, W, Ct, int(c_off), int(Cg), KH, KW, Ho, Wo, int(s), int(p),
-                       Og, int(ldy), _st(x), int(f32))
+                       Og, int(ldy), f32, _st(x))
         if need_dx:
             if s == 1:
                 # dgrad = forward conv of dy with the mirrored, transposed filter — which the kernel's TMA loads read straight
                 # out of the forward weights (MN-major boxes of the mirrored tap): no flipped copy
                 L().conv_fprop(dym.data_ptr() - dy_coff * es, wb.data_ptr(), dx.data_ptr() + c_off * es, 0, N, Ho, Wo, int(ldy), int(dy_coff),
-                               Og, KH, KW, H, W, 1, KH - 1 - int(p), int(Cg), Ct, 0, int(not f32), 1, _st(x), int(f32))
+                               Og, KH, KW, H, W, 1, KH - 1 - int(p), int(Cg), Ct, 0, 1, f32, _st(x))
             else:
                 colK = KH * KW * Cg
                 Kp = (colK + 7) // 8 * 8
                 dcol = gemm(dym, _w2d(w, colK, Kp), M, Kp, Og, b_mn=True, lda=ldy, ldb=Kp)
-                (L().col2im_f32 if f32 else L().col2im)(dcol.data_ptr(), dx.data_ptr(), N, H, W, Ct, int(c_off), int(Cg), KH, KW, Ho, Wo,
-                                                        int(s), int(p), Kp, _st(x))
+                L().col2im(dcol.data_ptr(), dx.data_ptr(), N, H, W, Ct, int(c_off), int(Cg), KH, KW, Ho, Wo, int(s), int(p), Kp, f32, _st(x))
         return dw, db
     col, Kp, K = col if col is not None else _im2col(x, c_off, Cg, KH, KW, Ho, Wo, s, p)   # forward's matrix is reused
     dw = dw_out if dw_out is not None else torch.empty((Og, KH, KW, Cg), dtype=torch.float32, device=dev)
@@ -410,8 +394,8 @@ def _conv_bwd_group(x, w, y, dy, dx, o_off, c_off, Cg, s, p, relu, need_dx, dw_o
             gemm(dym, w2, M, Kp, Og, b_mn=True, out=dx.view(M, Ct), lda=ldy, ldb=Kp, ldc=Ct)
         else:
             dcol = gemm(dym, w2, M, Kp, Og, b_mn=True, lda=ldy, ldb=Kp)
-            (L().col2im_f32 if _is32(x) else L().col2im)(dcol.data_ptr(), dx.data_ptr(), N, H, W, Ct, int(c_off), int(Cg), KH, KW, Ho, Wo,
-                                                         int(s), int(p), Kp, _st(x))
+            L().col2im(dcol.data_ptr(), dx.data_ptr(), N, H, W, Ct, int(c_off), int(Cg), KH, KW, Ho, Wo, int(s), int(p), Kp,
+                       int(_is32(x)), _st(x))
     return dw, db
 
 
@@ -460,20 +444,20 @@ def conv2d_group2_bias_act_bwd(x, w0, w1, y, dy, stride, pad, relu, need_dx, out
         dev = x.device
         db0 = outs[1] if outs[1] is not None else torch.empty(Og, dtype=torch.float32, device=dev)
         db1 = outs[3] if outs[3] is not None else torch.empty(Og, dtype=torch.float32, device=dev)
-        es, f32 = x.element_size(), _is32(x)
+        es, f32 = x.element_size(), int(_is32(x))
         if pre_masked:
             dym = dy
         else:
             dym = torch.empty((M, Ot), dtype=x.dtype, device=dev)
-            (L().relu_bias_bwd2_f32 if f32 else L().relu_bias_bwd2)(dy.data_ptr(), y.data_ptr(), dym.data_ptr(), db0.data_ptr(), db1.data_ptr(),
-                                                                     int(Og), int(M), int(Ot), int(Ot), int(bool(relu)), _st(x))
+            L().relu_bias_bwd(dy.data_ptr(), y.data_ptr(), dym.data_ptr(), db0.data_ptr(), db1.data_ptr(), int(Og), int(M), int(Ot), int(Ot),
+                              int(bool(relu)), f32, _st(x))
         dw0 = outs[0] if outs[0] is not None else torch.empty((Og, KH, KW, Cg), dtype=torch.float32, device=dev)
         dw1 = outs[2] if outs[2] is not None else torch.empty((Og, KH, KW, Cg), dtype=torch.float32, device=dev)
         L().conv_wgrad2(dym.data_ptr(), dym.data_ptr() + Og * es, x.data_ptr(), dw0.data_ptr(), dw1.data_ptr(), N, H, W, Ct, 0, int(Cg), int(Cg),
-                        KH, KW, Ho, Wo, int(stride), int(pad), Og, int(Ot), _st(x), int(f32))
+                        KH, KW, Ho, Wo, int(stride), int(pad), Og, int(Ot), f32, _st(x))
         if need_dx:
             L().conv_fprop2(dym.data_ptr(), wb0.data_ptr(), wb1.data_ptr(), dx.data_ptr(), dx.data_ptr() + Cg * es, 0, 0, N, Ho, Wo, int(Ot), 0,
-                            int(Og), int(Og), KH, KW, H, W, 1, KH - 1 - int(pad), int(Cg), Ct, 0, int(not f32), 1, _st(x), int(f32))
+                            int(Og), int(Og), KH, KW, H, W, 1, KH - 1 - int(pad), int(Cg), Ct, 0, 1, f32, _st(x))
         return dx, (dw0, db0, dw1, db1)
     dw0, db0 = _conv_bwd_group(x, w0, y, dy, dx, 0, 0, Cg, stride, pad, relu, need_dx, outs[0], outs[1],
                                col=cols[0] if cols else None, pre_masked=pre_masked)
@@ -490,8 +474,8 @@ def pool2d_fwd(x, ksize, stride, pad, mode):
     y = torch.empty((N, Ho, Wo, C), dtype=x.dtype, device=x.device)
     is_max = mode == "max"
     arg = torch.empty((N, Ho, Wo, C), dtype=torch.uint8, device=x.device) if is_max else None
-    (L().pool_fwd_f32 if _is32(x) else L().pool_fwd)(x.data_ptr(), y.data_ptr(), _p(arg), N, H, W, C, Ho, Wo, int(ksize), int(stride),
-                                                     int(pad), int(is_max), _st(x))
+    L().pool_fwd(x.data_ptr(), y.data_ptr(), _p(arg), N, H, W, C, Ho, Wo, int(ksize), int(stride), int(pad), int(is_max), int(_is32(x)),
+                 _st(x))
     return y, arg
 
 
@@ -500,8 +484,8 @@ def pool2d_bwd_arg(dy, arg, xshape, ksize, stride, pad, mode):
     N, H, W, C = xshape
     Ho, Wo = dy.shape[1], dy.shape[2]
     dx = torch.empty(tuple(xshape), dtype=dy.dtype, device=dy.device)
-    (L().pool_bwd_f32 if _is32(dy) else L().pool_bwd)(dy.data_ptr(), _p(arg), dx.data_ptr(), N, H, W, C, Ho, Wo, int(ksize), int(stride),
-                                                      int(pad), int(mode == "max"), _st(dy))
+    L().pool_bwd(dy.data_ptr(), _p(arg), dx.data_ptr(), N, H, W, C, Ho, Wo, int(ksize), int(stride), int(pad), int(mode == "max"),
+                 int(_is32(dy)), _st(dy))
     return dx
 
 
@@ -509,8 +493,7 @@ def lrn(x, n=5, k=2.0, alpha=1e-4, beta=0.75):
     x = _bf(x).contiguous()
     C = x.shape[-1]
     y = torch.empty_like(x)
-    (L().lrn_fwd_f32 if _is32(x) else L().lrn_fwd)(x.data_ptr(), y.data_ptr(), x.numel() // C, C, int(n), float(k), float(alpha),
-                                                   float(beta), _st(x))
+    L().lrn_fwd(x.data_ptr(), y.data_ptr(), x.numel() // C, C, int(n), float(k), float(alpha), float(beta), int(_is32(x)), _st(x))
     return y, None
 
 
@@ -519,8 +502,8 @@ def lrn_bwd(x, dy, n=5, k=2.0, alpha=1e-4, beta=0.75):
     dy = _bf(dy).contiguous()
     C = x.shape[-1]
     dx = torch.empty_like(x)
-    (L().lrn_bwd_f32 if _is32(x) else L().lrn_bwd)(x.data_ptr(), dy.data_ptr(), dx.data_ptr(), x.numel() // C, C, int(n), float(k),
-                                                   float(alpha), float(beta), _st(x))
+    L().lrn_bwd(x.data_ptr(), dy.data_ptr(), dx.data_ptr(), x.numel() // C, C, int(n), float(k), float(alpha), float(beta), int(_is32(x)),
+                _st(x))
     return dx
 
 
@@ -530,15 +513,15 @@ def dropout_fwd(x, p_drop, layer_id):
     y = torch.empty_like(x)
     mask = torch.empty(x.shape, dtype=torch.uint8, device=x.device)
     step = step_counter(x.device)
-    (L().dropout_fwd_f32 if _is32(x) else L().dropout_fwd)(x.data_ptr(), y.data_ptr(), mask.data_ptr(), x.numel(), float(p_drop),
-                                                           int(rng_state()["seed"]), int(layer_id), step.data_ptr(), _st(x))
+    L().dropout_fwd(x.data_ptr(), y.data_ptr(), mask.data_ptr(), x.numel(), float(p_drop), int(rng_state()["seed"]), int(layer_id),
+                    step.data_ptr(), int(_is32(x)), _st(x))
     return y, mask
 
 
 def dropout_bwd(dy, mask):
     dy = _bf(dy).contiguous()
     dx = torch.empty_like(dy)
-    (L().dropout_bwd_f32 if _is32(dy) else L().dropout_bwd)(dy.data_ptr(), mask.data_ptr(), dx.data_ptr(), dy.numel(), _st(dy))
+    L().dropout_bwd(dy.data_ptr(), mask.data_ptr(), dx.data_ptr(), dy.numel(), int(_is32(dy)), _st(dy))
     return dx
 
 
@@ -550,8 +533,8 @@ def softmax_xent(logits, labels, weight=1.0):
     dl = torch.empty_like(lg)
     rowstat = torch.empty((B_, 3), dtype=torch.float32, device=lg.device)
     out3 = torch.empty(3, dtype=torch.float32, device=lg.device)
-    (L().softmax_xent_f32 if _is32(lg) else L().softmax_xent)(lg.data_ptr(), labels.data_ptr(), dl.data_ptr(), rowstat.data_ptr(),
-                                                              out3.data_ptr(), B_, C, float(weight), _st(lg))
+    L().softmax_xent(lg.data_ptr(), labels.data_ptr(), dl.data_ptr(), rowstat.data_ptr(), out3.data_ptr(), B_, C, float(weight),
+                     int(_is32(lg)), _st(lg))
     return out3[0], out3[1], out3[2], dl
 
 

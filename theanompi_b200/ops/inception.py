@@ -68,7 +68,7 @@ class _InceptFn(torch.autograd.Function):
             e = torch.cuda.Event(); e.record(s2); joins.append(e)
         with torch.cuda.stream(s3):
             s3.wait_event(fork)
-            (L.pool_fwd_f32 if ci._is32(x) else L.pool_fwd)(x.data_ptr(), pl.data_ptr(), arg.data_ptr(), N, H, W, C, H, W, 3, 1, 1, 1, ci._st(x))
+            L.pool_fwd(x.data_ptr(), pl.data_ptr(), arg.data_ptr(), N, H, W, C, H, W, 3, 1, 1, 1, int(ci._is32(x)), ci._st(x))
             ci._conv_fwd_group(pl, cw(wpj), bpj, y, n1 + n3 + n5, 0, C, 1, 0, True)
             e = torch.cuda.Event(); e.record(s3); joins.append(e)
         for e in joins:
@@ -111,7 +111,7 @@ class _InceptFn(torch.autograd.Function):
             s3.wait_event(fork)
             out["pj"] = ci._conv_bwd_group(pl, cw(wpj), y, dy, dpl, n1 + n3 + n5, 0, C, 1, 0, True, True, _gout(wpj), _gout(bpj))
             if need_dx:
-                (L.pool_bwd_f32 if ci._is32(x) else L.pool_bwd)(dpl.data_ptr(), arg.data_ptr(), dxd.data_ptr(), N, H, W, C, H, W, 3, 1, 1, 1, ci._st(x))
+                L.pool_bwd(dpl.data_ptr(), arg.data_ptr(), dxd.data_ptr(), N, H, W, C, H, W, 3, 1, 1, 1, int(ci._is32(x)), ci._st(x))
             e = torch.cuda.Event(); e.record(s3); joins.append(e)
         for e in joins:
             main.wait_event(e)
