@@ -88,9 +88,16 @@ void dropout_bwd(const void* dy, const void* mask, void* dx, long long n, int f3
 void advance_step(void* step, cudaStream_t st);
 void softmax_xent(const void* logits, const void* labels, void* dlogits, void* rowstat, void* out3, int B, int C, float weight, int f32,
                   cudaStream_t st);
-void relu_bias_bwd(const void* dy, const void* y, void* dym, void* db, void* db1, int c_split, long long R, int C, long long ld, int relu,
-                   int f32, cudaStream_t st);
-void bias_act(const void* acc, const void* bias, void* y, int R, int C, int relu, int f32, cudaStream_t st);
+// act: 0 none, 1 ReLU, 2 leaky ReLU (negative slope `slope`), 3 sigmoid (ACT_* in common.cuh)
+void relu_bias_bwd(const void* dy, const void* y, void* dym, void* db, void* db1, int c_split, long long R, int C, long long ld, int act,
+                   float slope, int f32, cudaStream_t st);
+void bias_act(const void* acc, const void* bias, void* y, int R, int C, int act, float slope, int f32, cudaStream_t st);
+// transposed-convolution forward: y[N,H,W,C] = act(col2im(dcol) + bias), dcol = x[N*Hi*Wi, Cin] · W[Cin, KH*KW*C] (row pitch ldcol);
+// channels >= c_real are written as zeros
+void col2im_bias_act(const void* dcol, void* y, const float* bias, int N, int H, int W, int C, int KH, int KW, int Hi, int Wi, int s, int p,
+                     long long ldcol, int act, float slope, int c_real, int f32, cudaStream_t st);
+void gan_loss(const void* scores, void* dscores, void* out, int B, int kind, float a, int f32, cudaStream_t st);
+void uniform_noise(void* out, long long n, unsigned long long seed, int stream, const void* step, int f32, cudaStream_t st);
 // bf16 only (packed-bf16 compares)
 void maxpool_relu_bias_bwd(const void* dyp, const void* arg, const void* y, void* dym, void* db0, void* db1, int c_split, int N, int H,
                            int W, int C, int Ho, int Wo, int k, int s, int p, cudaStream_t st);
@@ -104,9 +111,10 @@ void crop_mirror_norm(const void* x, int in_kind, const void* mean, int mean_mod
 
 // ---- bn_kernels.cu: batch norm (+ residual)(+ ReLU) forward / backward, residual add  (f32: fp32 activations, else bf16)
 void bn_forward(const void* x, const void* res, void* y, const void* gamma, const void* beta, void* mean, void* rstd, void* run_mean,
-                void* run_var, void* scratch, long long R, int C, float momentum, float eps, int training, int relu, int f32, cudaStream_t st);
+                void* run_var, void* scratch, long long R, int C, float momentum, float eps, int training, int act, float slope, int f32,
+                cudaStream_t st);
 void bn_backward(const void* x, const void* dy, const void* y, void* dx, void* dres, const void* gamma, const void* mean, const void* rstd,
-                 void* dgamma, void* dbeta, void* scratch, long long R, int C, int relu, int f32, cudaStream_t st);
+                 void* dgamma, void* dbeta, void* scratch, long long R, int C, int act, float slope, int f32, cudaStream_t st);
 void add_tensors(const void* a, const void* b, void* y, long long n, int f32, cudaStream_t st);
 void add4_tensors(const void* a, const void* b, const void* c, const void* d, void* y, long long n, int f32, cudaStream_t st);
 
@@ -125,6 +133,8 @@ void sgd_flat(void* W, const void* G, void* U, void* H, const void* block_group,
               int nesterov, float inv_k, long long lo, long long hi, int filter, cudaStream_t st);
 void adam_flat(void* W, const void* G, void* M, void* V, void* H, const void* block_group, const GroupTable& tab, const void* lr_ptr, void* step,
                float b1, float b2, float eps, long long lo, long long hi, cudaStream_t st);
+void rmsprop_flat(void* W, const void* G, void* V, void* H, const void* block_group, const GroupTable& tab, const void* lr_ptr, float alpha,
+                  float eps, float clip, long long lo, long long hi, cudaStream_t st);
 void fused_allreduce_sgd(const FusedArgs& a, int algo, int max_blocks, cudaStream_t st);
 // every rank pushes the fp32 master weights of the slice it owns in the two-shot partition of [lo, hi) to all peers
 void push_master_slices(const FusedArgs& a, int max_blocks, cudaStream_t st);

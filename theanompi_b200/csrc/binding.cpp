@@ -97,10 +97,17 @@ PYBIND11_MODULE(_tmpi_native, m) {
   m.def("maxpool_relu_bias_bwd", [](ptr_t dyp, ptr_t arg, ptr_t y, ptr_t dym, ptr_t db0, ptr_t db1, int c_split, int N, int H, int W, int C,
                                     int Ho, int Wo, int k, int s, int p, ptr_t st) {
     maxpool_relu_bias_bwd(P(dyp), P(arg), P(y), P(dym), P(db0), P(db1), c_split, N, H, W, C, Ho, Wo, k, s, p, S(st)); });
-  m.def("relu_bias_bwd", [](ptr_t dy, ptr_t y, ptr_t dym, ptr_t db, ptr_t db1, int c_split, long long R, int C, long long ld, int relu, int f32,
-                            ptr_t st) { relu_bias_bwd(P(dy), P(y), P(dym), P(db), P(db1), c_split, R, C, ld, relu, f32, S(st)); });
-  m.def("bias_act", [](ptr_t acc, ptr_t bias, ptr_t y, int R, int C, int relu, int f32, ptr_t st) {
-    bias_act(P(acc), P(bias), P(y), R, C, relu, f32, S(st)); });
+  m.def("relu_bias_bwd", [](ptr_t dy, ptr_t y, ptr_t dym, ptr_t db, ptr_t db1, int c_split, long long R, int C, long long ld, int act, float slope,
+                            int f32, ptr_t st) { relu_bias_bwd(P(dy), P(y), P(dym), P(db), P(db1), c_split, R, C, ld, act, slope, f32, S(st)); });
+  m.def("bias_act", [](ptr_t acc, ptr_t bias, ptr_t y, int R, int C, int act, float slope, int f32, ptr_t st) {
+    bias_act(P(acc), P(bias), P(y), R, C, act, slope, f32, S(st)); });
+  m.def("col2im_bias_act", [](ptr_t dcol, ptr_t y, ptr_t bias, int N, int H, int W, int C, int KH, int KW, int Hi, int Wi, int s, int p,
+                              long long ldcol, int act, float slope, int c_real, int f32, ptr_t st) {
+    col2im_bias_act(P(dcol), P(y), (const float*)P(bias), N, H, W, C, KH, KW, Hi, Wi, s, p, ldcol, act, slope, c_real, f32, S(st)); });
+  m.def("gan_loss", [](ptr_t scores, ptr_t dscores, ptr_t out, int B, int kind, float a, int f32, ptr_t st) {
+    gan_loss(P(scores), P(dscores), P(out), B, kind, a, f32, S(st)); });
+  m.def("uniform_noise", [](ptr_t out, long long n, unsigned long long seed, int stream, ptr_t step, int f32, ptr_t st) {
+    uniform_noise(P(out), n, seed, stream, P(step), f32, S(st)); });
   m.def("im2col", [](ptr_t x, ptr_t col, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho, int Wo, int s, int p,
                      long long ldcol, int f32, ptr_t st) { im2col(P(x), P(col), N, H, W, Ctot, c_off, Cg, KH, KW, Ho, Wo, s, p, ldcol, f32, S(st)); });
   m.def("col2im", [](ptr_t dcol, ptr_t dx, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho, int Wo, int s, int p,
@@ -113,12 +120,12 @@ PYBIND11_MODULE(_tmpi_native, m) {
 
   // ---------------------------------------------------------------- batch norm / residual
   m.def("bn_forward", [](ptr_t x, ptr_t res, ptr_t y, ptr_t gamma, ptr_t beta, ptr_t mean, ptr_t rstd, ptr_t run_mean, ptr_t run_var, ptr_t scratch,
-                         long long R, int C, float momentum, float eps, int training, int relu, int f32, ptr_t st) {
-    bn_forward(P(x), P(res), P(y), P(gamma), P(beta), P(mean), P(rstd), P(run_mean), P(run_var), P(scratch), R, C, momentum, eps, training, relu,
-               f32, S(st)); });
+                         long long R, int C, float momentum, float eps, int training, int act, float slope, int f32, ptr_t st) {
+    bn_forward(P(x), P(res), P(y), P(gamma), P(beta), P(mean), P(rstd), P(run_mean), P(run_var), P(scratch), R, C, momentum, eps, training, act,
+               slope, f32, S(st)); });
   m.def("bn_backward", [](ptr_t x, ptr_t dy, ptr_t y, ptr_t dx, ptr_t dres, ptr_t gamma, ptr_t mean, ptr_t rstd, ptr_t dgamma, ptr_t dbeta,
-                          ptr_t scratch, long long R, int C, int relu, int f32, ptr_t st) {
-    bn_backward(P(x), P(dy), P(y), P(dx), P(dres), P(gamma), P(mean), P(rstd), P(dgamma), P(dbeta), P(scratch), R, C, relu, f32, S(st)); });
+                          ptr_t scratch, long long R, int C, int act, float slope, int f32, ptr_t st) {
+    bn_backward(P(x), P(dy), P(y), P(dx), P(dres), P(gamma), P(mean), P(rstd), P(dgamma), P(dbeta), P(scratch), R, C, act, slope, f32, S(st)); });
   m.def("add4_tensors", [](ptr_t a, ptr_t b, ptr_t c, ptr_t d, ptr_t y, long long n, int f32, ptr_t st) {
     add4_tensors(P(a), P(b), P(c), P(d), P(y), n, f32, S(st)); });
   m.def("add_tensors", [](ptr_t a, ptr_t b, ptr_t y, long long n, int f32, ptr_t st) { add_tensors(P(a), P(b), P(y), n, f32, S(st)); });
@@ -143,6 +150,9 @@ PYBIND11_MODULE(_tmpi_native, m) {
   m.def("adam_flat", [](ptr_t W, ptr_t G, ptr_t M, ptr_t V, ptr_t H, ptr_t block_group, std::vector<float> lr_mult, std::vector<float> wd,
                         std::vector<int> exch, ptr_t lr_ptr, ptr_t step, float b1, float b2, float eps, long long lo, long long hi, ptr_t st) {
     adam_flat(P(W), P(G), P(M), P(V), P(H), P(block_group), make_table(lr_mult, wd, exch), P(lr_ptr), P(step), b1, b2, eps, lo, hi, S(st)); });
+  m.def("rmsprop_flat", [](ptr_t W, ptr_t G, ptr_t V, ptr_t H, ptr_t block_group, std::vector<float> lr_mult, std::vector<float> wd,
+                           std::vector<int> exch, ptr_t lr_ptr, float alpha, float eps, float clip, long long lo, long long hi, ptr_t st) {
+    rmsprop_flat(P(W), P(G), P(V), P(H), P(block_group), make_table(lr_mult, wd, exch), P(lr_ptr), alpha, eps, clip, lo, hi, S(st)); });
   m.def("easgd_elastic", [](ptr_t w, ptr_t h, ptr_t center, float alpha, long long n, int max_blocks, ptr_t st, int lockfree) {
     easgd_elastic(P(w), P(h), P(center), alpha, n, max_blocks, lockfree, S(st)); },
     py::arg("w"), py::arg("h"), py::arg("center"), py::arg("alpha"), py::arg("n"), py::arg("max_blocks"), py::arg("st"), py::arg("lockfree") = 0);

@@ -19,11 +19,12 @@ static inline int grid1(long long n, int block) { return (int)((n + block - 1) /
 
 // ---------------------------------------------------------------- column reductions over row slabs
 // MODE 0: a = Σ x, b = Σ x²            (forward statistics)
-// MODE 1: a = Σ g, b = Σ g·x̂          (backward: g = dy ⊙ [y > 0] when relu)
-template <typename T, int MODE>
+// MODE 1: a = Σ g, b = Σ g·x̂          (backward: g = dy ⊙ [y > 0] when relu; g = act'(y) ⊙ dy for ACT_LEAKY / ACT_SIGMOID)
+template <typename T, int MODE, int ACT>
 __global__ void __launch_bounds__(256) bn_colreduce_kernel(const T* __restrict__ x, const T* __restrict__ dy, const T* __restrict__ y,
                                                           const float* __restrict__ mean, const float* __restrict__ rstd, float* __restrict__ out_a,
-                                                          float* __restrict__ out_b, long long R, int C, int relu, int VT, int rows_per_cta) {
+                                                          float* __restrict__ out_b, long long R, int C, int relu, int VT, int rows_per_cta,
+                                                          float slope) {
   constexpr int N = VecIO<T>::N;
   extern __shared__ float sm[];                       // [2][RL][VT*N]
   const int nvec = C / N;
@@ -53,7 +54,7 @@ __global__ void __launch_bounds__(256) bn_colreduce_kernel(const T* __restrict__
           xr[u] = *reinterpret_cast<const uint4*>(x + rr * C + cv * N);
           if (MODE == 1) {
             gr[u] = *reinterpret_cast<const uint4*>(dy + rr * C + cv * N);
-            if (relu) yr[u] = *reinterpret_cast<const uint4*>(y + rr * C + cv * N);
+            if (ACT != ACT_FLAG || relu) yr[u] = *reinterpret_cast<const uint4*>(y + rr * C + cv * N);
           }
         }
       }
@@ -69,11 +70,12 @@ __global__ void __launch_bounds__(256) bn_colreduce_kernel(const T* __restrict__
           } else {
             float gv[N], yv[N];
             VecIO<T>::ld(reinterpret_cast<const T*>(&gr[u]), gv);
-            if (relu) VecIO<T>::ld(reinterpret_cast<const T*>(&yr[u]), yv);
+            if (ACT != ACT_FLAG || relu) VecIO<T>::ld(reinterpret_cast<const T*>(&yr[u]), yv);
 #pragma unroll
             for (int i = 0; i < N; ++i) {
               float g = gv[i];
-              if (relu && !(yv[i] > 0.f)) g = 0.f;
+              if (ACT == ACT_FLAG) { if (relu && !(yv[i] > 0.f)) g = 0.f; }
+              else g = act_bwd<ACT>(g, yv[i], slope);
               a[i] += g; b[i] += g * (xv[i] - mu[i]) * rs[i];
             }
           }
@@ -100,9 +102,9 @@ __global__ void __launch_bounds__(256) bn_colreduce_kernel(const T* __restrict__
   }
 }
 
-template <typename T, int MODE>
+template <typename T, int MODE, int ACT = ACT_FLAG>
 static void colreduce(const void* x, const void* dy, const void* y, const float* mean, const float* rstd, float* a, float* b, long long R,
-                      int C, int relu, cudaStream_t st) {
+                      int C, int relu, cudaStream_t st, float slope = 0.f) {
   constexpr int N = VecIO<T>::N;
   if (C % N) throw std::runtime_error("batch_norm: C must be a multiple of the 16-byte vector width");
   const int nvec = C / N;
@@ -116,7 +118,8 @@ static void colreduce(const void* x, const void* dy, const void* y, const float*
   const size_t smem = (size_t)2 * RL * VT * N * sizeof(float);
   check_cuda(cudaMemsetAsync(a, 0, (size_t)C * 4, st), "bn memset");
   check_cuda(cudaMemsetAsync(b, 0, (size_t)C * 4, st), "bn memset");
-  bn_colreduce_kernel<T, MODE><<<grid, 256, smem, st>>>((const T*)x, (const T*)dy, (const T*)y, mean, rstd, a, b, R, C, relu, VT, rows_per_cta);
+  bn_colreduce_kernel<T, MODE, ACT><<<grid, 256, smem, st>>>((const T*)x, (const T*)dy, (const T*)y, mean, rstd, a, b, R, C, relu, VT, rows_per_cta,
+                                                             slope);
 }
 
 // mean / rstd from the sums (training) or from the running statistics (eval); momentum update of the running statistics;
@@ -149,10 +152,10 @@ __global__ void bn_finalize_kernel(float* __restrict__ sum, float* __restrict__ 
 // Elementwise passes: thread = (channel vector cv, row lane); the per-channel coefficients are loaded ONCE per thread and the
 // thread then walks rows with a fixed stride — no per-element division (the first version did a 64-bit modulo per 16 bytes and
 // was issue-bound at ~5x the memory roofline), 32-bit offsets inside a row slab.
-template <typename T>
+template <typename T, int ACT>
 __global__ void __launch_bounds__(256) bn_apply_kernel(const T* __restrict__ x, const T* __restrict__ res, T* __restrict__ y,
                                                       const float* __restrict__ scale, const float* __restrict__ shift, long long R, int C,
-                                                      int relu, int VT, int rows_per_cta) {
+                                                      int relu, int VT, int rows_per_cta, float slope) {
   constexpr int N = VecIO<T>::N;
   const int nvec = C / N;
   const int RL = blockDim.x / VT;
@@ -183,7 +186,8 @@ __global__ void __launch_bounds__(256) bn_apply_kernel(const T* __restrict__ x, 
     for (int i = 0; i < N; ++i) {
       a[i] = fmaf(a[i], sc[i], sh[i]);
       if (rp) a[i] += ra[i];
-      if (relu) a[i] = fmaxf(a[i], 0.f);
+      if (ACT == ACT_FLAG) { if (relu) a[i] = fmaxf(a[i], 0.f); }
+      else a[i] = act_fwd<ACT>(a[i], slope);
     }
     VecIO<T>::st(yp + (unsigned)r * (unsigned)C, a);
     if (two) {
@@ -191,7 +195,8 @@ __global__ void __launch_bounds__(256) bn_apply_kernel(const T* __restrict__ x, 
       for (int i = 0; i < N; ++i) {
         b[i] = fmaf(b[i], sc[i], sh[i]);
         if (rp) b[i] += rb[i];
-        if (relu) b[i] = fmaxf(b[i], 0.f);
+        if (ACT == ACT_FLAG) { if (relu) b[i] = fmaxf(b[i], 0.f); }
+        else b[i] = act_fwd<ACT>(b[i], slope);
       }
       VecIO<T>::st(yp + (unsigned)r2 * (unsigned)C, b);
     }
@@ -209,10 +214,10 @@ __global__ void bn_bwd_coef_kernel(const float* __restrict__ gamma, const float*
   k[c] = k1; k[C + c] = k2; k[2 * C + c] = -k1 * dbeta[c] * inv_m - k2 * mean[c];
 }
 
-template <typename T>
+template <typename T, int ACT>
 __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const T* __restrict__ x, const T* __restrict__ dy, const T* __restrict__ y,
                                                           T* __restrict__ dx, T* __restrict__ dres, const float* __restrict__ k, long long R, int C,
-                                                          int relu, int VT, int rows_per_cta) {
+                                                          int relu, int VT, int rows_per_cta, float slope) {
   constexpr int N = VecIO<T>::N;
   const int nvec = C / N;
   const int RL = blockDim.x / VT;
@@ -234,11 +239,14 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const T* __restrict__
     float xv[N], g[N], out[N];
     VecIO<T>::ld(x + base + o, xv);
     VecIO<T>::ld(dy + base + o, g);
-    if (relu) {
+    if (ACT != ACT_FLAG || relu) {
       float yv[N];
       VecIO<T>::ld(y + base + o, yv);
 #pragma unroll
-      for (int i = 0; i < N; ++i) if (!(yv[i] > 0.f)) g[i] = 0.f;
+      for (int i = 0; i < N; ++i) {
+        if (ACT == ACT_FLAG) { if (!(yv[i] > 0.f)) g[i] = 0.f; }
+        else g[i] = act_bwd<ACT>(g[i], yv[i], slope);
+      }
     }
 #pragma unroll
     for (int i = 0; i < N; ++i) out[i] = fmaf(k1[i], g[i], fmaf(k2[i], xv[i], k3[i]));
@@ -290,9 +298,40 @@ static RowGeom row_geom(long long R, int nvec) {
 }
 
 // ---------------------------------------------------------------- launchers (f32 = 1: fp32 activations, else bf16)
+template <typename T>
+static void bn_apply_t(const void* x, const void* res, void* y, const float* s0, const float* s1, long long R, int C, int act, float slope,
+                       const RowGeom& g, cudaStream_t st) {
+#define BNA(A) bn_apply_kernel<T, A><<<g.grid, 256, 0, st>>>((const T*)x, (const T*)res, (T*)y, s0, s1, R, C, act, g.VT, g.rows_per_cta, slope)
+  if (act == ACT_NONE || act == ACT_RELU) BNA(ACT_FLAG);
+  else if (act == ACT_LEAKY) BNA(ACT_LEAKY);
+  else if (act == ACT_SIGMOID) BNA(ACT_SIGMOID);
+  else throw std::runtime_error("batch_norm: unknown activation");
+#undef BNA
+}
+
+template <typename T>
+static void bn_bwd_t(const void* x, const void* dy, const void* y, void* dx, void* dres, const float* mean, const float* rstd, void* dgamma,
+                     void* dbeta, const float* gamma, float* k, long long R, int C, int act, float slope, cudaStream_t st) {
+  constexpr int N = VecIO<T>::N;
+  if (act == ACT_NONE || act == ACT_RELU) colreduce<T, 1>(x, dy, y, mean, rstd, (float*)dbeta, (float*)dgamma, R, C, act, st);
+  else if (act == ACT_LEAKY) colreduce<T, 1, ACT_LEAKY>(x, dy, y, mean, rstd, (float*)dbeta, (float*)dgamma, R, C, act, st, slope);
+  else if (act == ACT_SIGMOID) colreduce<T, 1, ACT_SIGMOID>(x, dy, y, mean, rstd, (float*)dbeta, (float*)dgamma, R, C, act, st, slope);
+  else throw std::runtime_error("batch_norm: unknown activation");
+  bn_bwd_coef_kernel<<<grid1(C, 256), 256, 0, st>>>(gamma, mean, rstd, (const float*)dgamma, (const float*)dbeta, k, C, 1.f / (float)R);
+  const RowGeom g = row_geom(R, C / N);
+  if ((long long)g.rows_per_cta * C >= (1LL << 32)) throw std::runtime_error("batch_norm: row slab too large for 32-bit offsets");
+#define BNB(A) bn_bwd_apply_kernel<T, A><<<g.grid, 256, 0, st>>>((const T*)x, (const T*)dy, (const T*)y, (T*)dx, (T*)dres, k, R, C, act, g.VT, \
+                                                                g.rows_per_cta, slope)
+  if (act == ACT_LEAKY) BNB(ACT_LEAKY);
+  else if (act == ACT_SIGMOID) BNB(ACT_SIGMOID);
+  else BNB(ACT_FLAG);
+#undef BNB
+}
+
+// act: ACT_NONE / ACT_RELU / ACT_LEAKY (slope) / ACT_SIGMOID after the affine (and the residual add)
 void bn_forward(const void* x, const void* res, void* y, const void* gamma, const void* beta, void* mean, void* rstd, void* run_mean,
-                void* run_var, void* scratch /*2*C floats*/, long long R, int C, float momentum, float eps, int training, int relu, int f32,
-                cudaStream_t st) {
+                void* run_var, void* scratch /*2*C floats*/, long long R, int C, float momentum, float eps, int training, int act, float slope,
+                int f32, cudaStream_t st) {
   float* s0 = (float*)scratch; float* s1 = s0 + C;
   if (C % 4) throw std::runtime_error("batch_norm: C must be a multiple of 4");
   if (training) {
@@ -306,27 +345,17 @@ void bn_forward(const void* x, const void* res, void* y, const void* gamma, cons
   if (C % N) throw std::runtime_error("batch_norm: C must be a multiple of the 16-byte vector width");
   const RowGeom g = row_geom(R, C / N);
   if ((long long)g.rows_per_cta * C >= (1LL << 32)) throw std::runtime_error("batch_norm: row slab too large for 32-bit offsets");
-  if (f32) bn_apply_kernel<float><<<g.grid, 256, 0, st>>>((const float*)x, (const float*)res, (float*)y, s0, s1, R, C, relu, g.VT, g.rows_per_cta);
-  else bn_apply_kernel<__nv_bfloat16><<<g.grid, 256, 0, st>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)res, (__nv_bfloat16*)y, s0, s1, R, C,
-                                                               relu, g.VT, g.rows_per_cta);
+  if (f32) bn_apply_t<float>(x, res, y, s0, s1, R, C, act, slope, g, st);
+  else bn_apply_t<__nv_bfloat16>(x, res, y, s0, s1, R, C, act, slope, g, st);
   count_launch(training ? 3 : 2); TMPI_CHECK_LAUNCH("bn_forward"); ::tmpi::check_capture(st, "bn_forward");
 }
 
 // scratch: 3*C floats (the coefficients of the apply pass)
 void bn_backward(const void* x, const void* dy, const void* y, void* dx, void* dres, const void* gamma, const void* mean, const void* rstd,
-                 void* dgamma, void* dbeta, void* scratch, long long R, int C, int relu, int f32, cudaStream_t st) {
-  if (f32) colreduce<float, 1>(x, dy, y, (const float*)mean, (const float*)rstd, (float*)dbeta, (float*)dgamma, R, C, relu, st);
-  else colreduce<__nv_bfloat16, 1>(x, dy, y, (const float*)mean, (const float*)rstd, (float*)dbeta, (float*)dgamma, R, C, relu, st);
-  float* k = (float*)scratch;
-  bn_bwd_coef_kernel<<<grid1(C, 256), 256, 0, st>>>((const float*)gamma, (const float*)mean, (const float*)rstd, (const float*)dgamma,
-                                                    (const float*)dbeta, k, C, 1.f / (float)R);
-  const int N = f32 ? 4 : 8;
-  const RowGeom g = row_geom(R, C / N);
-  if ((long long)g.rows_per_cta * C >= (1LL << 32)) throw std::runtime_error("batch_norm: row slab too large for 32-bit offsets");
-  if (f32) bn_bwd_apply_kernel<float><<<g.grid, 256, 0, st>>>((const float*)x, (const float*)dy, (const float*)y, (float*)dx, (float*)dres, k, R, C,
-                                                              relu, g.VT, g.rows_per_cta);
-  else bn_bwd_apply_kernel<__nv_bfloat16><<<g.grid, 256, 0, st>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)dy, (const __nv_bfloat16*)y,
-                                                                  (__nv_bfloat16*)dx, (__nv_bfloat16*)dres, k, R, C, relu, g.VT, g.rows_per_cta);
+                 void* dgamma, void* dbeta, void* scratch, long long R, int C, int act, float slope, int f32, cudaStream_t st) {
+  auto M = (const float*)mean; auto RS = (const float*)rstd; auto G = (const float*)gamma; auto K = (float*)scratch;
+  if (f32) bn_bwd_t<float>(x, dy, y, dx, dres, M, RS, dgamma, dbeta, G, K, R, C, act, slope, st);
+  else bn_bwd_t<__nv_bfloat16>(x, dy, y, dx, dres, M, RS, dgamma, dbeta, G, K, R, C, act, slope, st);
   count_launch(3); TMPI_CHECK_LAUNCH("bn_backward"); ::tmpi::check_capture(st, "bn_backward");
 }
 

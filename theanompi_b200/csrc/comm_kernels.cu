@@ -189,6 +189,46 @@ void adam_flat(void* W, const void* G, void* M, void* V, void* H, const void* bl
   count_launch(2); TMPI_CHECK_LAUNCH("adam_flat"); ::tmpi::check_capture(st, "adam_flat");
 }
 
+// ============================================================================ flat RMSProp (the GANs' optimizer, torch.optim.RMSprop without momentum)
+// v = alpha v + (1 - alpha) g^2;  w -= lr * g / (sqrt(v) + eps);  then, when clip > 0, w = clamp(w, -clip, clip) (the WGAN critic's
+// weight clipping in the same pass).  lr from device memory, weight decay folded into g, bf16 shadow refreshed.
+__global__ void __launch_bounds__(kThreads) rmsprop_flat_kernel(float* __restrict__ W, const float* __restrict__ G, float* __restrict__ V,
+                                                                __nv_bfloat16* __restrict__ H, const uint8_t* __restrict__ block_group,
+                                                                GroupTable tab, const float* __restrict__ lr_ptr, float alpha, float eps,
+                                                                float clip, long long blk_lo, long long blk_hi) {
+  const float lr0 = *lr_ptr;
+  for (long long b = blk_lo + blockIdx.x; b < blk_hi; b += gridDim.x) {
+    const int g = block_group[b];
+    const float lr = lr0 * tab.lr_mult[g], wd = tab.wd[g];
+    const long long i = b * kArenaBlock + threadIdx.x * 4;
+    float4 w = *reinterpret_cast<const float4*>(W + i), v = *reinterpret_cast<const float4*>(V + i);
+    const float4 gg = *reinterpret_cast<const float4*>(G + i);
+#define TMPI_RMS1(Wc, Vc, Gc)                                         \
+  {                                                                  \
+    const float ge = Gc + wd * Wc;                                   \
+    Vc = alpha * Vc + (1.f - alpha) * ge * ge;                       \
+    Wc -= lr * ge / (sqrtf(Vc) + eps);                               \
+    if (clip > 0.f) Wc = fminf(fmaxf(Wc, -clip), clip);              \
+  }
+    TMPI_RMS1(w.x, v.x, gg.x) TMPI_RMS1(w.y, v.y, gg.y) TMPI_RMS1(w.z, v.z, gg.z) TMPI_RMS1(w.w, v.w, gg.w)
+#undef TMPI_RMS1
+    *reinterpret_cast<float4*>(W + i) = w;
+    *reinterpret_cast<float4*>(V + i) = v;
+    if (H) *reinterpret_cast<uint2*>(H + i) = pack_bf16x4(w);
+  }
+}
+
+void rmsprop_flat(void* W, const void* G, void* V, void* H, const void* block_group, const GroupTable& tab, const void* lr_ptr, float alpha,
+                  float eps, float clip, long long lo, long long hi, cudaStream_t st) {
+  if (lo % kArenaBlock || hi % kArenaBlock) throw std::runtime_error("rmsprop_flat: range must be block aligned");
+  const long long nb = (hi - lo) / kArenaBlock;
+  if (nb <= 0) return;
+  int grid = (int)std::min<long long>(nb, (long long)sm_count() * 8);
+  rmsprop_flat_kernel<<<grid, kThreads, 0, st>>>((float*)W, (const float*)G, (float*)V, (__nv_bfloat16*)H, (const uint8_t*)block_group, tab,
+                                                 (const float*)lr_ptr, alpha, eps, clip, lo / kArenaBlock, hi / kArenaBlock);
+  count_launch(); TMPI_CHECK_LAUNCH("rmsprop_flat"); ::tmpi::check_capture(st, "rmsprop_flat");
+}
+
 // ============================================================================ fused collectives
 __device__ __forceinline__ void local_block_update(const FusedArgs& a, const Hyper& h, long long b, int g) {
   const long long i = b * kArenaBlock + threadIdx.x * 4;

@@ -97,6 +97,23 @@ template <typename T> __device__ __forceinline__ T from_f(float v);
 template <> __device__ __forceinline__ __nv_bfloat16 from_f<__nv_bfloat16>(float v) { return f_to_bf16(v); }
 template <> __device__ __forceinline__ float from_f<float>(float v) { return v; }
 
+// Activation of a fused elementwise pass.  ACT_FLAG: identity or ReLU chosen by the kernel's runtime `relu` argument (the
+// instantiation every pre-existing launch uses, its code unchanged); the others are compile-time variants.  The backward mask is
+// computed from the activation's OUTPUT y: ReLU / leaky ReLU keep the sign of their input, sigmoid' = y (1 - y).
+enum : int { ACT_FLAG = -1, ACT_NONE = 0, ACT_RELU = 1, ACT_LEAKY = 2, ACT_SIGMOID = 3 };
+template <int ACT> __device__ __forceinline__ float act_fwd(float v, float slope) {
+  if (ACT == ACT_RELU) return fmaxf(v, 0.f);
+  if (ACT == ACT_LEAKY) return v > 0.f ? v : v * slope;
+  if (ACT == ACT_SIGMOID) return 1.f / (1.f + __expf(-v));
+  return v;
+}
+template <int ACT> __device__ __forceinline__ float act_bwd(float d, float y, float slope) {
+  if (ACT == ACT_RELU) return y > 0.f ? d : 0.f;
+  if (ACT == ACT_LEAKY) return y > 0.f ? d : d * slope;
+  if (ACT == ACT_SIGMOID) return d * y * (1.f - y);
+  return d;
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -495,6 +495,61 @@ void advance_step(void* step, cudaStream_t st) {
   count_launch(); TMPI_CHECK_LAUNCH("advance_step"); ::tmpi::check_capture(st, "advance_step");
 }
 
+// Uniform [0, 1) noise (GAN generator input): element i is word i % 4 of Philox(counter = (i / 4, *step), key = (seed, stream)),
+// scaled by 2^-24 after dropping the low 8 bits — ops/reference.py: uniform_noise draws the same numbers on the CPU.  The step is
+// read from device memory, so a replayed CUDA graph draws fresh noise.
+template <typename T>
+__global__ void uniform_noise_kernel(T* __restrict__ out, long long n, unsigned long long seed, uint32_t stream,
+                                     const unsigned long long* __restrict__ step) {
+  const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (q * 4 >= n) return;
+  const unsigned long long stp = *step;
+  uint32_t r[4];
+  philox4x32((uint32_t)q, (uint32_t)(q >> 32), (uint32_t)stp, (uint32_t)(stp >> 32), (uint32_t)seed, (uint32_t)(seed >> 32) ^ stream, r);
+#pragma unroll
+  for (int j = 0; j < 4; ++j)
+    if (q * 4 + j < n) out[q * 4 + j] = from_f<T>((float)(r[j] >> 8) * (1.f / 16777216.f));
+}
+void uniform_noise(void* out, long long n, unsigned long long seed, int stream, const void* step, int f32, cudaStream_t st) {
+  const int g = grid_for((n + 3) / 4, 256);
+  auto S = (const unsigned long long*)step;
+  if (f32) uniform_noise_kernel<float><<<g, 256, 0, st>>>((float*)out, n, seed, (uint32_t)stream, S);
+  else uniform_noise_kernel<__nv_bfloat16><<<g, 256, 0, st>>>((__nv_bfloat16*)out, n, seed, (uint32_t)stream, S);
+  count_launch(); TMPI_CHECK_LAUNCH("uniform_noise"); ::tmpi::check_capture(st, "uniform_noise");
+}
+
+// ============================================================================ GAN losses over a [B] score vector, + dscores
+// kind 0 (Wasserstein):   loss = a * mean(o),               d = a / B          (a = +1 fake / -1 real for the critic, -1 generator)
+// kind 1 (least squares): loss = 0.5 * mean((o - a)^2),     d = (o - a) / B    (a = target: 1 real / 0 fake, generator 1)
+// One CTA: B is the batch size.  out[0] = loss (device scalar, no host sync).
+template <typename T>
+__global__ void __launch_bounds__(256) gan_loss_kernel(const T* __restrict__ o, T* __restrict__ d, float* __restrict__ out, int B, int kind,
+                                                       float a) {
+  __shared__ float red[32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  const float invB = 1.f / (float)B;
+  float s = 0.f;
+  for (int i = threadIdx.x; i < B; i += blockDim.x) {
+    const float v = to_f(o[i]);
+    if (kind == 0) { s += v; d[i] = from_f<T>(a * invB); }
+    else { const float e = v - a; s += e * e; d[i] = from_f<T>(e * invB); }
+  }
+  s = warp_sum(s);
+  if (lane == 0) red[warp] = s;
+  __syncthreads();
+  if (warp == 0) {
+    float v = lane < nw ? red[lane] : 0.f;
+    v = warp_sum(v);
+    if (lane == 0) out[0] = kind == 0 ? a * v * invB : 0.5f * v * invB;
+  }
+}
+void gan_loss(const void* scores, void* dscores, void* out, int B, int kind, float a, int f32, cudaStream_t st) {
+  if (kind != 0 && kind != 1) throw std::runtime_error("gan_loss: kind must be 0 (wgan) or 1 (lsgan)");
+  if (f32) gan_loss_kernel<float><<<1, 256, 0, st>>>((const float*)scores, (float*)dscores, (float*)out, B, kind, a);
+  else gan_loss_kernel<__nv_bfloat16><<<1, 256, 0, st>>>((const __nv_bfloat16*)scores, (__nv_bfloat16*)dscores, (float*)out, B, kind, a);
+  count_launch(); TMPI_CHECK_LAUNCH("gan_loss"); ::tmpi::check_capture(st, "gan_loss");
+}
+
 // ============================================================================ softmax + NLL + errors + dlogits
 // one CTA per row; rowstat[b] = {nll, err1, err5}; dlogits = (softmax - onehot) * scale
 template <typename T>
@@ -572,13 +627,14 @@ void softmax_xent(const void* logits, const void* labels, void* dlogits, void* r
   count_launch(); TMPI_CHECK_LAUNCH("rowstat_mean"); ::tmpi::check_capture(st, "rowstat_mean");
 }
 
-// ============================================================================ ReLU mask + bias gradient
-// dym = dy * (y > 0) (contiguous [R, C]);  db[c] += sum_r dym[r, c]   (db pre-zeroed by the launcher)
+// ============================================================================ activation mask + bias gradient
+// dym = act'(y) * dy (contiguous [R, C]; ReLU: dy * (y > 0));  db[c] += sum_r dym[r, c]   (db pre-zeroed by the launcher)
 // dy / y have row pitch ld (elements) so channel slices of a wider tensor work (grouped conv).
-template <typename T, bool RELU, bool WRITE>
+template <typename T, int ACT, bool WRITE>
 __global__ void relu_bias_bwd_kernel(const T* __restrict__ dy, const T* __restrict__ y,
                                      T* __restrict__ dym, float* __restrict__ db, float* __restrict__ db1, int c_split,
-                                     long long R, int C, long long ld, int VT, int rows_per_cta) {
+                                     long long R, int C, long long ld, int VT, int rows_per_cta, float slope) {
+  constexpr bool RELU = ACT != ACT_NONE;              // y is read
   using V = VecIO<T>;
   constexpr int N = V::N;
   extern __shared__ float sm[];                       // [RL][VT*N]
@@ -613,7 +669,10 @@ __global__ void relu_bias_bwd_kernel(const T* __restrict__ dy, const T* __restri
             float v[N];
             V::unpack(yv[u], v);
 #pragma unroll
-            for (int i = 0; i < N; ++i) if (!(v[i] > 0.f)) d[i] = 0.f;
+            for (int i = 0; i < N; ++i) {
+              if (ACT == ACT_RELU) { if (!(v[i] > 0.f)) d[i] = 0.f; }
+              else d[i] = act_bwd<ACT>(d[i], v[i], slope);
+            }
           }
           if (WRITE) *reinterpret_cast<typename V::Raw*>(dym + rr * C + cv * N) = V::pack(d);
 #pragma unroll
@@ -643,7 +702,7 @@ __global__ void relu_bias_bwd_kernel(const T* __restrict__ dy, const T* __restri
 // pass db1 = nullptr / c_split = C for a single bias vector.
 template <typename T>
 static void relu_bias_bwd_t(const void* dy, const void* y, void* dym, void* db, void* db1, int c_split, long long R, int C, long long ld,
-                            int relu, cudaStream_t st) {
+                            int act, float slope, cudaStream_t st) {
   constexpr int N = VecIO<T>::N;
   const int nvec = C / N;
   const int VT = nvec < 32 ? nvec : 32;
@@ -659,24 +718,31 @@ static void relu_bias_bwd_t(const void* dy, const void* y, void* dym, void* db, 
   if (db && c_split < C) check_cuda(cudaMemsetAsync(db1, 0, (size_t)(C - c_split) * 4, st), "relu_bias_bwd memset");
   const bool write = dym != nullptr;
   auto DY = (const T*)dy; auto Y = (const T*)y; auto DM = (T*)dym; auto DB = (float*)db; auto DB1 = (float*)db1;
-  if (relu && write) relu_bias_bwd_kernel<T, true, true><<<grid, 256, smem, st>>>(DY, Y, DM, DB, DB1, c_split, R, C, ld, VT, rows_per_cta);
-  else if (relu) relu_bias_bwd_kernel<T, true, false><<<grid, 256, smem, st>>>(DY, Y, DM, DB, DB1, c_split, R, C, ld, VT, rows_per_cta);
-  else if (write) relu_bias_bwd_kernel<T, false, true><<<grid, 256, smem, st>>>(DY, Y, DM, DB, DB1, c_split, R, C, ld, VT, rows_per_cta);
-  else relu_bias_bwd_kernel<T, false, false><<<grid, 256, smem, st>>>(DY, Y, DM, DB, DB1, c_split, R, C, ld, VT, rows_per_cta);
+#define RBB(A, WR) relu_bias_bwd_kernel<T, A, WR><<<grid, 256, smem, st>>>(DY, Y, DM, DB, DB1, c_split, R, C, ld, VT, rows_per_cta, slope)
+  if ((act == ACT_LEAKY || act == ACT_SIGMOID) && !write) throw std::runtime_error("relu_bias_bwd: this activation mask needs the dym output");
+  if (act == ACT_RELU && write) RBB(ACT_RELU, true);
+  else if (act == ACT_RELU) RBB(ACT_RELU, false);
+  else if (act == ACT_LEAKY) RBB(ACT_LEAKY, true);
+  else if (act == ACT_SIGMOID) RBB(ACT_SIGMOID, true);
+  else if (act != ACT_NONE) throw std::runtime_error("relu_bias_bwd: unknown activation");
+  else if (write) RBB(ACT_NONE, true);
+  else RBB(ACT_NONE, false);
+#undef RBB
   count_launch(); TMPI_CHECK_LAUNCH("relu_bias_bwd"); ::tmpi::check_capture(st, "relu_bias_bwd");
 }
-void relu_bias_bwd(const void* dy, const void* y, void* dym, void* db, void* db1, int c_split, long long R, int C, long long ld, int relu,
-                   int f32, cudaStream_t st) {
+void relu_bias_bwd(const void* dy, const void* y, void* dym, void* db, void* db1, int c_split, long long R, int C, long long ld, int act,
+                   float slope, int f32, cudaStream_t st) {
   need_vec(C, f32, "relu_bias_bwd");
-  if (f32) relu_bias_bwd_t<float>(dy, y, dym, db, db1, c_split, R, C, ld, relu, st);
-  else relu_bias_bwd_t<__nv_bfloat16>(dy, y, dym, db, db1, c_split, R, C, ld, relu, st);
+  if (f32) relu_bias_bwd_t<float>(dy, y, dym, db, db1, c_split, R, C, ld, act, slope, st);
+  else relu_bias_bwd_t<__nv_bfloat16>(dy, y, dym, db, db1, c_split, R, C, ld, act, slope, st);
 }
 
 // y[r, c] = act(acc[r, c] (fp32) + bias[c]), stored as T — finishing pass of a split-K forward GEMM (small-batch FC layers: the
 // parallelism has to come from splitting K, and split-K accumulates in fp32 with reductions, so bias / ReLU / cast run here).
-// The fp32 output may alias acc (in place).
-template <typename T>
-__global__ void bias_act_kernel(const float* __restrict__ acc, const float* __restrict__ bias, T* __restrict__ y, int R, int C, int relu) {
+// The fp32 output may alias acc (in place).  ACT_FLAG: ReLU when `relu` is set; ACT_LEAKY / ACT_SIGMOID: compile-time variants.
+template <typename T, int ACT>
+__global__ void bias_act_kernel(const float* __restrict__ acc, const float* __restrict__ bias, T* __restrict__ y, int R, int C, int relu,
+                                float slope) {
   constexpr int N = VecIO<T>::N;
   const int nvec = C >> VecIO<T>::LOG2N;
   const unsigned idx = blockIdx.x * blockDim.x + threadIdx.x;            // host guarantees R * nvec < 2^32
@@ -692,19 +758,32 @@ __global__ void bias_act_kernel(const float* __restrict__ acc, const float* __re
       v[j] += b.x; v[j + 1] += b.y; v[j + 2] += b.z; v[j + 3] += b.w;
     }
   }
-  if (relu) {
+  if (ACT == ACT_FLAG) {
+    if (relu) {
 #pragma unroll
-    for (int i = 0; i < N; ++i) v[i] = fmaxf(v[i], 0.f);
+      for (int i = 0; i < N; ++i) v[i] = fmaxf(v[i], 0.f);
+    }
+  } else {
+#pragma unroll
+    for (int i = 0; i < N; ++i) v[i] = act_fwd<ACT>(v[i], slope);
   }
   VecIO<T>::st(y + (size_t)r * C + cv * N, v);
 }
-void bias_act(const void* acc, const void* bias, void* y, int R, int C, int relu, int f32, cudaStream_t st) {
+template <typename T>
+static void bias_act_t(const float* acc, const float* bias, void* y, int R, int C, int act, float slope, long long total, cudaStream_t st) {
+  const int g = grid_for(total, 256);
+  if (act == ACT_NONE || act == ACT_RELU) bias_act_kernel<T, ACT_FLAG><<<g, 256, 0, st>>>(acc, bias, (T*)y, R, C, act, slope);
+  else if (act == ACT_LEAKY) bias_act_kernel<T, ACT_LEAKY><<<g, 256, 0, st>>>(acc, bias, (T*)y, R, C, act, slope);
+  else if (act == ACT_SIGMOID) bias_act_kernel<T, ACT_SIGMOID><<<g, 256, 0, st>>>(acc, bias, (T*)y, R, C, act, slope);
+  else throw std::runtime_error("bias_act: unknown activation");
+}
+void bias_act(const void* acc, const void* bias, void* y, int R, int C, int act, float slope, int f32, cudaStream_t st) {
   need_vec(C, f32, "bias_act");
   const long long total = (long long)R * (f32 ? C / 4 : C / 8);
   if (total >= (1LL << 32)) throw std::runtime_error("bias_act: tensor too large for 32-bit indexing");
   auto A = (const float*)acc; auto B = (const float*)bias;
-  if (f32) bias_act_kernel<float><<<grid_for(total, 256), 256, 0, st>>>(A, B, (float*)y, R, C, relu);
-  else bias_act_kernel<__nv_bfloat16><<<grid_for(total, 256), 256, 0, st>>>(A, B, (__nv_bfloat16*)y, R, C, relu);
+  if (f32) bias_act_t<float>(A, B, y, R, C, act, slope, total, st);
+  else bias_act_t<__nv_bfloat16>(A, B, y, R, C, act, slope, total, st);
   count_launch(); TMPI_CHECK_LAUNCH("bias_act"); ::tmpi::check_capture(st, "bias_act");
 }
 
@@ -939,8 +1018,12 @@ __global__ void __launch_bounds__(256) im2col_rows_kernel(const T* __restrict__ 
 }
 
 // dx[n,h,w,c_off+c] = sum over (kh,kw) with (h+p-kh)%s==0, (w+p-kw)%s==0 of dcol[m(n,ho,wo), (kh*KW+kw)*Cg + c]
-template <typename T>
-__global__ void col2im_vec_kernel(const T* __restrict__ dcol, T* __restrict__ dx, ConvGeom g) {
+// BIAS / ACT: the transposed-convolution forward, y = act(col2im(x · W) + b) with a per-channel fp32 bias, applied before the
+// single store; channels >= c_real (zero padding of a layer narrower than 16 bytes) are stored as 0.
+// <T, ACT_NONE, false> is the plain gather of the convolution's input gradient.
+template <typename T, int ACT, bool BIAS>
+__global__ void col2im_vec_kernel(const T* __restrict__ dcol, T* __restrict__ dx, ConvGeom g, const float* __restrict__ bias, float slope,
+                                  int c_real) {
   constexpr int N = VecIO<T>::N;
   const unsigned cvn = (unsigned)(g.Cg >> VecIO<T>::LOG2N);
   const unsigned idx = blockIdx.x * blockDim.x + threadIdx.x;           // host guarantees total < 2^32
@@ -968,6 +1051,16 @@ __global__ void col2im_vec_kernel(const T* __restrict__ dcol, T* __restrict__ dx
 #pragma unroll
       for (int i = 0; i < N; ++i) acc[i] += v[i];
     }
+  }
+  if (BIAS) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) acc[i] += __ldg(bias + cv * N + i);
+  }
+#pragma unroll
+  for (int i = 0; i < N; ++i) acc[i] = act_fwd<ACT>(acc[i], slope);
+  if (BIAS || ACT != ACT_NONE) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) if (cv * N + i >= c_real) acc[i] = 0.f;
   }
   VecIO<T>::st(dx + (((long long)n * g.H + h) * g.W + w) * g.Ctot + g.c_off + cv * N, acc);
 }
@@ -1003,9 +1096,38 @@ void col2im(const void* dcol, void* dx, int N, int H, int W, int Ctot, int c_off
   ConvGeom g{N, H, W, Ctot, c_off, Cg, KH, KW, Ho, Wo, s, p, ldcol, KH * KW * Cg};
   long long total = (long long)N * H * W * (Cg / V);
   if (total >= (1LL << 32)) throw std::runtime_error("col2im: tensor too large for 32-bit indexing");
-  if (f32) col2im_vec_kernel<float><<<grid_for(total, 256), 256, 0, st>>>((const float*)dcol, (float*)dx, g);
-  else col2im_vec_kernel<__nv_bfloat16><<<grid_for(total, 256), 256, 0, st>>>((const __nv_bfloat16*)dcol, (__nv_bfloat16*)dx, g);
+  if (f32) col2im_vec_kernel<float, ACT_NONE, false><<<grid_for(total, 256), 256, 0, st>>>((const float*)dcol, (float*)dx, g, nullptr, 0.f, 0);
+  else col2im_vec_kernel<__nv_bfloat16, ACT_NONE, false><<<grid_for(total, 256), 256, 0, st>>>((const __nv_bfloat16*)dcol, (__nv_bfloat16*)dx, g,
+                                                                                               nullptr, 0.f, 0);
   count_launch(); TMPI_CHECK_LAUNCH("col2im"); ::tmpi::check_capture(st, "col2im");
+}
+
+template <typename T>
+static void col2im_bias_act_t(const void* dcol, void* y, const ConvGeom& g, const float* bias, int act, float slope, int c_real,
+                              long long total, cudaStream_t st) {
+  const int gr = grid_for(total, 256);
+  auto D = (const T*)dcol; auto Y = (T*)y;
+#define C2I(A) (bias ? col2im_vec_kernel<T, A, true><<<gr, 256, 0, st>>>(D, Y, g, bias, slope, c_real) \
+                     : col2im_vec_kernel<T, A, false><<<gr, 256, 0, st>>>(D, Y, g, bias, slope, c_real))
+  if (act == ACT_NONE) C2I(ACT_NONE);
+  else if (act == ACT_RELU) C2I(ACT_RELU);
+  else if (act == ACT_LEAKY) C2I(ACT_LEAKY);
+  else if (act == ACT_SIGMOID) C2I(ACT_SIGMOID);
+  else throw std::runtime_error("col2im_bias_act: unknown activation");
+#undef C2I
+}
+void col2im_bias_act(const void* dcol, void* y, const float* bias, int N, int H, int W, int C, int KH, int KW, int Hi, int Wi, int s, int p,
+                     long long ldcol, int act, float slope, int c_real, int f32, cudaStream_t st) {
+  const int V = f32 ? 4 : 8;
+  if (C % V || ldcol % V) throw std::runtime_error(f32 ? "col2im_bias_act: channel counts must be multiples of 4"
+                                                       : "col2im_bias_act: channel counts must be multiples of 8");
+  ConvGeom g{N, H, W, C, 0, C, KH, KW, Hi, Wi, s, p, ldcol, KH * KW * C};
+  const long long total = (long long)N * H * W * (C / V);
+  if (total >= (1LL << 32)) throw std::runtime_error("col2im_bias_act: tensor too large for 32-bit indexing");
+  if (act == ACT_NONE && !bias && c_real < C) throw std::runtime_error("col2im_bias_act: padded channels need a bias or an activation");
+  if (f32) col2im_bias_act_t<float>(dcol, y, g, bias, act, slope, c_real, total, st);
+  else col2im_bias_act_t<__nv_bfloat16>(dcol, y, g, bias, act, slope, c_real, total, st);
+  count_launch(); TMPI_CHECK_LAUNCH("col2im_bias_act"); ::tmpi::check_capture(st, "col2im_bias_act");
 }
 
 // ============================================================================ small utility kernels

@@ -2,7 +2,7 @@
 swap session (``examples/bsp/session_gap.cfg``): 32×32×3 images, same contract."""
 import numpy as np
 
-from .wgan import WGAN
+from .wgan import WGAN, NativeWGAN
 
 
 class _CifarIter(object):
@@ -32,3 +32,11 @@ class LSGAN(WGAN):
     def make_data(self, config):
         from ..data.cifar10 import Cifar10_data
         return _CifarIter(Cifar10_data(verbose=False, **config.get("data_kwargs", {})), self.batch_size)
+
+
+class NativeLSGAN(NativeWGAN):
+    """:class:`LSGAN` (CIFAR-10) on the native kernels (see :class:`NativeWGAN`)."""
+    loss_kind = "lsgan"
+    learning_rate = 1e-4
+    image_size, image_ch = 32, 3
+    make_data = LSGAN.make_data

@@ -15,6 +15,8 @@ import numpy as np
 import torch
 import torch.nn as nn
 
+from ... import ops
+from ..base import ModelBase
 from ..torch_base import TorchModelBase, tag_module_params
 
 num_epochs = 100
@@ -208,3 +210,283 @@ class WGAN(TorchModelBase):
                 with torch.no_grad():
                     for p, k in zip(params, sorted(f.files, key=lambda s: int(s.split("_")[1]))):
                         p.copy_(torch.from_numpy(f[k]).to(p.device))
+
+
+# ---------------------------------------------------------------------------------------------------------------- native
+class NativeWGAN(ModelBase):
+    """The same GAN on the hand-written sm_90a kernels (CPU: the reference ops), NHWC, with the contract of :class:`WGAN`.
+
+    Generator: FC 100→1024, BN, ReLU; FC →128·s4·s4, BN, ReLU; transposed conv 5×5/2 →64, BN, ReLU; transposed conv 5×5/2 →image,
+    sigmoid.  Critic: conv 5×5/2 →64, leaky ReLU; conv 5×5/2 →128, BN, leaky ReLU; FC →1024, BN, leaky ReLU; FC →1.  The image
+    layer is padded to 16-byte channels (8 in bf16, 4 in fp32) with zero weights; its padded channels are stored as zeros, so the
+    critic's padded input weights get zero gradient and stay zero.  The critic parameters are the exchanged arena (``params``);
+    the generator has its own local arena.  Both train with :class:`FlatRMSProp` (the critic's ±0.01 clip in the same pass).
+    On the GPU the critic step and the generator step are two captured CUDA graphs; ``train_iter`` copies each real batch into
+    a static buffer and replays the critic graph ``critic_runs`` times, then the generator graph.  Noise is Philox keyed by a
+    device step counter the graphs advance."""
+    loss_kind = "wgan"
+    n_epochs = num_epochs
+    batch_size = file_batch_size = batchsize
+    learning_rate = initial_eta
+    image_size, image_ch = 28, 1
+    bias_lr_mult = 1.0
+    nz = 100
+
+    def __init__(self, config):
+        super().__init__(config)
+        from ...ops import cuda_impl, functional as F_
+        from ...parallel.arena import FlatArena
+        from ...utils.opt import FlatRMSProp
+        self.F = F_
+        self.name = "Wasserstein_GAN" if self.loss_kind == "wgan" else "LSGAN"
+        self.n_epochs = config.get("n_epochs", self.n_epochs)
+        self.epochsize = config.get("epochsize", epochsize)
+        self.data = self.make_data(config)
+        self.n_subb = 1
+        self.cp = cp = 4 if self.precision == "tf32" else 8              # 16-byte channel padding of the image
+        self.seed = int(config.get("seed", 1234))
+        g = torch.Generator().manual_seed(self.seed)
+        S, s4, C = self.image_size, self.image_size // 4, self.image_ch
+
+        def u(*shape, fan_in, cols=None):
+            t = (torch.rand(*shape, generator=g) * 2 - 1) / fan_in ** 0.5
+            if cols is not None:
+                t[..., cols:] = 0
+            return t
+
+        def named(ts, names):
+            for t, n in zip(ts, names):
+                t.pname = n
+                t.requires_grad_(True)
+            return ts
+
+        ones, zeros = torch.ones, torch.zeros
+        gen = [u(1024, self.nz, fan_in=self.nz), zeros(1024), ones(1024), zeros(1024),
+               u(s4 * s4 * 128, 1024, fan_in=1024), zeros(s4 * s4 * 128), ones(s4 * s4 * 128), zeros(s4 * s4 * 128),
+               u(128, 5, 5, 64, fan_in=128 * 25), zeros(64), ones(64), zeros(64),
+               u(64, 5, 5, cp, fan_in=64 * 25, cols=C), zeros(cp)]
+        crit = [u(64, 5, 5, cp, fan_in=C * 25, cols=C), zeros(64),
+                u(128, 5, 5, 64, fan_in=64 * 25), zeros(128), ones(128), zeros(128),
+                u(1024, s4 * s4 * 128, fan_in=s4 * s4 * 128), zeros(1024), ones(1024), zeros(1024),
+                u(1, 1024, fan_in=1024), zeros(1)]
+        # GAN critics / generators: every parameter (BN included) follows the same rule, as in the torch twin
+        named(gen, ["W" if t.dim() > 1 else "b" for t in gen]); named(crit, ["W" if t.dim() > 1 else "b" for t in crit])
+        self.finalize(crit, [t.pname for t in crit], (self.batch_size, S, S, cp))
+        self.critic_params = self.params
+        for p in self.critic_params:
+            p.gaccum = True                  # the critic loss sums a real and a fake pass
+        self.gen_arena = FlatArena(gen, [t.pname for t in gen], self.device, bias_lr_mult=1.0,
+                                   shadow=False if self.precision == "tf32" else None)
+        self.generator_params = gen
+        self.gen_lr = self.gen_arena.hyper
+        self.gen_arena.hyper[0] = float(self.base_lr)
+        self.opt_c = FlatRMSProp(self.arena, clip=clip if self.loss_kind == "wgan" else 0.0)
+        self.opt_g = FlatRMSProp(self.gen_arena)
+        dev = self.device
+        self.bn_stats = {k: (torch.zeros(n, device=dev), torch.ones(n, device=dev))
+                         for k, n in (("g1", 1024), ("g2", s4 * s4 * 128), ("g3", 64), ("c2", 128), ("c3", 1024))}
+        self.step = torch.zeros(1, dtype=torch.int64, device=dev)          # noise counter, advanced by every step
+        self.real_raw = torch.zeros((self.batch_size, S, S, C), dtype=torch.float32, device=dev)
+        self.generator_updates = 0
+        self.critic_scores, self.generator_scores, self.c_list, self.g_list = [], [], [], []
+        self.current_info = None
+        self.init_view = False
+        self._train_gen = self.data.iterate("train", seed=1234 + self.rank)
+        self._val_gen = self.data.iterate("val", shuffle=False)
+        self.data.n_batch_train = self.epochsize
+        self.data.n_batch_val = 1
+        self._graphs = {}
+        self._cuda_impl = cuda_impl if self.cuda else None
+
+    make_data = WGAN.make_data
+
+    # ---- network
+    def _bn(self, x, gamma, beta, key, training, act):
+        m, v = self.bn_stats[key]
+        return self.F.batch_norm(x, gamma, beta, m, v, training=training, relu=act)
+
+    def generator(self, z, training=True):
+        F_, p = self.F, self.generator_params
+        s4 = self.image_size // 4
+        h = self._bn(F_.linear_bias_act(z, p[0], p[1], relu=False), p[2], p[3], "g1", training, True)
+        h = self._bn(F_.linear_bias_act(h, p[4], p[5], relu=False), p[6], p[7], "g2", training, True)
+        h = h.reshape(z.shape[0], s4, s4, 128)
+        h = self._bn(F_.conv_transpose2d_bias_act(h, p[8], p[9], 2, 2, 1, "none"), p[10], p[11], "g3", training, True)
+        return F_.conv_transpose2d_bias_act(h, p[12], p[13], 2, 2, 1, "sigmoid", c_real=self.image_ch)
+
+    def critic(self, x, training=True):
+        F_, p = self.F, self.critic_params
+        h = F_.conv2d_bias_act(x, p[0], p[1], 2, 2, 1, relu="leaky")
+        h = self._bn(F_.conv2d_bias_act(h, p[2], p[3], 2, 2, 1, relu=False), p[4], p[5], "c2", training, "leaky")
+        h = h.reshape(x.shape[0], -1)
+        h = self._bn(F_.linear_bias_act(h, p[6], p[7], relu=False), p[8], p[9], "c3", training, "leaky")
+        return F_.linear_bias_act(h, p[10], p[11], relu=False)
+
+    def _noise(self, n, stream):
+        if self.cuda:
+            return self._cuda_impl.uniform_noise((n, self.nz), self.seed, stream, self.step)
+        return ops.reference.uniform_noise((n, self.nz), self.seed, stream, int(self.step))
+
+    def _advance(self):
+        if self.cuda:
+            ci = self._cuda_impl
+            ci.L().advance_step(self.step.data_ptr(), ci._st(self.step))
+        else:
+            self.step += 1
+
+    def _stage_real(self):
+        """The static real batch in the critic's padded channel layout (a native normalise/pad pass on the GPU)."""
+        B, S = self.batch_size, self.image_size
+        if self.cuda:
+            z = torch.zeros((B, 2), dtype=torch.int32, device=self.device)
+            return self._cuda_impl.crop_mirror_normalize(self.real_raw, torch.zeros(1, device=self.device), 1.0, (S, S), z,
+                                                         z[:, 0].to(torch.uint8), c_out=self.cp)
+        x = torch.zeros((B, S, S, self.cp))
+        x[..., :self.image_ch] = self.real_raw
+        return x
+
+    def _losses(self, real, fake):
+        gl = self.F.gan_loss
+        if self.loss_kind == "wgan":
+            return gl(self.critic(fake), "wgan", 1.0) + gl(self.critic(real), "wgan", -1.0)
+        return gl(self.critic(real), "lsgan", 1.0) + gl(self.critic(fake), "lsgan", 0.0)
+
+    def _critic_body(self):
+        self.arena.G.zero_()
+        with torch.no_grad():
+            fake = self.generator(self._noise(self.batch_size, 0))
+        loss = self._losses(self._stage_real(), fake)
+        loss.backward()
+        with torch.no_grad():
+            self.opt_c.step()
+        self._advance()
+        return (-loss if self.loss_kind == "wgan" else loss).detach()
+
+    def _gen_body(self):
+        o = self.critic(self.generator(self._noise(self.batch_size, 1)))
+        loss = self.F.gan_loss(o, self.loss_kind, -1.0 if self.loss_kind == "wgan" else 1.0)
+        loss.backward()
+        with torch.no_grad():
+            self.opt_g.step()
+        self._advance()
+        return loss.detach()
+
+    def _run(self, kind):
+        """Eager on the CPU / without graphs; on the GPU: two eager warm-up runs on the capture stream, then capture, then
+        replays (the ModelBase protocol, once per step kind)."""
+        body = self._critic_body if kind == "critic" else self._gen_body
+        if not self.use_graph:
+            return body()
+        st = self._graphs.get(kind)
+        if st is None:
+            st = self._graphs[kind] = {"warm": 0, "graph": None, "stream": torch.cuda.Stream(device=self.device)}
+        s = st["stream"]
+        if st["graph"] is None:
+            cur = torch.cuda.current_stream(self.device)
+            s.wait_stream(cur)
+            if st["warm"] < 2:
+                st["warm"] += 1
+                with torch.cuda.stream(s):
+                    out = body()
+                cur.wait_stream(s)
+                return out
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.stream(s):
+                with torch.cuda.graph(g, stream=s, capture_error_mode="thread_local"):
+                    out = body()
+            cur.wait_stream(s)
+            st["graph"], st["out"] = g, out
+        st["graph"].replay()
+        return st["out"].clone()
+
+    # ---- contract
+    def compile_iter_fns(self, sync_type="avg", **kw):
+        self.sync_type = "avg"
+        self.vels, self.vels2 = [], []
+        self.train_iter_fn = self.val_iter_fn = None
+
+    def _load_real(self, gen):
+        x, _ = next(gen)
+        self.real_raw.copy_(torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32)).reshape(self.real_raw.shape))
+
+    def train_iter(self, count, recorder):
+        if self.loss_kind == "wgan":
+            critic_runs = 50 if (self.generator_updates < 5 or self.generator_updates % 100 == 0) else 2
+            critic_runs = self.config.get("critic_runs", critic_runs)
+        else:
+            critic_runs = 1
+        scores = []
+        recorder.start()
+        for _ in range(critic_runs):
+            self._load_real(self._train_gen)
+            scores.append(self._run("critic"))
+            count += 1
+        g_score = self._run("gen")
+        self.critic_scores.extend(scores)
+        self.generator_scores.append(g_score)
+        self.generator_updates += 1
+        recorder.train_error(count, sum(scores) / len(scores), g_score)
+        recorder.end("calc")
+        return count
+
+    def val_iter(self, count, recorder):
+        self._load_real(self._val_gen)
+        with torch.no_grad():
+            fake = self.generator(self._noise(self.batch_size, 2), training=False)
+            o_real, o_fake = self.critic(self._stage_real(), training=False), self.critic(fake, training=False)
+            if self.loss_kind == "wgan":
+                c, g = o_fake.float().mean() - o_real.float().mean(), -o_fake.float().mean()
+            else:
+                c = 0.5 * ((o_real.float() - 1) ** 2).mean() + 0.5 * (o_fake.float() ** 2).mean()
+                g = 0.5 * ((o_fake.float() - 1) ** 2).mean()
+        recorder.val_error(count, -c if self.loss_kind == "wgan" else c, g, 0)
+
+    def reset_iter(self, *args, **kwargs):
+        pass
+
+    def print_info(self, recorder, verbose=True):
+        if not self.generator_scores:
+            return
+        g_ = float(torch.stack([s.float() for s in self.generator_scores]).mean())
+        c_ = float(torch.stack([s.float() for s in self.critic_scores]).mean())
+        self.g_list.append(g_); self.c_list.append(c_)
+        if verbose:
+            print("\nEpoch %d\n  generator score:\t\t%s\n  %s:\t\t%s" % (self.epoch, g_, "Wasserstein distance" if self.loss_kind == "wgan" else "critic loss", c_))
+        self.critic_scores[:] = []; self.generator_scores[:] = []
+        if verbose and self.config.get("plot", False):
+            with torch.no_grad():
+                s = self.generator(self._noise(42, 3), training=False)[..., 0].float().cpu().numpy()
+            S = self.image_size
+            img = s.reshape(6, 7, S, S).transpose(0, 2, 1, 3).reshape(6 * S, 7 * S)
+            if not self.init_view:
+                self.init_view = True
+                recorder.plot_init(name="scores", save=True); recorder.plot_init(name="sample", save=True)
+            recorder.plot(name="sample", image=img, cmap="gray")
+            recorder.plot(name="scores", lines=[(list(range(len(self.c_list))), self.c_list, "critic"),
+                                                (list(range(len(self.g_list))), self.g_list, "generator")])
+
+    def adjust_hyperp(self, epoch):
+        if epoch >= self.n_epochs // 2:
+            lr = self.learning_rate * 2 * (1 - float(epoch) / self.n_epochs)
+            self.shared_lr.set_value(lr)
+            self.gen_arena.hyper[0] = lr
+
+    save = WGAN.save
+
+    def load(self, path, epoch):
+        WGAN.load(self, path, epoch)
+        self.arena.refresh_shadow(); self.gen_arena.refresh_shadow()
+
+    def extra_state(self):
+        """Batch-norm running statistics, the generator arena, both RMSProp averages, the noise step and the schedule."""
+        return {"bn": {k: (m.detach().cpu(), v.detach().cpu()) for k, (m, v) in self.bn_stats.items()},
+                "gen_arena": self.gen_arena.state_dict(), "rms_c": self.opt_c.state_dict(), "rms_g": self.opt_g.state_dict(),
+                "step": int(self.step), "generator_updates": self.generator_updates}
+
+    def load_extra_state(self, sd):
+        for k, (m, v) in sd["bn"].items():
+            self.bn_stats[k][0].copy_(m); self.bn_stats[k][1].copy_(v)
+        self.gen_arena.load_state_dict(sd["gen_arena"])
+        self.opt_c.load_state_dict(sd["rms_c"]); self.opt_g.load_state_dict(sd["rms_g"])
+        self.step.fill_(int(sd["step"]))
+        self.generator_updates = int(sd["generator_updates"])

@@ -34,6 +34,15 @@ def _is32(t):
     return t.dtype == F32
 
 
+ACT = {"none": 0, "relu": 1, "leaky": 2, "sigmoid": 3}     # activation codes of the native kernels (ACT_* in csrc/common.cuh)
+LEAKY_SLOPE = 0.2                                          # negative slope of "leaky" (the DCGAN critic's LeakyReLU(0.2))
+
+
+def _act(relu):
+    """Activation code of a ``relu`` argument: a bool (ReLU or identity) or an activation name from :data:`ACT`."""
+    return ACT[relu] if isinstance(relu, str) else int(bool(relu))
+
+
 def _al(t):
     """Elements per 16 bytes (TMA / vector alignment unit): 8 for bf16, 4 for fp32."""
     return 16 // t.element_size()
@@ -113,32 +122,33 @@ def linear_bias_act(x, w, b, relu=True):
     xa, lda = _rows8(x2)
     wa, ldb = _rows8(_bf(w))
     bias = b.float() if b is not None and b.dtype != torch.float32 else b
-    if FC_SPLITK and B_ <= 128 and I >= 1024 and O % 8 == 0:
+    if (FC_SPLITK and B_ <= 128 and I >= 1024 and O % 8 == 0) or _act(relu) > 1:
         # small-batch FC forward is a weight stream: one m-tile, so the parallelism comes from n-tiles x split-K (fp32
         # reductions into a scratch tile), followed by a tiny bias + ReLU (+ bf16 cast) pass; fp32 output is finished in
         # place.  (The fused-epilogue kernel needs 32-wide tiles to fill the machine and then re-reads the activations 128
-        # times through L2: 37 us vs 13 us for fc6.)
+        # times through L2: 37 us vs 13 us for fc6.)  Leaky ReLU / sigmoid are not in the GEMM epilogue and take this path too.
         f32 = _is32(x2)
         acc = gemm(xa, wa, B_, O, I, out_dtype=torch.float32, lda=lda, ldb=ldb)
         y = acc if f32 else torch.empty((B_, O), dtype=BF16, device=x2.device)
-        L().bias_act(acc.data_ptr(), _p(bias), y.data_ptr(), int(B_), int(O), int(bool(relu)), int(f32), _st(x2))
+        L().bias_act(acc.data_ptr(), _p(bias), y.data_ptr(), int(B_), int(O), _act(relu), LEAKY_SLOPE, int(f32), _st(x2))
         return y
     return gemm(xa, wa, B_, O, I, bias=bias, bias_mode=1 if b is not None else 0, relu=relu, lda=lda, ldb=ldb)
 
 
 def _mask_and_bias_grad(dy, y, relu, db_out, R, C, ld, need_db=True):
-    """dym = dy ⊙ (y > 0) (contiguous [R, C]) and db = Σ_rows dym in one pass."""
+    """dym = dy ⊙ act'(y) (ReLU: dy ⊙ (y > 0); contiguous [R, C]) and db = Σ_rows dym in one pass."""
     dev = dy.device
-    if not need_db and not relu and ld == C:
+    act = _act(relu)
+    if not need_db and not act and ld == C:
         return dy, None                                    # bias-free linear conv (a BatchNormal follows): nothing to do
     db = db_out if db_out is not None else torch.empty(C, dtype=torch.float32, device=dev)
-    if relu or ld != C:
+    if act or ld != C:
         dym = torch.empty((R, C), dtype=dy.dtype, device=dev)
-        L().relu_bias_bwd(dy.data_ptr(), _p(y), dym.data_ptr(), db.data_ptr(), 0, int(C), int(R), int(C), int(ld), int(bool(relu)),
+        L().relu_bias_bwd(dy.data_ptr(), _p(y), dym.data_ptr(), db.data_ptr(), 0, int(C), int(R), int(C), int(ld), _act(relu), LEAKY_SLOPE,
                           int(_is32(dy)), _st(dy))
     else:
         dym = dy
-        L().relu_bias_bwd(dy.data_ptr(), 0, 0, db.data_ptr(), 0, int(C), int(R), int(C), int(ld), 0, int(_is32(dy)), _st(dy))
+        L().relu_bias_bwd(dy.data_ptr(), 0, 0, db.data_ptr(), 0, int(C), int(R), int(C), int(ld), 0, 0.0, int(_is32(dy)), _st(dy))
     return dym, db
 
 
@@ -181,9 +191,8 @@ def _linear_bwd_padded(x2, w, y, dy, relu, need_dx, dw_out, db_out):
     Op, Ip = (O + 7) // 8 * 8, (I + 7) // 8 * 8
     dev = x2.device
     dt = x2.dtype
-    dyf = dy.float()
-    if relu:
-        dyf = dyf * (y > 0)
+    from .reference import act_bwd
+    dyf = act_bwd(dy.float(), y.float(), relu)
     db = dyf.sum(0)
     dyp = torch.zeros((B_, Op), dtype=dt, device=dev); dyp[:, :O] = dyf
     xp = torch.zeros((B_, Ip), dtype=dt, device=dev); xp[:, :I] = x2
@@ -311,11 +320,30 @@ def _conv_s2d_bwd(xs, w, y, dy, relu, g, dw_out, db_out, pre_masked=False):
     return dw, db
 
 
+def _conv_fwd_act(x, w, b, s, p, act, Ho, Wo):
+    """Convolution followed by an activation the GEMM epilogue does not have (leaky ReLU, sigmoid): im2col, an fp32-output GEMM,
+    then one bias + activation pass.  Returns (y, the im2col matrix for the backward)."""
+    N = x.shape[0]
+    O, KH, KW, _ = w.shape
+    col, Kp, K = _im2col(x, 0, x.shape[3], KH, KW, Ho, Wo, s, p)
+    M = N * Ho * Wo
+    acc = gemm(col, _w2d(w, K, Kp), M, O, K, out_dtype=torch.float32, lda=Kp, ldb=Kp)
+    f32 = _is32(x)
+    y = acc.view(N, Ho, Wo, O) if f32 else torch.empty((N, Ho, Wo, O), dtype=BF16, device=x.device)
+    L().bias_act(acc.data_ptr(), _p(b), y.data_ptr(), int(M), int(O), _act(act), LEAKY_SLOPE, int(f32), _st(x))
+    return y, (col, Kp, K)
+
+
 def conv2d_bias_act(x, w, b, stride=1, pad=0, groups=1, relu=True, return_cols=False):
     x = _bf(x).contiguous()
     N, H, W, C = x.shape
     O, KH, KW, Cg = w.shape
     assert Cg * groups == C
+    if _act(relu) > 1:
+        if groups != 1:
+            raise RuntimeError("leaky ReLU / sigmoid convolutions are single-group")
+        y, col = _conv_fwd_act(x, w, b, stride, pad, relu, *_out_hw(H, W, KH, KW, stride, pad))
+        return (y, [col]) if return_cols else y
     g = _s2d_geom(H, W, C, KH, KW, stride, pad) if (groups == 1 and O % 8 == 0) else None
     if g is not None:
         y, xs = _conv_s2d_fwd(x, w, b, relu, g)
@@ -330,7 +358,13 @@ def conv2d_bias_act(x, w, b, stride=1, pad=0, groups=1, relu=True, return_cols=F
     return (y, cols) if return_cols else y
 
 
+def _relu_only(relu, what):
+    if _act(relu) > 1:
+        raise RuntimeError("%s supports ReLU or no activation only" % what)
+
+
 def conv2d_group2_bias_act(x, w0, b0, w1, b1, stride, pad, relu, return_cols=False):
+    _relu_only(relu, "conv2d_group2_bias_act")
     x = _bf(x).contiguous()
     N, H, W, C = x.shape
     Og, KH, KW, Cg = w0.shape
@@ -428,6 +462,7 @@ def conv2d_bias_act_bwd(x, w, y, dy, stride, pad, groups, relu, need_dx, dw_out=
 
 def conv2d_group2_bias_act_bwd(x, w0, w1, y, dy, stride, pad, relu, need_dx, outs=(None, None, None, None), cols=None,
                                pre_masked=False):
+    _relu_only(relu, "conv2d_group2_bias_act_bwd")
     x = _bf(x).contiguous()
     dy = _bf(dy).contiguous()
     Og, KH, KW, Cg = w0.shape
@@ -450,7 +485,7 @@ def conv2d_group2_bias_act_bwd(x, w0, w1, y, dy, stride, pad, relu, need_dx, out
         else:
             dym = torch.empty((M, Ot), dtype=x.dtype, device=dev)
             L().relu_bias_bwd(dy.data_ptr(), y.data_ptr(), dym.data_ptr(), db0.data_ptr(), db1.data_ptr(), int(Og), int(M), int(Ot), int(Ot),
-                              int(bool(relu)), f32, _st(x))
+                              _act(relu), LEAKY_SLOPE, f32, _st(x))
         dw0 = outs[0] if outs[0] is not None else torch.empty((Og, KH, KW, Cg), dtype=torch.float32, device=dev)
         dw1 = outs[2] if outs[2] is not None else torch.empty((Og, KH, KW, Cg), dtype=torch.float32, device=dev)
         L().conv_wgrad2(dym.data_ptr(), dym.data_ptr() + Og * es, x.data_ptr(), dw0.data_ptr(), dw1.data_ptr(), N, H, W, Ct, 0, int(Cg), int(Cg),
@@ -464,6 +499,52 @@ def conv2d_group2_bias_act_bwd(x, w0, w1, y, dy, stride, pad, relu, need_dx, out
     dw1, db1 = _conv_bwd_group(x, w1, y, dy, dx, Og, Cg, Cg, stride, pad, relu, need_dx, outs[2], outs[3],
                                col=cols[1] if cols else None, pre_masked=pre_masked)
     return dx, (dw0, db0, dw1, db1)
+
+
+# --------------------------------------------------------------------------- transposed convolution (NHWC)
+def _convT_out_hw(Hi, Wi, KH, KW, s, p, op):
+    return (Hi - 1) * s - 2 * p + KH + op, (Wi - 1) * s - 2 * p + KW + op
+
+
+def conv_transpose2d_bias_act(x, w, b, stride, pad, output_padding=0, relu=False, c_real=None):
+    """Transposed convolution = the input gradient of a stride-``stride`` convolution: ``y = act(col2im(x · W) + b)``.
+
+    ``w`` is ``[Cin, KH, KW, Cout]``, the OHWI weight of the forward convolution that maps y-space to x-space.  The product is
+    the wgmma GEMM (x K-major, W MN-major); the gather, bias and activation are one ``col2im_bias_act`` pass.  Output channels
+    ``>= c_real`` (zero padding of a layer narrower than 16 bytes) are written as zeros; that needs ReLU or sigmoid, whose
+    backward mask is zero at a zero output, so the padded channels get zero gradient whatever the consumer sends back."""
+    x = _bf(x).contiguous()
+    N, Hi, Wi, Cin = x.shape
+    _, KH, KW, Cout = w.shape
+    assert w.shape[0] == Cin and 0 <= output_padding < stride
+    if c_real is not None and c_real < Cout and _act(relu) not in (ACT["relu"], ACT["sigmoid"]):
+        raise RuntimeError("conv_transpose2d: padded output channels need a ReLU or sigmoid activation")
+    if Cin % _al(x) or Cout % _al(x):
+        raise RuntimeError("conv_transpose2d: channel counts must be multiples of 16 bytes")
+    H, W = _convT_out_hw(Hi, Wi, KH, KW, stride, pad, output_padding)
+    K = KH * KW * Cout
+    Kp = (K + 7) // 8 * 8
+    dcol = gemm(x.view(-1, Cin), _w2d(w, K, Kp), N * Hi * Wi, Kp, Cin, b_mn=True, lda=Cin, ldb=Kp)
+    y = torch.empty((N, H, W, Cout), dtype=x.dtype, device=x.device)
+    L().col2im_bias_act(dcol.data_ptr(), y.data_ptr(), _p(b), N, H, W, Cout, KH, KW, Hi, Wi, int(stride), int(pad), Kp, _act(relu), LEAKY_SLOPE,
+                        int(Cout if c_real is None else c_real), int(_is32(x)), _st(x))
+    return y
+
+
+def conv_transpose2d_bias_act_bwd(x, w, y, dy, stride, pad, relu, need_dx, dw_out=None, db_out=None):
+    """Backward of :func:`conv_transpose2d_bias_act`: the activation mask and bias gradient in one pass, ``dx`` = the forward
+    convolution of the masked gradient with the same weight, ``dW`` = that convolution's weight gradient with the roles of its
+    input and output gradient swapped (x is the "output gradient", the masked dy the "input").  Padded output channels have
+    y = 0, where the ReLU / sigmoid mask is 0: their weight and bias gradients are exactly zero."""
+    x = _bf(x).contiguous()
+    dy = _bf(dy).contiguous()
+    N, H, W, Cout = y.shape
+    M = N * H * W
+    dym, db = _mask_and_bias_grad(dy.view(M, Cout), y.view(M, Cout), relu, db_out.view(-1) if db_out is not None else None, M, Cout, Cout)
+    dym = dym.view(N, H, W, Cout)
+    dx = conv2d_bias_act(dym, w, None, stride, pad, 1, False) if need_dx else None
+    _, dw, _ = conv2d_bias_act_bwd(dym, w, x, x, stride, pad, 1, False, False, dw_out=dw_out, pre_masked=True, need_db=False)
+    return dx, dw, db
 
 
 # --------------------------------------------------------------------------- pool / LRN / dropout / loss
@@ -538,6 +619,23 @@ def softmax_xent(logits, labels, weight=1.0):
     return out3[0], out3[1], out3[2], dl
 
 
+def gan_loss(scores, kind, a):
+    """GAN loss over a ``[B, 1]`` (or ``[B]``) score vector and its gradient in one launch; see :func:`reference.gan_loss`."""
+    sc = _bf(scores).contiguous()
+    d = torch.empty_like(sc)
+    out = torch.empty(1, dtype=F32, device=sc.device)
+    L().gan_loss(sc.data_ptr(), d.data_ptr(), out.data_ptr(), int(sc.numel()), {"wgan": 0, "lsgan": 1}[kind], float(a), int(_is32(sc)), _st(sc))
+    return out[0], d
+
+
+def uniform_noise(shape, seed, stream, step, dtype=None):
+    """Uniform [0, 1) noise from Philox keyed by (seed, stream) and the int64 device step counter ``step`` (read by the kernel, so
+    every replay of a captured step draws fresh numbers); :func:`reference.uniform_noise` draws the same numbers on the CPU."""
+    out = torch.empty(tuple(shape), dtype=dtype or ADT(), device=step.device)
+    L().uniform_noise(out.data_ptr(), out.numel(), int(seed), int(stream), step.data_ptr(), int(_is32(out)), _st(step))
+    return out
+
+
 # --------------------------------------------------------------------------- batch norm (+ residual)(+ ReLU), residual add
 def batch_norm_fwd(x, gamma, beta, run_mean, run_var, training, momentum, eps, relu, res=None):
     x = _bf(x).contiguous()
@@ -556,7 +654,7 @@ def batch_norm_fwd(x, gamma, beta, run_mean, run_var, training, momentum, eps, r
         assert run_mean is not None and run_var is not None
     L().bn_forward(x.data_ptr(), _p(res), y.data_ptr(), gamma.data_ptr(), beta.data_ptr(), mean.data_ptr(), rstd.data_ptr(),
                    _p(run_mean), _p(run_var), scratch.data_ptr(), int(R), int(C), float(momentum), float(eps), int(bool(training)),
-                   int(bool(relu)), int(_is32(x)), _st(x))
+                   _act(relu), LEAKY_SLOPE, int(_is32(x)), _st(x))
     return y, mean, rstd
 
 
@@ -573,7 +671,7 @@ def batch_norm_bwd(x, dy, y, gamma, mean, rstd, relu, need_dres, dgamma_out=None
     dbeta = dbeta_out.view(-1) if dbeta_out is not None else torch.empty(C, dtype=F32, device=dev)
     scratch = torch.empty(3 * C, dtype=F32, device=dev)
     L().bn_backward(x.data_ptr(), dy.data_ptr(), _p(y) if relu else 0, dx.data_ptr(), _p(dres), gamma.data_ptr(), mean.data_ptr(),
-                    rstd.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), scratch.data_ptr(), int(R), int(C), int(bool(relu)),
+                    rstd.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), scratch.data_ptr(), int(R), int(C), _act(relu), LEAKY_SLOPE,
                     int(_is32(x)), _st(x))
     if need_dres and not relu:
         dres = dy

@@ -101,7 +101,7 @@ def _fused_pool_ok(x, relu, pool):
     # (bf16 path only: the fused kernel works on packed bf16 lanes; the fp32 / tf32 path runs pool-backward and ReLU-mask +
     # bias-gradient as two kernels)
     # TMPI_DETERMINISTIC=1 also takes the two-kernel route: the fused kernel reduces the bias gradient with cross-CTA atomics
-    return (pool is not None and x.is_cuda and relu and pool[3] == "max" and x.dtype == torch.bfloat16
+    return (pool is not None and x.is_cuda and relu in (True, "relu") and pool[3] == "max" and x.dtype == torch.bfloat16
             and os.environ.get("TMPI_DETERMINISTIC") != "1")
 
 
@@ -260,6 +260,39 @@ class _ConvG2Fn(torch.autograd.Function):
 
 def conv2d_group2_bias_act(x, w0, b0, w1, b1, stride=1, pad=0, relu=True, pool=None):
     return _ConvG2Fn.apply(x, w0, b0, w1, b1, stride, pad, relu, pool)
+
+
+# --------------------------------------------------------------------------- transposed conv
+class _ConvTFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, w, b, stride, pad, output_padding, act, c_real):
+        impl = _impl(x)
+        y = impl.conv_transpose2d_bias_act(x, compute_weight(w), b, stride, pad, output_padding, act, c_real)
+        ctx.save_for_backward(x, y)
+        ctx.w, ctx.b, ctx.cfg = w, b, (stride, pad, act)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, y = ctx.saved_tensors
+        w, b = ctx.w, ctx.b
+        stride, pad, act = ctx.cfg
+        impl = _impl(x)
+        need_dx = ctx.needs_input_grad[0]
+        if impl is ref:
+            dx, dw, db = ref.conv_transpose2d_bias_act_bwd(x, compute_weight(w), y, dy, stride, pad, act, need_dx)
+        else:
+            dx, dw, db = impl.conv_transpose2d_bias_act_bwd(x, compute_weight(w), y, dy, stride, pad, act, need_dx,
+                                                            dw_out=_gout(w), db_out=_gout(b))
+        gb = _sink(b, db)
+        gw = _sink(w, dw)
+        return dx, gw, gb, None, None, None, None, None
+
+
+def conv_transpose2d_bias_act(x, w, b, stride, pad, output_padding=0, act="none", c_real=None):
+    """NHWC transposed convolution + bias + activation (``act``: "none", "relu", "leaky", "sigmoid"); ``w`` is
+    ``[Cin, KH, KW, Cout]``.  Output channels ``>= c_real`` are zero (16-byte channel padding of a narrow layer)."""
+    return _ConvTFn.apply(x, w, b, stride, pad, output_padding, act, c_real)
 
 
 # --------------------------------------------------------------------------- batch norm (+ residual)(+ ReLU)
@@ -467,6 +500,26 @@ class _SoftmaxXentFn(torch.autograd.Function):
 def softmax_xent(logits, labels):
     """Returns (mean NLL, top-1 error, top-5 error) — fused on CUDA."""
     return _SoftmaxXentFn.apply(logits, labels)
+
+
+# --------------------------------------------------------------------------- GAN losses
+class _GanLossFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, scores, kind, a):
+        loss, d = _impl(scores).gan_loss(scores, kind, a)
+        ctx.save_for_backward(d.view_as(scores))
+        return loss
+
+    @staticmethod
+    def backward(ctx, gl):
+        (d,) = ctx.saved_tensors
+        return (d * gl.to(d.dtype)), None, None
+
+
+def gan_loss(scores, kind, a):
+    """WGAN (``kind="wgan"``: ``a * mean(scores)``) or least-squares (``"lsgan"``: ``0.5 * mean((scores - a)^2)``) loss as a
+    device scalar; its gradient comes from the same launch (see :func:`reference.gan_loss`)."""
+    return _GanLossFn.apply(scores, kind, a)
 
 
 # --------------------------------------------------------------------------- data aug

@@ -10,8 +10,36 @@ used c01b / bc01 (``theanompi/models/layers2.py:430-560``).
 """
 from __future__ import annotations
 
+import numpy as np
 import torch
 import torch.nn.functional as F
+
+LEAKY_SLOPE = 0.2        # negative slope of the "leaky" activation (the DCGAN critic's LeakyReLU(0.2))
+
+
+def act_fwd(y, relu):
+    """Activation named by a ``relu`` argument: a bool (ReLU or identity) or one of "none", "relu", "leaky", "sigmoid"."""
+    a = relu if isinstance(relu, str) else ("relu" if relu else "none")
+    if a == "relu":
+        return torch.relu(y)
+    if a == "leaky":
+        return F.leaky_relu(y, LEAKY_SLOPE)
+    if a == "sigmoid":
+        return torch.sigmoid(y)
+    assert a == "none", a
+    return y
+
+
+def act_bwd(dy, y, relu):
+    """``dy`` times the activation's derivative, computed from its output ``y``."""
+    a = relu if isinstance(relu, str) else ("relu" if relu else "none")
+    if a == "relu":
+        return dy * (y > 0).to(dy.dtype)
+    if a == "leaky":
+        return torch.where(y > 0, dy, dy * LEAKY_SLOPE)
+    if a == "sigmoid":
+        return dy * y * (1 - y)
+    return dy
 
 
 def _nchw(x):
@@ -26,15 +54,12 @@ def _nhwc(x):
 def conv2d_bias_act(x, w, b, stride=1, pad=0, groups=1, relu=True):
     """conv + bias + ReLU (ref ``layers2.py:380-388``)."""
     y = F.conv2d(_nchw(x), w.permute(0, 3, 1, 2), b, stride=stride, padding=pad, groups=groups)
-    if relu:
-        y = torch.relu(y)
-    return _nhwc(y)
+    return _nhwc(act_fwd(y, relu))
 
 
 def conv2d_bias_act_bwd(x, w, y, dy, stride=1, pad=0, groups=1, relu=True, need_dx=True):
-    """Returns (dx, dw, db) given the forward output ``y`` (for the ReLU mask)."""
-    if relu:
-        dy = dy * (y > 0).to(dy.dtype)
+    """Returns (dx, dw, db) given the forward output ``y`` (for the activation mask)."""
+    dy = act_bwd(dy, y, relu)
     xn, wn, dyn = _nchw(x), w.permute(0, 3, 1, 2), _nchw(dy)
     dx = None
     if need_dx:
@@ -46,16 +71,39 @@ def conv2d_bias_act_bwd(x, w, y, dy, stride=1, pad=0, groups=1, relu=True, need_
     return dx, dw, db
 
 
+# --------------------------------------------------------------------------- transposed conv
+def conv_transpose2d_bias_act(x, w, b, stride, pad, output_padding=0, relu=False, c_real=None):
+    """Transposed conv + bias + activation, NHWC; ``w`` is ``[Cin, KH, KW, Cout]`` (the OHWI weight of the convolution that
+    maps y-space back to x-space — ``torch.nn.ConvTranspose2d``'s ``[Cin, Cout, KH, KW]`` permuted).  Output channels
+    ``>= c_real`` are zero (padding of a layer narrower than 16 bytes)."""
+    if c_real is not None and c_real < w.shape[-1] and relu not in (True, "relu", "sigmoid"):
+        raise RuntimeError("conv_transpose2d: padded output channels need a ReLU or sigmoid activation")
+    y = F.conv_transpose2d(_nchw(x), w.permute(0, 3, 1, 2), b, stride=stride, padding=pad, output_padding=output_padding)
+    y = _nhwc(act_fwd(y, relu))
+    if c_real is not None and c_real < y.shape[-1]:
+        y[..., c_real:] = 0
+    return y
+
+
+def conv_transpose2d_bias_act_bwd(x, w, y, dy, stride, pad, relu, need_dx=True):
+    """Returns (dx, dw, db) of :func:`conv_transpose2d_bias_act`: dx is the forward convolution of the masked gradient, dw
+    that convolution's weight gradient with x in the role of its output gradient."""
+    dym = act_bwd(dy, y, relu)
+    wn = w.permute(0, 3, 1, 2)                       # [Cin, Cout, KH, KW] = conv weight [O, I, KH, KW] of y-space -> x-space
+    dx = _nhwc(F.conv2d(_nchw(dym), wn, None, stride=stride, padding=pad)) if need_dx else None
+    dw = torch.nn.grad.conv2d_weight(_nchw(dym), wn.shape, _nchw(x), stride=stride, padding=pad).permute(0, 2, 3, 1).contiguous()
+    return dx, dw, dym.sum(dim=(0, 1, 2))
+
+
 # --------------------------------------------------------------------------- linear
 def linear_bias_act(x, w, b, relu=True):
     """FC + bias + ReLU (ref ``layers2.py:927-929``); ``w`` is ``[n_out, n_in]``."""
     y = F.linear(x, w, b)
-    return torch.relu(y) if relu else y
+    return act_fwd(y, relu)
 
 
 def linear_bias_act_bwd(x, w, y, dy, relu=True, need_dx=True):
-    if relu:
-        dy = dy * (y > 0).to(dy.dtype)
+    dy = act_bwd(dy, y, relu)
     dx = dy @ w if need_dx else None
     dw = dy.t() @ x
     db = dy.sum(0)
@@ -141,6 +189,50 @@ def softmax_xent(logits, labels):
     return loss, err1, err5, dlogits
 
 
+# --------------------------------------------------------------------------- GAN losses / noise
+def gan_loss(scores, kind, a):
+    """Loss over the critic's scores and d loss / d scores.
+    ``wgan``:  ``a * mean(o)``            (a = +1 fake / -1 real batch of the critic loss, -1 for the generator)
+    ``lsgan``: ``0.5 * mean((o - a)^2)``  (a = target: 1 real / 0 fake, 1 for the generator)."""
+    o = scores.float()
+    B = o.numel()
+    if kind == "wgan":
+        return a * o.mean(), torch.full_like(o, a / B)
+    assert kind == "lsgan", kind
+    e = o - a
+    return 0.5 * (e * e).mean(), e / B
+
+
+_PHILOX_M = (0xD2511F53, 0xCD9E8D57)
+_PHILOX_W = (0x9E3779B9, 0xBB67AE85)
+
+
+def _philox4x32(c, k0, k1):
+    """Philox4x32-10 over uint64 arrays holding 32-bit words (csrc/nn_kernels.cu: philox4x32)."""
+    M32 = np.uint64(0xFFFFFFFF)
+    c0, c1, c2, c3 = (np.asarray(v, dtype=np.uint64) & M32 for v in c)
+    k0, k1 = np.uint64(k0), np.uint64(k1)
+    for _ in range(10):
+        p0 = c0 * np.uint64(_PHILOX_M[0])
+        p1 = c2 * np.uint64(_PHILOX_M[1])
+        c0, c1, c2, c3 = ((p1 >> np.uint64(32)) ^ c1 ^ k0, p1 & M32, (p0 >> np.uint64(32)) ^ c3 ^ k1, p0 & M32)
+        k0, k1 = (k0 + np.uint64(_PHILOX_W[0])) & M32, (k1 + np.uint64(_PHILOX_W[1])) & M32
+    return c0, c1, c2, c3
+
+
+def uniform_noise(shape, seed, stream, step, device="cpu"):
+    """Uniform [0, 1) noise, bit-identical (in fp32) to the CUDA ``uniform_noise`` kernel: element i is word i % 4 of
+    Philox(counter = (i // 4, step), key = (seed, stream)) with its low 8 bits dropped, times 2^-24."""
+    n = int(np.prod(shape))
+    q = np.arange((n + 3) // 4, dtype=np.uint64)
+    seed, step = int(seed) & (2 ** 64 - 1), int(step)
+    r = _philox4x32((q, q >> np.uint64(32), np.full_like(q, step & 0xFFFFFFFF), np.full_like(q, step >> 32)),
+                    seed & 0xFFFFFFFF, ((seed >> 32) ^ int(stream)) & 0xFFFFFFFF)
+    words = np.stack(r, axis=1).reshape(-1)[:n]
+    u = (words >> np.uint64(8)).astype(np.float32) * np.float32(1.0 / 16777216.0)
+    return torch.from_numpy(u.reshape(shape)).to(device)
+
+
 # --------------------------------------------------------------------------- optimizer (flat arena)
 def sgd_flat(w, g, u, lr_mult, wd, lr, mu, nesterov, inv_k, w_half=None):
     """One momentum-SGD step over flat fp32 buffers with per-element
@@ -159,6 +251,24 @@ def sgd_flat(w, g, u, lr_mult, wd, lr, mu, nesterov, inv_k, w_half=None):
     if w_half is not None:
         w_half.copy_(w)
     return w, u
+
+
+def rmsprop_flat(w, g, v, lr_mult, wd, lr, alpha=0.99, eps=1e-8, clip=0.0, w_half=None):
+    """One RMSProp step over flat fp32 buffers, ``torch.optim.RMSprop`` without momentum, plus an optional clip:
+
+        g_eff = g + wd * w
+        v     = alpha * v + (1 - alpha) * g_eff^2
+        w    -= lr * lr_mult * g_eff / (sqrt(v) + eps)
+        w     = clamp(w, -clip, clip)                  (clip > 0: the WGAN critic's weight clipping)
+    """
+    g_eff = g + wd * w
+    v.mul_(alpha).addcmul_(g_eff, g_eff, value=1 - alpha)
+    w.sub_(lr * lr_mult * g_eff / (v.sqrt() + eps))
+    if clip > 0:
+        w.clamp_(-clip, clip)
+    if w_half is not None:
+        w_half.copy_(w)
+    return w, v
 
 
 def easgd_elastic(w, c, alpha):
@@ -222,9 +332,7 @@ def batch_norm_fwd(x, gamma, beta, run_mean, run_var, training, momentum, eps, r
     y = (xf - mean) * (rstd * gamma.float()) + beta.float()
     if res is not None:
         y = y + res.float()
-    if relu:
-        y = torch.relu(y)
-    return y.to(x.dtype), mean, rstd
+    return act_fwd(y, relu).to(x.dtype), mean, rstd
 
 
 def batch_norm_bwd(x, dy, y, gamma, mean, rstd, relu, need_dres):
@@ -232,7 +340,7 @@ def batch_norm_bwd(x, dy, y, gamma, mean, rstd, relu, need_dres):
     C = x.shape[-1]
     g = dy.float()
     if relu:
-        g = g * (y.float() > 0)
+        g = act_bwd(g, y.float(), relu)
     xh = (x.float() - mean) * rstd
     g2, xh2 = g.reshape(-1, C), xh.reshape(-1, C)
     R = g2.shape[0]

@@ -136,6 +136,37 @@ class FlatAdam(object):
         self.V.copy_(sd["V"].to(self.V.device)); self.t.fill_(int(sd["t"]))
 
 
+class FlatRMSProp(object):
+    """RMSProp over the whole arena in one native kernel (``csrc/comm_kernels.cu: rmsprop_flat_kernel``): the squared-gradient
+    average in an extra flat buffer, lr read from ``arena.hyper[0]`` on the device, the bf16 shadow refreshed in the same pass —
+    the step is CUDA-graph capturable.  ``torch.optim.RMSprop(alpha=0.99, eps=1e-8)`` without momentum, the optimizer of the
+    reference's GANs (``lasagne_model_zoo/wgan.py:18-59``), plus an optional clip of the updated weights to ``[-clip, clip]``
+    (the WGAN critic's weight clipping, folded into the same pass)."""
+
+    def __init__(self, arena, alpha=0.99, eps=1e-8, clip=0.0):
+        self.arena, self.alpha, self.eps, self.clip = arena, alpha, eps, clip
+        self.V = torch.zeros_like(arena.W)
+
+    def step(self, lr=None):
+        a = self.arena
+        nat = _native_for(a.W)
+        if nat is not None:
+            from ..ops.cuda_impl import L, _table, _p, _st
+            lrm, wd, ex = _table(a)
+            L().rmsprop_flat(a.W.data_ptr(), a.G.data_ptr(), self.V.data_ptr(), _p(a.H), a.block_group.data_ptr(), lrm, wd, ex,
+                             a.hyper.data_ptr(), float(self.alpha), float(self.eps), float(self.clip), 0, int(a.numel), _st(a.W))
+            return
+        lr = float(a.hyper[0]) if lr is None else lr
+        ref.rmsprop_flat(a.W, a.G, self.V, a.lr_mult_vector(), a.wd_vector(), lr, self.alpha, self.eps, self.clip,
+                         w_half=a.H)
+
+    def state_dict(self):
+        return {"V": self.V.detach().cpu()}
+
+    def load_state_dict(self, sd):
+        self.V.copy_(sd["V"].to(self.V.device))
+
+
 # --------------------------------------------------------------------------- classic split (API parity)
 def _ex(a):
     return a.exch_vector()
