@@ -135,6 +135,12 @@ void adam_flat(void* W, const void* G, void* M, void* V, void* H, const void* bl
                float b1, float b2, float eps, long long lo, long long hi, cudaStream_t st);
 void rmsprop_flat(void* W, const void* G, void* V, void* H, const void* block_group, const GroupTable& tab, const void* lr_ptr, float alpha,
                   float eps, float clip, long long lo, long long hi, cudaStream_t st);
+// U = the arena's update accumulator, V = the squared-gradient average (an extra flat buffer)
+void adadelta_flat(void* W, const void* G, void* U, void* V, void* H, const void* block_group, const GroupTable& tab, const void* lr_ptr,
+                   float rho, float eps, long long lo, long long hi, cudaStream_t st);
+// M = the arena's momentum region, R / S = gradient and squared-gradient averages (extra flat buffers)
+void rmsprop_centered_flat(void* W, const void* G, void* M, void* R, void* S, void* H, const void* block_group, const GroupTable& tab,
+                           const void* lr_ptr, float rho, float mu, float eps, long long lo, long long hi, cudaStream_t st);
 void fused_allreduce_sgd(const FusedArgs& a, int algo, int max_blocks, cudaStream_t st);
 // every rank pushes the fp32 master weights of the slice it owns in the two-shot partition of [lo, hi) to all peers
 void push_master_slices(const FusedArgs& a, int max_blocks, cudaStream_t st);

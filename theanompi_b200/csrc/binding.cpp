@@ -153,6 +153,14 @@ PYBIND11_MODULE(_tmpi_native, m) {
   m.def("rmsprop_flat", [](ptr_t W, ptr_t G, ptr_t V, ptr_t H, ptr_t block_group, std::vector<float> lr_mult, std::vector<float> wd,
                            std::vector<int> exch, ptr_t lr_ptr, float alpha, float eps, float clip, long long lo, long long hi, ptr_t st) {
     rmsprop_flat(P(W), P(G), P(V), P(H), P(block_group), make_table(lr_mult, wd, exch), P(lr_ptr), alpha, eps, clip, lo, hi, S(st)); });
+  m.def("adadelta_flat", [](ptr_t W, ptr_t G, ptr_t U, ptr_t V, ptr_t H, ptr_t block_group, std::vector<float> lr_mult, std::vector<float> wd,
+                            std::vector<int> exch, ptr_t lr_ptr, float rho, float eps, long long lo, long long hi, ptr_t st) {
+    adadelta_flat(P(W), P(G), P(U), P(V), P(H), P(block_group), make_table(lr_mult, wd, exch), P(lr_ptr), rho, eps, lo, hi, S(st)); });
+  m.def("rmsprop_centered_flat", [](ptr_t W, ptr_t G, ptr_t M, ptr_t R, ptr_t S_, ptr_t H, ptr_t block_group, std::vector<float> lr_mult,
+                                    std::vector<float> wd, std::vector<int> exch, ptr_t lr_ptr, float rho, float mu, float eps, long long lo,
+                                    long long hi, ptr_t st) {
+    rmsprop_centered_flat(P(W), P(G), P(M), P(R), P(S_), P(H), P(block_group), make_table(lr_mult, wd, exch), P(lr_ptr), rho, mu, eps, lo, hi,
+                          S(st)); });
   m.def("easgd_elastic", [](ptr_t w, ptr_t h, ptr_t center, float alpha, long long n, int max_blocks, ptr_t st, int lockfree) {
     easgd_elastic(P(w), P(h), P(center), alpha, n, max_blocks, lockfree, S(st)); },
     py::arg("w"), py::arg("h"), py::arg("center"), py::arg("alpha"), py::arg("n"), py::arg("max_blocks"), py::arg("st"), py::arg("lockfree") = 0);

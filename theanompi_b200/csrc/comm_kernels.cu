@@ -10,6 +10,7 @@
 //     [→ push the updated slice to the peers] → flag barrier.
 //
 //   sgd_flat            k = 1 instance (no peers): fused momentum-SGD over a block range
+//   adam_flat, rmsprop_flat, adadelta_flat, rmsprop_centered_flat   the other local optimizers, one pass over a block range each
 //   fused_oneshot_sgd   every rank reduces the whole range itself (latency-optimal, small buckets)
 //   fused_twoshot_sgd   reduce-scatter → update owned slice → push updated weights to all peers (bandwidth-optimal)
 //   fused_nvls_sgd      same with multimem.ld_reduce / multimem.st (reduction + broadcast inside the NVSwitch)
@@ -227,6 +228,99 @@ void rmsprop_flat(void* W, const void* G, void* V, void* H, const void* block_gr
   rmsprop_flat_kernel<<<grid, kThreads, 0, st>>>((float*)W, (const float*)G, (float*)V, (__nv_bfloat16*)H, (const uint8_t*)block_group, tab,
                                                  (const float*)lr_ptr, alpha, eps, clip, lo / kArenaBlock, hi / kArenaBlock);
   count_launch(); TMPI_CHECK_LAUNCH("rmsprop_flat"); ::tmpi::check_capture(st, "rmsprop_flat");
+}
+
+// ============================================================================ flat Adadelta (the LSTM's default optimizer, torch.optim.Adadelta)
+// v = rho v + (1 - rho) g^2;  d = sqrt(u + eps) / sqrt(v + eps) * g;  u = rho u + (1 - rho) d^2;  w -= lr * d.  u is the arena's U
+// region, v an extra flat buffer; lr from device memory, weight decay folded into g, bf16 shadow refreshed.
+__global__ void __launch_bounds__(kThreads) adadelta_flat_kernel(float* __restrict__ W, const float* __restrict__ G, float* __restrict__ U,
+                                                                 float* __restrict__ V, __nv_bfloat16* __restrict__ H,
+                                                                 const uint8_t* __restrict__ block_group, GroupTable tab,
+                                                                 const float* __restrict__ lr_ptr, float rho, float eps, long long blk_lo,
+                                                                 long long blk_hi) {
+  const float lr0 = *lr_ptr;
+  for (long long b = blk_lo + blockIdx.x; b < blk_hi; b += gridDim.x) {
+    const int g = block_group[b];
+    const float lr = lr0 * tab.lr_mult[g], wd = tab.wd[g];
+    const long long i = b * kArenaBlock + threadIdx.x * 4;
+    float4 w = *reinterpret_cast<const float4*>(W + i), u = *reinterpret_cast<const float4*>(U + i);
+    float4 v = *reinterpret_cast<const float4*>(V + i);
+    const float4 gg = *reinterpret_cast<const float4*>(G + i);
+#define TMPI_ADADELTA1(Wc, Uc, Vc, Gc)                                \
+  {                                                                  \
+    const float ge = Gc + wd * Wc;                                   \
+    Vc = rho * Vc + (1.f - rho) * ge * ge;                           \
+    const float d = sqrtf(Uc + eps) / sqrtf(Vc + eps) * ge;          \
+    Uc = rho * Uc + (1.f - rho) * d * d;                             \
+    Wc -= lr * d;                                                    \
+  }
+    TMPI_ADADELTA1(w.x, u.x, v.x, gg.x) TMPI_ADADELTA1(w.y, u.y, v.y, gg.y) TMPI_ADADELTA1(w.z, u.z, v.z, gg.z)
+    TMPI_ADADELTA1(w.w, u.w, v.w, gg.w)
+#undef TMPI_ADADELTA1
+    *reinterpret_cast<float4*>(W + i) = w;
+    *reinterpret_cast<float4*>(U + i) = u;
+    *reinterpret_cast<float4*>(V + i) = v;
+    if (H) *reinterpret_cast<uint2*>(H + i) = pack_bf16x4(w);
+  }
+}
+
+void adadelta_flat(void* W, const void* G, void* U, void* V, void* H, const void* block_group, const GroupTable& tab, const void* lr_ptr,
+                   float rho, float eps, long long lo, long long hi, cudaStream_t st) {
+  if (lo % kArenaBlock || hi % kArenaBlock) throw std::runtime_error("adadelta_flat: range must be block aligned");
+  const long long nb = (hi - lo) / kArenaBlock;
+  if (nb <= 0) return;
+  int grid = (int)std::min<long long>(nb, (long long)sm_count() * 8);
+  adadelta_flat_kernel<<<grid, kThreads, 0, st>>>((float*)W, (const float*)G, (float*)U, (float*)V, (__nv_bfloat16*)H, (const uint8_t*)block_group,
+                                                  tab, (const float*)lr_ptr, rho, eps, lo / kArenaBlock, hi / kArenaBlock);
+  count_launch(); TMPI_CHECK_LAUNCH("adadelta_flat"); ::tmpi::check_capture(st, "adadelta_flat");
+}
+
+// ============================================================================ flat centred RMSProp with momentum (the reference LSTM's rmsprop)
+// r = rho r + (1 - rho) g;  s = rho s + (1 - rho) g^2;  m = mu m - lr * g / sqrt(s - r^2 + eps);  w += m.  m is the arena's U region,
+// r and s are extra flat buffers; eps sits inside the square root.  lr from device memory, weight decay folded into g, bf16 shadow
+// refreshed.
+__global__ void __launch_bounds__(kThreads) rmsprop_centered_flat_kernel(float* __restrict__ W, const float* __restrict__ G,
+                                                                         float* __restrict__ M, float* __restrict__ R, float* __restrict__ S,
+                                                                         __nv_bfloat16* __restrict__ H, const uint8_t* __restrict__ block_group,
+                                                                         GroupTable tab, const float* __restrict__ lr_ptr, float rho, float mu,
+                                                                         float eps, long long blk_lo, long long blk_hi) {
+  const float lr0 = *lr_ptr;
+  for (long long b = blk_lo + blockIdx.x; b < blk_hi; b += gridDim.x) {
+    const int g = block_group[b];
+    const float lr = lr0 * tab.lr_mult[g], wd = tab.wd[g];
+    const long long i = b * kArenaBlock + threadIdx.x * 4;
+    float4 w = *reinterpret_cast<const float4*>(W + i), m = *reinterpret_cast<const float4*>(M + i);
+    float4 r = *reinterpret_cast<const float4*>(R + i), s = *reinterpret_cast<const float4*>(S + i);
+    const float4 gg = *reinterpret_cast<const float4*>(G + i);
+#define TMPI_CRMS1(Wc, Mc, Rc, Sc, Gc)                                \
+  {                                                                  \
+    const float ge = Gc + wd * Wc;                                   \
+    Rc = rho * Rc + (1.f - rho) * ge;                                \
+    Sc = rho * Sc + (1.f - rho) * ge * ge;                           \
+    Mc = mu * Mc - lr * ge / sqrtf(Sc - Rc * Rc + eps);              \
+    Wc += Mc;                                                        \
+  }
+    TMPI_CRMS1(w.x, m.x, r.x, s.x, gg.x) TMPI_CRMS1(w.y, m.y, r.y, s.y, gg.y) TMPI_CRMS1(w.z, m.z, r.z, s.z, gg.z)
+    TMPI_CRMS1(w.w, m.w, r.w, s.w, gg.w)
+#undef TMPI_CRMS1
+    *reinterpret_cast<float4*>(W + i) = w;
+    *reinterpret_cast<float4*>(M + i) = m;
+    *reinterpret_cast<float4*>(R + i) = r;
+    *reinterpret_cast<float4*>(S + i) = s;
+    if (H) *reinterpret_cast<uint2*>(H + i) = pack_bf16x4(w);
+  }
+}
+
+void rmsprop_centered_flat(void* W, const void* G, void* M, void* R, void* S, void* H, const void* block_group, const GroupTable& tab,
+                           const void* lr_ptr, float rho, float mu, float eps, long long lo, long long hi, cudaStream_t st) {
+  if (lo % kArenaBlock || hi % kArenaBlock) throw std::runtime_error("rmsprop_centered_flat: range must be block aligned");
+  const long long nb = (hi - lo) / kArenaBlock;
+  if (nb <= 0) return;
+  int grid = (int)std::min<long long>(nb, (long long)sm_count() * 8);
+  rmsprop_centered_flat_kernel<<<grid, kThreads, 0, st>>>((float*)W, (const float*)G, (float*)M, (float*)R, (float*)S, (__nv_bfloat16*)H,
+                                                          (const uint8_t*)block_group, tab, (const float*)lr_ptr, rho, mu, eps,
+                                                          lo / kArenaBlock, hi / kArenaBlock);
+  count_launch(); TMPI_CHECK_LAUNCH("rmsprop_centered_flat"); ::tmpi::check_capture(st, "rmsprop_centered_flat");
 }
 
 // ============================================================================ fused collectives

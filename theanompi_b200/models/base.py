@@ -102,7 +102,9 @@ class ModelBase(object):
         self._gstream = None
         self._warm = 0
         self._tail = None
-        self.exchanger = None          # set by the BSP worker for fused / overlapped exchange
+        self._graphs = {}              # keyed step graphs (run_keyed_step)
+        self._graph_pool = None
+        self.exchanger = None         # set by the BSP worker for fused / overlapped exchange
         self.h2d_bytes_last = 0
 
     # ------------------------------------------------------------------ construction helpers
@@ -265,6 +267,40 @@ class ModelBase(object):
             raise
         torch.cuda.current_stream().wait_stream(s)
         self._graph, self._graph_out = g, out
+
+    def run_keyed_step(self, key, body):
+        """Run ``body()`` — a whole training step that reads only static buffers — as a replay of the CUDA graph captured for
+        ``key`` (any hashable: a step kind, a sequence-length bucket, ...).  Without graphs (CPU, ``cuda_graph=False``) ``body`` runs
+        eagerly.  Per key: two eager warm-up runs on the capture stream (the protocol of :meth:`forward_backward`), then the
+        capture, then replays.  All keys share one capture stream and one graph memory pool: their graphs never replay
+        concurrently.  A replay overwrites the previous outputs, so the returned tensors are copies."""
+        if not self.use_graph:
+            return body()
+        if self._gstream is None:
+            self._gstream = torch.cuda.Stream(device=self.device)
+        st = self._graphs.get(key)
+        if st is None:
+            st = self._graphs[key] = {"warm": 0, "graph": None, "out": None}
+        if st["graph"] is None:
+            s, cur = self._gstream, torch.cuda.current_stream(self.device)
+            s.wait_stream(cur)
+            if st["warm"] < 2:
+                st["warm"] += 1
+                with torch.cuda.stream(s):
+                    out = body()
+                cur.wait_stream(s)
+                return out
+            if self._graph_pool is None:
+                self._graph_pool = torch.cuda.graph_pool_handle()
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.stream(s):
+                with torch.cuda.graph(g, pool=self._graph_pool, stream=s, capture_error_mode="thread_local"):
+                    out = body()
+            cur.wait_stream(s)
+            st["graph"], st["out"] = g, out
+        st["graph"].replay()
+        out = st["out"]
+        return tuple(t.clone() for t in out) if isinstance(out, tuple) else out.clone()
 
     def set_step_tail(self, fn):
         """Register work that runs right after backward as part of the step — and

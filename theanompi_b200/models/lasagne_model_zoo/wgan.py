@@ -295,7 +295,6 @@ class NativeWGAN(ModelBase):
         self._val_gen = self.data.iterate("val", shuffle=False)
         self.data.n_batch_train = self.epochsize
         self.data.n_batch_val = 1
-        self._graphs = {}
         self._cuda_impl = cuda_impl if self.cuda else None
 
     make_data = WGAN.make_data
@@ -372,32 +371,8 @@ class NativeWGAN(ModelBase):
         return loss.detach()
 
     def _run(self, kind):
-        """Eager on the CPU / without graphs; on the GPU: two eager warm-up runs on the capture stream, then capture, then
-        replays (the ModelBase protocol, once per step kind)."""
-        body = self._critic_body if kind == "critic" else self._gen_body
-        if not self.use_graph:
-            return body()
-        st = self._graphs.get(kind)
-        if st is None:
-            st = self._graphs[kind] = {"warm": 0, "graph": None, "stream": torch.cuda.Stream(device=self.device)}
-        s = st["stream"]
-        if st["graph"] is None:
-            cur = torch.cuda.current_stream(self.device)
-            s.wait_stream(cur)
-            if st["warm"] < 2:
-                st["warm"] += 1
-                with torch.cuda.stream(s):
-                    out = body()
-                cur.wait_stream(s)
-                return out
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.stream(s):
-                with torch.cuda.graph(g, stream=s, capture_error_mode="thread_local"):
-                    out = body()
-            cur.wait_stream(s)
-            st["graph"], st["out"] = g, out
-        st["graph"].replay()
-        return st["out"].clone()
+        """Eager on the CPU / without graphs; on the GPU one captured graph per step kind (:meth:`ModelBase.run_keyed_step`)."""
+        return self.run_keyed_step(kind, self._critic_body if kind == "critic" else self._gen_body)
 
     # ---- contract
     def compile_iter_fns(self, sync_type="avg", **kw):

@@ -6,9 +6,11 @@ its model-contract adapter ``lstm_theanompi_outdated.py`` with rank-sharded ``IM
 ``LSTM`` runs on the hand-written kernels: embedding gather / scatter, the input projection of all time steps as one
 wgmma GEMM, the masked recurrence as ONE autograd node (per step: one small GEMM + one fused cell kernel; the recurrent
 weight gradient of the whole sequence is a single GEMM), masked mean pooling, dropout, softmax head (``ops/rnn.py``,
-``csrc/rnn_kernels.cu``).  ``LSTMTorch`` is the same model on ``torch.nn.LSTM`` (cuDNN), kept as the library yardstick.
-Sequences are never split across devices (the reference has no sequence parallelism, SURVEY §5.7).  Without the IMDB pickle
-a synthetic corpus with class-dependent token statistics is generated.
+``csrc/rnn_kernels.cu``), and the update as one flat optimizer launch (Adadelta, the reference's centred RMSProp or SGD,
+``config['optimizer']``); on the GPU each step is a CUDA graph per sequence-length bucket.  ``LSTMTorch`` is the same model on
+``torch.nn.LSTM`` (cuDNN), kept as the library yardstick.  Sequences are never split across devices (the reference has no
+sequence parallelism, SURVEY §5.7).  Without the IMDB pickle a synthetic corpus with class-dependent token statistics is
+generated, with lengths drawn from ``data_kwargs['seq_len'] = (lo, hi)``.
 """
 from __future__ import annotations
 
@@ -30,7 +32,7 @@ max_epochs = 100
 
 
 class IMDB_Data(object):
-    def __init__(self, rank=0, size=1, n_synthetic=512, seed=0, maxlen=maxlen, n_words=n_words):
+    def __init__(self, rank=0, size=1, n_synthetic=512, seed=0, maxlen=maxlen, n_words=n_words, seq_len=(20, 80)):
         path = os.environ.get("TMPI_IMDB_PATH", "./imdb.pkl")
         rs = np.random.RandomState(seed)
         if os.path.exists(path):
@@ -43,7 +45,7 @@ class IMDB_Data(object):
             ys = rs.randint(0, 2, n_synthetic)
             xs = []
             for y in ys:
-                L = rs.randint(20, 80)
+                L = min(rs.randint(*seq_len), maxlen)                           # lengths drawn from [lo, hi)
                 base = rs.randint(2, n_words, L)
                 marks = rs.rand(L) < 0.3
                 base[marks] = (2 + y * 50 + rs.randint(0, 50, marks.sum()))        # sentiment-bearing tokens
@@ -80,16 +82,48 @@ class LSTMNet(nn.Module):
         return self.out(self.drop(pooled))
 
 
+BUCKET = 16                 # graph buckets: the time length of a batch is padded up to a multiple of this
+
+
+def bucket_len(T, maxlen):
+    """Time length of the graph bucket that holds a batch of ``T`` steps: ``T`` rounded up to a multiple of :data:`BUCKET`, capped at
+    the bucket that holds ``maxlen``."""
+    cap = -(-maxlen // BUCKET) * BUCKET
+    if T > cap:
+        raise ValueError("batch of %d time steps is longer than maxlen %d" % (T, maxlen))
+    return min(-(-T // BUCKET) * BUCKET, cap)
+
+
+def pad_batch(x, m, T):
+    """Pad a ``[B, t]`` batch to ``T`` steps with token id 0 and mask 0 (the masked carry makes padded steps no-ops)."""
+    xp, mp = np.zeros((x.shape[0], T), dtype=x.dtype), np.zeros((m.shape[0], T), dtype=m.dtype)
+    xp[:, :x.shape[1]], mp[:, :m.shape[1]] = x, m
+    return xp, mp
+
+
 class LSTM(ModelBase):
+    """``config['optimizer']``: ``'adadelta'`` (default, lr 1.0), ``'rmsprop'`` (the reference's centred RMSProp with momentum,
+    lr 1e-4) or ``'sgd'`` (``p - lr·g``, lr 1e-4), the three optimizers of the reference's ``train_lstm``; ``learning_rate``
+    overrides the lr.  Each is one flat native launch over the arena.  On the GPU every training step is one CUDA graph per
+    sequence-length bucket (:func:`bucket_len`): the batch is padded to its bucket, copied into the bucket's static buffers and
+    the bucket's graph (forward, backward, update) is replayed.  ``cuda_graph=False`` and the CPU run the step eagerly on the
+    unpadded batch; validation is always eager."""
     n_epochs = max_epochs
     batch_size = file_batch_size = batch_size
     learning_rate = 1.0
     weight_decay = 0.0
     bias_lr_mult = 1.0
+    optimizers = {"adadelta": 1.0, "rmsprop": 1e-4, "sgd": 1e-4}        # default lr per optimizer (ref train_lstm)
 
     def __init__(self, config):
         super().__init__(config)
         self.name = "LSTM"
+        self.opt_name = config.get("optimizer", "adadelta")
+        if self.opt_name not in self.optimizers:
+            raise ValueError("LSTM optimizer must be one of %s, not %r" % (sorted(self.optimizers), self.opt_name))
+        self.learning_rate = float(config.get("learning_rate", self.optimizers[self.opt_name]))
+        self.base_lr = np.float32(self.learning_rate)
+        self.opt = None
         from . import layers2
         from .layers2 import Constant, Normal, _tag
         layers2.reseed(123)
@@ -117,6 +151,7 @@ class LSTM(ModelBase):
         self.best_err, self.bad_counter, self.patience = 1.0, 0, config.get("patience", patience)
         self._train_it = None
         self.training = True
+        self._buckets = {}
 
     def forward_logits(self, x, mask):
         """x: int64 [B, T] token ids, mask: float [B, T]."""
@@ -132,17 +167,67 @@ class LSTM(ModelBase):
         pooled = ops.dropout(pooled, 0.5, self.training, layer_id=0)
         return ops.linear_bias_act(pooled, self.Wo.val, self.bo.val, False)
 
+    def _make_opt(self):
+        if self.opt is None:
+            from ..utils.opt import FlatAdadelta, FlatCenteredRMSProp, FlatSGD
+            if self.opt_name == "adadelta":
+                self.opt = FlatAdadelta(self.arena)                    # ref :284-342
+            elif self.opt_name == "rmsprop":
+                self.opt = FlatCenteredRMSProp(self.arena)             # ref :376-402
+            else:
+                self.opt = FlatSGD(self.arena, mu=0.0, use_momentum=False)       # ref :256-281: p - lr·g
+        return self.opt
+
     def compile_iter_fns(self, sync_type="avg", **kw):
         self.sync_type = "avg"
-        self.torch_opt = torch.optim.Adadelta(self.params, lr=1.0, rho=0.95, eps=1e-6)     # ref :284-342
+        self._make_opt()
         self.vels, self.vels2 = [], []
 
     def _to(self, x, m, y):
         d = self.device
         return torch.from_numpy(x).to(d), torch.from_numpy(m).to(d), torch.from_numpy(y).to(d)
 
-    def train_iter(self, count, recorder):
+    def _train_body(self, x, m, y):
+        """Forward, backward and the flat update of one batch (device tensors); returns device scalars (cost, error)."""
         from .. import ops
+        self.arena.G.zero_()
+        cost, err, _ = ops.softmax_xent(self.forward_logits(x, m), y)
+        cost.backward()                                            # the kernels write the gradients into the arena's G views
+        with torch.no_grad():
+            if self.opt_name == "sgd":
+                self.opt.step(self.shared_lr.get_value())          # (the native kernel reads lr from the device)
+            else:
+                self.opt.step()
+        self._after_step()
+        return cost.detach(), err.detach()
+
+    def _stage(self, x, m, y):
+        """Copy a batch, padded to its bucket, into the bucket's static device buffers (one H2D copy from pinned staging).
+        Returns the bucket length and the static ``(x, mask, y)``."""
+        Tb = bucket_len(x.shape[1], self.data.maxlen)
+        b = self._buckets.get(Tb)
+        if b is None:
+            B = self.batch_size
+            nx, nm = B * Tb * 8, B * Tb * 4
+
+            def views(raw):
+                return (raw[:nx].view(torch.int64).view(B, Tb), raw[nx:nx + nm].view(torch.float32).view(B, Tb),
+                        raw[nx + nm:].view(torch.int64))
+            pin = torch.zeros(nx + nm + B * 8, dtype=torch.uint8, pin_memory=True)
+            dev = torch.zeros(nx + nm + B * 8, dtype=torch.uint8, device=self.device)
+            b = self._buckets[Tb] = {"pin": pin, "dev": dev, "host": views(pin), "static": views(dev), "event": None}
+        if b["event"] is not None:
+            b["event"].synchronize()          # the host runs ahead of the device: the last copy out of this staging buffer has run
+        xp, mp = pad_batch(x, m, Tb)
+        hx, hm, hy = b["host"]
+        hx.numpy()[:] = xp; hm.numpy()[:] = mp; hy.numpy()[:] = y
+        b["dev"].copy_(b["pin"], non_blocking=True)
+        if b["event"] is None:
+            b["event"] = torch.cuda.Event()
+        b["event"].record(torch.cuda.current_stream(self.device))
+        return Tb, b["static"]
+
+    def train_iter(self, count, recorder):
         if self._train_it is None:
             self._train_it = self.data.batches("train", self.batch_size, True, seed=self.epoch)
         try:
@@ -151,18 +236,13 @@ class LSTM(ModelBase):
             self._train_it = self.data.batches("train", self.batch_size, True, seed=self.epoch + 1000)
             x, m, y = next(self._train_it)
         recorder.start()
-        x, m, y = self._to(x, m, y)
         self.training = True
-        self.arena.G.zero_()
-        logits = self.forward_logits(x, m)
-        cost, err, _ = ops.softmax_xent(logits, y)
-        cost.backward()
-        for p in self.params:                                      # the kernels wrote the gradients into the arena's G views
-            p.grad = p.gbuf
-        self.torch_opt.step()
-        self.arena.refresh_shadow()
-        self._after_step()
-        recorder.train_error(count, cost.detach(), err.detach())
+        if self.use_graph:
+            Tb, (xs, ms, ys) = self._stage(x, m, y)
+            cost, err = self.run_keyed_step(Tb, lambda: self._train_body(xs, ms, ys))
+        else:
+            cost, err = self._train_body(*self._to(x, m, y))
+        recorder.train_error(count, cost, err)
         recorder.end("calc")
 
     def val_iter(self, count, recorder):
@@ -186,6 +266,21 @@ class LSTM(ModelBase):
             if self.bad_counter > self.patience:
                 return "stop"
         return self.data.n_batch_val            # one call covers the whole validation set
+
+    def extra_state(self):
+        """The optimizer's extra buffers (its U-region state travels with the arena), its name and the early-stopping state."""
+        opt = self._make_opt()
+        return {"optimizer": self.opt_name, "opt": opt.state_dict() if hasattr(opt, "state_dict") else {},
+                "best_err": self.best_err, "bad_counter": self.bad_counter}
+
+    def load_extra_state(self, sd):
+        if sd.get("optimizer") != self.opt_name:
+            raise ValueError("checkpoint was written by an LSTM trained with optimizer %r; this model uses %r"
+                             % (sd.get("optimizer"), self.opt_name))
+        opt = self._make_opt()
+        if hasattr(opt, "load_state_dict"):
+            opt.load_state_dict(sd["opt"])
+        self.best_err, self.bad_counter = float(sd["best_err"]), int(sd["bad_counter"])
 
     def reset_iter(self, mode):
         if mode == "train":

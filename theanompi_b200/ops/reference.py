@@ -271,6 +271,44 @@ def rmsprop_flat(w, g, v, lr_mult, wd, lr, alpha=0.99, eps=1e-8, clip=0.0, w_hal
     return w, v
 
 
+def adadelta_flat(w, g, u, v, lr_mult, wd, lr, rho=0.95, eps=1e-6, w_half=None):
+    """One Adadelta step over flat fp32 buffers, ``torch.optim.Adadelta`` (the reference LSTM's ``adadelta`` at lr = 1):
+
+        g_eff = g + wd * w
+        v     = rho * v + (1 - rho) * g_eff^2
+        d     = sqrt(u + eps) / sqrt(v + eps) * g_eff
+        u     = rho * u + (1 - rho) * d^2
+        w    -= lr * lr_mult * d
+    """
+    g_eff = g + wd * w
+    v.mul_(rho).addcmul_(g_eff, g_eff, value=1 - rho)
+    d = (u + eps).sqrt_().div_((v + eps).sqrt_()).mul_(g_eff)
+    u.mul_(rho).addcmul_(d, d, value=1 - rho)
+    w.sub_(lr * lr_mult * d)
+    if w_half is not None:
+        w_half.copy_(w)
+    return w, u, v
+
+
+def rmsprop_centered_flat(w, g, m, r, s, lr_mult, wd, lr, rho=0.95, mu=0.9, eps=1e-4, w_half=None):
+    """One step of the reference LSTM's ``rmsprop`` (centred, with momentum, eps inside the square root) over flat fp32 buffers:
+
+        g_eff = g + wd * w
+        r     = rho * r + (1 - rho) * g_eff
+        s     = rho * s + (1 - rho) * g_eff^2
+        m     = mu * m - lr * lr_mult * g_eff / sqrt(s - r^2 + eps)
+        w    += m
+    """
+    g_eff = g + wd * w
+    r.mul_(rho).add_(g_eff, alpha=1 - rho)
+    s.mul_(rho).addcmul_(g_eff, g_eff, value=1 - rho)
+    m.mul_(mu).sub_(lr * lr_mult * g_eff / (s - r * r + eps).sqrt())
+    w.add_(m)
+    if w_half is not None:
+        w_half.copy_(w)
+    return w, m, r, s
+
+
 def easgd_elastic(w, c, alpha):
     """EASGD elastic move (ref ``exchanger.py:188-211``) with both sides updated
     from the SAME difference: ``d = alpha (w - c); w -= d; c += d``."""

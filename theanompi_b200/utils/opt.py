@@ -167,6 +167,67 @@ class FlatRMSProp(object):
         self.V.copy_(sd["V"].to(self.V.device))
 
 
+class FlatAdadelta(object):
+    """Adadelta over the whole arena in one native kernel (``csrc/comm_kernels.cu: adadelta_flat_kernel``): the update accumulator
+    in the arena's U region (saved with the arena), the squared-gradient average in an extra flat buffer, lr read from
+    ``arena.hyper[0]`` on the device, the bf16 shadow refreshed in the same pass — the step is CUDA-graph capturable.
+    ``torch.optim.Adadelta(rho=0.95, eps=1e-6)``, which at lr = 1 is the reference LSTM's ``adadelta`` (``models/lstm.py:284-342``)."""
+
+    def __init__(self, arena, rho=0.95, eps=1e-6):
+        self.arena, self.rho, self.eps = arena, rho, eps
+        self.V = torch.zeros_like(arena.W)
+
+    def step(self, lr=None):
+        a = self.arena
+        nat = _native_for(a.W)
+        if nat is not None:
+            from ..ops.cuda_impl import L, _table, _p, _st
+            lrm, wd, ex = _table(a)
+            L().adadelta_flat(a.W.data_ptr(), a.G.data_ptr(), a.U.data_ptr(), self.V.data_ptr(), _p(a.H), a.block_group.data_ptr(), lrm, wd,
+                              ex, a.hyper.data_ptr(), float(self.rho), float(self.eps), 0, int(a.numel), _st(a.W))
+            return
+        lr = float(a.hyper[0]) if lr is None else lr
+        ref.adadelta_flat(a.W, a.G, a.U, self.V, a.lr_mult_vector(), a.wd_vector(), lr, self.rho, self.eps, w_half=a.H)
+
+    def state_dict(self):
+        return {"V": self.V.detach().cpu()}
+
+    def load_state_dict(self, sd):
+        self.V.copy_(sd["V"].to(self.V.device))
+
+
+class FlatCenteredRMSProp(object):
+    """The reference LSTM's ``rmsprop`` (``models/lstm.py:376-402``: centred, momentum 0.9, eps 1e-4 inside the square root) over
+    the whole arena in one native kernel (``csrc/comm_kernels.cu: rmsprop_centered_flat_kernel``): the momentum in the arena's U
+    region, the gradient and squared-gradient averages in two extra flat buffers, lr read from ``arena.hyper[0]`` on the device,
+    the bf16 shadow refreshed in the same pass — the step is CUDA-graph capturable."""
+
+    def __init__(self, arena, rho=0.95, mu=0.9, eps=1e-4):
+        self.arena, self.rho, self.mu, self.eps = arena, rho, mu, eps
+        self.R = torch.zeros_like(arena.W)
+        self.S = torch.zeros_like(arena.W)
+
+    def step(self, lr=None):
+        a = self.arena
+        nat = _native_for(a.W)
+        if nat is not None:
+            from ..ops.cuda_impl import L, _table, _p, _st
+            lrm, wd, ex = _table(a)
+            L().rmsprop_centered_flat(a.W.data_ptr(), a.G.data_ptr(), a.U.data_ptr(), self.R.data_ptr(), self.S.data_ptr(), _p(a.H),
+                                      a.block_group.data_ptr(), lrm, wd, ex, a.hyper.data_ptr(), float(self.rho), float(self.mu),
+                                      float(self.eps), 0, int(a.numel), _st(a.W))
+            return
+        lr = float(a.hyper[0]) if lr is None else lr
+        ref.rmsprop_centered_flat(a.W, a.G, a.U, self.R, self.S, a.lr_mult_vector(), a.wd_vector(), lr, self.rho, self.mu, self.eps,
+                                  w_half=a.H)
+
+    def state_dict(self):
+        return {"R": self.R.detach().cpu(), "S": self.S.detach().cpu()}
+
+    def load_state_dict(self, sd):
+        self.R.copy_(sd["R"].to(self.R.device)); self.S.copy_(sd["S"].to(self.S.device))
+
+
 # --------------------------------------------------------------------------- classic split (API parity)
 def _ex(a):
     return a.exch_vector()
