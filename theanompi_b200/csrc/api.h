@@ -61,6 +61,10 @@ int gemm_plan_tall(long long M, int nt, int out_bf16, int sms);   // 1 = 256-row
 // f32 = 1: fp32 operands through wgmma tf32 (fp32 output), else bf16 operands
 void gemm(const void* A, const void* B, void* C, const float* bias, int M, int N, int K, long long lda, long long ldb, long long ldc,
           int a_mn, int b_mn, int out_bf16, int bias_mode, int relu, float alpha, int bn_hint, int splitk, int f32, cudaStream_t st);
+// FC weight gradient A^T B (A: [K, M], B: [K, N], both MN-major) applied as a momentum-SGD step to W / U [M, N] (fp32, row pitch
+// ldw) and the bf16 shadow H (may be null) in the GEMM epilogue, the same arithmetic as sgd_flat; lr is read from lr_ptr[0]
+void gemm_sgd(const void* A, const void* B, void* W, void* U, void* H, const void* lr_ptr, float lr_mult, float wd, float mu, int nesterov,
+              float inv_k, int M, int N, int K, long long lda, long long ldb, long long ldw, int f32, cudaStream_t st);
 
 void conv_fprop(const void* x, const void* w, void* y, const float* bias, int N, int H, int W, int Ctot, int c_off, int Cg, int KH,
                 int KW, int Ho, int Wo, int S, int P, int O, long long ldc, int relu, int dgrad, int f32, cudaStream_t st);

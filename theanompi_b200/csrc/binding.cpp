@@ -59,6 +59,12 @@ PYBIND11_MODULE(_tmpi_native, m) {
   }, py::arg("A"), py::arg("B"), py::arg("C"), py::arg("bias"), py::arg("M"), py::arg("N"), py::arg("K"), py::arg("lda"), py::arg("ldb"),
      py::arg("ldc"), py::arg("a_mn"), py::arg("b_mn"), py::arg("out_bf16"), py::arg("bias_mode"), py::arg("relu"), py::arg("alpha"),
      py::arg("bn_hint"), py::arg("splitk"), py::arg("f32"), py::arg("st"));
+  m.def("gemm_sgd", [](ptr_t A, ptr_t B, ptr_t W, ptr_t U, ptr_t H, ptr_t lr_ptr, float lr_mult, float wd, float mu, int nesterov, float inv_k,
+                       int M, int N, int K, long long lda, long long ldb, long long ldw, int f32, ptr_t st) {
+    gemm_sgd(P(A), P(B), P(W), P(U), P(H), P(lr_ptr), lr_mult, wd, mu, nesterov, inv_k, M, N, K, lda, ldb, ldw, f32, S(st));
+  }, py::arg("A"), py::arg("B"), py::arg("W"), py::arg("U"), py::arg("H"), py::arg("lr_ptr"), py::arg("lr_mult"), py::arg("wd"),
+     py::arg("mu"), py::arg("nesterov"), py::arg("inv_k"), py::arg("M"), py::arg("N"), py::arg("K"), py::arg("lda"), py::arg("ldb"),
+     py::arg("ldw"), py::arg("f32"), py::arg("st"));
 
   // convolution strides are named Sd (S is the stream cast)
   m.def("conv_fprop", [](ptr_t x, ptr_t w, ptr_t y, ptr_t bias, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho, int Wo,

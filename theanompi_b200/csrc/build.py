@@ -27,9 +27,9 @@ SO_PATH = os.path.join(PKG, "_tmpi_native.so")
 OBJ_DIR = os.path.join(HERE, "_obj")
 STAMP = os.path.join(PKG, "_tmpi_native.hash")
 
-CU_SOURCES = ["gemm_wgmma.cu", "nn_kernels.cu", "bn_kernels.cu", "rnn_kernels.cu", "comm_kernels.cu"]
+CU_SOURCES = ["gemm_wgmma.cu", "gemm_sgd.cu", "nn_kernels.cu", "bn_kernels.cu", "rnn_kernels.cu", "comm_kernels.cu"]
 CPP_SOURCES = ["peer_arena.cpp", "binding.cpp"]
-HEADERS = ["common.cuh", "api.h", "peer_arena.h"]
+HEADERS = ["common.cuh", "gemm_wgmma.cuh", "api.h", "peer_arena.h"]
 
 CUDA_HOME = os.environ.get("CUDA_HOME", "/usr/local/cuda")
 NVCC = os.path.join(CUDA_HOME, "bin", "nvcc")

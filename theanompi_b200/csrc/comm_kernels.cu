@@ -59,10 +59,6 @@ __device__ __forceinline__ void mc_st_f4(float* mc, float4 v) {
 __device__ __forceinline__ void mc_st_u2(void* mc, uint2 v) {
   asm volatile("multimem.st.relaxed.sys.global.v2.f32 [%0], {%1, %2};" ::"l"(mc), "f"(__uint_as_float(v.x)), "f"(__uint_as_float(v.y)) : "memory");
 }
-__device__ __forceinline__ uint2 pack_bf16x4(float4 v) {
-  __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
-  uint2 r; r.x = *reinterpret_cast<uint32_t*>(&a); r.y = *reinterpret_cast<uint32_t*>(&b); return r;
-}
 __device__ __forceinline__ float4 unpack_bf16x4(uint2 u) {
   float2 a = __bfloat1622float2(*reinterpret_cast<__nv_bfloat162*>(&u.x)), b = __bfloat1622float2(*reinterpret_cast<__nv_bfloat162*>(&u.y));
   return make_float4(a.x, a.y, b.x, b.y);
@@ -95,21 +91,6 @@ __device__ __forceinline__ void block_barrier(const CommCtx& c) {
   }
   __syncthreads();
   if (threadIdx.x == 0) *ep = target;
-}
-
-// ------------------------------------------------------------------ the SGD math (one float4)
-struct Hyper { float lr, mu, inv_k; int nesterov; };
-
-__device__ __forceinline__ void sgd4(float4& w, float4& u, const float4& gsum, const Hyper& h, float lrm, float wd) {
-  const float lr = h.lr * lrm;
-#define TMPI_SGD1(W, U, G)                                   \
-  {                                                          \
-    const float ge = G * h.inv_k + wd * W;                   \
-    U = h.mu * U + ge;                                       \
-    W -= lr * (h.nesterov ? (ge + h.mu * U) : U);            \
-  }
-  TMPI_SGD1(w.x, u.x, gsum.x) TMPI_SGD1(w.y, u.y, gsum.y) TMPI_SGD1(w.z, u.z, gsum.z) TMPI_SGD1(w.w, u.w, gsum.w)
-#undef TMPI_SGD1
 }
 
 // ============================================================================ k = 1: local fused SGD

@@ -114,6 +114,28 @@ template <int ACT> __device__ __forceinline__ float act_bwd(float d, float y, fl
   return d;
 }
 
+__device__ __forceinline__ uint2 pack_bf16x4(float4 v) {
+  __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
+  uint2 r; r.x = *reinterpret_cast<uint32_t*>(&a); r.y = *reinterpret_cast<uint32_t*>(&b); return r;
+}
+
+// ------------------------------------------------------------------ the SGD math (one float4)
+// Shared by the flat optimizer kernels (comm_kernels.cu) and the SGD epilogue of the wgrad GEMM (gemm_wgmma.cu): both must
+// produce the same bits for the same (W, U, G).
+struct Hyper { float lr, mu, inv_k; int nesterov; };
+
+__device__ __forceinline__ void sgd4(float4& w, float4& u, const float4& gsum, const Hyper& h, float lrm, float wd) {
+  const float lr = h.lr * lrm;
+#define TMPI_SGD1(W, U, G)                                   \
+  {                                                          \
+    const float ge = G * h.inv_k + wd * W;                   \
+    U = h.mu * U + ge;                                       \
+    W -= lr * (h.nesterov ? (ge + h.mu * U) : U);            \
+  }
+  TMPI_SGD1(w.x, u.x, gsum.x) TMPI_SGD1(w.y, u.y, gsum.y) TMPI_SGD1(w.z, u.z, gsum.z) TMPI_SGD1(w.w, u.w, gsum.w)
+#undef TMPI_SGD1
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -455,6 +455,11 @@ class ModelBase(object):
 
     def grad_norms(self):
         """L2 grad-norm monitor (ref ``alex_net.py:311-320``): (sum, max) of log10 norms."""
+        armed = [p for p in self.arena.params if getattr(p, "sgd_epilogue", None) is not None]
+        if armed:
+            # their wgrad GEMMs apply the update instead of writing G (utils/opt.py: FlatSGD.arm)
+            raise RuntimeError("grad_norms(): %d weights are updated in their wgrad GEMM epilogue and have no gradient in G; set "
+                               "monitor_grad = True before compile_iter_fns()" % len(armed))
         norms = torch.stack([g.float().norm() for g in self.arena.views("G")]).clamp_min(1e-30).log10()
         return [float(norms.sum()), float(norms.max())]
 

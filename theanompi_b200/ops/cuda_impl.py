@@ -166,19 +166,42 @@ def maxpool_relu_bias_bwd(dyp, arg, y, pool, db0, db1=None):
     return dym
 
 
-def linear_bias_act_bwd(x, w, y, dy, relu, need_dx, dw_out=None, db_out=None):
+def gemm_sgd(a, b, p, M, N, K, lda, ldb):
+    """Weight gradient ``op(a)^T op(b)`` of the armed parameter ``p`` (``utils.opt.FlatSGD.arm``) applied as its momentum-SGD
+    step inside the GEMM epilogue: ``p`` (fp32 master in the arena), its momentum and its bf16 shadow are updated in place and
+    the gradient is never written.  Same arithmetic and lr source (``arena.hyper[0]``) as ``sgd_flat``."""
+    arena, sgd = p.arena, p.sgd_epilogue
+    lrm, wd, _ = _table(arena)
+    g = p.arena_group
+    off = p.arena_off
+    u = arena.U[off:off + p.numel()]
+    L().gemm_sgd(a.data_ptr(), b.data_ptr(), p.data_ptr(), u.data_ptr(), _p(p.shadow), arena.hyper.data_ptr(), float(lrm[g]),
+                 float(wd[g]), float(sgd.mu), int(bool(sgd.nesterov)), 1.0, int(M), int(N), int(K), int(lda), int(ldb),
+                 int(p.shape[1]), int(_is32(a)), _st(a))
+
+
+def linear_bias_act_bwd(x, w, y, dy, relu, need_dx, dw_out=None, db_out=None, sgd_param=None):
+    """``sgd_param``: the master weight armed for the SGD epilogue (see :func:`gemm_sgd`); its gradient is then applied rather
+    than returned (``dw`` is None)."""
     x2 = _bf(x).contiguous()
     dy = _bf(dy).contiguous()
     B_, I = x2.shape
     O = w.shape[0]
     al = _al(x2)
     if O % al or I % al:
+        if sgd_param is not None:
+            raise RuntimeError("linear_bias_act_bwd: weight %s is armed for the GEMM SGD epilogue but needs the padded path"
+                               % (tuple(w.shape),))
         return _linear_bwd_padded(x2, w, y, dy, relu, need_dx, dw_out, db_out)
     dym, db = _mask_and_bias_grad(dy, y, relu, db_out.view(-1) if db_out is not None else None, B_, O, O)
     wb = _bf(w)
     dx = None
     if need_dx:
         dx = gemm(dym, wb, B_, I, O, a_mn=False, b_mn=True, lda=O, ldb=I)
+    if sgd_param is not None:
+        # after the dx GEMM, which reads the weights of this step
+        gemm_sgd(dym, x2, sgd_param, O, I, B_, lda=O, ldb=I)
+        return dx, None, db
     dw = dw_out if dw_out is not None else torch.empty((O, I), dtype=torch.float32, device=x.device)
     gemm(dym, x2, O, I, B_, a_mn=True, b_mn=True, out=dw, lda=O, ldb=I, ldc=I)
     return dx, dw, db

@@ -85,7 +85,8 @@ class _LinearFn(torch.autograd.Function):
             dx, dw, db = ref.linear_bias_act_bwd(x, wc, y, dy, ctx.relu, need_dx)
         else:
             dx, dw, db = impl.linear_bias_act_bwd(x, wc, y, dy, ctx.relu, need_dx,
-                                                  dw_out=_gout(w), db_out=_gout(b))
+                                                  dw_out=_gout(w), db_out=_gout(b),
+                                                  sgd_param=w if getattr(w, "sgd_epilogue", None) is not None else None)
         gb = _sink(b, db)
         gw = _sink(w, dw)
         return dx, gw, gb, None

@@ -37,6 +37,7 @@ from __future__ import annotations
 import torch
 
 from ..ops import reference as ref
+from ..parallel.arena import BLOCK
 
 
 class SharedScalar(object):
@@ -63,19 +64,71 @@ def _native_for(t):
     return None
 
 
+def _fc_fusable(p, block):
+    """Can ``p``'s weight gradient be consumed by the SGD epilogue of its wgrad GEMM?  It must come from ONE fp32 GEMM straight
+    into ``gbuf`` (native FC / Softmax weights, ``rs_ok``), not be accumulated over several passes, and its shape must take the
+    un-padded path of ``cuda_impl.linear_bias_act_bwd`` (both dimensions multiples of ``block`` = elements per 16 bytes)."""
+    return (getattr(p, "rs_ok", False) and p.dim() == 2 and not getattr(p, "gaccum", False)
+            and p.shape[0] % block == 0 and p.shape[1] % block == 0)
+
+
+def complement_ranges(arena, armed):
+    """Arena element ranges ``[lo, hi)`` (block aligned, sorted) NOT covered by the parameters at indices ``armed``."""
+    out, lo = [], 0
+    for i in sorted(armed, key=lambda j: arena.offsets[j]):
+        o = arena.offsets[i]
+        end = o + -(-arena.sizes[i] // BLOCK) * BLOCK
+        if o > lo:
+            out.append((lo, o))
+        lo = max(lo, end)
+    if lo < arena.numel:
+        out.append((lo, arena.numel))
+    return out
+
+
 class FlatSGD(object):
-    """Fused momentum-SGD over the whole arena (or a block range)."""
+    """Fused momentum-SGD over the whole arena (or a block range).
+
+    :meth:`arm` (single GPU, k = 1) moves the update of the FC / Softmax weights into the epilogue of their weight-gradient GEMM
+    (``cuda_impl.gemm_sgd``): their fp32 gradient is never written, and ``step(lr, 1)`` updates only the rest of the arena."""
 
     def __init__(self, arena, mu=0.9, nesterov=False, use_momentum=True):
         self.arena = arena
         self.mu = mu if use_momentum else 0.0
         self.nesterov = nesterov
+        self.armed = []
+        self.rest = None              # complement of the armed weights, set by arm()
+
+    def arm(self, model, enable=True):
+        """Arm the eligible weights of ``model`` (CUDA, no gradient monitoring: that reads G); ``enable=False`` disarms.
+        ``model.monitor_grad`` is read here, when the iteration functions are compiled: set it before; ``grad_norms()`` refuses
+        to run while weights are armed."""
+        a = self.arena
+        for p in a.params:
+            p.sgd_epilogue = None
+        self.armed, self.rest = [], None
+        if not enable or not a.W.is_cuda or getattr(model, "monitor_grad", False):
+            return
+        dt = getattr(model, "act_dtype", None)
+        block = 16 // torch.empty((), dtype=dt).element_size() if dt is not None else 8
+        self.armed = [i for i, p in enumerate(a.params) if _fc_fusable(p, block)]
+        for i in self.armed:
+            p = a.params[i]
+            p.sgd_epilogue = self
+            p.arena_group = a.group_of[i]
+        self.rest = complement_ranges(a, self.armed)
 
     def step(self, lr, k=1, src="G", lo=0, hi=None, only_local=False, only_exchanged=False):
         a = self.arena
-        hi = a.numel if hi is None else hi
         g = getattr(a, src)
         nat = _native_for(a.W)
+        if nat is not None and self.rest is not None and k == 1 and src == "G" and (lo, hi) == (0, None) \
+                and not (only_local or only_exchanged):
+            # the armed weights were updated by their wgrad GEMMs during backward
+            for rlo, rhi in self.rest:
+                nat.sgd_flat(a, g, lr, self.mu, self.nesterov, 1.0, rlo, rhi)
+            return
+        hi = a.numel if hi is None else hi
         if nat is not None:
             nat.sgd_flat(a, g, lr, self.mu, self.nesterov, 1.0 / k, lo, hi,
                          only_local=only_local, only_exchanged=only_exchanged)
@@ -233,10 +286,11 @@ def _ex(a):
     return a.exch_vector()
 
 
-def _pre_post_msgd(model, use_nesterov, k):
+def _pre_post_msgd(model, use_nesterov, k, arm=True):
     """BSP_MSGD: aggregate momentum."""
     a, mu = model.arena, (model.mu if model.use_momentum else 0.0)
     sgd = FlatSGD(a, mu, use_nesterov, True)
+    sgd.arm(model, k == 1 and arm)
 
     def pre():
         lr = model.shared_lr.get_value()
@@ -260,10 +314,11 @@ def _pre_post_msgd(model, use_nesterov, k):
     return pre, post, "U"
 
 
-def _pre_post_msgd_grad(model, use_nesterov, k):
+def _pre_post_msgd_grad(model, use_nesterov, k, arm=True):
     """_BSP_MSGD: aggregate gradient."""
     a, mu = model.arena, (model.mu if model.use_momentum else 0.0)
     sgd = FlatSGD(a, mu, use_nesterov, True)
+    sgd.arm(model, k == 1 and arm)
 
     def pre():
         lr = model.shared_lr.get_value()
@@ -288,9 +343,10 @@ def _pre_post_msgd_grad(model, use_nesterov, k):
     return pre, post, "G"
 
 
-def _pre_post_sgd(model, k):
+def _pre_post_sgd(model, k, arm=True):
     a = model.arena
     sgd = FlatSGD(a, 0.0, False, False)
+    sgd.arm(model, k == 1 and arm)
 
     def pre():
         lr = model.shared_lr.get_value()
@@ -323,16 +379,16 @@ def _publish(model, pre, post, send_region, k):
     return pre, post
 
 
-def BSP_MSGD(model, use_nesterov_momentum, k=1):
-    return _publish(model, *_pre_post_msgd(model, use_nesterov_momentum, k), k)
+def BSP_MSGD(model, use_nesterov_momentum, k=1, arm=True):
+    return _publish(model, *_pre_post_msgd(model, use_nesterov_momentum, k, arm), k)
 
 
-def _BSP_MSGD(model, use_nesterov_momentum, k=1):
-    return _publish(model, *_pre_post_msgd_grad(model, use_nesterov_momentum, k), k)
+def _BSP_MSGD(model, use_nesterov_momentum, k=1, arm=True):
+    return _publish(model, *_pre_post_msgd_grad(model, use_nesterov_momentum, k, arm), k)
 
 
-def BSP_SGD(model, k=1):
-    return _publish(model, *_pre_post_sgd(model, k), k)
+def BSP_SGD(model, k=1, arm=True):
+    return _publish(model, *_pre_post_sgd(model, k, arm), k)
 
 
 def _clip_paramlist(param_list, scale=10):
@@ -343,12 +399,14 @@ def _clip_paramlist(param_list, scale=10):
     return param_list
 
 
-def prepare_update_dict(model, k=1, aggregate="momentum"):
+def prepare_update_dict(model, k=1, aggregate="momentum", arm=True):
+    """``arm``: at k = 1, let the FC weight-gradient GEMMs apply the update of their weights (:meth:`FlatSGD.arm`); only valid
+    when the returned ``pre`` is what updates the arena after every backward."""
     if model.use_momentum:
         if aggregate == "gradient":
-            return _BSP_MSGD(model, model.use_nesterov_momentum, k=k)
-        return BSP_MSGD(model, model.use_nesterov_momentum, k=k)
-    return BSP_SGD(model, k=k)
+            return _BSP_MSGD(model, model.use_nesterov_momentum, k=k, arm=arm)
+        return BSP_MSGD(model, model.use_nesterov_momentum, k=k, arm=arm)
+    return BSP_SGD(model, k=k, arm=arm)
 
 
 def pre_model_iter_fn(model, k=1, f_train=True, f_val=True, aggregate="momentum", fused_tail=None):
@@ -361,7 +419,7 @@ def pre_model_iter_fn(model, k=1, f_train=True, f_val=True, aggregate="momentum"
     the model's *step tail* so it is part of the CUDA-graph-captured step, and
     ``descent_vel`` is a no-op."""
     if f_train:
-        pre, post = prepare_update_dict(model, k=k, aggregate=aggregate)
+        pre, post = prepare_update_dict(model, k=k, aggregate=aggregate, arm=fused_tail is None)
         tail = fused_tail if fused_tail is not None else (pre if k == 1 else None)
         model.set_step_tail(tail)
 
