@@ -62,7 +62,7 @@ int gemm_plan_tall(long long M, int nt, int out_bf16, int sms);   // 1 = 256-row
 void gemm(const void* A, const void* B, void* C, const float* bias, int M, int N, int K, long long lda, long long ldb, long long ldc,
           int a_mn, int b_mn, int out_bf16, int bias_mode, int relu, float alpha, int bn_hint, int splitk, int f32, cudaStream_t st);
 // FC weight gradient A^T B (A: [K, M], B: [K, N], both MN-major) applied as a momentum-SGD step to W / U [M, N] (fp32, row pitch
-// ldw) and the bf16 shadow H (may be null) in the GEMM epilogue, the same arithmetic as sgd_flat; lr is read from lr_ptr[0]
+// ldw) and the bf16 shadow H (may be null) in the GEMM epilogue, the same arithmetic as flat_update's SGD rule; lr is read from lr_ptr[0]
 void gemm_sgd(const void* A, const void* B, void* W, void* U, void* H, const void* lr_ptr, float lr_mult, float wd, float mu, int nesterov,
               float inv_k, int M, int N, int K, long long lda, long long ldb, long long ldw, int f32, cudaStream_t st);
 
@@ -133,18 +133,31 @@ void masked_mean_fwd(const void* h, const void* mask, void* out, int Tn, int B, 
 void masked_mean_bwd(const void* dout, const void* mask, void* dh, int Tn, int B, int H, int f32, cudaStream_t st);
 
 // ---- comm_kernels.cu
-void sgd_flat(void* W, const void* G, void* U, void* H, const void* block_group, const GroupTable& tab, const void* lr_ptr, float mu,
-              int nesterov, float inv_k, long long lo, long long hi, int filter, cudaStream_t st);
-void adam_flat(void* W, const void* G, void* M, void* V, void* H, const void* block_group, const GroupTable& tab, const void* lr_ptr, void* step,
-               float b1, float b2, float eps, long long lo, long long hi, cudaStream_t st);
-void rmsprop_flat(void* W, const void* G, void* V, void* H, const void* block_group, const GroupTable& tab, const void* lr_ptr, float alpha,
-                  float eps, float clip, long long lo, long long hi, cudaStream_t st);
-// U = the arena's update accumulator, V = the squared-gradient average (an extra flat buffer)
-void adadelta_flat(void* W, const void* G, void* U, void* V, void* H, const void* block_group, const GroupTable& tab, const void* lr_ptr,
-                   float rho, float eps, long long lo, long long hi, cudaStream_t st);
-// M = the arena's momentum region, R / S = gradient and squared-gradient averages (extra flat buffers)
-void rmsprop_centered_flat(void* W, const void* G, void* M, void* R, void* S, void* H, const void* block_group, const GroupTable& tab,
-                           const void* lr_ptr, float rho, float mu, float eps, long long lo, long long hi, cudaStream_t st);
+// One step of a local flat optimizer over the arena elements [lo, hi) (multiples of kArenaBlock): one launch, two for Adam (its
+// step counter advances after the update).  lr is read from lr_ptr[0] on the device.
+//   rule                   S (the rule's state; the arena's U region first)   hp (float hyperparameters)
+//   FLAT_SGD               U                                                   mu, nesterov (0 / 1), inv_k
+//   FLAT_ADAM              M (U), V                                            b1, b2, eps           (+ step)
+//   FLAT_RMSPROP           V                                                   alpha, eps, clip
+//   FLAT_ADADELTA          U, V                                                rho, eps
+//   FLAT_RMSPROP_CENTERED  M (U), R, S                                         rho, mu, eps
+enum FlatRuleId : int { FLAT_SGD = 0, FLAT_ADAM, FLAT_RMSPROP, FLAT_ADADELTA, FLAT_RMSPROP_CENTERED };
+struct FlatUpdateArgs {
+  int rule;
+  void* W;
+  const void* G;
+  void* S[3];
+  void* H;                               // bf16 shadow of W, or null
+  const void* block_group;
+  GroupTable tab;
+  const void* lr_ptr;
+  void* step;                            // Adam: device step counter (uint64), else null
+  const float* hp;
+  int n_hp;
+  long long lo, hi;
+  int filter;                            // SGD: 0 all groups, 1 only non-exchanged groups, 2 only exchanged groups
+};
+void flat_update(const FlatUpdateArgs& a, cudaStream_t st);
 void fused_allreduce_sgd(const FusedArgs& a, int algo, int max_blocks, cudaStream_t st);
 // every rank pushes the fp32 master weights of the slice it owns in the two-shot partition of [lo, hi) to all peers
 void push_master_slices(const FusedArgs& a, int max_blocks, cudaStream_t st);

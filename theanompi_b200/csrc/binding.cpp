@@ -149,24 +149,13 @@ PYBIND11_MODULE(_tmpi_native, m) {
   m.def("masked_mean_bwd", [](ptr_t dout, ptr_t mask, ptr_t dh, int Tn, int B, int H, int f32, ptr_t st) { masked_mean_bwd(P(dout), P(mask), P(dh), Tn, B, H, f32, S(st)); });
 
   // ---------------------------------------------------------------- optimizer / legacy kernels
-  m.def("sgd_flat", [](ptr_t W, ptr_t G, ptr_t U, ptr_t H, ptr_t block_group, std::vector<float> lr_mult, std::vector<float> wd,
-                       std::vector<int> exch, ptr_t lr_ptr, float mu, int nesterov, float inv_k, long long lo, long long hi, int filter,
-                       ptr_t st) {
-    sgd_flat(P(W), P(G), P(U), P(H), P(block_group), make_table(lr_mult, wd, exch), P(lr_ptr), mu, nesterov, inv_k, lo, hi, filter, S(st)); });
-  m.def("adam_flat", [](ptr_t W, ptr_t G, ptr_t M, ptr_t V, ptr_t H, ptr_t block_group, std::vector<float> lr_mult, std::vector<float> wd,
-                        std::vector<int> exch, ptr_t lr_ptr, ptr_t step, float b1, float b2, float eps, long long lo, long long hi, ptr_t st) {
-    adam_flat(P(W), P(G), P(M), P(V), P(H), P(block_group), make_table(lr_mult, wd, exch), P(lr_ptr), P(step), b1, b2, eps, lo, hi, S(st)); });
-  m.def("rmsprop_flat", [](ptr_t W, ptr_t G, ptr_t V, ptr_t H, ptr_t block_group, std::vector<float> lr_mult, std::vector<float> wd,
-                           std::vector<int> exch, ptr_t lr_ptr, float alpha, float eps, float clip, long long lo, long long hi, ptr_t st) {
-    rmsprop_flat(P(W), P(G), P(V), P(H), P(block_group), make_table(lr_mult, wd, exch), P(lr_ptr), alpha, eps, clip, lo, hi, S(st)); });
-  m.def("adadelta_flat", [](ptr_t W, ptr_t G, ptr_t U, ptr_t V, ptr_t H, ptr_t block_group, std::vector<float> lr_mult, std::vector<float> wd,
-                            std::vector<int> exch, ptr_t lr_ptr, float rho, float eps, long long lo, long long hi, ptr_t st) {
-    adadelta_flat(P(W), P(G), P(U), P(V), P(H), P(block_group), make_table(lr_mult, wd, exch), P(lr_ptr), rho, eps, lo, hi, S(st)); });
-  m.def("rmsprop_centered_flat", [](ptr_t W, ptr_t G, ptr_t M, ptr_t R, ptr_t S_, ptr_t H, ptr_t block_group, std::vector<float> lr_mult,
-                                    std::vector<float> wd, std::vector<int> exch, ptr_t lr_ptr, float rho, float mu, float eps, long long lo,
-                                    long long hi, ptr_t st) {
-    rmsprop_centered_flat(P(W), P(G), P(M), P(R), P(S_), P(H), P(block_group), make_table(lr_mult, wd, exch), P(lr_ptr), rho, mu, eps, lo, hi,
-                          S(st)); });
+  m.attr("FLAT_RULES") = py::dict(py::arg("sgd") = (int)FLAT_SGD, py::arg("adam") = (int)FLAT_ADAM, py::arg("rmsprop") = (int)FLAT_RMSPROP,
+                                   py::arg("adadelta") = (int)FLAT_ADADELTA, py::arg("rmsprop_centered") = (int)FLAT_RMSPROP_CENTERED);
+  m.def("flat_update", [](int rule, ptr_t W, ptr_t G, ptr_t S0, ptr_t S1, ptr_t S2, ptr_t H, ptr_t block_group, std::vector<float> lr_mult,
+                          std::vector<float> wd, std::vector<int> exch, ptr_t lr_ptr, ptr_t step, std::vector<float> hp, long long lo,
+                          long long hi, int filter, ptr_t st) {
+    flat_update(FlatUpdateArgs{rule, P(W), P(G), {P(S0), P(S1), P(S2)}, P(H), P(block_group), make_table(lr_mult, wd, exch), P(lr_ptr),
+                               P(step), hp.data(), (int)hp.size(), lo, hi, filter}, S(st)); });
   m.def("easgd_elastic", [](ptr_t w, ptr_t h, ptr_t center, float alpha, long long n, int max_blocks, ptr_t st, int lockfree) {
     easgd_elastic(P(w), P(h), P(center), alpha, n, max_blocks, lockfree, S(st)); },
     py::arg("w"), py::arg("h"), py::arg("center"), py::arg("alpha"), py::arg("n"), py::arg("max_blocks"), py::arg("st"), py::arg("lockfree") = 0);

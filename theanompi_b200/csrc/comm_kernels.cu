@@ -9,8 +9,8 @@
 //     flag barrier → read all peers' gradients → average → weight-decay/momentum/lr update → bf16 shadow
 //     [→ push the updated slice to the peers] → flag barrier.
 //
-//   sgd_flat            k = 1 instance (no peers): fused momentum-SGD over a block range
-//   adam_flat, rmsprop_flat, adadelta_flat, rmsprop_centered_flat   the other local optimizers, one pass over a block range each
+//   flat_update_kernel<Rule>   k = 1 (no peers): one local optimizer pass over a block range (SGD = sgd4, Adam, RMSProp,
+//                              Adadelta, centred RMSProp)
 //   fused_oneshot_sgd   every rank reduces the whole range itself (latency-optimal, small buckets)
 //   fused_twoshot_sgd   reduce-scatter → update owned slice → push updated weights to all peers (bandwidth-optimal)
 //   fused_nvls_sgd      same with multimem.ld_reduce / multimem.st (reduction + broadcast inside the NVSwitch)
@@ -93,55 +93,48 @@ __device__ __forceinline__ void block_barrier(const CommCtx& c) {
   if (threadIdx.x == 0) *ep = target;
 }
 
-// ============================================================================ k = 1: local fused SGD
+// ============================================================================ k = 1: the local flat optimizers
+// One kernel template walks the arena blocks [blk_lo, blk_hi): it looks up the block's group, loads W, G and the rule's kState
+// state vectors as float4, lets the rule update them, stores them and refreshes the bf16 shadow.  lr is read from device memory
+// once per launch, so a captured CUDA graph follows lr changes.  A rule holds its hyperparameters (built inside the kernel from
+// scalar launch arguments, which keeps each instantiation's code identical to a hand-written kernel) and its per-element
+// update; `prologue` computes per-launch constants, `skip` drops whole blocks by group.
+struct FlatRule {
+  static constexpr bool kAdvancesStep = false;
+  __device__ __forceinline__ void prologue(const unsigned long long* step) {}
+  __device__ __forceinline__ bool skip(const GroupTable& tab, int g) const { return false; }
+};
+
+// momentum SGD, `common.cuh: sgd4` (the arithmetic of the GEMM SGD epilogue and the fused collectives).  State: U.
 // filter: 0 all groups, 1 only non-exchanged (BN) groups, 2 only exchanged groups
-__global__ void __launch_bounds__(kThreads) sgd_flat_kernel(float* __restrict__ W, const float* __restrict__ G, float* __restrict__ U,
-                                                            __nv_bfloat16* __restrict__ H, const uint8_t* __restrict__ block_group,
-                                                            GroupTable tab, const float* __restrict__ lr_ptr, float mu, int nesterov,
-                                                            float inv_k, long long blk_lo, long long blk_hi, int filter) {
-  const Hyper h{*lr_ptr, mu, inv_k, nesterov};
-  for (long long b = blk_lo + blockIdx.x; b < blk_hi; b += gridDim.x) {
-    const int g = block_group[b];
-    if ((filter == 1 && tab.exch[g]) || (filter == 2 && !tab.exch[g])) continue;
-    const long long i = b * kArenaBlock + threadIdx.x * 4;
-    float4 w = *reinterpret_cast<const float4*>(W + i);
-    float4 u = *reinterpret_cast<const float4*>(U + i);
-    const float4 gg = *reinterpret_cast<const float4*>(G + i);
-    sgd4(w, u, gg, h, tab.lr_mult[g], tab.wd[g]);
-    *reinterpret_cast<float4*>(W + i) = w;
-    *reinterpret_cast<float4*>(U + i) = u;
-    if (H) *reinterpret_cast<uint2*>(H + i) = pack_bf16x4(w);
+struct SgdRule : FlatRule {
+  static constexpr int kState = 1;
+  float mu, inv_k;
+  int nesterov, filter;
+  __device__ __forceinline__ SgdRule(float a, float b, float, int i, int j) : mu(a), inv_k(b), nesterov(i), filter(j) {}
+  __device__ __forceinline__ bool skip(const GroupTable& tab, int g) const {
+    return (filter == 1 && tab.exch[g]) || (filter == 2 && !tab.exch[g]);
   }
-}
+  __device__ __forceinline__ void apply(float4& w, float4* s, const float4& gg, float lr0, float lrm, float wd) const {
+    sgd4(w, s[0], gg, Hyper{lr0, mu, inv_k, nesterov}, lrm, wd);
+  }
+};
 
-void sgd_flat(void* W, const void* G, void* U, void* H, const void* block_group, const GroupTable& tab, const void* lr_ptr, float mu,
-              int nesterov, float inv_k, long long lo, long long hi, int filter, cudaStream_t st) {
-  if (lo % kArenaBlock || hi % kArenaBlock) throw std::runtime_error("sgd_flat: range must be block aligned");
-  const long long nb = (hi - lo) / kArenaBlock;
-  if (nb <= 0) return;
-  int grid = (int)std::min<long long>(nb, (long long)sm_count() * 8);
-  sgd_flat_kernel<<<grid, kThreads, 0, st>>>((float*)W, (const float*)G, (float*)U, (__nv_bfloat16*)H, (const uint8_t*)block_group, tab,
-                                             (const float*)lr_ptr, mu, nesterov, inv_k, lo / kArenaBlock, hi / kArenaBlock, filter);
-  count_launch(); TMPI_CHECK_LAUNCH("sgd_flat"); ::tmpi::check_capture(st, "sgd_flat");
-}
-
-// ============================================================================ flat Adam (Wide-ResNet's optimizer, ref keras_model_zoo/wresnet.py:159)
+// Adam (Wide-ResNet's optimizer, ref keras_model_zoo/wresnet.py:159).  State: M (the arena's U), V.
 // m = b1 m + (1 - b1) g;  v = b2 v + (1 - b2) g^2;  w -= lr * (m / (1 - b1^t)) / (sqrt(v / (1 - b2^t)) + eps), t read from a
-// device counter (the captured CUDA graph keeps counting), lr from device memory, weight decay folded into g, bf16 shadow refreshed.
-__global__ void __launch_bounds__(kThreads) adam_flat_kernel(float* __restrict__ W, const float* __restrict__ G, float* __restrict__ M,
-                                                             float* __restrict__ V, __nv_bfloat16* __restrict__ H,
-                                                             const uint8_t* __restrict__ block_group, GroupTable tab,
-                                                             const float* __restrict__ lr_ptr, const unsigned long long* __restrict__ step,
-                                                             float b1, float b2, float eps, long long blk_lo, long long blk_hi) {
-  const float t = (float)(*step + 1ull);
-  const float c1 = 1.f / (1.f - __powf(b1, t)), c2 = 1.f / (1.f - __powf(b2, t));
-  const float lr0 = *lr_ptr;
-  for (long long b = blk_lo + blockIdx.x; b < blk_hi; b += gridDim.x) {
-    const int g = block_group[b];
-    const float lr = lr0 * tab.lr_mult[g], wd = tab.wd[g];
-    const long long i = b * kArenaBlock + threadIdx.x * 4;
-    float4 w = *reinterpret_cast<const float4*>(W + i), m = *reinterpret_cast<const float4*>(M + i), v = *reinterpret_cast<const float4*>(V + i);
-    const float4 gg = *reinterpret_cast<const float4*>(G + i);
+// device counter that adam_advance_kernel bumps after the update (the captured CUDA graph keeps counting).
+struct AdamRule : FlatRule {
+  static constexpr int kState = 2;
+  static constexpr bool kAdvancesStep = true;
+  float b1, b2, eps, c1, c2;
+  __device__ __forceinline__ AdamRule(float a, float b, float c, int, int) : b1(a), b2(b), eps(c) {}
+  __device__ __forceinline__ void prologue(const unsigned long long* step) {
+    const float t = (float)(*step + 1ull);
+    c1 = 1.f / (1.f - __powf(b1, t)); c2 = 1.f / (1.f - __powf(b2, t));
+  }
+  __device__ __forceinline__ void apply(float4& w, float4* s, const float4& gg, float lr0, float lrm, float wd) const {
+    const float lr = lr0 * lrm;
+    float4 &m = s[0], &v = s[1];
 #define TMPI_ADAM1(Wc, Mc, Vc, Gc)                                    \
   {                                                                  \
     const float ge = Gc + wd * Wc;                                   \
@@ -151,40 +144,20 @@ __global__ void __launch_bounds__(kThreads) adam_flat_kernel(float* __restrict__
   }
     TMPI_ADAM1(w.x, m.x, v.x, gg.x) TMPI_ADAM1(w.y, m.y, v.y, gg.y) TMPI_ADAM1(w.z, m.z, v.z, gg.z) TMPI_ADAM1(w.w, m.w, v.w, gg.w)
 #undef TMPI_ADAM1
-    *reinterpret_cast<float4*>(W + i) = w;
-    *reinterpret_cast<float4*>(M + i) = m;
-    *reinterpret_cast<float4*>(V + i) = v;
-    if (H) *reinterpret_cast<uint2*>(H + i) = pack_bf16x4(w);
   }
-}
+};
 __global__ void adam_advance_kernel(unsigned long long* step) { if (threadIdx.x == 0 && blockIdx.x == 0) *step += 1ull; }
 
-void adam_flat(void* W, const void* G, void* M, void* V, void* H, const void* block_group, const GroupTable& tab, const void* lr_ptr, void* step,
-               float b1, float b2, float eps, long long lo, long long hi, cudaStream_t st) {
-  if (lo % kArenaBlock || hi % kArenaBlock) throw std::runtime_error("adam_flat: range must be block aligned");
-  const long long nb = (hi - lo) / kArenaBlock;
-  if (nb <= 0) return;
-  int grid = (int)std::min<long long>(nb, (long long)sm_count() * 8);
-  adam_flat_kernel<<<grid, kThreads, 0, st>>>((float*)W, (const float*)G, (float*)M, (float*)V, (__nv_bfloat16*)H, (const uint8_t*)block_group, tab,
-                                              (const float*)lr_ptr, (const unsigned long long*)step, b1, b2, eps, lo / kArenaBlock, hi / kArenaBlock);
-  adam_advance_kernel<<<1, 32, 0, st>>>((unsigned long long*)step);
-  count_launch(2); TMPI_CHECK_LAUNCH("adam_flat"); ::tmpi::check_capture(st, "adam_flat");
-}
-
-// ============================================================================ flat RMSProp (the GANs' optimizer, torch.optim.RMSprop without momentum)
+// RMSProp (the GANs' optimizer, torch.optim.RMSprop without momentum).  State: V.
 // v = alpha v + (1 - alpha) g^2;  w -= lr * g / (sqrt(v) + eps);  then, when clip > 0, w = clamp(w, -clip, clip) (the WGAN critic's
-// weight clipping in the same pass).  lr from device memory, weight decay folded into g, bf16 shadow refreshed.
-__global__ void __launch_bounds__(kThreads) rmsprop_flat_kernel(float* __restrict__ W, const float* __restrict__ G, float* __restrict__ V,
-                                                                __nv_bfloat16* __restrict__ H, const uint8_t* __restrict__ block_group,
-                                                                GroupTable tab, const float* __restrict__ lr_ptr, float alpha, float eps,
-                                                                float clip, long long blk_lo, long long blk_hi) {
-  const float lr0 = *lr_ptr;
-  for (long long b = blk_lo + blockIdx.x; b < blk_hi; b += gridDim.x) {
-    const int g = block_group[b];
-    const float lr = lr0 * tab.lr_mult[g], wd = tab.wd[g];
-    const long long i = b * kArenaBlock + threadIdx.x * 4;
-    float4 w = *reinterpret_cast<const float4*>(W + i), v = *reinterpret_cast<const float4*>(V + i);
-    const float4 gg = *reinterpret_cast<const float4*>(G + i);
+// weight clipping in the same pass).
+struct RmspropRule : FlatRule {
+  static constexpr int kState = 1;
+  float alpha, eps, clip;
+  __device__ __forceinline__ RmspropRule(float a, float b, float c, int, int) : alpha(a), eps(b), clip(c) {}
+  __device__ __forceinline__ void apply(float4& w, float4* s, const float4& gg, float lr0, float lrm, float wd) const {
+    const float lr = lr0 * lrm;
+    float4& v = s[0];
 #define TMPI_RMS1(Wc, Vc, Gc)                                         \
   {                                                                  \
     const float ge = Gc + wd * Wc;                                   \
@@ -194,39 +167,18 @@ __global__ void __launch_bounds__(kThreads) rmsprop_flat_kernel(float* __restric
   }
     TMPI_RMS1(w.x, v.x, gg.x) TMPI_RMS1(w.y, v.y, gg.y) TMPI_RMS1(w.z, v.z, gg.z) TMPI_RMS1(w.w, v.w, gg.w)
 #undef TMPI_RMS1
-    *reinterpret_cast<float4*>(W + i) = w;
-    *reinterpret_cast<float4*>(V + i) = v;
-    if (H) *reinterpret_cast<uint2*>(H + i) = pack_bf16x4(w);
   }
-}
+};
 
-void rmsprop_flat(void* W, const void* G, void* V, void* H, const void* block_group, const GroupTable& tab, const void* lr_ptr, float alpha,
-                  float eps, float clip, long long lo, long long hi, cudaStream_t st) {
-  if (lo % kArenaBlock || hi % kArenaBlock) throw std::runtime_error("rmsprop_flat: range must be block aligned");
-  const long long nb = (hi - lo) / kArenaBlock;
-  if (nb <= 0) return;
-  int grid = (int)std::min<long long>(nb, (long long)sm_count() * 8);
-  rmsprop_flat_kernel<<<grid, kThreads, 0, st>>>((float*)W, (const float*)G, (float*)V, (__nv_bfloat16*)H, (const uint8_t*)block_group, tab,
-                                                 (const float*)lr_ptr, alpha, eps, clip, lo / kArenaBlock, hi / kArenaBlock);
-  count_launch(); TMPI_CHECK_LAUNCH("rmsprop_flat"); ::tmpi::check_capture(st, "rmsprop_flat");
-}
-
-// ============================================================================ flat Adadelta (the LSTM's default optimizer, torch.optim.Adadelta)
-// v = rho v + (1 - rho) g^2;  d = sqrt(u + eps) / sqrt(v + eps) * g;  u = rho u + (1 - rho) d^2;  w -= lr * d.  u is the arena's U
-// region, v an extra flat buffer; lr from device memory, weight decay folded into g, bf16 shadow refreshed.
-__global__ void __launch_bounds__(kThreads) adadelta_flat_kernel(float* __restrict__ W, const float* __restrict__ G, float* __restrict__ U,
-                                                                 float* __restrict__ V, __nv_bfloat16* __restrict__ H,
-                                                                 const uint8_t* __restrict__ block_group, GroupTable tab,
-                                                                 const float* __restrict__ lr_ptr, float rho, float eps, long long blk_lo,
-                                                                 long long blk_hi) {
-  const float lr0 = *lr_ptr;
-  for (long long b = blk_lo + blockIdx.x; b < blk_hi; b += gridDim.x) {
-    const int g = block_group[b];
-    const float lr = lr0 * tab.lr_mult[g], wd = tab.wd[g];
-    const long long i = b * kArenaBlock + threadIdx.x * 4;
-    float4 w = *reinterpret_cast<const float4*>(W + i), u = *reinterpret_cast<const float4*>(U + i);
-    float4 v = *reinterpret_cast<const float4*>(V + i);
-    const float4 gg = *reinterpret_cast<const float4*>(G + i);
+// Adadelta (the LSTM's default optimizer, torch.optim.Adadelta).  State: U (the arena's update accumulator), V.
+// v = rho v + (1 - rho) g^2;  d = sqrt(u + eps) / sqrt(v + eps) * g;  u = rho u + (1 - rho) d^2;  w -= lr * d.
+struct AdadeltaRule : FlatRule {
+  static constexpr int kState = 2;
+  float rho, eps;
+  __device__ __forceinline__ AdadeltaRule(float a, float b, float, int, int) : rho(a), eps(b) {}
+  __device__ __forceinline__ void apply(float4& w, float4* s, const float4& gg, float lr0, float lrm, float wd) const {
+    const float lr = lr0 * lrm;
+    float4 &u = s[0], &v = s[1];
 #define TMPI_ADADELTA1(Wc, Uc, Vc, Gc)                                \
   {                                                                  \
     const float ge = Gc + wd * Wc;                                   \
@@ -238,41 +190,18 @@ __global__ void __launch_bounds__(kThreads) adadelta_flat_kernel(float* __restri
     TMPI_ADADELTA1(w.x, u.x, v.x, gg.x) TMPI_ADADELTA1(w.y, u.y, v.y, gg.y) TMPI_ADADELTA1(w.z, u.z, v.z, gg.z)
     TMPI_ADADELTA1(w.w, u.w, v.w, gg.w)
 #undef TMPI_ADADELTA1
-    *reinterpret_cast<float4*>(W + i) = w;
-    *reinterpret_cast<float4*>(U + i) = u;
-    *reinterpret_cast<float4*>(V + i) = v;
-    if (H) *reinterpret_cast<uint2*>(H + i) = pack_bf16x4(w);
   }
-}
+};
 
-void adadelta_flat(void* W, const void* G, void* U, void* V, void* H, const void* block_group, const GroupTable& tab, const void* lr_ptr,
-                   float rho, float eps, long long lo, long long hi, cudaStream_t st) {
-  if (lo % kArenaBlock || hi % kArenaBlock) throw std::runtime_error("adadelta_flat: range must be block aligned");
-  const long long nb = (hi - lo) / kArenaBlock;
-  if (nb <= 0) return;
-  int grid = (int)std::min<long long>(nb, (long long)sm_count() * 8);
-  adadelta_flat_kernel<<<grid, kThreads, 0, st>>>((float*)W, (const float*)G, (float*)U, (float*)V, (__nv_bfloat16*)H, (const uint8_t*)block_group,
-                                                  tab, (const float*)lr_ptr, rho, eps, lo / kArenaBlock, hi / kArenaBlock);
-  count_launch(); TMPI_CHECK_LAUNCH("adadelta_flat"); ::tmpi::check_capture(st, "adadelta_flat");
-}
-
-// ============================================================================ flat centred RMSProp with momentum (the reference LSTM's rmsprop)
-// r = rho r + (1 - rho) g;  s = rho s + (1 - rho) g^2;  m = mu m - lr * g / sqrt(s - r^2 + eps);  w += m.  m is the arena's U region,
-// r and s are extra flat buffers; eps sits inside the square root.  lr from device memory, weight decay folded into g, bf16 shadow
-// refreshed.
-__global__ void __launch_bounds__(kThreads) rmsprop_centered_flat_kernel(float* __restrict__ W, const float* __restrict__ G,
-                                                                         float* __restrict__ M, float* __restrict__ R, float* __restrict__ S,
-                                                                         __nv_bfloat16* __restrict__ H, const uint8_t* __restrict__ block_group,
-                                                                         GroupTable tab, const float* __restrict__ lr_ptr, float rho, float mu,
-                                                                         float eps, long long blk_lo, long long blk_hi) {
-  const float lr0 = *lr_ptr;
-  for (long long b = blk_lo + blockIdx.x; b < blk_hi; b += gridDim.x) {
-    const int g = block_group[b];
-    const float lr = lr0 * tab.lr_mult[g], wd = tab.wd[g];
-    const long long i = b * kArenaBlock + threadIdx.x * 4;
-    float4 w = *reinterpret_cast<const float4*>(W + i), m = *reinterpret_cast<const float4*>(M + i);
-    float4 r = *reinterpret_cast<const float4*>(R + i), s = *reinterpret_cast<const float4*>(S + i);
-    const float4 gg = *reinterpret_cast<const float4*>(G + i);
+// centred RMSProp with momentum (the reference LSTM's rmsprop).  State: M (the arena's U), R, S; eps sits inside the square root.
+// r = rho r + (1 - rho) g;  s = rho s + (1 - rho) g^2;  m = mu m - lr * g / sqrt(s - r^2 + eps);  w += m.
+struct CenteredRmspropRule : FlatRule {
+  static constexpr int kState = 3;
+  float rho, mu, eps;
+  __device__ __forceinline__ CenteredRmspropRule(float a, float b, float c, int, int) : rho(a), mu(b), eps(c) {}
+  __device__ __forceinline__ void apply(float4& w, float4* s, const float4& gg, float lr0, float lrm, float wd) const {
+    const float lr = lr0 * lrm;
+    float4 &m = s[0], &r = s[1], &sq = s[2];
 #define TMPI_CRMS1(Wc, Mc, Rc, Sc, Gc)                                \
   {                                                                  \
     const float ge = Gc + wd * Wc;                                   \
@@ -281,27 +210,71 @@ __global__ void __launch_bounds__(kThreads) rmsprop_centered_flat_kernel(float* 
     Mc = mu * Mc - lr * ge / sqrtf(Sc - Rc * Rc + eps);              \
     Wc += Mc;                                                        \
   }
-    TMPI_CRMS1(w.x, m.x, r.x, s.x, gg.x) TMPI_CRMS1(w.y, m.y, r.y, s.y, gg.y) TMPI_CRMS1(w.z, m.z, r.z, s.z, gg.z)
-    TMPI_CRMS1(w.w, m.w, r.w, s.w, gg.w)
+    TMPI_CRMS1(w.x, m.x, r.x, sq.x, gg.x) TMPI_CRMS1(w.y, m.y, r.y, sq.y, gg.y) TMPI_CRMS1(w.z, m.z, r.z, sq.z, gg.z)
+    TMPI_CRMS1(w.w, m.w, r.w, sq.w, gg.w)
 #undef TMPI_CRMS1
+  }
+};
+
+template <class Rule>
+__global__ void __launch_bounds__(kThreads) flat_update_kernel(float* __restrict__ W, const float* __restrict__ G, float* __restrict__ S0,
+                                                               float* __restrict__ S1, float* __restrict__ S2, __nv_bfloat16* __restrict__ H,
+                                                               const uint8_t* __restrict__ block_group, GroupTable tab,
+                                                               const float* __restrict__ lr_ptr, const unsigned long long* __restrict__ step,
+                                                               float ha, float hb, float hc, int ia, int ib, long long blk_lo,
+                                                               long long blk_hi) {
+  Rule r(ha, hb, hc, ia, ib);
+  r.prologue(step);
+  const float lr0 = *lr_ptr;
+  for (long long b = blk_lo + blockIdx.x; b < blk_hi; b += gridDim.x) {
+    const int g = block_group[b];
+    if (r.skip(tab, g)) continue;
+    const long long i = b * kArenaBlock + threadIdx.x * 4;
+    float4 w = *reinterpret_cast<const float4*>(W + i), s[Rule::kState];
+    s[0] = *reinterpret_cast<const float4*>(S0 + i);
+    if constexpr (Rule::kState > 1) s[1] = *reinterpret_cast<const float4*>(S1 + i);
+    if constexpr (Rule::kState > 2) s[2] = *reinterpret_cast<const float4*>(S2 + i);
+    const float4 gg = *reinterpret_cast<const float4*>(G + i);
+    r.apply(w, s, gg, lr0, tab.lr_mult[g], tab.wd[g]);
     *reinterpret_cast<float4*>(W + i) = w;
-    *reinterpret_cast<float4*>(M + i) = m;
-    *reinterpret_cast<float4*>(R + i) = r;
-    *reinterpret_cast<float4*>(S + i) = s;
+    *reinterpret_cast<float4*>(S0 + i) = s[0];
+    if constexpr (Rule::kState > 1) *reinterpret_cast<float4*>(S1 + i) = s[1];
+    if constexpr (Rule::kState > 2) *reinterpret_cast<float4*>(S2 + i) = s[2];
     if (H) *reinterpret_cast<uint2*>(H + i) = pack_bf16x4(w);
   }
 }
 
-void rmsprop_centered_flat(void* W, const void* G, void* M, void* R, void* S, void* H, const void* block_group, const GroupTable& tab,
-                           const void* lr_ptr, float rho, float mu, float eps, long long lo, long long hi, cudaStream_t st) {
-  if (lo % kArenaBlock || hi % kArenaBlock) throw std::runtime_error("rmsprop_centered_flat: range must be block aligned");
-  const long long nb = (hi - lo) / kArenaBlock;
+// ha, hb, hc, ia, ib: the rule's hyperparameters, in the order of its constructor
+template <class Rule>
+static void launch_flat_update(const char* name, const FlatUpdateArgs& a, float ha, float hb, float hc, int ia, int ib, cudaStream_t st) {
+  if (a.lo % kArenaBlock || a.hi % kArenaBlock) throw std::runtime_error(std::string(name) + ": range must be block aligned");
+  const long long nb = (a.hi - a.lo) / kArenaBlock;
   if (nb <= 0) return;
   int grid = (int)std::min<long long>(nb, (long long)sm_count() * 8);
-  rmsprop_centered_flat_kernel<<<grid, kThreads, 0, st>>>((float*)W, (const float*)G, (float*)M, (float*)R, (float*)S, (__nv_bfloat16*)H,
-                                                          (const uint8_t*)block_group, tab, (const float*)lr_ptr, rho, mu, eps,
-                                                          lo / kArenaBlock, hi / kArenaBlock);
-  count_launch(); TMPI_CHECK_LAUNCH("rmsprop_centered_flat"); ::tmpi::check_capture(st, "rmsprop_centered_flat");
+  flat_update_kernel<Rule><<<grid, kThreads, 0, st>>>((float*)a.W, (const float*)a.G, (float*)a.S[0], (float*)a.S[1], (float*)a.S[2],
+                                                      (__nv_bfloat16*)a.H, (const uint8_t*)a.block_group, a.tab, (const float*)a.lr_ptr,
+                                                      (const unsigned long long*)a.step, ha, hb, hc, ia, ib, a.lo / kArenaBlock,
+                                                      a.hi / kArenaBlock);
+  if (Rule::kAdvancesStep) adam_advance_kernel<<<1, 32, 0, st>>>((unsigned long long*)a.step);
+  count_launch(Rule::kAdvancesStep ? 2 : 1); TMPI_CHECK_LAUNCH(name); ::tmpi::check_capture(st, name);
+}
+
+void flat_update(const FlatUpdateArgs& a, cudaStream_t st) {
+  static const char* const names[] = {"sgd_flat", "adam_flat", "rmsprop_flat", "adadelta_flat", "rmsprop_centered_flat"};
+  static const int n_hp[] = {3, 3, 3, 2, 3};
+  if (a.rule < FLAT_SGD || a.rule > FLAT_RMSPROP_CENTERED) throw std::runtime_error("flat_update: unknown rule " + std::to_string(a.rule));
+  const char* name = names[a.rule];
+  if (a.n_hp != n_hp[a.rule])
+    throw std::runtime_error(std::string(name) + ": expected " + std::to_string(n_hp[a.rule]) + " hyperparameters");
+  if (a.rule == FLAT_ADAM && !a.step) throw std::runtime_error("adam_flat: needs a step counter");
+  const float* h = a.hp;
+  switch (a.rule) {
+    case FLAT_SGD: launch_flat_update<SgdRule>(name, a, h[0], h[2], 0.f, h[1] != 0.f, a.filter, st); break;
+    case FLAT_ADAM: launch_flat_update<AdamRule>(name, a, h[0], h[1], h[2], 0, 0, st); break;
+    case FLAT_RMSPROP: launch_flat_update<RmspropRule>(name, a, h[0], h[1], h[2], 0, 0, st); break;
+    case FLAT_ADADELTA: launch_flat_update<AdadeltaRule>(name, a, h[0], h[1], 0.f, 0, 0, st); break;
+    default: launch_flat_update<CenteredRmspropRule>(name, a, h[0], h[1], h[2], 0, 0, st); break;
+  }
 }
 
 // ============================================================================ fused collectives

@@ -194,10 +194,7 @@ class LSTM(ModelBase):
         cost, err, _ = ops.softmax_xent(self.forward_logits(x, m), y)
         cost.backward()                                            # the kernels write the gradients into the arena's G views
         with torch.no_grad():
-            if self.opt_name == "sgd":
-                self.opt.step(self.shared_lr.get_value())          # (the native kernel reads lr from the device)
-            else:
-                self.opt.step()
+            self.opt.step()                                        # lr from arena.hyper[0] (= shared_lr)
         self._after_step()
         return cost.detach(), err.detach()
 
@@ -270,16 +267,14 @@ class LSTM(ModelBase):
     def extra_state(self):
         """The optimizer's extra buffers (its U-region state travels with the arena), its name and the early-stopping state."""
         opt = self._make_opt()
-        return {"optimizer": self.opt_name, "opt": opt.state_dict() if hasattr(opt, "state_dict") else {},
+        return {"optimizer": self.opt_name, "opt": opt.state_dict(),
                 "best_err": self.best_err, "bad_counter": self.bad_counter}
 
     def load_extra_state(self, sd):
         if sd.get("optimizer") != self.opt_name:
             raise ValueError("checkpoint was written by an LSTM trained with optimizer %r; this model uses %r"
                              % (sd.get("optimizer"), self.opt_name))
-        opt = self._make_opt()
-        if hasattr(opt, "load_state_dict"):
-            opt.load_state_dict(sd["opt"])
+        self._make_opt().load_state_dict(sd["opt"])
         self.best_err, self.bad_counter = float(sd["best_err"]), int(sd["bad_counter"])
 
     def reset_iter(self, mode):

@@ -169,7 +169,7 @@ def maxpool_relu_bias_bwd(dyp, arg, y, pool, db0, db1=None):
 def gemm_sgd(a, b, p, M, N, K, lda, ldb):
     """Weight gradient ``op(a)^T op(b)`` of the armed parameter ``p`` (``utils.opt.FlatSGD.arm``) applied as its momentum-SGD
     step inside the GEMM epilogue: ``p`` (fp32 master in the arena), its momentum and its bf16 shadow are updated in place and
-    the gradient is never written.  Same arithmetic and lr source (``arena.hyper[0]``) as ``sgd_flat``."""
+    the gradient is never written.  Same arithmetic and lr source (``arena.hyper[0]``) as ``flat_update(arena, "sgd", ...)``."""
     arena, sgd = p.arena, p.sgd_epilogue
     lrm, wd, _ = _table(arena)
     g = p.arena_group
@@ -746,11 +746,23 @@ def _table(arena):
     return arena._tab_cache
 
 
-def sgd_flat(arena, g, lr, mu, nesterov, inv_k, lo, hi, only_local=False, only_exchanged=False):
-    """Fused momentum-SGD over arena elements [lo, hi).  ``lr`` is read from
-    ``arena.hyper[0]`` on the device (so a captured CUDA graph follows lr changes)."""
+def flat_update(arena, rule, hyper, state, step=None, g=None, lo=0, hi=None, filt=0):
+    """One step of the local flat optimizer ``rule`` (a key of ``FLAT_RULES``: sgd, adam, rmsprop, adadelta,
+    rmsprop_centered) over arena elements [lo, hi) in one launch (``csrc/comm_kernels.cu: flat_update_kernel``; Adam adds
+    the launch that advances its ``step`` counter).  ``state``: the rule's flat fp32 buffers, the arena's U region first when
+    the rule uses it; ``hyper``: its float hyper-parameters (order in ``csrc/api.h``); ``filt`` (SGD): 1 only non-exchanged
+    groups, 2 only exchanged groups.  lr is read from ``arena.hyper[0]`` on the device, so a captured CUDA graph follows lr
+    changes, and the bf16 shadow is refreshed in the same pass."""
     lrm, wd, ex = _table(arena)
+    S = [t.data_ptr() for t in state] + [0] * (3 - len(state))
+    lib = L()
+    lib.flat_update(lib.FLAT_RULES[rule], arena.W.data_ptr(), (arena.G if g is None else g).data_ptr(), *S, _p(arena.H),
+                    arena.block_group.data_ptr(), lrm, wd, ex, arena.hyper.data_ptr(), _p(step), [float(v) for v in hyper],
+                    int(lo), int(arena.numel if hi is None else hi), int(filt), _st(arena.W))
+
+
+def sgd_flat(arena, g, lr, mu, nesterov, inv_k, lo, hi, only_local=False, only_exchanged=False):
+    """Fused momentum-SGD over arena elements [lo, hi): ``flat_update``'s SGD rule.  ``lr`` is not used: the kernel reads
+    ``arena.hyper[0]`` on the device (so a captured CUDA graph follows lr changes)."""
     filt = 1 if only_local else (2 if only_exchanged else 0)
-    H = arena.H
-    L().sgd_flat(arena.W.data_ptr(), g.data_ptr(), arena.U.data_ptr(), _p(H), arena.block_group.data_ptr(), lrm, wd, ex,
-                 arena.hyper.data_ptr(), float(mu), int(bool(nesterov)), float(inv_k), int(lo), int(hi), filt, _st(arena.W))
+    flat_update(arena, "sgd", (mu, float(bool(nesterov)), inv_k), [arena.U], g=g, lo=lo, hi=hi, filt=filt)

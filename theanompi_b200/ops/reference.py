@@ -253,6 +253,24 @@ def sgd_flat(w, g, u, lr_mult, wd, lr, mu, nesterov, inv_k, w_half=None):
     return w, u
 
 
+def adam_flat(w, g, m, v, lr_mult, wd, lr, b1=0.9, b2=0.999, eps=1e-8, t=1, w_half=None):
+    """One Adam step over flat fp32 buffers (Keras / ``torch.optim.Adam``), ``t`` = the 1-based step number:
+
+        g_eff = g + wd * w
+        m     = b1 * m + (1 - b1) * g_eff
+        v     = b2 * v + (1 - b2) * g_eff^2
+        w    -= lr * lr_mult * (m / (1 - b1^t)) / (sqrt(v / (1 - b2^t)) + eps)
+    """
+    g_eff = g + wd * w
+    m.mul_(b1).add_(g_eff, alpha=1 - b1)
+    v.mul_(b2).addcmul_(g_eff, g_eff, value=1 - b2)
+    mh, vh = m / (1 - b1 ** t), v / (1 - b2 ** t)
+    w.sub_(lr * lr_mult * mh / (vh.sqrt() + eps))
+    if w_half is not None:
+        w_half.copy_(w)
+    return w, m, v
+
+
 def rmsprop_flat(w, g, v, lr_mult, wd, lr, alpha=0.99, eps=1e-8, clip=0.0, w_half=None):
     """One RMSProp step over flat fp32 buffers, ``torch.optim.RMSprop`` without momentum, plus an optional clip:
 

@@ -57,13 +57,6 @@ class SharedScalar(object):
         self._buf[self._i] = float(v)
 
 
-def _native_for(t):
-    if t.is_cuda:
-        from ..ops import cuda_impl
-        return cuda_impl
-    return None
-
-
 def _fc_fusable(p, block):
     """Can ``p``'s weight gradient be consumed by the SGD epilogue of its wgrad GEMM?  It must come from ONE fp32 GEMM straight
     into ``gbuf`` (native FC / Softmax weights, ``rs_ok``), not be accumulated over several passes, and its shape must take the
@@ -86,14 +79,63 @@ def complement_ranges(arena, armed):
     return out
 
 
-class FlatSGD(object):
-    """Fused momentum-SGD over the whole arena (or a block range).
+class FlatOptimizer(object):
+    """A local optimizer over the whole flat arena.  On CUDA one native launch per step (``csrc/comm_kernels.cu:
+    flat_update_kernel``, Adam adds the launch that advances its step counter), with lr read from ``arena.hyper[0]`` on the
+    device and the bf16 shadow refreshed in the same pass, so the step is CUDA-graph capturable.  On the CPU the same update
+    runs through its ``ops/reference.py`` function.
+
+    A subclass names its kernel ``rule``, whether the rule keeps state in the arena's U region (``uses_u``), its extra flat
+    ``buffers`` (zero-initialised, saved by :meth:`state_dict` under their names), its ``reference`` function and, in
+    :meth:`hyper`, its float hyper-parameters in the order both take them."""
+
+    rule = None
+    uses_u = True
+    buffers = ()
+    reference = None
+    t = None                         # device step counter of a rule that reads one (Adam)
+
+    def __init__(self, arena):
+        self.arena = arena
+        for name in self.buffers:
+            setattr(self, name, torch.zeros_like(arena.W))
+
+    def hyper(self):
+        raise NotImplementedError
+
+    def _state(self):
+        return ([self.arena.U] if self.uses_u else []) + [getattr(self, n) for n in self.buffers]
+
+    def step(self, lr=None):
+        a = self.arena
+        if a.W.is_cuda:
+            from ..ops import cuda_impl
+            cuda_impl.flat_update(a, self.rule, self.hyper(), self._state(), step=self.t)
+            return
+        self._reference_step(float(a.hyper[0]) if lr is None else lr)
+
+    def _reference_step(self, lr):
+        a = self.arena
+        type(self).reference(a.W, a.G, *self._state(), a.lr_mult_vector(), a.wd_vector(), lr, *self.hyper(), w_half=a.H)
+
+    def state_dict(self):
+        return {n: getattr(self, n).detach().cpu() for n in self.buffers}
+
+    def load_state_dict(self, sd):
+        for n in self.buffers:
+            getattr(self, n).copy_(sd[n].to(self.arena.W.device))
+
+
+class FlatSGD(FlatOptimizer):
+    """Fused momentum-SGD over the whole arena (or a block range); momentum in the arena's U region.
 
     :meth:`arm` (single GPU, k = 1) moves the update of the FC / Softmax weights into the epilogue of their weight-gradient GEMM
     (``cuda_impl.gemm_sgd``): their fp32 gradient is never written, and ``step(lr, 1)`` updates only the rest of the arena."""
 
+    rule = "sgd"
+
     def __init__(self, arena, mu=0.9, nesterov=False, use_momentum=True):
-        self.arena = arena
+        super().__init__(arena)
         self.mu = mu if use_momentum else 0.0
         self.nesterov = nesterov
         self.armed = []
@@ -118,21 +160,19 @@ class FlatSGD(object):
             p.arena_group = a.group_of[i]
         self.rest = complement_ranges(a, self.armed)
 
-    def step(self, lr, k=1, src="G", lo=0, hi=None, only_local=False, only_exchanged=False):
+    def step(self, lr=None, k=1, src="G", lo=0, hi=None, only_local=False, only_exchanged=False):
         a = self.arena
         g = getattr(a, src)
-        nat = _native_for(a.W)
-        if nat is not None and self.rest is not None and k == 1 and src == "G" and (lo, hi) == (0, None) \
-                and not (only_local or only_exchanged):
-            # the armed weights were updated by their wgrad GEMMs during backward
-            for rlo, rhi in self.rest:
-                nat.sgd_flat(a, g, lr, self.mu, self.nesterov, 1.0, rlo, rhi)
+        if a.W.is_cuda:
+            from ..ops import cuda_impl
+            ranges = [(lo, a.numel if hi is None else hi)]
+            if self.rest is not None and k == 1 and src == "G" and (lo, hi) == (0, None) and not (only_local or only_exchanged):
+                ranges = self.rest    # the armed weights were updated by their wgrad GEMMs during backward
+            for rlo, rhi in ranges:
+                cuda_impl.sgd_flat(a, g, lr, self.mu, self.nesterov, 1.0 / k, rlo, rhi, only_local, only_exchanged)
             return
+        lr = float(a.hyper[0]) if lr is None else lr
         hi = a.numel if hi is None else hi
-        if nat is not None:
-            nat.sgd_flat(a, g, lr, self.mu, self.nesterov, 1.0 / k, lo, hi,
-                         only_local=only_local, only_exchanged=only_exchanged)
-            return
         sl = slice(lo, hi)
         lrm, wd = a.lr_mult_vector()[sl], a.wd_vector()[sl]
         w, gg, u = a.W[sl], g[sl], a.U[sl]
@@ -152,133 +192,75 @@ class FlatSGD(object):
             a.H[sl].copy_(w)
 
 
-class FlatAdam(object):
-    """Adam over the whole arena in one native kernel (``csrc/comm_kernels.cu: adam_flat_kernel``): first moment in the arena's
-    U region, second moment in an extra flat buffer, step counter and lr in device memory — the step is CUDA-graph capturable.
-    The reference's Wide-ResNet uses Keras Adam (``keras_model_zoo/wresnet.py:159``)."""
+class FlatAdam(FlatOptimizer):
+    """Adam: first moment in the arena's U region, second moment in ``V``, step counter ``t`` in device memory.  The
+    reference's Wide-ResNet uses Keras Adam (``keras_model_zoo/wresnet.py:159``)."""
+
+    rule, buffers = "adam", ("V",)
 
     def __init__(self, arena, b1=0.9, b2=0.999, eps=1e-8):
-        self.arena, self.b1, self.b2, self.eps = arena, b1, b2, eps
-        self.V = torch.zeros_like(arena.W)
+        super().__init__(arena)
+        self.b1, self.b2, self.eps = b1, b2, eps
         self.t = torch.zeros(1, dtype=torch.int64, device=arena.W.device)
 
-    def step(self, lr=None):
+    def hyper(self):
+        return (self.b1, self.b2, self.eps)
+
+    def _reference_step(self, lr):
         a = self.arena
-        nat = _native_for(a.W)
-        if nat is not None:
-            from ..ops.cuda_impl import L, _table, _p, _st
-            lrm, wd, ex = _table(a)
-            L().adam_flat(a.W.data_ptr(), a.G.data_ptr(), a.U.data_ptr(), self.V.data_ptr(), _p(a.H), a.block_group.data_ptr(), lrm, wd, ex,
-                          a.hyper.data_ptr(), self.t.data_ptr(), float(self.b1), float(self.b2), float(self.eps), 0, int(a.numel), _st(a.W))
-            return
-        lr = float(a.hyper[0]) if lr is None else lr
         self.t += 1
-        t = float(self.t)
-        g = a.G + a.wd_vector() * a.W
-        a.U.mul_(self.b1).add_(g, alpha=1 - self.b1)
-        self.V.mul_(self.b2).addcmul_(g, g, value=1 - self.b2)
-        mh, vh = a.U / (1 - self.b1 ** t), self.V / (1 - self.b2 ** t)
-        a.W.sub_(lr * a.lr_mult_vector() * mh / (vh.sqrt() + self.eps))
-        if a.H is not None:
-            a.H.copy_(a.W)
+        ref.adam_flat(a.W, a.G, a.U, self.V, a.lr_mult_vector(), a.wd_vector(), lr, *self.hyper(), t=float(self.t), w_half=a.H)
 
     def state_dict(self):
-        return {"V": self.V.detach().cpu(), "t": int(self.t)}
+        return dict(super().state_dict(), t=int(self.t))
 
     def load_state_dict(self, sd):
-        self.V.copy_(sd["V"].to(self.V.device)); self.t.fill_(int(sd["t"]))
+        super().load_state_dict(sd)
+        self.t.fill_(int(sd["t"]))
 
 
-class FlatRMSProp(object):
-    """RMSProp over the whole arena in one native kernel (``csrc/comm_kernels.cu: rmsprop_flat_kernel``): the squared-gradient
-    average in an extra flat buffer, lr read from ``arena.hyper[0]`` on the device, the bf16 shadow refreshed in the same pass —
-    the step is CUDA-graph capturable.  ``torch.optim.RMSprop(alpha=0.99, eps=1e-8)`` without momentum, the optimizer of the
-    reference's GANs (``lasagne_model_zoo/wgan.py:18-59``), plus an optional clip of the updated weights to ``[-clip, clip]``
-    (the WGAN critic's weight clipping, folded into the same pass)."""
+class FlatRMSProp(FlatOptimizer):
+    """RMSProp, the squared-gradient average in ``V``: ``torch.optim.RMSprop(alpha=0.99, eps=1e-8)`` without momentum, the
+    optimizer of the reference's GANs (``lasagne_model_zoo/wgan.py:18-59``), plus an optional clip of the updated weights to
+    ``[-clip, clip]`` (the WGAN critic's weight clipping, folded into the same pass)."""
+
+    rule, uses_u, buffers, reference = "rmsprop", False, ("V",), ref.rmsprop_flat
 
     def __init__(self, arena, alpha=0.99, eps=1e-8, clip=0.0):
-        self.arena, self.alpha, self.eps, self.clip = arena, alpha, eps, clip
-        self.V = torch.zeros_like(arena.W)
+        super().__init__(arena)
+        self.alpha, self.eps, self.clip = alpha, eps, clip
 
-    def step(self, lr=None):
-        a = self.arena
-        nat = _native_for(a.W)
-        if nat is not None:
-            from ..ops.cuda_impl import L, _table, _p, _st
-            lrm, wd, ex = _table(a)
-            L().rmsprop_flat(a.W.data_ptr(), a.G.data_ptr(), self.V.data_ptr(), _p(a.H), a.block_group.data_ptr(), lrm, wd, ex,
-                             a.hyper.data_ptr(), float(self.alpha), float(self.eps), float(self.clip), 0, int(a.numel), _st(a.W))
-            return
-        lr = float(a.hyper[0]) if lr is None else lr
-        ref.rmsprop_flat(a.W, a.G, self.V, a.lr_mult_vector(), a.wd_vector(), lr, self.alpha, self.eps, self.clip,
-                         w_half=a.H)
-
-    def state_dict(self):
-        return {"V": self.V.detach().cpu()}
-
-    def load_state_dict(self, sd):
-        self.V.copy_(sd["V"].to(self.V.device))
+    def hyper(self):
+        return (self.alpha, self.eps, self.clip)
 
 
-class FlatAdadelta(object):
-    """Adadelta over the whole arena in one native kernel (``csrc/comm_kernels.cu: adadelta_flat_kernel``): the update accumulator
-    in the arena's U region (saved with the arena), the squared-gradient average in an extra flat buffer, lr read from
-    ``arena.hyper[0]`` on the device, the bf16 shadow refreshed in the same pass — the step is CUDA-graph capturable.
-    ``torch.optim.Adadelta(rho=0.95, eps=1e-6)``, which at lr = 1 is the reference LSTM's ``adadelta`` (``models/lstm.py:284-342``)."""
+class FlatAdadelta(FlatOptimizer):
+    """Adadelta, the update accumulator in the arena's U region (saved with the arena), the squared-gradient average in ``V``:
+    ``torch.optim.Adadelta(rho=0.95, eps=1e-6)``, which at lr = 1 is the reference LSTM's ``adadelta``
+    (``models/lstm.py:284-342``)."""
+
+    rule, buffers, reference = "adadelta", ("V",), ref.adadelta_flat
 
     def __init__(self, arena, rho=0.95, eps=1e-6):
-        self.arena, self.rho, self.eps = arena, rho, eps
-        self.V = torch.zeros_like(arena.W)
+        super().__init__(arena)
+        self.rho, self.eps = rho, eps
 
-    def step(self, lr=None):
-        a = self.arena
-        nat = _native_for(a.W)
-        if nat is not None:
-            from ..ops.cuda_impl import L, _table, _p, _st
-            lrm, wd, ex = _table(a)
-            L().adadelta_flat(a.W.data_ptr(), a.G.data_ptr(), a.U.data_ptr(), self.V.data_ptr(), _p(a.H), a.block_group.data_ptr(), lrm, wd,
-                              ex, a.hyper.data_ptr(), float(self.rho), float(self.eps), 0, int(a.numel), _st(a.W))
-            return
-        lr = float(a.hyper[0]) if lr is None else lr
-        ref.adadelta_flat(a.W, a.G, a.U, self.V, a.lr_mult_vector(), a.wd_vector(), lr, self.rho, self.eps, w_half=a.H)
-
-    def state_dict(self):
-        return {"V": self.V.detach().cpu()}
-
-    def load_state_dict(self, sd):
-        self.V.copy_(sd["V"].to(self.V.device))
+    def hyper(self):
+        return (self.rho, self.eps)
 
 
-class FlatCenteredRMSProp(object):
-    """The reference LSTM's ``rmsprop`` (``models/lstm.py:376-402``: centred, momentum 0.9, eps 1e-4 inside the square root) over
-    the whole arena in one native kernel (``csrc/comm_kernels.cu: rmsprop_centered_flat_kernel``): the momentum in the arena's U
-    region, the gradient and squared-gradient averages in two extra flat buffers, lr read from ``arena.hyper[0]`` on the device,
-    the bf16 shadow refreshed in the same pass — the step is CUDA-graph capturable."""
+class FlatCenteredRMSProp(FlatOptimizer):
+    """The reference LSTM's ``rmsprop`` (``models/lstm.py:376-402``: centred, momentum 0.9, eps 1e-4 inside the square root):
+    the momentum in the arena's U region, the gradient and squared-gradient averages in ``R`` and ``S``."""
+
+    rule, buffers, reference = "rmsprop_centered", ("R", "S"), ref.rmsprop_centered_flat
 
     def __init__(self, arena, rho=0.95, mu=0.9, eps=1e-4):
-        self.arena, self.rho, self.mu, self.eps = arena, rho, mu, eps
-        self.R = torch.zeros_like(arena.W)
-        self.S = torch.zeros_like(arena.W)
+        super().__init__(arena)
+        self.rho, self.mu, self.eps = rho, mu, eps
 
-    def step(self, lr=None):
-        a = self.arena
-        nat = _native_for(a.W)
-        if nat is not None:
-            from ..ops.cuda_impl import L, _table, _p, _st
-            lrm, wd, ex = _table(a)
-            L().rmsprop_centered_flat(a.W.data_ptr(), a.G.data_ptr(), a.U.data_ptr(), self.R.data_ptr(), self.S.data_ptr(), _p(a.H),
-                                      a.block_group.data_ptr(), lrm, wd, ex, a.hyper.data_ptr(), float(self.rho), float(self.mu),
-                                      float(self.eps), 0, int(a.numel), _st(a.W))
-            return
-        lr = float(a.hyper[0]) if lr is None else lr
-        ref.rmsprop_centered_flat(a.W, a.G, a.U, self.R, self.S, a.lr_mult_vector(), a.wd_vector(), lr, self.rho, self.mu, self.eps,
-                                  w_half=a.H)
-
-    def state_dict(self):
-        return {"R": self.R.detach().cpu(), "S": self.S.detach().cpu()}
-
-    def load_state_dict(self, sd):
-        self.R.copy_(sd["R"].to(self.R.device)); self.S.copy_(sd["S"].to(self.S.device))
+    def hyper(self):
+        return (self.rho, self.mu, self.eps)
 
 
 # --------------------------------------------------------------------------- classic split (API parity)
