@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <tuple>
 #include "common.cuh"
 
 namespace tmpi {
@@ -58,6 +59,10 @@ void gemm_rs_add_range(const void* c_lo, const void* c_hi, long long blo, long l
 void gemm_rs_clear();
 int gemm_plan_splits(int tiles, int num_kb, int sms);          // split-K factor the launcher would pick
 int gemm_plan_tall(long long M, int nt, int out_bf16, int sms);   // 1 = 256-row CTA tiles   // bottleneck probe knobs of the wgmma GEMM (see Params::dbg)
+// (BN, MT, split-K slices) an implicit-GEMM convolution launch would use.  kind 0 fprop, 1 dgrad, 2 wgrad; fprop / dgrad:
+// M = output pixels, N = output channels, num_kb = taps x channel chunks; wgrad: M = output channels, N = (tap, channel-chunk)
+// boxes x box width, num_kb = pixel blocks.  tall_ok: the output may use 256-row tiles (bf16 output, or K-major tf32).
+std::tuple<int, int, int> gemm_plan_conv(int kind, long long M, int N, int groups, int num_kb, int tall_ok, int sms);
 // f32 = 1: fp32 operands through wgmma tf32 (fp32 output), else bf16 operands
 void gemm(const void* A, const void* B, void* C, const float* bias, int M, int N, int K, long long lda, long long ldb, long long ldc,
           int a_mn, int b_mn, int out_bf16, int bias_mode, int relu, float alpha, int bn_hint, int splitk, int f32, cudaStream_t st);

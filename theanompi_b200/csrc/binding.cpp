@@ -52,6 +52,7 @@ PYBIND11_MODULE(_tmpi_native, m) {
   m.def("gemm_rs_clear", &gemm_rs_clear);
   m.def("gemm_plan_splits", &gemm_plan_splits);
   m.def("gemm_plan_tall", &gemm_plan_tall);
+  m.def("gemm_plan_conv", &gemm_plan_conv);
   m.def("gemm", [](ptr_t A, ptr_t B, ptr_t C, ptr_t bias, int M, int N, int K, long long lda, long long ldb, long long ldc, int a_mn, int b_mn,
                    int out_bf16, int bias_mode, int relu, float alpha, int bn_hint, int splitk, int f32, ptr_t st) {
     gemm(P(A), P(B), P(C), (const float*)P(bias), M, N, K, lda, ldb, ldc, a_mn, b_mn, out_bf16, bias_mode, relu, alpha, bn_hint, splitk, f32,

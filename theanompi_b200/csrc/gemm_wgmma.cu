@@ -44,6 +44,43 @@ static bool use_tall_tiles(long long M, int nt, int eligible, int sms) {
   return w2 * 17 <= w1 * 10;
 }
 
+// Tile of an implicit-GEMM convolution: the layout-legal (BN, MT) with the least estimated time.  A persistent launch takes
+// waves x (time of one tile); a tile costs (its k-blocks + kTileOverheadKb for pipeline fill and epilogue) x (the columns of
+// wgmma work it issues per k-block, MT x BN, zero-filled columns past N included, + a fixed per-k-block cost of barrier waits
+// and wgmma.wait_group worth kKblockCols columns).  256-row tiles are candidates only where use_tall_tiles accepts them;
+// split-K (wgrad) is planned per candidate exactly as the launcher will run it.
+//   kind 0 fprop: K-major weights, BN 64 / 96 / 128 / 192;  kind 1 dgrad: MN-major weights, BN a whole number of 64-wide
+//   bf16 atoms;  kind 2 wgrad: fp32 split-K output, 128-row tiles of BN / ATOM (tap, channel-chunk) boxes.
+//   N: output columns (wgrad: boxes x ATOM, the columns the kernel issues).  BN = 192 tiles are 128 rows only: 2 x 96
+//   accumulators per thread would not fit next to the rest of the consumer's registers.
+struct ConvTile { int bn, mt, splits; };
+static ConvTile choose_conv_tile(int kind, long long M, int N, int groups, int num_kb, int tall_ok, int sms) {
+  static const int kCand[7][2] = {{128, 2}, {128, 1}, {192, 1}, {96, 2}, {96, 1}, {64, 2}, {64, 1}};   // ties: first wins
+  const int kTileOverheadKb = 4, kKblockCols = 64;
+  // 3-box wgrad tiles only for deep reductions: on an H100 they paid off for AlexNet-128b's conv1 / conv2 wgrads (6050 /
+  // 1458 pixel blocks) but cost GoogLeNet-32b about 1.5 % of its step with the shallow (25-400 block) wgrads of its inception
+  // layers, which the cost model above does not see
+  const int kWideWgradMinKb = 1024;
+  ConvTile best{0, 0, 1};
+  long long best_cost = -1;
+  for (const auto& c : kCand) {
+    const int bn = c[0], mt = c[1];
+    if (bn == 96 && kind != 0) continue;
+    if (kind == 2 && (bn == 64 || mt == 2)) continue;
+    if (kind == 2 && bn == 192 && num_kb < kWideWgradMinKb) continue;
+    const int nt = (N + bn - 1) / bn;
+    if (mt == 2 && !use_tall_tiles(M, nt * groups, tall_ok, sms)) continue;
+    const long long tiles = ((M + mt * BM - 1) / (mt * BM)) * nt * groups;
+    int splits = kind == 2 ? choose_splits((int)tiles, num_kb, sms) : 1;
+    const int kb_per = (num_kb + splits - 1) / splits;
+    splits = (num_kb + kb_per - 1) / kb_per;
+    const long long waves = (tiles * splits + sms - 1) / sms;
+    const long long cost = waves * (kb_per + kTileOverheadKb) * (mt * bn + kKblockCols);
+    if (best_cost < 0 || cost < best_cost) { best_cost = cost; best = {bn, mt, splits}; }
+  }
+  return best;
+}
+
 }  // namespace wgmma
 
 void gemm_set_debug(int flags) { wgmma::g_dbg = flags; }
@@ -99,6 +136,10 @@ void gemm_rs_clear() {
 // host-side planning helpers, exported so the wave arithmetic can be unit-tested without a GPU
 int gemm_plan_splits(int tiles, int num_kb, int sms) { return wgmma::choose_splits(tiles, num_kb, sms); }
 int gemm_plan_tall(long long M, int nt, int out_bf16, int sms) { return wgmma::use_tall_tiles(M, nt, out_bf16, sms) ? 1 : 0; }
+std::tuple<int, int, int> gemm_plan_conv(int kind, long long M, int N, int groups, int num_kb, int tall_ok, int sms) {
+  const wgmma::ConvTile t = wgmma::choose_conv_tile(kind, M, N, groups, num_kb, tall_ok, sms);
+  return {t.bn, t.mt, t.splits};
+}
 
 // C[M,N] (ldc) = alpha * op(A) op(B) + bias, optional ReLU.
 //   a_mn == 0: A is [M, K] with row pitch lda (elements);  a_mn == 1: A is [K, M] with row pitch lda.
@@ -265,7 +306,11 @@ static void conv_fprop_groups(int ngroups, const void* x, const int* c_off, cons
   if (M <= 0 || O <= 0) return;
   if (M >= (1LL << 31)) throw std::runtime_error("conv_fprop: too many output pixels");
   if (ESZ == 4) out_bf16 = 0;
-  const int BN = O > 64 ? 128 : 64;
+  const int c_chunks = (Cg + BK - 1) / BK, num_kb = KH * KW * c_chunks;
+  // tall tiles: bf16 outputs; on the tf32 path K-major operands only (dgrad's weights are MN-major)
+  const ConvTile tile = choose_conv_tile(dgrad ? 1 : 0, M, O, ngroups, num_kb, ESZ == 2 ? out_bf16 : !dgrad, sm_count());
+  const int BN = tile.bn;
+  const bool tall = tile.mt == 2;
   Params p;
   p.C = y[0]; p.bias = bias[0]; p.alpha = 1.f; p.M = (int)M; p.N = O; p.K = KH * KW * Cg; p.ldc = ldc; p.a_mn = 0; p.b_mn = dgrad ? 1 : 0;
   p.groups = ngroups; p.C1 = ngroups > 1 ? y[1] : nullptr; p.bias1 = ngroups > 1 ? bias[1] : nullptr;
@@ -273,11 +318,10 @@ static void conv_fprop_groups(int ngroups, const void* x, const int* c_off, cons
   if (ngroups > 1 && ((bias[0] == nullptr) != (bias[1] == nullptr))) throw std::runtime_error("conv_fprop: both groups need a bias or none");
   if (dgrad && (S != 1 || ((O * ESZ) % 16) != 0)) throw std::runtime_error("conv dgrad through the fprop kernel needs stride 1 and 16-byte channel rows");
   p.nt = (O + BN - 1) / BN; p.splits = 1;
-  const bool tall = use_tall_tiles(M, p.nt * ngroups, ESZ == 2 ? out_bf16 : !dgrad, sm_count());
   p.mt = tall ? (int)((M + 2 * BM - 1) / (2 * BM)) : (int)((M + BM - 1) / BM);
   p.group_m = 0;
-  p.conv_mode = 1; p.cHo = Ho; p.cWo = Wo; p.cS = S; p.cP = P; p.cKH = KH; p.cKW = KW; p.cCg = Cg; p.c_chunks = (Cg + BK - 1) / BK;
-  p.num_kb = KH * KW * p.c_chunks; p.kb_per_split = p.num_kb;
+  p.conv_mode = 1; p.cHo = Ho; p.cWo = Wo; p.cS = S; p.cP = P; p.cKH = KH; p.cKW = KW; p.cCg = Cg; p.c_chunks = c_chunks;
+  p.num_kb = num_kb; p.kb_per_split = p.num_kb;
   CUtensorMap ta[2], tb[2];
   for (int g = 0; g < ngroups; ++g) {
     ta[g] = make_im2col_map(x, N, H, W, Ctot, c_off[g], Cg, KH, KW, S, P, BM, ESZ, 0);                     // K-major (channels = K)
@@ -285,8 +329,13 @@ static void conv_fprop_groups(int ngroups, const void* x, const int* c_off, cons
   }
   const CUtensorMap* a1 = ngroups > 1 ? &ta[1] : nullptr;
   const CUtensorMap* b1 = ngroups > 1 ? &tb[1] : nullptr;
-  if (tall) { if (BN == 128) launch<T, 128, 2>(ta[0], tb[0], p, 1, st, a1, b1); else launch<T, 64, 2>(ta[0], tb[0], p, 1, st, a1, b1); }
+  if (tall) {
+    if (BN == 128) launch<T, 128, 2>(ta[0], tb[0], p, 1, st, a1, b1);
+    else if (BN == 96) launch<T, 96, 2>(ta[0], tb[0], p, 1, st, a1, b1);
+    else launch<T, 64, 2>(ta[0], tb[0], p, 1, st, a1, b1);
+  } else if (BN == 192) launch<T, 192, 1>(ta[0], tb[0], p, 1, st, a1, b1);
   else if (BN == 128) launch<T, 128, 1>(ta[0], tb[0], p, 1, st, a1, b1);
+  else if (BN == 96) launch<T, 96, 1>(ta[0], tb[0], p, 1, st, a1, b1);
   else launch<T, 64, 1>(ta[0], tb[0], p, 1, st, a1, b1);
 }
 
@@ -300,19 +349,20 @@ static void conv_wgrad_groups(int ngroups, const void* const* dy, const void* x,
   const long long M = (long long)N * Ho * Wo;
   if (M <= 0 || O <= 0) return;
   if (M >= (1LL << 31)) throw std::runtime_error("conv_wgrad: too many output pixels");
-  const int sms = sm_count();
-  const int BN = 128;                                  // BN / ATOM (tap, channel-chunk) boxes per n-tile: fewer re-reads of dy
+  const int c_chunks = (Cg + ATOM - 1) / ATOM, num_kb = (int)((M + BK - 1) / BK);
+  // BN / ATOM (tap, channel-chunk) boxes per n-tile: wider tiles re-read dy fewer times
+  const ConvTile tile = choose_conv_tile(2, O, KH * KW * c_chunks * ATOM, ngroups, num_kb, 0, sm_count());
+  const int BN = tile.bn;
   Params p;
   p.C = dw[0]; p.bias = nullptr; p.alpha = 1.f; p.M = O; p.N = KH * KW * Cg; p.K = (int)M; p.ldc = (long long)KH * KW * Cg; p.a_mn = 1; p.b_mn = 1;
   p.groups = ngroups; p.C1 = ngroups > 1 ? dw[1] : nullptr; p.bias1 = nullptr;
   p.out_bf16 = 0; p.bias_mode = 0; p.relu = 0;
   p.group_m = 0;
-  p.conv_mode = 2; p.cHo = Ho; p.cWo = Wo; p.cS = S; p.cP = P; p.cKH = KH; p.cKW = KW; p.cCg = Cg; p.c_chunks = (Cg + ATOM - 1) / ATOM;
+  p.conv_mode = 2; p.cHo = Ho; p.cWo = Wo; p.cS = S; p.cP = P; p.cKH = KH; p.cKW = KW; p.cCg = Cg; p.c_chunks = c_chunks;
   p.mt = (O + BM - 1) / BM; p.nt = (KH * KW * p.c_chunks + BN / ATOM - 1) / (BN / ATOM);
-  p.num_kb = (int)((M + BK - 1) / BK);
-  int splits = choose_splits(p.mt * p.nt * ngroups, p.num_kb, sms);
+  p.num_kb = num_kb;
+  const int splits = tile.splits;
   p.kb_per_split = (p.num_kb + splits - 1) / splits;
-  splits = (p.num_kb + p.kb_per_split - 1) / p.kb_per_split;
   p.splits = splits; p.atomic_out = splits > 1;
   CUtensorMap ta[2], tb[2];
   for (int g = 0; g < ngroups; ++g) {
@@ -320,7 +370,10 @@ static void conv_wgrad_groups(int ngroups, const void* const* dy, const void* x,
     ta[g] = make_tmap(dy[g], (uint64_t)O, (uint64_t)M, (uint64_t)ldy * ESZ, (uint32_t)BK, ESZ, 1);          // both operands MN-major
     tb[g] = make_im2col_map(x, N, H, W, Ctot, c_off[g], Cg, KH, KW, S, P, BK, ESZ, 1);
   }
-  launch<T, 128, 1>(ta[0], tb[0], p, splits, st, ngroups > 1 ? &ta[1] : nullptr, ngroups > 1 ? &tb[1] : nullptr);
+  const CUtensorMap* a1 = ngroups > 1 ? &ta[1] : nullptr;
+  const CUtensorMap* b1 = ngroups > 1 ? &tb[1] : nullptr;
+  if (BN == 192) launch<T, 192, 1>(ta[0], tb[0], p, splits, st, a1, b1);
+  else launch<T, 128, 1>(ta[0], tb[0], p, splits, st, a1, b1);
 }
 }  // namespace wgmma
 

@@ -277,6 +277,37 @@ __device__ __forceinline__ void wgmma(float (&d)[64], uint64_t da, uint64_t db, 
                : "l"(da), "l"(db), "r"(scale_d));
 }
 
+// n96 / n192: the tile widths the convolution planner picks for 96- and 192-channel outputs (see choose_conv_tile)
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma(float (&d)[48], uint64_t da, uint64_t db, uint32_t scale_d, WgBF16<96, TA, TB>) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, %51, %52;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+               : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma(float (&d)[96], uint64_t da, uint64_t db, uint32_t scale_d, WgBF16<192, TA, TB>) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %98, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n192k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, %96, %97, p, 1, 1, %99, %100;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])
+               : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
+}
+
+__device__ __forceinline__ void wgmma(float (&d)[48], uint64_t da, uint64_t db, uint32_t scale_d, WgTF32<96>) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n96k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+               : "l"(da), "l"(db), "r"(scale_d));
+}
+
+__device__ __forceinline__ void wgmma(float (&d)[96], uint64_t da, uint64_t db, uint32_t scale_d, WgTF32<192>) {
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %98, 0;\n\t"
+               "wgmma.mma_async.sync.aligned.m64n192k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, %96, %97, p, 1, 1;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])
+               : "l"(da), "l"(db), "r"(scale_d));
+}
+
 // Hopper shared-memory matrix descriptor (cute::GMMA::GmmaDescriptor bit layout): start address, leading / stride byte
 // offsets in 16-byte units, layout type 1 = SWIZZLE_128B.
 //   K-major:  8-row groups 1024 B apart (SBO); LBO unused (a wgmma's K extent stays inside one 128 B swizzle row).
@@ -290,20 +321,47 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t 
   return d;
 }
 
-// One k-block of wgmmas for a consumer warpgroup: BK / MMA_K steps x MT sub-tiles, all against the same B descriptor.
-// a_step / b_step: descriptor advance per step (K-major: 32 B; MN-major: MMA_K k-rows of 128 B).
-template <typename T, int BN, int MT, int TA, int TB>
+// One k-block of wgmmas for a consumer warpgroup, issued as one group and retired before returning: STEPS k-steps x the first
+// LIVE of the MT sub-tiles, all against the same B descriptor.  a_step / b_step: descriptor advance per step (K-major: 32 B;
+// MN-major: MMA_K k-rows of 128 B).
+template <typename T, int BN, int MT, int TA, int TB, int STEPS, int LIVE>
 __device__ __forceinline__ void mma_kblock(float (&acc)[MT][BN / 2], uint64_t da, uint64_t db, uint32_t a_step, uint32_t b_step) {
-  constexpr int STEPS = Elem<T>::BK / Elem<T>::MMA_K;
   constexpr uint64_t SUB = (uint64_t)(BM * 128) >> 4;
+#pragma unroll
+  for (int u = 0; u < MT; ++u) acc_fence(acc[u]);
+  wgmma_fence();
 #pragma unroll
   for (int k = 0; k < STEPS; ++k) {
 #pragma unroll
-    for (int u = 0; u < MT; ++u) {
+    for (int u = 0; u < LIVE; ++u) {
       if constexpr (Elem<T>::TF32) wgmma(acc[u], da + u * SUB + a_step * k, db + b_step * k, 1u, WgTF32<BN>{});
       else wgmma(acc[u], da + u * SUB + a_step * k, db + b_step * k, 1u, WgBF16<BN, TA, TB>{});
     }
   }
+  wgmma_commit();
+  wgmma_wait0();
+#pragma unroll
+  for (int u = 0; u < MT; ++u) acc_fence(acc[u]);
+}
+
+// The k-block with warpgroup-uniform trims: `steps` <= BK / MMA_K k-steps (the steps past a partial channel chunk would only
+// multiply the boxes' zero fill) and the first `n_live` sub-tiles (the rest hold no row of this warpgroup below M).  Each
+// count selects a whole fence / wgmma / commit / wait sequence: a branch between the wgmmas of one group makes ptxas
+// serialize every wgmma of the kernel (C7520).
+template <typename T, int BN, int MT, int TA, int TB, int LIVE>
+__device__ __forceinline__ void mma_kblock_steps(float (&acc)[MT][BN / 2], uint64_t da, uint64_t db, uint32_t a_step, uint32_t b_step,
+                                                 int steps) {
+  static_assert(Elem<T>::BK / Elem<T>::MMA_K == 4, "k-steps per k-block");
+  if (steps == 4) mma_kblock<T, BN, MT, TA, TB, 4, LIVE>(acc, da, db, a_step, b_step);
+  else if (steps == 3) mma_kblock<T, BN, MT, TA, TB, 3, LIVE>(acc, da, db, a_step, b_step);
+  else if (steps == 2) mma_kblock<T, BN, MT, TA, TB, 2, LIVE>(acc, da, db, a_step, b_step);
+  else mma_kblock<T, BN, MT, TA, TB, 1, LIVE>(acc, da, db, a_step, b_step);
+}
+template <typename T, int BN, int MT, int TA, int TB>
+__device__ __forceinline__ void mma_kblock_trim(float (&acc)[MT][BN / 2], uint64_t da, uint64_t db, uint32_t a_step, uint32_t b_step,
+                                                int steps, int n_live) {
+  if (MT == 2 && n_live == 1) mma_kblock_steps<T, BN, MT, TA, TB, 1>(acc, da, db, a_step, b_step, steps);
+  else mma_kblock_steps<T, BN, MT, TA, TB, MT>(acc, da, db, a_step, b_step, steps);
 }
 
 // tf32 MN-major tile (32-element atoms of 32 k-rows x 128 B, 4 KB apart, 128 B swizzle) → K-major 128 B-swizzled rows,
@@ -401,7 +459,7 @@ gemm_wgmma(const __grid_constant__ CUtensorMap tmap_a0, const __grid_constant__ 
       tile_mn(p, rem, mti, nti);
       const int m0 = mti * TM, n0 = nti * BN;
       const int kb0 = split * p.kb_per_split, kb1 = min(num_kb_total, kb0 + p.kb_per_split);
-      // sub-tiles that start beyond M are not loaded at all (their wgmmas chew on stale smem; the epilogue drops the rows)
+      // sub-tiles that start beyond M are not loaded at all (the consumers issue no wgmma for them; the epilogue drops the rows)
       const int n_sub = (MT == 2 && m0 + BM < p.M) ? 2 : 1;
       if (p.conv_mode == 1) {
         // ---- conv fprop / dgrad: A = im2col box [128 pixels x BK ch] of filter tap (r_, s_), channel chunk cc; B = weights
@@ -544,6 +602,11 @@ gemm_wgmma(const __grid_constant__ CUtensorMap tmap_a0, const __grid_constant__ 
   const int lr = lane / vec_per_row, lv = lane % vec_per_row;
   const bool ld_ok = (((long long)p.ldc * esz) % 16) == 0;
   const int fr = lane >> 2, fc = 2 * (lane & 3);   // accumulator fragment: rows fr, fr + 8 / columns fc, fc + 1 of each 8
+  // fprop / dgrad k-blocks walk (tap, channel chunk) with the chunk fastest; the last chunk of a tap holds only
+  // Cg - (c_chunks - 1) * BK channels, and the k-steps past them would multiply the boxes' zero fill
+  constexpr int STEPS = BK / MMA_K;
+  const int k_chunks = p.conv_mode == 1 ? p.c_chunks : 1;
+  const int tail_steps = p.conv_mode == 1 ? (p.cCg - (p.c_chunks - 1) * BK + MMA_K - 1) / MMA_K : STEPS;
   float acc[MT][BN / 2];
   int stage = 0; uint32_t phase = 0;
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -554,36 +617,39 @@ gemm_wgmma(const __grid_constant__ CUtensorMap tmap_a0, const __grid_constant__ 
     tile_mn(p, rem, mti, nti);
     const int m0 = mti * TM, n0 = nti * BN;
     const int kb0 = split * p.kb_per_split, kb1 = min(num_kb_total, kb0 + p.kb_per_split);
+    // sub-tiles in which this warpgroup owns at least one row below M (a prefix of the MT sub-tiles); a warpgroup with none
+    // issues no wgmma for the tile but still hands every slot back
+    int n_live = 0;
+#pragma unroll
+    for (int u = 0; u < MT; ++u) n_live += (m0 + u * BM + 64 * cw < p.M) ? 1 : 0;
+    int cc = kb0 % k_chunks;
 #pragma unroll
     for (int u = 0; u < MT; ++u)
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[u][i] = 0.f;
     for (int kb = kb0; kb < kb1; ++kb) {
       mbar_wait(full_bar(stage), phase);
+      const int steps = cc == k_chunks - 1 ? tail_steps : STEPS;
+      if (++cc == k_chunks) cc = 0;
       const uint32_t sa = smem_base + stage * C::STAGE_BYTES;
       uint32_t a_addr = sa + (uint32_t)cw * (64 * 128), b_addr = sa + C::A_BYTES;
-      if constexpr (C::XPOSE) {
-        if (xa || xb) {
-          wg_bar(cw);                              // every warp of the group is past the previous k-block's wgmmas
-          if (xa) { xpose_tf32(generic(xa_base), generic(a_addr), 64, ctid); a_addr = xa_base; }
-          if (xb) { xpose_tf32(generic(xb_base), generic(b_addr), BN, ctid); b_addr = xb_base; }
-          fence_proxy_async();                     // generic-proxy writes → visible to wgmma
-          wg_bar(cw);
+      if (n_live > 0) {
+        if constexpr (C::XPOSE) {
+          if (xa || xb) {
+            wg_bar(cw);                              // every warp of the group is past the previous k-block's wgmmas
+            if (xa) { xpose_tf32(generic(xa_base), generic(a_addr), 64, ctid); a_addr = xa_base; }
+            if (xb) { xpose_tf32(generic(xb_base), generic(b_addr), BN, ctid); b_addr = xb_base; }
+            fence_proxy_async();                     // generic-proxy writes → visible to wgmma
+            wg_bar(cw);
+          }
         }
-      }
-      if (!skip_mma) {
-        const uint64_t da = make_smem_desc(a_addr, a_lbo, 1024u), db = make_smem_desc(b_addr, b_lbo, 1024u);
-#pragma unroll
-        for (int u = 0; u < MT; ++u) acc_fence(acc[u]);
-        wgmma_fence();
-        if (mode == 0) mma_kblock<T, BN, MT, 0, 0>(acc, da, db, a_step, b_step);
-        else if (mode == 1) mma_kblock<T, BN, MT, 1, 0>(acc, da, db, a_step, b_step);
-        else if (mode == 2) mma_kblock<T, BN, MT, 0, 1>(acc, da, db, a_step, b_step);
-        else mma_kblock<T, BN, MT, 1, 1>(acc, da, db, a_step, b_step);
-        wgmma_commit();
-        wgmma_wait0();
-#pragma unroll
-        for (int u = 0; u < MT; ++u) acc_fence(acc[u]);
+        if (!skip_mma) {
+          const uint64_t da = make_smem_desc(a_addr, a_lbo, 1024u), db = make_smem_desc(b_addr, b_lbo, 1024u);
+          if (mode == 0) mma_kblock_trim<T, BN, MT, 0, 0>(acc, da, db, a_step, b_step, steps, n_live);
+          else if (mode == 1) mma_kblock_trim<T, BN, MT, 1, 0>(acc, da, db, a_step, b_step, steps, n_live);
+          else if (mode == 2) mma_kblock_trim<T, BN, MT, 0, 1>(acc, da, db, a_step, b_step, steps, n_live);
+          else mma_kblock_trim<T, BN, MT, 1, 1>(acc, da, db, a_step, b_step, steps, n_live);
+        }
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(empty_bar(stage));           // this warp is done with the slot
