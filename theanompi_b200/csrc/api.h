@@ -146,7 +146,8 @@ void masked_mean_bwd(const void* dout, const void* mask, void* dh, int Tn, int B
 //   FLAT_RMSPROP           V                                                   alpha, eps, clip
 //   FLAT_ADADELTA          U, V                                                rho, eps
 //   FLAT_RMSPROP_CENTERED  M (U), R, S                                         rho, mu, eps
-enum FlatRuleId : int { FLAT_SGD = 0, FLAT_ADAM, FLAT_RMSPROP, FLAT_ADADELTA, FLAT_RMSPROP_CENTERED };
+//   FLAT_LARS              U                                                   mu, nesterov (0 / 1), inv_k   (+ block_tensor, tensor_scale)
+enum FlatRuleId : int { FLAT_SGD = 0, FLAT_ADAM, FLAT_RMSPROP, FLAT_ADADELTA, FLAT_RMSPROP_CENTERED, FLAT_LARS };
 struct FlatUpdateArgs {
   int rule;
   void* W;
@@ -160,9 +161,29 @@ struct FlatUpdateArgs {
   const float* hp;
   int n_hp;
   long long lo, hi;
-  int filter;                            // SGD: 0 all groups, 1 only non-exchanged groups, 2 only exchanged groups
+  int filter;                            // SGD, LARS: 0 all groups, 1 only non-exchanged groups, 2 only exchanged groups
+  const void* block_tensor;              // LARS: tensor index of every arena block (int32), else null
+  const void* tensor_scale;              // LARS: trust ratio of every tensor (fp32, written by lars_trust), else null
 };
 void flat_update(const FlatUpdateArgs& a, cudaStream_t st);
+// LARS trust ratios over the whole arena, two launches: per-block sums of squares of W and G into partial ([n_blocks, 2] fp32),
+// then one CTA per tensor: norms[t] = {‖W‖, ‖G‖·inv_k} ([n_tensors, 2] fp32) and trust[t] = eta·‖W‖ / (‖g‖ + wd·‖W‖) for the
+// weight group (group 0) when both norms are positive, else 1.  tensor_span: [n_tensors, 2] int64 {element offset, size}.
+struct LarsTrustArgs {
+  const void* W;
+  const void* G;
+  const void* block_tensor;
+  const void* tensor_span;
+  const void* block_group;
+  GroupTable tab;
+  float inv_k, eta;
+  long long n_blocks;
+  int n_tensors;
+  void* partial;
+  void* norms;
+  void* trust;
+};
+void lars_trust(const LarsTrustArgs& a, cudaStream_t st);
 void fused_allreduce_sgd(const FusedArgs& a, int algo, int max_blocks, cudaStream_t st);
 // every rank pushes the fp32 master weights of the slice it owns in the two-shot partition of [lo, hi) to all peers
 void push_master_slices(const FusedArgs& a, int max_blocks, cudaStream_t st);

@@ -98,11 +98,13 @@ __device__ __forceinline__ void block_barrier(const CommCtx& c) {
 // state vectors as float4, lets the rule update them, stores them and refreshes the bf16 shadow.  lr is read from device memory
 // once per launch, so a captured CUDA graph follows lr changes.  A rule holds its hyperparameters (built inside the kernel from
 // scalar launch arguments, which keeps each instantiation's code identical to a hand-written kernel) and its per-element
-// update; `prologue` computes per-launch constants, `skip` drops whole blocks by group.
+// update; `prologue` computes per-launch constants, `skip` drops whole blocks by group, `enter_block` loads per-block constants
+// through the block → tensor table (LARS: the tensor's trust ratio).
 struct FlatRule {
   static constexpr bool kAdvancesStep = false;
   __device__ __forceinline__ void prologue(const unsigned long long* step) {}
   __device__ __forceinline__ bool skip(const GroupTable& tab, int g) const { return false; }
+  __device__ __forceinline__ void enter_block(long long b, const int* block_tensor, const float* tensor_scale) {}
 };
 
 // momentum SGD, `common.cuh: sgd4` (the arithmetic of the GEMM SGD epilogue and the fused collectives).  State: U.
@@ -216,19 +218,35 @@ struct CenteredRmspropRule : FlatRule {
   }
 };
 
+// LARS (layer-wise adaptive rate scaling, You, Gitman and Ginsburg 2017): momentum SGD with the effective gradient of every tensor
+// scaled by its trust ratio t (lars_trust below), i.e. sgd4 with inv_k·t and wd·t.  State: U.  filter as SgdRule.
+struct LarsRule : SgdRule {
+  float t_inv_k = 0.f, t = 0.f;
+  __device__ __forceinline__ LarsRule(float a, float b, float c, int i, int j) : SgdRule(a, b, c, i, j) {}
+  __device__ __forceinline__ void enter_block(long long b, const int* block_tensor, const float* tensor_scale) {
+    t = tensor_scale[block_tensor[b]];
+    t_inv_k = inv_k * t;
+  }
+  __device__ __forceinline__ void apply(float4& w, float4* s, const float4& gg, float lr0, float lrm, float wd) const {
+    sgd4(w, s[0], gg, Hyper{lr0, mu, t_inv_k, nesterov}, lrm, wd * t);
+  }
+};
+
 template <class Rule>
 __global__ void __launch_bounds__(kThreads) flat_update_kernel(float* __restrict__ W, const float* __restrict__ G, float* __restrict__ S0,
                                                                float* __restrict__ S1, float* __restrict__ S2, __nv_bfloat16* __restrict__ H,
                                                                const uint8_t* __restrict__ block_group, GroupTable tab,
                                                                const float* __restrict__ lr_ptr, const unsigned long long* __restrict__ step,
                                                                float ha, float hb, float hc, int ia, int ib, long long blk_lo,
-                                                               long long blk_hi) {
+                                                               long long blk_hi, const int* __restrict__ block_tensor,
+                                                               const float* __restrict__ tensor_scale) {
   Rule r(ha, hb, hc, ia, ib);
   r.prologue(step);
   const float lr0 = *lr_ptr;
   for (long long b = blk_lo + blockIdx.x; b < blk_hi; b += gridDim.x) {
     const int g = block_group[b];
     if (r.skip(tab, g)) continue;
+    r.enter_block(b, block_tensor, tensor_scale);
     const long long i = b * kArenaBlock + threadIdx.x * 4;
     float4 w = *reinterpret_cast<const float4*>(W + i), s[Rule::kState];
     s[0] = *reinterpret_cast<const float4*>(S0 + i);
@@ -254,27 +272,106 @@ static void launch_flat_update(const char* name, const FlatUpdateArgs& a, float 
   flat_update_kernel<Rule><<<grid, kThreads, 0, st>>>((float*)a.W, (const float*)a.G, (float*)a.S[0], (float*)a.S[1], (float*)a.S[2],
                                                       (__nv_bfloat16*)a.H, (const uint8_t*)a.block_group, a.tab, (const float*)a.lr_ptr,
                                                       (const unsigned long long*)a.step, ha, hb, hc, ia, ib, a.lo / kArenaBlock,
-                                                      a.hi / kArenaBlock);
+                                                      a.hi / kArenaBlock, (const int*)a.block_tensor, (const float*)a.tensor_scale);
   if (Rule::kAdvancesStep) adam_advance_kernel<<<1, 32, 0, st>>>((unsigned long long*)a.step);
   count_launch(Rule::kAdvancesStep ? 2 : 1); TMPI_CHECK_LAUNCH(name); ::tmpi::check_capture(st, name);
 }
 
 void flat_update(const FlatUpdateArgs& a, cudaStream_t st) {
-  static const char* const names[] = {"sgd_flat", "adam_flat", "rmsprop_flat", "adadelta_flat", "rmsprop_centered_flat"};
-  static const int n_hp[] = {3, 3, 3, 2, 3};
-  if (a.rule < FLAT_SGD || a.rule > FLAT_RMSPROP_CENTERED) throw std::runtime_error("flat_update: unknown rule " + std::to_string(a.rule));
+  static const char* const names[] = {"sgd_flat", "adam_flat", "rmsprop_flat", "adadelta_flat", "rmsprop_centered_flat", "lars_flat"};
+  static const int n_hp[] = {3, 3, 3, 2, 3, 3};
+  if (a.rule < FLAT_SGD || a.rule > FLAT_LARS) throw std::runtime_error("flat_update: unknown rule " + std::to_string(a.rule));
   const char* name = names[a.rule];
   if (a.n_hp != n_hp[a.rule])
     throw std::runtime_error(std::string(name) + ": expected " + std::to_string(n_hp[a.rule]) + " hyperparameters");
   if (a.rule == FLAT_ADAM && !a.step) throw std::runtime_error("adam_flat: needs a step counter");
+  if (a.rule == FLAT_LARS && (!a.block_tensor || !a.tensor_scale)) throw std::runtime_error("lars_flat: needs the block → tensor table and the trust ratios");
   const float* h = a.hp;
   switch (a.rule) {
     case FLAT_SGD: launch_flat_update<SgdRule>(name, a, h[0], h[2], 0.f, h[1] != 0.f, a.filter, st); break;
     case FLAT_ADAM: launch_flat_update<AdamRule>(name, a, h[0], h[1], h[2], 0, 0, st); break;
     case FLAT_RMSPROP: launch_flat_update<RmspropRule>(name, a, h[0], h[1], h[2], 0, 0, st); break;
     case FLAT_ADADELTA: launch_flat_update<AdadeltaRule>(name, a, h[0], h[1], 0.f, 0, 0, st); break;
-    default: launch_flat_update<CenteredRmspropRule>(name, a, h[0], h[1], h[2], 0, 0, st); break;
+    case FLAT_RMSPROP_CENTERED: launch_flat_update<CenteredRmspropRule>(name, a, h[0], h[1], h[2], 0, 0, st); break;
+    default: launch_flat_update<LarsRule>(name, a, h[0], h[2], 0.f, h[1] != 0.f, a.filter, st); break;
   }
+}
+
+// ============================================================================ LARS trust ratios
+// Pass 1: for every arena block of [blk_lo, blk_hi), the sums of squares of W and of the gradient over the block's real elements
+// (those below the end of its tensor) → partial[b] = {Σw², Σg²}.  One block per CTA iteration, one float4 per thread, warp shuffles
+// and a fixed-order sum over the 8 warps: no atomics, so the result does not depend on the grid.
+__global__ void __launch_bounds__(kThreads) lars_partial_kernel(const float* __restrict__ W, const float* __restrict__ G,
+                                                                const int* __restrict__ block_tensor, const long long* __restrict__ tensor_span,
+                                                                float2* __restrict__ partial, long long blk_lo, long long blk_hi) {
+  __shared__ float2 red[kThreads / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (long long b = blk_lo + blockIdx.x; b < blk_hi; b += gridDim.x) {
+    const long long i = b * kArenaBlock + threadIdx.x * 4;
+    const int t = block_tensor[b];
+    const long long end = tensor_span[2 * t] + tensor_span[2 * t + 1];
+    float4 w = *reinterpret_cast<const float4*>(W + i), g = *reinterpret_cast<const float4*>(G + i);
+    if (i + 4 > end) {                                   // the tensor's last block: zero the padding past its end
+      if (i + 0 >= end) { w.x = 0.f; g.x = 0.f; }
+      if (i + 1 >= end) { w.y = 0.f; g.y = 0.f; }
+      if (i + 2 >= end) { w.z = 0.f; g.z = 0.f; }
+      if (i + 3 >= end) { w.w = 0.f; g.w = 0.f; }
+    }
+    float sw = w.x * w.x + w.y * w.y + w.z * w.z + w.w * w.w;
+    float sg = g.x * g.x + g.y * g.y + g.z * g.z + g.w * g.w;
+    sw = warp_sum(sw); sg = warp_sum(sg);
+    if (lane == 0) red[warp] = make_float2(sw, sg);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      float2 s = red[0];
+#pragma unroll
+      for (int k = 1; k < kThreads / 32; ++k) { s.x += red[k].x; s.y += red[k].y; }
+      partial[b] = s;
+    }
+    __syncthreads();                                     // red[] is reused by the next block
+  }
+}
+
+// Pass 2: one CTA per tensor sums its block partials in fp64 in a fixed order and writes norms[t] = {‖W‖, ‖g‖} (g = G·inv_k) and
+// the trust ratio: eta·‖W‖ / (‖g‖ + wd·‖W‖) for the weight group when both norms are positive, else 1.
+constexpr int kLarsGroupW = 0;                           // parallel/arena.py G_W
+__global__ void __launch_bounds__(kThreads) lars_finalize_kernel(const float2* __restrict__ partial, const long long* __restrict__ tensor_span,
+                                                                 const uint8_t* __restrict__ block_group, GroupTable tab, float inv_k, float eta,
+                                                                 float2* __restrict__ norms, float* __restrict__ trust) {
+  __shared__ double red[2][kThreads / 32];
+  const int t = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long b0 = tensor_span[2 * t] / kArenaBlock, nb = ceil_div64(tensor_span[2 * t + 1], kArenaBlock);
+  double sw = 0.0, sg = 0.0;
+  for (long long k = threadIdx.x; k < nb; k += kThreads) {
+    const float2 p = partial[b0 + k];
+    sw += (double)p.x; sg += (double)p.y;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) { sw += __shfl_xor_sync(0xffffffffu, sw, o); sg += __shfl_xor_sync(0xffffffffu, sg, o); }
+  if (lane == 0) { red[0][warp] = sw; red[1][warp] = sg; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    sw = red[0][0]; sg = red[1][0];
+    for (int k = 1; k < kThreads / 32; ++k) { sw += red[0][k]; sg += red[1][k]; }
+    const double wn = sqrt(sw), gn = sqrt(sg) * (double)inv_k;
+    const int grp = nb > 0 ? block_group[b0] : -1;      // an empty tensor owns no block
+    double tr = 1.0;
+    if (grp == kLarsGroupW && wn > 0.0 && gn > 0.0) tr = (double)eta * wn / (gn + (double)tab.wd[grp] * wn);
+    norms[t] = make_float2((float)wn, (float)gn);
+    trust[t] = (float)tr;
+  }
+}
+
+void lars_trust(const LarsTrustArgs& a, cudaStream_t st) {
+  if (a.n_blocks <= 0 || a.n_tensors <= 0) return;
+  const int grid = (int)std::min<long long>(a.n_blocks, (long long)sm_count() * 8);
+  lars_partial_kernel<<<grid, kThreads, 0, st>>>((const float*)a.W, (const float*)a.G, (const int*)a.block_tensor,
+                                                 (const long long*)a.tensor_span, (float2*)a.partial, 0, a.n_blocks);
+  TMPI_CHECK_LAUNCH("lars_partial");
+  lars_finalize_kernel<<<a.n_tensors, kThreads, 0, st>>>((const float2*)a.partial, (const long long*)a.tensor_span,
+                                                         (const uint8_t*)a.block_group, a.tab, a.inv_k, a.eta, (float2*)a.norms,
+                                                         (float*)a.trust);
+  count_launch(2); TMPI_CHECK_LAUNCH("lars_finalize"); ::tmpi::check_capture(st, "lars_trust");
 }
 
 // ============================================================================ fused collectives

@@ -90,6 +90,9 @@ class ModelBase(object):
         self.step_idx = 0
         self.mu = self.momentum
         self.eta = self.weight_decay
+        # 'sgd' (momentum SGD) or 'lars' (the same with a per-tensor trust ratio, utils/opt.py: FlatLARS) for large global batches
+        self.optimizer = config.get("optimizer", "sgd")
+        self.lars_eta = float(config.get("lars_eta", 0.001))
         self.base_lr = np.float32(self.learning_rate)
         self.current_t = self.subb_t = 0
         self.current_v = self.subb_v = 0
@@ -336,10 +339,19 @@ class ModelBase(object):
         """``sync_type='cdd'``: split step (get_vel / exchange / descent_vel);
         ``'avg'``: self-contained local update (k = 1), the exchanger then averages
         weights.  Fixes SURVEY §2.9 #5/#7: every model accepts ``sync_type`` and 'avg'
-        really updates."""
+        really updates.
+
+        ``optimizer='lars'`` needs each tensor's whole reduced gradient before it updates any of its elements, so it runs on the
+        split strategies (``ar``, ``nccl32``, ``nccl16``, ``asa32``, ``p2p32``, …) and not on a fused exchange (``fused_tail``)."""
+        if self.optimizer not in ("sgd", "lars"):
+            raise ValueError("%s: optimizer must be 'sgd' or 'lars', not %r" % (self.name, self.optimizer))
+        k = self.size if sync_type == "cdd" else 1
+        if self.optimizer == "lars" and fused_tail is not None:
+            raise ValueError("optimizer='lars' needs every tensor's whole reduced gradient before its update; the fused exchange "
+                             "strategies (fused*, oneshot*, twoshot*, nvls*, fused_rs) update bucket slices as they are reduced. "
+                             "Use a split strategy: ar, nccl32, nccl16, asa32, asa16 or p2p32")
         start = time.time()
         self.sync_type = sync_type
-        k = self.size if sync_type == "cdd" else 1
         if k > 1 and fused_tail is None:
             _ = self.arena.R                      # allocate the receive region
         pre_model_iter_fn(self, k, aggregate=aggregate, fused_tail=fused_tail)

@@ -746,19 +746,34 @@ def _table(arena):
     return arena._tab_cache
 
 
-def flat_update(arena, rule, hyper, state, step=None, g=None, lo=0, hi=None, filt=0):
+def flat_update(arena, rule, hyper, state, step=None, g=None, lo=0, hi=None, filt=0, trust=None):
     """One step of the local flat optimizer ``rule`` (a key of ``FLAT_RULES``: sgd, adam, rmsprop, adadelta,
-    rmsprop_centered) over arena elements [lo, hi) in one launch (``csrc/comm_kernels.cu: flat_update_kernel``; Adam adds
+    rmsprop_centered, lars) over arena elements [lo, hi) in one launch (``csrc/comm_kernels.cu: flat_update_kernel``; Adam adds
     the launch that advances its ``step`` counter).  ``state``: the rule's flat fp32 buffers, the arena's U region first when
-    the rule uses it; ``hyper``: its float hyper-parameters (order in ``csrc/api.h``); ``filt`` (SGD): 1 only non-exchanged
-    groups, 2 only exchanged groups.  lr is read from ``arena.hyper[0]`` on the device, so a captured CUDA graph follows lr
-    changes, and the bf16 shadow is refreshed in the same pass."""
+    the rule uses it; ``hyper``: its float hyper-parameters (order in ``csrc/api.h``); ``filt`` (SGD, LARS): 1 only
+    non-exchanged groups, 2 only exchanged groups; ``trust`` (LARS): the per-tensor trust ratios from :func:`lars_trust`.  lr is
+    read from ``arena.hyper[0]`` on the device, so a captured CUDA graph follows lr changes, and the bf16 shadow is refreshed in
+    the same pass."""
     lrm, wd, ex = _table(arena)
     S = [t.data_ptr() for t in state] + [0] * (3 - len(state))
     lib = L()
     lib.flat_update(lib.FLAT_RULES[rule], arena.W.data_ptr(), (arena.G if g is None else g).data_ptr(), *S, _p(arena.H),
                     arena.block_group.data_ptr(), lrm, wd, ex, arena.hyper.data_ptr(), _p(step), [float(v) for v in hyper],
-                    int(lo), int(arena.numel if hi is None else hi), int(filt), _st(arena.W))
+                    int(lo), int(arena.numel if hi is None else hi), int(filt),
+                    0 if trust is None else arena.block_tensor.data_ptr(), _p(trust), _st(arena.W))
+
+
+def lars_trust(arena, g, inv_k, eta, partial, norms, trust):
+    """LARS trust ratios of every arena tensor from W and the gradient region ``g`` (two launches, ``csrc/comm_kernels.cu:
+    lars_partial_kernel, lars_finalize_kernel``): ``partial`` [n_blocks, 2] receives the per-block sums of squares, ``norms``
+    [n_tensors, 2] ‖W‖ and ‖g·inv_k‖, ``trust`` [n_tensors] eta·‖W‖ / (‖g‖ + wd·‖W‖) for the weight group (1 elsewhere and when a
+    norm is zero).  Every input is read from device memory, so the launches can be captured in a CUDA graph."""
+    for t, shape in ((partial, (arena.n_blocks, 2)), (norms, (len(arena.sizes), 2)), (trust, (len(arena.sizes),))):
+        assert t.dtype == torch.float32 and t.is_contiguous() and tuple(t.shape) == shape, (t.dtype, tuple(t.shape), shape)
+    lrm, wd, ex = _table(arena)
+    L().lars_trust(arena.W.data_ptr(), g.data_ptr(), arena.block_tensor.data_ptr(), arena.tensor_span.data_ptr(),
+                   arena.block_group.data_ptr(), lrm, wd, ex, float(inv_k), float(eta), int(arena.n_blocks), len(arena.sizes),
+                   partial.data_ptr(), norms.data_ptr(), trust.data_ptr(), _st(arena.W))
 
 
 def sgd_flat(arena, g, lr, mu, nesterov, inv_k, lo, hi, only_local=False, only_exchanged=False):

@@ -327,6 +327,38 @@ def rmsprop_centered_flat(w, g, m, r, s, lr_mult, wd, lr, rho=0.95, mu=0.9, eps=
     return w, m, r, s
 
 
+def lars_flat(w, g, u, offsets, sizes, groups, group_lr_mult, group_wd, lr, mu, nesterov, eta=0.001, inv_k=1.0, update=None,
+              w_half=None):
+    """One LARS step (layer-wise adaptive rate scaling) over flat fp32 buffers laid out as a :class:`FlatArena`: tensor ``i`` is
+    ``[offsets[i], offsets[i] + sizes[i])`` in hyper-parameter group ``groups[i]``.  Per tensor, with g = G·inv_k:
+
+        trust = eta·‖W‖ / (‖g‖ + wd·‖W‖)   for the weight group when ‖W‖ > 0 and ‖g‖ > 0, else 1
+        momentum SGD (:func:`sgd_flat`) with inv_k·trust and wd·trust in place of inv_k and wd
+
+    Norms are accumulated in fp64 over the tensor's real elements.  ``update``: per-tensor booleans, the tensors to update (all
+    when None); the trust ratios of every tensor are computed.  Returns (trust [n] fp32, norms [n, 2] fp32: ‖W‖, ‖g‖)."""
+    from ..parallel.arena import G_W
+    n, eta = len(offsets), float(np.float32(eta))
+    trust = torch.ones(n, dtype=torch.float32)
+    norms = torch.zeros(n, 2, dtype=torch.float32)
+    for i, (o, s, grp) in enumerate(zip(offsets, sizes, groups)):
+        sl = slice(o, o + s)
+        wn = float(w[sl].double().norm())
+        gn = float(g[sl].double().norm()) * float(np.float32(inv_k))
+        wd = float(group_wd[grp])
+        norms[i, 0], norms[i, 1] = wn, gn
+        if grp == G_W and wn > 0 and gn > 0:
+            trust[i] = eta * wn / (gn + wd * wn)
+        if update is not None and not update[i]:
+            continue
+        t = np.float32(trust[i])
+        sgd_flat(w[sl], g[sl], u[sl], float(group_lr_mult[grp]), float(np.float32(wd) * t), lr, mu, nesterov,
+                 float(np.float32(inv_k) * t))
+        if w_half is not None:
+            w_half[sl].copy_(w[sl])
+    return trust, norms
+
+
 def easgd_elastic(w, c, alpha):
     """EASGD elastic move (ref ``exchanger.py:188-211``) with both sides updated
     from the SAME difference: ``d = alpha (w - c); w -= d; c += d``."""

@@ -87,6 +87,11 @@ class FlatArena(object):
         for o, s, g in zip(self.offsets, self.sizes, self.group_of):
             bg[o // BLOCK:(o + int(math.ceil(s / BLOCK)) * BLOCK) // BLOCK] = g
         self.block_group_np = bg
+        # per-tensor reductions (LARS norms): the tensor of every block, and every tensor's {element offset, size}
+        bt = np.zeros(self.n_blocks, dtype=np.int32)
+        for t, (o, s) in enumerate(zip(self.offsets, self.sizes)):
+            bt[o // BLOCK:(o + int(math.ceil(s / BLOCK)) * BLOCK) // BLOCK] = t
+        self.block_tensor_np = bt
 
         # ---- storage: one allocation, carved into regions (256 B aligned)
         self._regions = {}
@@ -115,6 +120,8 @@ class FlatArena(object):
 
         dev = self.device
         self.block_group = torch.from_numpy(bg).to(dev)
+        self.block_tensor = torch.from_numpy(bt).to(dev)
+        self.tensor_span = torch.tensor(list(zip(self.offsets, self.sizes)), dtype=torch.int64, device=dev).view(n, 2)
         self.group_lr_mult = torch.from_numpy(lr_mult).to(dev)
         self.group_wd = torch.from_numpy(wd).to(dev)
         self.group_exch = torch.from_numpy(exch).to(dev)

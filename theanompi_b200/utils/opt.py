@@ -17,6 +17,9 @@ flat arena (one launch each):
 ``BSP_SGD``    no momentum           (``opt.py:271-330``)
                pre : G ← lr·m · (G + ηW) / k       send = G
                post: W ← W − R
+``BSP_LARS``   :class:`FlatLARS`, aggregate gradient (``config['optimizer'] = 'lars'``; no counterpart in the reference)
+               pre : batch-norm groups             send = G
+               post: LARS step from R / k
 
 (m = per-group lr multiplier: 1 for 'W', 2 for 'b'; η only on 'W'; BN gamma/beta
 are updated locally in the pre step and never exchanged, ``opt.py:207-226``.)
@@ -263,6 +266,47 @@ class FlatCenteredRMSProp(FlatOptimizer):
         return (self.rho, self.mu, self.eps)
 
 
+class FlatLARS(FlatOptimizer):
+    """LARS (layer-wise adaptive rate scaling; You, Gitman and Ginsburg, 2017): momentum SGD in which every weight tensor's
+    effective gradient is scaled by its trust ratio ``eta·‖W‖ / (‖g‖ + wd·‖W‖)``; biases and batch-norm parameters keep ratio 1.
+    Momentum lives in the arena's U region, so checkpoints carry it.
+
+    On CUDA a step is three launches that read only device memory (CUDA-graph capturable, bit-reproducible): per-block sums of
+    squares, one per-tensor reduction that writes :attr:`norms` ([n_tensors, 2]: ‖W‖, ‖g‖) and :attr:`trust` ([n_tensors]), and
+    the ``flat_update`` pass of the LARS rule.  The update needs every tensor's whole gradient before it changes any element, so
+    LARS never runs in the FC weight-gradient GEMM epilogue (:meth:`FlatSGD.arm`)."""
+
+    rule = "lars"
+
+    def __init__(self, arena, mu=0.9, nesterov=False, eta=0.001):
+        super().__init__(arena)
+        self.mu, self.nesterov, self.eta = mu, nesterov, eta
+        n, dev = len(arena.sizes), arena.W.device
+        self.trust = torch.ones(n, dtype=torch.float32, device=dev)
+        self.norms = torch.zeros(n, 2, dtype=torch.float32, device=dev)
+        self._partial = torch.zeros(arena.n_blocks, 2, dtype=torch.float32, device=dev) if arena.W.is_cuda else None
+
+    def step(self, lr=None, k=1, src="G", only_local=False, only_exchanged=False):
+        """``k``: the gradient region holds the sum of k gradients (inv_k = 1/k); ``src``: that region ("G", or "R" after the
+        exchange); ``only_local`` / ``only_exchanged``: update only the non-exchanged (batch-norm) or only the exchanged groups."""
+        a = self.arena
+        g = getattr(a, src)
+        if a.W.is_cuda:
+            from ..ops import cuda_impl
+            cuda_impl.lars_trust(a, g, 1.0 / k, self.eta, self._partial, self.norms, self.trust)
+            filt = 1 if only_local else (2 if only_exchanged else 0)
+            cuda_impl.flat_update(a, "lars", (self.mu, float(bool(self.nesterov)), 1.0 / k), [a.U], g=g, filt=filt, trust=self.trust)
+            return
+        update = None
+        if only_local or only_exchanged:
+            update = [m != only_local for m in a.exchanged_mask()]
+        trust, norms = ref.lars_flat(a.W, g, a.U, a.offsets, a.sizes, a.group_of, a.group_lr_mult_np, a.group_wd_np,
+                                     float(a.hyper[0]) if lr is None else lr, self.mu, self.nesterov, self.eta, 1.0 / k,
+                                     update=update, w_half=a.H)
+        self.trust.copy_(trust)
+        self.norms.copy_(norms)
+
+
 # --------------------------------------------------------------------------- classic split (API parity)
 def _ex(a):
     return a.exch_vector()
@@ -349,6 +393,25 @@ def _pre_post_sgd(model, k, arm=True):
     return pre, post, "G"
 
 
+def _pre_post_lars(model, k):
+    """LARS, aggregate gradient.  k = 1: the whole step in ``pre``.  k > 1: ``pre`` updates the non-exchanged (batch-norm) groups
+    and sends G; ``post`` updates the exchanged groups from R = Σ_ranks G, so the trust ratios come from the averaged gradient."""
+    lars = model.lars = FlatLARS(model.arena, model.mu if model.use_momentum else 0.0, model.use_nesterov_momentum, model.lars_eta)
+
+    def pre():
+        if k == 1:
+            lars.step()
+            return
+        lars.step(only_local=True)
+
+    def post():
+        if k == 1:
+            return
+        lars.step(k=k, src="R", only_exchanged=True)
+
+    return pre, post, "G"
+
+
 def _publish(model, pre, post, send_region, k):
     a = model.arena
     mask = a.exchanged_mask()
@@ -373,6 +436,10 @@ def BSP_SGD(model, k=1, arm=True):
     return _publish(model, *_pre_post_sgd(model, k, arm), k)
 
 
+def BSP_LARS(model, k=1):
+    return _publish(model, *_pre_post_lars(model, k), k)
+
+
 def _clip_paramlist(param_list, scale=10):
     """``T.clip(param,-10,10)`` helper (ref ``opt.py:67-75``; unused there too)."""
     with torch.no_grad():
@@ -383,7 +450,10 @@ def _clip_paramlist(param_list, scale=10):
 
 def prepare_update_dict(model, k=1, aggregate="momentum", arm=True):
     """``arm``: at k = 1, let the FC weight-gradient GEMMs apply the update of their weights (:meth:`FlatSGD.arm`); only valid
-    when the returned ``pre`` is what updates the arena after every backward."""
+    when the returned ``pre`` is what updates the arena after every backward.  ``model.optimizer == 'lars'``: :func:`BSP_LARS`,
+    which never arms."""
+    if getattr(model, "optimizer", "sgd") == "lars":
+        return BSP_LARS(model, k=k)
     if model.use_momentum:
         if aggregate == "gradient":
             return _BSP_MSGD(model, model.use_nesterov_momentum, k=k, arm=arm)
