@@ -147,7 +147,8 @@ void masked_mean_bwd(const void* dout, const void* mask, void* dh, int Tn, int B
 //   FLAT_ADADELTA          U, V                                                rho, eps
 //   FLAT_RMSPROP_CENTERED  M (U), R, S                                         rho, mu, eps
 //   FLAT_LARS              U                                                   mu, nesterov (0 / 1), inv_k   (+ block_tensor, tensor_scale)
-enum FlatRuleId : int { FLAT_SGD = 0, FLAT_ADAM, FLAT_RMSPROP, FLAT_ADADELTA, FLAT_RMSPROP_CENTERED, FLAT_LARS };
+//   FLAT_LAMB              M (U), V (read only: lamb_trust advanced them)      b1, b2, eps           (+ step, block_tensor, tensor_scale)
+enum FlatRuleId : int { FLAT_SGD = 0, FLAT_ADAM, FLAT_RMSPROP, FLAT_ADADELTA, FLAT_RMSPROP_CENTERED, FLAT_LARS, FLAT_LAMB };
 struct FlatUpdateArgs {
   int rule;
   void* W;
@@ -157,13 +158,13 @@ struct FlatUpdateArgs {
   const void* block_group;
   GroupTable tab;
   const void* lr_ptr;
-  void* step;                            // Adam: device step counter (uint64), else null
+  void* step;                            // Adam, LAMB: device step counter (uint64; LAMB: not advanced by a filter-1 pass), else null
   const float* hp;
   int n_hp;
   long long lo, hi;
-  int filter;                            // SGD, LARS: 0 all groups, 1 only non-exchanged groups, 2 only exchanged groups
-  const void* block_tensor;              // LARS: tensor index of every arena block (int32), else null
-  const void* tensor_scale;              // LARS: trust ratio of every tensor (fp32, written by lars_trust), else null
+  int filter;                            // SGD, LARS, LAMB: 0 all groups, 1 only non-exchanged groups, 2 only exchanged groups
+  const void* block_tensor;              // LARS, LAMB: tensor index of every arena block (int32), else null
+  const void* tensor_scale;              // LARS, LAMB: trust ratio of every tensor (fp32, from lars_trust / lamb_trust), else null
 };
 void flat_update(const FlatUpdateArgs& a, cudaStream_t st);
 // LARS trust ratios over the whole arena, two launches: per-block sums of squares of W and G into partial ([n_blocks, 2] fp32),
@@ -184,6 +185,29 @@ struct LarsTrustArgs {
   void* trust;
 };
 void lars_trust(const LarsTrustArgs& a, cudaStream_t st);
+// LAMB passes 1 and 2 over the blocks whose group `filter` keeps (as in flat_update), two launches: with g = G·inv_k and t = *step + 1,
+// advance M (the arena's U) and V in place and write the per-block sums of squares of W and of the update direction
+// r = (M·c1) / (sqrt(V·c2) + eps) + wd·W into partial; then norms[t] = {‖W‖, ‖r‖} and trust[t] = ‖W‖ / ‖r‖ for the weight group
+// when both norms are positive, else 1.  Neither W, G nor the counter changes: the FLAT_LAMB flat_update pass follows.
+struct LambTrustArgs {
+  const void* W;
+  const void* G;
+  void* M;
+  void* V;
+  const void* step;
+  float b1, b2, eps, inv_k;
+  int filter;
+  const void* block_tensor;
+  const void* tensor_span;
+  const void* block_group;
+  GroupTable tab;
+  long long n_blocks;
+  int n_tensors;
+  void* partial;
+  void* norms;
+  void* trust;
+};
+void lamb_trust(const LambTrustArgs& a, cudaStream_t st);
 void fused_allreduce_sgd(const FusedArgs& a, int algo, int max_blocks, cudaStream_t st);
 // every rank pushes the fp32 master weights of the slice it owns in the two-shot partition of [lo, hi) to all peers
 void push_master_slices(const FusedArgs& a, int max_blocks, cudaStream_t st);

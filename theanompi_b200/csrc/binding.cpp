@@ -152,7 +152,7 @@ PYBIND11_MODULE(_tmpi_native, m) {
   // ---------------------------------------------------------------- optimizer / legacy kernels
   m.attr("FLAT_RULES") = py::dict(py::arg("sgd") = (int)FLAT_SGD, py::arg("adam") = (int)FLAT_ADAM, py::arg("rmsprop") = (int)FLAT_RMSPROP,
                                    py::arg("adadelta") = (int)FLAT_ADADELTA, py::arg("rmsprop_centered") = (int)FLAT_RMSPROP_CENTERED,
-                                   py::arg("lars") = (int)FLAT_LARS);
+                                   py::arg("lars") = (int)FLAT_LARS, py::arg("lamb") = (int)FLAT_LAMB);
   m.def("flat_update", [](int rule, ptr_t W, ptr_t G, ptr_t S0, ptr_t S1, ptr_t S2, ptr_t H, ptr_t block_group, std::vector<float> lr_mult,
                           std::vector<float> wd, std::vector<int> exch, ptr_t lr_ptr, ptr_t step, std::vector<float> hp, long long lo,
                           long long hi, int filter, ptr_t block_tensor, ptr_t tensor_scale, ptr_t st) {
@@ -163,6 +163,11 @@ PYBIND11_MODULE(_tmpi_native, m) {
                          ptr_t partial, ptr_t norms, ptr_t trust, ptr_t st) {
     lars_trust(LarsTrustArgs{P(W), P(G), P(block_tensor), P(tensor_span), P(block_group), make_table(lr_mult, wd, exch), inv_k, eta,
                              n_blocks, n_tensors, P(partial), P(norms), P(trust)}, S(st)); });
+  m.def("lamb_trust", [](ptr_t W, ptr_t G, ptr_t M, ptr_t V, ptr_t step, float b1, float b2, float eps, float inv_k, int filter,
+                         ptr_t block_tensor, ptr_t tensor_span, ptr_t block_group, std::vector<float> lr_mult, std::vector<float> wd,
+                         std::vector<int> exch, long long n_blocks, int n_tensors, ptr_t partial, ptr_t norms, ptr_t trust, ptr_t st) {
+    lamb_trust(LambTrustArgs{P(W), P(G), P(M), P(V), P(step), b1, b2, eps, inv_k, filter, P(block_tensor), P(tensor_span), P(block_group),
+                             make_table(lr_mult, wd, exch), n_blocks, n_tensors, P(partial), P(norms), P(trust)}, S(st)); });
   m.def("easgd_elastic", [](ptr_t w, ptr_t h, ptr_t center, float alpha, long long n, int max_blocks, ptr_t st, int lockfree) {
     easgd_elastic(P(w), P(h), P(center), alpha, n, max_blocks, lockfree, S(st)); },
     py::arg("w"), py::arg("h"), py::arg("center"), py::arg("alpha"), py::arg("n"), py::arg("max_blocks"), py::arg("st"), py::arg("lockfree") = 0);

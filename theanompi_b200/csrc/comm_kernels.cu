@@ -99,24 +99,29 @@ __device__ __forceinline__ void block_barrier(const CommCtx& c) {
 // once per launch, so a captured CUDA graph follows lr changes.  A rule holds its hyperparameters (built inside the kernel from
 // scalar launch arguments, which keeps each instantiation's code identical to a hand-written kernel) and its per-element
 // update; `prologue` computes per-launch constants, `skip` drops whole blocks by group, `enter_block` loads per-block constants
-// through the block → tensor table (LARS: the tensor's trust ratio).
+// through the block → tensor table (LARS, LAMB: the tensor's trust ratio).  A rule that takes its direction from state written by
+// an earlier pass (LAMB) neither reads G (kReadsG) nor stores its state back (kWritesState).
 struct FlatRule {
   static constexpr bool kAdvancesStep = false;
+  static constexpr bool kReadsG = true;
+  static constexpr bool kWritesState = true;
   __device__ __forceinline__ void prologue(const unsigned long long* step) {}
   __device__ __forceinline__ bool skip(const GroupTable& tab, int g) const { return false; }
   __device__ __forceinline__ void enter_block(long long b, const int* block_tensor, const float* tensor_scale) {}
 };
 
-// momentum SGD, `common.cuh: sgd4` (the arithmetic of the GEMM SGD epilogue and the fused collectives).  State: U.
 // filter: 0 all groups, 1 only non-exchanged (BN) groups, 2 only exchanged groups
+__device__ __forceinline__ bool filtered_out(const GroupTable& tab, int g, int filter) {
+  return (filter == 1 && tab.exch[g]) || (filter == 2 && !tab.exch[g]);
+}
+
+// momentum SGD, `common.cuh: sgd4` (the arithmetic of the GEMM SGD epilogue and the fused collectives).  State: U.  filter as above.
 struct SgdRule : FlatRule {
   static constexpr int kState = 1;
   float mu, inv_k;
   int nesterov, filter;
   __device__ __forceinline__ SgdRule(float a, float b, float, int i, int j) : mu(a), inv_k(b), nesterov(i), filter(j) {}
-  __device__ __forceinline__ bool skip(const GroupTable& tab, int g) const {
-    return (filter == 1 && tab.exch[g]) || (filter == 2 && !tab.exch[g]);
-  }
+  __device__ __forceinline__ bool skip(const GroupTable& tab, int g) const { return filtered_out(tab, g, filter); }
   __device__ __forceinline__ void apply(float4& w, float4* s, const float4& gg, float lr0, float lrm, float wd) const {
     sgd4(w, s[0], gg, Hyper{lr0, mu, inv_k, nesterov}, lrm, wd);
   }
@@ -232,6 +237,45 @@ struct LarsRule : SgdRule {
   }
 };
 
+// LAMB (You et al. 2019, "Large Batch Optimization for Deep Learning"): Adam moments, decoupled weight decay and a per-tensor trust
+// ratio ‖W‖ / ‖r‖ on the update direction r.  A step is three passes: lamb_moments_kernel advances M and V and writes the per-block
+// sums of squares of W and r, lars_finalize_kernel turns them into the trust ratios, and LambRule recomputes r from the new M, V
+// (with the same helper) and applies it.  Both passes read the step counter before adam_advance_kernel bumps it.
+// Bias corrections of step t = *step + 1, c1 = 1 / (1 − b1^t), c2 = 1 / (1 − b2^t), in fp64: 1 − b2^t of the first steps is small.
+__device__ __forceinline__ void lamb_bias_corrections(const unsigned long long* step, float b1, float b2, float& c1, float& c2) {
+  const double t = (double)(*step + 1ull);
+  c1 = (float)(1.0 / (1.0 - pow((double)b1, t)));
+  c2 = (float)(1.0 / (1.0 - pow((double)b2, t)));
+}
+// the update direction of one element from its advanced moments: r = (m·c1) / (sqrt(v·c2) + eps) + wd·w
+__device__ __forceinline__ float lamb_dir(float w, float m, float v, float c1, float c2, float eps, float wd) {
+  return (m * c1) / (sqrtf(v * c2) + eps) + wd * w;
+}
+
+// Pass 3 of a LAMB step: w -= lr·lr_mult·trust·r.  State: M (the arena's U), V, both only read here.  filter as SgdRule.
+struct LambRule : FlatRule {
+  static constexpr int kState = 2;
+  static constexpr bool kAdvancesStep = true;              // after a pass with filter != 1 (launch_flat_update)
+  static constexpr bool kReadsG = false;
+  static constexpr bool kWritesState = false;
+  float b1, b2, eps, c1 = 0.f, c2 = 0.f, t = 0.f;
+  int filter;
+  __device__ __forceinline__ LambRule(float a, float b, float c, int i, int) : b1(a), b2(b), eps(c), filter(i) {}
+  __device__ __forceinline__ void prologue(const unsigned long long* step) { lamb_bias_corrections(step, b1, b2, c1, c2); }
+  __device__ __forceinline__ bool skip(const GroupTable& tab, int g) const { return filtered_out(tab, g, filter); }
+  __device__ __forceinline__ void enter_block(long long b, const int* block_tensor, const float* tensor_scale) {
+    t = tensor_scale[block_tensor[b]];
+  }
+  __device__ __forceinline__ void apply(float4& w, float4* s, const float4&, float lr0, float lrm, float wd) const {
+    const float lr = lr0 * lrm * t;
+    const float4 &m = s[0], &v = s[1];
+    w.x -= lr * lamb_dir(w.x, m.x, v.x, c1, c2, eps, wd);
+    w.y -= lr * lamb_dir(w.y, m.y, v.y, c1, c2, eps, wd);
+    w.z -= lr * lamb_dir(w.z, m.z, v.z, c1, c2, eps, wd);
+    w.w -= lr * lamb_dir(w.w, m.w, v.w, c1, c2, eps, wd);
+  }
+};
+
 template <class Rule>
 __global__ void __launch_bounds__(kThreads) flat_update_kernel(float* __restrict__ W, const float* __restrict__ G, float* __restrict__ S0,
                                                                float* __restrict__ S1, float* __restrict__ S2, __nv_bfloat16* __restrict__ H,
@@ -252,12 +296,15 @@ __global__ void __launch_bounds__(kThreads) flat_update_kernel(float* __restrict
     s[0] = *reinterpret_cast<const float4*>(S0 + i);
     if constexpr (Rule::kState > 1) s[1] = *reinterpret_cast<const float4*>(S1 + i);
     if constexpr (Rule::kState > 2) s[2] = *reinterpret_cast<const float4*>(S2 + i);
-    const float4 gg = *reinterpret_cast<const float4*>(G + i);
+    float4 gg = {};
+    if constexpr (Rule::kReadsG) gg = *reinterpret_cast<const float4*>(G + i);
     r.apply(w, s, gg, lr0, tab.lr_mult[g], tab.wd[g]);
     *reinterpret_cast<float4*>(W + i) = w;
-    *reinterpret_cast<float4*>(S0 + i) = s[0];
-    if constexpr (Rule::kState > 1) *reinterpret_cast<float4*>(S1 + i) = s[1];
-    if constexpr (Rule::kState > 2) *reinterpret_cast<float4*>(S2 + i) = s[2];
+    if constexpr (Rule::kWritesState) {
+      *reinterpret_cast<float4*>(S0 + i) = s[0];
+      if constexpr (Rule::kState > 1) *reinterpret_cast<float4*>(S1 + i) = s[1];
+      if constexpr (Rule::kState > 2) *reinterpret_cast<float4*>(S2 + i) = s[2];
+    }
     if (H) *reinterpret_cast<uint2*>(H + i) = pack_bf16x4(w);
   }
 }
@@ -273,19 +320,24 @@ static void launch_flat_update(const char* name, const FlatUpdateArgs& a, float 
                                                       (__nv_bfloat16*)a.H, (const uint8_t*)a.block_group, a.tab, (const float*)a.lr_ptr,
                                                       (const unsigned long long*)a.step, ha, hb, hc, ia, ib, a.lo / kArenaBlock,
                                                       a.hi / kArenaBlock, (const int*)a.block_tensor, (const float*)a.tensor_scale);
-  if (Rule::kAdvancesStep) adam_advance_kernel<<<1, 32, 0, st>>>((unsigned long long*)a.step);
-  count_launch(Rule::kAdvancesStep ? 2 : 1); TMPI_CHECK_LAUNCH(name); ::tmpi::check_capture(st, name);
+  // a filter-1 (batch-norm only) pass is followed by the filter-2 pass of the same step, which advances the counter
+  const bool advance = Rule::kAdvancesStep && a.filter != 1;
+  if (advance) adam_advance_kernel<<<1, 32, 0, st>>>((unsigned long long*)a.step);
+  count_launch(advance ? 2 : 1); TMPI_CHECK_LAUNCH(name); ::tmpi::check_capture(st, name);
 }
 
 void flat_update(const FlatUpdateArgs& a, cudaStream_t st) {
-  static const char* const names[] = {"sgd_flat", "adam_flat", "rmsprop_flat", "adadelta_flat", "rmsprop_centered_flat", "lars_flat"};
-  static const int n_hp[] = {3, 3, 3, 2, 3, 3};
-  if (a.rule < FLAT_SGD || a.rule > FLAT_LARS) throw std::runtime_error("flat_update: unknown rule " + std::to_string(a.rule));
+  static const char* const names[] = {"sgd_flat", "adam_flat", "rmsprop_flat", "adadelta_flat", "rmsprop_centered_flat", "lars_flat",
+                                      "lamb_flat"};
+  static const int n_hp[] = {3, 3, 3, 2, 3, 3, 3};
+  if (a.rule < FLAT_SGD || a.rule > FLAT_LAMB) throw std::runtime_error("flat_update: unknown rule " + std::to_string(a.rule));
   const char* name = names[a.rule];
   if (a.n_hp != n_hp[a.rule])
     throw std::runtime_error(std::string(name) + ": expected " + std::to_string(n_hp[a.rule]) + " hyperparameters");
   if (a.rule == FLAT_ADAM && !a.step) throw std::runtime_error("adam_flat: needs a step counter");
   if (a.rule == FLAT_LARS && (!a.block_tensor || !a.tensor_scale)) throw std::runtime_error("lars_flat: needs the block → tensor table and the trust ratios");
+  if (a.rule == FLAT_LAMB && !a.step) throw std::runtime_error("lamb_flat: needs a step counter");
+  if (a.rule == FLAT_LAMB && (!a.block_tensor || !a.tensor_scale)) throw std::runtime_error("lamb_flat: needs the block → tensor table and the trust ratios");
   const float* h = a.hp;
   switch (a.rule) {
     case FLAT_SGD: launch_flat_update<SgdRule>(name, a, h[0], h[2], 0.f, h[1] != 0.f, a.filter, st); break;
@@ -293,7 +345,8 @@ void flat_update(const FlatUpdateArgs& a, cudaStream_t st) {
     case FLAT_RMSPROP: launch_flat_update<RmspropRule>(name, a, h[0], h[1], h[2], 0, 0, st); break;
     case FLAT_ADADELTA: launch_flat_update<AdadeltaRule>(name, a, h[0], h[1], 0.f, 0, 0, st); break;
     case FLAT_RMSPROP_CENTERED: launch_flat_update<CenteredRmspropRule>(name, a, h[0], h[1], h[2], 0, 0, st); break;
-    default: launch_flat_update<LarsRule>(name, a, h[0], h[2], 0.f, h[1] != 0.f, a.filter, st); break;
+    case FLAT_LARS: launch_flat_update<LarsRule>(name, a, h[0], h[2], 0.f, h[1] != 0.f, a.filter, st); break;
+    default: launch_flat_update<LambRule>(name, a, h[0], h[1], h[2], a.filter, 0, st); break;
   }
 }
 
@@ -372,6 +425,82 @@ void lars_trust(const LarsTrustArgs& a, cudaStream_t st) {
                                                          (const uint8_t*)a.block_group, a.tab, a.inv_k, a.eta, (float2*)a.norms,
                                                          (float*)a.trust);
   count_launch(2); TMPI_CHECK_LAUNCH("lars_finalize"); ::tmpi::check_capture(st, "lars_trust");
+}
+
+// ============================================================================ LAMB trust ratios
+// Pass 1 of a LAMB step, over the blocks of [blk_lo, blk_hi) that `filter` keeps: with g = G·inv_k, advance the moments
+// M = b1·M + (1 − b1)·g, V = b2·V + (1 − b2)·g² and write partial[b] = {Σw², Σr²} over the block's real elements, r = lamb_dir(...).
+// W and G are only read.  A skipped block keeps the partial sums of the last pass that covered it.  The reduction is the one of
+// lars_partial_kernel: no atomics, so the result does not depend on the grid.
+__global__ void __launch_bounds__(kThreads) lamb_moments_kernel(const float* __restrict__ W, const float* __restrict__ G, float* __restrict__ M,
+                                                                float* __restrict__ V, const uint8_t* __restrict__ block_group, GroupTable tab,
+                                                                const unsigned long long* __restrict__ step, float b1, float b2, float eps,
+                                                                float inv_k, int filter, const int* __restrict__ block_tensor,
+                                                                const long long* __restrict__ tensor_span, float2* __restrict__ partial,
+                                                                long long blk_lo, long long blk_hi) {
+  __shared__ float2 red[kThreads / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  float c1, c2;
+  lamb_bias_corrections(step, b1, b2, c1, c2);
+  for (long long b = blk_lo + blockIdx.x; b < blk_hi; b += gridDim.x) {
+    const int grp = block_group[b];
+    if (filtered_out(tab, grp, filter)) continue;          // the same for the whole CTA
+    const float wd = tab.wd[grp];
+    const long long i = b * kArenaBlock + threadIdx.x * 4;
+    const int t = block_tensor[b];
+    const long long end = tensor_span[2 * t] + tensor_span[2 * t + 1];
+    float4 w = *reinterpret_cast<const float4*>(W + i), m = *reinterpret_cast<const float4*>(M + i);
+    float4 v = *reinterpret_cast<const float4*>(V + i);
+    const float4 g = *reinterpret_cast<const float4*>(G + i);
+#define TMPI_LAMB_MOM(c)                                                 \
+  {                                                                     \
+    const float ge = g.c * inv_k;                                       \
+    m.c = b1 * m.c + (1.f - b1) * ge;                                   \
+    v.c = b2 * v.c + (1.f - b2) * ge * ge;                              \
+  }
+    TMPI_LAMB_MOM(x) TMPI_LAMB_MOM(y) TMPI_LAMB_MOM(z) TMPI_LAMB_MOM(w)
+#undef TMPI_LAMB_MOM
+    *reinterpret_cast<float4*>(M + i) = m;
+    *reinterpret_cast<float4*>(V + i) = v;
+    float4 r = make_float4(lamb_dir(w.x, m.x, v.x, c1, c2, eps, wd), lamb_dir(w.y, m.y, v.y, c1, c2, eps, wd),
+                           lamb_dir(w.z, m.z, v.z, c1, c2, eps, wd), lamb_dir(w.w, m.w, v.w, c1, c2, eps, wd));
+    if (i + 4 > end) {                                     // the tensor's last block: zero the padding past its end
+      if (i + 0 >= end) { w.x = 0.f; r.x = 0.f; }
+      if (i + 1 >= end) { w.y = 0.f; r.y = 0.f; }
+      if (i + 2 >= end) { w.z = 0.f; r.z = 0.f; }
+      if (i + 3 >= end) { w.w = 0.f; r.w = 0.f; }
+    }
+    float sw = w.x * w.x + w.y * w.y + w.z * w.z + w.w * w.w;
+    float sr = r.x * r.x + r.y * r.y + r.z * r.z + r.w * r.w;
+    sw = warp_sum(sw); sr = warp_sum(sr);
+    if (lane == 0) red[warp] = make_float2(sw, sr);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      float2 s = red[0];
+#pragma unroll
+      for (int k = 1; k < kThreads / 32; ++k) { s.x += red[k].x; s.y += red[k].y; }
+      partial[b] = s;
+    }
+    __syncthreads();                                       // red[] is reused by the next block
+  }
+}
+
+void lamb_trust(const LambTrustArgs& a, cudaStream_t st) {
+  if (a.n_blocks <= 0 || a.n_tensors <= 0) return;
+  if (!a.step) throw std::runtime_error("lamb_trust: needs a step counter");
+  const int grid = (int)std::min<long long>(a.n_blocks, (long long)sm_count() * 8);
+  lamb_moments_kernel<<<grid, kThreads, 0, st>>>((const float*)a.W, (const float*)a.G, (float*)a.M, (float*)a.V,
+                                                 (const uint8_t*)a.block_group, a.tab, (const unsigned long long*)a.step, a.b1, a.b2,
+                                                 a.eps, a.inv_k, a.filter, (const int*)a.block_tensor, (const long long*)a.tensor_span,
+                                                 (float2*)a.partial, 0, a.n_blocks);
+  TMPI_CHECK_LAUNCH("lamb_moments");
+  // the decay is already inside r: with eta = 1 and no wd, the LARS finalize writes {‖W‖, ‖r‖} and trust = ‖W‖ / ‖r‖
+  GroupTable no_wd = a.tab;
+  for (float& d : no_wd.wd) d = 0.f;
+  lars_finalize_kernel<<<a.n_tensors, kThreads, 0, st>>>((const float2*)a.partial, (const long long*)a.tensor_span,
+                                                         (const uint8_t*)a.block_group, no_wd, 1.f, 1.f, (float2*)a.norms,
+                                                         (float*)a.trust);
+  count_launch(2); TMPI_CHECK_LAUNCH("lars_finalize"); ::tmpi::check_capture(st, "lamb_trust");
 }
 
 // ============================================================================ fused collectives

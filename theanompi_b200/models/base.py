@@ -90,7 +90,8 @@ class ModelBase(object):
         self.step_idx = 0
         self.mu = self.momentum
         self.eta = self.weight_decay
-        # 'sgd' (momentum SGD) or 'lars' (the same with a per-tensor trust ratio, utils/opt.py: FlatLARS) for large global batches
+        # 'sgd' (momentum SGD) or 'lars' (the same with a per-tensor trust ratio, utils/opt.py: FlatLARS) for large global batches,
+        # or 'lamb' (Adam moments with per-tensor trust ratios, utils/opt.py: FlatLAMB)
         self.optimizer = config.get("optimizer", "sgd")
         self.lars_eta = float(config.get("lars_eta", 0.001))
         self.base_lr = np.float32(self.learning_rate)
@@ -341,15 +342,16 @@ class ModelBase(object):
         weights.  Fixes SURVEY §2.9 #5/#7: every model accepts ``sync_type`` and 'avg'
         really updates.
 
-        ``optimizer='lars'`` needs each tensor's whole reduced gradient before it updates any of its elements, so it runs on the
-        split strategies (``ar``, ``nccl32``, ``nccl16``, ``asa32``, ``p2p32``, …) and not on a fused exchange (``fused_tail``)."""
-        if self.optimizer not in ("sgd", "lars"):
-            raise ValueError("%s: optimizer must be 'sgd' or 'lars', not %r" % (self.name, self.optimizer))
+        ``optimizer='lars'`` and ``'lamb'`` need each tensor's whole reduced gradient before they update any of its elements, so
+        they run on the split strategies (``ar``, ``nccl32``, ``nccl16``, ``asa32``, ``p2p32``, …) and not on a fused exchange
+        (``fused_tail``)."""
+        if self.optimizer not in ("sgd", "lars", "lamb"):
+            raise ValueError("%s: optimizer must be 'lamb', 'sgd' or 'lars', not %r" % (self.name, self.optimizer))
         k = self.size if sync_type == "cdd" else 1
-        if self.optimizer == "lars" and fused_tail is not None:
-            raise ValueError("optimizer='lars' needs every tensor's whole reduced gradient before its update; the fused exchange "
+        if self.optimizer in ("lars", "lamb") and fused_tail is not None:
+            raise ValueError("optimizer=%r needs every tensor's whole reduced gradient before its update; the fused exchange "
                              "strategies (fused*, oneshot*, twoshot*, nvls*, fused_rs) update bucket slices as they are reduced. "
-                             "Use a split strategy: ar, nccl32, nccl16, asa32, asa16 or p2p32")
+                             "Use a split strategy: ar, nccl32, nccl16, asa32, asa16 or p2p32" % self.optimizer)
         start = time.time()
         self.sync_type = sync_type
         if k > 1 and fused_tail is None:
@@ -480,13 +482,19 @@ class ModelBase(object):
         return [l for l in (getattr(self, "layers", None) or []) if isinstance(l, BatchNormal)]
 
     def extra_state(self):
-        """Batch-norm running statistics (not parameters, so not in the arena)."""
-        return {"bn": [(l.running_mean.detach().cpu(), l.running_var.detach().cpu()) for l in self._bn_layers()]}
+        """Batch-norm running statistics (not parameters, so not in the arena) and the LAMB second moment and step counter (its
+        first moment is the arena's U region)."""
+        sd = {"bn": [(l.running_mean.detach().cpu(), l.running_var.detach().cpu()) for l in self._bn_layers()]}
+        if getattr(self, "lamb", None) is not None:
+            sd["lamb"] = self.lamb.state_dict()
+        return sd
 
     def load_extra_state(self, sd):
         for l, (m, v) in zip(self._bn_layers(), sd.get("bn", [])):
             l.running_mean = m.to(self.device).clone()
             l.running_var = v.to(self.device).clone()
+        if "lamb" in sd and getattr(self, "lamb", None) is not None:
+            self.lamb.load_state_dict(sd["lamb"])
 
     def cleanup(self):
         if getattr(self.data, "para_load", False) and hasattr(self.data, "para_load_close"):

@@ -150,8 +150,9 @@ class Wide_ResNet(ModelBase):
 
     def compile_iter_fns(self, sync_type="avg", aggregate="momentum", fused_tail=None):
         """Adam is self-contained (ref ``wresnet.py:152-159``): weights are averaged across workers (``sync_type='avg'``).
-        ``optimizer='sgd'`` or ``'lars'`` trains through the flat momentum-SGD / LARS path of every other native model."""
-        if self.config.get("optimizer", "adam") in ("sgd", "lars"):
+        ``optimizer='sgd'``, ``'lars'`` or ``'lamb'`` trains through the flat momentum-SGD / LARS / LAMB path of every other native
+        model, which also gives ``sync_type='cdd'`` on the split exchange strategies."""
+        if self.config.get("optimizer", "adam") in ("sgd", "lars", "lamb"):
             return super().compile_iter_fns(sync_type, aggregate, fused_tail)
         if sync_type != "avg" and self.size > 1:
             raise ValueError("Wide_ResNet trains with Adam: only sync_type='avg' is supported (as in the reference, wresnet.py:152-153)")

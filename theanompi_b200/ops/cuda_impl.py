@@ -748,10 +748,11 @@ def _table(arena):
 
 def flat_update(arena, rule, hyper, state, step=None, g=None, lo=0, hi=None, filt=0, trust=None):
     """One step of the local flat optimizer ``rule`` (a key of ``FLAT_RULES``: sgd, adam, rmsprop, adadelta,
-    rmsprop_centered, lars) over arena elements [lo, hi) in one launch (``csrc/comm_kernels.cu: flat_update_kernel``; Adam adds
-    the launch that advances its ``step`` counter).  ``state``: the rule's flat fp32 buffers, the arena's U region first when
-    the rule uses it; ``hyper``: its float hyper-parameters (order in ``csrc/api.h``); ``filt`` (SGD, LARS): 1 only
-    non-exchanged groups, 2 only exchanged groups; ``trust`` (LARS): the per-tensor trust ratios from :func:`lars_trust`.  lr is
+    rmsprop_centered, lars, lamb) over arena elements [lo, hi) in one launch (``csrc/comm_kernels.cu: flat_update_kernel``; Adam
+    and LAMB add the launch that advances their ``step`` counter, LAMB not after a ``filt`` = 1 pass).  ``state``: the rule's flat
+    fp32 buffers, the arena's U region first when the rule uses it; ``hyper``: its float hyper-parameters (order in
+    ``csrc/api.h``); ``filt`` (SGD, LARS, LAMB): 1 only non-exchanged groups, 2 only exchanged groups; ``trust`` (LARS, LAMB): the
+    per-tensor trust ratios from :func:`lars_trust` / :func:`lamb_trust`.  lr is
     read from ``arena.hyper[0]`` on the device, so a captured CUDA graph follows lr changes, and the bf16 shadow is refreshed in
     the same pass."""
     lrm, wd, ex = _table(arena)
@@ -774,6 +775,25 @@ def lars_trust(arena, g, inv_k, eta, partial, norms, trust):
     L().lars_trust(arena.W.data_ptr(), g.data_ptr(), arena.block_tensor.data_ptr(), arena.tensor_span.data_ptr(),
                    arena.block_group.data_ptr(), lrm, wd, ex, float(inv_k), float(eta), int(arena.n_blocks), len(arena.sizes),
                    partial.data_ptr(), norms.data_ptr(), trust.data_ptr(), _st(arena.W))
+
+
+def lamb_trust(arena, g, m, v, step, b1, b2, eps, inv_k, filt, partial, norms, trust):
+    """Passes 1 and 2 of a LAMB step over the groups that ``filt`` keeps (0 all, 1 only non-exchanged, 2 only exchanged; two
+    launches, ``csrc/comm_kernels.cu: lamb_moments_kernel, lars_finalize_kernel``): advance the moments ``m`` (the arena's U) and
+    ``v`` from the gradient region ``g`` times ``inv_k``, with the bias corrections of step ``step + 1`` (``step``: the device
+    counter, not advanced here), then write ``norms`` [n_tensors, 2] ‖W‖ and ‖r‖ of the update direction r and ``trust``
+    [n_tensors] ‖W‖ / ‖r‖ for the weight group (1 elsewhere and when a norm is zero).  ``partial`` [n_blocks, 2] receives the
+    per-block sums of squares.  The ``flat_update`` pass of the ``lamb`` rule applies the step."""
+    for t, shape in ((partial, (arena.n_blocks, 2)), (norms, (len(arena.sizes), 2)), (trust, (len(arena.sizes),))):
+        assert t.dtype == torch.float32 and t.is_contiguous() and tuple(t.shape) == shape, (t.dtype, tuple(t.shape), shape)
+    for t in (m, v):
+        assert t.dtype == torch.float32 and t.is_contiguous() and t.numel() == arena.W.numel(), (t.dtype, tuple(t.shape))
+    assert step.dtype == torch.int64 and step.numel() == 1 and step.is_cuda, (step.dtype, tuple(step.shape))
+    lrm, wd, ex = _table(arena)
+    L().lamb_trust(arena.W.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), step.data_ptr(), float(b1), float(b2), float(eps),
+                   float(inv_k), int(filt), arena.block_tensor.data_ptr(), arena.tensor_span.data_ptr(), arena.block_group.data_ptr(),
+                   lrm, wd, ex, int(arena.n_blocks), len(arena.sizes), partial.data_ptr(), norms.data_ptr(), trust.data_ptr(),
+                   _st(arena.W))
 
 
 def sgd_flat(arena, g, lr, mu, nesterov, inv_k, lo, hi, only_local=False, only_exchanged=False):

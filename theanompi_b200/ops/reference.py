@@ -359,6 +359,39 @@ def lars_flat(w, g, u, offsets, sizes, groups, group_lr_mult, group_wd, lr, mu, 
     return trust, norms
 
 
+def lamb_flat(w, g, m, v, trust, norms, offsets, sizes, groups, group_lr_mult, group_wd, lr, b1=0.9, b2=0.999, eps=1e-6, t=1,
+              inv_k=1.0, update=None, w_half=None):
+    """One LAMB step (You et al., 2019) over flat fp32 buffers laid out as a :class:`FlatArena` (see :func:`lars_flat`), ``t`` = the
+    1-based step number.  Per tensor, with g = G·inv_k:
+
+        m     = b1·m + (1 − b1)·g
+        v     = b2·v + (1 − b2)·g²
+        r     = (m / (1 − b1^t)) / (sqrt(v / (1 − b2^t)) + eps) + wd·w          (decoupled weight decay)
+        trust = ‖W‖ / ‖r‖   for the weight group when ‖W‖ > 0 and ‖r‖ > 0, else 1
+        w    -= lr·lr_mult·trust·r
+
+    Norms are accumulated in fp64 over the tensor's real elements.  ``update``: per-tensor booleans, the tensors to update (all when
+    None); only their rows of ``trust`` [n] and ``norms`` [n, 2] (‖W‖, ‖r‖) are written, as on the device."""
+    from ..parallel.arena import G_W
+    b1, b2, inv_k = float(np.float32(b1)), float(np.float32(b2)), float(np.float32(inv_k))
+    c1, c2 = 1.0 / (1.0 - b1 ** t), 1.0 / (1.0 - b2 ** t)
+    for i, (o, s, grp) in enumerate(zip(offsets, sizes, groups)):
+        if update is not None and not update[i]:
+            continue
+        sl = slice(o, o + s)
+        ge = g[sl] * inv_k
+        m[sl].mul_(b1).add_(ge, alpha=1 - b1)
+        v[sl].mul_(b2).addcmul_(ge, ge, value=1 - b2)
+        r = (m[sl] * c1) / ((v[sl] * c2).sqrt() + eps) + float(group_wd[grp]) * w[sl]
+        wn, rn = float(w[sl].double().norm()), float(r.double().norm())
+        norms[i, 0], norms[i, 1] = wn, rn
+        trust[i] = wn / rn if (grp == G_W and wn > 0 and rn > 0) else 1.0
+        w[sl].sub_(lr * float(group_lr_mult[grp]) * float(trust[i]) * r)
+        if w_half is not None:
+            w_half[sl].copy_(w[sl])
+    return trust, norms
+
+
 def easgd_elastic(w, c, alpha):
     """EASGD elastic move (ref ``exchanger.py:188-211``) with both sides updated
     from the SAME difference: ``d = alpha (w - c); w -= d; c += d``."""

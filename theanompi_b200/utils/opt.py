@@ -20,6 +20,9 @@ flat arena (one launch each):
 ``BSP_LARS``   :class:`FlatLARS`, aggregate gradient (``config['optimizer'] = 'lars'``; no counterpart in the reference)
                pre : batch-norm groups             send = G
                post: LARS step from R / k
+``BSP_LAMB``   :class:`FlatLAMB`, aggregate gradient (``config['optimizer'] = 'lamb'``; no counterpart in the reference)
+               pre : batch-norm groups             send = G
+               post: LAMB step from R / k
 
 (m = per-group lr multiplier: 1 for 'W', 2 for 'b'; η only on 'W'; BN gamma/beta
 are updated locally in the pre step and never exchanged, ``opt.py:207-226``.)
@@ -307,6 +310,60 @@ class FlatLARS(FlatOptimizer):
         self.norms.copy_(norms)
 
 
+class FlatLAMB(FlatOptimizer):
+    """LAMB (You et al., 2019, "Large Batch Optimization for Deep Learning"): Adam moments (first in the arena's U region, second in
+    ``V``, step counter ``t`` in device memory) with decoupled weight decay, r = m̂ / (sqrt(v̂) + eps) + wd·W, and every weight
+    tensor's step scaled by its trust ratio ``‖W‖ / ‖r‖``; biases and batch-norm parameters keep ratio 1.  With every ratio 1 it is
+    AdamW, not :class:`FlatAdam` (which adds the decay to the gradient).
+
+    On CUDA a step is three launches plus the counter's, all reading only device memory (CUDA-graph capturable, bit-reproducible):
+    the moments and the per-block sums of squares of W and r, one per-tensor reduction that writes :attr:`norms` ([n_tensors, 2]:
+    ‖W‖, ‖r‖) and :attr:`trust` ([n_tensors]), and the ``flat_update`` pass of the LAMB rule, which recomputes r from the new
+    moments.  G is left as it was.  Like LARS, LAMB never runs in the FC weight-gradient GEMM epilogue."""
+
+    rule, buffers = "lamb", ("V",)
+
+    def __init__(self, arena, b1=0.9, b2=0.999, eps=1e-6):
+        super().__init__(arena)
+        self.b1, self.b2, self.eps = b1, b2, eps
+        n, dev = len(arena.sizes), arena.W.device
+        self.t = torch.zeros(1, dtype=torch.int64, device=dev)
+        self.trust = torch.ones(n, dtype=torch.float32, device=dev)
+        self.norms = torch.zeros(n, 2, dtype=torch.float32, device=dev)
+        self._partial = torch.zeros(arena.n_blocks, 2, dtype=torch.float32, device=dev) if arena.W.is_cuda else None
+
+    def hyper(self):
+        return (self.b1, self.b2, self.eps)
+
+    def step(self, lr=None, k=1, src="G", only_local=False, only_exchanged=False):
+        """``k``: the gradient region holds the sum of k gradients (inv_k = 1/k); ``src``: that region ("G", or "R" after the
+        exchange); ``only_local`` / ``only_exchanged``: update only the non-exchanged (batch-norm) or only the exchanged groups.
+        An ``only_local`` step does not advance :attr:`t`: the ``only_exchanged`` step of the same training step does."""
+        a = self.arena
+        g = getattr(a, src)
+        filt = 1 if only_local else (2 if only_exchanged else 0)
+        if a.W.is_cuda:
+            from ..ops import cuda_impl
+            cuda_impl.lamb_trust(a, g, a.U, self.V, self.t, *self.hyper(), 1.0 / k, filt, self._partial, self.norms, self.trust)
+            cuda_impl.flat_update(a, "lamb", self.hyper(), [a.U, self.V], step=self.t, g=g, filt=filt, trust=self.trust)
+            return
+        update = None
+        if filt:
+            update = [m != only_local for m in a.exchanged_mask()]
+        ref.lamb_flat(a.W, g, a.U, self.V, self.trust, self.norms, a.offsets, a.sizes, a.group_of, a.group_lr_mult_np,
+                      a.group_wd_np, float(a.hyper[0]) if lr is None else lr, *self.hyper(), t=int(self.t) + 1, inv_k=1.0 / k,
+                      update=update, w_half=a.H)
+        if filt != 1:
+            self.t += 1
+
+    def state_dict(self):
+        return dict(super().state_dict(), t=int(self.t))
+
+    def load_state_dict(self, sd):
+        super().load_state_dict(sd)
+        self.t.fill_(int(sd["t"]))
+
+
 # --------------------------------------------------------------------------- classic split (API parity)
 def _ex(a):
     return a.exch_vector()
@@ -412,6 +469,25 @@ def _pre_post_lars(model, k):
     return pre, post, "G"
 
 
+def _pre_post_lamb(model, k):
+    """LAMB, aggregate gradient, as :func:`_pre_post_lars`: k = 1, the whole step in ``pre``; k > 1, ``pre`` updates the batch-norm
+    groups and sends G, ``post`` updates the exchanged groups from R = Σ_ranks G and advances the step counter."""
+    lamb = model.lamb = FlatLAMB(model.arena)
+
+    def pre():
+        if k == 1:
+            lamb.step()
+            return
+        lamb.step(only_local=True)
+
+    def post():
+        if k == 1:
+            return
+        lamb.step(k=k, src="R", only_exchanged=True)
+
+    return pre, post, "G"
+
+
 def _publish(model, pre, post, send_region, k):
     a = model.arena
     mask = a.exchanged_mask()
@@ -440,6 +516,10 @@ def BSP_LARS(model, k=1):
     return _publish(model, *_pre_post_lars(model, k), k)
 
 
+def BSP_LAMB(model, k=1):
+    return _publish(model, *_pre_post_lamb(model, k), k)
+
+
 def _clip_paramlist(param_list, scale=10):
     """``T.clip(param,-10,10)`` helper (ref ``opt.py:67-75``; unused there too)."""
     with torch.no_grad():
@@ -450,10 +530,13 @@ def _clip_paramlist(param_list, scale=10):
 
 def prepare_update_dict(model, k=1, aggregate="momentum", arm=True):
     """``arm``: at k = 1, let the FC weight-gradient GEMMs apply the update of their weights (:meth:`FlatSGD.arm`); only valid
-    when the returned ``pre`` is what updates the arena after every backward.  ``model.optimizer == 'lars'``: :func:`BSP_LARS`,
-    which never arms."""
-    if getattr(model, "optimizer", "sgd") == "lars":
+    when the returned ``pre`` is what updates the arena after every backward.  ``model.optimizer == 'lars'`` / ``'lamb'``:
+    :func:`BSP_LARS` / :func:`BSP_LAMB`, which never arm."""
+    optimizer = getattr(model, "optimizer", "sgd")
+    if optimizer == "lars":
         return BSP_LARS(model, k=k)
+    if optimizer == "lamb":
+        return BSP_LAMB(model, k=k)
     if model.use_momentum:
         if aggregate == "gradient":
             return _BSP_MSGD(model, model.use_nesterov_momentum, k=k, arm=arm)
