@@ -148,7 +148,16 @@ void masked_mean_bwd(const void* dout, const void* mask, void* dh, int Tn, int B
 //   FLAT_RMSPROP_CENTERED  M (U), R, S                                         rho, mu, eps
 //   FLAT_LARS              U                                                   mu, nesterov (0 / 1), inv_k   (+ block_tensor, tensor_scale)
 //   FLAT_LAMB              M (U), V (read only: lamb_trust advanced them)      b1, b2, eps           (+ step, block_tensor, tensor_scale)
+// clip (the first five rules): the ClipRecord grad_clip_norm wrote for this step.  The step then uses s·g; when the norm is not finite
+// it changes nothing, Adam's counter included.
 enum FlatRuleId : int { FLAT_SGD = 0, FLAT_ADAM, FLAT_RMSPROP, FLAT_ADADELTA, FLAT_RMSPROP_CENTERED, FLAT_LARS, FLAT_LAMB };
+// device record of one gradient-norm clipping step (16 bytes)
+struct ClipRecord {
+  float norm;                            // ‖g‖ over the real elements, before clipping
+  float scale;                           // s = min(1, max_norm / (norm + 1e-6)); 0 when the step is skipped
+  int finite;                            // 0: the norm is NaN or Inf and the step is skipped
+  int pad;
+};
 struct FlatUpdateArgs {
   int rule;
   void* W;
@@ -165,8 +174,23 @@ struct FlatUpdateArgs {
   int filter;                            // SGD, LARS, LAMB: 0 all groups, 1 only non-exchanged groups, 2 only exchanged groups
   const void* block_tensor;              // LARS, LAMB: tensor index of every arena block (int32), else null
   const void* tensor_scale;              // LARS, LAMB: trust ratio of every tensor (fp32, from lars_trust / lamb_trust), else null
+  const void* clip;                      // gradient-norm clipping: the step's ClipRecord, else null
 };
 void flat_update(const FlatUpdateArgs& a, cudaStream_t st);
+// Global gradient-norm clipping over the whole arena, two launches: per-block Σg² over the real elements of G into partial ([n_blocks]
+// fp32), then one CTA sums them in fp64 in a fixed order and writes *rec; when the norm is not finite it adds 1 to *skipped (uint64).
+// G is not changed: the clip pointer of the flat_update pass that follows applies s.
+struct GradClipArgs {
+  const void* G;
+  const void* block_tensor;
+  const void* tensor_span;
+  long long n_blocks;
+  float max_norm;
+  void* partial;
+  void* rec;
+  void* skipped;
+};
+void grad_clip_norm(const GradClipArgs& a, cudaStream_t st);
 // LARS trust ratios over the whole arena, two launches: per-block sums of squares of W and G into partial ([n_blocks, 2] fp32),
 // then one CTA per tensor: norms[t] = {‖W‖, ‖G‖·inv_k} ([n_tensors, 2] fp32) and trust[t] = eta·‖W‖ / (‖g‖ + wd·‖W‖) for the
 // weight group (group 0) when both norms are positive, else 1.  tensor_span: [n_tensors, 2] int64 {element offset, size}.

@@ -155,9 +155,12 @@ PYBIND11_MODULE(_tmpi_native, m) {
                                    py::arg("lars") = (int)FLAT_LARS, py::arg("lamb") = (int)FLAT_LAMB);
   m.def("flat_update", [](int rule, ptr_t W, ptr_t G, ptr_t S0, ptr_t S1, ptr_t S2, ptr_t H, ptr_t block_group, std::vector<float> lr_mult,
                           std::vector<float> wd, std::vector<int> exch, ptr_t lr_ptr, ptr_t step, std::vector<float> hp, long long lo,
-                          long long hi, int filter, ptr_t block_tensor, ptr_t tensor_scale, ptr_t st) {
+                          long long hi, int filter, ptr_t block_tensor, ptr_t tensor_scale, ptr_t clip, ptr_t st) {
     flat_update(FlatUpdateArgs{rule, P(W), P(G), {P(S0), P(S1), P(S2)}, P(H), P(block_group), make_table(lr_mult, wd, exch), P(lr_ptr),
-                               P(step), hp.data(), (int)hp.size(), lo, hi, filter, P(block_tensor), P(tensor_scale)}, S(st)); });
+                               P(step), hp.data(), (int)hp.size(), lo, hi, filter, P(block_tensor), P(tensor_scale), P(clip)}, S(st)); });
+  m.def("grad_clip_norm", [](ptr_t G, ptr_t block_tensor, ptr_t tensor_span, long long n_blocks, float max_norm, ptr_t partial, ptr_t rec,
+                             ptr_t skipped, ptr_t st) {
+    grad_clip_norm(GradClipArgs{P(G), P(block_tensor), P(tensor_span), n_blocks, max_norm, P(partial), P(rec), P(skipped)}, S(st)); });
   m.def("lars_trust", [](ptr_t W, ptr_t G, ptr_t block_tensor, ptr_t tensor_span, ptr_t block_group, std::vector<float> lr_mult,
                          std::vector<float> wd, std::vector<int> exch, float inv_k, float eta, long long n_blocks, int n_tensors,
                          ptr_t partial, ptr_t norms, ptr_t trust, ptr_t st) {

@@ -18,6 +18,7 @@
 //   easgd_elastic       d = α(w − c); w −= d; c += d   on the center's memory over NVLink   (exchanger.py:188-211)
 //   gosgd_*             push / merge / pull-merge of weights with push-sum weights α     (exchanger.py:450-462)
 //   K1..K5 of the reference (float2half/half2float, sumfloats/sumhalfs, vecadd/vecaddhalf) for the legacy strategies.
+#include <type_traits>
 #include "common.cuh"
 #include "api.h"
 
@@ -101,13 +102,17 @@ __device__ __forceinline__ void block_barrier(const CommCtx& c) {
 // update; `prologue` computes per-launch constants, `skip` drops whole blocks by group, `enter_block` loads per-block constants
 // through the block → tensor table (LARS, LAMB: the tensor's trust ratio).  A rule that takes its direction from state written by
 // an earlier pass (LAMB) neither reads G (kReadsG) nor stores its state back (kWritesState).
+// Global gradient-norm clipping (the kClip instantiations, grad_clip_norm below) makes the step use s·g: the kernel multiplies every
+// loaded gradient by s, or, for a rule that already scales the gradient by a launch constant (kFoldsClip), folds s into it.
 struct FlatRule {
   static constexpr bool kAdvancesStep = false;
   static constexpr bool kReadsG = true;
   static constexpr bool kWritesState = true;
+  static constexpr bool kFoldsClip = false;
   __device__ __forceinline__ void prologue(const unsigned long long* step) {}
   __device__ __forceinline__ bool skip(const GroupTable& tab, int g) const { return false; }
   __device__ __forceinline__ void enter_block(long long b, const int* block_tensor, const float* tensor_scale) {}
+  __device__ __forceinline__ void fold_clip(float s) {}
 };
 
 // filter: 0 all groups, 1 only non-exchanged (BN) groups, 2 only exchanged groups
@@ -118,10 +123,12 @@ __device__ __forceinline__ bool filtered_out(const GroupTable& tab, int g, int f
 // momentum SGD, `common.cuh: sgd4` (the arithmetic of the GEMM SGD epilogue and the fused collectives).  State: U.  filter as above.
 struct SgdRule : FlatRule {
   static constexpr int kState = 1;
+  static constexpr bool kFoldsClip = true;                 // g·inv_k·s
   float mu, inv_k;
   int nesterov, filter;
   __device__ __forceinline__ SgdRule(float a, float b, float, int i, int j) : mu(a), inv_k(b), nesterov(i), filter(j) {}
   __device__ __forceinline__ bool skip(const GroupTable& tab, int g) const { return filtered_out(tab, g, filter); }
+  __device__ __forceinline__ void fold_clip(float s) { inv_k = __fmul_rn(inv_k, s); }
   __device__ __forceinline__ void apply(float4& w, float4* s, const float4& gg, float lr0, float lrm, float wd) const {
     sgd4(w, s[0], gg, Hyper{lr0, mu, inv_k, nesterov}, lrm, wd);
   }
@@ -154,6 +161,10 @@ struct AdamRule : FlatRule {
   }
 };
 __global__ void adam_advance_kernel(unsigned long long* step) { if (threadIdx.x == 0 && blockIdx.x == 0) *step += 1ull; }
+// the same after a clipped step: a skipped step (non-finite gradient norm) does not advance the counter
+__global__ void adam_advance_clip_kernel(unsigned long long* step, const ClipRecord* __restrict__ clip) {
+  if (threadIdx.x == 0 && blockIdx.x == 0 && clip->finite) *step += 1ull;
+}
 
 // RMSProp (the GANs' optimizer, torch.optim.RMSprop without momentum).  State: V.
 // v = alpha v + (1 - alpha) g^2;  w -= lr * g / (sqrt(v) + eps);  then, when clip > 0, w = clamp(w, -clip, clip) (the WGAN critic's
@@ -276,15 +287,25 @@ struct LambRule : FlatRule {
   }
 };
 
-template <class Rule>
+// kClip: `clip` is the record grad_clip_norm wrote for this step.  A step whose gradient norm is not finite returns before it touches
+// memory; otherwise the gradient is scaled by clip->scale.  __fmul_rn is never contracted into an FMA, so with s = 1 every later
+// operation sees the same operands as without clipping and the step is bit-identical to the kClip = false instantiation.
+template <class Rule, bool kClip = false>
 __global__ void __launch_bounds__(kThreads) flat_update_kernel(float* __restrict__ W, const float* __restrict__ G, float* __restrict__ S0,
                                                                float* __restrict__ S1, float* __restrict__ S2, __nv_bfloat16* __restrict__ H,
                                                                const uint8_t* __restrict__ block_group, GroupTable tab,
                                                                const float* __restrict__ lr_ptr, const unsigned long long* __restrict__ step,
                                                                float ha, float hb, float hc, int ia, int ib, long long blk_lo,
                                                                long long blk_hi, const int* __restrict__ block_tensor,
-                                                               const float* __restrict__ tensor_scale) {
+                                                               const float* __restrict__ tensor_scale, const ClipRecord* __restrict__ clip) {
   Rule r(ha, hb, hc, ia, ib);
+  float cs = 1.f;
+  if constexpr (kClip) {
+    const ClipRecord rec = *clip;
+    if (!rec.finite) return;                              // skipped step: W, H and the state stay as they are
+    cs = rec.scale;
+    if constexpr (Rule::kFoldsClip) r.fold_clip(cs);
+  }
   r.prologue(step);
   const float lr0 = *lr_ptr;
   for (long long b = blk_lo + blockIdx.x; b < blk_hi; b += gridDim.x) {
@@ -298,6 +319,9 @@ __global__ void __launch_bounds__(kThreads) flat_update_kernel(float* __restrict
     if constexpr (Rule::kState > 2) s[2] = *reinterpret_cast<const float4*>(S2 + i);
     float4 gg = {};
     if constexpr (Rule::kReadsG) gg = *reinterpret_cast<const float4*>(G + i);
+    if constexpr (kClip && !Rule::kFoldsClip) {
+      gg.x = __fmul_rn(gg.x, cs); gg.y = __fmul_rn(gg.y, cs); gg.z = __fmul_rn(gg.z, cs); gg.w = __fmul_rn(gg.w, cs);
+    }
     r.apply(w, s, gg, lr0, tab.lr_mult[g], tab.wd[g]);
     *reinterpret_cast<float4*>(W + i) = w;
     if constexpr (Rule::kWritesState) {
@@ -310,20 +334,29 @@ __global__ void __launch_bounds__(kThreads) flat_update_kernel(float* __restrict
 }
 
 // ha, hb, hc, ia, ib: the rule's hyperparameters, in the order of its constructor
-template <class Rule>
+template <class Rule, bool kClip = false>
 static void launch_flat_update(const char* name, const FlatUpdateArgs& a, float ha, float hb, float hc, int ia, int ib, cudaStream_t st) {
   if (a.lo % kArenaBlock || a.hi % kArenaBlock) throw std::runtime_error(std::string(name) + ": range must be block aligned");
   const long long nb = (a.hi - a.lo) / kArenaBlock;
   if (nb <= 0) return;
   int grid = (int)std::min<long long>(nb, (long long)sm_count() * 8);
-  flat_update_kernel<Rule><<<grid, kThreads, 0, st>>>((float*)a.W, (const float*)a.G, (float*)a.S[0], (float*)a.S[1], (float*)a.S[2],
-                                                      (__nv_bfloat16*)a.H, (const uint8_t*)a.block_group, a.tab, (const float*)a.lr_ptr,
-                                                      (const unsigned long long*)a.step, ha, hb, hc, ia, ib, a.lo / kArenaBlock,
-                                                      a.hi / kArenaBlock, (const int*)a.block_tensor, (const float*)a.tensor_scale);
+  flat_update_kernel<Rule, kClip><<<grid, kThreads, 0, st>>>((float*)a.W, (const float*)a.G, (float*)a.S[0], (float*)a.S[1],
+                                                             (float*)a.S[2], (__nv_bfloat16*)a.H, (const uint8_t*)a.block_group, a.tab,
+                                                             (const float*)a.lr_ptr, (const unsigned long long*)a.step, ha, hb, hc, ia, ib,
+                                                             a.lo / kArenaBlock, a.hi / kArenaBlock, (const int*)a.block_tensor,
+                                                             (const float*)a.tensor_scale, (const ClipRecord*)a.clip);
   // a filter-1 (batch-norm only) pass is followed by the filter-2 pass of the same step, which advances the counter
   const bool advance = Rule::kAdvancesStep && a.filter != 1;
-  if (advance) adam_advance_kernel<<<1, 32, 0, st>>>((unsigned long long*)a.step);
+  if (advance && kClip) adam_advance_clip_kernel<<<1, 32, 0, st>>>((unsigned long long*)a.step, (const ClipRecord*)a.clip);
+  else if (advance) adam_advance_kernel<<<1, 32, 0, st>>>((unsigned long long*)a.step);
   count_launch(advance ? 2 : 1); TMPI_CHECK_LAUNCH(name); ::tmpi::check_capture(st, name);
+}
+
+template <class Rule>
+static void launch_flat_update_clip(const char* name, const FlatUpdateArgs& a, float ha, float hb, float hc, int ia, int ib,
+                                    cudaStream_t st) {
+  if (a.clip) launch_flat_update<Rule, true>(name, a, ha, hb, hc, ia, ib, st);
+  else launch_flat_update<Rule, false>(name, a, ha, hb, hc, ia, ib, st);
 }
 
 void flat_update(const FlatUpdateArgs& a, cudaStream_t st) {
@@ -338,13 +371,15 @@ void flat_update(const FlatUpdateArgs& a, cudaStream_t st) {
   if (a.rule == FLAT_LARS && (!a.block_tensor || !a.tensor_scale)) throw std::runtime_error("lars_flat: needs the block → tensor table and the trust ratios");
   if (a.rule == FLAT_LAMB && !a.step) throw std::runtime_error("lamb_flat: needs a step counter");
   if (a.rule == FLAT_LAMB && (!a.block_tensor || !a.tensor_scale)) throw std::runtime_error("lamb_flat: needs the block → tensor table and the trust ratios");
+  if (a.clip && (a.rule == FLAT_LARS || a.rule == FLAT_LAMB))
+    throw std::runtime_error(std::string(name) + ": gradient-norm clipping is for the sgd, adam, rmsprop, adadelta and rmsprop_centered rules");
   const float* h = a.hp;
   switch (a.rule) {
-    case FLAT_SGD: launch_flat_update<SgdRule>(name, a, h[0], h[2], 0.f, h[1] != 0.f, a.filter, st); break;
-    case FLAT_ADAM: launch_flat_update<AdamRule>(name, a, h[0], h[1], h[2], 0, 0, st); break;
-    case FLAT_RMSPROP: launch_flat_update<RmspropRule>(name, a, h[0], h[1], h[2], 0, 0, st); break;
-    case FLAT_ADADELTA: launch_flat_update<AdadeltaRule>(name, a, h[0], h[1], 0.f, 0, 0, st); break;
-    case FLAT_RMSPROP_CENTERED: launch_flat_update<CenteredRmspropRule>(name, a, h[0], h[1], h[2], 0, 0, st); break;
+    case FLAT_SGD: launch_flat_update_clip<SgdRule>(name, a, h[0], h[2], 0.f, h[1] != 0.f, a.filter, st); break;
+    case FLAT_ADAM: launch_flat_update_clip<AdamRule>(name, a, h[0], h[1], h[2], 0, 0, st); break;
+    case FLAT_RMSPROP: launch_flat_update_clip<RmspropRule>(name, a, h[0], h[1], h[2], 0, 0, st); break;
+    case FLAT_ADADELTA: launch_flat_update_clip<AdadeltaRule>(name, a, h[0], h[1], 0.f, 0, 0, st); break;
+    case FLAT_RMSPROP_CENTERED: launch_flat_update_clip<CenteredRmspropRule>(name, a, h[0], h[1], h[2], 0, 0, st); break;
     case FLAT_LARS: launch_flat_update<LarsRule>(name, a, h[0], h[2], 0.f, h[1] != 0.f, a.filter, st); break;
     default: launch_flat_update<LambRule>(name, a, h[0], h[1], h[2], a.filter, 0, st); break;
   }
@@ -354,16 +389,21 @@ void flat_update(const FlatUpdateArgs& a, cudaStream_t st) {
 // Pass 1: for every arena block of [blk_lo, blk_hi), the sums of squares of W and of the gradient over the block's real elements
 // (those below the end of its tensor) → partial[b] = {Σw², Σg²}.  One block per CTA iteration, one float4 per thread, warp shuffles
 // and a fixed-order sum over the 8 warps: no atomics, so the result does not depend on the grid.
+// kW = false (gradient clipping): W is not read and partial[b] = Σg² alone, so the pass moves 4 B per element.
+template <bool kW>
 __global__ void __launch_bounds__(kThreads) lars_partial_kernel(const float* __restrict__ W, const float* __restrict__ G,
                                                                 const int* __restrict__ block_tensor, const long long* __restrict__ tensor_span,
-                                                                float2* __restrict__ partial, long long blk_lo, long long blk_hi) {
+                                                                std::conditional_t<kW, float2, float>* __restrict__ partial,
+                                                                long long blk_lo, long long blk_hi) {
   __shared__ float2 red[kThreads / 32];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (long long b = blk_lo + blockIdx.x; b < blk_hi; b += gridDim.x) {
     const long long i = b * kArenaBlock + threadIdx.x * 4;
     const int t = block_tensor[b];
     const long long end = tensor_span[2 * t] + tensor_span[2 * t + 1];
-    float4 w = *reinterpret_cast<const float4*>(W + i), g = *reinterpret_cast<const float4*>(G + i);
+    float4 w = {}, g;
+    if constexpr (kW) w = *reinterpret_cast<const float4*>(W + i);
+    g = *reinterpret_cast<const float4*>(G + i);
     if (i + 4 > end) {                                   // the tensor's last block: zero the padding past its end
       if (i + 0 >= end) { w.x = 0.f; g.x = 0.f; }
       if (i + 1 >= end) { w.y = 0.f; g.y = 0.f; }
@@ -372,14 +412,16 @@ __global__ void __launch_bounds__(kThreads) lars_partial_kernel(const float* __r
     }
     float sw = w.x * w.x + w.y * w.y + w.z * w.z + w.w * w.w;
     float sg = g.x * g.x + g.y * g.y + g.z * g.z + g.w * g.w;
-    sw = warp_sum(sw); sg = warp_sum(sg);
+    if constexpr (kW) sw = warp_sum(sw);
+    sg = warp_sum(sg);
     if (lane == 0) red[warp] = make_float2(sw, sg);
     __syncthreads();
     if (threadIdx.x == 0) {
       float2 s = red[0];
 #pragma unroll
       for (int k = 1; k < kThreads / 32; ++k) { s.x += red[k].x; s.y += red[k].y; }
-      partial[b] = s;
+      if constexpr (kW) partial[b] = s;
+      else partial[b] = s.y;
     }
     __syncthreads();                                     // red[] is reused by the next block
   }
@@ -418,8 +460,8 @@ __global__ void __launch_bounds__(kThreads) lars_finalize_kernel(const float2* _
 void lars_trust(const LarsTrustArgs& a, cudaStream_t st) {
   if (a.n_blocks <= 0 || a.n_tensors <= 0) return;
   const int grid = (int)std::min<long long>(a.n_blocks, (long long)sm_count() * 8);
-  lars_partial_kernel<<<grid, kThreads, 0, st>>>((const float*)a.W, (const float*)a.G, (const int*)a.block_tensor,
-                                                 (const long long*)a.tensor_span, (float2*)a.partial, 0, a.n_blocks);
+  lars_partial_kernel<true><<<grid, kThreads, 0, st>>>((const float*)a.W, (const float*)a.G, (const int*)a.block_tensor,
+                                                       (const long long*)a.tensor_span, (float2*)a.partial, 0, a.n_blocks);
   TMPI_CHECK_LAUNCH("lars_partial");
   lars_finalize_kernel<<<a.n_tensors, kThreads, 0, st>>>((const float2*)a.partial, (const long long*)a.tensor_span,
                                                          (const uint8_t*)a.block_group, a.tab, a.inv_k, a.eta, (float2*)a.norms,
@@ -501,6 +543,47 @@ void lamb_trust(const LambTrustArgs& a, cudaStream_t st) {
                                                          (const uint8_t*)a.block_group, no_wd, 1.f, 1.f, (float2*)a.norms,
                                                          (float*)a.trust);
   count_launch(2); TMPI_CHECK_LAUNCH("lars_finalize"); ::tmpi::check_capture(st, "lamb_trust");
+}
+
+// ============================================================================ global gradient-norm clipping
+// Pass 1 is lars_partial_kernel<false>: partial[b] = Σg² over the real elements of block b.  Pass 2: one CTA sums the n_blocks partials
+// in fp64 (every thread a fixed stride of them, then the warps in a fixed order: no atomics, the same result on every run) and writes
+// the record the kClip flat_update pass reads.  torch.nn.utils.clip_grad_norm_ semantics: s = min(1, max_norm / (n + 1e-6)).
+__global__ void __launch_bounds__(kThreads) clip_finalize_kernel(const float* __restrict__ partial, long long n_blocks, float max_norm,
+                                                                 ClipRecord* __restrict__ rec, unsigned long long* __restrict__ skipped) {
+  __shared__ double red[kThreads / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  double s = 0.0;
+  for (long long k = threadIdx.x; k < n_blocks; k += kThreads) s += (double)partial[k];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) red[warp] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    s = red[0];
+    for (int k = 1; k < kThreads / 32; ++k) s += red[k];
+    const double n = sqrt(s);
+    const bool finite = isfinite(n);
+    ClipRecord r;
+    r.norm = (float)n;
+    r.scale = finite ? (float)fmin(1.0, (double)max_norm / (n + 1e-6)) : 0.f;
+    r.finite = finite ? 1 : 0;
+    r.pad = 0;
+    *rec = r;
+    if (!finite) *skipped += 1ull;
+  }
+}
+
+void grad_clip_norm(const GradClipArgs& a, cudaStream_t st) {
+  if (a.n_blocks <= 0) throw std::runtime_error("grad_clip_norm: empty arena");
+  if (!(a.max_norm > 0.f)) throw std::runtime_error("grad_clip_norm: max_norm must be positive");
+  const int grid = (int)std::min<long long>(a.n_blocks, (long long)sm_count() * 8);
+  lars_partial_kernel<false><<<grid, kThreads, 0, st>>>(nullptr, (const float*)a.G, (const int*)a.block_tensor,
+                                                        (const long long*)a.tensor_span, (float*)a.partial, 0, a.n_blocks);
+  TMPI_CHECK_LAUNCH("clip_partial");
+  clip_finalize_kernel<<<1, kThreads, 0, st>>>((const float*)a.partial, a.n_blocks, a.max_norm, (ClipRecord*)a.rec,
+                                               (unsigned long long*)a.skipped);
+  count_launch(2); TMPI_CHECK_LAUNCH("clip_finalize"); ::tmpi::check_capture(st, "grad_clip_norm");
 }
 
 // ============================================================================ fused collectives

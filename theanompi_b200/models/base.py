@@ -94,6 +94,11 @@ class ModelBase(object):
         # or 'lamb' (Adam moments with per-tensor trust ratios, utils/opt.py: FlatLAMB)
         self.optimizer = config.get("optimizer", "sgd")
         self.lars_eta = float(config.get("lars_eta", 0.001))
+        # global gradient-norm clipping of every step (torch.nn.utils.clip_grad_norm_; utils/opt.py: FlatOptimizer.set_grad_clip):
+        # the maximum L2 norm of the whole gradient, None (default) = off
+        gc = config.get("grad_clip")
+        self.grad_clip = None if gc is None else float(gc)
+        self.clip_opt = None
         self.base_lr = np.float32(self.learning_rate)
         self.current_t = self.subb_t = 0
         self.current_v = self.subb_v = 0
@@ -344,7 +349,10 @@ class ModelBase(object):
 
         ``optimizer='lars'`` and ``'lamb'`` need each tensor's whole reduced gradient before they update any of its elements, so
         they run on the split strategies (``ar``, ``nccl32``, ``nccl16``, ``asa32``, ``p2p32``, …) and not on a fused exchange
-        (``fused_tail``)."""
+        (``fused_tail``).
+
+        ``grad_clip`` needs the global norm of the whole gradient before any element is updated: it runs on local k = 1 steps only
+        (see :meth:`check_grad_clip`)."""
         if self.optimizer not in ("sgd", "lars", "lamb"):
             raise ValueError("%s: optimizer must be 'lamb', 'sgd' or 'lars', not %r" % (self.name, self.optimizer))
         k = self.size if sync_type == "cdd" else 1
@@ -352,6 +360,7 @@ class ModelBase(object):
             raise ValueError("optimizer=%r needs every tensor's whole reduced gradient before its update; the fused exchange "
                              "strategies (fused*, oneshot*, twoshot*, nvls*, fused_rs) update bucket slices as they are reduced. "
                              "Use a split strategy: ar, nccl32, nccl16, asa32, asa16 or p2p32" % self.optimizer)
+        self.check_grad_clip(k, fused_tail)
         start = time.time()
         self.sync_type = sync_type
         if k > 1 and fused_tail is None:
@@ -359,6 +368,26 @@ class ModelBase(object):
         pre_model_iter_fn(self, k, aggregate=aggregate, fused_tail=fused_tail)
         if self.verbose:
             print("Compile time: %.3f s" % (time.time() - start))
+
+    def check_grad_clip(self, k=1, fused_tail=None, optimizer=None):
+        """Refuse ``grad_clip`` where the native step cannot clip by the global norm: with ``optimizer`` (default: the model's)
+        'lars' or 'lamb', whose trust ratios already normalise every tensor's step, and on any step that is not a local k = 1
+        update (BSP ``sync_type='cdd'`` with more than one worker, a fused exchange strategy's ``fused_tail``), which would need
+        the norm of the reduced gradient before any slice is updated."""
+        if self.grad_clip is None:
+            return
+        supported = ("grad_clip runs on the local k = 1 steps of the sgd, adam, rmsprop, adadelta and rmsprop_centered flat "
+                     "optimizers: one worker, BSP sync_type='avg' with a split strategy, EASGD, ASGD or GOSGD")
+        if not self.grad_clip > 0:
+            raise ValueError("%s: grad_clip must be a positive maximum norm or None, not %r" % (self.name, self.grad_clip))
+        opt = self.optimizer if optimizer is None else optimizer
+        if opt in ("lars", "lamb"):
+            raise ValueError("%s: grad_clip does not combine with optimizer=%r, whose trust ratios already normalise every "
+                             "tensor's step; %s" % (self.name, opt, supported))
+        if fused_tail is not None or k > 1:
+            raise ValueError("%s: grad_clip needs the global norm of the reduced gradient before any update, which %s does not "
+                             "have; %s" % (self.name, "a fused exchange strategy" if fused_tail is not None
+                                           else "sync_type='cdd' with %d workers" % k, supported))
 
     # ------------------------------------------------------------------ data movement
     def _labels_to_device(self, labels):
@@ -487,6 +516,8 @@ class ModelBase(object):
         sd = {"bn": [(l.running_mean.detach().cpu(), l.running_var.detach().cpu()) for l in self._bn_layers()]}
         if getattr(self, "lamb", None) is not None:
             sd["lamb"] = self.lamb.state_dict()
+        if self.clip_opt is not None:                   # the SGD step's skip counter (gradient clipping)
+            sd["grad_clip"] = self.clip_opt.state_dict()
         return sd
 
     def load_extra_state(self, sd):
@@ -495,6 +526,8 @@ class ModelBase(object):
             l.running_var = v.to(self.device).clone()
         if "lamb" in sd and getattr(self, "lamb", None) is not None:
             self.lamb.load_state_dict(sd["lamb"])
+        if "grad_clip" in sd and self.clip_opt is not None:
+            self.clip_opt.load_state_dict(sd["grad_clip"])
 
     def cleanup(self):
         if getattr(self.data, "para_load", False) and hasattr(self.data, "para_load_close"):

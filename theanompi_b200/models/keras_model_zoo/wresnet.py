@@ -156,9 +156,12 @@ class Wide_ResNet(ModelBase):
             return super().compile_iter_fns(sync_type, aggregate, fused_tail)
         if sync_type != "avg" and self.size > 1:
             raise ValueError("Wide_ResNet trains with Adam: only sync_type='avg' is supported (as in the reference, wresnet.py:152-153)")
+        self.check_grad_clip(optimizer="adam")
         from ...utils.opt import FlatAdam
         self.sync_type = "avg"
         self.adam = FlatAdam(self.arena)
+        if self.grad_clip is not None:
+            self.adam.set_grad_clip(self.grad_clip)           # its skip counter is saved with the Adam state
         self.set_step_tail(lambda: self.adam.step())
         self.get_vel = lambda subb=0: self.forward_backward(subb)
         self.descent_vel = lambda: None

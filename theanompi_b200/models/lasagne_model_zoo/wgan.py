@@ -96,6 +96,7 @@ class WGAN(TorchModelBase):
         return 0.5 * ((self.critic(fake) - 1) ** 2).mean()
 
     def compile_iter_fns(self, sync_type="avg", **kw):
+        self.refuse_grad_clip()
         self.sync_type = "avg"
         self.opt_c = torch.optim.RMSprop(self.critic_params, lr=self.learning_rate)
         self.opt_g = torch.optim.RMSprop(self.generator_params, lr=self.learning_rate)
@@ -223,7 +224,14 @@ class NativeWGAN(ModelBase):
     the generator has its own local arena.  Both train with :class:`FlatRMSProp` (the critic's ±0.01 clip in the same pass).
     On the GPU the critic step and the generator step are two captured CUDA graphs; ``train_iter`` copies each real batch into
     a static buffer and replays the critic graph ``critic_runs`` times, then the generator graph.  Noise is Philox keyed by a
-    device step counter the graphs advance."""
+    device step counter the graphs advance.
+
+    ``grad_clip=5`` gives the reference MNIST GANs' gradient rescaling, g·5 / max(5, ‖g‖) (``wgan.py:18-59``, ``lsgan.py:14-55``),
+    with the critic's and the generator's gradients clipped separately, each by the norm of its own arena.  It differs from the
+    reference in two ways.  The reference takes the square root twice (``wgan.py:29-31``), so its threshold is effectively on
+    ‖g‖^½; here it is on the true norm.  On a non-finite norm the reference substitutes g = 0.1·W; here the step is skipped and
+    ``opt_c.skipped`` / ``opt_g.skipped`` count it.  The reference's CIFAR-10 LSGAN uses plain RMSProp without rescaling, so there
+    ``grad_clip`` is simply available."""
     loss_kind = "wgan"
     n_epochs = num_epochs
     batch_size = file_batch_size = batchsize
@@ -282,6 +290,9 @@ class NativeWGAN(ModelBase):
         self.gen_arena.hyper[0] = float(self.base_lr)
         self.opt_c = FlatRMSProp(self.arena, clip=clip if self.loss_kind == "wgan" else 0.0)
         self.opt_g = FlatRMSProp(self.gen_arena)
+        if self.grad_clip is not None:                   # each arena by its own gradient norm, as the reference's MNIST GANs
+            self.opt_c.set_grad_clip(self.grad_clip)
+            self.opt_g.set_grad_clip(self.grad_clip)
         dev = self.device
         self.bn_stats = {k: (torch.zeros(n, device=dev), torch.ones(n, device=dev))
                          for k, n in (("g1", 1024), ("g2", s4 * s4 * 128), ("g3", 64), ("c2", 128), ("c3", 1024))}

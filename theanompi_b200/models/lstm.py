@@ -104,7 +104,8 @@ def pad_batch(x, m, T):
 class LSTM(ModelBase):
     """``config['optimizer']``: ``'adadelta'`` (default, lr 1.0), ``'rmsprop'`` (the reference's centred RMSProp with momentum,
     lr 1e-4) or ``'sgd'`` (``p - lr·g``, lr 1e-4), the three optimizers of the reference's ``train_lstm``; ``learning_rate``
-    overrides the lr.  Each is one flat native launch over the arena.  On the GPU every training step is one CUDA graph per
+    overrides the lr.  Each is one flat native launch over the arena; ``grad_clip`` (a maximum global gradient norm, the usual
+    control for recurrent nets) adds the two norm launches before it.  On the GPU every training step is one CUDA graph per
     sequence-length bucket (:func:`bucket_len`): the batch is padded to its bucket, copied into the bucket's static buffers and
     the bucket's graph (forward, backward, update) is replayed.  ``cuda_graph=False`` and the CPU run the step eagerly on the
     unpadded batch; validation is always eager."""
@@ -176,9 +177,12 @@ class LSTM(ModelBase):
                 self.opt = FlatCenteredRMSProp(self.arena)             # ref :376-402
             else:
                 self.opt = FlatSGD(self.arena, mu=0.0, use_momentum=False)       # ref :256-281: p - lr·g
+            if self.grad_clip is not None:
+                self.opt.set_grad_clip(self.grad_clip)                 # inside each bucket's captured step
         return self.opt
 
     def compile_iter_fns(self, sync_type="avg", **kw):
+        self.check_grad_clip()
         self.sync_type = "avg"
         self._make_opt()
         self.vels, self.vels2 = [], []
@@ -313,6 +317,7 @@ class LSTMTorch(TorchModelBase):
         return torch.optim.Adadelta(params, lr=1.0, rho=0.95, eps=1e-6)
 
     def compile_iter_fns(self, sync_type="avg", **kw):
+        self.refuse_grad_clip()
         self.sync_type = "avg"
         self.torch_opt = self.make_torch_optimizer(self.params)
         self.vels, self.vels2 = [], []

@@ -99,7 +99,15 @@ class TorchModelBase(ModelBase):
             return c, e, e5
         self.val_fn = val_fn
 
+    def refuse_grad_clip(self):
+        """The torch twins step through ``torch.optim`` or their own flat SGD without a clipping pass: refuse ``grad_clip`` rather than
+        train unclipped."""
+        if self.grad_clip is not None:
+            raise ValueError("%s: grad_clip is not supported by the torch twins; it runs on the native models (AlexNet, GoogLeNet, "
+                             "Cifar10_model, VGG16, ResNet50, Wide_ResNet, LSTM, NativeWGAN, NativeLSGAN)" % self.name)
+
     def compile_iter_fns(self, sync_type="avg", aggregate="momentum", fused_tail=None):
+        self.refuse_grad_clip()
         self.torch_opt = self.make_torch_optimizer(self.params)
         if self.torch_opt is None:
             return super().compile_iter_fns(sync_type, aggregate, fused_tail)

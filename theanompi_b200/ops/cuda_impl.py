@@ -746,22 +746,37 @@ def _table(arena):
     return arena._tab_cache
 
 
-def flat_update(arena, rule, hyper, state, step=None, g=None, lo=0, hi=None, filt=0, trust=None):
+def flat_update(arena, rule, hyper, state, step=None, g=None, lo=0, hi=None, filt=0, trust=None, clip=None):
     """One step of the local flat optimizer ``rule`` (a key of ``FLAT_RULES``: sgd, adam, rmsprop, adadelta,
     rmsprop_centered, lars, lamb) over arena elements [lo, hi) in one launch (``csrc/comm_kernels.cu: flat_update_kernel``; Adam
     and LAMB add the launch that advances their ``step`` counter, LAMB not after a ``filt`` = 1 pass).  ``state``: the rule's flat
     fp32 buffers, the arena's U region first when the rule uses it; ``hyper``: its float hyper-parameters (order in
     ``csrc/api.h``); ``filt`` (SGD, LARS, LAMB): 1 only non-exchanged groups, 2 only exchanged groups; ``trust`` (LARS, LAMB): the
-    per-tensor trust ratios from :func:`lars_trust` / :func:`lamb_trust`.  lr is
-    read from ``arena.hyper[0]`` on the device, so a captured CUDA graph follows lr changes, and the bf16 shadow is refreshed in
-    the same pass."""
+    per-tensor trust ratios from :func:`lars_trust` / :func:`lamb_trust`; ``clip`` (the first five rules): the record
+    :func:`grad_clip_norm` wrote for this step, so the step uses s·g, or changes nothing (Adam's counter included) when the
+    gradient norm is not finite.  lr is read from ``arena.hyper[0]`` on the device, so a captured CUDA graph follows lr changes,
+    and the bf16 shadow is refreshed in the same pass."""
     lrm, wd, ex = _table(arena)
     S = [t.data_ptr() for t in state] + [0] * (3 - len(state))
     lib = L()
     lib.flat_update(lib.FLAT_RULES[rule], arena.W.data_ptr(), (arena.G if g is None else g).data_ptr(), *S, _p(arena.H),
                     arena.block_group.data_ptr(), lrm, wd, ex, arena.hyper.data_ptr(), _p(step), [float(v) for v in hyper],
                     int(lo), int(arena.numel if hi is None else hi), int(filt),
-                    0 if trust is None else arena.block_tensor.data_ptr(), _p(trust), _st(arena.W))
+                    0 if trust is None else arena.block_tensor.data_ptr(), _p(trust), _p(clip), _st(arena.W))
+
+
+def grad_clip_norm(arena, g, max_norm, partial, rec, skipped):
+    """The global L2 norm n of the gradient region ``g`` over the real elements of every arena tensor, for gradient clipping
+    (two launches, ``csrc/comm_kernels.cu: lars_partial_kernel<false>, clip_finalize_kernel``): ``partial`` [n_blocks] receives
+    the per-block sums of squares, ``rec`` (4 x fp32, ``csrc/api.h: ClipRecord``) n, s = min(1, max_norm / (n + 1e-6)) and the
+    int32 flag "n is finite"; ``skipped`` (int64 [1]) is incremented when it is not.  ``g`` is not changed.  Every input is read
+    from device memory, so the launches can be captured in a CUDA graph."""
+    assert partial.dtype == torch.float32 and partial.is_contiguous() and tuple(partial.shape) == (arena.n_blocks,), tuple(partial.shape)
+    assert rec.dtype == torch.float32 and rec.is_contiguous() and rec.numel() == 4, (rec.dtype, tuple(rec.shape))
+    assert skipped.dtype == torch.int64 and skipped.numel() == 1 and skipped.is_cuda, (skipped.dtype, tuple(skipped.shape))
+    assert g.dtype == torch.float32 and g.is_contiguous() and g.numel() == arena.numel, (g.dtype, tuple(g.shape))
+    L().grad_clip_norm(g.data_ptr(), arena.block_tensor.data_ptr(), arena.tensor_span.data_ptr(), int(arena.n_blocks),
+                       float(max_norm), partial.data_ptr(), rec.data_ptr(), skipped.data_ptr(), _st(arena.W))
 
 
 def lars_trust(arena, g, inv_k, eta, partial, norms, trust):
@@ -796,8 +811,8 @@ def lamb_trust(arena, g, m, v, step, b1, b2, eps, inv_k, filt, partial, norms, t
                    _st(arena.W))
 
 
-def sgd_flat(arena, g, lr, mu, nesterov, inv_k, lo, hi, only_local=False, only_exchanged=False):
+def sgd_flat(arena, g, lr, mu, nesterov, inv_k, lo, hi, only_local=False, only_exchanged=False, clip=None):
     """Fused momentum-SGD over arena elements [lo, hi): ``flat_update``'s SGD rule.  ``lr`` is not used: the kernel reads
     ``arena.hyper[0]`` on the device (so a captured CUDA graph follows lr changes)."""
     filt = 1 if only_local else (2 if only_exchanged else 0)
-    flat_update(arena, "sgd", (mu, float(bool(nesterov)), inv_k), [arena.U], g=g, lo=lo, hi=hi, filt=filt)
+    flat_update(arena, "sgd", (mu, float(bool(nesterov)), inv_k), [arena.U], g=g, lo=lo, hi=hi, filt=filt, clip=clip)

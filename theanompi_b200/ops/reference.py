@@ -10,6 +10,8 @@ used c01b / bc01 (``theanompi/models/layers2.py:430-560``).
 """
 from __future__ import annotations
 
+import math
+
 import numpy as np
 import torch
 import torch.nn.functional as F
@@ -234,6 +236,24 @@ def uniform_noise(shape, seed, stream, step, device="cpu"):
 
 
 # --------------------------------------------------------------------------- optimizer (flat arena)
+def clip_scale(g, offsets, sizes, max_norm):
+    """Global gradient-norm clipping (``torch.nn.utils.clip_grad_norm_``) over a flat fp32 gradient laid out as a :class:`FlatArena`
+    (tensor ``i`` is ``[offsets[i], offsets[i] + sizes[i])``; the padding between tensors is ignored):
+
+        n = ‖g‖₂ over the real elements, accumulated in fp64
+        s = min(1, max_norm / (n + 1e-6))      rounded to fp32, as the device record holds it
+
+    Returns ``(n, s, finite)``.  When n is NaN or Inf, ``finite`` is False, s = 0 and the step is to be skipped."""
+    sq = 0.0
+    for o, s in zip(offsets, sizes):
+        v = g[o:o + s].double()
+        sq += float(torch.dot(v, v))
+    n = math.sqrt(sq)
+    if not math.isfinite(n):
+        return n, 0.0, False
+    return n, float(np.float32(min(1.0, float(np.float32(max_norm)) / (n + 1e-6)))), True
+
+
 def sgd_flat(w, g, u, lr_mult, wd, lr, mu, nesterov, inv_k, w_half=None):
     """One momentum-SGD step over flat fp32 buffers with per-element
     ``lr_mult`` / ``wd`` vectors (broadcastable).  Semantics of the reference's

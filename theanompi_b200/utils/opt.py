@@ -40,6 +40,7 @@ wrong sign; we implement the standard form  ``w ← w − lr (g_eff + μ u_new)`
 """
 from __future__ import annotations
 
+import numpy as np
 import torch
 
 from ..ops import reference as ref
@@ -93,13 +94,19 @@ class FlatOptimizer(object):
 
     A subclass names its kernel ``rule``, whether the rule keeps state in the arena's U region (``uses_u``), its extra flat
     ``buffers`` (zero-initialised, saved by :meth:`state_dict` under their names), its ``reference`` function and, in
-    :meth:`hyper`, its float hyper-parameters in the order both take them."""
+    :meth:`hyper`, its float hyper-parameters in the order both take them.
+
+    :meth:`set_grad_clip` adds global gradient-norm clipping to every step (``torch.nn.utils.clip_grad_norm_``).  On CUDA that is
+    two more launches before the update (``cuda_impl.grad_clip_norm``), whose record the update pass reads: it applies s·g, or
+    returns before it touches memory when the norm is NaN or Inf.  G itself is not changed."""
 
     rule = None
     uses_u = True
     buffers = ()
     reference = None
     t = None                         # device step counter of a rule that reads one (Adam)
+    max_norm = None                  # gradient clipping threshold (set_grad_clip), None: off
+    skipped = None                   # with clipping: int64 [1], the number of steps skipped for a non-finite gradient norm
 
     def __init__(self, arena):
         self.arena = arena
@@ -112,31 +119,90 @@ class FlatOptimizer(object):
     def _state(self):
         return ([self.arena.U] if self.uses_u else []) + [getattr(self, n) for n in self.buffers]
 
+    # ---- global gradient-norm clipping
+    def set_grad_clip(self, max_norm):
+        """Before every step, compute the global L2 norm n of the gradient over the real elements of every arena tensor.  A finite n
+        scales the step's gradient by s = min(1, max_norm / (n + 1e-6)) (``torch.nn.utils.clip_grad_norm_``; weight decay is added
+        after the scaling).  A NaN or Inf n skips the step: W, the bf16 shadow, the optimizer state and Adam's counter are left as
+        they are, and :attr:`skipped` counts it.  ``None`` turns clipping off.  On CUDA ``max_norm`` is a launch argument: a step
+        captured in a CUDA graph keeps the value it was captured with."""
+        if max_norm is None:
+            self.max_norm = None
+            return
+        if self.rule in ("lars", "lamb"):
+            raise ValueError("gradient-norm clipping is for the sgd, adam, rmsprop, adadelta and rmsprop_centered flat optimizers; "
+                             "%s's trust ratios already normalise every tensor's step" % self.rule.upper())
+        max_norm = float(max_norm)
+        if not max_norm > 0:
+            raise ValueError("grad_clip must be a positive maximum norm, not %r" % max_norm)
+        self.max_norm = max_norm
+        if self.skipped is None:
+            dev = self.arena.W.device
+            self._clip_rec = torch.zeros(4, dtype=torch.float32, device=dev)      # csrc/api.h: ClipRecord
+            self.skipped = torch.zeros(1, dtype=torch.int64, device=dev)
+            self._clip_partial = torch.zeros(self.arena.n_blocks, dtype=torch.float32, device=dev) if self.arena.W.is_cuda else None
+
+    @property
+    def grad_norm(self):
+        """The global gradient norm of the last clipped step, before clipping (a device scalar); None without clipping."""
+        return None if self.max_norm is None else self._clip_rec[0]
+
+    def _clip_cuda(self, g):
+        """With clipping on, the two norm launches over ``g``; returns the record the update pass reads (None: no clipping)."""
+        if self.max_norm is None:
+            return None
+        from ..ops import cuda_impl
+        cuda_impl.grad_clip_norm(self.arena, g, self.max_norm, self._clip_partial, self._clip_rec, self.skipped)
+        return self._clip_rec
+
+    def _clip_cpu(self, g):
+        """The CPU twin of :meth:`_clip_cuda`: returns s (1.0 without clipping), or None when the step is skipped."""
+        if self.max_norm is None:
+            return 1.0
+        a = self.arena
+        n, s, finite = ref.clip_scale(g, a.offsets, a.sizes, self.max_norm)
+        self._clip_rec[0], self._clip_rec[1] = n, s
+        self._clip_rec[2:3].view(torch.int32).fill_(int(finite))
+        if not finite:
+            self.skipped += 1
+            return None
+        return s
+
     def step(self, lr=None):
         a = self.arena
         if a.W.is_cuda:
             from ..ops import cuda_impl
-            cuda_impl.flat_update(a, self.rule, self.hyper(), self._state(), step=self.t)
+            cuda_impl.flat_update(a, self.rule, self.hyper(), self._state(), step=self.t, clip=self._clip_cuda(a.G))
             return
-        self._reference_step(float(a.hyper[0]) if lr is None else lr)
+        s = self._clip_cpu(a.G)
+        if s is None:
+            return
+        self._reference_step(float(a.hyper[0]) if lr is None else lr, a.G if s == 1.0 else a.G * s)
 
-    def _reference_step(self, lr):
+    def _reference_step(self, lr, g):
         a = self.arena
-        type(self).reference(a.W, a.G, *self._state(), a.lr_mult_vector(), a.wd_vector(), lr, *self.hyper(), w_half=a.H)
+        type(self).reference(a.W, g, *self._state(), a.lr_mult_vector(), a.wd_vector(), lr, *self.hyper(), w_half=a.H)
 
     def state_dict(self):
-        return {n: getattr(self, n).detach().cpu() for n in self.buffers}
+        sd = {n: getattr(self, n).detach().cpu() for n in self.buffers}
+        if self.max_norm is not None:
+            sd["skipped"] = int(self.skipped)
+        return sd
 
     def load_state_dict(self, sd):
         for n in self.buffers:
             getattr(self, n).copy_(sd[n].to(self.arena.W.device))
+        if self.max_norm is not None and "skipped" in sd:
+            self.skipped.fill_(int(sd["skipped"]))
 
 
 class FlatSGD(FlatOptimizer):
     """Fused momentum-SGD over the whole arena (or a block range); momentum in the arena's U region.
 
     :meth:`arm` (single GPU, k = 1) moves the update of the FC / Softmax weights into the epilogue of their weight-gradient GEMM
-    (``cuda_impl.gemm_sgd``): their fp32 gradient is never written, and ``step(lr, 1)`` updates only the rest of the arena."""
+    (``cuda_impl.gemm_sgd``): their fp32 gradient is never written, and ``step(lr, 1)`` updates only the rest of the arena.  With
+    gradient clipping (:meth:`FlatOptimizer.set_grad_clip`) nothing is armed: an epilogue would update its weight before the
+    global norm exists.  The clipping factor is folded into inv_k."""
 
     rule = "sgd"
 
@@ -155,7 +221,7 @@ class FlatSGD(FlatOptimizer):
         for p in a.params:
             p.sgd_epilogue = None
         self.armed, self.rest = [], None
-        if not enable or not a.W.is_cuda or getattr(model, "monitor_grad", False):
+        if not enable or not a.W.is_cuda or getattr(model, "monitor_grad", False) or self.max_norm is not None:
             return
         dt = getattr(model, "act_dtype", None)
         block = 16 // torch.empty((), dtype=dt).element_size() if dt is not None else 8
@@ -167,16 +233,24 @@ class FlatSGD(FlatOptimizer):
         self.rest = complement_ranges(a, self.armed)
 
     def step(self, lr=None, k=1, src="G", lo=0, hi=None, only_local=False, only_exchanged=False):
+        """With clipping, the norm is the one of the whole gradient region ``src``, whatever range or groups the step updates."""
         a = self.arena
         g = getattr(a, src)
         if a.W.is_cuda:
             from ..ops import cuda_impl
+            clip = self._clip_cuda(g)
             ranges = [(lo, a.numel if hi is None else hi)]
             if self.rest is not None and k == 1 and src == "G" and (lo, hi) == (0, None) and not (only_local or only_exchanged):
                 ranges = self.rest    # the armed weights were updated by their wgrad GEMMs during backward
             for rlo, rhi in ranges:
-                cuda_impl.sgd_flat(a, g, lr, self.mu, self.nesterov, 1.0 / k, rlo, rhi, only_local, only_exchanged)
+                cuda_impl.sgd_flat(a, g, lr, self.mu, self.nesterov, 1.0 / k, rlo, rhi, only_local, only_exchanged, clip=clip)
             return
+        inv_k = 1.0 / k
+        if self.max_norm is not None:
+            s = self._clip_cpu(g)
+            if s is None:
+                return
+            inv_k = float(np.float32(inv_k) * np.float32(s))          # the kernel's inv_k·s in fp32
         lr = float(a.hyper[0]) if lr is None else lr
         hi = a.numel if hi is None else hi
         sl = slice(lo, hi)
@@ -189,11 +263,11 @@ class FlatSGD(FlatOptimizer):
             if idx.numel() == 0:
                 return
             w2, u2 = w[idx].clone(), u[idx].clone()
-            ref.sgd_flat(w2, gg[idx], u2, lrm[idx], wd[idx], lr, self.mu, self.nesterov, 1.0 / k)
+            ref.sgd_flat(w2, gg[idx], u2, lrm[idx], wd[idx], lr, self.mu, self.nesterov, inv_k)
             w[idx] = w2
             u[idx] = u2
         else:
-            ref.sgd_flat(w, gg, u, lrm, wd, lr, self.mu, self.nesterov, 1.0 / k)
+            ref.sgd_flat(w, gg, u, lrm, wd, lr, self.mu, self.nesterov, inv_k)
         if a.H is not None:
             a.H[sl].copy_(w)
 
@@ -212,10 +286,10 @@ class FlatAdam(FlatOptimizer):
     def hyper(self):
         return (self.b1, self.b2, self.eps)
 
-    def _reference_step(self, lr):
+    def _reference_step(self, lr, g):
         a = self.arena
         self.t += 1
-        ref.adam_flat(a.W, a.G, a.U, self.V, a.lr_mult_vector(), a.wd_vector(), lr, *self.hyper(), t=float(self.t), w_half=a.H)
+        ref.adam_flat(a.W, g, a.U, self.V, a.lr_mult_vector(), a.wd_vector(), lr, *self.hyper(), t=float(self.t), w_half=a.H)
 
     def state_dict(self):
         return dict(super().state_dict(), t=int(self.t))
@@ -226,9 +300,11 @@ class FlatAdam(FlatOptimizer):
 
 
 class FlatRMSProp(FlatOptimizer):
-    """RMSProp, the squared-gradient average in ``V``: ``torch.optim.RMSprop(alpha=0.99, eps=1e-8)`` without momentum, the
-    optimizer of the reference's GANs (``lasagne_model_zoo/wgan.py:18-59``), plus an optional clip of the updated weights to
-    ``[-clip, clip]`` (the WGAN critic's weight clipping, folded into the same pass)."""
+    """RMSProp, the squared-gradient average in ``V``: ``torch.optim.RMSprop(alpha=0.99, eps=1e-8)`` without momentum, plus an
+    optional clip of the updated weights to ``[-clip, clip]`` (the WGAN critic's weight clipping, folded into the same pass).  It
+    is the optimizer of the torch GAN twins, not the reference's: the reference's MNIST GANs (``lasagne_model_zoo/wgan.py:18-59``)
+    use a centred RMSProp with momentum 0.5 that rescales the gradient by its norm first.  That rescaling is
+    :meth:`FlatOptimizer.set_grad_clip` (``grad_clip=5``)."""
 
     rule, uses_u, buffers, reference = "rmsprop", False, ("V",), ref.rmsprop_flat
 
@@ -369,10 +445,23 @@ def _ex(a):
     return a.exch_vector()
 
 
+def _set_clip(model, opt, k):
+    """``model.grad_clip``: clip the gradient of every step of ``opt`` by its global norm (:meth:`FlatOptimizer.set_grad_clip`);
+    ``model.clip_opt`` is then ``opt``, whose skip counter the checkpoints carry.  Only a local k = 1 step has the whole gradient
+    before it updates anything."""
+    if getattr(model, "grad_clip", None) is None:
+        return
+    if k != 1:
+        raise ValueError("grad_clip needs the global norm of the reduced gradient before any update; it runs on local k = 1 steps only")
+    opt.set_grad_clip(model.grad_clip)
+    model.clip_opt = opt
+
+
 def _pre_post_msgd(model, use_nesterov, k, arm=True):
     """BSP_MSGD: aggregate momentum."""
     a, mu = model.arena, (model.mu if model.use_momentum else 0.0)
     sgd = FlatSGD(a, mu, use_nesterov, True)
+    _set_clip(model, sgd, k)
     sgd.arm(model, k == 1 and arm)
 
     def pre():
@@ -401,6 +490,7 @@ def _pre_post_msgd_grad(model, use_nesterov, k, arm=True):
     """_BSP_MSGD: aggregate gradient."""
     a, mu = model.arena, (model.mu if model.use_momentum else 0.0)
     sgd = FlatSGD(a, mu, use_nesterov, True)
+    _set_clip(model, sgd, k)
     sgd.arm(model, k == 1 and arm)
 
     def pre():
@@ -429,6 +519,7 @@ def _pre_post_msgd_grad(model, use_nesterov, k, arm=True):
 def _pre_post_sgd(model, k, arm=True):
     a = model.arena
     sgd = FlatSGD(a, 0.0, False, False)
+    _set_clip(model, sgd, k)
     sgd.arm(model, k == 1 and arm)
 
     def pre():
