@@ -92,10 +92,10 @@ def conv_case(name, N, H, W, C, O, K, s, p, groups=1, dgrad=True):
 
     def g():
         if G == 1:
-            L.conv_wgrad(dy.data_ptr(), x.data_ptr(), dws[0].data_ptr(), N, H, W, C, 0, C, K, K, Ho, Ho, s, p, O, O, 0, S())
+            L.conv_wgrad(dy.data_ptr(), x.data_ptr(), dws[0].data_ptr(), N, H, W, C, 0, C, K, K, Ho, Ho, s, p, O, O, 0, 0, S())
         else:
             L.conv_wgrad2(dy.data_ptr(), dy.data_ptr() + O * es, x.data_ptr(), dws[0].data_ptr(), dws[1].data_ptr(), N, H, W, C * G,
-                          0, C, C, K, K, Ho, Ho, s, p, O, O * G, 0, S())
+                          0, C, C, K, K, Ho, Ho, s, p, O, O * G, 0, 0, S())
 
     cases = [(name + " fprop", f, useful, issued_macs(0, M, O, C, K * K, G))]
     if dgrad:

@@ -63,9 +63,11 @@ int gemm_plan_tall(long long M, int nt, int out_bf16, int sms);   // 1 = 256-row
 // M = output pixels, N = output channels, num_kb = taps x channel chunks; wgrad: M = output channels, N = (tap, channel-chunk)
 // boxes x box width, num_kb = pixel blocks.  tall_ok: the output may use 256-row tiles (bf16 output, or K-major tf32).
 std::tuple<int, int, int> gemm_plan_conv(int kind, long long M, int N, int groups, int num_kb, int tall_ok, int sms);
-// f32 = 1: fp32 operands through wgmma tf32 (fp32 output), else bf16 operands
+// f32 = 1: fp32 operands through wgmma tf32 (fp32 output), else bf16 operands.  accumulate = 1: C += the product (fp32 output
+// without bias / ReLU; gradient accumulation): the epilogue reduces every tile into C and the split-K clear is skipped
 void gemm(const void* A, const void* B, void* C, const float* bias, int M, int N, int K, long long lda, long long ldb, long long ldc,
-          int a_mn, int b_mn, int out_bf16, int bias_mode, int relu, float alpha, int bn_hint, int splitk, int f32, cudaStream_t st);
+          int a_mn, int b_mn, int out_bf16, int bias_mode, int relu, float alpha, int bn_hint, int splitk, int f32, cudaStream_t st,
+          int accumulate = 0);
 // FC weight gradient A^T B (A: [K, M], B: [K, N], both MN-major) applied as a momentum-SGD step to W / U [M, N] (fp32, row pitch
 // ldw) and the bf16 shadow H (may be null) in the GEMM epilogue, the same arithmetic as flat_update's SGD rule; lr is read from lr_ptr[0]
 void gemm_sgd(const void* A, const void* B, void* W, void* U, void* H, const void* lr_ptr, float lr_mult, float wd, float mu, int nesterov,
@@ -73,17 +75,20 @@ void gemm_sgd(const void* A, const void* B, void* W, void* U, void* H, const voi
 
 void conv_fprop(const void* x, const void* w, void* y, const float* bias, int N, int H, int W, int Ctot, int c_off, int Cg, int KH,
                 int KW, int Ho, int Wo, int S, int P, int O, long long ldc, int relu, int dgrad, int f32, cudaStream_t st);
+// accumulate = 1: dw += the weight gradient (gradient accumulation), else dw = it
 void conv_wgrad(const void* dy, const void* x, void* dw, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho,
-                int Wo, int S, int P, int O, long long ldy, int f32, cudaStream_t st);
+                int Wo, int S, int P, int O, long long ldy, int accumulate, int f32, cudaStream_t st);
 // both groups of a 2-group convolution in one persistent launch (see gemm_wgmma.cu)
 void conv_fprop2(const void* x, const void* w0, const void* w1, void* y0, void* y1, const float* bias0, const float* bias1, int N, int H,
                  int W, int Ctot, int c_off0, int c_off1, int Cg, int KH, int KW, int Ho, int Wo, int S, int P, int O, long long ldc,
                  int relu, int dgrad, int f32, cudaStream_t st);
 void conv_wgrad2(const void* dy0, const void* dy1, const void* x, void* dw0, void* dw1, int N, int H, int W, int Ctot, int c_off0,
-                 int c_off1, int Cg, int KH, int KW, int Ho, int Wo, int S, int P, int O, long long ldy, int f32, cudaStream_t st);
+                 int c_off1, int Cg, int KH, int KW, int Ho, int Wo, int S, int P, int O, long long ldy, int accumulate, int f32,
+                 cudaStream_t st);
 
 // ---- nn_kernels.cu  (f32: fp32 activations, C % 4 == 0; else bf16, C % 8 == 0)
 void space_to_depth(const void* x, void* y, int N, int H, int W, int C, int S, int Hs, int Ws, int Cp, int P, int f32, cudaStream_t st);
+// dir 0: pack a filter for the space-to-depth conv; 1: unpack its fp32 weight gradient (store); 2: unpack and add into dst
 void s2d_filter(const void* src, void* dst, int O, int KH, int KW, int C, int S, int KHs, int KWs, int Cp, int dir, int f32, cudaStream_t st);
 void lrn_fwd(const void* x, void* y, long long rows, int C, int n, float k, float alpha, float beta, int f32, cudaStream_t st);
 void lrn_bwd(const void* x, const void* dy, void* dx, long long rows, int C, int n, float k, float alpha, float beta, int f32, cudaStream_t st);
@@ -95,11 +100,14 @@ void dropout_fwd(const void* x, void* y, void* mask, long long n, float p_drop, 
                  cudaStream_t st);
 void dropout_bwd(const void* dy, const void* mask, void* dx, long long n, int f32, cudaStream_t st);
 void advance_step(void* step, cudaStream_t st);
-void softmax_xent(const void* logits, const void* labels, void* dlogits, void* rowstat, void* out3, int B, int C, float weight, int f32,
-                  cudaStream_t st);
-// act: 0 none, 1 ReLU, 2 leaky ReLU (negative slope `slope`), 3 sigmoid (ACT_* in common.cuh)
+// out3 = {weight · mean NLL, top-1 error, top-5 error}; dlogits = (softmax − onehot) · grad_weight / B (grad_weight = weight / n under
+// n-micro-batch gradient accumulation, so the accumulated gradient is the mean over the window)
+void softmax_xent(const void* logits, const void* labels, void* dlogits, void* rowstat, void* out3, int B, int C, float weight,
+                  float grad_weight, int f32, cudaStream_t st);
+// act: 0 none, 1 ReLU, 2 leaky ReLU (negative slope `slope`), 3 sigmoid (ACT_* in common.cuh).  accumulate = 1: db / db1 += the bias
+// gradient (no clear)
 void relu_bias_bwd(const void* dy, const void* y, void* dym, void* db, void* db1, int c_split, long long R, int C, long long ld, int act,
-                   float slope, int f32, cudaStream_t st);
+                   float slope, int accumulate, int f32, cudaStream_t st);
 void bias_act(const void* acc, const void* bias, void* y, int R, int C, int act, float slope, int f32, cudaStream_t st);
 // transposed-convolution forward: y[N,H,W,C] = act(col2im(dcol) + bias), dcol = x[N*Hi*Wi, Cin] · W[Cin, KH*KW*C] (row pitch ldcol);
 // channels >= c_real are written as zeros
@@ -107,9 +115,9 @@ void col2im_bias_act(const void* dcol, void* y, const float* bias, int N, int H,
                      long long ldcol, int act, float slope, int c_real, int f32, cudaStream_t st);
 void gan_loss(const void* scores, void* dscores, void* out, int B, int kind, float a, int f32, cudaStream_t st);
 void uniform_noise(void* out, long long n, unsigned long long seed, int stream, const void* step, int f32, cudaStream_t st);
-// bf16 only (packed-bf16 compares)
+// bf16 only (packed-bf16 compares).  accumulate = 1: db0 / db1 += the bias gradient (no clear)
 void maxpool_relu_bias_bwd(const void* dyp, const void* arg, const void* y, void* dym, void* db0, void* db1, int c_split, int N, int H,
-                           int W, int C, int Ho, int Wo, int k, int s, int p, cudaStream_t st);
+                           int W, int C, int Ho, int Wo, int k, int s, int p, int accumulate, cudaStream_t st);
 void im2col(const void* x, void* col, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho, int Wo, int s, int p,
             long long ldcol, int f32, cudaStream_t st);
 void col2im(const void* dcol, void* dx, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho, int Wo, int s, int p,
@@ -122,8 +130,10 @@ void crop_mirror_norm(const void* x, int in_kind, const void* mean, int mean_mod
 void bn_forward(const void* x, const void* res, void* y, const void* gamma, const void* beta, void* mean, void* rstd, void* run_mean,
                 void* run_var, void* scratch, long long R, int C, float momentum, float eps, int training, int act, float slope, int f32,
                 cudaStream_t st);
+// scratch: 3*C floats, 5*C with accumulate = 1 (dgamma / dbeta += this batch's gradients; dx is computed from this batch's sums, which
+// go to the scratch, exactly as without accumulate)
 void bn_backward(const void* x, const void* dy, const void* y, void* dx, void* dres, const void* gamma, const void* mean, const void* rstd,
-                 void* dgamma, void* dbeta, void* scratch, long long R, int C, int act, float slope, int f32, cudaStream_t st);
+                 void* dgamma, void* dbeta, void* scratch, long long R, int C, int act, float slope, int accumulate, int f32, cudaStream_t st);
 void add_tensors(const void* a, const void* b, void* y, long long n, int f32, cudaStream_t st);
 void add4_tensors(const void* a, const void* b, const void* c, const void* d, void* y, long long n, int f32, cudaStream_t st);
 

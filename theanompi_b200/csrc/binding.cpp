@@ -54,12 +54,12 @@ PYBIND11_MODULE(_tmpi_native, m) {
   m.def("gemm_plan_tall", &gemm_plan_tall);
   m.def("gemm_plan_conv", &gemm_plan_conv);
   m.def("gemm", [](ptr_t A, ptr_t B, ptr_t C, ptr_t bias, int M, int N, int K, long long lda, long long ldb, long long ldc, int a_mn, int b_mn,
-                   int out_bf16, int bias_mode, int relu, float alpha, int bn_hint, int splitk, int f32, ptr_t st) {
+                   int out_bf16, int bias_mode, int relu, float alpha, int bn_hint, int splitk, int f32, ptr_t st, int accumulate) {
     gemm(P(A), P(B), P(C), (const float*)P(bias), M, N, K, lda, ldb, ldc, a_mn, b_mn, out_bf16, bias_mode, relu, alpha, bn_hint, splitk, f32,
-         S(st));
+         S(st), accumulate);
   }, py::arg("A"), py::arg("B"), py::arg("C"), py::arg("bias"), py::arg("M"), py::arg("N"), py::arg("K"), py::arg("lda"), py::arg("ldb"),
      py::arg("ldc"), py::arg("a_mn"), py::arg("b_mn"), py::arg("out_bf16"), py::arg("bias_mode"), py::arg("relu"), py::arg("alpha"),
-     py::arg("bn_hint"), py::arg("splitk"), py::arg("f32"), py::arg("st"));
+     py::arg("bn_hint"), py::arg("splitk"), py::arg("f32"), py::arg("st"), py::arg("accumulate") = 0);
   m.def("gemm_sgd", [](ptr_t A, ptr_t B, ptr_t W, ptr_t U, ptr_t H, ptr_t lr_ptr, float lr_mult, float wd, float mu, int nesterov, float inv_k,
                        int M, int N, int K, long long lda, long long ldb, long long ldw, int f32, ptr_t st) {
     gemm_sgd(P(A), P(B), P(W), P(U), P(H), P(lr_ptr), lr_mult, wd, mu, nesterov, inv_k, M, N, K, lda, ldb, ldw, f32, S(st));
@@ -72,15 +72,16 @@ PYBIND11_MODULE(_tmpi_native, m) {
                          int Sd, int Pd, int O, long long ldc, int relu, int dgrad, int f32, ptr_t st) {
     conv_fprop(P(x), P(w), P(y), (const float*)P(bias), N, H, W, Ctot, c_off, Cg, KH, KW, Ho, Wo, Sd, Pd, O, ldc, relu, dgrad, f32, S(st)); });
   m.def("conv_wgrad", [](ptr_t dy, ptr_t x, ptr_t dw, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho, int Wo, int Sd,
-                         int Pd, int O, long long ldy, int f32, ptr_t st) {
-    conv_wgrad(P(dy), P(x), P(dw), N, H, W, Ctot, c_off, Cg, KH, KW, Ho, Wo, Sd, Pd, O, ldy, f32, S(st)); });
+                         int Pd, int O, long long ldy, int accumulate, int f32, ptr_t st) {
+    conv_wgrad(P(dy), P(x), P(dw), N, H, W, Ctot, c_off, Cg, KH, KW, Ho, Wo, Sd, Pd, O, ldy, accumulate, f32, S(st)); });
   m.def("conv_fprop2", [](ptr_t x, ptr_t w0, ptr_t w1, ptr_t y0, ptr_t y1, ptr_t b0, ptr_t b1, int N, int H, int W, int Ctot, int c_off0, int c_off1,
                           int Cg, int KH, int KW, int Ho, int Wo, int Sd, int Pd, int O, long long ldc, int relu, int dgrad, int f32, ptr_t st) {
     conv_fprop2(P(x), P(w0), P(w1), P(y0), P(y1), (const float*)P(b0), (const float*)P(b1), N, H, W, Ctot, c_off0, c_off1, Cg, KH, KW, Ho, Wo,
                 Sd, Pd, O, ldc, relu, dgrad, f32, S(st)); });
   m.def("conv_wgrad2", [](ptr_t dy0, ptr_t dy1, ptr_t x, ptr_t dw0, ptr_t dw1, int N, int H, int W, int Ctot, int c_off0, int c_off1, int Cg,
-                          int KH, int KW, int Ho, int Wo, int Sd, int Pd, int O, long long ldy, int f32, ptr_t st) {
-    conv_wgrad2(P(dy0), P(dy1), P(x), P(dw0), P(dw1), N, H, W, Ctot, c_off0, c_off1, Cg, KH, KW, Ho, Wo, Sd, Pd, O, ldy, f32, S(st)); });
+                          int KH, int KW, int Ho, int Wo, int Sd, int Pd, int O, long long ldy, int accumulate, int f32, ptr_t st) {
+    conv_wgrad2(P(dy0), P(dy1), P(x), P(dw0), P(dw1), N, H, W, Ctot, c_off0, c_off1, Cg, KH, KW, Ho, Wo, Sd, Pd, O, ldy, accumulate, f32,
+                S(st)); });
   m.def("space_to_depth", [](ptr_t x, ptr_t y, int N, int H, int W, int C, int Sd, int Hs, int Ws, int Cp, int Pd, int f32, ptr_t st) {
     space_to_depth(P(x), P(y), N, H, W, C, Sd, Hs, Ws, Cp, Pd, f32, S(st)); });
   m.def("s2d_filter", [](ptr_t src, ptr_t dst, int O, int KH, int KW, int C, int Sd, int KHs, int KWs, int Cp, int dir, int f32, ptr_t st) {
@@ -99,13 +100,15 @@ PYBIND11_MODULE(_tmpi_native, m) {
     dropout_fwd(P(x), P(y), P(mask), n, p, seed, layer, P(step), f32, S(st)); });
   m.def("dropout_bwd", [](ptr_t dy, ptr_t mask, ptr_t dx, long long n, int f32, ptr_t st) { dropout_bwd(P(dy), P(mask), P(dx), n, f32, S(st)); });
   m.def("advance_step", [](ptr_t step, ptr_t st) { advance_step(P(step), S(st)); });
-  m.def("softmax_xent", [](ptr_t logits, ptr_t labels, ptr_t dlogits, ptr_t rowstat, ptr_t out3, int B, int C, float weight, int f32, ptr_t st) {
-    softmax_xent(P(logits), P(labels), P(dlogits), P(rowstat), P(out3), B, C, weight, f32, S(st)); });
+  m.def("softmax_xent", [](ptr_t logits, ptr_t labels, ptr_t dlogits, ptr_t rowstat, ptr_t out3, int B, int C, float weight, float grad_weight,
+                           int f32, ptr_t st) {
+    softmax_xent(P(logits), P(labels), P(dlogits), P(rowstat), P(out3), B, C, weight, grad_weight, f32, S(st)); });
   m.def("maxpool_relu_bias_bwd", [](ptr_t dyp, ptr_t arg, ptr_t y, ptr_t dym, ptr_t db0, ptr_t db1, int c_split, int N, int H, int W, int C,
-                                    int Ho, int Wo, int k, int s, int p, ptr_t st) {
-    maxpool_relu_bias_bwd(P(dyp), P(arg), P(y), P(dym), P(db0), P(db1), c_split, N, H, W, C, Ho, Wo, k, s, p, S(st)); });
+                                    int Ho, int Wo, int k, int s, int p, int accumulate, ptr_t st) {
+    maxpool_relu_bias_bwd(P(dyp), P(arg), P(y), P(dym), P(db0), P(db1), c_split, N, H, W, C, Ho, Wo, k, s, p, accumulate, S(st)); });
   m.def("relu_bias_bwd", [](ptr_t dy, ptr_t y, ptr_t dym, ptr_t db, ptr_t db1, int c_split, long long R, int C, long long ld, int act, float slope,
-                            int f32, ptr_t st) { relu_bias_bwd(P(dy), P(y), P(dym), P(db), P(db1), c_split, R, C, ld, act, slope, f32, S(st)); });
+                            int accumulate, int f32, ptr_t st) {
+    relu_bias_bwd(P(dy), P(y), P(dym), P(db), P(db1), c_split, R, C, ld, act, slope, accumulate, f32, S(st)); });
   m.def("bias_act", [](ptr_t acc, ptr_t bias, ptr_t y, int R, int C, int act, float slope, int f32, ptr_t st) {
     bias_act(P(acc), P(bias), P(y), R, C, act, slope, f32, S(st)); });
   m.def("col2im_bias_act", [](ptr_t dcol, ptr_t y, ptr_t bias, int N, int H, int W, int C, int KH, int KW, int Hi, int Wi, int s, int p,
@@ -131,8 +134,9 @@ PYBIND11_MODULE(_tmpi_native, m) {
     bn_forward(P(x), P(res), P(y), P(gamma), P(beta), P(mean), P(rstd), P(run_mean), P(run_var), P(scratch), R, C, momentum, eps, training, act,
                slope, f32, S(st)); });
   m.def("bn_backward", [](ptr_t x, ptr_t dy, ptr_t y, ptr_t dx, ptr_t dres, ptr_t gamma, ptr_t mean, ptr_t rstd, ptr_t dgamma, ptr_t dbeta,
-                          ptr_t scratch, long long R, int C, int act, float slope, int f32, ptr_t st) {
-    bn_backward(P(x), P(dy), P(y), P(dx), P(dres), P(gamma), P(mean), P(rstd), P(dgamma), P(dbeta), P(scratch), R, C, act, slope, f32, S(st)); });
+                          ptr_t scratch, long long R, int C, int act, float slope, int accumulate, int f32, ptr_t st) {
+    bn_backward(P(x), P(dy), P(y), P(dx), P(dres), P(gamma), P(mean), P(rstd), P(dgamma), P(dbeta), P(scratch), R, C, act, slope, accumulate, f32,
+                S(st)); });
   m.def("add4_tensors", [](ptr_t a, ptr_t b, ptr_t c, ptr_t d, ptr_t y, long long n, int f32, ptr_t st) {
     add4_tensors(P(a), P(b), P(c), P(d), P(y), n, f32, S(st)); });
   m.def("add_tensors", [](ptr_t a, ptr_t b, ptr_t y, long long n, int f32, ptr_t st) { add_tensors(P(a), P(b), P(y), n, f32, S(st)); });

@@ -214,6 +214,21 @@ __global__ void bn_bwd_coef_kernel(const float* __restrict__ gamma, const float*
   k[c] = k1; k[C + c] = k2; k[2 * C + c] = -k1 * dbeta[c] * inv_m - k2 * mean[c];
 }
 
+// accumulate mode: the same coefficients from THIS batch's sums (sb = Σg, sg = Σg·x̂ in the scratch), which one thread per channel
+// then adds into the accumulated dβ / dγ (one fp32 add per element: deterministic)
+__global__ void bn_bwd_coef_accum_kernel(const float* __restrict__ gamma, const float* __restrict__ mean, const float* __restrict__ rstd,
+                                         const float* __restrict__ sg, const float* __restrict__ sb, float* __restrict__ dgamma,
+                                         float* __restrict__ dbeta, float* __restrict__ k, int C, float inv_m) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const float g = sg[c], b = sb[c];
+  const float k1 = gamma[c] * rstd[c];
+  const float k2 = -k1 * rstd[c] * g * inv_m;
+  k[c] = k1; k[C + c] = k2; k[2 * C + c] = -k1 * b * inv_m - k2 * mean[c];
+  dgamma[c] += g;
+  dbeta[c] += b;
+}
+
 template <typename T, int ACT>
 __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const T* __restrict__ x, const T* __restrict__ dy, const T* __restrict__ y,
                                                           T* __restrict__ dx, T* __restrict__ dres, const float* __restrict__ k, long long R, int C,
@@ -311,13 +326,19 @@ static void bn_apply_t(const void* x, const void* res, void* y, const float* s0,
 
 template <typename T>
 static void bn_bwd_t(const void* x, const void* dy, const void* y, void* dx, void* dres, const float* mean, const float* rstd, void* dgamma,
-                     void* dbeta, const float* gamma, float* k, long long R, int C, int act, float slope, cudaStream_t st) {
+                     void* dbeta, const float* gamma, float* k, long long R, int C, int act, float slope, int accumulate, cudaStream_t st) {
   constexpr int N = VecIO<T>::N;
-  if (act == ACT_NONE || act == ACT_RELU) colreduce<T, 1>(x, dy, y, mean, rstd, (float*)dbeta, (float*)dgamma, R, C, act, st);
-  else if (act == ACT_LEAKY) colreduce<T, 1, ACT_LEAKY>(x, dy, y, mean, rstd, (float*)dbeta, (float*)dgamma, R, C, act, st, slope);
-  else if (act == ACT_SIGMOID) colreduce<T, 1, ACT_SIGMOID>(x, dy, y, mean, rstd, (float*)dbeta, (float*)dgamma, R, C, act, st, slope);
+  // accumulate: this batch's sums go to the scratch after the coefficients (k[3C, 5C)), not into the accumulated dγ / dβ
+  float* sb = accumulate ? k + 3 * C : (float*)dbeta;
+  float* sg = accumulate ? k + 4 * C : (float*)dgamma;
+  if (act == ACT_NONE || act == ACT_RELU) colreduce<T, 1>(x, dy, y, mean, rstd, sb, sg, R, C, act, st);
+  else if (act == ACT_LEAKY) colreduce<T, 1, ACT_LEAKY>(x, dy, y, mean, rstd, sb, sg, R, C, act, st, slope);
+  else if (act == ACT_SIGMOID) colreduce<T, 1, ACT_SIGMOID>(x, dy, y, mean, rstd, sb, sg, R, C, act, st, slope);
   else throw std::runtime_error("batch_norm: unknown activation");
-  bn_bwd_coef_kernel<<<grid1(C, 256), 256, 0, st>>>(gamma, mean, rstd, (const float*)dgamma, (const float*)dbeta, k, C, 1.f / (float)R);
+  if (accumulate)
+    bn_bwd_coef_accum_kernel<<<grid1(C, 256), 256, 0, st>>>(gamma, mean, rstd, sg, sb, (float*)dgamma, (float*)dbeta, k, C, 1.f / (float)R);
+  else
+    bn_bwd_coef_kernel<<<grid1(C, 256), 256, 0, st>>>(gamma, mean, rstd, (const float*)dgamma, (const float*)dbeta, k, C, 1.f / (float)R);
   const RowGeom g = row_geom(R, C / N);
   if ((long long)g.rows_per_cta * C >= (1LL << 32)) throw std::runtime_error("batch_norm: row slab too large for 32-bit offsets");
 #define BNB(A) bn_bwd_apply_kernel<T, A><<<g.grid, 256, 0, st>>>((const T*)x, (const T*)dy, (const T*)y, (T*)dx, (T*)dres, k, R, C, act, g.VT, \
@@ -350,12 +371,12 @@ void bn_forward(const void* x, const void* res, void* y, const void* gamma, cons
   count_launch(training ? 3 : 2); TMPI_CHECK_LAUNCH("bn_forward"); ::tmpi::check_capture(st, "bn_forward");
 }
 
-// scratch: 3*C floats (the coefficients of the apply pass)
+// scratch: 3*C floats (the coefficients of the apply pass), 5*C with accumulate (+ this batch's Σg, Σg·x̂)
 void bn_backward(const void* x, const void* dy, const void* y, void* dx, void* dres, const void* gamma, const void* mean, const void* rstd,
-                 void* dgamma, void* dbeta, void* scratch, long long R, int C, int act, float slope, int f32, cudaStream_t st) {
+                 void* dgamma, void* dbeta, void* scratch, long long R, int C, int act, float slope, int accumulate, int f32, cudaStream_t st) {
   auto M = (const float*)mean; auto RS = (const float*)rstd; auto G = (const float*)gamma; auto K = (float*)scratch;
-  if (f32) bn_bwd_t<float>(x, dy, y, dx, dres, M, RS, dgamma, dbeta, G, K, R, C, act, slope, st);
-  else bn_bwd_t<__nv_bfloat16>(x, dy, y, dx, dres, M, RS, dgamma, dbeta, G, K, R, C, act, slope, st);
+  if (f32) bn_bwd_t<float>(x, dy, y, dx, dres, M, RS, dgamma, dbeta, G, K, R, C, act, slope, accumulate, st);
+  else bn_bwd_t<__nv_bfloat16>(x, dy, y, dx, dres, M, RS, dgamma, dbeta, G, K, R, C, act, slope, accumulate, st);
   count_launch(3); TMPI_CHECK_LAUNCH("bn_backward"); ::tmpi::check_capture(st, "bn_backward");
 }
 

@@ -145,12 +145,14 @@ std::tuple<int, int, int> gemm_plan_conv(int kind, long long M, int N, int group
 //   a_mn == 0: A is [M, K] with row pitch lda (elements);  a_mn == 1: A is [K, M] with row pitch lda.
 //   b_mn == 0: B is [N, K] with row pitch ldb;             b_mn == 1: B is [K, N] with row pitch ldb.
 //   bn_hint: 0 = auto, else 32/64/128.  splitk: 0 = auto, 1 = none, >1 = forced (fp32 output only, no bias/relu).
+//   accumulate = 1: C += op(A) op(B) (fp32 output only, no bias/relu): every tile reaches C through the epilogue's fp32 reductions
+//   and the split-K clear is skipped (gradient accumulation into the arena's G).
 //   T = __nv_bfloat16: bf16 operands (wgmma bf16), bf16 or fp32 output.  T = float: fp32 operands (wgmma tf32), fp32 output.
 namespace wgmma {
 template <typename T>
 static void gemm_host(const void* A, const void* B, void* C, const float* bias, int M, int N, int K, long long lda, long long ldb,
                       long long ldc, int a_mn, int b_mn, int out_bf16, int bias_mode, int relu, float alpha, int bn_hint, int splitk,
-                      cudaStream_t st) {
+                      int accumulate, cudaStream_t st) {
   using E = Elem<T>;
   constexpr int BK = E::BK, ATOM = E::ATOM, ESZ = E::ESZ;
   if (M <= 0 || N <= 0 || K <= 0) return;
@@ -158,6 +160,7 @@ static void gemm_host(const void* A, const void* B, void* C, const float* bias, 
   const int mt = (M + BM - 1) / BM;
   const bool fused_epi = bias_mode != 0 || relu;
   const bool can_split = (!out_bf16) && !fused_epi;
+  if (accumulate && !can_split) throw std::runtime_error("gemm: accumulate needs an fp32 output without bias / ReLU");
   int BN = bn_hint;
   if (BN == 0) {
     BN = 128;
@@ -181,7 +184,7 @@ static void gemm_host(const void* A, const void* B, void* C, const float* bias, 
 
   Params p;
   p.C = C; p.bias = bias; p.alpha = alpha; p.M = M; p.N = N; p.K = K; p.ldc = ldc; p.a_mn = a_mn; p.b_mn = b_mn;
-  p.out_bf16 = out_bf16; p.bias_mode = bias ? bias_mode : 0; p.relu = relu; p.kb_per_split = kb_per; p.atomic_out = splits > 1;
+  p.out_bf16 = out_bf16; p.bias_mode = bias ? bias_mode : 0; p.relu = relu; p.kb_per_split = kb_per; p.atomic_out = splits > 1 || accumulate;
   // tall tiles: bf16 path — bf16 outputs (fprop / dgrad); tf32 path — un-split outputs of K-major operands
   const int tall_ok = ESZ == 2 ? out_bf16 : (!a_mn && !b_mn);
   const bool tall = splits == 1 && BN >= 64 && use_tall_tiles(M, nt, tall_ok, sms);
@@ -190,10 +193,10 @@ static void gemm_host(const void* A, const void* B, void* C, const float* bias, 
   p.cHo = p.cWo = p.cS = p.cP = p.cKH = p.cKW = p.cCg = p.c_chunks = 0;
   // wgrad outputs registered for the fused reduce-scatter: every vector is red.add-ed into its owner's G (the exchange kernel
   // clears G after consuming it, so there is no memset here — a memset would race with the peers' adds)
-  const bool rs = (!out_bf16) && bias_mode == 0 && !relu && alpha == 1.f && (ldc % 4) == 0 && rs_lookup(C, p);
+  const bool rs = !accumulate && (!out_bf16) && bias_mode == 0 && !relu && alpha == 1.f && (ldc % 4) == 0 && rs_lookup(C, p);
   if (rs) {
     p.atomic_out = 1;
-  } else if (splits > 1) {
+  } else if (splits > 1 && !accumulate) {
     // split-K accumulates with fp32 atomics: clear the (possibly strided) output first
     check_cuda(cudaMemset2DAsync(C, (size_t)ldc * 4, 0, (size_t)N * 4, (size_t)M, st), "gemm split-K memset");
   }
@@ -211,9 +214,10 @@ static void gemm_host(const void* A, const void* B, void* C, const float* bias, 
 
 void gemm(const void* A, const void* B, void* C, const float* bias, int M, int N, int K, long long lda, long long ldb,
           long long ldc, int a_mn, int b_mn, int out_bf16, int bias_mode, int relu, float alpha, int bn_hint, int splitk, int f32,
-          cudaStream_t st) {
-  if (f32) wgmma::gemm_host<float>(A, B, C, bias, M, N, K, lda, ldb, ldc, a_mn, b_mn, 0, bias_mode, relu, alpha, bn_hint, splitk, st);
-  else wgmma::gemm_host<__nv_bfloat16>(A, B, C, bias, M, N, K, lda, ldb, ldc, a_mn, b_mn, out_bf16, bias_mode, relu, alpha, bn_hint, splitk, st);
+          cudaStream_t st, int accumulate) {
+  if (f32) wgmma::gemm_host<float>(A, B, C, bias, M, N, K, lda, ldb, ldc, a_mn, b_mn, 0, bias_mode, relu, alpha, bn_hint, splitk, accumulate, st);
+  else wgmma::gemm_host<__nv_bfloat16>(A, B, C, bias, M, N, K, lda, ldb, ldc, a_mn, b_mn, out_bf16, bias_mode, relu, alpha, bn_hint, splitk,
+                                       accumulate, st);
 }
 
 // ------------------------------------------------------------------ implicit-GEMM convolution (TMA im2col)
@@ -341,9 +345,11 @@ static void conv_fprop_groups(int ngroups, const void* x, const int* c_off, cons
 
 // dw[O][KH*KW][Cg] (fp32, contiguous) = sum over pixels dy[pix, o] * im2col(x)[pix, (tap, c)]   (dy: [M, O], row pitch ldy)
 // ngroups = 2: both groups in one launch (dy[g] = the group's channel slice of the output gradient, x slice c_off[g], dw[g]).
+// accumulate = 1: dw += ... through the epilogue's fp32 reductions, without the split-K clear.
 template <typename T>
 static void conv_wgrad_groups(int ngroups, const void* const* dy, const void* x, void* const* dw, const int* c_off, int N, int H, int W,
-                              int Ctot, int Cg, int KH, int KW, int Ho, int Wo, int S, int P, int O, long long ldy, cudaStream_t st) {
+                              int Ctot, int Cg, int KH, int KW, int Ho, int Wo, int S, int P, int O, long long ldy, int accumulate,
+                              cudaStream_t st) {
   using E = Elem<T>;
   constexpr int BK = E::BK, ATOM = E::ATOM, ESZ = E::ESZ;
   const long long M = (long long)N * Ho * Wo;
@@ -363,10 +369,10 @@ static void conv_wgrad_groups(int ngroups, const void* const* dy, const void* x,
   p.num_kb = num_kb;
   const int splits = tile.splits;
   p.kb_per_split = (p.num_kb + splits - 1) / splits;
-  p.splits = splits; p.atomic_out = splits > 1;
+  p.splits = splits; p.atomic_out = splits > 1 || accumulate;
   CUtensorMap ta[2], tb[2];
   for (int g = 0; g < ngroups; ++g) {
-    if (splits > 1) check_cuda(cudaMemsetAsync(dw[g], 0, (size_t)O * KH * KW * Cg * 4, st), "conv_wgrad memset");
+    if (splits > 1 && !accumulate) check_cuda(cudaMemsetAsync(dw[g], 0, (size_t)O * KH * KW * Cg * 4, st), "conv_wgrad memset");
     ta[g] = make_tmap(dy[g], (uint64_t)O, (uint64_t)M, (uint64_t)ldy * ESZ, (uint32_t)BK, ESZ, 1);          // both operands MN-major
     tb[g] = make_im2col_map(x, N, H, W, Ctot, c_off[g], Cg, KH, KW, S, P, BK, ESZ, 1);
   }
@@ -394,17 +400,18 @@ void conv_fprop2(const void* x, const void* w0, const void* w1, void* y0, void* 
 }
 
 void conv_wgrad(const void* dy, const void* x, void* dw, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho,
-                int Wo, int S, int P, int O, long long ldy, int f32, cudaStream_t st) {
+                int Wo, int S, int P, int O, long long ldy, int accumulate, int f32, cudaStream_t st) {
   const void* dys[1] = {dy}; void* dws[1] = {dw};
-  if (f32) wgmma::conv_wgrad_groups<float>(1, dys, x, dws, &c_off, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldy, st);
-  else wgmma::conv_wgrad_groups<__nv_bfloat16>(1, dys, x, dws, &c_off, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldy, st);
+  if (f32) wgmma::conv_wgrad_groups<float>(1, dys, x, dws, &c_off, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldy, accumulate, st);
+  else wgmma::conv_wgrad_groups<__nv_bfloat16>(1, dys, x, dws, &c_off, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldy, accumulate, st);
 }
 
 void conv_wgrad2(const void* dy0, const void* dy1, const void* x, void* dw0, void* dw1, int N, int H, int W, int Ctot, int c_off0,
-                 int c_off1, int Cg, int KH, int KW, int Ho, int Wo, int S, int P, int O, long long ldy, int f32, cudaStream_t st) {
+                 int c_off1, int Cg, int KH, int KW, int Ho, int Wo, int S, int P, int O, long long ldy, int accumulate, int f32,
+                 cudaStream_t st) {
   const void* dys[2] = {dy0, dy1}; void* dws[2] = {dw0, dw1}; const int co[2] = {c_off0, c_off1};
-  if (f32) wgmma::conv_wgrad_groups<float>(2, dys, x, dws, co, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldy, st);
-  else wgmma::conv_wgrad_groups<__nv_bfloat16>(2, dys, x, dws, co, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldy, st);
+  if (f32) wgmma::conv_wgrad_groups<float>(2, dys, x, dws, co, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldy, accumulate, st);
+  else wgmma::conv_wgrad_groups<__nv_bfloat16>(2, dys, x, dws, co, N, H, W, Ctot, Cg, KH, KW, Ho, Wo, S, P, O, ldy, accumulate, st);
 }
 
 }  // namespace tmpi

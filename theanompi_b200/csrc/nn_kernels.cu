@@ -617,18 +617,21 @@ __global__ void rowstat_mean_kernel(const float* __restrict__ rowstat, float* __
   }
 }
 
-void softmax_xent(const void* logits, const void* labels, void* dlogits, void* rowstat, void* out3, int B, int C, float weight, int f32,
-                  cudaStream_t st) {
+// the reported loss carries `weight`, the gradient `grad_weight` (weight / n under gradient accumulation over n micro-batches)
+void softmax_xent(const void* logits, const void* labels, void* dlogits, void* rowstat, void* out3, int B, int C, float weight,
+                  float grad_weight, int f32, cudaStream_t st) {
   auto LB = (const long long*)labels; auto RS = (float*)rowstat;
-  if (f32) softmax_xent_kernel<float><<<B, 256, 0, st>>>((const float*)logits, LB, (float*)dlogits, RS, C, weight / (float)B);
-  else softmax_xent_kernel<__nv_bfloat16><<<B, 256, 0, st>>>((const __nv_bfloat16*)logits, LB, (__nv_bfloat16*)dlogits, RS, C, weight / (float)B);
+  const float scale = grad_weight / (float)B;
+  if (f32) softmax_xent_kernel<float><<<B, 256, 0, st>>>((const float*)logits, LB, (float*)dlogits, RS, C, scale);
+  else softmax_xent_kernel<__nv_bfloat16><<<B, 256, 0, st>>>((const __nv_bfloat16*)logits, LB, (__nv_bfloat16*)dlogits, RS, C, scale);
   count_launch(); TMPI_CHECK_LAUNCH("softmax_xent"); ::tmpi::check_capture(st, "softmax_xent");
   rowstat_mean_kernel<<<1, 256, 0, st>>>((const float*)rowstat, (float*)out3, B, weight);
   count_launch(); TMPI_CHECK_LAUNCH("rowstat_mean"); ::tmpi::check_capture(st, "rowstat_mean");
 }
 
 // ============================================================================ activation mask + bias gradient
-// dym = act'(y) * dy (contiguous [R, C]; ReLU: dy * (y > 0));  db[c] += sum_r dym[r, c]   (db pre-zeroed by the launcher)
+// dym = act'(y) * dy (contiguous [R, C]; ReLU: dy * (y > 0));  db[c] += sum_r dym[r, c]   (db pre-zeroed by the launcher, unless it
+// accumulates a gradient over several micro-batches)
 // dy / y have row pitch ld (elements) so channel slices of a wider tensor work (grouped conv).
 template <typename T, int ACT, bool WRITE>
 __global__ void relu_bias_bwd_kernel(const T* __restrict__ dy, const T* __restrict__ y,
@@ -702,7 +705,7 @@ __global__ void relu_bias_bwd_kernel(const T* __restrict__ dy, const T* __restri
 // pass db1 = nullptr / c_split = C for a single bias vector.
 template <typename T>
 static void relu_bias_bwd_t(const void* dy, const void* y, void* dym, void* db, void* db1, int c_split, long long R, int C, long long ld,
-                            int act, float slope, cudaStream_t st) {
+                            int act, float slope, int accumulate, cudaStream_t st) {
   constexpr int N = VecIO<T>::N;
   const int nvec = C / N;
   const int VT = nvec < 32 ? nvec : 32;
@@ -714,8 +717,8 @@ static void relu_bias_bwd_t(const void* dy, const void* y, void* dym, void* db, 
   dim3 grid((unsigned)((R + rows_per_cta - 1) / rows_per_cta), (unsigned)((nvec + VT - 1) / VT));
   const size_t smem = (size_t)RL * VT * N * sizeof(float);
   if (!db1 || c_split > C) c_split = C;
-  if (db) check_cuda(cudaMemsetAsync(db, 0, (size_t)c_split * 4, st), "relu_bias_bwd memset");
-  if (db && c_split < C) check_cuda(cudaMemsetAsync(db1, 0, (size_t)(C - c_split) * 4, st), "relu_bias_bwd memset");
+  if (db && !accumulate) check_cuda(cudaMemsetAsync(db, 0, (size_t)c_split * 4, st), "relu_bias_bwd memset");
+  if (db && !accumulate && c_split < C) check_cuda(cudaMemsetAsync(db1, 0, (size_t)(C - c_split) * 4, st), "relu_bias_bwd memset");
   const bool write = dym != nullptr;
   auto DY = (const T*)dy; auto Y = (const T*)y; auto DM = (T*)dym; auto DB = (float*)db; auto DB1 = (float*)db1;
 #define RBB(A, WR) relu_bias_bwd_kernel<T, A, WR><<<grid, 256, smem, st>>>(DY, Y, DM, DB, DB1, c_split, R, C, ld, VT, rows_per_cta, slope)
@@ -731,10 +734,10 @@ static void relu_bias_bwd_t(const void* dy, const void* y, void* dym, void* db, 
   count_launch(); TMPI_CHECK_LAUNCH("relu_bias_bwd"); ::tmpi::check_capture(st, "relu_bias_bwd");
 }
 void relu_bias_bwd(const void* dy, const void* y, void* dym, void* db, void* db1, int c_split, long long R, int C, long long ld, int act,
-                   float slope, int f32, cudaStream_t st) {
+                   float slope, int accumulate, int f32, cudaStream_t st) {
   need_vec(C, f32, "relu_bias_bwd");
-  if (f32) relu_bias_bwd_t<float>(dy, y, dym, db, db1, c_split, R, C, ld, act, slope, st);
-  else relu_bias_bwd_t<__nv_bfloat16>(dy, y, dym, db, db1, c_split, R, C, ld, act, slope, st);
+  if (f32) relu_bias_bwd_t<float>(dy, y, dym, db, db1, c_split, R, C, ld, act, slope, accumulate, st);
+  else relu_bias_bwd_t<__nv_bfloat16>(dy, y, dym, db, db1, c_split, R, C, ld, act, slope, accumulate, st);
 }
 
 // y[r, c] = act(acc[r, c] (fp32) + bias[c]), stored as T — finishing pass of a split-K forward GEMM (small-batch FC layers: the
@@ -891,7 +894,7 @@ __global__ void __launch_bounds__(256) maxpool_relu_bias_bwd_kernel(const __nv_b
 }
 
 void maxpool_relu_bias_bwd(const void* dyp, const void* arg, const void* y, void* dym, void* db0, void* db1, int c_split, int N, int H,
-                           int W, int C, int Ho, int Wo, int k, int s, int p, cudaStream_t st) {
+                           int W, int C, int Ho, int Wo, int k, int s, int p, int accumulate, cudaStream_t st) {
   if (C % 8) throw std::runtime_error("maxpool_relu_bias_bwd: C must be a multiple of 8");
   if ((long long)H * W * C >= (1LL << 31)) throw std::runtime_error("maxpool_relu_bias_bwd: image too large for 32-bit in-image offsets");
   PoolGeom g{N, H, W, C, Ho, Wo, k, s, p};
@@ -901,8 +904,8 @@ void maxpool_relu_bias_bwd(const void* dyp, const void* arg, const void* y, void
   dim3 grid((unsigned)N * H, (unsigned)((nvec + VT - 1) / VT));
   const size_t smem = (size_t)RL * VT * 8 * sizeof(float);
   if (c_split > C) c_split = C;
-  check_cuda(cudaMemsetAsync(db0, 0, (size_t)c_split * 4, st), "maxpool_relu_bias_bwd memset");
-  if (c_split < C) check_cuda(cudaMemsetAsync(db1, 0, (size_t)(C - c_split) * 4, st), "maxpool_relu_bias_bwd memset");
+  if (!accumulate) check_cuda(cudaMemsetAsync(db0, 0, (size_t)c_split * 4, st), "maxpool_relu_bias_bwd memset");
+  if (!accumulate && c_split < C) check_cuda(cudaMemsetAsync(db1, 0, (size_t)(C - c_split) * 4, st), "maxpool_relu_bias_bwd memset");
   const int maxw = (k + s - 1) / s;
   auto DYP = (const __nv_bfloat16*)dyp; auto A = (const uint8_t*)arg; auto Y = (const __nv_bfloat16*)y; auto DM = (__nv_bfloat16*)dym;
   if (maxw == 1) maxpool_relu_bias_bwd_kernel<1, true><<<grid, 256, smem, st>>>(DYP, A, Y, DM, (float*)db0, (float*)db1, c_split, g, VT);
@@ -1209,7 +1212,7 @@ void space_to_depth(const void* x, void* y, int N, int H, int W, int C, int S, i
 }
 
 // w [O][KH][KW][C]  <->  ws [O][KHs][KWs][Cp]   with  ws[o, a, b, (dy*S+dx)*C + c] = w[o, S*a+dy, S*b+dx, c]  (0 outside the filter)
-// dir 0: pack the filter of storage type T (w -> ws);  dir 1: unpack the fp32 gradient (gs -> g)
+// dir 0: pack the filter of storage type T (w -> ws);  dir 1: unpack the fp32 gradient (gs -> g);  dir 2: unpack and add (g += ...)
 template <typename T>
 __global__ void s2d_filter_kernel(const void* __restrict__ src, void* __restrict__ dst, int O, int KH, int KW, int C, int S, int KHs, int KWs,
                                   int Cp, int dir) {
@@ -1234,8 +1237,9 @@ __global__ void s2d_filter_kernel(const void* __restrict__ src, void* __restrict
       const int kw = t % KW; t /= KW;
       const int kh = t % KH; const int o = t / KH;
       const int a = kh / S, dy = kh % S, b = kw / S, dx = kw % S;
-      reinterpret_cast<float*>(dst)[i] =
-          reinterpret_cast<const float*>(src)[(((long long)o * KHs + a) * KWs + b) * Cp + (dy * S + dx) * C + c];
+      const float v = reinterpret_cast<const float*>(src)[(((long long)o * KHs + a) * KWs + b) * Cp + (dy * S + dx) * C + c];
+      if (dir == 2) reinterpret_cast<float*>(dst)[i] += v;
+      else reinterpret_cast<float*>(dst)[i] = v;
     }
   }
 }

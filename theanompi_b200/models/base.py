@@ -62,6 +62,7 @@ class ModelBase(object):
     monitor_grad = False
     bias_lr_mult = 2.0             # biases train with 2x lr in the reference's optimizer (lib/opt.py:181-268)
     graph_safe = True              # False: the step draws host-side randomness / has host control flow → never auto-capture
+    supports_grad_accum = True     # config['grad_accum'] > 1 (False: the model refuses it at compile_iter_fns)
     name = "Model"
 
     def __init__(self, config):
@@ -99,6 +100,12 @@ class ModelBase(object):
         gc = config.get("grad_clip")
         self.grad_clip = None if gc is None else float(gc)
         self.clip_opt = None
+        # gradient accumulation: every optimizer step follows grad_accum micro-steps of batch_size samples whose mean gradient builds
+        # up in the arena's G region (forward_backward; checked by check_grad_accum)
+        self.grad_accum = config.get("grad_accum", 1)
+        self.n_updates = 0             # optimizer steps taken (windows completed)
+        self.n_discarded = 0           # micro-steps of windows still open at reset_iter('train'), whose gradients were dropped
+        self._micro = 0                # micro-steps done in the open window
         self.base_lr = np.float32(self.learning_rate)
         self.current_t = self.subb_t = 0
         self.current_v = self.subb_v = 0
@@ -188,6 +195,9 @@ class ModelBase(object):
         else:
             self.x_in.copy_(self.shared_x[subb_ind * B:(subb_ind + 1) * B], non_blocking=True)
             self.y_in.copy_(self.shared_y[subb_ind * B:(subb_ind + 1) * B], non_blocking=True)
+        if self.grad_accum > 1:
+            return self._micro_step()
+        self.n_updates += 1
         if not self.use_graph:
             return self._step_body()
         if self._graph is None:
@@ -238,6 +248,75 @@ class ModelBase(object):
             self._dbg_capture("step tail")
         self._after_step()
         return out
+
+    # ------------------------------------------------------------------ gradient accumulation
+    def micro_step_kind(self):
+        """Kind of the next micro-step of a ``grad_accum`` = n window: 'first' (the backward stores G), 'mid' (it adds into G) or
+        'last' (it adds into G, then the step tail updates the weights).  n = 2 has no 'mid'."""
+        if self._micro == 0:
+            return "first"
+        return "last" if self._micro == self.grad_accum - 1 else "mid"
+
+    def _micro_step(self):
+        """One micro-step on the input buffers: with graphs, a replay of the CUDA graph captured for its kind (the three kinds share
+        one graph pool); a capture that fails under ``cuda_graph='auto'`` falls back to eager steps."""
+        kind = self.micro_step_kind()
+        out = None
+        if self.use_graph:
+            try:
+                out = self.run_keyed_step(("grad_accum", kind), lambda: self._accum_body(kind))
+            except Exception as e:  # noqa: BLE001
+                if not self._graph_auto:
+                    raise
+                print("[%s] CUDA-graph capture of the %s micro-step failed (%s: %s) — running eager"
+                      % (getattr(self, "name", type(self).__name__), kind, type(e).__name__, str(e)[:200]))
+                self.use_graph = False
+                self._drop_accum_graphs()
+                torch.cuda.synchronize()
+        if out is None:
+            out = self._accum_body(kind)
+        self._micro += 1
+        if kind == "last":
+            self._micro = 0
+            self.n_updates += 1
+        return out
+
+    def _accum_body(self, kind):
+        """Forward + backward of one micro-step under the accumulate switch (ops.accum): G is stored by 'first' and added to by
+        'mid' / 'last', the loss gradient carries 1/n; the step tail runs after 'last' only."""
+        with ops.accum.mode(kind != "first", float(np.float32(1.0 / self.grad_accum))):
+            out = self._fwd_bwd_eager()
+        self._dbg_capture("forward+backward (%s micro-step)" % kind)
+        if kind == "last" and self._tail is not None:
+            with torch.no_grad():
+                self._tail()
+            self._dbg_capture("step tail")
+        self._after_step()
+        return out
+
+    def _drop_accum_graphs(self):
+        self._graphs = {k: v for k, v in self._graphs.items() if not (isinstance(k, tuple) and k[0] == "grad_accum")}
+
+    def check_grad_accum(self, fused_tail=None):
+        """Refuse ``grad_accum`` > 1 where it is not implemented: models without it (the LSTM, the GANs, the torch twins), more than
+        one worker (BSP, EASGD, GOSGD: the exchange would have to wait for the end of a window) and a fused exchange strategy's
+        ``fused_tail`` (its bucket launches fire during every backward)."""
+        n = self.grad_accum
+        if isinstance(n, bool) or not isinstance(n, (int, np.integer)) or n < 1:
+            raise ValueError("%s: grad_accum must be an int >= 1, not %r" % (self.name, n))
+        self.grad_accum = n = int(n)
+        if n == 1:
+            return
+        supported = ("grad_accum > 1 runs on one worker (size = 1) with a local optimizer step: AlexNet, GoogLeNet, Cifar10_model, "
+                     "VGG16, ResNet50 and Wide_ResNet, with optimizer 'sgd', 'lars', 'lamb' or Wide_ResNet's 'adam', and grad_clip")
+        if not self.supports_grad_accum:
+            raise ValueError("%s does not accumulate gradients (grad_accum = %d); %s" % (self.name, n, supported))
+        if self.size > 1:
+            raise ValueError("%s: grad_accum = %d with %d workers is not implemented: the exchange would have to happen once per "
+                             "window; %s" % (self.name, n, self.size, supported))
+        if fused_tail is not None:
+            raise ValueError("%s: grad_accum = %d does not combine with a fused exchange strategy, whose bucket launches fire during "
+                             "every backward; %s" % (self.name, n, supported))
 
     def _dbg_capture(self, where):
         """TMPI_DEBUG_CAPTURE=1: name the stage that invalidated an ongoing CUDA-graph capture."""
@@ -318,6 +397,7 @@ class ModelBase(object):
         self._tail = fn
         self._graph = None
         self._warm = 0
+        self._drop_accum_graphs()
 
     def compile_val(self):
         def val_fn(subb_ind=0):
@@ -355,6 +435,7 @@ class ModelBase(object):
         (see :meth:`check_grad_clip`)."""
         if self.optimizer not in ("sgd", "lars", "lamb"):
             raise ValueError("%s: optimizer must be 'lamb', 'sgd' or 'lars', not %r" % (self.name, self.optimizer))
+        self.check_grad_accum(fused_tail)
         k = self.size if sync_type == "cdd" else 1
         if self.optimizer in ("lars", "lamb") and fused_tail is not None:
             raise ValueError("optimizer=%r needs every tensor's whole reduced gradient before its update; the fused exchange "
@@ -432,6 +513,10 @@ class ModelBase(object):
         if mode == "train":
             self.current_t = self.subb_t = 0
             self.last_one_t = False
+            # a gradient-accumulation window still open at the end of the epoch is dropped: the next micro-step is a 'first' again,
+            # which overwrites G
+            self.n_discarded += self._micro
+            self._micro = 0
         else:
             self.current_v = self.subb_v = 0
             self.last_one_v = False

@@ -157,6 +157,7 @@ class Wide_ResNet(ModelBase):
         if sync_type != "avg" and self.size > 1:
             raise ValueError("Wide_ResNet trains with Adam: only sync_type='avg' is supported (as in the reference, wresnet.py:152-153)")
         self.check_grad_clip(optimizer="adam")
+        self.check_grad_accum(fused_tail)
         from ...utils.opt import FlatAdam
         self.sync_type = "avg"
         self.adam = FlatAdam(self.arena)

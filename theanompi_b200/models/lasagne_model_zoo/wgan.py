@@ -97,6 +97,7 @@ class WGAN(TorchModelBase):
 
     def compile_iter_fns(self, sync_type="avg", **kw):
         self.refuse_grad_clip()
+        self.check_grad_accum()
         self.sync_type = "avg"
         self.opt_c = torch.optim.RMSprop(self.critic_params, lr=self.learning_rate)
         self.opt_g = torch.optim.RMSprop(self.generator_params, lr=self.learning_rate)
@@ -232,6 +233,7 @@ class NativeWGAN(ModelBase):
     ‖g‖^½; here it is on the true norm.  On a non-finite norm the reference substitutes g = 0.1·W; here the step is skipped and
     ``opt_c.skipped`` / ``opt_g.skipped`` count it.  The reference's CIFAR-10 LSGAN uses plain RMSProp without rescaling, so there
     ``grad_clip`` is simply available."""
+    supports_grad_accum = False    # its critic / generator steps keep their own gaccum accumulation
     loss_kind = "wgan"
     n_epochs = num_epochs
     batch_size = file_batch_size = batchsize
@@ -387,6 +389,7 @@ class NativeWGAN(ModelBase):
 
     # ---- contract
     def compile_iter_fns(self, sync_type="avg", **kw):
+        self.check_grad_accum()
         self.sync_type = "avg"
         self.vels, self.vels2 = [], []
         self.train_iter_fn = self.val_iter_fn = None

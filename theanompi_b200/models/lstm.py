@@ -109,6 +109,7 @@ class LSTM(ModelBase):
     sequence-length bucket (:func:`bucket_len`): the batch is padded to its bucket, copied into the bucket's static buffers and
     the bucket's graph (forward, backward, update) is replayed.  ``cuda_graph=False`` and the CPU run the step eagerly on the
     unpadded batch; validation is always eager."""
+    supports_grad_accum = False    # one graph per sequence-length bucket, each with its own update
     n_epochs = max_epochs
     batch_size = file_batch_size = batch_size
     learning_rate = 1.0
@@ -183,6 +184,7 @@ class LSTM(ModelBase):
 
     def compile_iter_fns(self, sync_type="avg", **kw):
         self.check_grad_clip()
+        self.check_grad_accum()
         self.sync_type = "avg"
         self._make_opt()
         self.vels, self.vels2 = [], []
@@ -318,6 +320,7 @@ class LSTMTorch(TorchModelBase):
 
     def compile_iter_fns(self, sync_type="avg", **kw):
         self.refuse_grad_clip()
+        self.check_grad_accum()
         self.sync_type = "avg"
         self.torch_opt = self.make_torch_optimizer(self.params)
         self.vels, self.vels2 = [], []

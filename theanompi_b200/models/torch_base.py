@@ -41,6 +41,7 @@ def tag_module_params(module):
 class TorchModelBase(ModelBase):
     optimizer_name = "flat_sgd"
     autocast = True
+    supports_grad_accum = False    # torch autograd writes .grad: the native accumulate mode does not reach it
 
     def finalize_torch(self, module, input_shape, exchanged=None):
         self.module = module.to(self.device)
@@ -108,6 +109,7 @@ class TorchModelBase(ModelBase):
 
     def compile_iter_fns(self, sync_type="avg", aggregate="momentum", fused_tail=None):
         self.refuse_grad_clip()
+        self.check_grad_accum(fused_tail)
         self.torch_opt = self.make_torch_optimizer(self.params)
         if self.torch_opt is None:
             return super().compile_iter_fns(sync_type, aggregate, fused_tail)

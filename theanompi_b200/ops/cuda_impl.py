@@ -10,6 +10,11 @@ transposed copies unnecessary:
     dgrad     dx = dy · W        A = dy  (K-major)   B = W   (MN-major)               → bf16
     wgrad     dW = dyᵀ · x       A = dy  (MN-major)  B = x   (MN-major)  split-K      → fp32 (straight into the arena's G)
 
+Gradient accumulation (:mod:`.accum`): while the switch is on, every kernel that writes a parameter gradient into an arena G view
+adds into it instead (GEMM / implicit-conv wgrad through the epilogue's fp32 reductions, bias and batch-norm gradients without their
+clears).  A gradient of a parameter without a G view goes to a fresh scratch buffer, which is stored into as without the switch
+(``functional._sink`` then adds it into its destination).
+
 Everything raises if the extension is missing — there is no eager fallback on a GPU.
 """
 from __future__ import annotations
@@ -18,7 +23,7 @@ import os
 
 import torch
 
-from . import native, precision
+from . import accum, native, precision
 
 _STEP = {}          # device index -> int64[1] step counter used by the dropout Philox stream
 BF16 = torch.bfloat16
@@ -60,6 +65,21 @@ def _p(t):
     return 0 if t is None else t.data_ptr()
 
 
+def _acc(*outs):
+    """1 while the backward accumulates (:mod:`.accum`) and one of ``outs`` — the parameter-gradient outputs of one launch — is a G
+    view, so the launch adds; else 0 (the launch stores)."""
+    return int(accum.accumulating() and any(o is not None for o in outs))
+
+
+def grad_buffer(shape, out=None, device=None, acc=0):
+    """``out`` (a parameter's gradient view in the arena), else a fresh fp32 scratch buffer: uninitialised, since the launch stores
+    into it, or zeros when ``acc`` — the launch that writes it also adds into another output that is a G view (two parameter sets
+    in one launch, only one of them with a view)."""
+    if out is not None:
+        return out
+    return (torch.zeros if acc else torch.empty)(shape, dtype=torch.float32, device=device)
+
+
 def step_counter(device):
     idx = torch.device(device).index
     if idx is None:
@@ -96,9 +116,10 @@ def _rows8(t2d):
 
 # --------------------------------------------------------------------------- GEMM
 def gemm(a, b, M, N, K, a_mn=False, b_mn=False, out=None, out_dtype=None, bias=None, bias_mode=0,
-         relu=False, alpha=1.0, lda=None, ldb=None, ldc=None, bn=0, splitk=0):
+         relu=False, alpha=1.0, lda=None, ldb=None, ldc=None, bn=0, splitk=0, accumulate=False):
     """``out[M,N] = alpha * op(a) @ op(b) (+bias)(ReLU)``; ``a``/``b`` are bf16 tensors whose
-    storage is described by (major flag, leading dimension)."""
+    storage is described by (major flag, leading dimension).  ``accumulate``: ``out += alpha * op(a) @ op(b)`` (fp32 ``out``, no
+    bias / ReLU)."""
     dev = a.device
     tf32 = _is32(a)
     assert a.dtype == b.dtype, "GEMM operands must share a dtype"
@@ -108,9 +129,11 @@ def gemm(a, b, M, N, K, a_mn=False, b_mn=False, out=None, out_dtype=None, bias=N
         ldc = out.stride(0) if out.dim() == 2 else N
     if bias is not None:
         assert bias.dtype == torch.float32
+    if accumulate:
+        assert out.dtype == torch.float32 and bias is None and not relu, "an accumulating GEMM adds an fp32 product into out"
     L().gemm(a.data_ptr(), b.data_ptr(), out.data_ptr(), _p(bias), int(M), int(N), int(K), int(lda), int(ldb),
              int(ldc), int(bool(a_mn)), int(bool(b_mn)), int(out.dtype == BF16), int(bias_mode), int(bool(relu)),
-             float(alpha), int(bn), int(splitk), int(tf32), _st(a))
+             float(alpha), int(bn), int(splitk), int(tf32), _st(a), int(bool(accumulate)))
     return out
 
 
@@ -135,26 +158,29 @@ def linear_bias_act(x, w, b, relu=True):
     return gemm(xa, wa, B_, O, I, bias=bias, bias_mode=1 if b is not None else 0, relu=relu, lda=lda, ldb=ldb)
 
 
-def _mask_and_bias_grad(dy, y, relu, db_out, R, C, ld, need_db=True):
-    """dym = dy ⊙ act'(y) (ReLU: dy ⊙ (y > 0); contiguous [R, C]) and db = Σ_rows dym in one pass."""
+def _mask_and_bias_grad(dy, y, relu, db_out, R, C, ld, need_db=True, acc=None):
+    """dym = dy ⊙ act'(y) (ReLU: dy ⊙ (y > 0); contiguous [R, C]) and db = Σ_rows dym in one pass.  ``acc``: add into ``db_out``
+    (default: while accumulating, when ``db_out`` is a G view)."""
     dev = dy.device
     act = _act(relu)
     if not need_db and not act and ld == C:
         return dy, None                                    # bias-free linear conv (a BatchNormal follows): nothing to do
-    db = db_out if db_out is not None else torch.empty(C, dtype=torch.float32, device=dev)
+    acc = _acc(db_out) if acc is None else int(acc)
+    db = grad_buffer(C, db_out, dev)
     if act or ld != C:
         dym = torch.empty((R, C), dtype=dy.dtype, device=dev)
         L().relu_bias_bwd(dy.data_ptr(), _p(y), dym.data_ptr(), db.data_ptr(), 0, int(C), int(R), int(C), int(ld), _act(relu), LEAKY_SLOPE,
-                          int(_is32(dy)), _st(dy))
+                          acc, int(_is32(dy)), _st(dy))
     else:
         dym = dy
-        L().relu_bias_bwd(dy.data_ptr(), 0, 0, db.data_ptr(), 0, int(C), int(R), int(C), int(ld), 0, 0.0, int(_is32(dy)), _st(dy))
+        L().relu_bias_bwd(dy.data_ptr(), 0, 0, db.data_ptr(), 0, int(C), int(R), int(C), int(ld), 0, 0.0, acc, int(_is32(dy)), _st(dy))
     return dym, db
 
 
-def maxpool_relu_bias_bwd(dyp, arg, y, pool, db0, db1=None):
+def maxpool_relu_bias_bwd(dyp, arg, y, pool, db0, db1=None, accumulate=False):
     """Backward of conv(+ReLU)→max-pool up to the conv's masked output gradient, in one kernel: scatter the pooled
-    gradient through the argmax, apply the ReLU mask, accumulate the bias gradient(s).  Returns dym, shaped like y."""
+    gradient through the argmax, apply the ReLU mask, reduce the bias gradient(s) into ``db0`` (/ ``db1``), or add it there with
+    ``accumulate``.  Returns dym, shaped like y."""
     dyp = _bf(dyp).contiguous()
     N, H, W, C = y.shape
     Ho, Wo = dyp.shape[1], dyp.shape[2]
@@ -162,7 +188,7 @@ def maxpool_relu_bias_bwd(dyp, arg, y, pool, db0, db1=None):
     dym = torch.empty((N, H, W, C), dtype=BF16, device=y.device)
     c_split = C if db1 is None else int(db0.numel())
     L().maxpool_relu_bias_bwd(dyp.data_ptr(), arg.data_ptr(), y.data_ptr(), dym.data_ptr(), db0.data_ptr(), _p(db1), c_split,
-                              N, H, W, C, Ho, Wo, k, s_, p_, _st(y))
+                              N, H, W, C, Ho, Wo, k, s_, p_, int(bool(accumulate)), _st(y))
     return dym
 
 
@@ -188,6 +214,9 @@ def linear_bias_act_bwd(x, w, y, dy, relu, need_dx, dw_out=None, db_out=None, sg
     B_, I = x2.shape
     O = w.shape[0]
     al = _al(x2)
+    if sgd_param is not None and accum.accumulating():
+        raise RuntimeError("linear_bias_act_bwd: weight %s is armed for the GEMM SGD epilogue, which does not accumulate gradients"
+                           % (tuple(w.shape),))
     if O % al or I % al:
         if sgd_param is not None:
             raise RuntimeError("linear_bias_act_bwd: weight %s is armed for the GEMM SGD epilogue but needs the padded path"
@@ -202,13 +231,14 @@ def linear_bias_act_bwd(x, w, y, dy, relu, need_dx, dw_out=None, db_out=None, sg
         # after the dx GEMM, which reads the weights of this step
         gemm_sgd(dym, x2, sgd_param, O, I, B_, lda=O, ldb=I)
         return dx, None, db
-    dw = dw_out if dw_out is not None else torch.empty((O, I), dtype=torch.float32, device=x.device)
-    gemm(dym, x2, O, I, B_, a_mn=True, b_mn=True, out=dw, lda=O, ldb=I, ldc=I)
+    dw = grad_buffer((O, I), dw_out, x.device)
+    gemm(dym, x2, O, I, B_, a_mn=True, b_mn=True, out=dw, lda=O, ldb=I, ldc=I, accumulate=_acc(dw_out))
     return dx, dw, db
 
 
 def _linear_bwd_padded(x2, w, y, dy, relu, need_dx, dw_out, db_out):
-    """Shapes whose pitches violate the 16-byte TMA rule (e.g. a 10-class test head): pad to 8."""
+    """Shapes whose pitches violate the 16-byte TMA rule (e.g. a 10-class test head): pad to 8.  The padded product goes to a
+    scratch buffer, so an accumulating backward adds it into the gradient views afterwards."""
     B_, I = x2.shape
     O = w.shape[0]
     Op, Ip = (O + 7) // 8 * 8, (I + 7) // 8 * 8
@@ -224,10 +254,11 @@ def _linear_bwd_padded(x2, w, y, dy, relu, need_dx, dw_out, db_out):
     dwp = torch.empty((Op, Ip), dtype=torch.float32, device=dev)
     gemm(dyp, xp, Op, Ip, B_, a_mn=True, b_mn=True, out=dwp, lda=Op, ldb=Ip, ldc=Ip)
     dw = dwp[:O, :I]
+    acc = accum.accumulating()
     if dw_out is not None:
-        dw_out.copy_(dw); dw = dw_out
+        (dw_out.add_ if acc else dw_out.copy_)(dw); dw = dw_out
     if db_out is not None:
-        db_out.view(-1).copy_(db); db = db_out
+        (db_out.view(-1).add_ if acc else db_out.view(-1).copy_)(db); db = db_out
     return dx, dw, db
 
 
@@ -337,9 +368,10 @@ def _conv_s2d_bwd(xs, w, y, dy, relu, g, dw_out, db_out, pre_masked=False):
         dym, db = _mask_and_bias_grad(dy.view(M, O), y.view(M, O), relu, db_out.view(-1) if db_out is not None else None, M, O, O)
     dws = torch.empty((O, KHs, KWs, Cp), dtype=torch.float32, device=dev)
     f32 = int(_is32(xs))
-    L().conv_wgrad(dym.data_ptr(), xs.data_ptr(), dws.data_ptr(), N, Hs, Ws, Cp, 0, Cp, KHs, KWs, Ho, Wo, 1, 0, O, O, f32, _st(xs))
-    dw = dw_out if dw_out is not None else torch.empty((O, KH, KW, C), dtype=torch.float32, device=dev)
-    L().s2d_filter(dws.data_ptr(), dw.data_ptr(), O, KH, KW, C, S, KHs, KWs, Cp, 1, f32, _st(xs))
+    L().conv_wgrad(dym.data_ptr(), xs.data_ptr(), dws.data_ptr(), N, Hs, Ws, Cp, 0, Cp, KHs, KWs, Ho, Wo, 1, 0, O, O, 0, f32, _st(xs))
+    dw = grad_buffer((O, KH, KW, C), dw_out, dev)
+    # the space-to-depth gradient is scratch: it is stored, and the unpack adds it into dw while the backward accumulates
+    L().s2d_filter(dws.data_ptr(), dw.data_ptr(), O, KH, KW, C, S, KHs, KWs, Cp, 2 if _acc(dw_out) else 1, f32, _st(xs))
     return dw, db
 
 
@@ -405,7 +437,11 @@ def conv2d_group2_bias_act(x, w0, b0, w1, b1, stride, pad, relu, return_cols=Fal
     return (y, cols) if return_cols else y
 
 
-def _conv_bwd_group(x, w, y, dy, dx, o_off, c_off, Cg, s, p, relu, need_dx, dw_out, db_out, col=None, pre_masked=False, need_db=True):
+def _conv_bwd_group(x, w, y, dy, dx, o_off, c_off, Cg, s, p, relu, need_dx, dw_out, db_out, col=None, pre_masked=False, need_db=True,
+                    acc_w=None, acc_b=None):
+    """``acc_w`` / ``acc_b``: add the weight / bias gradient into ``dw_out`` / ``db_out`` (default: while accumulating, when the
+    output is a G view)."""
+    acc_w = _acc(dw_out) if acc_w is None else int(acc_w)
     N, H, W, Ct = x.shape
     Og, KH, KW, _ = w.shape
     Ho, Wo, Ot = y.shape[1], y.shape[2], y.shape[3]
@@ -418,16 +454,16 @@ def _conv_bwd_group(x, w, y, dy, dx, o_off, c_off, Cg, s, p, relu, need_dx, dw_o
         # group's channel slice of the full tensor in place (row pitch Ot)
         dym, db, ldy, dy_coff = dyv, db_out, Ot, o_off
     else:
-        dym, db = _mask_and_bias_grad(dyv, yv, relu, db_out.view(-1) if db_out is not None else None, M, Og, Ot, need_db)
+        dym, db = _mask_and_bias_grad(dyv, yv, relu, db_out.view(-1) if db_out is not None else None, M, Og, Ot, need_db, acc=acc_b)
         ldy, dy_coff = Og, 0
     wb = _bf(w)
     if col is None and _implicit_ok(x, wb, c_off, Cg, Ot, o_off):
         # ---- implicit GEMM backward: wgrad gathers im2col(x) by TMA; dgrad (stride 1) is a forward conv of dy with the
         # flipped / transposed filter, written straight into dx's channel slice.
-        dw = dw_out if dw_out is not None else torch.empty((Og, KH, KW, Cg), dtype=torch.float32, device=dev)
+        dw = grad_buffer((Og, KH, KW, Cg), dw_out, dev)
         es, f32 = x.element_size(), int(_is32(x))
         L().conv_wgrad(dym.data_ptr(), x.data_ptr(), dw.data_ptr(), N, H, W, Ct, int(c_off), int(Cg), KH, KW, Ho, Wo, int(s), int(p),
-                       Og, int(ldy), f32, _st(x))
+                       Og, int(ldy), acc_w, f32, _st(x))
         if need_dx:
             if s == 1:
                 # dgrad = forward conv of dy with the mirrored, transposed filter — which the kernel's TMA loads read straight
@@ -441,9 +477,9 @@ def _conv_bwd_group(x, w, y, dy, dx, o_off, c_off, Cg, s, p, relu, need_dx, dw_o
                 L().col2im(dcol.data_ptr(), dx.data_ptr(), N, H, W, Ct, int(c_off), int(Cg), KH, KW, Ho, Wo, int(s), int(p), Kp, f32, _st(x))
         return dw, db
     col, Kp, K = col if col is not None else _im2col(x, c_off, Cg, KH, KW, Ho, Wo, s, p)   # forward's matrix is reused
-    dw = dw_out if dw_out is not None else torch.empty((Og, KH, KW, Cg), dtype=torch.float32, device=dev)
+    dw = grad_buffer((Og, KH, KW, Cg), dw_out, dev)
     # wgrad: dW[Og, K] = dymᵀ[Og, M] · col[M, K]   (both operands MN-major, split-K over M)
-    gemm(dym, col, Og, K, M, a_mn=True, b_mn=True, out=dw.view(Og, K), lda=ldy, ldb=Kp, ldc=K)
+    gemm(dym, col, Og, K, M, a_mn=True, b_mn=True, out=dw.view(Og, K), lda=ldy, ldb=Kp, ldc=K, accumulate=acc_w)
     if need_dx:
         w2 = _w2d(w, K, Kp)
         one_by_one = (KH == 1 and KW == 1 and s == 1 and p == 0 and c_off == 0 and Cg == Ct)
@@ -475,11 +511,13 @@ def conv2d_bias_act_bwd(x, w, y, dy, stride, pad, groups, relu, need_dx, dw_out=
         dw, db = _conv_bwd_group(x, w, y, dy, dx, 0, 0, Cg, stride, pad, relu, need_dx, dw_out, db_out,
                                  col=cols[0] if cols else None, pre_masked=pre_masked, need_db=need_db)
         return dx, dw, db
-    dw = dw_out if dw_out is not None else torch.empty(tuple(w.shape), dtype=torch.float32, device=x.device)
-    db = db_out if db_out is not None else torch.empty(O, dtype=torch.float32, device=x.device)
+    acc_w, acc_b = _acc(dw_out), _acc(db_out)
+    dw = grad_buffer(tuple(w.shape), dw_out, x.device)
+    db = grad_buffer(O, db_out, x.device)
     for g in range(groups):
         _conv_bwd_group(x, w[g * Og:(g + 1) * Og], y, dy, dx, g * Og, g * Cg, Cg, stride, pad, relu, need_dx,
-                        dw[g * Og:(g + 1) * Og], db[g * Og:(g + 1) * Og], col=cols[g] if cols else None, pre_masked=pre_masked)
+                        dw[g * Og:(g + 1) * Og], db[g * Og:(g + 1) * Og], col=cols[g] if cols else None, pre_masked=pre_masked,
+                        acc_w=acc_w, acc_b=acc_b)
     return dx, dw, db
 
 
@@ -500,19 +538,19 @@ def conv2d_group2_bias_act_bwd(x, w0, w1, y, dy, stride, pad, relu, need_dx, out
         Ho, Wo = y.shape[1], y.shape[2]
         M = N * Ho * Wo
         dev = x.device
-        db0 = outs[1] if outs[1] is not None else torch.empty(Og, dtype=torch.float32, device=dev)
-        db1 = outs[3] if outs[3] is not None else torch.empty(Og, dtype=torch.float32, device=dev)
+        # one launch writes both groups' bias (weight) gradients: it adds when either output is a G view
+        acc_b, acc_w = _acc(outs[1], outs[3]), _acc(outs[0], outs[2])
+        db0, db1 = grad_buffer(Og, outs[1], dev, acc_b), grad_buffer(Og, outs[3], dev, acc_b)
         es, f32 = x.element_size(), int(_is32(x))
         if pre_masked:
             dym = dy
         else:
             dym = torch.empty((M, Ot), dtype=x.dtype, device=dev)
             L().relu_bias_bwd(dy.data_ptr(), y.data_ptr(), dym.data_ptr(), db0.data_ptr(), db1.data_ptr(), int(Og), int(M), int(Ot), int(Ot),
-                              _act(relu), LEAKY_SLOPE, f32, _st(x))
-        dw0 = outs[0] if outs[0] is not None else torch.empty((Og, KH, KW, Cg), dtype=torch.float32, device=dev)
-        dw1 = outs[2] if outs[2] is not None else torch.empty((Og, KH, KW, Cg), dtype=torch.float32, device=dev)
+                              _act(relu), LEAKY_SLOPE, acc_b, f32, _st(x))
+        dw0, dw1 = grad_buffer((Og, KH, KW, Cg), outs[0], dev, acc_w), grad_buffer((Og, KH, KW, Cg), outs[2], dev, acc_w)
         L().conv_wgrad2(dym.data_ptr(), dym.data_ptr() + Og * es, x.data_ptr(), dw0.data_ptr(), dw1.data_ptr(), N, H, W, Ct, 0, int(Cg), int(Cg),
-                        KH, KW, Ho, Wo, int(stride), int(pad), Og, int(Ot), f32, _st(x))
+                        KH, KW, Ho, Wo, int(stride), int(pad), Og, int(Ot), acc_w, f32, _st(x))
         if need_dx:
             L().conv_fprop2(dym.data_ptr(), wb0.data_ptr(), wb1.data_ptr(), dx.data_ptr(), dx.data_ptr() + Cg * es, 0, 0, N, Ho, Wo, int(Ot), 0,
                             int(Og), int(Og), KH, KW, H, W, 1, KH - 1 - int(pad), int(Cg), Ct, 0, 1, f32, _st(x))
@@ -629,7 +667,9 @@ def dropout_bwd(dy, mask):
     return dx
 
 
-def softmax_xent(logits, labels, weight=1.0):
+def softmax_xent(logits, labels, weight=1.0, grad_scale=1.0):
+    """(weight · mean NLL, top-1 error, top-5 error, dlogits); dlogits is the gradient of the mean NLL times weight · grad_scale
+    (``grad_scale`` = 1/n under gradient accumulation over n micro-batches), scaled in fp32 inside the kernel."""
     lg = _bf(logits).contiguous()
     B_, C = lg.shape
     labels = labels.contiguous()
@@ -638,7 +678,7 @@ def softmax_xent(logits, labels, weight=1.0):
     rowstat = torch.empty((B_, 3), dtype=torch.float32, device=lg.device)
     out3 = torch.empty(3, dtype=torch.float32, device=lg.device)
     L().softmax_xent(lg.data_ptr(), labels.data_ptr(), dl.data_ptr(), rowstat.data_ptr(), out3.data_ptr(), B_, C, float(weight),
-                     int(_is32(lg)), _st(lg))
+                     float(weight) * float(grad_scale), int(_is32(lg)), _st(lg))
     return out3[0], out3[1], out3[2], dl
 
 
@@ -690,12 +730,14 @@ def batch_norm_bwd(x, dy, y, gamma, mean, rstd, relu, need_dres, dgamma_out=None
     dx = torch.empty_like(x)
     # without a ReLU the residual branch receives dy itself: nothing to write
     dres = torch.empty_like(x) if (need_dres and relu) else None
-    dgamma = dgamma_out.view(-1) if dgamma_out is not None else torch.empty(C, dtype=F32, device=dev)
-    dbeta = dbeta_out.view(-1) if dbeta_out is not None else torch.empty(C, dtype=F32, device=dev)
-    scratch = torch.empty(3 * C, dtype=F32, device=dev)
+    acc = _acc(dgamma_out, dbeta_out)
+    dgamma = grad_buffer(C, dgamma_out.view(-1) if dgamma_out is not None else None, dev, acc)
+    dbeta = grad_buffer(C, dbeta_out.view(-1) if dbeta_out is not None else None, dev, acc)
+    # accumulating: the batch's Σg, Σg·x̂ go to the scratch (the dx coefficients need them, not the running totals in G)
+    scratch = torch.empty((5 if acc else 3) * C, dtype=F32, device=dev)
     L().bn_backward(x.data_ptr(), dy.data_ptr(), _p(y) if relu else 0, dx.data_ptr(), _p(dres), gamma.data_ptr(), mean.data_ptr(),
                     rstd.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), scratch.data_ptr(), int(R), int(C), _act(relu), LEAKY_SLOPE,
-                    int(_is32(x)), _st(x))
+                    acc, int(_is32(x)), _st(x))
     if need_dres and not relu:
         dres = dy
     return dx, dres, dgamma, dbeta

@@ -13,6 +13,8 @@ fp32 gradient straight into it and then fires ``on_ready`` — that callback is
 what lets the BSP exchanger launch the fused allreduce+SGD kernel for a bucket
 on a side stream while backward is still running on the main stream
 (the reference is strictly sequential, ``theanompi/worker.py:94-97``).
+
+Under gradient accumulation (:mod:`.accum`) the kernels add into those views and the CPU path adds in :func:`_sink`.
 """
 from __future__ import annotations
 
@@ -20,6 +22,7 @@ import torch
 
 import os
 
+from . import accum
 from . import reference as ref
 
 CACHE_COL = os.environ.get("TMPI_CACHE_COL", "1") != "0"
@@ -46,7 +49,7 @@ def _sink(p, grad):
     if gbuf is None:
         return grad.to(p.dtype).view_as(p)
     if grad is not None and grad.data_ptr() != gbuf.data_ptr():
-        if getattr(p, "gaccum", False):
+        if getattr(p, "gaccum", False) or accum.accumulating():
             gbuf.add_(grad.view_as(gbuf))
         else:
             gbuf.copy_(grad.view_as(gbuf))
@@ -159,9 +162,9 @@ class _ConvFn(torch.autograd.Function):
             db_out = _gout(b)
             if pool is not None:
                 if _fused_pool_ok(x, relu, pool) and ctx.has_arg:
-                    if db_out is None:
-                        db_out = torch.empty(b.numel(), dtype=torch.float32, device=x.device)
-                    dy = impl.maxpool_relu_bias_bwd(dy, ctx.saved_tensors[2], y, pool, db_out, None)
+                    acc = impl._acc(db_out)
+                    db_out = impl.grad_buffer(b.numel(), db_out, x.device)
+                    dy = impl.maxpool_relu_bias_bwd(dy, ctx.saved_tensors[2], y, pool, db_out, None, accumulate=acc)
                     pre = True
                 else:
                     dy = impl.pool2d_bwd_arg(dy, ctx.saved_tensors[2] if ctx.has_arg else None, tuple(y.shape), *pool)
@@ -240,11 +243,9 @@ class _ConvG2Fn(torch.autograd.Function):
             db0, db1 = _gout(b0), _gout(b1)
             if pool is not None:
                 if _fused_pool_ok(x, relu, pool) and ctx.has_arg:
-                    if db0 is None:
-                        db0 = torch.empty(b0.numel(), dtype=torch.float32, device=x.device)
-                    if db1 is None:
-                        db1 = torch.empty(b1.numel(), dtype=torch.float32, device=x.device)
-                    dy = impl.maxpool_relu_bias_bwd(dy, ctx.saved_tensors[2], y, pool, db0, db1)
+                    acc = impl._acc(db0, db1)
+                    db0, db1 = impl.grad_buffer(b0.numel(), db0, x.device, acc), impl.grad_buffer(b1.numel(), db1, x.device, acc)
+                    dy = impl.maxpool_relu_bias_bwd(dy, ctx.saved_tensors[2], y, pool, db0, db1, accumulate=acc)
                     pre = True
                 else:
                     dy = impl.pool2d_bwd_arg(dy, ctx.saved_tensors[2] if ctx.has_arg else None, tuple(y.shape), *pool)
@@ -485,7 +486,8 @@ def dropout(x, p_drop, training, layer_id=0):
 class _SoftmaxXentFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, logits, labels):
-        loss, err1, err5, dlogits = _impl(logits).softmax_xent(logits, labels)
+        # under gradient accumulation over n micro-batches dlogits carries 1/n (in fp32, inside the kernel); the loss does not
+        loss, err1, err5, dlogits = _impl(logits).softmax_xent(logits, labels, grad_scale=accum.grad_scale())
         ctx.save_for_backward(dlogits)
         ctx.in_dtype = logits.dtype
         ctx.mark_non_differentiable(err1, err5)

@@ -173,9 +173,9 @@ def dropout(x, p_drop, mask):
 
 
 # --------------------------------------------------------------------------- softmax + NLL
-def softmax_xent(logits, labels):
-    """mean NLL, top-1 error, top-5 error, and d(mean NLL)/dlogits
-    (ref ``layers2.py:952-997``)."""
+def softmax_xent(logits, labels, grad_scale=1.0):
+    """mean NLL, top-1 error, top-5 error, and d(mean NLL)/dlogits times ``grad_scale`` (1/n under gradient accumulation over n
+    micro-batches) (ref ``layers2.py:952-997``)."""
     lg = logits.float()
     lsm = F.log_softmax(lg, dim=1)
     B = lg.shape[0]
@@ -188,6 +188,8 @@ def softmax_xent(logits, labels):
     dlogits = lsm.exp()
     dlogits[torch.arange(B, device=lg.device), labels] -= 1.0
     dlogits = dlogits / B
+    if grad_scale != 1.0:
+        dlogits = dlogits * grad_scale
     return loss, err1, err5, dlogits
 
 

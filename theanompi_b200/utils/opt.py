@@ -202,7 +202,8 @@ class FlatSGD(FlatOptimizer):
     :meth:`arm` (single GPU, k = 1) moves the update of the FC / Softmax weights into the epilogue of their weight-gradient GEMM
     (``cuda_impl.gemm_sgd``): their fp32 gradient is never written, and ``step(lr, 1)`` updates only the rest of the arena.  With
     gradient clipping (:meth:`FlatOptimizer.set_grad_clip`) nothing is armed: an epilogue would update its weight before the
-    global norm exists.  The clipping factor is folded into inv_k."""
+    global norm exists.  Nor with gradient accumulation (``model.grad_accum`` > 1): the epilogue would update the weight on every
+    micro-step.  The clipping factor is folded into inv_k."""
 
     rule = "sgd"
 
@@ -221,7 +222,8 @@ class FlatSGD(FlatOptimizer):
         for p in a.params:
             p.sgd_epilogue = None
         self.armed, self.rest = [], None
-        if not enable or not a.W.is_cuda or getattr(model, "monitor_grad", False) or self.max_norm is not None:
+        if (not enable or not a.W.is_cuda or getattr(model, "monitor_grad", False) or self.max_norm is not None
+                or getattr(model, "grad_accum", 1) > 1):
             return
         dt = getattr(model, "act_dtype", None)
         block = 16 // torch.empty((), dtype=dt).element_size() if dt is not None else 8
