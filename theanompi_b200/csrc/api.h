@@ -242,6 +242,20 @@ struct LambTrustArgs {
   void* trust;
 };
 void lamb_trust(const LambTrustArgs& a, cudaStream_t st);
+// Per-update learning-rate schedule, one single-thread launch: with u = *counter (uint64), write lr(u) to *lr (fp32, the arena's
+// hyper[0]) and u + 1 to *counter.  Warm-up for u < warmup: peak·(start + (1 − start)·u / warmup); after it, with
+// q = clamp((u − warmup) / (total − warmup), 0, 1): constant peak, cosine final + (peak − final)·½(1 + cos πq), poly
+// final + (peak − final)·(1 − q)^power, or multistep peak·gamma^(number of milestones ≤ u).  fp64, rounded once to fp32.
+enum LrPolicy : int { LR_CONSTANT = 0, LR_COSINE, LR_POLY, LR_MULTISTEP };
+constexpr int kMaxLrMilestones = 8;
+struct LrScheduleParams {
+  int policy;
+  int n_milestones;
+  long long warmup, total;
+  double start, peak, final_lr, power, gamma;
+  long long milestones[kMaxLrMilestones];
+};
+void lr_schedule(const LrScheduleParams& p, void* counter, void* lr, cudaStream_t st);
 void fused_allreduce_sgd(const FusedArgs& a, int algo, int max_blocks, cudaStream_t st);
 // every rank pushes the fp32 master weights of the slice it owns in the two-shot partition of [lo, hi) to all peers
 void push_master_slices(const FusedArgs& a, int max_blocks, cudaStream_t st);

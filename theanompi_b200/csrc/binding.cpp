@@ -175,6 +175,17 @@ PYBIND11_MODULE(_tmpi_native, m) {
                          std::vector<int> exch, long long n_blocks, int n_tensors, ptr_t partial, ptr_t norms, ptr_t trust, ptr_t st) {
     lamb_trust(LambTrustArgs{P(W), P(G), P(M), P(V), P(step), b1, b2, eps, inv_k, filter, P(block_tensor), P(tensor_span), P(block_group),
                              make_table(lr_mult, wd, exch), n_blocks, n_tensors, P(partial), P(norms), P(trust)}, S(st)); });
+  m.attr("LR_POLICIES") = py::dict(py::arg("constant") = (int)LR_CONSTANT, py::arg("cosine") = (int)LR_COSINE,
+                                    py::arg("poly") = (int)LR_POLY, py::arg("multistep") = (int)LR_MULTISTEP);
+  m.def("lr_schedule", [](int policy, long long warmup, long long total, double start, double peak, double final_lr, double power,
+                          double gamma, std::vector<long long> milestones, ptr_t counter, ptr_t lr, ptr_t st) {
+    if (milestones.size() > (size_t)kMaxLrMilestones) throw std::runtime_error("lr_schedule: at most 8 milestones");
+    LrScheduleParams p{};
+    p.policy = policy; p.n_milestones = (int)milestones.size(); p.warmup = warmup; p.total = total;
+    p.start = start; p.peak = peak; p.final_lr = final_lr; p.power = power; p.gamma = gamma;
+    for (size_t k = 0; k < milestones.size(); ++k) p.milestones[k] = milestones[k];
+    lr_schedule(p, P(counter), P(lr), S(st));
+  });
   m.def("easgd_elastic", [](ptr_t w, ptr_t h, ptr_t center, float alpha, long long n, int max_blocks, ptr_t st, int lockfree) {
     easgd_elastic(P(w), P(h), P(center), alpha, n, max_blocks, lockfree, S(st)); },
     py::arg("w"), py::arg("h"), py::arg("center"), py::arg("alpha"), py::arg("n"), py::arg("max_blocks"), py::arg("st"), py::arg("lockfree") = 0);

@@ -166,6 +166,36 @@ __global__ void adam_advance_clip_kernel(unsigned long long* step, const ClipRec
   if (threadIdx.x == 0 && blockIdx.x == 0 && clip->finite) *step += 1ull;
 }
 
+// Per-update learning-rate schedule (ops/reference.py: lr_at is the same formula on the host).  One thread: lr(u) for the update
+// index u = *counter, in fp64 and rounded once to fp32, into *lr (the arena's hyper[0]), then *counter = u + 1.  Every operation
+// with a correctly rounded result is spelled as an _rn intrinsic, so it is never contracted into an FMA (the build uses
+// --use_fast_math): warm-up, constant and multistep values are bit-equal to the host's; cosine and poly go through cos / pow.
+__global__ void lr_schedule_kernel(LrScheduleParams p, unsigned long long* __restrict__ counter, float* __restrict__ lr) {
+  const long long u = (long long)*counter;
+  double v = p.peak;
+  if (u < p.warmup) {
+    v = __dmul_rn(p.peak, __dadd_rn(p.start, __ddiv_rn(__dmul_rn(__dsub_rn(1.0, p.start), (double)u), (double)p.warmup)));
+  } else if (p.policy == LR_MULTISTEP) {
+    for (int k = 0; k < p.n_milestones; ++k)
+      if (u >= p.milestones[k]) v = __dmul_rn(v, p.gamma);
+  } else if (p.policy != LR_CONSTANT) {
+    const double q = fmin(fmax(__ddiv_rn((double)(u - p.warmup), (double)(p.total - p.warmup)), 0.0), 1.0);
+    const double f = p.policy == LR_COSINE ? __dmul_rn(0.5, __dadd_rn(1.0, cos(__dmul_rn(3.141592653589793, q))))
+                                           : pow(__dsub_rn(1.0, q), p.power);
+    v = __dadd_rn(p.final_lr, __dmul_rn(__dsub_rn(p.peak, p.final_lr), f));
+  }
+  *lr = __double2float_rn(v);
+  *counter = (unsigned long long)u + 1ull;
+}
+
+void lr_schedule(const LrScheduleParams& p, void* counter, void* lr, cudaStream_t st) {
+  if (p.policy < LR_CONSTANT || p.policy > LR_MULTISTEP) throw std::runtime_error("lr_schedule: unknown policy " + std::to_string(p.policy));
+  if (p.n_milestones < 0 || p.n_milestones > kMaxLrMilestones) throw std::runtime_error("lr_schedule: at most 8 milestones");
+  if (!counter || !lr) throw std::runtime_error("lr_schedule: needs the update counter and the lr slot");
+  lr_schedule_kernel<<<1, 1, 0, st>>>(p, (unsigned long long*)counter, (float*)lr);
+  count_launch(); TMPI_CHECK_LAUNCH("lr_schedule"); ::tmpi::check_capture(st, "lr_schedule");
+}
+
 // RMSProp (the GANs' optimizer, torch.optim.RMSprop without momentum).  State: V.
 // v = alpha v + (1 - alpha) g^2;  w -= lr * g / (sqrt(v) + eps);  then, when clip > 0, w = clamp(w, -clip, clip) (the WGAN critic's
 // weight clipping in the same pass).

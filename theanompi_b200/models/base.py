@@ -29,7 +29,7 @@ import torch
 from .. import ops
 from ..parallel.arena import FlatArena
 from ..utils import nvtx
-from ..utils.opt import FlatSGD, SharedScalar, pre_model_iter_fn
+from ..utils.opt import FlatSGD, LrSchedule, SharedScalar, pre_model_iter_fn
 from .layers2 import BatchNormal, Crop, Dropout, count_params
 
 
@@ -63,6 +63,7 @@ class ModelBase(object):
     bias_lr_mult = 2.0             # biases train with 2x lr in the reference's optimizer (lib/opt.py:181-268)
     graph_safe = True              # False: the step draws host-side randomness / has host control flow → never auto-capture
     supports_grad_accum = True     # config['grad_accum'] > 1 (False: the model refuses it at compile_iter_fns)
+    supports_lr_schedule = True    # config['lr_schedule'] (False: the model refuses it at compile_iter_fns)
     name = "Model"
 
     def __init__(self, config):
@@ -106,6 +107,10 @@ class ModelBase(object):
         self.n_updates = 0             # optimizer steps taken (windows completed)
         self.n_discarded = 0           # micro-steps of windows still open at reset_iter('train'), whose gradients were dropped
         self._micro = 0                # micro-steps done in the open window
+        # per-update learning-rate schedule (a dict, utils/opt.py: LrSchedule; None = off): a device launch at the start of every
+        # update's step writes lr; built by setup_lr_schedule at compile_iter_fns
+        self.lr_schedule = config.get("lr_schedule")
+        self.lr_sched = None
         self.base_lr = np.float32(self.learning_rate)
         self.current_t = self.subb_t = 0
         self.current_v = self.subb_v = 0
@@ -240,6 +245,7 @@ class ModelBase(object):
         return self._graph_out
 
     def _step_body(self):
+        self._schedule_lr()
         out = self._fwd_bwd_eager()
         self._dbg_capture("forward+backward")
         if self._tail is not None:
@@ -284,6 +290,8 @@ class ModelBase(object):
     def _accum_body(self, kind):
         """Forward + backward of one micro-step under the accumulate switch (ops.accum): G is stored by 'first' and added to by
         'mid' / 'last', the loss gradient carries 1/n; the step tail runs after 'last' only."""
+        if kind == "first":
+            self._schedule_lr()                  # every micro-step of a window trains with the lr of its update
         with ops.accum.mode(kind != "first", float(np.float32(1.0 / self.grad_accum))):
             out = self._fwd_bwd_eager()
         self._dbg_capture("forward+backward (%s micro-step)" % kind)
@@ -317,6 +325,37 @@ class ModelBase(object):
         if fused_tail is not None:
             raise ValueError("%s: grad_accum = %d does not combine with a fused exchange strategy, whose bucket launches fire during "
                              "every backward; %s" % (self.name, n, supported))
+
+    # ------------------------------------------------------------------ per-update learning-rate schedule
+    @property
+    def updates_per_epoch(self):
+        """Optimizer updates in one epoch of this worker: its train batches × sub-batches, over the gradient-accumulation window."""
+        return self.data.n_batch_train * self.n_subb // self.grad_accum
+
+    def setup_lr_schedule(self):
+        """Build ``config['lr_schedule']`` (:class:`LrSchedule`, peak = the model's learning_rate, total_steps by default
+        n_epochs × :attr:`updates_per_epoch`); a malformed dict, or a model that does not support a schedule, is a ValueError."""
+        self.lr_sched = None
+        if self.lr_schedule is None:
+            return
+        if not self.supports_lr_schedule:
+            raise ValueError("%s: lr_schedule is not supported; it runs on AlexNet, GoogLeNet, Cifar10_model, VGG16, ResNet50, "
+                             "Wide_ResNet and the LSTM" % self.name)
+        self.lr_sched = LrSchedule(self.arena, self.lr_schedule, self.learning_rate, int(self.n_epochs) * self.updates_per_epoch)
+
+    def _schedule_lr(self):
+        """The first launch of a step that starts an update: lr(u) into arena.hyper[0] before anything reads it."""
+        if self.lr_sched is not None:
+            self.lr_sched.step()
+
+    def _report_lr(self, dropped=False):
+        """Once per epoch, at reset_iter('train'): the host copy of shared_lr (recorder, lr_<epoch>.npy, checkpoints, prints) takes
+        the lr of the epoch's last update, read from the device once.  After a ``dropped`` window arena.hyper[0] holds the dropped
+        window's lr, so the host evaluates the last update's (``reference.lr_at``) from the update index instead."""
+        if self.lr_sched is None:
+            return
+        u = int(self.lr_sched.u) if dropped else 0
+        self.shared_lr.mirror(self.lr_sched.lr_at(u - 1) if u > 0 else self.lr_sched.value())
 
     def _dbg_capture(self, where):
         """TMPI_DEBUG_CAPTURE=1: name the stage that invalidated an ongoing CUDA-graph capture."""
@@ -436,6 +475,7 @@ class ModelBase(object):
         if self.optimizer not in ("sgd", "lars", "lamb"):
             raise ValueError("%s: optimizer must be 'lamb', 'sgd' or 'lars', not %r" % (self.name, self.optimizer))
         self.check_grad_accum(fused_tail)
+        self.setup_lr_schedule()
         k = self.size if sync_type == "cdd" else 1
         if self.optimizer in ("lars", "lamb") and fused_tail is not None:
             raise ValueError("optimizer=%r needs every tensor's whole reduced gradient before its update; the fused exchange "
@@ -514,9 +554,13 @@ class ModelBase(object):
             self.current_t = self.subb_t = 0
             self.last_one_t = False
             # a gradient-accumulation window still open at the end of the epoch is dropped: the next micro-step is a 'first' again,
-            # which overwrites G
+            # which overwrites G; it gives its update index back to the schedule, so the next window trains with the same lr
+            dropped = self._micro > 0 and self.lr_sched is not None
+            if dropped:
+                self.lr_sched.give_back()
             self.n_discarded += self._micro
             self._micro = 0
+            self._report_lr(dropped)
         else:
             self.current_v = self.subb_v = 0
             self.last_one_v = False
@@ -568,7 +612,10 @@ class ModelBase(object):
             self.subb_v += 1
 
     def adjust_hyperp(self, epoch):
-        """Once per epoch (ref ``alex_net.py:569-579``, ``googlenet.py:925-945``)."""
+        """Once per epoch (ref ``alex_net.py:569-579``, ``googlenet.py:925-945``).  A per-update ``lr_schedule`` owns lr: nothing
+        changes here."""
+        if self.lr_sched is not None:
+            return
         if self.lr_policy == "step":
             if epoch in self.lr_step:
                 self.shared_lr.set_value(np.float32(self.shared_lr.get_value() * self.lr_gamma))
@@ -603,6 +650,8 @@ class ModelBase(object):
             sd["lamb"] = self.lamb.state_dict()
         if self.clip_opt is not None:                   # the SGD step's skip counter (gradient clipping)
             sd["grad_clip"] = self.clip_opt.state_dict()
+        if self.lr_sched is not None:                   # the update index of the lr schedule
+            sd["lr_schedule"] = self.lr_sched.state_dict()
         return sd
 
     def load_extra_state(self, sd):
@@ -613,6 +662,8 @@ class ModelBase(object):
             self.lamb.load_state_dict(sd["lamb"])
         if "grad_clip" in sd and self.clip_opt is not None:
             self.clip_opt.load_state_dict(sd["grad_clip"])
+        if "lr_schedule" in sd and self.lr_sched is not None:
+            self.lr_sched.load_state_dict(sd["lr_schedule"])
 
     def cleanup(self):
         if getattr(self.data, "para_load", False) and hasattr(self.data, "para_load_close"):

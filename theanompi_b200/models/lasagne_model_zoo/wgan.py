@@ -98,6 +98,7 @@ class WGAN(TorchModelBase):
     def compile_iter_fns(self, sync_type="avg", **kw):
         self.refuse_grad_clip()
         self.check_grad_accum()
+        self.setup_lr_schedule()
         self.sync_type = "avg"
         self.opt_c = torch.optim.RMSprop(self.critic_params, lr=self.learning_rate)
         self.opt_g = torch.optim.RMSprop(self.generator_params, lr=self.learning_rate)
@@ -234,6 +235,7 @@ class NativeWGAN(ModelBase):
     ``opt_c.skipped`` / ``opt_g.skipped`` count it.  The reference's CIFAR-10 LSGAN uses plain RMSProp without rescaling, so there
     ``grad_clip`` is simply available."""
     supports_grad_accum = False    # its critic / generator steps keep their own gaccum accumulation
+    supports_lr_schedule = False   # two arenas and critic / generator step ratios: the reference's per-epoch decay
     loss_kind = "wgan"
     n_epochs = num_epochs
     batch_size = file_batch_size = batchsize
@@ -390,6 +392,7 @@ class NativeWGAN(ModelBase):
     # ---- contract
     def compile_iter_fns(self, sync_type="avg", **kw):
         self.check_grad_accum()
+        self.setup_lr_schedule()
         self.sync_type = "avg"
         self.vels, self.vels2 = [], []
         self.train_iter_fn = self.val_iter_fn = None

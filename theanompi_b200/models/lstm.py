@@ -185,6 +185,7 @@ class LSTM(ModelBase):
     def compile_iter_fns(self, sync_type="avg", **kw):
         self.check_grad_clip()
         self.check_grad_accum()
+        self.setup_lr_schedule()
         self.sync_type = "avg"
         self._make_opt()
         self.vels, self.vels2 = [], []
@@ -196,6 +197,7 @@ class LSTM(ModelBase):
     def _train_body(self, x, m, y):
         """Forward, backward and the flat update of one batch (device tensors); returns device scalars (cost, error)."""
         from .. import ops
+        self._schedule_lr()                                        # one model-wide update counter for every bucket's graph
         self.arena.G.zero_()
         cost, err, _ = ops.softmax_xent(self.forward_logits(x, m), y)
         cost.backward()                                            # the kernels write the gradients into the arena's G views
@@ -273,8 +275,10 @@ class LSTM(ModelBase):
     def extra_state(self):
         """The optimizer's extra buffers (its U-region state travels with the arena), its name and the early-stopping state."""
         opt = self._make_opt()
-        return {"optimizer": self.opt_name, "opt": opt.state_dict(),
-                "best_err": self.best_err, "bad_counter": self.bad_counter}
+        sd = {"optimizer": self.opt_name, "opt": opt.state_dict(), "best_err": self.best_err, "bad_counter": self.bad_counter}
+        if self.lr_sched is not None:
+            sd["lr_schedule"] = self.lr_sched.state_dict()
+        return sd
 
     def load_extra_state(self, sd):
         if sd.get("optimizer") != self.opt_name:
@@ -282,10 +286,13 @@ class LSTM(ModelBase):
                              % (sd.get("optimizer"), self.opt_name))
         self._make_opt().load_state_dict(sd["opt"])
         self.best_err, self.bad_counter = float(sd["best_err"]), int(sd["bad_counter"])
+        if "lr_schedule" in sd and self.lr_sched is not None:
+            self.lr_sched.load_state_dict(sd["lr_schedule"])
 
     def reset_iter(self, mode):
         if mode == "train":
             self._train_it = None
+            self._report_lr()
 
     def adjust_hyperp(self, epoch):
         pass
@@ -321,6 +328,7 @@ class LSTMTorch(TorchModelBase):
     def compile_iter_fns(self, sync_type="avg", **kw):
         self.refuse_grad_clip()
         self.check_grad_accum()
+        self.setup_lr_schedule()
         self.sync_type = "avg"
         self.torch_opt = self.make_torch_optimizer(self.params)
         self.vels, self.vels2 = [], []

@@ -42,6 +42,7 @@ class TorchModelBase(ModelBase):
     optimizer_name = "flat_sgd"
     autocast = True
     supports_grad_accum = False    # torch autograd writes .grad: the native accumulate mode does not reach it
+    supports_lr_schedule = False   # the library yardsticks keep the per-epoch lr policies
 
     def finalize_torch(self, module, input_shape, exchanged=None):
         self.module = module.to(self.device)
@@ -110,6 +111,7 @@ class TorchModelBase(ModelBase):
     def compile_iter_fns(self, sync_type="avg", aggregate="momentum", fused_tail=None):
         self.refuse_grad_clip()
         self.check_grad_accum(fused_tail)
+        self.setup_lr_schedule()
         self.torch_opt = self.make_torch_optimizer(self.params)
         if self.torch_opt is None:
             return super().compile_iter_fns(sync_type, aggregate, fused_tail)

@@ -853,6 +853,17 @@ def lamb_trust(arena, g, m, v, step, b1, b2, eps, inv_k, filt, partial, norms, t
                    _st(arena.W))
 
 
+def lr_schedule_step(arena, sched, counter):
+    """One launch of ``csrc/comm_kernels.cu: lr_schedule_kernel``: with u = ``counter`` (int64 [1] on the arena's device), write the
+    schedule's lr(u) to ``arena.hyper[0]`` and u + 1 to ``counter``.  ``sched``: the validated parameters (``utils/opt.py:
+    LrSchedule``).  Reads only device memory, so it can be captured in a CUDA graph."""
+    assert counter.dtype == torch.int64 and counter.numel() == 1 and counter.device == arena.hyper.device, (counter.dtype, counter.device)
+    lib = L()
+    lib.lr_schedule(lib.LR_POLICIES[sched.decay], int(sched.warmup_steps), int(sched.total_steps), float(sched.warmup_start),
+                    float(sched.peak), float(sched.final_lr), float(sched.power), float(sched.gamma), [int(m) for m in sched.milestones],
+                    counter.data_ptr(), arena.hyper.data_ptr(), _st(arena.hyper))
+
+
 def sgd_flat(arena, g, lr, mu, nesterov, inv_k, lo, hi, only_local=False, only_exchanged=False, clip=None):
     """Fused momentum-SGD over arena elements [lo, hi): ``flat_update``'s SGD rule.  ``lr`` is not used: the kernel reads
     ``arena.hyper[0]`` on the device (so a captured CUDA graph follows lr changes)."""

@@ -256,6 +256,35 @@ def clip_scale(g, offsets, sizes, max_norm):
     return n, float(np.float32(min(1.0, float(np.float32(max_norm)) / (n + 1e-6)))), True
 
 
+def lr_at(u, peak, decay="constant", warmup_steps=0, warmup_start=0.0, total_steps=None, final_lr=0.0, power=1.0, gamma=0.1,
+          milestones=()):
+    """Learning rate of optimizer update ``u`` (0, 1, 2, ...) under a per-update schedule (``csrc/comm_kernels.cu:
+    lr_schedule_kernel``), evaluated in fp64 and rounded once to fp32:
+
+        u < W (warm-up)   peak·(s + (1 − s)·u / W)                                 W = warmup_steps, s = warmup_start
+        then, with p = clamp((u − W) / (T − W), 0, 1), T = total_steps:
+          constant        peak
+          cosine          final + (peak − final)·½(1 + cos πp)
+          poly            final + (peak − final)·(1 − p)^power
+          multistep       peak·gamma^(number of milestones ≤ u)                    (gamma multiplied in once per milestone)"""
+    u, W, peak = int(u), int(warmup_steps), float(peak)
+    if u < W:
+        s = float(warmup_start)
+        return np.float32(peak * (s + (1.0 - s) * u / W))
+    if decay == "constant":
+        return np.float32(peak)
+    if decay == "multistep":
+        lr = peak
+        for m in milestones:
+            if u >= m:
+                lr *= float(gamma)
+        return np.float32(lr)
+    p = min(max((u - W) / (int(total_steps) - W), 0.0), 1.0)
+    final = float(final_lr)
+    f = 0.5 * (1.0 + math.cos(math.pi * p)) if decay == "cosine" else (1.0 - p) ** float(power)
+    return np.float32(final + (peak - final) * f)
+
+
 def sgd_flat(w, g, u, lr_mult, wd, lr, mu, nesterov, inv_k, w_half=None):
     """One momentum-SGD step over flat fp32 buffers with per-element
     ``lr_mult`` / ``wd`` vectors (broadcastable).  Semantics of the reference's

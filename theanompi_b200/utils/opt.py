@@ -63,6 +63,110 @@ class SharedScalar(object):
         self._host = float(v)
         self._buf[self._i] = float(v)
 
+    def mirror(self, v):
+        """Set the host copy only: the device element already holds ``v`` (a per-update :class:`LrSchedule` wrote it)."""
+        self._host = float(v)
+
+
+class LrSchedule(object):
+    """Per-update learning-rate schedule (``config['lr_schedule']``, a dict), the lr of update u = 0, 1, 2, ... written to
+    ``arena.hyper[0]`` by one single-thread launch at the start of each update's step (``cuda_impl.lr_schedule_step``), inside
+    the captured CUDA graph: replays follow the schedule with no host work.  The CPU applies ``reference.lr_at`` instead.
+
+    Keys (``peak`` is the model's learning_rate):
+      ``warmup_steps`` W >= 0 (0), ``warmup_start`` s in [0, 1] (0): for u < W, lr = peak·(s + (1 − s)·u / W);
+      ``decay``: 'constant' (default), 'cosine', 'poly' (``power`` >= 0, default 1) or 'multistep' (``milestones``: at most 8
+      strictly increasing update indices >= W; ``gamma``, default 0.1);
+      ``total_steps`` T > W (default: the model's n_epochs × updates_per_epoch), ``final_lr`` (0): the end of cosine and poly.
+
+    The update index ``u`` (int64 [1], on the arena's device) is checkpointed by :meth:`state_dict`."""
+
+    KEYS = ("warmup_steps", "warmup_start", "decay", "total_steps", "final_lr", "power", "gamma", "milestones")
+    DECAYS = ("constant", "cosine", "poly", "multistep")
+    MAX_MILESTONES = 8
+
+    def __init__(self, arena, cfg, peak, total_steps):
+        if not isinstance(cfg, dict):
+            raise ValueError("lr_schedule must be a dict or None, not %r" % (cfg,))
+        unknown = sorted(set(cfg) - set(self.KEYS))
+        if unknown:
+            raise ValueError("lr_schedule: unknown key %r; the keys are %s" % (unknown[0], ", ".join(self.KEYS)))
+        self.arena = arena
+        self.peak = float(peak)
+        self.decay = cfg.get("decay", "constant")
+        if self.decay not in self.DECAYS:
+            raise ValueError("lr_schedule['decay'] must be one of %s, not %r" % (", ".join(self.DECAYS), self.decay))
+        self.warmup_steps = self._int(cfg, "warmup_steps", 0)
+        if self.warmup_steps < 0:
+            raise ValueError("lr_schedule['warmup_steps'] must be >= 0, not %d" % self.warmup_steps)
+        self.total_steps = self._int(cfg, "total_steps", total_steps)
+        if not self.warmup_steps < self.total_steps:
+            raise ValueError("lr_schedule['total_steps'] (%d) must be greater than warmup_steps (%d)"
+                             % (self.total_steps, self.warmup_steps))
+        self.warmup_start = self._float(cfg, "warmup_start", 0.0)
+        if not 0.0 <= self.warmup_start <= 1.0:
+            raise ValueError("lr_schedule['warmup_start'] must be in [0, 1], not %r" % self.warmup_start)
+        self.final_lr = self._float(cfg, "final_lr", 0.0)
+        self.power = self._float(cfg, "power", 1.0)
+        if not self.power >= 0.0:
+            raise ValueError("lr_schedule['power'] must be >= 0, not %r" % self.power)
+        self.gamma = self._float(cfg, "gamma", 0.1)
+        ms = cfg.get("milestones", ())
+        if not isinstance(ms, (list, tuple)) or any(isinstance(m, bool) or not isinstance(m, (int, np.integer)) for m in ms):
+            raise ValueError("lr_schedule['milestones'] must be a list of update indices, not %r" % (ms,))
+        self.milestones = tuple(int(m) for m in ms)
+        if len(self.milestones) > self.MAX_MILESTONES:
+            raise ValueError("lr_schedule['milestones'] holds at most %d update indices, not %d" % (self.MAX_MILESTONES, len(ms)))
+        if any(b <= a for a, b in zip(self.milestones, self.milestones[1:])):
+            raise ValueError("lr_schedule['milestones'] must be strictly increasing: %r" % (self.milestones,))
+        if self.milestones and self.milestones[0] < self.warmup_steps:
+            raise ValueError("lr_schedule['milestones'] must be >= warmup_steps (%d): %r" % (self.warmup_steps, self.milestones))
+        self.u = torch.zeros(1, dtype=torch.int64, device=arena.hyper.device)
+
+    @staticmethod
+    def _int(cfg, key, default):
+        v = cfg.get(key, default)
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+            raise ValueError("lr_schedule[%r] must be an int, not %r" % (key, v))
+        return int(v)
+
+    @staticmethod
+    def _float(cfg, key, default):
+        v = cfg.get(key, default)
+        if isinstance(v, bool) or not isinstance(v, (int, float, np.number)) or not np.isfinite(v):
+            raise ValueError("lr_schedule[%r] must be a finite number, not %r" % (key, v))
+        return float(v)
+
+    def lr_at(self, u):
+        """The schedule's lr of update ``u`` (``reference.lr_at``, an np.float32)."""
+        return ref.lr_at(u, self.peak, self.decay, self.warmup_steps, self.warmup_start, self.total_steps, self.final_lr, self.power,
+                         self.gamma, self.milestones)
+
+    def step(self):
+        """Start an update: lr(u) into ``arena.hyper[0]``, u += 1 (on CUDA one launch that reads only device memory)."""
+        a = self.arena
+        if a.hyper.is_cuda:
+            from ..ops import cuda_impl
+            cuda_impl.lr_schedule_step(a, self, self.u)
+            return
+        a.hyper[0] = float(self.lr_at(int(self.u)))
+        self.u += 1
+
+    def give_back(self):
+        """Return the index of an update that was started but dropped (an open gradient-accumulation window at the end of an
+        epoch): one device decrement, outside any graph.  The next update recomputes the same lr."""
+        self.u -= 1
+
+    def value(self):
+        """The lr the last :meth:`step` wrote (reads ``arena.hyper[0]``: a device read)."""
+        return float(self.arena.hyper[0])
+
+    def state_dict(self):
+        return {"u": int(self.u)}
+
+    def load_state_dict(self, sd):
+        self.u.fill_(int(sd["u"]))
+
 
 def _fc_fusable(p, block):
     """Can ``p``'s weight gradient be consumed by the SGD epilogue of its wgrad GEMM?  It must come from ONE fp32 GEMM straight
@@ -459,6 +563,19 @@ def _set_clip(model, opt, k):
     model.clip_opt = opt
 
 
+def _step_lr(model):
+    """The lr argument of a :class:`FlatSGD` step in a closure: the host value of ``shared_lr``, or None under a per-update
+    :class:`LrSchedule`, so that the CPU step reads ``arena.hyper[0]`` as the kernel does."""
+    return None if getattr(model, "lr_sched", None) is not None else model.shared_lr.get_value()
+
+
+def _device_lr(model):
+    """The lr of a torch expression in a closure: the host value of ``shared_lr``, or under a per-update :class:`LrSchedule`
+    ``arena.hyper[0]`` as a device scalar, which the schedule's launch earlier in the step wrote.  A host read there would break
+    the capture of a step that runs the closure."""
+    return model.arena.hyper[0] if getattr(model, "lr_sched", None) is not None else model.shared_lr.get_value()
+
+
 def _pre_post_msgd(model, use_nesterov, k, arm=True):
     """BSP_MSGD: aggregate momentum."""
     a, mu = model.arena, (model.mu if model.use_momentum else 0.0)
@@ -467,7 +584,7 @@ def _pre_post_msgd(model, use_nesterov, k, arm=True):
     sgd.arm(model, k == 1 and arm)
 
     def pre():
-        lr = model.shared_lr.get_value()
+        lr = _step_lr(model)
         if k == 1:
             sgd.step(lr, 1)
             return
@@ -480,7 +597,7 @@ def _pre_post_msgd(model, use_nesterov, k, arm=True):
     def post():
         if k == 1:
             return
-        lr = model.shared_lr.get_value()
+        lr = _device_lr(model)
         ex = _ex(a)
         a.W.sub_(torch.where(ex, lr * a.lr_mult_vector() * a.R / float(k), torch.zeros_like(a.W)))
         a.refresh_shadow()
@@ -496,7 +613,7 @@ def _pre_post_msgd_grad(model, use_nesterov, k, arm=True):
     sgd.arm(model, k == 1 and arm)
 
     def pre():
-        lr = model.shared_lr.get_value()
+        lr = _step_lr(model)
         if k == 1:
             sgd.step(lr, 1)
             return
@@ -507,7 +624,7 @@ def _pre_post_msgd_grad(model, use_nesterov, k, arm=True):
     def post():
         if k == 1:
             return
-        lr = model.shared_lr.get_value()
+        lr = _device_lr(model)
         ex = _ex(a)
         u_new = mu * a.U + a.R
         step = a.R + mu * u_new if use_nesterov else u_new
@@ -525,12 +642,13 @@ def _pre_post_sgd(model, k, arm=True):
     sgd.arm(model, k == 1 and arm)
 
     def pre():
-        lr = model.shared_lr.get_value()
+        lr = _step_lr(model)
         if k == 1:
             sgd.step(lr, 1)
             return
         sgd.step(lr, 1, only_local=True)
         ex = _ex(a)
+        lr = _device_lr(model)
         a.G.copy_(torch.where(ex, lr * a.lr_mult_vector() * (a.G + a.wd_vector() * a.W) / float(k), a.G))
 
     def post():

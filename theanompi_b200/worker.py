@@ -78,7 +78,12 @@ class BSP_Worker(MPI_GPU_Process):
             self.start_epoch = 0
 
     def lr_warmup(self, model, epoch):
-        """Geometric warm-up lr → lr·size over 5 epochs (ref ``worker.py:34-63``)."""
+        """Geometric warm-up lr → lr·size over 5 epochs (ref ``worker.py:34-63``).  A model with a per-update ``lr_schedule`` states
+        the peak lr for the global batch itself: the schedule owns lr and nothing is scaled here."""
+        if getattr(model, "lr_sched", None) is not None:
+            if self.verbose:
+                print("per-update lr schedule: lr %f at the last update before epoch %d" % (model.shared_lr.get_value(), epoch))
+            return
         if epoch == 0:
             self.warmup_epochs = 5.0
             self.power_base = pow(self.size, 1.0 / self.warmup_epochs)
