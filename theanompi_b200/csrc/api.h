@@ -101,9 +101,10 @@ void dropout_fwd(const void* x, void* y, void* mask, long long n, float p_drop, 
 void dropout_bwd(const void* dy, const void* mask, void* dx, long long n, int f32, cudaStream_t st);
 void advance_step(void* step, cudaStream_t st);
 // out3 = {weight · mean NLL, top-1 error, top-5 error}; dlogits = (softmax − onehot) · grad_weight / B (grad_weight = weight / n under
-// n-micro-batch gradient accumulation, so the accumulated gradient is the mean over the window)
+// n-micro-batch gradient accumulation, so the accumulated gradient is the mean over the window).  label_smoothing ε in (0, 1]: the
+// target is (1 − ε)·onehot + ε / C in both the loss and dlogits (soft-target cross-entropy); ε = 0 is the plain NLL
 void softmax_xent(const void* logits, const void* labels, void* dlogits, void* rowstat, void* out3, int B, int C, float weight,
-                  float grad_weight, int f32, cudaStream_t st);
+                  float grad_weight, float label_smoothing, int f32, cudaStream_t st);
 // act: 0 none, 1 ReLU, 2 leaky ReLU (negative slope `slope`), 3 sigmoid (ACT_* in common.cuh).  accumulate = 1: db / db1 += the bias
 // gradient (no clear)
 void relu_bias_bwd(const void* dy, const void* y, void* dym, void* db, void* db1, int c_split, long long R, int C, long long ld, int act,

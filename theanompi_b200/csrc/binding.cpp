@@ -101,8 +101,8 @@ PYBIND11_MODULE(_tmpi_native, m) {
   m.def("dropout_bwd", [](ptr_t dy, ptr_t mask, ptr_t dx, long long n, int f32, ptr_t st) { dropout_bwd(P(dy), P(mask), P(dx), n, f32, S(st)); });
   m.def("advance_step", [](ptr_t step, ptr_t st) { advance_step(P(step), S(st)); });
   m.def("softmax_xent", [](ptr_t logits, ptr_t labels, ptr_t dlogits, ptr_t rowstat, ptr_t out3, int B, int C, float weight, float grad_weight,
-                           int f32, ptr_t st) {
-    softmax_xent(P(logits), P(labels), P(dlogits), P(rowstat), P(out3), B, C, weight, grad_weight, f32, S(st)); });
+                           float label_smoothing, int f32, ptr_t st) {
+    softmax_xent(P(logits), P(labels), P(dlogits), P(rowstat), P(out3), B, C, weight, grad_weight, label_smoothing, f32, S(st)); });
   m.def("maxpool_relu_bias_bwd", [](ptr_t dyp, ptr_t arg, ptr_t y, ptr_t dym, ptr_t db0, ptr_t db1, int c_split, int N, int H, int W, int C,
                                     int Ho, int Wo, int k, int s, int p, int accumulate, ptr_t st) {
     maxpool_relu_bias_bwd(P(dyp), P(arg), P(y), P(dym), P(db0), P(db1), c_split, N, H, W, C, Ho, Wo, k, s, p, accumulate, S(st)); });

@@ -552,9 +552,11 @@ void gan_loss(const void* scores, void* dscores, void* out, int B, int kind, flo
 
 // ============================================================================ softmax + NLL + errors + dlogits
 // one CTA per row; rowstat[b] = {nll, err1, err5}; dlogits = (softmax - onehot) * scale
-template <typename T>
+// kSmooth (label smoothing ε): the target is q = on·onehot + off with on = 1 − ε, off = ε / C, so rowstat[3b] is the soft-target
+// cross-entropy −Σ q·log p = log se − on·(z_y − max) − off·Σ(z − max) and dlogits = (softmax − q) * scale; err1 / err5 are unchanged
+template <typename T, bool kSmooth>
 __global__ void softmax_xent_kernel(const T* __restrict__ logits, const long long* __restrict__ labels,
-                                    T* __restrict__ dlogits, float* __restrict__ rowstat, int C, float scale) {
+                                    T* __restrict__ dlogits, float* __restrict__ rowstat, int C, float scale, float on, float off) {
   const int b = blockIdx.x;
   const T* row = logits + (long long)b * C;
   const int label = (int)labels[b];
@@ -571,11 +573,12 @@ __global__ void softmax_xent_kernel(const T* __restrict__ logits, const long lon
   mx = bcast;
   __syncthreads();
   const float lab = to_f(row[label]);
-  float se = 0.f, gt = 0.f;
+  float se = 0.f, gt = 0.f, sz = 0.f;
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     const float v = to_f(row[c]);
     se += __expf(v - mx);
     gt += (v > lab || (v == lab && c < label)) ? 1.f : 0.f;     // rank of the label's logit
+    if constexpr (kSmooth) sz += v - mx;
   }
   se = warp_sum(se); gt = warp_sum(gt);
   if (lane == 0) { red[warp] = se; }
@@ -589,14 +592,22 @@ __global__ void softmax_xent_kernel(const T* __restrict__ logits, const long lon
   if (warp == 0) { float v = lane < nw ? red[lane] : 0.f; v = warp_sum(v); if (lane == 0) bcast = v; }
   __syncthreads();
   gt = bcast;
+  if constexpr (kSmooth) {                                      // Σ(z − max) to thread 0 (red is free: its last readers passed the barrier)
+    sz = warp_sum(sz);
+    if (lane == 0) red[warp] = sz;
+    __syncthreads();
+    if (warp == 0) { float v = lane < nw ? red[lane] : 0.f; sz = warp_sum(v); }
+  }
   const float inv = 1.f / se;
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     float pr = __expf(to_f(row[c]) - mx) * inv;
-    if (c == label) pr -= 1.f;
+    if constexpr (kSmooth) { pr -= off; if (c == label) pr -= on; }
+    else { if (c == label) pr -= 1.f; }
     dlogits[(long long)b * C + c] = from_f<T>(pr * scale);
   }
   if (threadIdx.x == 0) {
-    rowstat[3 * b + 0] = -(lab - mx - __logf(se));
+    if constexpr (kSmooth) rowstat[3 * b + 0] = __logf(se) - on * (lab - mx) - off * sz;
+    else rowstat[3 * b + 0] = -(lab - mx - __logf(se));
     rowstat[3 * b + 1] = gt >= 1.f ? 1.f : 0.f;
     rowstat[3 * b + 2] = gt >= 5.f ? 1.f : 0.f;
   }
@@ -617,13 +628,22 @@ __global__ void rowstat_mean_kernel(const float* __restrict__ rowstat, float* __
   }
 }
 
-// the reported loss carries `weight`, the gradient `grad_weight` (weight / n under gradient accumulation over n micro-batches)
+// the reported loss carries `weight`, the gradient `grad_weight` (weight / n under gradient accumulation over n micro-batches);
+// label_smoothing ε = 0 runs the plain NLL instantiation, ε in (0, 1] the soft-target one
 void softmax_xent(const void* logits, const void* labels, void* dlogits, void* rowstat, void* out3, int B, int C, float weight,
-                  float grad_weight, int f32, cudaStream_t st) {
+                  float grad_weight, float label_smoothing, int f32, cudaStream_t st) {
+  if (!(label_smoothing >= 0.f && label_smoothing <= 1.f)) throw std::runtime_error("softmax_xent: label_smoothing must be in [0, 1]");
   auto LB = (const long long*)labels; auto RS = (float*)rowstat;
   const float scale = grad_weight / (float)B;
-  if (f32) softmax_xent_kernel<float><<<B, 256, 0, st>>>((const float*)logits, LB, (float*)dlogits, RS, C, scale);
-  else softmax_xent_kernel<__nv_bfloat16><<<B, 256, 0, st>>>((const __nv_bfloat16*)logits, LB, (__nv_bfloat16*)dlogits, RS, C, scale);
+  const bool smooth = label_smoothing != 0.f;
+  const float on = 1.f - label_smoothing, off = label_smoothing / (float)C;
+  if (f32) {
+    auto k = smooth ? softmax_xent_kernel<float, true> : softmax_xent_kernel<float, false>;
+    k<<<B, 256, 0, st>>>((const float*)logits, LB, (float*)dlogits, RS, C, scale, on, off);
+  } else {
+    auto k = smooth ? softmax_xent_kernel<__nv_bfloat16, true> : softmax_xent_kernel<__nv_bfloat16, false>;
+    k<<<B, 256, 0, st>>>((const __nv_bfloat16*)logits, LB, (__nv_bfloat16*)dlogits, RS, C, scale, on, off);
+  }
   count_launch(); TMPI_CHECK_LAUNCH("softmax_xent"); ::tmpi::check_capture(st, "softmax_xent");
   rowstat_mean_kernel<<<1, 256, 0, st>>>((const float*)rowstat, (float*)out3, B, weight);
   count_launch(); TMPI_CHECK_LAUNCH("rowstat_mean"); ::tmpi::check_capture(st, "rowstat_mean");

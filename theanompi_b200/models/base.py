@@ -21,6 +21,7 @@ needs re-capture; costs/errors stay on the device until the recorder prints.
 """
 from __future__ import annotations
 
+import math
 import time
 
 import numpy as np
@@ -64,6 +65,7 @@ class ModelBase(object):
     graph_safe = True              # False: the step draws host-side randomness / has host control flow → never auto-capture
     supports_grad_accum = True     # config['grad_accum'] > 1 (False: the model refuses it at compile_iter_fns)
     supports_lr_schedule = True    # config['lr_schedule'] (False: the model refuses it at compile_iter_fns)
+    supports_label_smoothing = True    # config['label_smoothing'] > 0 (False: no classifier head; refused at compile_iter_fns)
     name = "Model"
 
     def __init__(self, config):
@@ -111,6 +113,9 @@ class ModelBase(object):
         # update's step writes lr; built by setup_lr_schedule at compile_iter_fns
         self.lr_schedule = config.get("lr_schedule")
         self.lr_sched = None
+        # label smoothing ε of the training loss (cross-entropy against (1 − ε)·onehot + ε / C; 0 = plain NLL); validation stays
+        # plain NLL.  Checked by check_label_smoothing at compile_iter_fns
+        self.label_smoothing = config.get("label_smoothing", 0.0)
         self.base_lr = np.float32(self.learning_rate)
         self.current_t = self.subb_t = 0
         self.current_v = self.subb_v = 0
@@ -178,14 +183,17 @@ class ModelBase(object):
         """Return logits-layer output; must leave ``self.output_layer`` evaluated."""
         raise NotImplementedError
 
-    def loss(self, x, y):
+    def loss(self, x, y, label_smoothing=0.0):
+        """(cost, top-1 error, top-5 error); the cost is the mean NLL, or with ``label_smoothing`` ε > 0 the cross-entropy against
+        (1 − ε)·onehot + ε / C."""
         self.forward(x)
         sm = self.output_layer
-        return sm.negative_log_likelihood(y), sm.errors(y), sm.errors_top_x(y)
+        return sm.negative_log_likelihood(y, label_smoothing), sm.errors(y), sm.errors_top_x(y)
 
     # ------------------------------------------------------------------ step functions
     def _fwd_bwd_eager(self):
-        cost, err, err5 = self.loss(self.x_in, self.y_in)
+        # the training loss carries the label smoothing (read on the host here, so a captured step keeps the ε it was captured with)
+        cost, err, err5 = self.loss(self.x_in, self.y_in, self.label_smoothing)
         self._dbg_capture("forward")
         cost.backward()
         return cost.detach(), err.detach()
@@ -325,6 +333,20 @@ class ModelBase(object):
         if fused_tail is not None:
             raise ValueError("%s: grad_accum = %d does not combine with a fused exchange strategy, whose bucket launches fire during "
                              "every backward; %s" % (self.name, n, supported))
+
+    # ------------------------------------------------------------------ label smoothing
+    def check_label_smoothing(self):
+        """``config['label_smoothing']`` must be a finite real ε in [0, 1] (not a bool), and ε > 0 needs a classifier head; anything
+        else is a ValueError that names the key."""
+        eps = self.label_smoothing
+        ok = not isinstance(eps, bool) and isinstance(eps, (int, float, np.integer, np.floating))
+        if not (ok and math.isfinite(eps) and 0.0 <= eps <= 1.0):
+            raise ValueError("%s: label_smoothing must be a real number in [0, 1], not %r" % (self.name, eps))
+        self.label_smoothing = float(eps)
+        if self.label_smoothing and not self.supports_label_smoothing:
+            raise ValueError("%s has no classifier head: label_smoothing = %r is not supported; it applies to the softmax "
+                             "cross-entropy of AlexNet, GoogLeNet, Cifar10_model, VGG16, ResNet50, Wide_ResNet, the LSTM and their "
+                             "torch twins" % (self.name, eps))
 
     # ------------------------------------------------------------------ per-update learning-rate schedule
     @property
@@ -475,6 +497,7 @@ class ModelBase(object):
         if self.optimizer not in ("sgd", "lars", "lamb"):
             raise ValueError("%s: optimizer must be 'lamb', 'sgd' or 'lars', not %r" % (self.name, self.optimizer))
         self.check_grad_accum(fused_tail)
+        self.check_label_smoothing()
         self.setup_lr_schedule()
         k = self.size if sync_type == "cdd" else 1
         if self.optimizer in ("lars", "lamb") and fused_tail is not None:

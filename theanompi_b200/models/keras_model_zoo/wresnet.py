@@ -158,6 +158,7 @@ class Wide_ResNet(ModelBase):
             raise ValueError("Wide_ResNet trains with Adam: only sync_type='avg' is supported (as in the reference, wresnet.py:152-153)")
         self.check_grad_clip(optimizer="adam")
         self.check_grad_accum(fused_tail)
+        self.check_label_smoothing()
         self.setup_lr_schedule()
         from ...utils.opt import FlatAdam
         self.sync_type = "avg"

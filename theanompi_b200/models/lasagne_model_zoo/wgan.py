@@ -44,6 +44,7 @@ def build_critic(in_ch=1, size=28):
 
 
 class WGAN(TorchModelBase):
+    supports_label_smoothing = False   # no classifier head
     loss_kind = "wgan"
     n_epochs = num_epochs
     batch_size = file_batch_size = batchsize
@@ -98,6 +99,7 @@ class WGAN(TorchModelBase):
     def compile_iter_fns(self, sync_type="avg", **kw):
         self.refuse_grad_clip()
         self.check_grad_accum()
+        self.check_label_smoothing()
         self.setup_lr_schedule()
         self.sync_type = "avg"
         self.opt_c = torch.optim.RMSprop(self.critic_params, lr=self.learning_rate)
@@ -236,6 +238,7 @@ class NativeWGAN(ModelBase):
     ``grad_clip`` is simply available."""
     supports_grad_accum = False    # its critic / generator steps keep their own gaccum accumulation
     supports_lr_schedule = False   # two arenas and critic / generator step ratios: the reference's per-epoch decay
+    supports_label_smoothing = False   # no classifier head
     loss_kind = "wgan"
     n_epochs = num_epochs
     batch_size = file_batch_size = batchsize
@@ -392,6 +395,7 @@ class NativeWGAN(ModelBase):
     # ---- contract
     def compile_iter_fns(self, sync_type="avg", **kw):
         self.check_grad_accum()
+        self.check_label_smoothing()
         self.setup_lr_schedule()
         self.sync_type = "avg"
         self.vels, self.vels2 = [], []

@@ -590,9 +590,13 @@ class Softmax(Layer):
         self._cache = None
         return self.logits
 
-    def _eval(self, y):
-        if self._cache is None or self._cache[0] is not y:
-            self._cache = (y,) + tuple(ops.softmax_xent(self.logits, y))
+    def _eval(self, y, label_smoothing=None):
+        """(y, ε, loss, err1, err5) of one launch on this forward's logits, cached per (y, ε); ``label_smoothing`` None takes a
+        cached launch of any ε (the errors do not depend on it), else ε = 0."""
+        c = self._cache
+        if c is None or c[0] is not y or (label_smoothing is not None and c[1] != label_smoothing):
+            eps = label_smoothing or 0.0
+            self._cache = (y, eps) + tuple(ops.softmax_xent(self.logits, y, eps))
         return self._cache
 
     @property
@@ -603,18 +607,19 @@ class Softmax(Layer):
     def y_pred(self):
         return self.logits.argmax(1)
 
-    def negative_log_likelihood(self, y):
-        return self._eval(y)[1]
+    def negative_log_likelihood(self, y, label_smoothing=0.0):
+        """Mean NLL of ``y``; ``label_smoothing`` ε > 0 gives the cross-entropy against (1 − ε)·onehot + ε / C instead."""
+        return self._eval(y, label_smoothing)[2]
 
     def errors(self, y):
-        return self._eval(y)[2]
+        return self._eval(y)[3]
 
     def errors_top_x(self, y, num_top=5):
         if num_top != 5:
             lg = self.logits.float()
             topk = lg.topk(num_top, dim=1).indices
             return 1.0 - (topk == y[:, None]).any(1).float().mean()
-        return self._eval(y)[3]
+        return self._eval(y)[4]
 
 
 # =========================================================================== graph helpers

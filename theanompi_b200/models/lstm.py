@@ -185,6 +185,7 @@ class LSTM(ModelBase):
     def compile_iter_fns(self, sync_type="avg", **kw):
         self.check_grad_clip()
         self.check_grad_accum()
+        self.check_label_smoothing()
         self.setup_lr_schedule()
         self.sync_type = "avg"
         self._make_opt()
@@ -199,7 +200,7 @@ class LSTM(ModelBase):
         from .. import ops
         self._schedule_lr()                                        # one model-wide update counter for every bucket's graph
         self.arena.G.zero_()
-        cost, err, _ = ops.softmax_xent(self.forward_logits(x, m), y)
+        cost, err, _ = ops.softmax_xent(self.forward_logits(x, m), y, self.label_smoothing)
         cost.backward()                                            # the kernels write the gradients into the arena's G views
         with torch.no_grad():
             self.opt.step()                                        # lr from arena.hyper[0] (= shared_lr)
@@ -328,6 +329,7 @@ class LSTMTorch(TorchModelBase):
     def compile_iter_fns(self, sync_type="avg", **kw):
         self.refuse_grad_clip()
         self.check_grad_accum()
+        self.check_label_smoothing()
         self.setup_lr_schedule()
         self.sync_type = "avg"
         self.torch_opt = self.make_torch_optimizer(self.params)
@@ -352,7 +354,7 @@ class LSTMTorch(TorchModelBase):
         for p in self.params:
             p.grad = p.gbuf
         logits = self.module(x, m)
-        cost = nn.functional.cross_entropy(logits, y)
+        cost = nn.functional.cross_entropy(logits, y, label_smoothing=self.label_smoothing)
         cost.backward()
         self.torch_opt.step()
         err = (logits.argmax(1) != y).float().mean()

@@ -71,9 +71,9 @@ class TorchModelBase(ModelBase):
                 return self.module(x)
         return self.module(x.float())
 
-    def loss(self, x, y):
+    def loss(self, x, y, label_smoothing=0.0):
         logits = self.forward(x).float()
-        cost = torch.nn.functional.cross_entropy(logits, y)
+        cost = torch.nn.functional.cross_entropy(logits, y, label_smoothing=label_smoothing)
         with torch.no_grad():
             pred = logits.argmax(1)
             err = (pred != y).float().mean()
@@ -87,7 +87,7 @@ class TorchModelBase(ModelBase):
             if p.grad is None or p.grad.data_ptr() != p.gbuf.data_ptr():
                 p.grad = p.gbuf
         self.module.train()
-        cost, err, err5 = self.loss(self.x_in, self.y_in)
+        cost, err, err5 = self.loss(self.x_in, self.y_in, self.label_smoothing)
         cost.backward()
         return cost.detach(), err.detach()
 
@@ -111,6 +111,7 @@ class TorchModelBase(ModelBase):
     def compile_iter_fns(self, sync_type="avg", aggregate="momentum", fused_tail=None):
         self.refuse_grad_clip()
         self.check_grad_accum(fused_tail)
+        self.check_label_smoothing()
         self.setup_lr_schedule()
         self.torch_opt = self.make_torch_optimizer(self.params)
         if self.torch_opt is None:

@@ -667,9 +667,10 @@ def dropout_bwd(dy, mask):
     return dx
 
 
-def softmax_xent(logits, labels, weight=1.0, grad_scale=1.0):
+def softmax_xent(logits, labels, weight=1.0, grad_scale=1.0, label_smoothing=0.0):
     """(weight · mean NLL, top-1 error, top-5 error, dlogits); dlogits is the gradient of the mean NLL times weight · grad_scale
-    (``grad_scale`` = 1/n under gradient accumulation over n micro-batches), scaled in fp32 inside the kernel."""
+    (``grad_scale`` = 1/n under gradient accumulation over n micro-batches), scaled in fp32 inside the kernel.  ``label_smoothing``
+    ε > 0 makes the loss and dlogits those of the soft target (1 − ε)·onehot + ε / C, in the same launch."""
     lg = _bf(logits).contiguous()
     B_, C = lg.shape
     labels = labels.contiguous()
@@ -678,7 +679,7 @@ def softmax_xent(logits, labels, weight=1.0, grad_scale=1.0):
     rowstat = torch.empty((B_, 3), dtype=torch.float32, device=lg.device)
     out3 = torch.empty(3, dtype=torch.float32, device=lg.device)
     L().softmax_xent(lg.data_ptr(), labels.data_ptr(), dl.data_ptr(), rowstat.data_ptr(), out3.data_ptr(), B_, C, float(weight),
-                     float(weight) * float(grad_scale), int(_is32(lg)), _st(lg))
+                     float(weight) * float(grad_scale), float(label_smoothing), int(_is32(lg)), _st(lg))
     return out3[0], out3[1], out3[2], dl
 
 

@@ -485,9 +485,10 @@ def dropout(x, p_drop, training, layer_id=0):
 # --------------------------------------------------------------------------- softmax + NLL
 class _SoftmaxXentFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, logits, labels):
+    def forward(ctx, logits, labels, label_smoothing):
         # under gradient accumulation over n micro-batches dlogits carries 1/n (in fp32, inside the kernel); the loss does not
-        loss, err1, err5, dlogits = _impl(logits).softmax_xent(logits, labels, grad_scale=accum.grad_scale())
+        loss, err1, err5, dlogits = _impl(logits).softmax_xent(logits, labels, grad_scale=accum.grad_scale(),
+                                                               label_smoothing=label_smoothing)
         ctx.save_for_backward(dlogits)
         ctx.in_dtype = logits.dtype
         ctx.mark_non_differentiable(err1, err5)
@@ -497,12 +498,13 @@ class _SoftmaxXentFn(torch.autograd.Function):
     def backward(ctx, gl, g1, g5):
         (dlogits,) = ctx.saved_tensors
         # gl is a 0-dim tensor on the same device: no host sync, graph-capturable
-        return (dlogits * gl.to(dlogits.dtype)).to(ctx.in_dtype), None
+        return (dlogits * gl.to(dlogits.dtype)).to(ctx.in_dtype), None, None
 
 
-def softmax_xent(logits, labels):
-    """Returns (mean NLL, top-1 error, top-5 error) — fused on CUDA."""
-    return _SoftmaxXentFn.apply(logits, labels)
+def softmax_xent(logits, labels, label_smoothing=0.0):
+    """Returns (mean NLL, top-1 error, top-5 error) — fused on CUDA.  ``label_smoothing`` ε > 0: the loss (and its gradient) is the
+    cross-entropy against the soft target (1 − ε)·onehot + ε / C, as ``F.cross_entropy(..., label_smoothing=ε)``."""
+    return _SoftmaxXentFn.apply(logits, labels, float(label_smoothing))
 
 
 # --------------------------------------------------------------------------- GAN losses

@@ -173,21 +173,34 @@ def dropout(x, p_drop, mask):
 
 
 # --------------------------------------------------------------------------- softmax + NLL
-def softmax_xent(logits, labels, grad_scale=1.0):
-    """mean NLL, top-1 error, top-5 error, and d(mean NLL)/dlogits times ``grad_scale`` (1/n under gradient accumulation over n
-    micro-batches) (ref ``layers2.py:952-997``)."""
+def softmax_xent(logits, labels, grad_scale=1.0, weight=1.0, label_smoothing=0.0):
+    """weight · mean NLL, top-1 error, top-5 error, and d(mean NLL)/dlogits times weight · ``grad_scale`` (1/n under gradient
+    accumulation over n micro-batches) (ref ``layers2.py:952-997``).  ``label_smoothing`` ε > 0: the loss and its gradient are those
+    of the soft target (1 − ε)·onehot + ε / C (``F.cross_entropy(..., label_smoothing=ε)``); the errors do not change."""
     lg = logits.float()
     lsm = F.log_softmax(lg, dim=1)
     B = lg.shape[0]
-    loss = -lsm[torch.arange(B, device=lg.device), labels].mean()
+    rows = torch.arange(B, device=lg.device)
+    if label_smoothing:
+        eps = float(label_smoothing)
+        loss = -((1.0 - eps) * lsm[rows, labels] + eps * lsm.mean(1)).mean()
+    else:
+        loss = -lsm[rows, labels].mean()
     pred = lg.argmax(1)
     err1 = (pred != labels).float().mean()
     k = min(5, lg.shape[1])
     topk = lg.topk(k, dim=1).indices
     err5 = 1.0 - (topk == labels[:, None]).any(1).float().mean()
     dlogits = lsm.exp()
-    dlogits[torch.arange(B, device=lg.device), labels] -= 1.0
+    if label_smoothing:
+        dlogits[rows, labels] -= 1.0 - eps
+        dlogits -= eps / lg.shape[1]
+    else:
+        dlogits[rows, labels] -= 1.0
     dlogits = dlogits / B
+    if weight != 1.0:
+        loss = loss * weight
+        grad_scale = grad_scale * weight
     if grad_scale != 1.0:
         dlogits = dlogits * grad_scale
     return loss, err1, err5, dlogits
