@@ -105,6 +105,36 @@ void advance_step(void* step, cudaStream_t st);
 // target is (1 − ε)·onehot + ε / C in both the loss and dlogits (soft-target cross-entropy); ε = 0 is the plain NLL
 void softmax_xent(const void* logits, const void* labels, void* dlogits, void* rowstat, void* out3, int B, int C, float weight,
                   float grad_weight, float label_smoothing, int f32, cudaStream_t st);
+// Mixup / CutMix (ops/mixup.py owns the same layout on the Python side).  One MixRecord per training step, written by mix_draw on
+// the device and read by mix_batch and softmax_xent_mix: sample i is paired with j = B − 1 − i and trains against
+// λ·s(y_i) + (1 − λ)·s(y_j), s the (smoothed) one-hot target.
+enum MixMode : int { MIX_NONE = 0, MIX_MIXUP = 1, MIX_CUTMIX = 2 };
+struct MixRecord {                       // 64 bytes
+  int mode;                              // MixMode
+  float lam;                             // effective λ: the weight of y_i (1 when mode = MIX_NONE; CutMix: 1 − box area / (H·W))
+  double lam_raw;                        // the Beta(α, α) draw (1 when mode = MIX_NONE)
+  int cy, cx;                            // CutMix: box centre (0 otherwise)
+  int y0, y1, x0, x1;                    // CutMix: the clipped box [y0, y1) × [x0, x1) (0 otherwise)
+  int H, W;                              // image size the box refers to
+  int pad[4];
+};
+static_assert(sizeof(MixRecord) == 64, "MixRecord layout is shared with ops/mixup.py");
+struct MixParams {
+  double alpha, cutmix_alpha;            // Beta(α, α) of Mixup / of CutMix; 0 disables that mode
+  double switch_prob, prob;              // P(CutMix | both enabled), P(mix at all)
+  unsigned long long seed;
+  int rank;
+  int H, W;
+};
+// rec[t] = the draw of step counter value *step + t, t < n (the training step launches n = 1)
+void mix_draw(const MixParams& p, const void* step, void* rec, int n, cudaStream_t st);
+// in place on the NHWC batch x [B, H, W, C]: Mixup x_i ← λ·x_i + (1 − λ)·x_j (fp32, rounded once), CutMix swaps the box between
+// x_i and x_j; MIX_NONE leaves x untouched
+void mix_batch(void* x, const void* rec, int B, int H, int W, int C, int f32, cudaStream_t st);
+// softmax_xent against the mixed soft target of rec (label j from labels[B − 1 − b]); err1 / err5 count against y_i when λ ≥ ½,
+// else y_j
+void softmax_xent_mix(const void* logits, const void* labels, const void* rec, void* dlogits, void* rowstat, void* out3, int B, int C,
+                      float weight, float grad_weight, float label_smoothing, int f32, cudaStream_t st);
 // act: 0 none, 1 ReLU, 2 leaky ReLU (negative slope `slope`), 3 sigmoid (ACT_* in common.cuh).  accumulate = 1: db / db1 += the bias
 // gradient (no clear)
 void relu_bias_bwd(const void* dy, const void* y, void* dym, void* db, void* db1, int c_split, long long R, int C, long long ld, int act,

@@ -103,6 +103,14 @@ PYBIND11_MODULE(_tmpi_native, m) {
   m.def("softmax_xent", [](ptr_t logits, ptr_t labels, ptr_t dlogits, ptr_t rowstat, ptr_t out3, int B, int C, float weight, float grad_weight,
                            float label_smoothing, int f32, ptr_t st) {
     softmax_xent(P(logits), P(labels), P(dlogits), P(rowstat), P(out3), B, C, weight, grad_weight, label_smoothing, f32, S(st)); });
+  m.attr("MIX_RECORD_BYTES") = (int)sizeof(MixRecord);
+  m.def("mix_draw", [](double alpha, double cutmix_alpha, double switch_prob, double prob, unsigned long long seed, int rank, int H, int W,
+                       ptr_t step, ptr_t rec, int n, ptr_t st) {
+    mix_draw(MixParams{alpha, cutmix_alpha, switch_prob, prob, seed, rank, H, W}, P(step), P(rec), n, S(st)); });
+  m.def("mix_batch", [](ptr_t x, ptr_t rec, int B, int H, int W, int C, int f32, ptr_t st) { mix_batch(P(x), P(rec), B, H, W, C, f32, S(st)); });
+  m.def("softmax_xent_mix", [](ptr_t logits, ptr_t labels, ptr_t rec, ptr_t dlogits, ptr_t rowstat, ptr_t out3, int B, int C, float weight,
+                               float grad_weight, float label_smoothing, int f32, ptr_t st) {
+    softmax_xent_mix(P(logits), P(labels), P(rec), P(dlogits), P(rowstat), P(out3), B, C, weight, grad_weight, label_smoothing, f32, S(st)); });
   m.def("maxpool_relu_bias_bwd", [](ptr_t dyp, ptr_t arg, ptr_t y, ptr_t dym, ptr_t db0, ptr_t db1, int c_split, int N, int H, int W, int C,
                                     int Ho, int Wo, int k, int s, int p, int accumulate, ptr_t st) {
     maxpool_relu_bias_bwd(P(dyp), P(arg), P(y), P(dym), P(db0), P(db1), c_split, N, H, W, C, Ho, Wo, k, s, p, accumulate, S(st)); });

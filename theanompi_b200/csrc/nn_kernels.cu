@@ -649,6 +649,230 @@ void softmax_xent(const void* logits, const void* labels, void* dlogits, void* r
   count_launch(); TMPI_CHECK_LAUNCH("rowstat_mean"); ::tmpi::check_capture(st, "rowstat_mean");
 }
 
+// ============================================================================ Mixup / CutMix
+// The draw of one step (ops/reference.py: mix_draw is the same on the host).  Philox4x32-10 with key (seed_lo, seed_hi ^ rank) and
+// counter (j, 0xFFFFFFFF, step_lo, step_hi), j the block index within the step.  Dropout's and uniform_noise's second counter word
+// is the high word of a non-negative 64-bit element index, at most 0x7FFFFFFF, so none of their blocks is ever one of these,
+// whatever the keys.  Blocks: j = 0 the gate, switch and centre words; j = 1 the two U^(1/α) boosts; j = 2 + k attempt k of the
+// Gamma draw X, j = 2 + kMixAttempts + k attempt k of Y.  Every correctly rounded fp64 operation is an _rn intrinsic, so
+// --use_fast_math cannot contract it; log, cos and pow are the libdevice functions.
+constexpr int kMixAttempts = 16;         // Marsaglia–Tsang accepts ≥ 95 % of attempts: running out is ~1e-21 per variate
+constexpr uint32_t kMixCounterTag = 0xFFFFFFFFu;
+
+__device__ __forceinline__ double mix_u01(uint32_t w) { return __dmul_rn(__dadd_rn((double)w, 0.5), 2.3283064365386963e-10); }  // (0, 1)
+
+// Gamma(a) by Marsaglia–Tsang from Box–Muller normals (a < 1: Gamma(a + 1)·U^(1/a)); false if every attempt was rejected
+__device__ bool mix_gamma(double a, double boost_u, uint32_t j0, uint32_t s_lo, uint32_t s_hi, uint32_t k0, uint32_t k1, double* out) {
+  const double ae = a < 1.0 ? __dadd_rn(a, 1.0) : a;
+  const double d = __dsub_rn(ae, 1.0 / 3.0);
+  const double c = __ddiv_rn(1.0, __dsqrt_rn(__dmul_rn(9.0, d)));
+  for (int k = 0; k < kMixAttempts; ++k) {
+    uint32_t r[4];
+    philox4x32(j0 + (uint32_t)k, kMixCounterTag, s_lo, s_hi, k0, k1, r);
+    const double x = __dmul_rn(__dsqrt_rn(__dmul_rn(-2.0, log(mix_u01(r[0])))), cos(__dmul_rn(6.283185307179586, mix_u01(r[1]))));
+    double v = __dadd_rn(1.0, __dmul_rn(c, x));
+    if (v <= 0.0) continue;
+    v = __dmul_rn(__dmul_rn(v, v), v);
+    const double u = mix_u01(r[2]), x2 = __dmul_rn(x, x);
+    if (u < __dsub_rn(1.0, __dmul_rn(__dmul_rn(0.0331, x2), x2)) ||
+        log(u) < __dadd_rn(__dmul_rn(0.5, x2), __dmul_rn(d, __dadd_rn(__dsub_rn(1.0, v), log(v))))) {
+      double g = __dmul_rn(d, v);
+      if (a < 1.0) g = __dmul_rn(g, pow(boost_u, __ddiv_rn(1.0, a)));
+      *out = g;
+      return true;
+    }
+  }
+  return false;
+}
+
+__global__ void mix_draw_kernel(MixParams p, const unsigned long long* __restrict__ step, MixRecord* __restrict__ rec, int n) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n) return;
+  const unsigned long long s = *step + (unsigned long long)t;
+  const uint32_t s_lo = (uint32_t)s, s_hi = (uint32_t)(s >> 32);
+  const uint32_t k0 = (uint32_t)p.seed, k1 = (uint32_t)(p.seed >> 32) ^ (uint32_t)p.rank;
+  MixRecord r = {};
+  r.mode = MIX_NONE; r.lam = 1.f; r.lam_raw = 1.0; r.H = p.H; r.W = p.W;
+  uint32_t w0[4], w1[4];
+  philox4x32(0u, kMixCounterTag, s_lo, s_hi, k0, k1, w0);
+  if (mix_u01(w0[0]) < p.prob) {
+    const bool both = p.alpha > 0.0 && p.cutmix_alpha > 0.0;
+    const int mode = both ? (mix_u01(w0[1]) < p.switch_prob ? MIX_CUTMIX : MIX_MIXUP) : (p.cutmix_alpha > 0.0 ? MIX_CUTMIX : MIX_MIXUP);
+    const double a = mode == MIX_CUTMIX ? p.cutmix_alpha : p.alpha;
+    philox4x32(1u, kMixCounterTag, s_lo, s_hi, k0, k1, w1);
+    double gx, gy;
+    if (mix_gamma(a, mix_u01(w1[0]), 2u, s_lo, s_hi, k0, k1, &gx) &&
+        mix_gamma(a, mix_u01(w1[1]), 2u + kMixAttempts, s_lo, s_hi, k0, k1, &gy)) {
+      const double sum = __dadd_rn(gx, gy);
+      const double lam = sum > 0.0 ? __ddiv_rn(gx, sum) : 0.5;
+      r.mode = mode; r.lam_raw = lam;
+      if (mode == MIX_MIXUP) {
+        r.lam = __double2float_rn(lam);
+      } else {
+        const double cut = __dsqrt_rn(__dsub_rn(1.0, lam));
+        const int ch = (int)__dmul_rn((double)p.H, cut), cw = (int)__dmul_rn((double)p.W, cut);
+        r.cy = (int)(((unsigned long long)w0[2] * (unsigned)p.H) >> 32);
+        r.cx = (int)(((unsigned long long)w0[3] * (unsigned)p.W) >> 32);
+        r.y0 = min(max(r.cy - ch / 2, 0), p.H); r.y1 = min(max(r.cy + ch / 2, 0), p.H);
+        r.x0 = min(max(r.cx - cw / 2, 0), p.W); r.x1 = min(max(r.cx + cw / 2, 0), p.W);
+        const long long area = (long long)(r.y1 - r.y0) * (r.x1 - r.x0);
+        r.lam = __double2float_rn(__dsub_rn(1.0, __ddiv_rn((double)area, (double)((long long)p.H * p.W))));
+      }
+    }
+  }
+  rec[t] = r;
+}
+
+void mix_draw(const MixParams& p, const void* step, void* rec, int n, cudaStream_t st) {
+  if (n < 1 || p.H < 1 || p.W < 1) throw std::runtime_error("mix_draw: needs n >= 1 and a positive image size");
+  mix_draw_kernel<<<grid_for(n, 128), 128, 0, st>>>(p, (const unsigned long long*)step, (MixRecord*)rec, n);
+  count_launch(); TMPI_CHECK_LAUNCH("mix_draw"); ::tmpi::check_capture(st, "mix_draw");
+}
+
+// One thread per element position of a pair (i, j = B − 1 − i), blockIdx.y = i: it reads both rows and writes both, so the mix is
+// in place.  kVec: N-element 16-byte vectors (the row length n = H·W·C times sizeof(T) is a multiple of 16), else one element.  The
+// grid is sized for Mixup; CutMix CTAs whose elements lie outside the box rows return before touching the batch.
+template <typename T, bool kVec>
+__global__ void __launch_bounds__(256) mix_batch_kernel(T* __restrict__ x, const MixRecord* __restrict__ rec, int B, int H, int W, int C) {
+  constexpr int N = kVec ? VecIO<T>::N : 1;
+  __shared__ MixRecord r;
+  if (threadIdx.x == 0) r = *rec;
+  __syncthreads();
+  if (r.mode == MIX_NONE) return;
+  const long long rowlen = (long long)W * C, n = rowlen * H;
+  const long long cta0 = (long long)blockIdx.x * blockDim.x * N;
+  if (r.mode == MIX_CUTMIX) {
+    const long long cta1 = min(n, cta0 + (long long)blockDim.x * N) - 1;
+    if (cta1 / rowlen < r.y0 || cta0 / rowlen >= r.y1) return;
+  }
+  const long long e0 = cta0 + (long long)threadIdx.x * N;
+  if (e0 >= n) return;
+  const int i = blockIdx.y, j = B - 1 - i;
+  T* xi = x + (long long)i * n + e0;
+  T* xj = x + (long long)j * n + e0;
+  float a[N], b[N];
+  if constexpr (kVec) { VecIO<T>::ld(xi, a); VecIO<T>::ld(xj, b); }
+  else { a[0] = to_f(*xi); b[0] = to_f(*xj); }
+  bool any = false;
+  if (r.mode == MIX_MIXUP) {
+    const float lam = r.lam, oml = __fsub_rn(1.f, lam);
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+      const float na = __fadd_rn(__fmul_rn(lam, a[k]), __fmul_rn(oml, b[k]));
+      const float nb = __fadd_rn(__fmul_rn(lam, b[k]), __fmul_rn(oml, a[k]));
+      a[k] = na; b[k] = nb;
+    }
+    any = true;
+  } else {
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+      const long long e = e0 + k;
+      const int h = (int)(e / rowlen), w = (int)((e - (long long)h * rowlen) / C);
+      if (h >= r.y0 && h < r.y1 && w >= r.x0 && w < r.x1) { const float t = a[k]; a[k] = b[k]; b[k] = t; any = true; }
+    }
+  }
+  if (!any) return;
+  if constexpr (kVec) { VecIO<T>::st(xi, a); if (j != i) VecIO<T>::st(xj, b); }
+  else { *xi = from_f<T>(a[0]); if (j != i) *xj = from_f<T>(b[0]); }
+}
+
+void mix_batch(void* x, const void* rec, int B, int H, int W, int C, int f32, cudaStream_t st) {
+  const int pairs = (B + 1) / 2;
+  if (B < 1 || H < 1 || W < 1 || C < 1 || pairs > 65535) throw std::runtime_error("mix_batch: needs 1 <= B <= 131070 and a non-empty image");
+  const long long n = (long long)H * W * C;
+  const int esz = f32 ? 4 : 2;
+  const bool vec = (n * esz) % 16 == 0 && ((uintptr_t)x & 15) == 0;
+  const long long units = vec ? n * esz / 16 : n;
+  const dim3 grid((unsigned)grid_for(units, 256), (unsigned)pairs);
+  auto R = (const MixRecord*)rec;
+  if (f32) {
+    if (vec) mix_batch_kernel<float, true><<<grid, 256, 0, st>>>((float*)x, R, B, H, W, C);
+    else mix_batch_kernel<float, false><<<grid, 256, 0, st>>>((float*)x, R, B, H, W, C);
+  } else {
+    if (vec) mix_batch_kernel<__nv_bfloat16, true><<<grid, 256, 0, st>>>((__nv_bfloat16*)x, R, B, H, W, C);
+    else mix_batch_kernel<__nv_bfloat16, false><<<grid, 256, 0, st>>>((__nv_bfloat16*)x, R, B, H, W, C);
+  }
+  count_launch(); TMPI_CHECK_LAUNCH("mix_batch"); ::tmpi::check_capture(st, "mix_batch");
+}
+
+// softmax_xent_kernel against the mixed soft target q = on·(λ·onehot(y_i) + (1 − λ)·onehot(y_j)) + off (on = 1 − ε, off = ε / C;
+// ε = 0 gives off = 0 exactly), with λ = 1 when the record's mode is MIX_NONE:
+//   rowstat[3b] = log se − on·(λ·(z_i − max) + (1 − λ)·(z_j − max)) − off·Σ(z − max),   dlogits = (softmax − q) * scale,
+// and err1 / err5 rank the logit of the larger-weight label (y_i when λ ≥ ½, else y_j).
+template <typename T>
+__global__ void softmax_xent_mix_kernel(const T* __restrict__ logits, const long long* __restrict__ labels,
+                                        const MixRecord* __restrict__ rec, T* __restrict__ dlogits, float* __restrict__ rowstat, int C,
+                                        float scale, float on, float off) {
+  const int b = blockIdx.x;
+  const T* row = logits + (long long)b * C;
+  const int yi = (int)labels[b], yj = (int)labels[gridDim.x - 1 - b];
+  const float lam = rec->mode != MIX_NONE ? rec->lam : 1.f, oml = 1.f - lam;
+  const int label = lam >= 0.5f ? yi : yj;                      // the errors' label
+  __shared__ float red[32];
+  __shared__ float bcast;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  float mx = -INFINITY;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) mx = fmaxf(mx, to_f(row[c]));
+  mx = warp_max(mx);
+  if (lane == 0) red[warp] = mx;
+  __syncthreads();
+  if (warp == 0) { float v = lane < nw ? red[lane] : -INFINITY; v = warp_max(v); if (lane == 0) bcast = v; }
+  __syncthreads();
+  mx = bcast;
+  __syncthreads();
+  const float lab = to_f(row[label]);
+  float se = 0.f, gt = 0.f, sz = 0.f;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    const float v = to_f(row[c]);
+    se += __expf(v - mx);
+    gt += (v > lab || (v == lab && c < label)) ? 1.f : 0.f;     // rank of the errors' label's logit
+    sz += v - mx;
+  }
+  se = warp_sum(se); gt = warp_sum(gt); sz = warp_sum(sz);
+  if (lane == 0) red[warp] = se;
+  __syncthreads();
+  if (warp == 0) { float v = lane < nw ? red[lane] : 0.f; v = warp_sum(v); if (lane == 0) bcast = v; }
+  __syncthreads();
+  se = bcast;
+  __syncthreads();
+  if (lane == 0) red[warp] = gt;
+  __syncthreads();
+  if (warp == 0) { float v = lane < nw ? red[lane] : 0.f; v = warp_sum(v); if (lane == 0) bcast = v; }
+  __syncthreads();
+  gt = bcast;
+  __syncthreads();
+  if (lane == 0) red[warp] = sz;                                // Σ(z − max) to thread 0
+  __syncthreads();
+  if (warp == 0) { float v = lane < nw ? red[lane] : 0.f; sz = warp_sum(v); }
+  const float inv = 1.f / se;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    float pr = __expf(to_f(row[c]) - mx) * inv - off;
+    if (c == yi) pr -= on * lam;
+    if (c == yj) pr -= on * oml;
+    dlogits[(long long)b * C + c] = from_f<T>(pr * scale);
+  }
+  if (threadIdx.x == 0) {
+    rowstat[3 * b + 0] = __logf(se) - on * (lam * (to_f(row[yi]) - mx) + oml * (to_f(row[yj]) - mx)) - off * sz;
+    rowstat[3 * b + 1] = gt >= 1.f ? 1.f : 0.f;
+    rowstat[3 * b + 2] = gt >= 5.f ? 1.f : 0.f;
+  }
+}
+
+void softmax_xent_mix(const void* logits, const void* labels, const void* rec, void* dlogits, void* rowstat, void* out3, int B, int C,
+                      float weight, float grad_weight, float label_smoothing, int f32, cudaStream_t st) {
+  if (!(label_smoothing >= 0.f && label_smoothing <= 1.f)) throw std::runtime_error("softmax_xent_mix: label_smoothing must be in [0, 1]");
+  if (!rec) throw std::runtime_error("softmax_xent_mix: needs the step's mix record");
+  auto LB = (const long long*)labels; auto RS = (float*)rowstat; auto R = (const MixRecord*)rec;
+  const float scale = grad_weight / (float)B;
+  const float on = 1.f - label_smoothing, off = label_smoothing / (float)C;
+  if (f32) softmax_xent_mix_kernel<float><<<B, 256, 0, st>>>((const float*)logits, LB, R, (float*)dlogits, RS, C, scale, on, off);
+  else softmax_xent_mix_kernel<__nv_bfloat16><<<B, 256, 0, st>>>((const __nv_bfloat16*)logits, LB, R, (__nv_bfloat16*)dlogits, RS, C,
+                                                                   scale, on, off);
+  count_launch(); TMPI_CHECK_LAUNCH("softmax_xent_mix"); ::tmpi::check_capture(st, "softmax_xent_mix");
+  rowstat_mean_kernel<<<1, 256, 0, st>>>((const float*)rowstat, (float*)out3, B, weight);
+  count_launch(); TMPI_CHECK_LAUNCH("rowstat_mean"); ::tmpi::check_capture(st, "rowstat_mean");
+}
+
 // ============================================================================ activation mask + bias gradient
 // dym = act'(y) * dy (contiguous [R, C]; ReLU: dy * (y > 0));  db[c] += sum_r dym[r, c]   (db pre-zeroed by the launcher, unless it
 // accumulates a gradient over several micro-batches)

@@ -66,6 +66,7 @@ class ModelBase(object):
     supports_grad_accum = True     # config['grad_accum'] > 1 (False: the model refuses it at compile_iter_fns)
     supports_lr_schedule = True    # config['lr_schedule'] (False: the model refuses it at compile_iter_fns)
     supports_label_smoothing = True    # config['label_smoothing'] > 0 (False: no classifier head; refused at compile_iter_fns)
+    supports_mixup = True          # config['mixup'] (False: no image batch before a first convolution; refused at compile_iter_fns)
     name = "Model"
 
     def __init__(self, config):
@@ -116,6 +117,10 @@ class ModelBase(object):
         # label smoothing ε of the training loss (cross-entropy against (1 − ε)·onehot + ε / C; 0 = plain NLL); validation stays
         # plain NLL.  Checked by check_label_smoothing at compile_iter_fns
         self.label_smoothing = config.get("label_smoothing", 0.0)
+        # Mixup / CutMix of the training batch (a dict, ops/mixup.py; None = off): one draw per training step on the device, the
+        # batch mixed at the mix point (mix_input) and the loss taken against the mixed target.  Built by check_mixup
+        self.mixup = config.get("mixup")
+        self.mixer = None
         self.base_lr = np.float32(self.learning_rate)
         self.current_t = self.subb_t = 0
         self.current_v = self.subb_v = 0
@@ -183,17 +188,24 @@ class ModelBase(object):
         """Return logits-layer output; must leave ``self.output_layer`` evaluated."""
         raise NotImplementedError
 
-    def loss(self, x, y, label_smoothing=0.0):
+    def loss(self, x, y, label_smoothing=0.0, mix=None):
         """(cost, top-1 error, top-5 error); the cost is the mean NLL, or with ``label_smoothing`` ε > 0 the cross-entropy against
-        (1 − ε)·onehot + ε / C."""
+        (1 − ε)·onehot + ε / C.  ``mix``: the step's Mixup / CutMix record; the cost is then the cross-entropy against its mixed
+        target and the errors count against the label with the larger weight."""
         self.forward(x)
         sm = self.output_layer
-        return sm.negative_log_likelihood(y, label_smoothing), sm.errors(y), sm.errors_top_x(y)
+        return sm.negative_log_likelihood(y, label_smoothing, mix), sm.errors(y), sm.errors_top_x(y)
 
     # ------------------------------------------------------------------ step functions
     def _fwd_bwd_eager(self):
-        # the training loss carries the label smoothing (read on the host here, so a captured step keeps the ε it was captured with)
-        cost, err, err5 = self.loss(self.x_in, self.y_in, self.label_smoothing)
+        # the training loss carries the label smoothing (read on the host here, so a captured step keeps the ε it was captured with);
+        # with config['mixup'] the step's draw comes first, keyed by the device step counter, so every graph replay draws anew
+        if self.mixer is None:
+            cost, err, err5 = self.loss(self.x_in, self.y_in, self.label_smoothing)
+        else:
+            rec = self.mixer.draw()
+            self.mix_input(rec)
+            cost, err, err5 = self.loss(self.x_in, self.y_in, self.label_smoothing, mix=rec)
         self._dbg_capture("forward")
         cost.backward()
         return cost.detach(), err.detach()
@@ -348,6 +360,30 @@ class ModelBase(object):
                              "cross-entropy of AlexNet, GoogLeNet, Cifar10_model, VGG16, ResNet50, Wide_ResNet, the LSTM and their "
                              "torch twins" % (self.name, eps))
 
+    # ------------------------------------------------------------------ Mixup / CutMix
+    @property
+    def mix_hw(self):
+        """(H, W) of the batch at the mix point, the tensor that enters the first convolution: x_in by default."""
+        return tuple(self.input_shape[1:3])
+
+    def mix_input(self, rec):
+        """Mix this step's batch at the mix point as the record ``rec`` says: x_in, in place.  x_in is refilled from shared_x every
+        step; shared_x itself (the loader's buffer, sliced into sub-batches and read by validation) is never mixed."""
+        ops.mix_batch(self.x_in, rec)
+
+    def check_mixup(self):
+        """``config['mixup']`` must be None or a valid dict (ops/mixup.py: check_config; a ValueError names the offending key), and a
+        dict needs a model with an image batch before its first convolution; builds the step's :class:`Mixer`."""
+        self.mixer = None
+        if self.mixup is None:
+            return
+        from ..ops.mixup import Mixer, check_config
+        cfg = check_config(self.mixup)
+        if not self.supports_mixup:
+            raise ValueError("%s: mixup is not supported; it mixes the image batch of AlexNet, GoogLeNet, Cifar10_model, VGG16, "
+                             "ResNet50 and Wide_ResNet" % self.name)
+        self.mixer = Mixer(cfg, self.rank, self.mix_hw, self.device)
+
     # ------------------------------------------------------------------ per-update learning-rate schedule
     @property
     def updates_per_epoch(self):
@@ -498,6 +534,7 @@ class ModelBase(object):
             raise ValueError("%s: optimizer must be 'lamb', 'sgd' or 'lars', not %r" % (self.name, self.optimizer))
         self.check_grad_accum(fused_tail)
         self.check_label_smoothing()
+        self.check_mixup()
         self.setup_lr_schedule()
         k = self.size if sync_type == "cdd" else 1
         if self.optimizer in ("lars", "lamb") and fused_tail is not None:

@@ -4,6 +4,7 @@ Softmax10; batch 256, lr 0.01 ÷10 at {50,60,65}, μ 0.9, wd 1e-4 (``cifar10.py:
 The model the EASGD / GOSGD examples train."""
 from __future__ import annotations
 
+from .. import ops
 from .base import ModelBase
 from .layers2 import (FC, Constant, Conv, Crop, Dropout, Flatten, Normal, Pool, Softmax, Subtract,
                       forward_chain, get_layers, get_params)
@@ -55,8 +56,8 @@ class Cifar10_model(ModelBase):
         v, B, C = self.verbose, self.batch_size, self.channels
         sub = Subtract(input=None, input_shape=(B, self.data.height, self.data.width, C),
                        subtract_arr=self.data.rawdata[4], printinfo=v)
-        crop = Crop(input=sub, output_shape=(B, self.input_height, self.input_width, C),
-                    flag_batch=self.batch_crop_mirror, printinfo=v)
+        crop = self.crop = Crop(input=sub, output_shape=(B, self.input_height, self.input_width, C),
+                                flag_batch=self.batch_crop_mirror, printinfo=v)
         c1 = Conv(input=crop, convstride=1, padsize=0, W=Normal((64, 5, 5, C), std=0.05), b=Constant((64,), val=0), printinfo=v)
         p1 = Pool(input=c1, poolsize=2, poolstride=2, poolpad=0, mode="max", printinfo=v)
         c2 = Conv(input=p1, convstride=1, padsize=0, W=Normal((128, 5, 5, 64), std=0.05), b=Constant((128,), val=0), printinfo=v)
@@ -70,4 +71,17 @@ class Cifar10_model(ModelBase):
         self.output_layer = sm
 
     def forward(self, x):
-        return forward_chain(self.layers, x)
+        rec, self._mix_rec = getattr(self, "_mix_rec", None), None
+        if rec is None:
+            return forward_chain(self.layers, x)
+        k = self.layers.index(self.crop) + 1
+        return forward_chain(self.layers[k:], ops.mix_batch(forward_chain(self.layers[:k], x), rec))
+
+    # Mixup / CutMix mix the output of the in-graph Crop, the tensor that enters the first convolution: the CutMix box and λ refer
+    # to the 28×28 crop
+    @property
+    def mix_hw(self):
+        return (self.input_height, self.input_width)
+
+    def mix_input(self, rec):
+        self._mix_rec = rec                      # taken by the forward that follows

@@ -99,8 +99,8 @@ class Aux_tower(Layer):
             x = l.forward(x)
         return x
 
-    def negative_log_likelihood(self, y, label_smoothing=0.0):
-        return self.softmax_layer.negative_log_likelihood(y, label_smoothing)
+    def negative_log_likelihood(self, y, label_smoothing=0.0, mix=None):
+        return self.softmax_layer.negative_log_likelihood(y, label_smoothing, mix)
 
 
 class GoogLeNet(ModelBase):
@@ -177,13 +177,13 @@ class GoogLeNet(ModelBase):
         self._taps = taps
         return x
 
-    def loss(self, x, y, label_smoothing=0.0):
+    def loss(self, x, y, label_smoothing=0.0, mix=None):
         self.forward(x)
         sm = self.output_layer
-        cost = sm.negative_log_likelihood(y, label_smoothing)
+        cost = sm.negative_log_likelihood(y, label_smoothing, mix)
         if Dropout.layers and Dropout.layers[0].flag_on:          # aux towers only contribute while training
             self.aux1.forward(self._taps[id(self._tap1)])
             self.aux2.forward(self._taps[id(self._tap2)])
-            cost = (cost + 0.3 * self.aux1.negative_log_likelihood(y, label_smoothing)
-                    + 0.3 * self.aux2.negative_log_likelihood(y, label_smoothing))
+            cost = (cost + 0.3 * self.aux1.negative_log_likelihood(y, label_smoothing, mix)
+                    + 0.3 * self.aux2.negative_log_likelihood(y, label_smoothing, mix))
         return cost, sm.errors(y), sm.errors_top_x(y)

@@ -159,6 +159,7 @@ class Wide_ResNet(ModelBase):
         self.check_grad_clip(optimizer="adam")
         self.check_grad_accum(fused_tail)
         self.check_label_smoothing()
+        self.check_mixup()
         self.setup_lr_schedule()
         from ...utils.opt import FlatAdam
         self.sync_type = "avg"

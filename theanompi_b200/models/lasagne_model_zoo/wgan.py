@@ -45,6 +45,7 @@ def build_critic(in_ch=1, size=28):
 
 class WGAN(TorchModelBase):
     supports_label_smoothing = False   # no classifier head
+    supports_mixup = False             # no classifier head
     loss_kind = "wgan"
     n_epochs = num_epochs
     batch_size = file_batch_size = batchsize
@@ -100,6 +101,7 @@ class WGAN(TorchModelBase):
         self.refuse_grad_clip()
         self.check_grad_accum()
         self.check_label_smoothing()
+        self.check_mixup()
         self.setup_lr_schedule()
         self.sync_type = "avg"
         self.opt_c = torch.optim.RMSprop(self.critic_params, lr=self.learning_rate)
@@ -239,6 +241,7 @@ class NativeWGAN(ModelBase):
     supports_grad_accum = False    # its critic / generator steps keep their own gaccum accumulation
     supports_lr_schedule = False   # two arenas and critic / generator step ratios: the reference's per-epoch decay
     supports_label_smoothing = False   # no classifier head
+    supports_mixup = False             # no classifier head
     loss_kind = "wgan"
     n_epochs = num_epochs
     batch_size = file_batch_size = batchsize
@@ -396,6 +399,7 @@ class NativeWGAN(ModelBase):
     def compile_iter_fns(self, sync_type="avg", **kw):
         self.check_grad_accum()
         self.check_label_smoothing()
+        self.check_mixup()
         self.setup_lr_schedule()
         self.sync_type = "avg"
         self.vels, self.vels2 = [], []

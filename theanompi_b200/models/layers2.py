@@ -590,13 +590,14 @@ class Softmax(Layer):
         self._cache = None
         return self.logits
 
-    def _eval(self, y, label_smoothing=None):
-        """(y, ε, loss, err1, err5) of one launch on this forward's logits, cached per (y, ε); ``label_smoothing`` None takes a
-        cached launch of any ε (the errors do not depend on it), else ε = 0."""
+    def _eval(self, y, label_smoothing=None, mix=None):
+        """(y, ε, mix, loss, err1, err5) of one launch on this forward's logits, cached per (y, ε, mix record); ``label_smoothing``
+        None takes the cached launch whatever its ε and mix (the errors of a training step are those of its loss launch), else
+        ε = 0 and no mix."""
         c = self._cache
-        if c is None or c[0] is not y or (label_smoothing is not None and c[1] != label_smoothing):
+        if c is None or c[0] is not y or (label_smoothing is not None and (c[1] != label_smoothing or c[2] is not mix)):
             eps = label_smoothing or 0.0
-            self._cache = (y, eps) + tuple(ops.softmax_xent(self.logits, y, eps))
+            self._cache = (y, eps, mix) + tuple(ops.softmax_xent(self.logits, y, eps, mix))
         return self._cache
 
     @property
@@ -607,19 +608,20 @@ class Softmax(Layer):
     def y_pred(self):
         return self.logits.argmax(1)
 
-    def negative_log_likelihood(self, y, label_smoothing=0.0):
-        """Mean NLL of ``y``; ``label_smoothing`` ε > 0 gives the cross-entropy against (1 − ε)·onehot + ε / C instead."""
-        return self._eval(y, label_smoothing)[2]
+    def negative_log_likelihood(self, y, label_smoothing=0.0, mix=None):
+        """Mean NLL of ``y``; ``label_smoothing`` ε > 0 gives the cross-entropy against (1 − ε)·onehot + ε / C instead, and a Mixup /
+        CutMix record ``mix`` the cross-entropy against its mixed target (ops/mixup.py)."""
+        return self._eval(y, label_smoothing, mix)[3]
 
     def errors(self, y):
-        return self._eval(y)[3]
+        return self._eval(y)[4]
 
     def errors_top_x(self, y, num_top=5):
         if num_top != 5:
             lg = self.logits.float()
             topk = lg.topk(num_top, dim=1).indices
             return 1.0 - (topk == y[:, None]).any(1).float().mean()
-        return self._eval(y)[4]
+        return self._eval(y)[5]
 
 
 # =========================================================================== graph helpers

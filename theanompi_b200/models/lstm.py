@@ -109,6 +109,7 @@ class LSTM(ModelBase):
     sequence-length bucket (:func:`bucket_len`): the batch is padded to its bucket, copied into the bucket's static buffers and
     the bucket's graph (forward, backward, update) is replayed.  ``cuda_graph=False`` and the CPU run the step eagerly on the
     unpadded batch; validation is always eager."""
+    supports_mixup = False         # token input: nothing to mix
     supports_grad_accum = False    # one graph per sequence-length bucket, each with its own update
     n_epochs = max_epochs
     batch_size = file_batch_size = batch_size
@@ -186,6 +187,7 @@ class LSTM(ModelBase):
         self.check_grad_clip()
         self.check_grad_accum()
         self.check_label_smoothing()
+        self.check_mixup()
         self.setup_lr_schedule()
         self.sync_type = "avg"
         self._make_opt()
@@ -330,6 +332,7 @@ class LSTMTorch(TorchModelBase):
         self.refuse_grad_clip()
         self.check_grad_accum()
         self.check_label_smoothing()
+        self.check_mixup()
         self.setup_lr_schedule()
         self.sync_type = "avg"
         self.torch_opt = self.make_torch_optimizer(self.params)

@@ -43,6 +43,7 @@ class TorchModelBase(ModelBase):
     autocast = True
     supports_grad_accum = False    # torch autograd writes .grad: the native accumulate mode does not reach it
     supports_lr_schedule = False   # the library yardsticks keep the per-epoch lr policies
+    supports_mixup = False         # the library yardsticks train on the plain batch
 
     def finalize_torch(self, module, input_shape, exchanged=None):
         self.module = module.to(self.device)
@@ -112,6 +113,7 @@ class TorchModelBase(ModelBase):
         self.refuse_grad_clip()
         self.check_grad_accum(fused_tail)
         self.check_label_smoothing()
+        self.check_mixup()
         self.setup_lr_schedule()
         self.torch_opt = self.make_torch_optimizer(self.params)
         if self.torch_opt is None:

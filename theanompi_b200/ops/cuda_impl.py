@@ -667,10 +667,12 @@ def dropout_bwd(dy, mask):
     return dx
 
 
-def softmax_xent(logits, labels, weight=1.0, grad_scale=1.0, label_smoothing=0.0):
+def softmax_xent(logits, labels, weight=1.0, grad_scale=1.0, label_smoothing=0.0, mix=None):
     """(weight · mean NLL, top-1 error, top-5 error, dlogits); dlogits is the gradient of the mean NLL times weight · grad_scale
     (``grad_scale`` = 1/n under gradient accumulation over n micro-batches), scaled in fp32 inside the kernel.  ``label_smoothing``
-    ε > 0 makes the loss and dlogits those of the soft target (1 − ε)·onehot + ε / C, in the same launch."""
+    ε > 0 makes the loss and dlogits those of the soft target (1 − ε)·onehot + ε / C, in the same launch.  ``mix`` (the step's
+    Mixup / CutMix record on the device, ops/mixup.py) launches the mixing instantiation instead: the target is
+    λ·s(y_i) + (1 − λ)·s(y_j) with j = B − 1 − i (see reference.softmax_xent_mix)."""
     lg = _bf(logits).contiguous()
     B_, C = lg.shape
     labels = labels.contiguous()
@@ -678,9 +680,47 @@ def softmax_xent(logits, labels, weight=1.0, grad_scale=1.0, label_smoothing=0.0
     dl = torch.empty_like(lg)
     rowstat = torch.empty((B_, 3), dtype=torch.float32, device=lg.device)
     out3 = torch.empty(3, dtype=torch.float32, device=lg.device)
-    L().softmax_xent(lg.data_ptr(), labels.data_ptr(), dl.data_ptr(), rowstat.data_ptr(), out3.data_ptr(), B_, C, float(weight),
-                     float(weight) * float(grad_scale), float(label_smoothing), int(_is32(lg)), _st(lg))
+    if mix is None:
+        L().softmax_xent(lg.data_ptr(), labels.data_ptr(), dl.data_ptr(), rowstat.data_ptr(), out3.data_ptr(), B_, C, float(weight),
+                         float(weight) * float(grad_scale), float(label_smoothing), int(_is32(lg)), _st(lg))
+    else:
+        _check_record(mix, lg.device)
+        L().softmax_xent_mix(lg.data_ptr(), labels.data_ptr(), mix.data_ptr(), dl.data_ptr(), rowstat.data_ptr(), out3.data_ptr(), B_, C,
+                             float(weight), float(weight) * float(grad_scale), float(label_smoothing), int(_is32(lg)), _st(lg))
     return out3[0], out3[1], out3[2], dl
+
+
+def _check_record(rec, device):
+    from .mixup import RECORD_BYTES
+    if not (rec.is_cuda and rec.device == device and rec.dtype == torch.uint8 and rec.is_contiguous() and rec.numel() % RECORD_BYTES == 0
+            and rec.data_ptr() % 8 == 0):
+        raise ValueError("a mix record is a contiguous uint8 tensor of %d bytes on %s" % (RECORD_BYTES, device))
+
+
+def mix_draw(cfg, rank, hw, step, n=1, out=None):
+    """``n`` Mixup / CutMix records (uint8 [n · 64] on the step counter's device, or into ``out``): record t is the draw of step
+    counter value ``*step + t`` (one ``mix_draw_kernel`` launch that reads the int64 device counter ``step``, so a replayed CUDA graph
+    draws anew); ``cfg`` is a validated ``config['mixup']``, ``hw`` the image size at the mix point.  reference.mix_draw makes the
+    same draw on the CPU."""
+    from .mixup import RECORD_BYTES
+    rec = out if out is not None else torch.empty(n * RECORD_BYTES, dtype=torch.uint8, device=step.device)
+    _check_record(rec, step.device)
+    if rec.numel() != n * RECORD_BYTES:
+        raise ValueError("mix_draw: %d records need %d bytes, not %d" % (n, n * RECORD_BYTES, rec.numel()))
+    L().mix_draw(float(cfg["alpha"]), float(cfg["cutmix_alpha"]), float(cfg["switch_prob"]), float(cfg["prob"]), int(cfg["seed"]),
+                 int(rank), int(hw[0]), int(hw[1]), step.data_ptr(), rec.data_ptr(), int(n), _st(step))
+    return rec
+
+
+def mix_batch(x, rec):
+    """Mix the NHWC batch ``x`` in place as the device record ``rec`` says (one ``mix_batch_kernel`` launch; 16-byte vectors when a
+    row of H·W·C elements is a multiple of 16 bytes, else one element per thread).  Returns ``x``."""
+    if x.dim() != 4 or not x.is_contiguous() or x.dtype not in (BF16, F32):
+        raise ValueError("mix_batch: needs a contiguous bf16 or fp32 NHWC batch, not %s %s" % (x.dtype, tuple(x.shape)))
+    _check_record(rec, x.device)
+    B_, H, W, C = x.shape
+    L().mix_batch(x.data_ptr(), rec.data_ptr(), B_, H, W, C, int(_is32(x)), _st(x))
+    return x
 
 
 def gan_loss(scores, kind, a):

@@ -485,10 +485,10 @@ def dropout(x, p_drop, training, layer_id=0):
 # --------------------------------------------------------------------------- softmax + NLL
 class _SoftmaxXentFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, logits, labels, label_smoothing):
+    def forward(ctx, logits, labels, label_smoothing, mix):
         # under gradient accumulation over n micro-batches dlogits carries 1/n (in fp32, inside the kernel); the loss does not
         loss, err1, err5, dlogits = _impl(logits).softmax_xent(logits, labels, grad_scale=accum.grad_scale(),
-                                                               label_smoothing=label_smoothing)
+                                                               label_smoothing=label_smoothing, mix=mix)
         ctx.save_for_backward(dlogits)
         ctx.in_dtype = logits.dtype
         ctx.mark_non_differentiable(err1, err5)
@@ -498,13 +498,35 @@ class _SoftmaxXentFn(torch.autograd.Function):
     def backward(ctx, gl, g1, g5):
         (dlogits,) = ctx.saved_tensors
         # gl is a 0-dim tensor on the same device: no host sync, graph-capturable
-        return (dlogits * gl.to(dlogits.dtype)).to(ctx.in_dtype), None, None
+        return (dlogits * gl.to(dlogits.dtype)).to(ctx.in_dtype), None, None, None
 
 
-def softmax_xent(logits, labels, label_smoothing=0.0):
+def softmax_xent(logits, labels, label_smoothing=0.0, mix=None):
     """Returns (mean NLL, top-1 error, top-5 error) — fused on CUDA.  ``label_smoothing`` ε > 0: the loss (and its gradient) is the
-    cross-entropy against the soft target (1 − ε)·onehot + ε / C, as ``F.cross_entropy(..., label_smoothing=ε)``."""
-    return _SoftmaxXentFn.apply(logits, labels, float(label_smoothing))
+    cross-entropy against the soft target (1 − ε)·onehot + ε / C, as ``F.cross_entropy(..., label_smoothing=ε)``.  ``mix``: the
+    step's Mixup / CutMix record (ops/mixup.py); the target is then λ·s(y_i) + (1 − λ)·s(y_j) with j = B − 1 − i, and the errors count
+    against the label with the larger weight."""
+    return _SoftmaxXentFn.apply(logits, labels, float(label_smoothing), mix)
+
+
+def mix_draw(cfg, rank, hw, out):
+    """This step's Mixup / CutMix record (``cfg`` a validated ``config['mixup']``, ``hw`` the image size at the mix point) into
+    ``out``, a uint8 tensor of ops/mixup.py's 64 bytes: on CUDA drawn by the kernel from the device step counter, on the CPU by
+    :func:`reference.mix_draw` from the host one.  Returns ``out``."""
+    if out.is_cuda:
+        from . import cuda_impl
+        return cuda_impl.mix_draw(cfg, rank, hw, cuda_impl.step_counter(out.device), out=out)
+    from .mixup import encode
+    return out.copy_(encode(ref.mix_draw(cfg, cfg["seed"], rank, _RNG["step"], hw)))
+
+
+def mix_batch(x, rec):
+    """Mix the NHWC batch ``x`` in place (no autograd: it is an input) as the Mixup / CutMix record ``rec`` says; returns ``x``."""
+    if x.is_cuda:
+        from . import cuda_impl
+        return cuda_impl.mix_batch(x, rec)
+    with torch.no_grad():
+        return x.copy_(ref.mix_batch(x, rec))
 
 
 # --------------------------------------------------------------------------- GAN losses

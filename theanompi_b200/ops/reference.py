@@ -173,10 +173,13 @@ def dropout(x, p_drop, mask):
 
 
 # --------------------------------------------------------------------------- softmax + NLL
-def softmax_xent(logits, labels, grad_scale=1.0, weight=1.0, label_smoothing=0.0):
+def softmax_xent(logits, labels, grad_scale=1.0, weight=1.0, label_smoothing=0.0, mix=None):
     """weight · mean NLL, top-1 error, top-5 error, and d(mean NLL)/dlogits times weight · ``grad_scale`` (1/n under gradient
     accumulation over n micro-batches) (ref ``layers2.py:952-997``).  ``label_smoothing`` ε > 0: the loss and its gradient are those
-    of the soft target (1 − ε)·onehot + ε / C (``F.cross_entropy(..., label_smoothing=ε)``); the errors do not change."""
+    of the soft target (1 − ε)·onehot + ε / C (``F.cross_entropy(..., label_smoothing=ε)``); the errors do not change.  ``mix`` (a
+    Mixup / CutMix record, ops/mixup.py): see :func:`softmax_xent_mix`."""
+    if mix is not None:
+        return softmax_xent_mix(logits, labels, mix, grad_scale, weight, label_smoothing)
     lg = logits.float()
     lsm = F.log_softmax(lg, dim=1)
     B = lg.shape[0]
@@ -204,6 +207,28 @@ def softmax_xent(logits, labels, grad_scale=1.0, weight=1.0, label_smoothing=0.0
     if grad_scale != 1.0:
         dlogits = dlogits * grad_scale
     return loss, err1, err5, dlogits
+
+
+def softmax_xent_mix(logits, labels, mix, grad_scale=1.0, weight=1.0, label_smoothing=0.0):
+    """:func:`softmax_xent` against the mixed soft target q = λ·s(y_i) + (1 − λ)·s(y_j) of the record ``mix``, with j = B − 1 − i
+    and s(y) = (1 − ε)·onehot(y) + ε / C: the loss −Σ q·log p and its gradient (p − q) / B (times weight · grad_scale); the top-1 /
+    top-5 errors count against y_i when λ ≥ ½, else against y_j."""
+    lg = logits.float()
+    B, C = lg.shape
+    lam = mix_lambda(mix)
+    eps = float(label_smoothing)
+    lsm = F.log_softmax(lg, dim=1)
+
+    def soft(y):
+        return (1.0 - eps) * F.one_hot(y, C).float() + eps / C
+    q = lam * soft(labels) + (1.0 - lam) * soft(labels.flip(0))
+    loss = -(q * lsm).sum(1).mean()
+    ye = labels if lam >= 0.5 else labels.flip(0)
+    err1 = (lg.argmax(1) != ye).float().mean()
+    topk = lg.topk(min(5, C), dim=1).indices
+    err5 = 1.0 - (topk == ye[:, None]).any(1).float().mean()
+    dlogits = (lsm.exp() - q) / B * (grad_scale * weight)
+    return loss * weight, err1, err5, dlogits
 
 
 # --------------------------------------------------------------------------- GAN losses / noise
@@ -248,6 +273,119 @@ def uniform_noise(shape, seed, stream, step, device="cpu"):
     words = np.stack(r, axis=1).reshape(-1)[:n]
     u = (words >> np.uint64(8)).astype(np.float32) * np.float32(1.0 / 16777216.0)
     return torch.from_numpy(u.reshape(shape)).to(device)
+
+
+# --------------------------------------------------------------------------- Mixup / CutMix
+_MIX_TAG = 0xFFFFFFFF          # second counter word of every mix block (csrc/nn_kernels.cu: kMixCounterTag)
+_MIX_ATTEMPTS = 16             # Marsaglia–Tsang attempts per Gamma variate (kMixAttempts)
+
+
+def _mix_block(j, s, k0, k1):
+    """Philox block j of the mix draws of the steps ``s`` (uint64 array): counter (j, 0xFFFFFFFF, s_lo, s_hi)."""
+    M32 = np.uint64(0xFFFFFFFF)
+    return _philox4x32((np.full_like(s, j), np.full_like(s, _MIX_TAG), s & M32, s >> np.uint64(32)), k0, k1)
+
+
+def _mix_u01(w):
+    return (w.astype(np.float64) + 0.5) * 2.3283064365386963e-10
+
+
+def _mix_gamma(a, boost_u, j0, s, k0, k1):
+    """Gamma(a) per step (``a``: fp64 array) by Marsaglia–Tsang from Box–Muller normals, a < 1 boosted by U^(1/a), the operations in
+    the kernel's order; (values, accepted)."""
+    ae = np.where(a < 1.0, a + 1.0, a)
+    d = ae - 1.0 / 3.0
+    c = 1.0 / np.sqrt(9.0 * d)
+    g = np.zeros_like(a)
+    done = np.zeros(a.shape, dtype=bool)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        for k in range(_MIX_ATTEMPTS):
+            r = _mix_block(j0 + k, s, k0, k1)
+            x = np.sqrt(-2.0 * np.log(_mix_u01(r[0]))) * np.cos(6.283185307179586 * _mix_u01(r[1]))
+            v = 1.0 + c * x
+            ok = v > 0.0
+            v = (v * v) * v
+            u, x2 = _mix_u01(r[2]), x * x
+            acc = ok & ((u < 1.0 - (0.0331 * x2) * x2) | (np.log(u) < 0.5 * x2 + d * ((1.0 - v) + np.log(v))))
+            new = acc & ~done
+            g = np.where(new, d * v, g)
+            done |= acc
+    boost = np.power(boost_u, 1.0 / a)
+    return np.where(a < 1.0, g * boost, g), done
+
+
+def mix_draw(cfg, seed, rank, step, hw):
+    """The Mixup / CutMix draw of step counter value ``step`` (an int, or an array of them) for worker ``rank``, as the CUDA
+    ``mix_draw_kernel`` makes it (ops/mixup.py: RECORD; one record for an int step).  ``cfg`` is a validated ``config['mixup']``
+    (mixup.check_config), ``hw`` = (H, W) the image size at the mix point.
+
+    Philox4x32-10, key (seed_lo, seed_hi ^ rank), counter (j, 0xFFFFFFFF, step_lo, step_hi).  Block 0: the gate (mix when
+    U < prob), the switch (CutMix when both α > 0 and U < switch_prob) and the CutMix centre (⌊w·H / 2^32⌋, ⌊w·W / 2^32⌋); block 1
+    the U^(1/α) boosts of X and Y; blocks 2 + k and 2 + 16 + k attempt k of X and of Y ~ Gamma(α).  λ = X / (X + Y) in fp64.
+    Mixup: effective λ = fp32(λ).  CutMix (timm's rand_bbox): r = √(1 − λ), the box of ⌊H·r⌋ × ⌊W·r⌋ centred on (cy, cx) clipped to
+    the image, effective λ = fp32(1 − area / (H·W)).  A Gamma draw that rejects all 16 attempts leaves the step unmixed."""
+    from . import mixup
+    H, W = int(hw[0]), int(hw[1])
+    scalar = np.ndim(step) == 0
+    s = np.atleast_1d(np.asarray(step, dtype=np.int64)).astype(np.uint64)
+    seed = int(seed) & (2 ** 64 - 1)
+    k0, k1 = seed & 0xFFFFFFFF, ((seed >> 32) ^ int(rank)) & 0xFFFFFFFF
+    out = np.zeros(s.shape, dtype=mixup.RECORD)
+    out["mode"], out["lam"], out["lam_raw"], out["H"], out["W"] = mixup.MIX_NONE, 1.0, 1.0, H, W
+    w0 = _mix_block(0, s, k0, k1)
+    w1 = _mix_block(1, s, k0, k1)
+    gate = _mix_u01(w0[0]) < cfg["prob"]
+    if cfg["alpha"] > 0.0 and cfg["cutmix_alpha"] > 0.0:
+        cut = _mix_u01(w0[1]) < cfg["switch_prob"]
+    else:
+        cut = np.full(s.shape, cfg["cutmix_alpha"] > 0.0)
+    a = np.where(cut, cfg["cutmix_alpha"], cfg["alpha"])
+    gx, okx = _mix_gamma(a, _mix_u01(w1[0]), 2, s, k0, k1)
+    gy, oky = _mix_gamma(a, _mix_u01(w1[1]), 2 + _MIX_ATTEMPTS, s, k0, k1)
+    mix = gate & okx & oky
+    tot = gx + gy
+    with np.errstate(divide="ignore", invalid="ignore"):
+        lam = np.where(tot > 0.0, gx / tot, 0.5)
+    mu, cm = mix & ~cut, mix & cut
+    out["mode"][mu], out["lam_raw"][mu], out["lam"][mu] = mixup.MIX_MIXUP, lam[mu], lam[mu].astype(np.float32)
+    r = np.sqrt(1.0 - lam[cm])
+    ch, cw = (H * r).astype(np.int64), (W * r).astype(np.int64)
+    cy = ((w0[2][cm] * np.uint64(H)) >> np.uint64(32)).astype(np.int64)
+    cx = ((w0[3][cm] * np.uint64(W)) >> np.uint64(32)).astype(np.int64)
+    y0, y1 = np.clip(cy - ch // 2, 0, H), np.clip(cy + ch // 2, 0, H)
+    x0, x1 = np.clip(cx - cw // 2, 0, W), np.clip(cx + cw // 2, 0, W)
+    area = (y1 - y0) * (x1 - x0)
+    out["mode"][cm], out["lam_raw"][cm] = mixup.MIX_CUTMIX, lam[cm]
+    out["lam"][cm] = (1.0 - area.astype(np.float64) / float(H * W)).astype(np.float32)
+    for name, v in (("cy", cy), ("cx", cx), ("y0", y0), ("y1", y1), ("x0", x0), ("x1", x1)):
+        out[name][cm] = v
+    return out[0] if scalar else out
+
+
+def mix_lambda(rec):
+    """The weight of y_i in the step's target: the record's effective λ (an fp32 value), 1 when it does not mix."""
+    from . import mixup
+    r = mixup.decode(rec)
+    return float(np.float32(r["lam"])) if int(r["mode"]) != mixup.MIX_NONE else 1.0
+
+
+def mix_batch(x, rec):
+    """The batch ``x`` [B, H, W, C] mixed as the record says, sample i with j = B − 1 − i (``x.flip(0)``): Mixup
+    λ·x + (1 − λ)·x.flip(0) in fp32, rounded once to x's dtype; CutMix x with the box taken from x.flip(0); unmixed a copy."""
+    from . import mixup
+    r = mixup.decode(rec)
+    mode = int(r["mode"])
+    if mode == mixup.MIX_MIXUP:
+        xf = x.float()
+        lam = torch.tensor(float(r["lam"]), dtype=torch.float32)
+        return (lam * xf + (1.0 - lam) * xf.flip(0)).to(x.dtype)
+    out = x.clone()
+    if mode == mixup.MIX_CUTMIX:
+        if (int(r["H"]), int(r["W"])) != tuple(x.shape[1:3]):
+            raise ValueError("mix_batch: the record's box refers to %dx%d images, not %s" % (int(r["H"]), int(r["W"]), tuple(x.shape[1:3])))
+        y0, y1, x0, x1 = (int(r[k]) for k in ("y0", "y1", "x0", "x1"))
+        out[:, y0:y1, x0:x1, :] = x.flip(0)[:, y0:y1, x0:x1, :]
+    return out
 
 
 # --------------------------------------------------------------------------- optimizer (flat arena)
