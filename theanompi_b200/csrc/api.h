@@ -135,6 +135,10 @@ void mix_batch(void* x, const void* rec, int B, int H, int W, int C, int f32, cu
 // else y_j
 void softmax_xent_mix(const void* logits, const void* labels, const void* rec, void* dlogits, void* rowstat, void* out3, int B, int C,
                       float weight, float grad_weight, float label_smoothing, int f32, cudaStream_t st);
+// drop-path table (ops/drop_path.py owns the layout): out[l·B + n] = 0 when block l drops sample n at step counter *step, else
+// keep_scale[l] = fp32(1 / (1 − p_l)); thresh[l] = ⌈p_l·2^24⌉ (uint32), key (seed, rank)
+void drop_path_draw(const void* thresh, const void* keep_scale, int L, int B, unsigned long long seed, int rank, const void* step, void* out,
+                    cudaStream_t st);
 // act: 0 none, 1 ReLU, 2 leaky ReLU (negative slope `slope`), 3 sigmoid (ACT_* in common.cuh).  accumulate = 1: db / db1 += the bias
 // gradient (no clear)
 void relu_bias_bwd(const void* dy, const void* y, void* dym, void* db, void* db1, int c_split, long long R, int C, long long ld, int act,
@@ -158,14 +162,20 @@ void crop_mirror_norm(const void* x, int in_kind, const void* mean, int mean_mod
                       const void* flips, int N, int H, int W, int C, int ch, int cw, int Cout, cudaStream_t st);
 
 // ---- bn_kernels.cu: batch norm (+ residual)(+ ReLU) forward / backward, residual add  (f32: fp32 activations, else bf16)
+// drop_scale (optional, null = off): one row of the step's drop-path table, a float per sample of the `batch` samples (rows
+// r of sample r / (R / batch)); forward y = act(s_n·(γ·x̂ + β) + res) needs res, backward uses s_n·g for dγ, dβ and dx while
+// dres = g.  act must be ACT_NONE or ACT_RELU with a row.
 void bn_forward(const void* x, const void* res, void* y, const void* gamma, const void* beta, void* mean, void* rstd, void* run_mean,
-                void* run_var, void* scratch, long long R, int C, float momentum, float eps, int training, int act, float slope, int f32,
-                cudaStream_t st);
+                void* run_var, void* scratch, long long R, int C, float momentum, float eps, int training, int act, float slope,
+                const void* drop_scale, int batch, int f32, cudaStream_t st);
 // scratch: 3*C floats, 5*C with accumulate = 1 (dgamma / dbeta += this batch's gradients; dx is computed from this batch's sums, which
 // go to the scratch, exactly as without accumulate)
 void bn_backward(const void* x, const void* dy, const void* y, void* dx, void* dres, const void* gamma, const void* mean, const void* rstd,
-                 void* dgamma, void* dbeta, void* scratch, long long R, int C, int act, float slope, int accumulate, int f32, cudaStream_t st);
+                 void* dgamma, void* dbeta, void* scratch, long long R, int C, int act, float slope, int accumulate, const void* drop_scale,
+                 int batch, int f32, cudaStream_t st);
 void add_tensors(const void* a, const void* b, void* y, long long n, int f32, cudaStream_t st);
+// y = s_n·a + b over `batch` equal samples of n / batch elements (b null: y = s_n·a), s = one row of the drop-path table
+void add_scaled(const void* a, const void* b, const void* scale, void* y, long long n, int batch, int f32, cudaStream_t st);
 void add4_tensors(const void* a, const void* b, const void* c, const void* d, void* y, long long n, int f32, cudaStream_t st);
 
 // ---- rnn_kernels.cu: LSTM cell fwd / bwd, embedding gather / scatter, masked mean pooling  (f32: fp32 activations, else bf16)

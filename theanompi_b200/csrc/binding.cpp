@@ -138,13 +138,18 @@ PYBIND11_MODULE(_tmpi_native, m) {
 
   // ---------------------------------------------------------------- batch norm / residual
   m.def("bn_forward", [](ptr_t x, ptr_t res, ptr_t y, ptr_t gamma, ptr_t beta, ptr_t mean, ptr_t rstd, ptr_t run_mean, ptr_t run_var, ptr_t scratch,
-                         long long R, int C, float momentum, float eps, int training, int act, float slope, int f32, ptr_t st) {
+                         long long R, int C, float momentum, float eps, int training, int act, float slope, ptr_t drop_scale, int batch, int f32,
+                         ptr_t st) {
     bn_forward(P(x), P(res), P(y), P(gamma), P(beta), P(mean), P(rstd), P(run_mean), P(run_var), P(scratch), R, C, momentum, eps, training, act,
-               slope, f32, S(st)); });
+               slope, P(drop_scale), batch, f32, S(st)); });
   m.def("bn_backward", [](ptr_t x, ptr_t dy, ptr_t y, ptr_t dx, ptr_t dres, ptr_t gamma, ptr_t mean, ptr_t rstd, ptr_t dgamma, ptr_t dbeta,
-                          ptr_t scratch, long long R, int C, int act, float slope, int accumulate, int f32, ptr_t st) {
-    bn_backward(P(x), P(dy), P(y), P(dx), P(dres), P(gamma), P(mean), P(rstd), P(dgamma), P(dbeta), P(scratch), R, C, act, slope, accumulate, f32,
-                S(st)); });
+                          ptr_t scratch, long long R, int C, int act, float slope, int accumulate, ptr_t drop_scale, int batch, int f32, ptr_t st) {
+    bn_backward(P(x), P(dy), P(y), P(dx), P(dres), P(gamma), P(mean), P(rstd), P(dgamma), P(dbeta), P(scratch), R, C, act, slope, accumulate,
+                P(drop_scale), batch, f32, S(st)); });
+  m.def("add_scaled", [](ptr_t a, ptr_t b, ptr_t scale, ptr_t y, long long n, int batch, int f32, ptr_t st) {
+    add_scaled(P(a), P(b), P(scale), P(y), n, batch, f32, S(st)); });
+  m.def("drop_path_draw", [](ptr_t thresh, ptr_t keep_scale, int L, int B, unsigned long long seed, int rank, ptr_t step, ptr_t out, ptr_t st) {
+    drop_path_draw(P(thresh), P(keep_scale), L, B, seed, rank, P(step), P(out), S(st)); });
   m.def("add4_tensors", [](ptr_t a, ptr_t b, ptr_t c, ptr_t d, ptr_t y, long long n, int f32, ptr_t st) {
     add4_tensors(P(a), P(b), P(c), P(d), P(y), n, f32, S(st)); });
   m.def("add_tensors", [](ptr_t a, ptr_t b, ptr_t y, long long n, int f32, ptr_t st) { add_tensors(P(a), P(b), P(y), n, f32, S(st)); });

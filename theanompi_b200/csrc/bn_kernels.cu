@@ -9,6 +9,10 @@
 //   backward             reduce:   g = dy ⊙ [y > 0];  dβ = Σ g,  dγ = Σ g·x̂           (x̂ = (x − mean)·rstd)
 //                        apply:    dx = γ·rstd·(g − dβ/M − x̂·dγ/M);  d residual = g
 // M = N·H·W rows.  Each pass is one streaming kernel over the activation tensor (16-byte vectors).
+//
+// Drop-path (stochastic depth) is a compile-time variant (kDrop) of the apply pass and of both backward passes: with a row s of
+// the step's drop table (one fp32 scale per sample, ops/drop_path.py), y = act(s_n·(γ·x̂ + β) + residual), and the backward uses
+// g̃ = s_n·g in Σg, Σg·x̂ and dx while the residual still receives g.  The statistics stay those of the whole batch.
 #include "common.cuh"
 #include "api.h"
 #include <algorithm>
@@ -17,14 +21,28 @@ namespace tmpi {
 
 static inline int grid1(long long n, int block) { return (int)((n + block - 1) / block); }
 
+// Sample index n = r / hw of the rows a thread walks with a fixed stride: one division when the walk starts, then one carry per
+// step (the stride split once into whole samples q and leftover rows m), never a division per 16-byte vector.
+struct SampleWalk {
+  unsigned n, p, hw, q, m;
+  __device__ __forceinline__ void init(long long r, int hw_, int stride) {
+    hw = (unsigned)hw_;
+    n = (unsigned)(r / hw_); p = (unsigned)(r - (long long)n * hw_);
+    q = (unsigned)stride / hw; m = (unsigned)stride % hw;
+  }
+  __device__ __forceinline__ void step() { n += q; p += m; if (p >= hw) { p -= hw; ++n; } }
+};
+
 // ---------------------------------------------------------------- column reductions over row slabs
 // MODE 0: a = Σ x, b = Σ x²            (forward statistics)
 // MODE 1: a = Σ g, b = Σ g·x̂          (backward: g = dy ⊙ [y > 0] when relu; g = act'(y) ⊙ dy for ACT_LEAKY / ACT_SIGMOID)
-template <typename T, int MODE, int ACT>
+//         kDrop: g ← drop[r / hw]·g    (the drop-path scale of the row's sample)
+template <typename T, int MODE, int ACT, bool kDrop = false>
 __global__ void __launch_bounds__(256) bn_colreduce_kernel(const T* __restrict__ x, const T* __restrict__ dy, const T* __restrict__ y,
                                                           const float* __restrict__ mean, const float* __restrict__ rstd, float* __restrict__ out_a,
                                                           float* __restrict__ out_b, long long R, int C, int relu, int VT, int rows_per_cta,
-                                                          float slope) {
+                                                          float slope, const float* __restrict__ drop, int hw) {
+  static_assert(!kDrop || (MODE == 1 && ACT == ACT_FLAG), "drop-path: backward reduction with ReLU / identity only");
   constexpr int N = VecIO<T>::N;
   extern __shared__ float sm[];                       // [2][RL][VT*N]
   const int nvec = C / N;
@@ -45,6 +63,8 @@ __global__ void __launch_bounds__(256) bn_colreduce_kernel(const T* __restrict__
     // UR rows per trip, all (raw 16-byte) loads issued before any use — this pass is pure streaming, memory-level parallelism
     // is everything; the vectors stay packed until they are consumed so the trip fits in ~64 registers
     constexpr int UR = MODE == 0 ? 4 : 2;
+    SampleWalk w;
+    if constexpr (kDrop) w.init(r0 + tr, hw, RL);
     for (long long r = r0 + tr; r < rend; r += UR * RL) {
       uint4 xr[UR], gr[UR], yr[UR];
 #pragma unroll
@@ -71,15 +91,19 @@ __global__ void __launch_bounds__(256) bn_colreduce_kernel(const T* __restrict__
             float gv[N], yv[N];
             VecIO<T>::ld(reinterpret_cast<const T*>(&gr[u]), gv);
             if (ACT != ACT_FLAG || relu) VecIO<T>::ld(reinterpret_cast<const T*>(&yr[u]), yv);
+            float s = 1.f;
+            if constexpr (kDrop) s = __ldg(drop + w.n);
 #pragma unroll
             for (int i = 0; i < N; ++i) {
               float g = gv[i];
               if (ACT == ACT_FLAG) { if (relu && !(yv[i] > 0.f)) g = 0.f; }
               else g = act_bwd<ACT>(g, yv[i], slope);
+              if constexpr (kDrop) g *= s;
               a[i] += g; b[i] += g * (xv[i] - mu[i]) * rs[i];
             }
           }
         }
+        if constexpr (kDrop) w.step();
       }
     }
   }
@@ -102,9 +126,9 @@ __global__ void __launch_bounds__(256) bn_colreduce_kernel(const T* __restrict__
   }
 }
 
-template <typename T, int MODE, int ACT = ACT_FLAG>
+template <typename T, int MODE, int ACT = ACT_FLAG, bool kDrop = false>
 static void colreduce(const void* x, const void* dy, const void* y, const float* mean, const float* rstd, float* a, float* b, long long R,
-                      int C, int relu, cudaStream_t st, float slope = 0.f) {
+                      int C, int relu, cudaStream_t st, float slope = 0.f, const float* drop = nullptr, int hw = 1) {
   constexpr int N = VecIO<T>::N;
   if (C % N) throw std::runtime_error("batch_norm: C must be a multiple of the 16-byte vector width");
   const int nvec = C / N;
@@ -118,8 +142,8 @@ static void colreduce(const void* x, const void* dy, const void* y, const float*
   const size_t smem = (size_t)2 * RL * VT * N * sizeof(float);
   check_cuda(cudaMemsetAsync(a, 0, (size_t)C * 4, st), "bn memset");
   check_cuda(cudaMemsetAsync(b, 0, (size_t)C * 4, st), "bn memset");
-  bn_colreduce_kernel<T, MODE, ACT><<<grid, 256, smem, st>>>((const T*)x, (const T*)dy, (const T*)y, mean, rstd, a, b, R, C, relu, VT, rows_per_cta,
-                                                             slope);
+  bn_colreduce_kernel<T, MODE, ACT, kDrop><<<grid, 256, smem, st>>>((const T*)x, (const T*)dy, (const T*)y, mean, rstd, a, b, R, C, relu, VT,
+                                                                    rows_per_cta, slope, drop, hw);
 }
 
 // mean / rstd from the sums (training) or from the running statistics (eval); momentum update of the running statistics;
@@ -152,10 +176,12 @@ __global__ void bn_finalize_kernel(float* __restrict__ sum, float* __restrict__ 
 // Elementwise passes: thread = (channel vector cv, row lane); the per-channel coefficients are loaded ONCE per thread and the
 // thread then walks rows with a fixed stride — no per-element division (the first version did a 64-bit modulo per 16 bytes and
 // was issue-bound at ~5x the memory roofline), 32-bit offsets inside a row slab.
-template <typename T, int ACT>
+// kDrop: y = act(drop[r / hw]·(scale·x + shift) + res); the launcher guarantees a residual
+template <typename T, int ACT, bool kDrop = false>
 __global__ void __launch_bounds__(256) bn_apply_kernel(const T* __restrict__ x, const T* __restrict__ res, T* __restrict__ y,
                                                       const float* __restrict__ scale, const float* __restrict__ shift, long long R, int C,
-                                                      int relu, int VT, int rows_per_cta, float slope) {
+                                                      int relu, int VT, int rows_per_cta, float slope, const float* __restrict__ drop, int hw) {
+  static_assert(!kDrop || ACT == ACT_FLAG, "drop-path: ReLU / identity only");
   constexpr int N = VecIO<T>::N;
   const int nvec = C / N;
   const int RL = blockDim.x / VT;
@@ -174,18 +200,23 @@ __global__ void __launch_bounds__(256) bn_apply_kernel(const T* __restrict__ x, 
   const T* rp = res ? res + r0 * C + cv * N : nullptr;
   T* yp = y + r0 * C + cv * N;
   const int nrows = (int)(rend - r0);
+  SampleWalk w;
+  if constexpr (kDrop) w.init(r0 + tr, hw, RL);
   for (int r = tr; r < nrows; r += 2 * RL) {
     // two rows in flight per trip
     const int r2 = r + RL;
     const bool two = r2 < nrows;
     float a[N], b[N], ra[N], rb[N];
+    float sa = 1.f, sb = 1.f;
+    if constexpr (kDrop) { sa = __ldg(drop + w.n); w.step(); if (two) sb = __ldg(drop + w.n); w.step(); }
     VecIO<T>::ld(xp + (unsigned)r * (unsigned)C, a);
     if (two) VecIO<T>::ld(xp + (unsigned)r2 * (unsigned)C, b);
     if (rp) { VecIO<T>::ld(rp + (unsigned)r * (unsigned)C, ra); if (two) VecIO<T>::ld(rp + (unsigned)r2 * (unsigned)C, rb); }
 #pragma unroll
     for (int i = 0; i < N; ++i) {
       a[i] = fmaf(a[i], sc[i], sh[i]);
-      if (rp) a[i] += ra[i];
+      if constexpr (kDrop) a[i] = fmaf(sa, a[i], ra[i]);
+      else if (rp) a[i] += ra[i];
       if (ACT == ACT_FLAG) { if (relu) a[i] = fmaxf(a[i], 0.f); }
       else a[i] = act_fwd<ACT>(a[i], slope);
     }
@@ -194,7 +225,8 @@ __global__ void __launch_bounds__(256) bn_apply_kernel(const T* __restrict__ x, 
 #pragma unroll
       for (int i = 0; i < N; ++i) {
         b[i] = fmaf(b[i], sc[i], sh[i]);
-        if (rp) b[i] += rb[i];
+        if constexpr (kDrop) b[i] = fmaf(sb, b[i], rb[i]);
+        else if (rp) b[i] += rb[i];
         if (ACT == ACT_FLAG) { if (relu) b[i] = fmaxf(b[i], 0.f); }
         else b[i] = act_fwd<ACT>(b[i], slope);
       }
@@ -229,10 +261,13 @@ __global__ void bn_bwd_coef_accum_kernel(const float* __restrict__ gamma, const 
   dbeta[c] += b;
 }
 
-template <typename T, int ACT>
+// kDrop: dx from g̃ = drop[r / hw]·g (the coefficients k come from the Σ of g̃), dres = g
+template <typename T, int ACT, bool kDrop = false>
 __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const T* __restrict__ x, const T* __restrict__ dy, const T* __restrict__ y,
                                                           T* __restrict__ dx, T* __restrict__ dres, const float* __restrict__ k, long long R, int C,
-                                                          int relu, int VT, int rows_per_cta, float slope) {
+                                                          int relu, int VT, int rows_per_cta, float slope, const float* __restrict__ drop,
+                                                          int hw) {
+  static_assert(!kDrop || ACT == ACT_FLAG, "drop-path: ReLU / identity only");
   constexpr int N = VecIO<T>::N;
   const int nvec = C / N;
   const int RL = blockDim.x / VT;
@@ -249,9 +284,13 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const T* __restrict__
   const long long r0 = (long long)blockIdx.x * rows_per_cta;
   const int nrows = (int)(min(R, r0 + rows_per_cta) - r0);
   const long long base = r0 * C + cv * N;
+  SampleWalk w;
+  if constexpr (kDrop) w.init(r0 + tr, hw, RL);
   for (int r = tr; r < nrows; r += RL) {
     const unsigned o = (unsigned)r * (unsigned)C;
     float xv[N], g[N], out[N];
+    float s = 1.f;
+    if constexpr (kDrop) { s = __ldg(drop + w.n); w.step(); }
     VecIO<T>::ld(x + base + o, xv);
     VecIO<T>::ld(dy + base + o, g);
     if (ACT != ACT_FLAG || relu) {
@@ -264,7 +303,10 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const T* __restrict__
       }
     }
 #pragma unroll
-    for (int i = 0; i < N; ++i) out[i] = fmaf(k1[i], g[i], fmaf(k2[i], xv[i], k3[i]));
+    for (int i = 0; i < N; ++i) {
+      if constexpr (kDrop) out[i] = fmaf(k1[i], s * g[i], fmaf(k2[i], xv[i], k3[i]));
+      else out[i] = fmaf(k1[i], g[i], fmaf(k2[i], xv[i], k3[i]));
+    }
     VecIO<T>::st(dx + base + o, out);
     if (dres) VecIO<T>::st(dres + base + o, g);
   }
@@ -282,6 +324,29 @@ __global__ void __launch_bounds__(256) add_kernel(const T* __restrict__ a, const
 #pragma unroll
   for (int i = 0; i < N; ++i) av[i] += bv[i];
   VecIO<T>::st(y + idx * N, av);
+}
+
+// y = s_n·a + b per sample n = blockIdx.y (b absent: y = s_n·a) — the drop-path merge of a pre-activation block and its branch
+// gradient; the 2-D grid gives the sample index without any division
+template <typename T>
+__global__ void __launch_bounds__(256) add_scaled_kernel(const T* __restrict__ a, const T* __restrict__ b, const float* __restrict__ s,
+                                                        T* __restrict__ y, int vec_per_sample) {
+  constexpr int N = VecIO<T>::N;
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= vec_per_sample) return;
+  const long long e = ((long long)blockIdx.y * vec_per_sample + v) * N;
+  const float sn = __ldg(s + blockIdx.y);
+  float av[N], bv[N];
+  VecIO<T>::ld(a + e, av);
+  if (b) {
+    VecIO<T>::ld(b + e, bv);
+#pragma unroll
+    for (int i = 0; i < N; ++i) av[i] = fmaf(sn, av[i], bv[i]);
+  } else {
+#pragma unroll
+    for (int i = 0; i < N; ++i) av[i] *= sn;
+  }
+  VecIO<T>::st(y + e, av);
 }
 
 // y = a + b + c + d (gradient merge of the four inception branches)
@@ -315,9 +380,12 @@ static RowGeom row_geom(long long R, int nvec) {
 // ---------------------------------------------------------------- launchers (f32 = 1: fp32 activations, else bf16)
 template <typename T>
 static void bn_apply_t(const void* x, const void* res, void* y, const float* s0, const float* s1, long long R, int C, int act, float slope,
-                       const RowGeom& g, cudaStream_t st) {
-#define BNA(A) bn_apply_kernel<T, A><<<g.grid, 256, 0, st>>>((const T*)x, (const T*)res, (T*)y, s0, s1, R, C, act, g.VT, g.rows_per_cta, slope)
-  if (act == ACT_NONE || act == ACT_RELU) BNA(ACT_FLAG);
+                       const float* drop, int hw, const RowGeom& g, cudaStream_t st) {
+#define BNA(A) bn_apply_kernel<T, A><<<g.grid, 256, 0, st>>>((const T*)x, (const T*)res, (T*)y, s0, s1, R, C, act, g.VT, g.rows_per_cta, slope, \
+                                                             nullptr, 1)
+  if (drop) bn_apply_kernel<T, ACT_FLAG, true><<<g.grid, 256, 0, st>>>((const T*)x, (const T*)res, (T*)y, s0, s1, R, C, act, g.VT,
+                                                                        g.rows_per_cta, slope, drop, hw);
+  else if (act == ACT_NONE || act == ACT_RELU) BNA(ACT_FLAG);
   else if (act == ACT_LEAKY) BNA(ACT_LEAKY);
   else if (act == ACT_SIGMOID) BNA(ACT_SIGMOID);
   else throw std::runtime_error("batch_norm: unknown activation");
@@ -326,12 +394,14 @@ static void bn_apply_t(const void* x, const void* res, void* y, const float* s0,
 
 template <typename T>
 static void bn_bwd_t(const void* x, const void* dy, const void* y, void* dx, void* dres, const float* mean, const float* rstd, void* dgamma,
-                     void* dbeta, const float* gamma, float* k, long long R, int C, int act, float slope, int accumulate, cudaStream_t st) {
+                     void* dbeta, const float* gamma, float* k, long long R, int C, int act, float slope, int accumulate, const float* drop,
+                     int hw, cudaStream_t st) {
   constexpr int N = VecIO<T>::N;
   // accumulate: this batch's sums go to the scratch after the coefficients (k[3C, 5C)), not into the accumulated dγ / dβ
   float* sb = accumulate ? k + 3 * C : (float*)dbeta;
   float* sg = accumulate ? k + 4 * C : (float*)dgamma;
-  if (act == ACT_NONE || act == ACT_RELU) colreduce<T, 1>(x, dy, y, mean, rstd, sb, sg, R, C, act, st);
+  if (drop) colreduce<T, 1, ACT_FLAG, true>(x, dy, y, mean, rstd, sb, sg, R, C, act, st, 0.f, drop, hw);
+  else if (act == ACT_NONE || act == ACT_RELU) colreduce<T, 1>(x, dy, y, mean, rstd, sb, sg, R, C, act, st);
   else if (act == ACT_LEAKY) colreduce<T, 1, ACT_LEAKY>(x, dy, y, mean, rstd, sb, sg, R, C, act, st, slope);
   else if (act == ACT_SIGMOID) colreduce<T, 1, ACT_SIGMOID>(x, dy, y, mean, rstd, sb, sg, R, C, act, st, slope);
   else throw std::runtime_error("batch_norm: unknown activation");
@@ -342,19 +412,33 @@ static void bn_bwd_t(const void* x, const void* dy, const void* y, void* dx, voi
   const RowGeom g = row_geom(R, C / N);
   if ((long long)g.rows_per_cta * C >= (1LL << 32)) throw std::runtime_error("batch_norm: row slab too large for 32-bit offsets");
 #define BNB(A) bn_bwd_apply_kernel<T, A><<<g.grid, 256, 0, st>>>((const T*)x, (const T*)dy, (const T*)y, (T*)dx, (T*)dres, k, R, C, act, g.VT, \
-                                                                g.rows_per_cta, slope)
-  if (act == ACT_LEAKY) BNB(ACT_LEAKY);
+                                                                g.rows_per_cta, slope, nullptr, 1)
+  if (drop) bn_bwd_apply_kernel<T, ACT_FLAG, true><<<g.grid, 256, 0, st>>>((const T*)x, (const T*)dy, (const T*)y, (T*)dx, (T*)dres, k, R, C,
+                                                                            act, g.VT, g.rows_per_cta, slope, drop, hw);
+  else if (act == ACT_LEAKY) BNB(ACT_LEAKY);
   else if (act == ACT_SIGMOID) BNB(ACT_SIGMOID);
   else BNB(ACT_FLAG);
 #undef BNB
 }
 
 // act: ACT_NONE / ACT_RELU / ACT_LEAKY (slope) / ACT_SIGMOID after the affine (and the residual add)
+// drop-path: the rows of sample n = r / (R / batch) are scaled by drop_scale[n] (one row of the step's table); ReLU / identity only
+static int drop_hw(const void* drop_scale, long long R, int batch, int act, const char* who) {
+  if (!drop_scale) return 1;
+  if (batch < 1 || R % batch || R / batch > 0x7FFFFFFF)
+    throw std::runtime_error(std::string(who) + ": a drop-path scale row needs R = batch * rows-per-sample");
+  if (act != ACT_NONE && act != ACT_RELU) throw std::runtime_error(std::string(who) + ": drop-path takes ReLU or no activation");
+  return (int)(R / batch);
+}
+
 void bn_forward(const void* x, const void* res, void* y, const void* gamma, const void* beta, void* mean, void* rstd, void* run_mean,
                 void* run_var, void* scratch /*2*C floats*/, long long R, int C, float momentum, float eps, int training, int act, float slope,
-                int f32, cudaStream_t st) {
+                const void* drop_scale, int batch, int f32, cudaStream_t st) {
   float* s0 = (float*)scratch; float* s1 = s0 + C;
   if (C % 4) throw std::runtime_error("batch_norm: C must be a multiple of 4");
+  if (drop_scale && !res) throw std::runtime_error("batch_norm: a drop-path scale row scales the branch of a residual add: needs res");
+  const int hw = drop_hw(drop_scale, R, batch, act, "batch_norm");
+  auto D = (const float*)drop_scale;
   if (training) {
     if (f32) colreduce<float, 0>(x, nullptr, nullptr, nullptr, nullptr, s0, s1, R, C, 0, st);
     else colreduce<__nv_bfloat16, 0>(x, nullptr, nullptr, nullptr, nullptr, s0, s1, R, C, 0, st);
@@ -366,17 +450,20 @@ void bn_forward(const void* x, const void* res, void* y, const void* gamma, cons
   if (C % N) throw std::runtime_error("batch_norm: C must be a multiple of the 16-byte vector width");
   const RowGeom g = row_geom(R, C / N);
   if ((long long)g.rows_per_cta * C >= (1LL << 32)) throw std::runtime_error("batch_norm: row slab too large for 32-bit offsets");
-  if (f32) bn_apply_t<float>(x, res, y, s0, s1, R, C, act, slope, g, st);
-  else bn_apply_t<__nv_bfloat16>(x, res, y, s0, s1, R, C, act, slope, g, st);
+  if (f32) bn_apply_t<float>(x, res, y, s0, s1, R, C, act, slope, D, hw, g, st);
+  else bn_apply_t<__nv_bfloat16>(x, res, y, s0, s1, R, C, act, slope, D, hw, g, st);
   count_launch(training ? 3 : 2); TMPI_CHECK_LAUNCH("bn_forward"); ::tmpi::check_capture(st, "bn_forward");
 }
 
 // scratch: 3*C floats (the coefficients of the apply pass), 5*C with accumulate (+ this batch's Σg, Σg·x̂)
 void bn_backward(const void* x, const void* dy, const void* y, void* dx, void* dres, const void* gamma, const void* mean, const void* rstd,
-                 void* dgamma, void* dbeta, void* scratch, long long R, int C, int act, float slope, int accumulate, int f32, cudaStream_t st) {
+                 void* dgamma, void* dbeta, void* scratch, long long R, int C, int act, float slope, int accumulate, const void* drop_scale,
+                 int batch, int f32, cudaStream_t st) {
   auto M = (const float*)mean; auto RS = (const float*)rstd; auto G = (const float*)gamma; auto K = (float*)scratch;
-  if (f32) bn_bwd_t<float>(x, dy, y, dx, dres, M, RS, dgamma, dbeta, G, K, R, C, act, slope, accumulate, st);
-  else bn_bwd_t<__nv_bfloat16>(x, dy, y, dx, dres, M, RS, dgamma, dbeta, G, K, R, C, act, slope, accumulate, st);
+  const int hw = drop_hw(drop_scale, R, batch, act, "batch_norm");
+  auto D = (const float*)drop_scale;
+  if (f32) bn_bwd_t<float>(x, dy, y, dx, dres, M, RS, dgamma, dbeta, G, K, R, C, act, slope, accumulate, D, hw, st);
+  else bn_bwd_t<__nv_bfloat16>(x, dy, y, dx, dres, M, RS, dgamma, dbeta, G, K, R, C, act, slope, accumulate, D, hw, st);
   count_launch(3); TMPI_CHECK_LAUNCH("bn_backward"); ::tmpi::check_capture(st, "bn_backward");
 }
 
@@ -387,6 +474,18 @@ void add_tensors(const void* a, const void* b, void* y, long long n, int f32, cu
   if (f32) add_kernel<float><<<grid1(tv, 256), 256, 0, st>>>((const float*)a, (const float*)b, (float*)y, tv);
   else add_kernel<__nv_bfloat16><<<grid1(tv, 256), 256, 0, st>>>((const __nv_bfloat16*)a, (const __nv_bfloat16*)b, (__nv_bfloat16*)y, tv);
   count_launch(); TMPI_CHECK_LAUNCH("add_tensors"); ::tmpi::check_capture(st, "add_tensors");
+}
+
+void add_scaled(const void* a, const void* b, const void* scale, void* y, long long n, int batch, int f32, cudaStream_t st) {
+  const int N = f32 ? 4 : 8;
+  if (!scale || batch < 1 || batch > 65535 || n % batch || (n / batch) % N || n / batch / N > 0x7FFFFFFF)
+    throw std::runtime_error("add_scaled: needs a scale row and 1 <= batch <= 65535 samples of a multiple of 16 bytes each");
+  const int vps = (int)(n / batch / N);
+  const dim3 grid((unsigned)grid1(vps, 256), (unsigned)batch);
+  auto S = (const float*)scale;
+  if (f32) add_scaled_kernel<float><<<grid, 256, 0, st>>>((const float*)a, (const float*)b, S, (float*)y, vps);
+  else add_scaled_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>((const __nv_bfloat16*)a, (const __nv_bfloat16*)b, S, (__nv_bfloat16*)y, vps);
+  count_launch(); TMPI_CHECK_LAUNCH("add_scaled"); ::tmpi::check_capture(st, "add_scaled");
 }
 
 void add4_tensors(const void* a, const void* b, const void* c, const void* d, void* y, long long n, int f32, cudaStream_t st) {

@@ -729,6 +729,35 @@ void mix_draw(const MixParams& p, const void* step, void* rec, int n, cudaStream
   count_launch(); TMPI_CHECK_LAUNCH("mix_draw"); ::tmpi::check_capture(st, "mix_draw");
 }
 
+// ============================================================================ drop-path (stochastic depth) draw
+// out[l·B + n] = 0 if block l drops sample n this step, else keep_scale[l] (ops/reference.py: drop_path_draw is the same on the
+// host).  Philox4x32-10 with key (seed_lo, seed_hi ^ rank) and counter (n, l ^ kDropPathTag, step_lo, step_hi); the decision is
+// (word0 >> 8) < thresh[l], i.e. u = (word0 >> 8)·2^-24 < p_l with thresh[l] = ⌈p_l·2^24⌉ computed exactly on the host.  The tag
+// keeps the second counter word in [0xC0000000, 0xC000FFFF] (L < 2^16): dropout's and uniform_noise's second word is the high word
+// of a non-negative 64-bit index (at most 0x7FFFFFFF) and the mix draw's is 0xFFFFFFFF, so no block of another stream is ever one
+// of these, whatever the keys.
+constexpr uint32_t kDropPathTag = 0xC0000000u;
+
+__global__ void drop_path_draw_kernel(const uint32_t* __restrict__ thresh, const float* __restrict__ keep_scale, int L, int B,
+                                      unsigned long long seed, uint32_t rank, const unsigned long long* __restrict__ step,
+                                      float* __restrict__ out) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= L * B) return;
+  const int l = t / B, n = t - l * B;
+  const unsigned long long s = *step;
+  uint32_t r[4];
+  philox4x32((uint32_t)n, (uint32_t)l ^ kDropPathTag, (uint32_t)s, (uint32_t)(s >> 32), (uint32_t)seed, (uint32_t)(seed >> 32) ^ rank, r);
+  out[t] = (r[0] >> 8) < thresh[l] ? 0.f : keep_scale[l];
+}
+
+void drop_path_draw(const void* thresh, const void* keep_scale, int L, int B, unsigned long long seed, int rank, const void* step, void* out,
+                    cudaStream_t st) {
+  if (L < 1 || L > 65535 || B < 1 || (long long)L * B > 0x7FFFFFFF) throw std::runtime_error("drop_path_draw: needs 1 <= L <= 65535 blocks and B >= 1");
+  drop_path_draw_kernel<<<grid_for((long long)L * B, 256), 256, 0, st>>>((const uint32_t*)thresh, (const float*)keep_scale, L, B, seed,
+                                                                          (uint32_t)rank, (const unsigned long long*)step, (float*)out);
+  count_launch(); TMPI_CHECK_LAUNCH("drop_path_draw"); ::tmpi::check_capture(st, "drop_path_draw");
+}
+
 // One thread per element position of a pair (i, j = B − 1 − i), blockIdx.y = i: it reads both rows and writes both, so the mix is
 // in place.  kVec: N-element 16-byte vectors (the row length n = H·W·C times sizeof(T) is a multiple of 16), else one element.  The
 // grid is sized for Mixup; CutMix CTAs whose elements lie outside the box rows return before touching the batch.

@@ -67,6 +67,7 @@ class ModelBase(object):
     supports_lr_schedule = True    # config['lr_schedule'] (False: the model refuses it at compile_iter_fns)
     supports_label_smoothing = True    # config['label_smoothing'] > 0 (False: no classifier head; refused at compile_iter_fns)
     supports_mixup = True          # config['mixup'] (False: no image batch before a first convolution; refused at compile_iter_fns)
+    supports_drop_path = False     # config['drop_path_rate'] > 0 (True: residual blocks in self.body that read drop_row(l))
     name = "Model"
 
     def __init__(self, config):
@@ -121,6 +122,11 @@ class ModelBase(object):
         # batch mixed at the mix point (mix_input) and the loss taken against the mixed target.  Built by check_mixup
         self.mixup = config.get("mixup")
         self.mixer = None
+        # stochastic depth (ops/drop_path.py; 0 = off): one [blocks, batch] table drawn on the device per training step, block l's row
+        # scaling its residual branch per sample.  Built by check_drop_path; read through drop_row only during the training forward
+        self.drop_path_rate = config.get("drop_path_rate", 0.0)
+        self.drop_path = None
+        self._drop_on = False
         self.base_lr = np.float32(self.learning_rate)
         self.current_t = self.subb_t = 0
         self.current_v = self.subb_v = 0
@@ -200,12 +206,22 @@ class ModelBase(object):
     def _fwd_bwd_eager(self):
         # the training loss carries the label smoothing (read on the host here, so a captured step keeps the ε it was captured with);
         # with config['mixup'] the step's draw comes first, keyed by the device step counter, so every graph replay draws anew
-        if self.mixer is None:
-            cost, err, err5 = self.loss(self.x_in, self.y_in, self.label_smoothing)
-        else:
+        # with config['drop_path_rate'] the table is drawn next (after the mix draw) from the same counter, and only this forward reads
+        # it: validation and inference never drop
+        rec = None
+        if self.mixer is not None:
             rec = self.mixer.draw()
             self.mix_input(rec)
-            cost, err, err5 = self.loss(self.x_in, self.y_in, self.label_smoothing, mix=rec)
+        if self.drop_path is not None:
+            self.drop_path.draw()
+            self._drop_on = True
+        try:
+            if rec is None:
+                cost, err, err5 = self.loss(self.x_in, self.y_in, self.label_smoothing)
+            else:
+                cost, err, err5 = self.loss(self.x_in, self.y_in, self.label_smoothing, mix=rec)
+        finally:
+            self._drop_on = False
         self._dbg_capture("forward")
         cost.backward()
         return cost.detach(), err.detach()
@@ -384,6 +400,26 @@ class ModelBase(object):
                              "ResNet50 and Wide_ResNet" % self.name)
         self.mixer = Mixer(cfg, self.rank, self.mix_hw, self.device)
 
+    # ------------------------------------------------------------------ stochastic depth (drop-path)
+    def check_drop_path(self):
+        """``config['drop_path_rate']`` must be a finite real p in [0, 1) (ops/drop_path.py: check_rate; a ValueError names the key),
+        and p > 0 needs a model with residual blocks (``supports_drop_path``); builds the step's :class:`DropPath` over the
+        ``len(self.body)`` blocks."""
+        from ..ops.drop_path import KEY, DropPath, check_rate
+        self.drop_path = None
+        p = self.drop_path_rate = check_rate(self.drop_path_rate)
+        if p == 0.0:
+            return
+        if not self.supports_drop_path:
+            raise ValueError("%s: %s = %r is not supported; drop-path scales the residual blocks of ResNet50, ResNet152 and "
+                             "Wide_ResNet" % (self.name, KEY, p))
+        self.drop_path = DropPath(p, len(self.body), self.batch_size, self.rank, self.device)
+
+    def drop_row(self, l):
+        """Block l's row of this training step's drop-path table (fp32, one scale per sample), or None: outside the training
+        forward, without drop_path_rate, or where p_l = 0."""
+        return self.drop_path.row(l) if self._drop_on else None
+
     # ------------------------------------------------------------------ per-update learning-rate schedule
     @property
     def updates_per_epoch(self):
@@ -535,6 +571,7 @@ class ModelBase(object):
         self.check_grad_accum(fused_tail)
         self.check_label_smoothing()
         self.check_mixup()
+        self.check_drop_path()
         self.setup_lr_schedule()
         k = self.size if sync_type == "cdd" else 1
         if self.optimizer in ("lars", "lamb") and fused_tail is not None:

@@ -57,6 +57,7 @@ class WRN(nn.Module):
 
 
 class Wide_ResNet(ModelBase):
+    supports_drop_path = True      # one drop-path block per pre-activation block
     n_epochs, batch_size, file_batch_size, learning_rate = n_epochs, batch_size, file_batch_size, learning_rate
     weight_decay, momentum = 0.0, 0.9
     bias_lr_mult = 1.0             # Adam: one learning rate for every parameter
@@ -136,7 +137,7 @@ class Wide_ResNet(ModelBase):
         else:
             x = ((x.float() - self._mean) / 64.0).to(self.act_dtype)
         x = self.stem.forward(x)
-        for bn1, short, c1, bn2, c2 in self.body:                 # pre-activation block (ref :37-82)
+        for l, (bn1, short, c1, bn2, c2) in enumerate(self.body):     # pre-activation block (ref :37-82)
             if short is None:
                 x, s = ops.fork2(x)                               # identity shortcut: x feeds bn1 and the merge
                 o = bn1.forward(x)
@@ -144,7 +145,7 @@ class Wide_ResNet(ModelBase):
                 o, o2 = ops.fork2(bn1.forward(x))                 # projection shortcut reads the pre-activated tensor
                 s = short.forward(o2)
             o = c2.forward(bn2.forward(c1.forward(o)))
-            x = ops.add(o, s)
+            x = ops.add(o, s, drop=self.drop_row(l))              # s·branch + shortcut; s = block l's drop-path row
         bn, gap, flat, sm = self.head
         return sm.forward(flat.forward(gap.forward(bn.forward(x))))
 
@@ -160,6 +161,7 @@ class Wide_ResNet(ModelBase):
         self.check_grad_accum(fused_tail)
         self.check_label_smoothing()
         self.check_mixup()
+        self.check_drop_path()
         self.setup_lr_schedule()
         from ...utils.opt import FlatAdam
         self.sync_type = "avg"

@@ -66,6 +66,7 @@ class ResNet50Net(nn.Module):
 
 
 class ResNet50(ModelBase):
+    supports_drop_path = True      # one drop-path block per bottleneck
     n_epochs, momentum, weight_decay = n_epochs, momentum, weight_decay
     batch_size, file_batch_size, learning_rate = batch_size, file_batch_size, learning_rate
     lr_policy, lr_step = lr_policy, lr_step
@@ -147,12 +148,13 @@ class ResNet50(ModelBase):
         c, b, pool = self.stem
         x = pool.forward(b.forward(c.forward(x)))
         from ... import ops
-        for c1, b1, c2, b2, c3, b3, proj in self.body:
+        for l, (c1, b1, c2, b2, c3, b3, proj) in enumerate(self.body):
             x, xs = ops.fork2(x)                                  # two consumers: the branch and the shortcut
             short = xs if proj is None else proj[1].forward(proj[0].forward(xs))
             y = b1.forward(c1.forward(x))
             y = b2.forward(c2.forward(y))
-            x = b3.forward(c3.forward(y), residual=short)         # relu(bn(conv) + shortcut) in one kernel
+            # relu(s·bn(conv) + shortcut) in one kernel; s is block l's drop-path row (None: no drop)
+            x = b3.forward(c3.forward(y), residual=short, drop=self.drop_row(l))
         gap, flat, sm = self.head
         return sm.forward(flat.forward(gap.forward(x)))
 

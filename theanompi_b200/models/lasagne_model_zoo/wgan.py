@@ -102,6 +102,7 @@ class WGAN(TorchModelBase):
         self.check_grad_accum()
         self.check_label_smoothing()
         self.check_mixup()
+        self.check_drop_path()
         self.setup_lr_schedule()
         self.sync_type = "avg"
         self.opt_c = torch.optim.RMSprop(self.critic_params, lr=self.learning_rate)
@@ -400,6 +401,7 @@ class NativeWGAN(ModelBase):
         self.check_grad_accum()
         self.check_label_smoothing()
         self.check_mixup()
+        self.check_drop_path()
         self.setup_lr_schedule()
         self.sync_type = "avg"
         self.vels, self.vels2 = [], []

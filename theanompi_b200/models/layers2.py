@@ -442,12 +442,14 @@ class BatchNormal(Layer):
         if printinfo:
             self.print_shape()
 
-    def forward(self, x, residual=None):
+    def forward(self, x, residual=None, drop=None):
+        """``drop``: a drop-path row of the training step (ops/drop_path.py) that scales this layer's output per sample before the
+        residual add."""
         if self.running_mean.device != x.device:
             self.running_mean = self.running_mean.to(x.device)
             self.running_var = self.running_var.to(x.device)
         return ops.batch_norm(x, self.gamma.val, self.beta.val, self.running_mean, self.running_var, self.training,
-                              self.momentum, self.eps, self.relu, residual)
+                              self.momentum, self.eps, self.relu, residual, drop=drop)
 
     @staticmethod
     def SetTrainOn():

@@ -188,6 +188,7 @@ class LSTM(ModelBase):
         self.check_grad_accum()
         self.check_label_smoothing()
         self.check_mixup()
+        self.check_drop_path()
         self.setup_lr_schedule()
         self.sync_type = "avg"
         self._make_opt()
@@ -333,6 +334,7 @@ class LSTMTorch(TorchModelBase):
         self.check_grad_accum()
         self.check_label_smoothing()
         self.check_mixup()
+        self.check_drop_path()
         self.setup_lr_schedule()
         self.sync_type = "avg"
         self.torch_opt = self.make_torch_optimizer(self.params)

@@ -114,6 +114,7 @@ class TorchModelBase(ModelBase):
         self.check_grad_accum(fused_tail)
         self.check_label_smoothing()
         self.check_mixup()
+        self.check_drop_path()
         self.setup_lr_schedule()
         self.torch_opt = self.make_torch_optimizer(self.params)
         if self.torch_opt is None:

@@ -741,7 +741,15 @@ def uniform_noise(shape, seed, stream, step, dtype=None):
 
 
 # --------------------------------------------------------------------------- batch norm (+ residual)(+ ReLU), residual add
-def batch_norm_fwd(x, gamma, beta, run_mean, run_var, training, momentum, eps, relu, res=None):
+def _drop_row(drop, x):
+    """A drop-path row for ``x``: contiguous fp32 on x's device, one scale per sample of x's leading axis."""
+    if not (drop.is_cuda and drop.device == x.device and drop.dtype == F32 and drop.is_contiguous() and drop.numel() == x.shape[0]):
+        raise ValueError("a drop-path row is a contiguous fp32 tensor of %d scales on %s" % (x.shape[0], x.device))
+    return drop
+
+
+def batch_norm_fwd(x, gamma, beta, run_mean, run_var, training, momentum, eps, relu, res=None, drop=None):
+    """``drop``: a drop-path row (needs ``res``), y = act(s_n·(γ·x̂ + β) + res) in the apply pass (reference.batch_norm_fwd)."""
     x = _bf(x).contiguous()
     C = x.shape[-1]
     R = x.numel() // C
@@ -758,11 +766,12 @@ def batch_norm_fwd(x, gamma, beta, run_mean, run_var, training, momentum, eps, r
         assert run_mean is not None and run_var is not None
     L().bn_forward(x.data_ptr(), _p(res), y.data_ptr(), gamma.data_ptr(), beta.data_ptr(), mean.data_ptr(), rstd.data_ptr(),
                    _p(run_mean), _p(run_var), scratch.data_ptr(), int(R), int(C), float(momentum), float(eps), int(bool(training)),
-                   _act(relu), LEAKY_SLOPE, int(_is32(x)), _st(x))
+                   _act(relu), LEAKY_SLOPE, _p(drop if drop is None else _drop_row(drop, x)), int(x.shape[0]), int(_is32(x)), _st(x))
     return y, mean, rstd
 
 
-def batch_norm_bwd(x, dy, y, gamma, mean, rstd, relu, need_dres, dgamma_out=None, dbeta_out=None):
+def batch_norm_bwd(x, dy, y, gamma, mean, rstd, relu, need_dres, dgamma_out=None, dbeta_out=None, drop=None):
+    """``drop``: the forward's drop-path row; dx, dγ and dβ come from s_n·g, dres is g (reference.batch_norm_bwd)."""
     x = _bf(x).contiguous()
     dy = _bf(dy).contiguous()
     C = x.shape[-1]
@@ -778,7 +787,7 @@ def batch_norm_bwd(x, dy, y, gamma, mean, rstd, relu, need_dres, dgamma_out=None
     scratch = torch.empty((5 if acc else 3) * C, dtype=F32, device=dev)
     L().bn_backward(x.data_ptr(), dy.data_ptr(), _p(y) if relu else 0, dx.data_ptr(), _p(dres), gamma.data_ptr(), mean.data_ptr(),
                     rstd.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(), scratch.data_ptr(), int(R), int(C), _act(relu), LEAKY_SLOPE,
-                    acc, int(_is32(x)), _st(x))
+                    acc, _p(drop if drop is None else _drop_row(drop, x)), int(x.shape[0]), int(_is32(x)), _st(x))
     if need_dres and not relu:
         dres = dy
     return dx, dres, dgamma, dbeta
@@ -791,6 +800,29 @@ def add(a, b):
     y = torch.empty_like(a)
     L().add_tensors(a.data_ptr(), b.data_ptr(), y.data_ptr(), a.numel(), int(_is32(a)), _st(a))
     return y
+
+
+def add_scaled(a, s, b=None):
+    """y = s_n·a + b per sample n of the leading axis (``b`` None: s_n·a), ``s`` a drop-path row: one ``add_scaled_kernel`` launch
+    (each sample's elements must fill whole 16-byte vectors)."""
+    a = _bf(a).contiguous()
+    if b is not None:
+        b = _bf(b).contiguous()
+        assert b.shape == a.shape
+    y = torch.empty_like(a)
+    L().add_scaled(a.data_ptr(), _p(b), _drop_row(s, a).data_ptr(), y.data_ptr(), a.numel(), int(a.shape[0]), int(_is32(a)), _st(a))
+    return y
+
+
+def drop_path_draw(dp, step, out):
+    """The drop-path table of the device step counter ``step`` into ``out`` (fp32 [L, B]) for :class:`drop_path.DropPath` ``dp``,
+    keyed by the dropout seed and dp's rank: one ``drop_path_draw_kernel`` launch (reference.drop_path_draw on the CPU)."""
+    from .functional import rng_state
+    if not (out.is_cuda and out.dtype == F32 and out.is_contiguous() and tuple(out.shape) == (dp.L, dp.B) and out.device == step.device):
+        raise ValueError("drop_path_draw: the table is a contiguous fp32 [%d, %d] tensor on %s" % (dp.L, dp.B, step.device))
+    L().drop_path_draw(dp.thresh.data_ptr(), dp.keep.data_ptr(), dp.L, dp.B, int(rng_state()["seed"]) & (2 ** 64 - 1), dp.rank,
+                       step.data_ptr(), out.data_ptr(), _st(step))
+    return out
 
 
 # --------------------------------------------------------------------------- loader kernel

@@ -304,11 +304,12 @@ class _BatchNormFn(torch.autograd.Function):
     ``batch_norm`` + ``ElemwiseSumLayer`` + ``rectify`` (``lasagne_model_zoo/resnet50.py:14-77``)."""
 
     @staticmethod
-    def forward(ctx, x, gamma, beta, residual, run_mean, run_var, training, momentum, eps, relu):
+    def forward(ctx, x, gamma, beta, residual, run_mean, run_var, training, momentum, eps, relu, drop):
         impl = _impl(x)
-        y, mean, rstd = impl.batch_norm_fwd(x, gamma.detach(), beta.detach(), run_mean, run_var, training, momentum, eps, relu, residual)
+        y, mean, rstd = impl.batch_norm_fwd(x, gamma.detach(), beta.detach(), run_mean, run_var, training, momentum, eps, relu, residual,
+                                            drop=drop)
         ctx.gamma, ctx.beta = gamma, beta
-        ctx.relu, ctx.has_res = relu, residual is not None
+        ctx.relu, ctx.has_res, ctx.drop = relu, residual is not None, drop
         ctx.save_for_backward(x, y if relu else x.new_empty(0), mean, rstd)
         return y
 
@@ -319,23 +320,28 @@ class _BatchNormFn(torch.autograd.Function):
         impl = _impl(x)
         need_dres = ctx.has_res and ctx.needs_input_grad[3]
         if impl is ref:
-            dx, dres, dg, db = ref.batch_norm_bwd(x, dy, y, gamma.detach(), mean, rstd, ctx.relu, need_dres)
+            dx, dres, dg, db = ref.batch_norm_bwd(x, dy, y, gamma.detach(), mean, rstd, ctx.relu, need_dres, drop=ctx.drop)
         else:
             dx, dres, dg, db = impl.batch_norm_bwd(x, dy, y, gamma.detach(), mean, rstd, ctx.relu, need_dres,
-                                                   dgamma_out=_gout(gamma), dbeta_out=_gout(beta))
+                                                   dgamma_out=_gout(gamma), dbeta_out=_gout(beta), drop=ctx.drop)
         gb = _sink(beta, db)
         gg = _sink(gamma, dg)
-        return dx, gg, gb, dres, None, None, None, None, None, None
+        return dx, gg, gb, dres, None, None, None, None, None, None, None
 
 
-def batch_norm(x, gamma, beta, run_mean=None, run_var=None, training=True, momentum=0.1, eps=1e-5, relu=False, residual=None):
-    """Batch normalisation over all but the channel (last) axis, optionally fused with a residual add and a ReLU."""
-    return _BatchNormFn.apply(x, gamma, beta, residual, run_mean, run_var, training, momentum, eps, relu)
+def batch_norm(x, gamma, beta, run_mean=None, run_var=None, training=True, momentum=0.1, eps=1e-5, relu=False, residual=None, drop=None):
+    """Batch normalisation over all but the channel (last) axis, optionally fused with a residual add and a ReLU.  ``drop``: a
+    drop-path row (one fp32 scale s_n per sample, ops/drop_path.py) with a residual: y = relu(s_n·bn(x) + residual); the gradient
+    of x, γ and β is that of s_n·g, the residual's is g."""
+    return _BatchNormFn.apply(x, gamma, beta, residual, run_mean, run_var, training, momentum, eps, relu, drop)
 
 
 class _AddFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, a, b):
+    def forward(ctx, a, b, drop):
+        ctx.drop = drop
+        if drop is not None:
+            return _impl(a).add_scaled(a, drop, b)
         if a.is_cuda:
             from . import cuda_impl
             return cuda_impl.add(a, b)
@@ -343,7 +349,9 @@ class _AddFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dy):
-        return dy, dy
+        if ctx.drop is None:
+            return dy, dy, None
+        return _impl(dy).add_scaled(dy, ctx.drop), dy, None
 
 
 class _Fork2Fn(torch.autograd.Function):
@@ -373,9 +381,10 @@ def fork2(x):
     return _Fork2Fn.apply(x)
 
 
-def add(a, b):
-    """Residual merge ``a + b`` (native kernel on CUDA; the gradient passes to both branches unchanged)."""
-    return _AddFn.apply(a, b)
+def add(a, b, drop=None):
+    """Residual merge ``a + b`` (native kernel on CUDA; the gradient passes to both branches unchanged).  ``drop``: a drop-path row,
+    y = s_n·a + b, and the branch ``a`` gets s_n·dy."""
+    return _AddFn.apply(a, b, drop)
 
 
 # --------------------------------------------------------------------------- pool
@@ -518,6 +527,16 @@ def mix_draw(cfg, rank, hw, out):
         return cuda_impl.mix_draw(cfg, rank, hw, cuda_impl.step_counter(out.device), out=out)
     from .mixup import encode
     return out.copy_(encode(ref.mix_draw(cfg, cfg["seed"], rank, _RNG["step"], hw)))
+
+
+def drop_path_draw(dp, out):
+    """This step's drop-path table for :class:`drop_path.DropPath` ``dp`` into ``out`` (fp32 [L, B]): on CUDA drawn by the kernel
+    from the device step counter, on the CPU by :func:`reference.drop_path_draw` from the host one; both keyed by the dropout
+    seed.  Returns ``out``."""
+    if out.is_cuda:
+        from . import cuda_impl
+        return cuda_impl.drop_path_draw(dp, cuda_impl.step_counter(out.device), out)
+    return out.copy_(ref.drop_path_draw(dp.rates, _RNG["seed"], dp.rank, _RNG["step"], dp.B))
 
 
 def mix_batch(x, rec):

@@ -388,6 +388,26 @@ def mix_batch(x, rec):
     return out
 
 
+# --------------------------------------------------------------------------- drop-path (stochastic depth)
+def drop_path_draw(p_list, seed, rank, step, B):
+    """The drop-path table of step counter value ``step`` for worker ``rank`` (fp32 ``[L, B]``, ops/drop_path.py), as the CUDA
+    ``drop_path_draw_kernel`` writes it: entry (l, n) is 0 when (w >> 8)·2^-24 < p_l, else fp32(1 / (1 − p_l)), w word 0 of
+    Philox4x32-10 with key (seed_lo, seed_hi ^ rank) and counter (n, l ^ TAG, step_lo, step_hi).  ``p_list``: the block rates p_l."""
+    from . import drop_path
+    rates = np.asarray(p_list, dtype=np.float64)
+    L, B = rates.shape[0], int(B)
+    thresh, keep = drop_path.thresholds(rates).astype(np.uint64), drop_path.keep_scales(rates)
+    M32 = 0xFFFFFFFF
+    seed, step = int(seed) & (2 ** 64 - 1), int(step) & (2 ** 64 - 1)
+    l = np.repeat(np.arange(L, dtype=np.uint64), B)
+    n = np.tile(np.arange(B, dtype=np.uint64), L)
+    w0 = _philox4x32((n, l ^ np.uint64(drop_path.TAG), np.full_like(n, step & M32), np.full_like(n, step >> 32)),
+                     seed & M32, ((seed >> 32) ^ (int(rank) & M32)) & M32)[0]
+    li = l.astype(np.int64)
+    out = np.where((w0 >> np.uint64(8)) < thresh[li], np.float32(0.0), keep[li]).astype(np.float32)
+    return torch.from_numpy(out.reshape(L, B))
+
+
 # --------------------------------------------------------------------------- optimizer (flat arena)
 def clip_scale(g, offsets, sizes, max_norm):
     """Global gradient-norm clipping (``torch.nn.utils.clip_grad_norm_``) over a flat fp32 gradient laid out as a :class:`FlatArena`
@@ -634,9 +654,17 @@ def crop_mirror_normalize(x_u8, mean, std_scale, crop_hw, offsets, flips, out_dt
 
 
 # --------------------------------------------------------------------------- batch norm (+ residual)(+ ReLU), NHWC
-def batch_norm_fwd(x, gamma, beta, run_mean, run_var, training, momentum, eps, relu, res=None):
+def _per_sample(s, x):
+    """A drop-path row (one scale per sample of x's leading axis) shaped to broadcast over x."""
+    return s.float().reshape((x.shape[0],) + (1,) * (x.dim() - 1))
+
+
+def batch_norm_fwd(x, gamma, beta, run_mean, run_var, training, momentum, eps, relu, res=None, drop=None):
     """y = γ·(x − mean)·rstd + β [+ res] [ReLU]; statistics over all but the last (channel) axis.  Updates the running
-    statistics in place (momentum form, unbiased variance) when training.  Returns (y, mean, rstd)."""
+    statistics in place (momentum form, unbiased variance) when training.  ``drop`` (a drop-path row, one scale s_n per sample,
+    needs ``res``): y = act(s_n·(γ·x̂ + β) + res), the statistics still those of the whole batch.  Returns (y, mean, rstd)."""
+    if drop is not None and res is None:
+        raise ValueError("batch_norm: a drop-path row scales the branch of a residual add: needs res")
     xf = x.float()
     C = x.shape[-1]
     x2 = xf.reshape(-1, C)
@@ -653,21 +681,34 @@ def batch_norm_fwd(x, gamma, beta, run_mean, run_var, training, momentum, eps, r
         mean, var = run_mean.float(), run_var.float()
     rstd = torch.rsqrt(var + eps)
     y = (xf - mean) * (rstd * gamma.float()) + beta.float()
+    if drop is not None:
+        y = y * _per_sample(drop, x)
     if res is not None:
         y = y + res.float()
     return act_fwd(y, relu).to(x.dtype), mean, rstd
 
 
-def batch_norm_bwd(x, dy, y, gamma, mean, rstd, relu, need_dres):
-    """Returns (dx, dres, dgamma, dbeta) for :func:`batch_norm_fwd` in training mode."""
+def batch_norm_bwd(x, dy, y, gamma, mean, rstd, relu, need_dres, drop=None):
+    """Returns (dx, dres, dgamma, dbeta) for :func:`batch_norm_fwd` in training mode.  ``drop``: dx, dγ and dβ come from s_n·g,
+    the residual gets g."""
     C = x.shape[-1]
     g = dy.float()
     if relu:
         g = act_bwd(g, y.float(), relu)
+    gb = g if drop is None else g * _per_sample(drop, x)
     xh = (x.float() - mean) * rstd
-    g2, xh2 = g.reshape(-1, C), xh.reshape(-1, C)
+    g2, xh2 = gb.reshape(-1, C), xh.reshape(-1, C)
     R = g2.shape[0]
     dbeta = g2.sum(0)
     dgamma = (g2 * xh2).sum(0)
-    dx = (gamma.float() * rstd) * (g - dbeta / R - xh * (dgamma / R))
+    dx = (gamma.float() * rstd) * (gb - dbeta / R - xh * (dgamma / R))
     return dx.to(x.dtype), (g.to(x.dtype) if need_dres else None), dgamma, dbeta
+
+
+def add_scaled(a, s, b=None):
+    """s_n·a + b per sample n of the leading axis (b None: s_n·a) in fp32, rounded once to a's dtype: the drop-path merge of a
+    pre-activation block (y = s·branch + shortcut) and its branch gradient s·dy."""
+    y = a.float() * _per_sample(s, a)
+    if b is not None:
+        y = y + b.float()
+    return y.to(a.dtype)
