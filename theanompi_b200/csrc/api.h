@@ -160,6 +160,10 @@ void col2im(const void* dcol, void* dx, int N, int H, int W, int Ctot, int c_off
 void pad_rows(const void* src, void* dst, long long rows, int cols, long long src_ld, long long dst_ld, int f32, cudaStream_t st);
 void crop_mirror_norm(const void* x, int in_kind, const void* mean, int mean_mode, float scale, const void* cscale, void* out, int out_bf16, const void* offs,
                       const void* flips, int N, int H, int W, int C, int ch, int cw, int Cout, cudaStream_t st);
+// random-resized crop: uint8 NHWC x → bilinear resample of the normalised box boxes[n] = (y0, x0, h, w) (int32 [N, 4], 16-byte
+// aligned, inside the H × W image) to ch × cw, mirrored after the resize where flips[n]; out bf16 (out_bf16) or fp32 NHWC
+void resized_crop_mirror_norm(const void* x, const void* mean, int mean_mode, float scale, const void* cscale, void* out, int out_bf16,
+                              const void* boxes, const void* flips, int N, int H, int W, int C, int ch, int cw, cudaStream_t st);
 
 // ---- bn_kernels.cu: batch norm (+ residual)(+ ReLU) forward / backward, residual add  (f32: fp32 activations, else bf16)
 // drop_scale (optional, null = off): one row of the step's drop-path table, a float per sample of the `batch` samples (rows

@@ -1573,4 +1573,67 @@ void crop_mirror_norm(const void* x, int in_kind /*0 u8, 1 bf16, 2 f32*/, const 
   count_launch(); TMPI_CHECK_LAUNCH("crop_mirror_norm"); ::tmpi::check_capture(st, "crop_mirror_norm");
 }
 
+// ============================================================================ loader: random-resized crop → NHWC bf16/fp32
+// Output pixel (oy, ox) of image n is the bilinear resample of the normalised box (y0, x0, h, w) = boxes[n] to ch × cw, as
+// F.interpolate(mode='bilinear', align_corners=False, antialias=False), mirrored after the resize.  Each of the four taps is
+// normalised with its own mean (the per-pixel mean makes normalise-then-resize the definition).  Per axis of box length L:
+// s = max((o + ½)·L/out − ½, 0), i0 = ⌊s⌋, i1 = i0 + (i0 < L − 1), λ = s − i0, in fp32 as ATen's bilinear kernel computes it: an
+// IEEE division L/out and one fused multiply-add (explicit _rn intrinsics, so --use_fast_math changes neither; the unfused form
+// moves λ by an ulp of s, about 1.5e-5 at s ≈ 250).
+// Same grid as crop_mirror_norm_kernel: one CTA per output row (n, oy), so the box, the flip, both source rows and the y weight are
+// CTA-uniform; threads sweep ox with one multiply per coordinate, and adjacent ox gather the same or adjacent texels (L1 hits).
+__device__ __forceinline__ void rrc_axis(int o, float ratio, int L, int& i0, int& i1, float& lam) {
+  const float s = fmaxf(__fmaf_rn(ratio, (float)o + 0.5f, -0.5f), 0.f);
+  i0 = min((int)s, L - 1);
+  i1 = i0 + (i0 < L - 1 ? 1 : 0);
+  lam = fminf(fmaxf(s - (float)i0, 0.f), 1.f);
+}
+
+template <typename Tout>
+__global__ void __launch_bounds__(128) resized_crop_mirror_norm_kernel(const uint8_t* __restrict__ x, const float* __restrict__ mean,
+                                        int mean_mode, float scale, const float* __restrict__ cscale, Tout* __restrict__ out,
+                                        const int4* __restrict__ boxes, const uint8_t* __restrict__ flips, int H, int W, int C, int ch,
+                                        int cw) {
+  const int ox = blockIdx.y * blockDim.x + threadIdx.x;
+  if (ox >= cw) return;
+  const int oy = blockIdx.x % ch, n = blockIdx.x / ch;
+  const int4 b = boxes[n];                                               // (y0, x0, h, w), inside the image (host-drawn)
+  int iy0, iy1, ix0, ix1;
+  float ly, lx;
+  rrc_axis(oy, __fdiv_rn((float)b.z, (float)ch), b.z, iy0, iy1, ly);
+  rrc_axis(flips[n] ? cw - 1 - ox : ox, __fdiv_rn((float)b.w, (float)cw), b.w, ix0, ix1, lx);
+  // texel offsets inside one image (host checks H*W*C < 2^31)
+  const unsigned r0 = (unsigned)((b.x + iy0) * W + b.y) * (unsigned)C, r1 = (unsigned)((b.x + iy1) * W + b.y) * (unsigned)C;
+  const unsigned c0 = (unsigned)ix0 * (unsigned)C, c1 = (unsigned)ix1 * (unsigned)C;
+  const unsigned t00 = r0 + c0, t01 = r0 + c1, t10 = r1 + c0, t11 = r1 + c1;
+  const uint8_t* src = x + (long long)n * H * W * C;
+  const float wy0 = 1.f - ly, wx0 = 1.f - lx;
+  Tout* o = out + ((long long)blockIdx.x * cw + ox) * C;
+  auto tap = [&](unsigned t, int c, float s) {
+    const float m = mean_mode == 0 ? mean[0] : (mean_mode == 1 ? mean[c] : mean[t + c]);
+    return ((float)src[t + c] - m) * s;
+  };
+  auto blend = [&](int c, float s) {
+    return wy0 * (wx0 * tap(t00, c, s) + lx * tap(t01, c, s)) + ly * (wx0 * tap(t10, c, s) + lx * tap(t11, c, s));
+  };
+  if (C == 3) {
+    const float s0 = cscale ? scale * cscale[0] : scale, s1 = cscale ? scale * cscale[1] : scale, s2 = cscale ? scale * cscale[2] : scale;
+    const float v0 = blend(0, s0), v1 = blend(1, s1), v2 = blend(2, s2);
+    o[0] = (Tout)v0; o[1] = (Tout)v1; o[2] = (Tout)v2;
+    return;
+  }
+  for (int c = 0; c < C; ++c) o[c] = (Tout)blend(c, cscale ? scale * cscale[c] : scale);
+}
+
+void resized_crop_mirror_norm(const void* x, const void* mean, int mean_mode, float scale, const void* cscale, void* out, int out_bf16,
+                              const void* boxes, const void* flips, int N, int H, int W, int C, int ch, int cw, cudaStream_t st) {
+  if ((long long)H * W * C >= (1LL << 31) || (long long)N * ch >= (1LL << 31)) throw std::runtime_error("resized_crop_mirror_norm: image too large");
+  const dim3 g((unsigned)(N * ch), (unsigned)((cw + 127) / 128));
+  auto X = (const uint8_t*)x; auto M = (const float*)mean; auto CS = (const float*)cscale;
+  auto B = (const int4*)boxes; auto F = (const uint8_t*)flips;
+  if (out_bf16) resized_crop_mirror_norm_kernel<__nv_bfloat16><<<g, 128, 0, st>>>(X, M, mean_mode, scale, CS, (__nv_bfloat16*)out, B, F, H, W, C, ch, cw);
+  else resized_crop_mirror_norm_kernel<float><<<g, 128, 0, st>>>(X, M, mean_mode, scale, CS, (float*)out, B, F, H, W, C, ch, cw);
+  count_launch(); TMPI_CHECK_LAUNCH("resized_crop_mirror_norm"); ::tmpi::check_capture(st, "resized_crop_mirror_norm");
+}
+
 }  // namespace tmpi

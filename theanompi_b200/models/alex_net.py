@@ -39,6 +39,7 @@ seed_weight_on_pid = False
 
 
 class AlexNet(ModelBase):
+    supports_resized_crop = True
     n_epochs, momentum, weight_decay = n_epochs, momentum, weight_decay
     batch_size, file_batch_size, learning_rate = batch_size, file_batch_size, learning_rate
     lr_policy, lr_step = lr_policy, lr_step
@@ -74,7 +75,8 @@ class AlexNet(ModelBase):
         if self.data.para_load and not self.no_paraload:
             self.data.spawn_load()
             self.data.para_load_init(self.device, self.input_width, self.input_height,
-                                     self.rand_crop, self.batch_crop_mirror, out_dtype=self.act_dtype)
+                                     self.rand_crop, self.batch_crop_mirror, out_dtype=self.act_dtype,
+                                     resized_crop=self.resized_crop, rank=self.rank)
 
     def build_model(self):
         if self.verbose:

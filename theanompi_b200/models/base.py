@@ -68,6 +68,7 @@ class ModelBase(object):
     supports_label_smoothing = True    # config['label_smoothing'] > 0 (False: no classifier head; refused at compile_iter_fns)
     supports_mixup = True          # config['mixup'] (False: no image batch before a first convolution; refused at compile_iter_fns)
     supports_drop_path = False     # config['drop_path_rate'] > 0 (True: residual blocks in self.body that read drop_row(l))
+    supports_resized_crop = False  # config['random_resized_crop'] (True: ImageNet models fed by ParaLoader; refused at construction)
     name = "Model"
 
     def __init__(self, config):
@@ -127,6 +128,10 @@ class ModelBase(object):
         self.drop_path_rate = config.get("drop_path_rate", 0.0)
         self.drop_path = None
         self._drop_on = False
+        # random-resized crop of the training images (a dict, models/data/utils.py: check_resized_crop; None = off): per-image boxes
+        # drawn by the loader and resampled by its kernel on the copy stream.  Checked here because the model's constructor builds
+        # the loader; the training step never sees it
+        self.resized_crop = self.check_resized_crop(config.get("random_resized_crop"))
         self.base_lr = np.float32(self.learning_rate)
         self.current_t = self.subb_t = 0
         self.current_v = self.subb_v = 0
@@ -400,6 +405,24 @@ class ModelBase(object):
                              "ResNet50 and Wide_ResNet" % self.name)
         self.mixer = Mixer(cfg, self.rank, self.mix_hw, self.device)
 
+    # ------------------------------------------------------------------ random-resized crop
+    def check_resized_crop(self, cfg):
+        """The validated ``config['random_resized_crop']`` (models/data/utils.py: check_resized_crop; a ValueError names the key), or
+        None.  A dict needs a model whose ImageNet loader draws a random crop per image: ``supports_resized_crop``, and neither
+        ``batch_crop_mirror`` (one crop for the whole batch) nor ``rand_crop = False`` (always the centre crop)."""
+        from .data.utils import RRC_KEY, check_resized_crop
+        cfg = check_resized_crop(cfg)
+        if cfg is None:
+            return None
+        name = type(self).__name__
+        if not self.supports_resized_crop:
+            raise ValueError("%s: %s is not supported; it augments the ImageNet loader of AlexNet, GoogLeNet, VGG16, ResNet50, "
+                             "ResNet152 and ResNet50Torch" % (name, RRC_KEY))
+        if self.batch_crop_mirror or not self.rand_crop:
+            raise ValueError("%s: %s draws a random box per image, which contradicts %s" % (
+                name, RRC_KEY, "batch_crop_mirror = True" if self.batch_crop_mirror else "rand_crop = False"))
+        return cfg
+
     # ------------------------------------------------------------------ stochastic depth (drop-path)
     def check_drop_path(self):
         """``config['drop_path_rate']`` must be a finite real p in [0, 1) (ops/drop_path.py: check_rate; a ValueError names the key),
@@ -631,6 +654,10 @@ class ModelBase(object):
         nbytes = 0
         if loader is not None:
             if idx == 0:
+                # a new pass over the files: first consume the look-ahead issued for the last file of the previous pass, as
+                # reset_iter does.  Left outstanding, every later get() would return the batch one request behind its labels, and
+                # with two requests in flight the loader would refill the ring slot the trainer is still reading
+                loader.drain()
                 loader.set_mode(mode)
                 loader.request(img[idx], mode)
             loader.request(img[idx + 1] if not last else img[idx], mode)

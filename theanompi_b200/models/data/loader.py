@@ -31,20 +31,25 @@ import numpy as np
 import torch
 
 from ... import ops
-from .utils import draw_crops
+from .utils import draw_crops, draw_resized_crops, resized_crop_rng
 
 
 class LoadedBatch(object):
-    __slots__ = ("x", "slot", "ready", "item", "h2d_bytes")
+    """One loaded batch; ``boxes`` / ``flips``: the host copies of the random-resized-crop draw it was made with (None otherwise)."""
+    __slots__ = ("x", "slot", "ready", "item", "h2d_bytes", "boxes", "flips")
 
-    def __init__(self, x, slot, ready, item, h2d_bytes):
+    def __init__(self, x, slot, ready, item, h2d_bytes, boxes=None, flips=None):
         self.x, self.slot, self.ready, self.item, self.h2d_bytes = x, slot, ready, item, h2d_bytes
+        self.boxes, self.flips = boxes, flips
 
 
 class ParaLoader(object):
     def __init__(self, read_fn, device, raw_shape, crop_hw, mean, std_scale=1.0 / 255.0,
                  out_dtype=None, depth=2, rand_crop=True, batch_crop_mirror=False, seed=1234,
-                 threaded=True, host_buffers=None, on_close=None):
+                 threaded=True, host_buffers=None, on_close=None, resized_crop=None, rank=0):
+        """``resized_crop``: a validated ``config['random_resized_crop']`` (``utils.check_resized_crop``) or None; with it every
+        "train" batch is a random-resized crop drawn per image from the generator keyed by (its seed, ``rank``), and "val" batches
+        keep the centre crop."""
         self.read_fn = read_fn
         self.device = torch.device(device)
         self.cuda = self.device.type == "cuda"
@@ -72,7 +77,13 @@ class ParaLoader(object):
             self._ext_host = False
         self.host_offs = [torch.empty((N, 2), dtype=torch.int32, pin_memory=pin) for _ in range(depth)]
         self.host_flip = [torch.empty((N,), dtype=torch.uint8, pin_memory=pin) for _ in range(depth)]
+        self.resized_crop = resized_crop
+        if resized_crop is not None:
+            self.rrc_rng = resized_crop_rng(resized_crop, rank)
+            self.host_boxes = [torch.empty((N, 4), dtype=torch.int32, pin_memory=pin) for _ in range(depth)]
         if self.cuda:
+            if resized_crop is not None:
+                self.dev_boxes = [torch.empty((N, 4), dtype=torch.int32, device=self.device) for _ in range(depth)]
             self.stage = [torch.empty(self.raw_shape, dtype=torch.uint8, device=self.device) for _ in range(depth)]
             self.dev_offs = [torch.empty((N, 2), dtype=torch.int32, device=self.device) for _ in range(depth)]
             self.dev_flip = [torch.empty((N,), dtype=torch.uint8, device=self.device) for _ in range(depth)]
@@ -108,6 +119,8 @@ class ParaLoader(object):
             # the ring slot is refilled by another process as soon as we request the next file: the DMA out of it must have
             # finished before this slot comes round again — recorded below, awaited at the top of the next _produce(s)
             pass
+        if self.resized_crop is not None and mode == "train":
+            return self._produce_resized(s, src, item)
         offs, flips = draw_crops(N, (H, W), self.crop_hw, mode, self.rand_crop, self.batch_crop_mirror, self.rs)
         self.host_offs[s].numpy()[...] = offs
         self.host_flip[s].numpy()[...] = flips
@@ -128,6 +141,31 @@ class ParaLoader(object):
             self.out[s].copy_(x)
             ready = None
         return LoadedBatch(self.out[s], s, ready, item, self.h2d_bytes)
+
+    def _produce_resized(self, s, src, item):
+        """A "train" batch with ``resized_crop``: boxes and flips drawn on the host, the 16-byte box record copied next to the flips
+        and ``resized_crop_mirror_norm`` launched on the copy stream (the reference on the CPU)."""
+        N, H, W, C = self.raw_shape
+        boxes, flips = draw_resized_crops(N, (H, W), self.resized_crop["scale"], self.resized_crop["ratio"], self.rrc_rng)
+        self.host_boxes[s].numpy()[...] = boxes
+        self.host_flip[s].numpy()[...] = flips
+        nbytes = int(np.prod(self.raw_shape)) + N * 17
+        if self.cuda:
+            with torch.cuda.stream(self.copy_stream):
+                self.stage[s].copy_(src, non_blocking=True)
+                self.dev_boxes[s].copy_(self.host_boxes[s], non_blocking=True)
+                self.dev_flip[s].copy_(self.host_flip[s], non_blocking=True)
+                from ...ops import cuda_impl
+                cuda_impl.resized_crop_mirror_normalize(self.stage[s], self.mean, self.std_scale, self.crop_hw, self.dev_boxes[s],
+                                                        self.dev_flip[s], self.out_dtype, out=self.out[s])
+                ready = torch.cuda.Event()
+                ready.record(self.copy_stream)
+        else:
+            x = ops.reference.resized_crop_mirror_normalize(src, self.mean, self.std_scale, self.crop_hw, self.host_boxes[s],
+                                                            self.host_flip[s], self.out_dtype)
+            self.out[s].copy_(x)
+            ready = None
+        return LoadedBatch(self.out[s], s, ready, item, nbytes, boxes, flips)
 
     def _run(self):
         if self.cuda:

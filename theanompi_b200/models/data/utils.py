@@ -9,6 +9,7 @@ one pass after the pinned H2D copy.
 """
 from __future__ import annotations
 
+import math
 import os
 import pickle
 
@@ -94,6 +95,77 @@ def draw_crops(n, in_hw, out_hw, mode, rand_crop=True, batch_crop_mirror=False, 
     ox = rs.randint(0, W - cw + 1, n)
     flips = (rs.rand(n) > 0.5).astype(np.uint8)
     return np.stack([oy, ox], 1).astype(np.int32), flips
+
+
+RRC_KEY = "random_resized_crop"
+RRC_DEFAULTS = {"scale": (0.08, 1.0), "ratio": (3.0 / 4.0, 4.0 / 3.0), "seed": 0}
+RRC_ATTEMPTS = 10
+
+
+def _real(v):
+    return not isinstance(v, bool) and isinstance(v, (int, float, np.integer, np.floating)) and math.isfinite(v)
+
+
+def check_resized_crop(cfg):
+    """The validated ``config['random_resized_crop']`` with every key filled in (``scale`` and ``ratio`` as float pairs), or None for
+    None; anything else is a ValueError that names the key.  Lists and tuples are both accepted, so the value survives JSON."""
+    if cfg is None:
+        return None
+    if not isinstance(cfg, dict):
+        raise ValueError("%s must be a dict or None, not %r" % (RRC_KEY, cfg))
+    unknown = sorted(str(k) for k in cfg if k not in RRC_DEFAULTS)
+    if unknown:
+        raise ValueError("%s: unknown key %r; the keys are %s" % (RRC_KEY, unknown[0], ", ".join(RRC_DEFAULTS)))
+    out = {}
+    for k in ("scale", "ratio"):
+        v = cfg.get(k, RRC_DEFAULTS[k])
+        if not (isinstance(v, (list, tuple)) and len(v) == 2 and all(_real(e) for e in v)):
+            raise ValueError("%s[%r] must be two finite real numbers [lo, hi], not %r" % (RRC_KEY, k, v))
+        lo, hi = float(v[0]), float(v[1])
+        if not (0.0 < lo <= hi and (k == "ratio" or hi <= 1.0)):
+            raise ValueError("%s[%r] must satisfy %s, not %r" % (RRC_KEY, k, "0 < lo <= hi <= 1" if k == "scale" else "0 < lo <= hi", v))
+        out[k] = (lo, hi)
+    seed = cfg.get("seed", 0)
+    if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)):
+        raise ValueError("%s['seed'] must be an int, not %r" % (RRC_KEY, seed))
+    out["seed"] = int(seed) & (2 ** 64 - 1)
+    return out
+
+
+def resized_crop_rng(cfg, rank):
+    """The box / flip generator of one worker, keyed by (seed, rank); separate from the fixed-crop RandomState, so a run without the
+    key draws what it always drew."""
+    return np.random.default_rng([cfg["seed"], int(rank)])
+
+
+def draw_resized_crops(n, in_hw, scale, ratio, rng):
+    """Per-image boxes (y0, x0, h, w) (int32 [n, 4]) and flip flags (uint8 [n], p = ½), drawn as torchvision's
+    ``RandomResizedCrop.get_params``: up to 10 attempts of area H·W·U(scale) and ratio exp(U(log ratio)), w = round(√(area·r)),
+    h = round(√(area / r)) (round half to even); the first attempt that fits sits at a uniform position, an image without one
+    takes the centred box with the ratio clamped to its bounds.  All attempts of the batch are drawn at once."""
+    H, W = in_hw
+    lr = np.log(ratio)
+    area = (H * W) * rng.uniform(scale[0], scale[1], (n, RRC_ATTEMPTS))
+    r = np.exp(rng.uniform(lr[0], lr[1], (n, RRC_ATTEMPTS)))
+    w = np.rint(np.sqrt(area * r)).astype(np.int64)
+    h = np.rint(np.sqrt(area / r)).astype(np.int64)
+    fits = (w > 0) & (w <= W) & (h > 0) & (h <= H)
+    first = np.argmax(fits, axis=1)
+    ok = fits[np.arange(n), first]
+    h, w = h[np.arange(n), first], w[np.arange(n), first]
+    # the fallback, torchvision's centred box (at least one pixel: a ratio far outside the image's can round a side to 0)
+    in_r = W / H
+    if in_r < ratio[0]:
+        fh, fw = max(1, int(round(W / ratio[0]))), W
+    elif in_r > ratio[1]:
+        fh, fw = H, max(1, int(round(H * ratio[1])))
+    else:
+        fh, fw = H, W
+    h, w = np.where(ok, h, fh), np.where(ok, w, fw)
+    y0 = np.where(ok, rng.integers(0, H - h + 1), (H - fh) // 2)
+    x0 = np.where(ok, rng.integers(0, W - w + 1), (W - fw) // 2)
+    flips = (rng.random(n) < 0.5).astype(np.uint8)
+    return np.stack([y0, x0, h, w], 1).astype(np.int32), flips
 
 
 def crop_and_mirror(data, mode, rand_crop, flag_batch, cropsize, rs=None):

@@ -67,6 +67,7 @@ class ResNet50Net(nn.Module):
 
 class ResNet50(ModelBase):
     supports_drop_path = True      # one drop-path block per bottleneck
+    supports_resized_crop = True
     n_epochs, momentum, weight_decay = n_epochs, momentum, weight_decay
     batch_size, file_batch_size, learning_rate = batch_size, file_batch_size, learning_rate
     lr_policy, lr_step = lr_policy, lr_step
@@ -96,7 +97,8 @@ class ResNet50(ModelBase):
         if self.data.para_load and not self.no_paraload:
             self.data.spawn_load()
             self.data.para_load_init(self.device, self.input_width, self.input_height, self.rand_crop,
-                                     self.batch_crop_mirror, out_dtype=self.act_dtype)
+                                     self.batch_crop_mirror, out_dtype=self.act_dtype,
+                                     resized_crop=self.resized_crop, rank=self.rank)
 
     # ---- construction: every conv is bias-free and linear; BatchNormal carries the ReLU (and the shortcut add)
     def _conv(self, inp, cout, k, stride, pad, input_shape=None):
@@ -160,6 +162,7 @@ class ResNet50(ModelBase):
 
 
 class ResNet50Torch(TorchModelBase):
+    supports_resized_crop = True   # the same ImageNet loader as ResNet50
     n_epochs, momentum, weight_decay = n_epochs, momentum, weight_decay
     batch_size, file_batch_size, learning_rate = batch_size, file_batch_size, learning_rate
     lr_policy, lr_step = lr_policy, lr_step
@@ -186,4 +189,5 @@ class ResNet50Torch(TorchModelBase):
         if self.data.para_load and not self.no_paraload:
             self.data.spawn_load()
             self.data.para_load_init(self.device, self.input_width, self.input_height, self.rand_crop,
-                                     self.batch_crop_mirror, out_dtype=self.act_dtype)
+                                     self.batch_crop_mirror, out_dtype=self.act_dtype,
+                                     resized_crop=self.resized_crop, rank=self.rank)

@@ -30,6 +30,7 @@ CFG = [64, 64, "M", 128, 128, "M", 256, 256, 256, "M", 512, 512, 512, "M", 512, 
 
 
 class VGG16(ModelBase):
+    supports_resized_crop = True
     n_epochs, momentum, weight_decay = n_epochs, momentum, weight_decay
     batch_size, file_batch_size, learning_rate = batch_size, file_batch_size, learning_rate
     lr_policy, lr_step = lr_policy, lr_step
@@ -58,7 +59,8 @@ class VGG16(ModelBase):
         if self.data.para_load and not self.no_paraload:
             self.data.spawn_load()
             self.data.para_load_init(self.device, self.input_width, self.input_height, self.rand_crop,
-                                     self.batch_crop_mirror, out_dtype=self.act_dtype)
+                                     self.batch_crop_mirror, out_dtype=self.act_dtype,
+                                     resized_crop=self.resized_crop, rank=self.rank)
 
     def build_model(self):
         v, B = self.verbose, self.batch_size

@@ -853,6 +853,38 @@ def crop_mirror_normalize(x, mean, std_scale, crop_hw, offsets, flips, out_dtype
     return out
 
 
+def resized_crop_mirror_normalize(x, mean, std_scale, out_hw, boxes, flips, out_dtype=None, out=None):
+    """Random-resized crop of a uint8 NHWC batch (``nn_kernels.cu: resized_crop_mirror_norm_kernel``): image n's box
+    ``boxes[n] = (y0, x0, h, w)`` (int32 [N, 4] on the device, inside the image) normalised, bilinearly resampled to ``out_hw`` and
+    mirrored where ``flips[n]``.  Same mean / ``std_scale`` forms as :func:`crop_mirror_normalize`; see
+    :func:`reference.resized_crop_mirror_normalize`."""
+    out_dtype = out_dtype or ADT()
+    if x.dtype != torch.uint8:
+        raise ValueError("resized_crop_mirror_normalize takes a uint8 NHWC batch, not %s" % x.dtype)
+    x = x.contiguous()
+    N, H, W, C = x.shape
+    ch, cw = out_hw
+    mean = mean.float().contiguous()
+    mode = 0 if mean.numel() == 1 else (1 if mean.numel() == C else 2)
+    if mode == 2:
+        assert mean.numel() == H * W * C
+    if out is None:
+        out = torch.empty((N, ch, cw, C), dtype=out_dtype, device=x.device)
+    assert out.dtype in (BF16, torch.float32) and out.is_contiguous() and tuple(out.shape) == (N, ch, cw, C)
+    boxes = boxes.to(torch.int32).contiguous()
+    assert tuple(boxes.shape) == (N, 4) and boxes.device == x.device and boxes.data_ptr() % 16 == 0
+    flips = flips.to(torch.uint8).contiguous()
+    if isinstance(std_scale, torch.Tensor):
+        cs = std_scale.to(device=x.device, dtype=torch.float32).contiguous()
+        assert cs.numel() == C
+        sc, cs_ptr = 1.0, cs.data_ptr()
+    else:
+        sc, cs_ptr = float(std_scale), 0
+    L().resized_crop_mirror_norm(x.data_ptr(), mean.data_ptr(), mode, sc, cs_ptr, out.data_ptr(), int(out.dtype == BF16),
+                                 boxes.data_ptr(), flips.data_ptr(), N, H, W, C, ch, cw, _st(x))
+    return out
+
+
 # --------------------------------------------------------------------------- optimizer
 def _table(arena):
     if not hasattr(arena, "_tab_cache"):

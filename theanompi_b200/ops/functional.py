@@ -575,3 +575,12 @@ def crop_mirror_normalize(x, mean, std_scale, crop_hw, offsets, flips, out_dtype
         return cuda_impl.crop_mirror_normalize(x, mean, std_scale, crop_hw, offsets, flips, out_dtype)
     return ref.crop_mirror_normalize(x, mean, std_scale, crop_hw, offsets, flips,
                                      out_dtype or torch.float32)
+
+
+def resized_crop_mirror_normalize(x, mean, std_scale, out_hw, boxes, flips, out_dtype=None):
+    """Random-resized crop of a uint8 NHWC batch: the native kernel on CUDA, :func:`reference.resized_crop_mirror_normalize` on
+    the CPU."""
+    if x.is_cuda:
+        from . import cuda_impl
+        return cuda_impl.resized_crop_mirror_normalize(x, mean, std_scale, out_hw, boxes, flips, out_dtype)
+    return ref.resized_crop_mirror_normalize(x, mean, std_scale, out_hw, boxes, flips, out_dtype or torch.float32)

@@ -653,6 +653,29 @@ def crop_mirror_normalize(x_u8, mean, std_scale, crop_hw, offsets, flips, out_dt
     return out.to(out_dtype)
 
 
+def resized_crop_mirror_normalize(x_u8, mean, std_scale, out_hw, boxes, flips, out_dtype=torch.float32):
+    """Random-resized crop: ``(x - mean) * std_scale`` (each source pixel with its own mean) → image i's box
+    ``boxes[i] = (y0, x0, h, w)`` → ``F.interpolate(size=out_hw, mode='bilinear', align_corners=False, antialias=False)`` → optional
+    horizontal flip, as torchvision's ``RandomResizedCrop`` then ``RandomHorizontalFlip`` without the antialiasing filter.
+
+    x_u8 : [N, H, W, C] uint8;  mean: [H, W, C], [C] or scalar;  boxes: [N, 4] int, inside the image;  flips: [N] bool
+    """
+    import torch.nn.functional as F
+    N, H, W, C = x_u8.shape
+    if isinstance(std_scale, torch.Tensor):
+        std_scale = std_scale.to(device=x_u8.device, dtype=torch.float32)
+    x = (x_u8.float() - mean.float()) * std_scale
+    out = torch.empty((N,) + tuple(out_hw) + (C,), dtype=torch.float32, device=x.device)
+    for i in range(N):
+        y0, x0, h, w = (int(v) for v in boxes[i])
+        if not (h > 0 and w > 0 and 0 <= y0 <= H - h and 0 <= x0 <= W - w):
+            raise ValueError("resized_crop_mirror_normalize: box %r of image %d is not inside %d x %d" % ((y0, x0, h, w), i, H, W))
+        box = x[i, y0:y0 + h, x0:x0 + w, :].permute(2, 0, 1).unsqueeze(0)
+        y = F.interpolate(box, size=tuple(out_hw), mode="bilinear", align_corners=False, antialias=False)[0].permute(1, 2, 0)
+        out[i] = y.flip(1) if bool(flips[i]) else y
+    return out.to(out_dtype)
+
+
 # --------------------------------------------------------------------------- batch norm (+ residual)(+ ReLU), NHWC
 def _per_sample(s, x):
     """A drop-path row (one scale per sample of x's leading axis) shaped to broadcast over x."""
