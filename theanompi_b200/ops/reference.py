@@ -275,6 +275,24 @@ def uniform_noise(shape, seed, stream, step, device="cpu"):
     return torch.from_numpy(u.reshape(shape)).to(device)
 
 
+def dropout_mask_philox(n, p_drop, seed, layer, step):
+    """Keep-mask (bool [n], n a multiple of 8) of the CUDA ``dropout_fwd`` kernel, bit for bit: group j of 8 elements draws
+    Philox(counter = (j, step), key = (seed_lo, seed_hi ^ layer·0x9E3779B9)); element i of the group takes 16-bit half i & 1 of
+    word i >> 1 and is kept iff it is >= the threshold (uint32)(float(p_drop)·65536), so P(keep) = 1 − ⌊p·65536⌋ / 65536.
+    (:func:`dropout_mask` is the CPU execution path's own mask; this one is the kernel's host twin for tests.)"""
+    n = int(n)
+    if n % 8:
+        raise ValueError("dropout_mask_philox: n must be a multiple of 8")
+    j = np.arange(n // 8, dtype=np.uint64)
+    seed, step, layer = int(seed) & (2 ** 64 - 1), int(step) & (2 ** 64 - 1), int(layer) & 0xFFFFFFFF
+    r = _philox4x32((j, j >> np.uint64(32), np.full_like(j, step & 0xFFFFFFFF), np.full_like(j, step >> 32)),
+                    seed & 0xFFFFFFFF, ((seed >> 32) ^ (layer * 0x9E3779B9)) & 0xFFFFFFFF)
+    words = np.stack(r, axis=1)                                                           # [groups, 4]
+    halves = np.stack([words & np.uint64(0xFFFF), words >> np.uint64(16)], axis=2)      # [groups, 4, 2]: element i = (i >> 1, i & 1)
+    thr = np.uint64(int(np.float32(p_drop) * np.float32(65536.0)))
+    return torch.from_numpy((halves.reshape(-1) >= thr))
+
+
 # --------------------------------------------------------------------------- Mixup / CutMix
 _MIX_TAG = 0xFFFFFFFF          # second counter word of every mix block (csrc/nn_kernels.cu: kMixCounterTag)
 _MIX_ATTEMPTS = 16             # Marsaglia–Tsang attempts per Gamma variate (kMixAttempts)
