@@ -123,7 +123,7 @@ def model_steps(name, build, rates, rounds, steps):
         for _ in range(4):                            # the second warm-up and the CUDA-graph capture
             m.train_iter_fn(0)
     torch.cuda.synchronize()
-    assert all(m._graph is not None for m in models.values()), "a step was not captured"
+    assert all("step" in m.captured_steps() for m in models.values()), "a step was not captured"
     res = alternate({k: (lambda m=m: m.train_iter_fn(0)) for k, m in models.items()}, rounds, steps)
     print(json.dumps({name + "_ms_per_step": res, name + "_native_launches_per_step": launches}))
     for m in models.values():

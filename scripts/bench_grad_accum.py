@@ -42,7 +42,7 @@ def build(name, mod, cls, n, B, library=False, **cfg):
                                                         file_batch_size=n * B, cuda_graph=True, grad_accum=n, **cfg))
     m.compile_iter_fns("avg")
     if library:
-        body = m._accum_body
+        body = m._step_body
 
         def library_body(kind):
             # the flag is read when each micro-step kind's graph is captured
@@ -54,7 +54,7 @@ def build(name, mod, cls, n, B, library=False, **cfg):
                 for p in m.arena.params:
                     p.gaccum = False
 
-        m._accum_body = library_body
+        m._step_body = library_body
     torch.manual_seed(0)
     m.shared_x.copy_(torch.randint(0, 256, tuple(m.shared_x.shape), device="cuda:0").to(m.shared_x.dtype))
     m.shared_y.copy_(torch.randint(0, 10, (m.shared_y.shape[0],), device="cuda:0").to(m.shared_y.dtype))

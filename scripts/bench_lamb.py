@@ -107,7 +107,7 @@ def main():
         for _ in range(5):                            # eager warm-up and the CUDA-graph capture
             mm.train_iter_fn(0)
     torch.cuda.synchronize()
-    assert all(mm._graph is not None for mm in models.values()), "a step was not captured"
+    assert all("step" in mm.captured_steps() for mm in models.values()), "a step was not captured"
     res = {o: [] for o in models}
     for _ in range(args.rounds):
         for o, mm in models.items():

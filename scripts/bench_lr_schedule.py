@@ -51,7 +51,7 @@ def main():
         for _ in range(5):                            # eager warm-up and the CUDA-graph capture
             mm.train_iter_fn(0)
     torch.cuda.synchronize()
-    assert all(mm._graph is not None for mm in models.values()), "a step was not captured"
+    assert all("step" in mm.captured_steps() for mm in models.values()), "a step was not captured"
     res = alternate({k: (lambda mm=mm: mm.train_iter_fn(0)) for k, mm in models.items()}, args.rounds, args.steps)
     sched = models["sgd_warmup_cosine"].lr_sched
     print(json.dumps({"alexnet_b128_ms_per_step": res, "schedule": SCHED, "updates": int(sched.u), "lr_last": sched.value()}))

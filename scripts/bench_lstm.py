@@ -70,7 +70,7 @@ def main():
                     torch.cuda.synchronize()
                     res.append((time.perf_counter() - t) * 1000.0 / args.iters)
                 res.sort()
-                captured = sorted(k for k, s in getattr(m, "_graphs", {}).items() if s["graph"] is not None)
+                captured = sorted(m.captured_steps())
                 print(json.dumps({"arm": arm, "class": cls, "dtype": dtype, "seq_len": [lo, hi], "batch": m.batch_size, "H": 128,
                                   "mean_T": sum(b[0].shape[1] for b in batches) / len(batches), "buckets": sorted(first),
                                   "graphs_captured": captured, "ms_per_train_iter": res[len(res) // 2], "min": res[0],

@@ -116,7 +116,7 @@ def train_steps(name, build, rounds, steps):
         for _ in range(6):                            # eager warm-up and the CUDA-graph capture
             fn()
         torch.cuda.synchronize()
-        assert m._graph is not None, "the step was not captured"
+        assert "step" in m.captured_steps(), "the step was not captured"
     res = {k: [] for k in models}
     for _ in range(rounds):
         for k in models:

@@ -261,7 +261,7 @@ def runs(spec, runs_, steps=5):
         for i in range(steps):
             m.train_iter(i, rec)
         torch.cuda.synchronize()
-        used = m._graph is not None or any(v["graph"] is not None for v in m._graphs.values())
+        used = bool(m.captured_steps())
         out[name] = (m.arena.W.clone(), m.arena.U.clone(), float(rec.train_info["cost"][-1]), used)
         m.cleanup()
         del m

@@ -277,7 +277,7 @@ def _alexnet_run(graph, steps):
     return m, losses
 
 
-def test_graph_replay_matches_eager_bitwise():
+def test_kind_keyed_graph_replay_matches_eager_bitwise():
     """Deterministic mode, five windows (two eager warm-ups per kind, the captures, then two windows of replays): the three captured
     micro-step graphs give the weights and losses of eager launches bit for bit."""
     code = """
@@ -289,7 +289,7 @@ for name, graph in (("eager", False), ("graph", True)):
     m, losses = t._alexnet_run(graph, 15)
     assert m.use_graph == graph and m.n_updates == 5, (m.use_graph, m.n_updates)
     if graph:
-        assert sorted(k[1] for k in m._graphs if isinstance(k, tuple)) == ['first', 'last', 'mid']
+        assert sorted(m.captured_steps()) == ['first', 'last', 'mid']
     out[name] = (m.arena.W.clone(), losses)
 print('max |dW| graph/eager %%g' %% float((out['graph'][0] - out['eager'][0]).abs().max()))
 assert torch.equal(out['graph'][0], out['eager'][0]) and out['graph'][1] == out['eager'][1]
@@ -305,7 +305,7 @@ print('OK')
 def _library_route(m):
     """Make ``m``'s mid and last micro-steps take the library route of gradient accumulation: every parameter flagged ``gaccum``, so
     each gradient is stored into a scratch buffer and added into G by ``add_`` (as scripts/bench_grad_accum.py row d)."""
-    body = m._accum_body
+    body = m._step_body
 
     def library_body(kind):
         for p in m.arena.params:
@@ -316,10 +316,10 @@ def _library_route(m):
             for p in m.arena.params:
                 p.gaccum = False
 
-    m._accum_body = library_body
+    m._step_body = library_body
 
 
-def test_library_route_matches_native_accumulation():
+def test_library_step_body_matches_native_accumulation():
     """The library route (scratch gradient + add_) and the native accumulate modes compute the same windows: deterministic mode,
     two windows of AlexNet, bit for bit (both add each micro-batch's gradient onto G with one fp32 add per element)."""
     code = """

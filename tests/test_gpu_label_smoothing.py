@@ -81,8 +81,7 @@ def _train(m, steps, dev):
 
 
 def alexnet_runs(runs, steps=6):
-    """AlexNet-128b bf16, ``runs`` = [(name, cuda_graph, extra config)]: name → (W, U, losses, graph captured).  A graph replay
-    returns the same output tensor every step, so of a graph run's recorded losses only the last is that step's."""
+    """AlexNet-128b bf16, ``runs`` = [(name, cuda_graph, extra config)]: name → (W, U, losses, graph captured)."""
     from theanompi_b200.ops import cuda_impl
     mod, cls, cfg = ALEX
     out = {}
@@ -90,7 +89,7 @@ def alexnet_runs(runs, steps=6):
         cuda_impl._STEP.clear()
         m = _model(mod, cls, "cuda:0", cuda_graph=graph, **dict(cfg, **extra))
         losses = _train(m, steps, "cuda:0")
-        out[name] = (m.arena.W.clone(), m.arena.U.clone(), losses, m._graph is not None)
+        out[name] = (m.arena.W.clone(), m.arena.U.clone(), losses, "step" in m.captured_steps())
         m.cleanup()
         del m
     return out
@@ -191,7 +190,7 @@ def test_lstm_two_buckets_matches_cpu_reference(monkeypatch):
         m._train_it = iter(batches)
         costs[dev] = _train(m, len(batches), dev)
         if dev != "cpu":
-            graphs = sorted(k for k in m._graphs if m._graphs[k]["graph"] is not None)
+            graphs = sorted(m.captured_steps())
     print(costs, graphs)
     assert graphs == [16, 48], graphs
     for a, b in zip(costs["cpu"], costs["cuda:0"]):

@@ -121,7 +121,7 @@ def model_oracle(which):
         assert any(getattr(p, "sgd_epilogue", None) is not None for p in a.arena.params), "the FC SGD epilogue is not armed"
     lrs = _steps(a, n, rec)
     assert follows_schedule(lrs, float(a.learning_rate)), lrs
-    graphs = a._graph is not None or bool(a._graphs)
+    graphs = bool(a.captured_steps())
     wa = [a.arena.W.clone(), a.arena.U.clone()]
     a.cleanup()
     del a
@@ -162,7 +162,7 @@ def lstm_oracle():
             m.train_iter(i, rec)
             got.append(m.arena.hyper[0].clone())
         torch.cuda.synchronize()
-        runs.append(([float(v) for v in got], m.arena.W.clone(), sorted(k for k in m._graphs if m._graphs[k]["graph"] is not None)))
+        runs.append(([float(v) for v in got], m.arena.W.clone(), sorted(m.captured_steps())))
     return runs
 
 

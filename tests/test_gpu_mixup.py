@@ -187,8 +187,7 @@ def _train(m, steps, dev, recs=None):
 
 
 def alexnet_runs(runs, steps=6):
-    """AlexNet-128b bf16, ``runs`` = [(name, cuda_graph, extra config)]: name → (W, U, losses, graph captured).  A graph replay
-    returns the same output tensor every step, so of a graph run's recorded losses only the last is that step's."""
+    """AlexNet-128b bf16, ``runs`` = [(name, cuda_graph, extra config)]: name → (W, U, losses, graph captured)."""
     from theanompi_b200.ops import cuda_impl
     mod, cls, cfg = ALEX
     out = {}
@@ -196,7 +195,7 @@ def alexnet_runs(runs, steps=6):
         cuda_impl._STEP.clear()
         m = _model(mod, cls, "cuda:0", cuda_graph=graph, **dict(cfg, **extra))
         losses, _ = _train(m, steps, "cuda:0")
-        out[name] = (m.arena.W.clone(), m.arena.U.clone(), losses, m._graph is not None)
+        out[name] = (m.arena.W.clone(), m.arena.U.clone(), losses, "step" in m.captured_steps())
         m.cleanup()
         del m
     return out

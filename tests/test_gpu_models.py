@@ -44,6 +44,30 @@ def test_alexnet_graph_and_eager_agree():
     assert abs(losses[0] - losses[1]) < 0.15, losses
 
 
+def test_captured_steps_record_their_own_costs():
+    """Six AlexNet steps under a CUDA graph (two eager warm-ups, the capture, three replays): every cost the recorder keeps still
+    holds its own step's value after the loop, so the printed mean over a period is the mean of its steps.  The batches load on
+    the training thread (no_paraload): the host reads every cost back right after its step, and nothing else launches work while
+    the step is captured."""
+    from theanompi_b200.models import layers2
+    from theanompi_b200.models.alex_net import AlexNet
+    from theanompi_b200.utils.recorder import Recorder
+    layers2.reseed(); layers2.Dropout.layers.clear(); layers2.Crop.layers.clear()
+    m = AlexNet(dict(verbose=False, rank=0, size=1, device="cuda:0", batch_size=32, file_batch_size=32, cuda_graph=True,
+                     no_paraload=True, **IMNET))
+    m.compile_iter_fns("avg")
+    rec = Recorder(None, 10 ** 6, "AlexNet", False, device="cuda:0")
+    seen = []
+    for i in range(6):
+        m.train_iter(i, rec)
+        seen.append(float(rec.train_info["cost"][-1]))
+    kept = [float(c) for c in rec.train_info["cost"]]
+    m.cleanup()
+    assert len(set(seen[2:])) > 1, seen                  # the replays' costs differ, so a shared output tensor would show
+    assert kept == seen, (kept, seen)
+    assert m.captured_steps() == {"step"}
+
+
 def test_googlenet():
     _run("theanompi_b200.models.googlenet", "GoogLeNet", dict(batch_size=8, file_batch_size=16, **IMNET), steps=3)
 

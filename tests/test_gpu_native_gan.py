@@ -75,7 +75,7 @@ def test_native_gan_graph_and_eager_agree_and_launch_native_kernels(modelfile, m
     _steps(ms[0], 2)
     _steps(ms[1], 3)
     torch.cuda.synchronize()
-    assert set(ms[1]._graphs) == {"critic", "gen"} and all(s["graph"] is not None for s in ms[1]._graphs.values())
+    assert ms[1].captured_steps() == {"critic", "gen"}
     # bias / BN gradient sums use atomics, whose order differs between runs (see the test above): 0.987 was measured for LSGAN
     assert _cos(ms[0].arena.W - w0, ms[1].arena.W - w0) > 0.95
     assert _cos(ms[0].gen_arena.W, ms[1].gen_arena.W) > 0.9999

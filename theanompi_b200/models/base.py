@@ -63,6 +63,7 @@ class ModelBase(object):
     monitor_grad = False
     bias_lr_mult = 2.0             # biases train with 2x lr in the reference's optimizer (lib/opt.py:181-268)
     graph_safe = True              # False: the step draws host-side randomness / has host control flow → never auto-capture
+    supports_grad_clip = True      # config['grad_clip'] (False: the model's step has no clipping pass; refused at compile_iter_fns)
     supports_grad_accum = True     # config['grad_accum'] > 1 (False: the model refuses it at compile_iter_fns)
     supports_lr_schedule = True    # config['lr_schedule'] (False: the model refuses it at compile_iter_fns)
     supports_label_smoothing = True    # config['label_smoothing'] > 0 (False: no classifier head; refused at compile_iter_fns)
@@ -139,10 +140,7 @@ class ModelBase(object):
         self.compiled_train_fn_list = []
         self.train_iter_fn = None
         self.val_iter_fn = None
-        self._graph = None
-        self._graph_out = None
         self._gstream = None
-        self._warm = 0
         self._tail = None
         self._graphs = {}              # keyed step graphs (run_keyed_step)
         self._graph_pool = None
@@ -244,52 +242,21 @@ class ModelBase(object):
         if self.grad_accum > 1:
             return self._micro_step()
         self.n_updates += 1
-        if not self.use_graph:
-            return self._step_body()
-        if self._graph is None:
-            if self._gstream is None:
-                self._gstream = torch.cuda.Stream(device=self.device)
-            if self._warm < 2:
-                # Eager warm-up ON THE CAPTURE STREAM: autograd caches each leaf's AccumulateGrad node together
-                # with the stream that was current when it was first built; if that were the default stream the
-                # engine would make the capturing stream wait on uncaptured work at the end of backward
-                # (cudaErrorStreamCaptureIsolation).
-                self._warm += 1
-                cur = torch.cuda.current_stream(self.device)
-                self._gstream.wait_stream(cur)
-                with torch.cuda.stream(self._gstream):
-                    out = self._step_body()
-                cur.wait_stream(self._gstream)
-                return out
-            ok, why = True, ""
-            try:
-                self._capture()
-            except Exception as e:  # noqa: BLE001
-                if not self._graph_auto:
-                    raise
-                ok, why = False, "%s: %s" % (type(e).__name__, str(e)[:200])
-            ex = self.exchanger
-            if ex is not None and getattr(ex, "fused", False) and getattr(ex, "size", 1) > 1:
-                # the fused exchange pairs device-side barriers by launch order: either every rank replays the graph or
-                # every rank runs eager — agree on it (a capture that failed on one rank only would desynchronise them)
-                ok = all(ex.comm.allgather(bool(ok)))
-            if not ok:
-                print("[%s] CUDA-graph capture of the training step failed (%s) — running eager"
-                      % (getattr(self, "name", type(self).__name__), why or "on another rank"))
-                self.use_graph = False
-                self._graph = None
-                if ex is not None and hasattr(ex, "_reset_pending") and getattr(ex, "fused", False):
-                    ex._reset_pending()          # a half-captured step consumed some grad-ready callbacks
-                torch.cuda.synchronize()
-                return self._step_body()
-        self._graph.replay()
-        return self._graph_out
+        return self.run_keyed_step("step", self._step_body)
 
-    def _step_body(self):
-        self._schedule_lr()
-        out = self._fwd_bwd_eager()
-        self._dbg_capture("forward+backward")
-        if self._tail is not None:
+    def _step_body(self, kind="step"):
+        """Forward + backward of a whole training step (``kind`` 'step') or of a ``grad_accum`` micro-step ('first', 'mid' or
+        'last').  The micro kinds run under the accumulate switch (ops.accum): G is stored by 'first' and added to by 'mid' /
+        'last', the loss gradient carries 1/n.  The step tail runs after 'step' and 'last'."""
+        if kind in ("step", "first"):
+            self._schedule_lr()                  # every micro-step of a window trains with the lr of its update
+        if kind == "step":
+            out = self._fwd_bwd_eager()
+        else:
+            with ops.accum.mode(kind != "first", float(np.float32(1.0 / self.grad_accum))):
+                out = self._fwd_bwd_eager()
+        self._dbg_capture("forward+backward (%s)" % kind)
+        if kind in ("step", "last") and self._tail is not None:
             with torch.no_grad():
                 self._tail()
             self._dbg_capture("step tail")
@@ -305,46 +272,14 @@ class ModelBase(object):
         return "last" if self._micro == self.grad_accum - 1 else "mid"
 
     def _micro_step(self):
-        """One micro-step on the input buffers: with graphs, a replay of the CUDA graph captured for its kind (the three kinds share
-        one graph pool); a capture that fails under ``cuda_graph='auto'`` falls back to eager steps."""
+        """One micro-step on the input buffers, with graphs a replay of the CUDA graph captured for its kind."""
         kind = self.micro_step_kind()
-        out = None
-        if self.use_graph:
-            try:
-                out = self.run_keyed_step(("grad_accum", kind), lambda: self._accum_body(kind))
-            except Exception as e:  # noqa: BLE001
-                if not self._graph_auto:
-                    raise
-                print("[%s] CUDA-graph capture of the %s micro-step failed (%s: %s) — running eager"
-                      % (getattr(self, "name", type(self).__name__), kind, type(e).__name__, str(e)[:200]))
-                self.use_graph = False
-                self._drop_accum_graphs()
-                torch.cuda.synchronize()
-        if out is None:
-            out = self._accum_body(kind)
+        out = self.run_keyed_step(kind, lambda: self._step_body(kind))
         self._micro += 1
         if kind == "last":
             self._micro = 0
             self.n_updates += 1
         return out
-
-    def _accum_body(self, kind):
-        """Forward + backward of one micro-step under the accumulate switch (ops.accum): G is stored by 'first' and added to by
-        'mid' / 'last', the loss gradient carries 1/n; the step tail runs after 'last' only."""
-        if kind == "first":
-            self._schedule_lr()                  # every micro-step of a window trains with the lr of its update
-        with ops.accum.mode(kind != "first", float(np.float32(1.0 / self.grad_accum))):
-            out = self._fwd_bwd_eager()
-        self._dbg_capture("forward+backward (%s micro-step)" % kind)
-        if kind == "last" and self._tail is not None:
-            with torch.no_grad():
-                self._tail()
-            self._dbg_capture("step tail")
-        self._after_step()
-        return out
-
-    def _drop_accum_graphs(self):
-        self._graphs = {k: v for k, v in self._graphs.items() if not (isinstance(k, tuple) and k[0] == "grad_accum")}
 
     def check_grad_accum(self, fused_tail=None):
         """Refuse ``grad_accum`` > 1 where it is not implemented: models without it (the LSTM, the GANs, the torch twins), more than
@@ -491,69 +426,86 @@ class ModelBase(object):
         else:
             ops.advance_rng_step()
 
-    def _capture(self):
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        s = self._gstream
-        s.wait_stream(torch.cuda.current_stream())
-        inner = None
-        try:
-            with torch.cuda.stream(s):
-                with torch.cuda.graph(g, stream=s, capture_error_mode="thread_local"):
-                    try:
-                        out = self._step_body()
-                    except BaseException as e:       # capture_end would mask it with "invalidated"
-                        inner = e
-                        raise
-        except Exception:
-            if inner is not None:
-                raise inner
-            raise
-        torch.cuda.current_stream().wait_stream(s)
-        self._graph, self._graph_out = g, out
-
     def run_keyed_step(self, key, body):
         """Run ``body()`` — a whole training step that reads only static buffers — as a replay of the CUDA graph captured for
         ``key`` (any hashable: a step kind, a sequence-length bucket, ...).  Without graphs (CPU, ``cuda_graph=False``) ``body`` runs
-        eagerly.  Per key: two eager warm-up runs on the capture stream (the protocol of :meth:`forward_backward`), then the
-        capture, then replays.  All keys share one capture stream and one graph memory pool: their graphs never replay
-        concurrently.  A replay overwrites the previous outputs, so the returned tensors are copies."""
+        eagerly.  Per key: two eager warm-up runs on the capture stream, then the capture, then replays.  All keys share one
+        capture stream and one graph memory pool: only one graph of a model replays at a time.  A replay overwrites the graph's
+        outputs (a tensor or a tuple of scalars), so it returns copies, made by one launch.
+
+        Under ``cuda_graph='auto'`` a capture that fails turns graphs off for every key, and the step runs eagerly.  With a fused
+        exchange on more than one rank the ranks agree on it first, so that either all of them replay or all run eagerly."""
         if not self.use_graph:
             return body()
         if self._gstream is None:
             self._gstream = torch.cuda.Stream(device=self.device)
-        st = self._graphs.get(key)
-        if st is None:
-            st = self._graphs[key] = {"warm": 0, "graph": None, "out": None}
+            self._graph_pool = torch.cuda.graph_pool_handle()
+        st = self._graphs.setdefault(key, {"warm": 0, "graph": None, "out": None})
         if st["graph"] is None:
             s, cur = self._gstream, torch.cuda.current_stream(self.device)
             s.wait_stream(cur)
             if st["warm"] < 2:
+                # Eager warm-up ON THE CAPTURE STREAM: autograd caches each leaf's AccumulateGrad node together
+                # with the stream that was current when it was first built; if that were the default stream the
+                # engine would make the capturing stream wait on uncaptured work at the end of backward
+                # (cudaErrorStreamCaptureIsolation).
                 st["warm"] += 1
                 with torch.cuda.stream(s):
                     out = body()
                 cur.wait_stream(s)
                 return out
-            if self._graph_pool is None:
-                self._graph_pool = torch.cuda.graph_pool_handle()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.stream(s):
-                with torch.cuda.graph(g, pool=self._graph_pool, stream=s, capture_error_mode="thread_local"):
-                    out = body()
+            g, inner, why = torch.cuda.CUDAGraph(), None, ""
+            try:
+                with torch.cuda.stream(s), torch.cuda.graph(g, pool=self._graph_pool, stream=s, capture_error_mode="thread_local"):
+                    try:
+                        out = body()
+                    except BaseException as e:       # capture_end would mask it with "invalidated"
+                        inner = e
+                        raise
+            except Exception as e:  # noqa: BLE001
+                err = e if inner is None else inner
+                if not self._graph_auto or not isinstance(err, Exception):
+                    raise err
+                why = "%s: %s" % (type(err).__name__, str(err)[:200])
             cur.wait_stream(s)
+            ex = self.exchanger
+            fused = ex is not None and getattr(ex, "fused", False)
+            ok = not why
+            if fused and getattr(ex, "size", 1) > 1:
+                # the fused exchange pairs device-side barriers by launch order: either every rank replays the graph or
+                # every rank runs eager — agree on it (a capture that failed on one rank only would desynchronise them)
+                ok = all(ex.comm.allgather(ok))
+            if not ok:
+                print("[%s] CUDA-graph capture of the %r step failed (%s) — running eager" % (self.name, key, why or "on another rank"))
+                self.use_graph = False
+                self._graphs = {}
+                if fused and hasattr(ex, "_reset_pending"):
+                    ex._reset_pending()          # a half-captured step consumed some grad-ready callbacks
+                torch.cuda.synchronize()
+                return body()
             st["graph"], st["out"] = g, out
         st["graph"].replay()
         out = st["out"]
-        return tuple(t.clone() for t in out) if isinstance(out, tuple) else out.clone()
+        return torch.stack(out).unbind() if isinstance(out, tuple) else out.clone()
+
+    def captured_steps(self):
+        """The keys of :meth:`run_keyed_step` that replay a captured CUDA graph: 'step' (a training step), a micro-step kind, an
+        LSTM bucket length, ..."""
+        return {k for k, st in self._graphs.items() if st["graph"] is not None}
+
+    @property
+    def _graph(self):
+        """The captured graph of the training step (key 'step'), or None; read-only, for code that inspected it before
+        :meth:`captured_steps`."""
+        st = self._graphs.get("step")
+        return None if st is None else st["graph"]
 
     def set_step_tail(self, fn):
         """Register work that runs right after backward as part of the step — and
         therefore *inside* the captured CUDA graph: the local fused SGD (k = 1) or the
         fused allreduce+SGD exchange kernels (k > 1)."""
         self._tail = fn
-        self._graph = None
-        self._warm = 0
-        self._drop_accum_graphs()
+        self._graphs = {}
 
     def compile_val(self):
         def val_fn(subb_ind=0):
@@ -591,17 +543,8 @@ class ModelBase(object):
         (see :meth:`check_grad_clip`)."""
         if self.optimizer not in ("sgd", "lars", "lamb"):
             raise ValueError("%s: optimizer must be 'lamb', 'sgd' or 'lars', not %r" % (self.name, self.optimizer))
-        self.check_grad_accum(fused_tail)
-        self.check_label_smoothing()
-        self.check_mixup()
-        self.check_drop_path()
-        self.setup_lr_schedule()
         k = self.size if sync_type == "cdd" else 1
-        if self.optimizer in ("lars", "lamb") and fused_tail is not None:
-            raise ValueError("optimizer=%r needs every tensor's whole reduced gradient before its update; the fused exchange "
-                             "strategies (fused*, oneshot*, twoshot*, nvls*, fused_rs) update bucket slices as they are reduced. "
-                             "Use a split strategy: ar, nccl32, nccl16, asa32, asa16 or p2p32" % self.optimizer)
-        self.check_grad_clip(k, fused_tail)
+        self.setup_train_options(k, fused_tail)
         start = time.time()
         self.sync_type = sync_type
         if k > 1 and fused_tail is None:
@@ -610,6 +553,23 @@ class ModelBase(object):
         if self.verbose:
             print("Compile time: %.3f s" % (time.time() - start))
 
+    def setup_train_options(self, k=1, fused_tail=None, optimizer=None):
+        """Check and build the training options of the config for a step of ``k`` workers (k > 1: BSP ``sync_type='cdd'``),
+        ``fused_tail`` (a fused exchange strategy's step tail, or None) and ``optimizer`` (default: the model's): grad_accum,
+        label_smoothing, mixup, drop_path_rate, lr_schedule and grad_clip.  A model refuses every option it does not support here,
+        with a ValueError that names it."""
+        self.check_grad_accum(fused_tail)
+        self.check_label_smoothing()
+        self.check_mixup()
+        self.check_drop_path()
+        self.setup_lr_schedule()
+        opt = self.optimizer if optimizer is None else optimizer
+        if opt in ("lars", "lamb") and fused_tail is not None:
+            raise ValueError("optimizer=%r needs every tensor's whole reduced gradient before its update; the fused exchange "
+                             "strategies (fused*, oneshot*, twoshot*, nvls*, fused_rs) update bucket slices as they are reduced. "
+                             "Use a split strategy: ar, nccl32, nccl16, asa32, asa16 or p2p32" % opt)
+        self.check_grad_clip(k, fused_tail, opt)
+
     def check_grad_clip(self, k=1, fused_tail=None, optimizer=None):
         """Refuse ``grad_clip`` where the native step cannot clip by the global norm: with ``optimizer`` (default: the model's)
         'lars' or 'lamb', whose trust ratios already normalise every tensor's step, and on any step that is not a local k = 1
@@ -617,6 +577,9 @@ class ModelBase(object):
         the norm of the reduced gradient before any slice is updated."""
         if self.grad_clip is None:
             return
+        if not self.supports_grad_clip:
+            raise ValueError("%s: grad_clip is not supported by the torch twins; it runs on the native models (AlexNet, GoogLeNet, "
+                             "Cifar10_model, VGG16, ResNet50, Wide_ResNet, LSTM, NativeWGAN, NativeLSGAN)" % self.name)
         supported = ("grad_clip runs on the local k = 1 steps of the sgd, adam, rmsprop, adadelta and rmsprop_centered flat "
                      "optimizers: one worker, BSP sync_type='avg' with a split strategy, EASGD, ASGD or GOSGD")
         if not self.grad_clip > 0:

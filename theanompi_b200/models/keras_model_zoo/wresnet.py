@@ -157,12 +157,7 @@ class Wide_ResNet(ModelBase):
             return super().compile_iter_fns(sync_type, aggregate, fused_tail)
         if sync_type != "avg" and self.size > 1:
             raise ValueError("Wide_ResNet trains with Adam: only sync_type='avg' is supported (as in the reference, wresnet.py:152-153)")
-        self.check_grad_clip(optimizer="adam")
-        self.check_grad_accum(fused_tail)
-        self.check_label_smoothing()
-        self.check_mixup()
-        self.check_drop_path()
-        self.setup_lr_schedule()
+        self.setup_train_options(fused_tail=fused_tail, optimizer="adam")
         from ...utils.opt import FlatAdam
         self.sync_type = "avg"
         self.adam = FlatAdam(self.arena)

@@ -98,12 +98,7 @@ class WGAN(TorchModelBase):
         return 0.5 * ((self.critic(fake) - 1) ** 2).mean()
 
     def compile_iter_fns(self, sync_type="avg", **kw):
-        self.refuse_grad_clip()
-        self.check_grad_accum()
-        self.check_label_smoothing()
-        self.check_mixup()
-        self.check_drop_path()
-        self.setup_lr_schedule()
+        self.setup_train_options()
         self.sync_type = "avg"
         self.opt_c = torch.optim.RMSprop(self.critic_params, lr=self.learning_rate)
         self.opt_g = torch.optim.RMSprop(self.generator_params, lr=self.learning_rate)
@@ -398,11 +393,7 @@ class NativeWGAN(ModelBase):
 
     # ---- contract
     def compile_iter_fns(self, sync_type="avg", **kw):
-        self.check_grad_accum()
-        self.check_label_smoothing()
-        self.check_mixup()
-        self.check_drop_path()
-        self.setup_lr_schedule()
+        self.setup_train_options(optimizer="rmsprop")
         self.sync_type = "avg"
         self.vels, self.vels2 = [], []
         self.train_iter_fn = self.val_iter_fn = None

@@ -184,12 +184,7 @@ class LSTM(ModelBase):
         return self.opt
 
     def compile_iter_fns(self, sync_type="avg", **kw):
-        self.check_grad_clip()
-        self.check_grad_accum()
-        self.check_label_smoothing()
-        self.check_mixup()
-        self.check_drop_path()
-        self.setup_lr_schedule()
+        self.setup_train_options()
         self.sync_type = "avg"
         self._make_opt()
         self.vels, self.vels2 = [], []
@@ -330,12 +325,7 @@ class LSTMTorch(TorchModelBase):
         return torch.optim.Adadelta(params, lr=1.0, rho=0.95, eps=1e-6)
 
     def compile_iter_fns(self, sync_type="avg", **kw):
-        self.refuse_grad_clip()
-        self.check_grad_accum()
-        self.check_label_smoothing()
-        self.check_mixup()
-        self.check_drop_path()
-        self.setup_lr_schedule()
+        self.setup_train_options()
         self.sync_type = "avg"
         self.torch_opt = self.make_torch_optimizer(self.params)
         self.vels, self.vels2 = [], []

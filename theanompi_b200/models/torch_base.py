@@ -44,6 +44,7 @@ class TorchModelBase(ModelBase):
     supports_grad_accum = False    # torch autograd writes .grad: the native accumulate mode does not reach it
     supports_lr_schedule = False   # the library yardsticks keep the per-epoch lr policies
     supports_mixup = False         # the library yardsticks train on the plain batch
+    supports_grad_clip = False     # torch.optim or the flat SGD without a clipping pass: refused rather than trained unclipped
 
     def finalize_torch(self, module, input_shape, exchanged=None):
         self.module = module.to(self.device)
@@ -102,23 +103,11 @@ class TorchModelBase(ModelBase):
             return c, e, e5
         self.val_fn = val_fn
 
-    def refuse_grad_clip(self):
-        """The torch twins step through ``torch.optim`` or their own flat SGD without a clipping pass: refuse ``grad_clip`` rather than
-        train unclipped."""
-        if self.grad_clip is not None:
-            raise ValueError("%s: grad_clip is not supported by the torch twins; it runs on the native models (AlexNet, GoogLeNet, "
-                             "Cifar10_model, VGG16, ResNet50, Wide_ResNet, LSTM, NativeWGAN, NativeLSGAN)" % self.name)
-
     def compile_iter_fns(self, sync_type="avg", aggregate="momentum", fused_tail=None):
-        self.refuse_grad_clip()
-        self.check_grad_accum(fused_tail)
-        self.check_label_smoothing()
-        self.check_mixup()
-        self.check_drop_path()
-        self.setup_lr_schedule()
         self.torch_opt = self.make_torch_optimizer(self.params)
         if self.torch_opt is None:
             return super().compile_iter_fns(sync_type, aggregate, fused_tail)
+        self.setup_train_options(fused_tail=fused_tail)
         if sync_type != "avg" and self.size > 1:
             raise ValueError("%s has a self-contained torch optimizer: only sync_type='avg' is supported "
                              "(as in the reference, wresnet.py:152-153)" % self.name)
