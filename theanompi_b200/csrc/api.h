@@ -164,6 +164,13 @@ void crop_mirror_norm(const void* x, int in_kind, const void* mean, int mean_mod
 // aligned, inside the H × W image) to ch × cw, mirrored after the resize where flips[n]; out bf16 (out_bf16) or fp32 NHWC
 void resized_crop_mirror_norm(const void* x, const void* mean, int mean_mode, float scale, const void* cscale, void* out, int out_bf16,
                               const void* boxes, const void* flips, int N, int H, int W, int C, int ch, int cw, cudaStream_t st);
+// colour jitter + lighting on top of the resized crop (C = 3): out = (M·v̂ + K·μ + ℓ − m̂)·s_c, v̂ / m̂ the bilinear resample of the raw
+// box / of the mean; rec = fp32 [N, 24] (M, K, ℓ, 0; 16-byte aligned), mu = fp32 [N, 4] from crop_mean, or null when K ≡ 0
+void color_crop_mirror_norm(const void* x, const void* mean, int mean_mode, float scale, const void* cscale, void* out, int out_bf16,
+                            const void* boxes, const void* flips, const void* rec, const void* mu, int N, int H, int W, int ch, int cw,
+                            cudaStream_t st);
+// mu[n] = mean RGB (fp32 [N, 4], last lane 0) of the ch × cw bilinear resample of the raw uint8 box n (x: [N, H, W, 3])
+void crop_mean(const void* x, const void* boxes, void* mu, int N, int H, int W, int ch, int cw, cudaStream_t st);
 
 // ---- bn_kernels.cu: batch norm (+ residual)(+ ReLU) forward / backward, residual add  (f32: fp32 activations, else bf16)
 // drop_scale (optional, null = off): one row of the step's drop-path table, a float per sample of the `batch` samples (rows

@@ -138,6 +138,12 @@ PYBIND11_MODULE(_tmpi_native, m) {
   m.def("resized_crop_mirror_norm", [](ptr_t x, ptr_t mean, int mean_mode, float scale, ptr_t cscale, ptr_t out, int out_bf16, ptr_t boxes,
                                        ptr_t flips, int N, int H, int W, int C, int ch, int cw, ptr_t st) {
     resized_crop_mirror_norm(P(x), P(mean), mean_mode, scale, P(cscale), P(out), out_bf16, P(boxes), P(flips), N, H, W, C, ch, cw, S(st)); });
+  m.def("color_crop_mirror_norm", [](ptr_t x, ptr_t mean, int mean_mode, float scale, ptr_t cscale, ptr_t out, int out_bf16, ptr_t boxes,
+                                     ptr_t flips, ptr_t rec, ptr_t mu, int N, int H, int W, int ch, int cw, ptr_t st) {
+    color_crop_mirror_norm(P(x), P(mean), mean_mode, scale, P(cscale), P(out), out_bf16, P(boxes), P(flips), P(rec), P(mu), N, H, W, ch, cw,
+                           S(st)); });
+  m.def("crop_mean", [](ptr_t x, ptr_t boxes, ptr_t mu, int N, int H, int W, int ch, int cw, ptr_t st) {
+    crop_mean(P(x), P(boxes), P(mu), N, H, W, ch, cw, S(st)); });
 
   // ---------------------------------------------------------------- batch norm / residual
   m.def("bn_forward", [](ptr_t x, ptr_t res, ptr_t y, ptr_t gamma, ptr_t beta, ptr_t mean, ptr_t rstd, ptr_t run_mean, ptr_t run_var, ptr_t scratch,

@@ -1589,11 +1589,15 @@ __device__ __forceinline__ void rrc_axis(int o, float ratio, int L, int& i0, int
   lam = fminf(fmaxf(s - (float)i0, 0.f), 1.f);
 }
 
-template <typename Tout>
+// JITTER (colour jitter + lighting, C == 3): image n's 96-byte record rec[n] = (M, K, ℓ, 0) and its crop mean mu[n] (float4, null when
+// K ≡ 0) map the bilinear resample v̂ of the raw box to M·v̂ + K·μ + ℓ, which is then normalised with the same resample m̂ of the mean:
+// out = (M·v̂ + t − m̂)·s_c, t = K·μ + ℓ formed once per thread from CTA-uniform loads.  A box of the output's size (λ = 0) gives
+// v̂ = x and m̂ = m exactly, so the identity record reproduces crop_mirror_norm_kernel bit for bit.
+template <typename Tout, bool JITTER = false>
 __global__ void __launch_bounds__(128) resized_crop_mirror_norm_kernel(const uint8_t* __restrict__ x, const float* __restrict__ mean,
                                         int mean_mode, float scale, const float* __restrict__ cscale, Tout* __restrict__ out,
                                         const int4* __restrict__ boxes, const uint8_t* __restrict__ flips, int H, int W, int C, int ch,
-                                        int cw) {
+                                        int cw, const float4* __restrict__ rec = nullptr, const float4* __restrict__ mu = nullptr) {
   const int ox = blockIdx.y * blockDim.x + threadIdx.x;
   if (ox >= cw) return;
   const int oy = blockIdx.x % ch, n = blockIdx.x / ch;
@@ -1609,6 +1613,32 @@ __global__ void __launch_bounds__(128) resized_crop_mirror_norm_kernel(const uin
   const uint8_t* src = x + (long long)n * H * W * C;
   const float wy0 = 1.f - ly, wx0 = 1.f - lx;
   Tout* o = out + ((long long)blockIdx.x * cw + ox) * C;
+  if constexpr (JITTER) {
+    const float4* r = rec + 6 * n;
+    const float4 r0 = r[0], r1 = r[1], r2 = r[2], r3 = r[3], r4 = r[4], r5 = r[5];
+    // floats 0-8 M row-major (m00 m01 m02 m10 | m11 m12 m20 m21 | m22), 9-17 K the same way (k00 at r2.y), 18-20 ℓ (r4.z, r4.w, r5.x)
+    float t0 = r4.z, t1 = r4.w, t2 = r5.x;
+    if (mu) {
+      const float4 u = mu[n];
+      t0 = __fmaf_rn(r2.y, u.x, __fmaf_rn(r2.z, u.y, __fmaf_rn(r2.w, u.z, t0)));
+      t1 = __fmaf_rn(r3.x, u.x, __fmaf_rn(r3.y, u.y, __fmaf_rn(r3.z, u.z, t1)));
+      t2 = __fmaf_rn(r3.w, u.x, __fmaf_rn(r4.x, u.y, __fmaf_rn(r4.y, u.z, t2)));
+    }
+    auto bilerp = [&](const uint8_t* p, int c) {
+      return wy0 * (wx0 * (float)p[t00 + c] + lx * (float)p[t01 + c]) + ly * (wx0 * (float)p[t10 + c] + lx * (float)p[t11 + c]);
+    };
+    auto mhat = [&](int c) {
+      if (mean_mode != 2) return mean_mode == 0 ? mean[0] : mean[c];
+      return wy0 * (wx0 * mean[t00 + c] + lx * mean[t01 + c]) + ly * (wx0 * mean[t10 + c] + lx * mean[t11 + c]);
+    };
+    const float v0 = bilerp(src, 0), v1 = bilerp(src, 1), v2 = bilerp(src, 2);
+    const float a0 = __fmaf_rn(r0.x, v0, __fmaf_rn(r0.y, v1, __fmaf_rn(r0.z, v2, t0)));
+    const float a1 = __fmaf_rn(r0.w, v0, __fmaf_rn(r1.x, v1, __fmaf_rn(r1.y, v2, t1)));
+    const float a2 = __fmaf_rn(r1.z, v0, __fmaf_rn(r1.w, v1, __fmaf_rn(r2.x, v2, t2)));
+    const float s0 = cscale ? scale * cscale[0] : scale, s1 = cscale ? scale * cscale[1] : scale, s2 = cscale ? scale * cscale[2] : scale;
+    o[0] = (Tout)((a0 - mhat(0)) * s0); o[1] = (Tout)((a1 - mhat(1)) * s1); o[2] = (Tout)((a2 - mhat(2)) * s2);
+    return;
+  }
   auto tap = [&](unsigned t, int c, float s) {
     const float m = mean_mode == 0 ? mean[0] : (mean_mode == 1 ? mean[c] : mean[t + c]);
     return ((float)src[t + c] - m) * s;
@@ -1634,6 +1664,75 @@ void resized_crop_mirror_norm(const void* x, const void* mean, int mean_mode, fl
   if (out_bf16) resized_crop_mirror_norm_kernel<__nv_bfloat16><<<g, 128, 0, st>>>(X, M, mean_mode, scale, CS, (__nv_bfloat16*)out, B, F, H, W, C, ch, cw);
   else resized_crop_mirror_norm_kernel<float><<<g, 128, 0, st>>>(X, M, mean_mode, scale, CS, (float*)out, B, F, H, W, C, ch, cw);
   count_launch(); TMPI_CHECK_LAUNCH("resized_crop_mirror_norm"); ::tmpi::check_capture(st, "resized_crop_mirror_norm");
+}
+
+void color_crop_mirror_norm(const void* x, const void* mean, int mean_mode, float scale, const void* cscale, void* out, int out_bf16,
+                            const void* boxes, const void* flips, const void* rec, const void* mu, int N, int H, int W, int ch, int cw,
+                            cudaStream_t st) {
+  if ((long long)H * W * 3 >= (1LL << 31) || (long long)N * ch >= (1LL << 31)) throw std::runtime_error("color_crop_mirror_norm: image too large");
+  const dim3 g((unsigned)(N * ch), (unsigned)((cw + 127) / 128));
+  auto X = (const uint8_t*)x; auto M = (const float*)mean; auto CS = (const float*)cscale;
+  auto B = (const int4*)boxes; auto F = (const uint8_t*)flips; auto R = (const float4*)rec; auto U = (const float4*)mu;
+  if (out_bf16) resized_crop_mirror_norm_kernel<__nv_bfloat16, true><<<g, 128, 0, st>>>(X, M, mean_mode, scale, CS, (__nv_bfloat16*)out, B, F, H, W, 3, ch, cw, R, U);
+  else resized_crop_mirror_norm_kernel<float, true><<<g, 128, 0, st>>>(X, M, mean_mode, scale, CS, (float*)out, B, F, H, W, 3, ch, cw, R, U);
+  count_launch(); TMPI_CHECK_LAUNCH("color_crop_mirror_norm"); ::tmpi::check_capture(st, "color_crop_mirror_norm");
+}
+
+// ============================================================================ loader: mean RGB of each output crop (colour jitter's μ)
+// mu[n] = (Σ v̂) / (ch·cw) over the ch × cw output pixels of box n, v̂ the bilinear value of the raw uint8 box from the same rrc_axis
+// taps and the same arithmetic as the resize (the mirror does not change a sum).  One CTA per image, one warp per output row
+// (rows warp, warp + 16, ...), lanes stride the row; per-thread sums in a fixed order, then a shuffle tree and a tree over the 16
+// warps: no atomics, the same bits on every run.  A box of the output's size sums integers below 2^24 (256² · 255), exact in fp32.
+constexpr int CROP_MEAN_THREADS = 512;
+
+__global__ void __launch_bounds__(CROP_MEAN_THREADS) crop_mean_kernel(const uint8_t* __restrict__ x, const int4* __restrict__ boxes,
+                                                                      float4* __restrict__ mu, int H, int W, int ch, int cw) {
+  const int n = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int4 b = boxes[n];
+  const uint8_t* src = x + (long long)n * H * W * 3;
+  const float ry = __fdiv_rn((float)b.z, (float)ch), rx = __fdiv_rn((float)b.w, (float)cw);
+  float s0 = 0.f, s1 = 0.f, s2 = 0.f;
+  for (int oy = warp; oy < ch; oy += CROP_MEAN_THREADS / 32) {
+    int iy0, iy1;
+    float ly;
+    rrc_axis(oy, ry, b.z, iy0, iy1, ly);
+    const unsigned r0 = (unsigned)((b.x + iy0) * W + b.y) * 3u, r1 = (unsigned)((b.x + iy1) * W + b.y) * 3u;
+    const float wy0 = 1.f - ly;
+    for (int ox = lane; ox < cw; ox += 32) {
+      int ix0, ix1;
+      float lx;
+      rrc_axis(ox, rx, b.w, ix0, ix1, lx);
+      const unsigned t00 = r0 + 3u * ix0, t01 = r0 + 3u * ix1, t10 = r1 + 3u * ix0, t11 = r1 + 3u * ix1;
+      const float wx0 = 1.f - lx;
+      auto bilerp = [&](int c) {
+        return wy0 * (wx0 * (float)src[t00 + c] + lx * (float)src[t01 + c]) + ly * (wx0 * (float)src[t10 + c] + lx * (float)src[t11 + c]);
+      };
+      s0 += bilerp(0); s1 += bilerp(1); s2 += bilerp(2);
+    }
+  }
+  for (int d = 16; d > 0; d >>= 1) {
+    s0 += __shfl_xor_sync(0xffffffffu, s0, d); s1 += __shfl_xor_sync(0xffffffffu, s1, d); s2 += __shfl_xor_sync(0xffffffffu, s2, d);
+  }
+  __shared__ float part[3][CROP_MEAN_THREADS / 32];
+  if (lane == 0) { part[0][warp] = s0; part[1][warp] = s1; part[2][warp] = s2; }
+  __syncthreads();
+  if (warp == 0) {
+    const bool live = lane < CROP_MEAN_THREADS / 32;
+    s0 = live ? part[0][lane] : 0.f; s1 = live ? part[1][lane] : 0.f; s2 = live ? part[2][lane] : 0.f;
+    for (int d = 8; d > 0; d >>= 1) {
+      s0 += __shfl_xor_sync(0xffffffffu, s0, d); s1 += __shfl_xor_sync(0xffffffffu, s1, d); s2 += __shfl_xor_sync(0xffffffffu, s2, d);
+    }
+    if (lane == 0) {
+      const float p = (float)(ch * cw);
+      mu[n] = make_float4(__fdiv_rn(s0, p), __fdiv_rn(s1, p), __fdiv_rn(s2, p), 0.f);
+    }
+  }
+}
+
+void crop_mean(const void* x, const void* boxes, void* mu, int N, int H, int W, int ch, int cw, cudaStream_t st) {
+  if ((long long)H * W * 3 >= (1LL << 31) || (long long)ch * cw >= (1LL << 24)) throw std::runtime_error("crop_mean: image too large");
+  crop_mean_kernel<<<N, CROP_MEAN_THREADS, 0, st>>>((const uint8_t*)x, (const int4*)boxes, (float4*)mu, H, W, ch, cw);
+  count_launch(); TMPI_CHECK_LAUNCH("crop_mean"); ::tmpi::check_capture(st, "crop_mean");
 }
 
 }  // namespace tmpi

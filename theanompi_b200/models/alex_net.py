@@ -76,7 +76,8 @@ class AlexNet(ModelBase):
             self.data.spawn_load()
             self.data.para_load_init(self.device, self.input_width, self.input_height,
                                      self.rand_crop, self.batch_crop_mirror, out_dtype=self.act_dtype,
-                                     resized_crop=self.resized_crop, rank=self.rank)
+                                     resized_crop=self.resized_crop, rank=self.rank,
+                                     color_jitter=self.color_jitter)
 
     def build_model(self):
         if self.verbose:

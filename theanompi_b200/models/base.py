@@ -69,7 +69,9 @@ class ModelBase(object):
     supports_label_smoothing = True    # config['label_smoothing'] > 0 (False: no classifier head; refused at compile_iter_fns)
     supports_mixup = True          # config['mixup'] (False: no image batch before a first convolution; refused at compile_iter_fns)
     supports_drop_path = False     # config['drop_path_rate'] > 0 (True: residual blocks in self.body that read drop_row(l))
-    supports_resized_crop = False  # config['random_resized_crop'] (True: ImageNet models fed by ParaLoader; refused at construction)
+    # True: an ImageNet model fed by ParaLoader, so config['random_resized_crop'] and config['color_jitter'] reach its loader
+    # (refused at construction otherwise)
+    supports_resized_crop = False
     name = "Model"
 
     def __init__(self, config):
@@ -133,6 +135,9 @@ class ModelBase(object):
         # drawn by the loader and resampled by its kernel on the copy stream.  Checked here because the model's constructor builds
         # the loader; the training step never sees it
         self.resized_crop = self.check_resized_crop(config.get("random_resized_crop"))
+        # colour jitter and PCA lighting of the training images (a dict, models/data/utils.py: check_color_jitter; None = off):
+        # per-image colour maps drawn by the loader and applied by its crop kernel; like the crop, the training step never sees it
+        self.color_jitter = self.check_color_jitter(config.get("color_jitter"))
         self.base_lr = np.float32(self.learning_rate)
         self.current_t = self.subb_t = 0
         self.current_v = self.subb_v = 0
@@ -356,6 +361,16 @@ class ModelBase(object):
         if self.batch_crop_mirror or not self.rand_crop:
             raise ValueError("%s: %s draws a random box per image, which contradicts %s" % (
                 name, RRC_KEY, "batch_crop_mirror = True" if self.batch_crop_mirror else "rand_crop = False"))
+        return cfg
+
+    def check_color_jitter(self, cfg):
+        """The validated ``config['color_jitter']`` (models/data/utils.py: check_color_jitter; a ValueError names the key), or None.
+        A dict needs a model fed by the ImageNet loader (``supports_resized_crop``); any crop mode composes with it."""
+        from .data.utils import CJ_KEY, check_color_jitter
+        cfg = check_color_jitter(cfg)
+        if cfg is not None and not self.supports_resized_crop:
+            raise ValueError("%s: %s is not supported; it augments the ImageNet loader of AlexNet, GoogLeNet, VGG16, ResNet50, "
+                             "ResNet152 and ResNet50Torch" % (type(self).__name__, CJ_KEY))
         return cfg
 
     # ------------------------------------------------------------------ stochastic depth (drop-path)

@@ -169,27 +169,42 @@ class ImageNet_data(object):
     def load_batch(self, item, mode, model):
         """Serial (no loader) path of the reference (``alex_net.py:420-438``): read, normalise,
         crop/mirror on the host, return an NHWC float tensor.  With ``model.resized_crop`` a "train" batch is the random-resized
-        crop of :meth:`para_load_init`'s loader, drawn from this object's generator keyed by (seed, ``model.rank``)."""
+        crop of :meth:`para_load_init`'s loader, drawn from this object's generator keyed by (seed, ``model.rank``).  With
+        ``model.color_jitter`` a "train" batch also gets the loader's colour maps, drawn from a generator keyed by (seed, rank, 1),
+        on the same boxes or fixed crops as without it."""
         import torch
-        from .utils import crop_and_mirror
+        from ... import ops
+        from .utils import color_jitter_records, color_jitter_rng, crop_and_mirror, draw_crops
         raw = np.empty((self.file_batch_size, self.height, self.width, self.channels), dtype=np.uint8)
         src = self.read(item, raw)
         if src is not None:
             raw = src.numpy()
         rrc = getattr(model, "resized_crop", None)
+        cj = getattr(model, "color_jitter", None) if mode == "train" else None
+        n = raw.shape[0]
+        mean, cs = torch.from_numpy(self.rawdata[4]), torch.from_numpy(1.0 / 255.0 / self.rawdata[5])
         if rrc is not None and mode == "train":
-            from ... import ops
             from .utils import draw_resized_crops, resized_crop_rng
             if getattr(self, "_rrc_rng", None) is None:
                 self._rrc_rng = resized_crop_rng(rrc, model.rank)
-            boxes, flips = draw_resized_crops(raw.shape[0], (self.height, self.width), rrc["scale"], rrc["ratio"], self._rrc_rng)
-            t = ops.reference.resized_crop_mirror_normalize(torch.from_numpy(raw), torch.from_numpy(self.rawdata[4]),
-                                                            torch.from_numpy(1.0 / 255.0 / self.rawdata[5]),
-                                                            (model.input_height, model.input_width), boxes, flips)
+            out_hw = (model.input_height, model.input_width)
+            boxes, flips = draw_resized_crops(n, (self.height, self.width), rrc["scale"], rrc["ratio"], self._rrc_rng)
+            if cj is None:
+                t = ops.reference.resized_crop_mirror_normalize(torch.from_numpy(raw), mean, cs, out_hw, boxes, flips)
+        elif cj is not None:
+            # the same RandomState draw as crop_and_mirror below, so the key changes no crop
+            out_hw = (model.input_width, model.input_width)
+            offs, flips = draw_crops(n, (self.height, self.width), out_hw, mode, model.rand_crop, model.batch_crop_mirror)
+            boxes = np.concatenate([offs, np.tile(np.int32([out_hw]), (n, 1))], 1)
         else:
             arr = (raw.astype(np.float32) - self.rawdata[4]) / 255.0 / self.rawdata[5]
             arr = crop_and_mirror(arr, mode, model.rand_crop, model.batch_crop_mirror, model.input_width)
             t = torch.from_numpy(arr)
+        if cj is not None:
+            if getattr(self, "_cj_rng", None) is None:
+                self._cj_rng = color_jitter_rng(cj, model.rank)
+            records = color_jitter_records(n, cj, self._cj_rng)[0]
+            t = ops.reference.color_crop_mirror_normalize(torch.from_numpy(raw), mean, cs, out_hw, boxes, flips, records)
         if model.cuda:
             t = t.pin_memory().to(model.device, non_blocking=True)
         return t
@@ -202,16 +217,18 @@ class ImageNet_data(object):
         return None
 
     def para_load_init(self, device, input_width, input_height, rand_crop, batch_crop_mirror,
-                       out_dtype=None, depth=2, mode=None, resized_crop=None, rank=0):
+                       out_dtype=None, depth=2, mode=None, resized_crop=None, rank=0, color_jitter=None):
         """``mode='thread'`` (default): loader thread + pinned ring in this process.  ``mode='process'`` (or
         ``TMPI_LOADER=process``): a separate loader process fills a page-locked shared-memory ring (see ``proc_loader.py``) —
         the reference's ``proc_load_mpi.py`` child, minus its second CUDA context.  ``resized_crop`` (a validated
-        ``config['random_resized_crop']``) and ``rank`` go to the :class:`ParaLoader`, which draws the boxes in this process."""
+        ``config['random_resized_crop']``), ``color_jitter`` (a validated ``config['color_jitter']``) and ``rank`` go to the
+        :class:`ParaLoader`, which draws the boxes and the colour maps in this process."""
         from .loader import ParaLoader
         raw_shape = (self.file_batch_size, self.height, self.width, self.channels)
         mode = mode or os.environ.get("TMPI_LOADER", "thread")
         kw = dict(mean=self.rawdata[4], std_scale=1.0 / 255.0 / self.rawdata[5], out_dtype=out_dtype, depth=depth,
-                  rand_crop=rand_crop, batch_crop_mirror=batch_crop_mirror, resized_crop=resized_crop, rank=rank)
+                  rand_crop=rand_crop, batch_crop_mirror=batch_crop_mirror, resized_crop=resized_crop, rank=rank,
+                  color_jitter=color_jitter)
         if mode == "process":
             from .proc_loader import ProcReader
             self.proc_reader = ProcReader(raw_shape, depth=depth, seed=self._seed)

@@ -31,25 +31,29 @@ import numpy as np
 import torch
 
 from ... import ops
-from .utils import draw_crops, draw_resized_crops, resized_crop_rng
+from .utils import (CJ_RECORD_FLOATS, color_jitter_records, color_jitter_rng, draw_crops, draw_resized_crops,
+                    resized_crop_rng)
 
 
 class LoadedBatch(object):
-    """One loaded batch; ``boxes`` / ``flips``: the host copies of the random-resized-crop draw it was made with (None otherwise)."""
-    __slots__ = ("x", "slot", "ready", "item", "h2d_bytes", "boxes", "flips")
+    """One loaded batch; ``boxes`` / ``flips``: the host copies of the random-resized-crop draw it was made with, or of the fixed
+    crops as boxes of the output's size under colour jitter (None otherwise); ``records``: the colour-jitter records (None otherwise)."""
+    __slots__ = ("x", "slot", "ready", "item", "h2d_bytes", "boxes", "flips", "records")
 
-    def __init__(self, x, slot, ready, item, h2d_bytes, boxes=None, flips=None):
+    def __init__(self, x, slot, ready, item, h2d_bytes, boxes=None, flips=None, records=None):
         self.x, self.slot, self.ready, self.item, self.h2d_bytes = x, slot, ready, item, h2d_bytes
-        self.boxes, self.flips = boxes, flips
+        self.boxes, self.flips, self.records = boxes, flips, records
 
 
 class ParaLoader(object):
     def __init__(self, read_fn, device, raw_shape, crop_hw, mean, std_scale=1.0 / 255.0,
                  out_dtype=None, depth=2, rand_crop=True, batch_crop_mirror=False, seed=1234,
-                 threaded=True, host_buffers=None, on_close=None, resized_crop=None, rank=0):
+                 threaded=True, host_buffers=None, on_close=None, resized_crop=None, rank=0, color_jitter=None):
         """``resized_crop``: a validated ``config['random_resized_crop']`` (``utils.check_resized_crop``) or None; with it every
         "train" batch is a random-resized crop drawn per image from the generator keyed by (its seed, ``rank``), and "val" batches
-        keep the centre crop."""
+        keep the centre crop.  ``color_jitter``: a validated ``config['color_jitter']`` (``utils.check_color_jitter``) or None; with
+        it every "train" image gets a colour map drawn from the generator keyed by (its seed, ``rank``, 1), applied by the crop
+        kernel on the same boxes or fixed crops as without it; "val" batches are never jittered."""
         self.read_fn = read_fn
         self.device = torch.device(device)
         self.cuda = self.device.type == "cuda"
@@ -78,12 +82,21 @@ class ParaLoader(object):
         self.host_offs = [torch.empty((N, 2), dtype=torch.int32, pin_memory=pin) for _ in range(depth)]
         self.host_flip = [torch.empty((N,), dtype=torch.uint8, pin_memory=pin) for _ in range(depth)]
         self.resized_crop = resized_crop
+        self.color_jitter = color_jitter
         if resized_crop is not None:
             self.rrc_rng = resized_crop_rng(resized_crop, rank)
+        if color_jitter is not None:
+            self.cj_rng = color_jitter_rng(color_jitter, rank)
+            self.host_rec = [torch.empty((N, CJ_RECORD_FLOATS), dtype=torch.float32, pin_memory=pin) for _ in range(depth)]
+        boxed = resized_crop is not None or color_jitter is not None
+        if boxed:
             self.host_boxes = [torch.empty((N, 4), dtype=torch.int32, pin_memory=pin) for _ in range(depth)]
         if self.cuda:
-            if resized_crop is not None:
+            if boxed:
                 self.dev_boxes = [torch.empty((N, 4), dtype=torch.int32, device=self.device) for _ in range(depth)]
+            if color_jitter is not None:
+                self.dev_rec = [torch.empty((N, CJ_RECORD_FLOATS), dtype=torch.float32, device=self.device) for _ in range(depth)]
+                self.dev_mu = [torch.empty((N, 4), dtype=torch.float32, device=self.device) for _ in range(depth)]
             self.stage = [torch.empty(self.raw_shape, dtype=torch.uint8, device=self.device) for _ in range(depth)]
             self.dev_offs = [torch.empty((N, 2), dtype=torch.int32, device=self.device) for _ in range(depth)]
             self.dev_flip = [torch.empty((N,), dtype=torch.uint8, device=self.device) for _ in range(depth)]
@@ -119,8 +132,8 @@ class ParaLoader(object):
             # the ring slot is refilled by another process as soon as we request the next file: the DMA out of it must have
             # finished before this slot comes round again — recorded below, awaited at the top of the next _produce(s)
             pass
-        if self.resized_crop is not None and mode == "train":
-            return self._produce_resized(s, src, item)
+        if mode == "train" and (self.resized_crop is not None or self.color_jitter is not None):
+            return self._produce_boxed(s, src, item, mode)
         offs, flips = draw_crops(N, (H, W), self.crop_hw, mode, self.rand_crop, self.batch_crop_mirror, self.rs)
         self.host_offs[s].numpy()[...] = offs
         self.host_flip[s].numpy()[...] = flips
@@ -142,30 +155,54 @@ class ParaLoader(object):
             ready = None
         return LoadedBatch(self.out[s], s, ready, item, self.h2d_bytes)
 
-    def _produce_resized(self, s, src, item):
-        """A "train" batch with ``resized_crop``: boxes and flips drawn on the host, the 16-byte box record copied next to the flips
-        and ``resized_crop_mirror_norm`` launched on the copy stream (the reference on the CPU)."""
+    def _produce_boxed(self, s, src, item, mode):
+        """A "train" batch with ``resized_crop`` or ``color_jitter``: boxes (the random-resized-crop draw, or the fixed crops'
+        offsets with the output's size) and flips drawn on the host, the 16-byte box record copied next to the flips, and the
+        96-byte colour record with them under ``color_jitter``; then on the copy stream ``resized_crop_mirror_norm``, or
+        ``crop_mean`` (only when the contrast strength is > 0, since otherwise K ≡ 0) and ``color_crop_mirror_norm`` (the
+        references on the CPU)."""
         N, H, W, C = self.raw_shape
-        boxes, flips = draw_resized_crops(N, (H, W), self.resized_crop["scale"], self.resized_crop["ratio"], self.rrc_rng)
+        if self.resized_crop is not None:
+            boxes, flips = draw_resized_crops(N, (H, W), self.resized_crop["scale"], self.resized_crop["ratio"], self.rrc_rng)
+        else:
+            offs, flips = draw_crops(N, (H, W), self.crop_hw, mode, self.rand_crop, self.batch_crop_mirror, self.rs)
+            boxes = np.concatenate([offs, np.tile(np.int32([self.crop_hw]), (N, 1))], 1)
         self.host_boxes[s].numpy()[...] = boxes
         self.host_flip[s].numpy()[...] = flips
         nbytes = int(np.prod(self.raw_shape)) + N * 17
+        records = None
+        if self.color_jitter is not None:
+            records = color_jitter_records(N, self.color_jitter, self.cj_rng)[0]
+            self.host_rec[s].numpy()[...] = records
+            nbytes += N * 4 * CJ_RECORD_FLOATS
         if self.cuda:
             with torch.cuda.stream(self.copy_stream):
                 self.stage[s].copy_(src, non_blocking=True)
                 self.dev_boxes[s].copy_(self.host_boxes[s], non_blocking=True)
                 self.dev_flip[s].copy_(self.host_flip[s], non_blocking=True)
                 from ...ops import cuda_impl
-                cuda_impl.resized_crop_mirror_normalize(self.stage[s], self.mean, self.std_scale, self.crop_hw, self.dev_boxes[s],
-                                                        self.dev_flip[s], self.out_dtype, out=self.out[s])
+                if records is None:
+                    cuda_impl.resized_crop_mirror_normalize(self.stage[s], self.mean, self.std_scale, self.crop_hw, self.dev_boxes[s],
+                                                            self.dev_flip[s], self.out_dtype, out=self.out[s])
+                else:
+                    self.dev_rec[s].copy_(self.host_rec[s], non_blocking=True)
+                    mu = None
+                    if self.color_jitter["contrast"] > 0:
+                        mu = cuda_impl.crop_mean(self.stage[s], self.dev_boxes[s], self.crop_hw, out=self.dev_mu[s])
+                    cuda_impl.color_crop_mirror_normalize(self.stage[s], self.mean, self.std_scale, self.crop_hw, self.dev_boxes[s],
+                                                          self.dev_flip[s], self.dev_rec[s], mu, self.out_dtype, out=self.out[s])
                 ready = torch.cuda.Event()
                 ready.record(self.copy_stream)
         else:
-            x = ops.reference.resized_crop_mirror_normalize(src, self.mean, self.std_scale, self.crop_hw, self.host_boxes[s],
-                                                            self.host_flip[s], self.out_dtype)
+            if records is None:
+                x = ops.reference.resized_crop_mirror_normalize(src, self.mean, self.std_scale, self.crop_hw, self.host_boxes[s],
+                                                                self.host_flip[s], self.out_dtype)
+            else:
+                x = ops.reference.color_crop_mirror_normalize(src, self.mean, self.std_scale, self.crop_hw, self.host_boxes[s],
+                                                              self.host_flip[s], self.host_rec[s], self.out_dtype)
             self.out[s].copy_(x)
             ready = None
-        return LoadedBatch(self.out[s], s, ready, item, nbytes, boxes, flips)
+        return LoadedBatch(self.out[s], s, ready, item, nbytes, boxes, flips, records)
 
     def _run(self):
         if self.cuda:

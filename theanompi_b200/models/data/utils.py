@@ -168,6 +168,92 @@ def draw_resized_crops(n, in_hw, scale, ratio, rng):
     return np.stack([y0, x0, h, w], 1).astype(np.int32), flips
 
 
+CJ_KEY = "color_jitter"
+CJ_STRENGTHS = ("brightness", "contrast", "saturation", "lighting")
+CJ_DEFAULTS = {"brightness": 0.0, "contrast": 0.0, "saturation": 0.0, "lighting": 0.0, "seed": 0}
+CJ_GRAY = np.array([0.299, 0.587, 0.114])                      # fb.resnet.torch's grayscale weights
+# the ImageNet RGB eigen-decomposition of fb.resnet.torch's Lighting (Krizhevsky et al. 2012): eigenvalues and eigenvectors (columns)
+CJ_EIGVAL = np.array([0.2175, 0.0188, 0.0045])
+CJ_EIGVEC = np.array([[-0.5675, 0.7192, 0.4009],
+                      [-0.5808, -0.0045, -0.8140],
+                      [-0.5836, -0.6948, 0.4203]])
+CJ_RECORD_FLOATS = 24                                          # M (3×3), K (3×3), ℓ (3), 3 zeros: 96 bytes, six float4
+
+
+def check_color_jitter(cfg):
+    """The validated ``config['color_jitter']`` with every key filled in (the four strengths as floats in [0, 1], at least one of them
+    positive, and an int seed), or None for None; anything else is a ValueError that names the key."""
+    if cfg is None:
+        return None
+    if not isinstance(cfg, dict):
+        raise ValueError("%s must be a dict or None, not %r" % (CJ_KEY, cfg))
+    unknown = sorted(str(k) for k in cfg if k not in CJ_DEFAULTS)
+    if unknown:
+        raise ValueError("%s: unknown key %r; the keys are %s" % (CJ_KEY, unknown[0], ", ".join(CJ_DEFAULTS)))
+    out = {}
+    for k in CJ_STRENGTHS:
+        v = cfg.get(k, CJ_DEFAULTS[k])
+        if not _real(v):
+            raise ValueError("%s[%r] must be a finite real number, not %r" % (CJ_KEY, k, v))
+        if not 0.0 <= float(v) <= 1.0:
+            raise ValueError("%s[%r] must lie in [0, 1], not %r" % (CJ_KEY, k, v))
+        out[k] = float(v)
+    if not any(out[k] > 0.0 for k in CJ_STRENGTHS):
+        raise ValueError("%s: at least one of %s must be > 0" % (CJ_KEY, ", ".join(CJ_STRENGTHS)))
+    seed = cfg.get("seed", 0)
+    if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)):
+        raise ValueError("%s['seed'] must be an int, not %r" % (CJ_KEY, seed))
+    out["seed"] = int(seed) & (2 ** 64 - 1)
+    return out
+
+
+def color_jitter_rng(cfg, rank):
+    """The colour generator of one worker, keyed by (seed, rank, 1): apart from the random-resized-crop generator and the fixed-crop
+    RandomState, so turning the key on or off changes neither the boxes nor the crops drawn."""
+    return np.random.default_rng([cfg["seed"], int(rank), 1])
+
+
+def color_jitter_records(n, cfg, rng):
+    """Per-image colour maps of fb.resnet.torch's ``ColorJitter`` (brightness, saturation, contrast in a random order) then
+    ``Lighting``, composed into the affine map v' = M·v + K·μ + ℓ of an output pixel's RGB v (0…255) and the crop's mean RGB μ.
+
+    Each image draws, whatever the strengths: three uniforms for the factors (a, s, c) = 1 + U(−strength, strength), three uniforms
+    whose argsort is the order of the three operations (0 brightness, 1 saturation, 2 contrast; first applied first), three normals for
+    α = N(0, lighting).  All of the batch is drawn at once.  Starting from (M, K) = (I, 0), with G = 𝟙gᵀ the grayscale projection:
+    brightness (a·M, a·K); saturation P = s·I + (1 − s)·G, (P·M, P·K); contrast (c·M, c·K + (1 − c)·G·(M + K)), since the crop mean
+    of M·v + K·μ is (M + K)·μ.  ℓ = 255·E·(α ∘ λ).  Composed in float64, rounded once.  The three operations commute (g sums to 1),
+    so the order moves the record only by rounding; it is drawn so the stream follows fb.resnet.torch's ``RandomOrder``.
+
+    Returns (records float32 [n, 24]: M row-major, K row-major, ℓ, three zeros; factors float64 [n, 3] (a, s, c); order int64 [n, 3];
+    alpha float64 [n, 3])."""
+    u = rng.random((n, 6))
+    alpha = rng.standard_normal((n, 3)) * cfg["lighting"]
+    strength = np.array([cfg["brightness"], cfg["saturation"], cfg["contrast"]])
+    factors = 1.0 + strength * (2.0 * u[:, :3] - 1.0)
+    order = np.argsort(u[:, 3:], axis=1, kind="stable")
+    M, K, ell = color_jitter_maps(factors, order, alpha)
+    rec = np.zeros((n, CJ_RECORD_FLOATS), np.float32)
+    rec[:, 0:9] = M.reshape(n, 9)
+    rec[:, 9:18] = K.reshape(n, 9)
+    rec[:, 18:21] = ell
+    return rec, factors, order, alpha
+
+
+def color_jitter_maps(factors, order, alpha):
+    """The float64 (M [n, 3, 3], K [n, 3, 3], ℓ [n, 3]) of :func:`color_jitter_records` for given factors, orders and α."""
+    n = len(factors)
+    G = np.outer(np.ones(3), CJ_GRAY)
+    M = np.broadcast_to(np.eye(3), (n, 3, 3)).copy()
+    K = np.zeros((n, 3, 3))
+    a, s, c = (np.asarray(factors, np.float64)[:, i][:, None, None] for i in range(3))
+    P = s * np.eye(3) + (1.0 - s) * G
+    for pos in range(3):
+        op = np.asarray(order)[:, pos][:, None, None]
+        M, K = (np.where(op == 0, a * M, np.where(op == 1, P @ M, c * M)),
+                np.where(op == 0, a * K, np.where(op == 1, P @ K, c * K + (1.0 - c) * (G @ (M + K)))))
+    return M, K, 255.0 * (np.asarray(alpha, np.float64) * CJ_EIGVAL) @ CJ_EIGVEC.T
+
+
 def crop_and_mirror(data, mode, rand_crop, flag_batch, cropsize, rs=None):
     """Host reference: ``data`` is NHWC float/uint8; returns NHWC ``cropsize²`` crops."""
     n, H, W, C = data.shape

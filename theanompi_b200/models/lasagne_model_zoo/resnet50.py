@@ -98,7 +98,8 @@ class ResNet50(ModelBase):
             self.data.spawn_load()
             self.data.para_load_init(self.device, self.input_width, self.input_height, self.rand_crop,
                                      self.batch_crop_mirror, out_dtype=self.act_dtype,
-                                     resized_crop=self.resized_crop, rank=self.rank)
+                                     resized_crop=self.resized_crop, rank=self.rank,
+                                     color_jitter=self.color_jitter)
 
     # ---- construction: every conv is bias-free and linear; BatchNormal carries the ReLU (and the shortcut add)
     def _conv(self, inp, cout, k, stride, pad, input_shape=None):
@@ -190,4 +191,5 @@ class ResNet50Torch(TorchModelBase):
             self.data.spawn_load()
             self.data.para_load_init(self.device, self.input_width, self.input_height, self.rand_crop,
                                      self.batch_crop_mirror, out_dtype=self.act_dtype,
-                                     resized_crop=self.resized_crop, rank=self.rank)
+                                     resized_crop=self.resized_crop, rank=self.rank,
+                                     color_jitter=self.color_jitter)

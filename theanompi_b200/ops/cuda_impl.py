@@ -885,6 +885,61 @@ def resized_crop_mirror_normalize(x, mean, std_scale, out_hw, boxes, flips, out_
     return out
 
 
+def _color_inputs(name, x, boxes):
+    if x.dtype != torch.uint8 or x.dim() != 4 or x.shape[3] != 3:
+        raise ValueError("%s takes a uint8 NHWC batch with C = 3, not %s %s" % (name, x.dtype, tuple(x.shape)))
+    x = x.contiguous()
+    boxes = boxes.to(torch.int32).contiguous()
+    assert tuple(boxes.shape) == (x.shape[0], 4) and boxes.device == x.device and boxes.data_ptr() % 16 == 0
+    return x, boxes
+
+
+def crop_mean(x, boxes, out_hw, out=None):
+    """Mean RGB of each output crop (``nn_kernels.cu: crop_mean_kernel``): ``out[n, :3]`` is the mean over the ``out_hw`` pixels of the
+    bilinear resample of the raw box ``boxes[n]`` of the uint8 NHWC batch (C = 3), ``out[n, 3] = 0``; fp32 [N, 4], one launch, a
+    fixed-order reduction.  A box of the output's size gives the exact integer sum, divided once."""
+    x, boxes = _color_inputs("crop_mean", x, boxes)
+    N, H, W, _ = x.shape
+    ch, cw = out_hw
+    if out is None:
+        out = torch.empty((N, 4), dtype=torch.float32, device=x.device)
+    assert out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == (N, 4) and out.data_ptr() % 16 == 0
+    L().crop_mean(x.data_ptr(), boxes.data_ptr(), out.data_ptr(), N, H, W, ch, cw, _st(x))
+    return out
+
+
+def color_crop_mirror_normalize(x, mean, std_scale, out_hw, boxes, flips, records, mu=None, out_dtype=None, out=None):
+    """Colour jitter and lighting on the resized crop (``resized_crop_mirror_norm_kernel<_, true>``): with v̂ / m̂ the bilinear resample
+    of image n's raw box / of the mean, the output is ``(M·v̂ + K·μ + ℓ − m̂)·std_scale``, mirrored where ``flips[n]``.  ``records``:
+    fp32 [N, 24] on the device (M, K, ℓ, 0; ``utils.color_jitter_records``), 16-byte aligned; ``mu``: :func:`crop_mean`'s [N, 4], or
+    None when every K is 0.  A fixed crop is the box (y0, x0, ch, cw).  See :func:`reference.color_crop_mirror_normalize`."""
+    out_dtype = out_dtype or ADT()
+    x, boxes = _color_inputs("color_crop_mirror_normalize", x, boxes)
+    N, H, W, C = x.shape
+    ch, cw = out_hw
+    mean = mean.float().contiguous()
+    mode = 0 if mean.numel() == 1 else (1 if mean.numel() == C else 2)
+    if mode == 2:
+        assert mean.numel() == H * W * C
+    if out is None:
+        out = torch.empty((N, ch, cw, C), dtype=out_dtype, device=x.device)
+    assert out.dtype in (BF16, torch.float32) and out.is_contiguous() and tuple(out.shape) == (N, ch, cw, C)
+    flips = flips.to(torch.uint8).contiguous()
+    assert records.dtype == torch.float32 and records.is_contiguous() and tuple(records.shape) == (N, 24)
+    assert records.device == x.device and records.data_ptr() % 16 == 0
+    if mu is not None:
+        assert mu.dtype == torch.float32 and mu.is_contiguous() and tuple(mu.shape) == (N, 4) and mu.data_ptr() % 16 == 0
+    if isinstance(std_scale, torch.Tensor):
+        cs = std_scale.to(device=x.device, dtype=torch.float32).contiguous()
+        assert cs.numel() == C
+        sc, cs_ptr = 1.0, cs.data_ptr()
+    else:
+        sc, cs_ptr = float(std_scale), 0
+    L().color_crop_mirror_norm(x.data_ptr(), mean.data_ptr(), mode, sc, cs_ptr, out.data_ptr(), int(out.dtype == BF16), boxes.data_ptr(),
+                               flips.data_ptr(), records.data_ptr(), 0 if mu is None else mu.data_ptr(), N, H, W, ch, cw, _st(x))
+    return out
+
+
 # --------------------------------------------------------------------------- optimizer
 def _table(arena):
     if not hasattr(arena, "_tab_cache"):

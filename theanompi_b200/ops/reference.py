@@ -694,6 +694,40 @@ def resized_crop_mirror_normalize(x_u8, mean, std_scale, out_hw, boxes, flips, o
     return out.to(out_dtype)
 
 
+def color_crop_mirror_normalize(x_u8, mean, std_scale, out_hw, boxes, flips, records, out_dtype=torch.float32):
+    """Colour jitter and lighting on the (resized) crop: v = image i's raw box ``boxes[i] = (y0, x0, h, w)`` resampled to ``out_hw``
+    (``F.interpolate``, bilinear, ``align_corners=False``, no antialias), m̂ = the same resample of a per-pixel mean (a [C] or scalar
+    mean as it is), μ = the mean of v over the output pixels; the output is ``(M·v + K·μ + ℓ − m̂) * std_scale`` with (M, K, ℓ) from
+    ``records[i]`` (``models/data/utils.py: color_jitter_records``), then the optional horizontal flip.  A fixed crop is the box of
+    the output's size.  Values of M·v + K·μ + ℓ may leave [0, 255]: nothing is clamped, as in fb.resnet.torch.
+
+    x_u8 : [N, H, W, 3] uint8;  mean: [H, W, 3], [3] or scalar;  boxes: [N, 4] int, inside the image;  flips: [N];  records: [N, 24]
+    """
+    import torch.nn.functional as F
+    N, H, W, C = x_u8.shape
+    if isinstance(std_scale, torch.Tensor):
+        std_scale = std_scale.to(device=x_u8.device, dtype=torch.float32)
+    mean = torch.as_tensor(mean).float()
+    rec = torch.as_tensor(records).to(device=x_u8.device, dtype=torch.float32)
+    out = torch.empty((N,) + tuple(out_hw) + (C,), dtype=torch.float32, device=x_u8.device)
+
+    def resample(img, y0, x0, h, w):
+        box = img[y0:y0 + h, x0:x0 + w, :].permute(2, 0, 1).unsqueeze(0)
+        return F.interpolate(box, size=tuple(out_hw), mode="bilinear", align_corners=False, antialias=False)[0].permute(1, 2, 0)
+
+    for i in range(N):
+        y0, x0, h, w = (int(v) for v in boxes[i])
+        if not (h > 0 and w > 0 and 0 <= y0 <= H - h and 0 <= x0 <= W - w):
+            raise ValueError("color_crop_mirror_normalize: box %r of image %d is not inside %d x %d" % ((y0, x0, h, w), i, H, W))
+        v = resample(x_u8[i].float(), y0, x0, h, w)
+        m = resample(mean, y0, x0, h, w) if mean.dim() == 3 else mean
+        M, K, ell = rec[i, 0:9].view(3, 3), rec[i, 9:18].view(3, 3), rec[i, 18:21]
+        mu = v.reshape(-1, C).mean(0)
+        y = (v @ M.T + (K @ mu + ell) - m) * std_scale
+        out[i] = y.flip(1) if bool(flips[i]) else y
+    return out.to(out_dtype)
+
+
 # --------------------------------------------------------------------------- batch norm (+ residual)(+ ReLU), NHWC
 def _per_sample(s, x):
     """A drop-path row (one scale per sample of x's leading axis) shaped to broadcast over x."""
