@@ -171,6 +171,17 @@ void color_crop_mirror_norm(const void* x, const void* mean, int mean_mode, floa
                             cudaStream_t st);
 // mu[n] = mean RGB (fp32 [N, 4], last lane 0) of the ch × cw bilinear resample of the raw uint8 box n (x: [N, H, W, 3])
 void crop_mean(const void* x, const void* boxes, void* mu, int N, int H, int W, int ch, int cw, cudaStream_t st);
+// auto_augment (C = 3): the uint8 crop u (round-half-to-even of the bilinear resample of the raw box, mirrored; [N, ch, cw, 3]);
+// the per-slot point-op LUTs (uint8 [N, 3, 256]) from the ping buffer; one op slot ping → pong; the normalisation (u' − m̂)·s_c.
+// rec = fp32 [N, slots, 12], 16-byte aligned
+void aa_crop_u8(const void* x, void* u, const void* boxes, const void* flips, int N, int H, int W, int ch, int cw, cudaStream_t st);
+void aa_lut(const void* u, const void* rec, void* lut, int slot, int slots, int N, int ch, int cw, cudaStream_t st);
+void aa_apply(const void* in, void* out, const void* rec, const void* lut, int slot, int slots, int N, int ch, int cw, cudaStream_t st);
+void aa_normalize(const void* u, const void* mean, int mean_mode, float scale, const void* cscale, void* out, int out_bf16, const void* boxes,
+                  const void* flips, int N, int W, int ch, int cw, cudaStream_t st);
+// random erasing in place: out (bf16 (out_bf16) or fp32 NHWC [N, ch, cw, C]) is set to 0 inside box n = (i, j, h, w) (int32 [N, 4],
+// 16-byte aligned, inside the output; h = w = 0 erases nothing)
+void erase_boxes(void* out, int out_bf16, const void* boxes, int N, int ch, int cw, int C, cudaStream_t st);
 
 // ---- bn_kernels.cu: batch norm (+ residual)(+ ReLU) forward / backward, residual add  (f32: fp32 activations, else bf16)
 // drop_scale (optional, null = off): one row of the step's drop-path table, a float per sample of the `batch` samples (rows

@@ -144,6 +144,17 @@ PYBIND11_MODULE(_tmpi_native, m) {
                            S(st)); });
   m.def("crop_mean", [](ptr_t x, ptr_t boxes, ptr_t mu, int N, int H, int W, int ch, int cw, ptr_t st) {
     crop_mean(P(x), P(boxes), P(mu), N, H, W, ch, cw, S(st)); });
+  m.def("aa_crop_u8", [](ptr_t x, ptr_t u, ptr_t boxes, ptr_t flips, int N, int H, int W, int ch, int cw, ptr_t st) {
+    aa_crop_u8(P(x), P(u), P(boxes), P(flips), N, H, W, ch, cw, S(st)); });
+  m.def("aa_lut", [](ptr_t u, ptr_t rec, ptr_t lut, int slot, int slots, int N, int ch, int cw, ptr_t st) {
+    aa_lut(P(u), P(rec), P(lut), slot, slots, N, ch, cw, S(st)); });
+  m.def("aa_apply", [](ptr_t in, ptr_t out, ptr_t rec, ptr_t lut, int slot, int slots, int N, int ch, int cw, ptr_t st) {
+    aa_apply(P(in), P(out), P(rec), P(lut), slot, slots, N, ch, cw, S(st)); });
+  m.def("aa_normalize", [](ptr_t u, ptr_t mean, int mean_mode, float scale, ptr_t cscale, ptr_t out, int out_bf16, ptr_t boxes, ptr_t flips,
+                           int N, int W, int ch, int cw, ptr_t st) {
+    aa_normalize(P(u), P(mean), mean_mode, scale, P(cscale), P(out), out_bf16, P(boxes), P(flips), N, W, ch, cw, S(st)); });
+  m.def("erase_boxes", [](ptr_t out, int out_bf16, ptr_t boxes, int N, int ch, int cw, int C, ptr_t st) {
+    erase_boxes(P(out), out_bf16, P(boxes), N, ch, cw, C, S(st)); });
 
   // ---------------------------------------------------------------- batch norm / residual
   m.def("bn_forward", [](ptr_t x, ptr_t res, ptr_t y, ptr_t gamma, ptr_t beta, ptr_t mean, ptr_t rstd, ptr_t run_mean, ptr_t run_var, ptr_t scratch,

@@ -9,6 +9,7 @@
 #include "common.cuh"
 #include "api.h"
 #include <algorithm>
+#include <type_traits>
 
 namespace tmpi {
 
@@ -1613,6 +1614,14 @@ __global__ void __launch_bounds__(128) resized_crop_mirror_norm_kernel(const uin
   const uint8_t* src = x + (long long)n * H * W * C;
   const float wy0 = 1.f - ly, wx0 = 1.f - lx;
   Tout* o = out + ((long long)blockIdx.x * cw + ox) * C;
+  if constexpr (std::is_same_v<Tout, uint8_t>) {
+    // raw mode (auto_augment's uint8 crop): u = round-half-to-even of the bilinear resample v̂ of the raw box, no normalisation
+    for (int c = 0; c < C; ++c) {
+      const float v = wy0 * (wx0 * (float)src[t00 + c] + lx * (float)src[t01 + c]) + ly * (wx0 * (float)src[t10 + c] + lx * (float)src[t11 + c]);
+      o[c] = (uint8_t)__float2int_rn(v);
+    }
+    return;
+  }
   if constexpr (JITTER) {
     const float4* r = rec + 6 * n;
     const float4 r0 = r[0], r1 = r[1], r2 = r[2], r3 = r[3], r4 = r[4], r5 = r[5];
@@ -1733,6 +1742,235 @@ void crop_mean(const void* x, const void* boxes, void* mu, int N, int H, int W, 
   if ((long long)H * W * 3 >= (1LL << 31) || (long long)ch * cw >= (1LL << 24)) throw std::runtime_error("crop_mean: image too large");
   crop_mean_kernel<<<N, CROP_MEAN_THREADS, 0, st>>>((const uint8_t*)x, (const int4*)boxes, (float4*)mu, H, W, ch, cw);
   count_launch(); TMPI_CHECK_LAUNCH("crop_mean"); ::tmpi::check_capture(st, "crop_mean");
+}
+
+// ============================================================================ loader: TrivialAugmentWide / RandAugment on the uint8 crop
+// torchvision.transforms.v2's uint8 ops, one op slot at a time, on the [N, ch, cw, 3] uint8 crop u.  rec[n] = 12 floats per slot: op id,
+// scalar (factor, Solarize threshold or Posterize bits), 1 − factor (blends), 0, the fp32 inverse affine matrix (6), 0, 0.
+// aa_lut_kernel builds image n's per-channel 256-entry LUT for the point ops (Brightness, Contrast, Posterize, Solarize, AutoContrast,
+// Equalize) from the ping buffer, with the image-wide statistics they need; aa_apply_kernel maps ping → pong; aa_normalize_kernel
+// writes (u' − m̂)·s_c.  The fp32 expressions are torchvision's: a separate multiply and a fused add for the blends (ATen's vectorised
+// a + α·b), truncating casts after a clamp to [0, 255], an fma chain and a floor for the grey level.
+enum AaOp { AA_IDENTITY, AA_SHEARX, AA_SHEARY, AA_TRANSX, AA_TRANSY, AA_ROTATE, AA_BRIGHTNESS, AA_COLOR, AA_CONTRAST, AA_SHARPNESS,
+            AA_POSTERIZE, AA_SOLARIZE, AA_AUTOCONTRAST, AA_EQUALIZE };
+constexpr int AA_REC = 12;
+constexpr int AA_LUT_THREADS = 512;
+
+__device__ __forceinline__ uint8_t aa_clamp_trunc(float v) { return (uint8_t)(int)fminf(fmaxf(v, 0.f), 255.f); }
+__device__ __forceinline__ float aa_gray(float r, float g, float b) {
+  return floorf(__fmaf_rn(b, 0.114f, __fmaf_rn(g, 0.587f, __fmul_rn(r, 0.2989f))));
+}
+
+// One CTA per image; images whose op in this slot is not a point op return at once.  Reductions in shared memory (integer sums,
+// min / max, a shared-memory histogram): no global atomics, the same bits on every run.
+__global__ void __launch_bounds__(AA_LUT_THREADS) aa_lut_kernel(const uint8_t* __restrict__ u, const float* __restrict__ rec,
+                                                                 uint8_t* __restrict__ lut, int slot, int slots, int P) {
+  const int n = blockIdx.x, tid = threadIdx.x;
+  const float* r = rec + ((long long)n * slots + slot) * AA_REC;
+  const int op = (int)r[0];
+  if (!(op == AA_BRIGHTNESS || op == AA_CONTRAST || op == AA_POSTERIZE || op == AA_SOLARIZE || op == AA_AUTOCONTRAST || op == AA_EQUALIZE)) return;
+  const float f = r[1], d = r[2];
+  const uint8_t* src = u + (long long)n * P * 3;
+  uint8_t* L = lut + (long long)n * 768;
+  __shared__ int hist[3][256];
+  __shared__ int red[3][AA_LUT_THREADS / 32];
+  __shared__ float mean_s;
+  if (op == AA_CONTRAST) {
+    int sum = 0;                                            // floored grey levels: an exact integer sum (< 2^24 for 256² images)
+    for (int p = tid; p < P; p += AA_LUT_THREADS) sum += (int)aa_gray(src[3 * p], src[3 * p + 1], src[3 * p + 2]);
+    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    if ((tid & 31) == 0) red[0][tid >> 5] = sum;
+    __syncthreads();
+    if (tid == 0) {
+      long long t = 0;
+      for (int w = 0; w < AA_LUT_THREADS / 32; ++w) t += red[0][w];
+      mean_s = __fdiv_rn((float)t, (float)P);
+    }
+    __syncthreads();
+    const float mterm = mean_s;
+    for (int i = tid; i < 768; i += AA_LUT_THREADS) L[i] = aa_clamp_trunc(__fmaf_rn(mterm, d, __fmul_rn((float)(i & 255), f)));
+  } else if (op == AA_AUTOCONTRAST) {
+    int mn0 = 255, mn1 = 255, mn2 = 255, mx0 = 0, mx1 = 0, mx2 = 0;
+    for (int p = tid; p < P; p += AA_LUT_THREADS) {
+      const int a = src[3 * p], b = src[3 * p + 1], c = src[3 * p + 2];
+      mn0 = min(mn0, a); mn1 = min(mn1, b); mn2 = min(mn2, c); mx0 = max(mx0, a); mx1 = max(mx1, b); mx2 = max(mx2, c);
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+      mn0 = min(mn0, __shfl_xor_sync(0xffffffffu, mn0, o)); mn1 = min(mn1, __shfl_xor_sync(0xffffffffu, mn1, o));
+      mn2 = min(mn2, __shfl_xor_sync(0xffffffffu, mn2, o)); mx0 = max(mx0, __shfl_xor_sync(0xffffffffu, mx0, o));
+      mx1 = max(mx1, __shfl_xor_sync(0xffffffffu, mx1, o)); mx2 = max(mx2, __shfl_xor_sync(0xffffffffu, mx2, o));
+    }
+    if ((tid & 31) == 0) { red[0][tid >> 5] = mn0 | (mx0 << 16); red[1][tid >> 5] = mn1 | (mx1 << 16); red[2][tid >> 5] = mn2 | (mx2 << 16); }
+    __syncthreads();
+    for (int i = tid; i < 768; i += AA_LUT_THREADS) {
+      const int c = i >> 8;
+      int mn = 255, mx = 0;
+      for (int w = 0; w < AA_LUT_THREADS / 32; ++w) { mn = min(mn, red[c][w] & 0xffff); mx = max(mx, red[c][w] >> 16); }
+      float lo = (float)mn, inv = __fmul_rn((float)(mx - mn), 1.0f / 255.0f);
+      if (mx == mn) { lo = 0.f; inv = 1.f; }
+      L[i] = aa_clamp_trunc(__fdiv_rn(__fsub_rn((float)(i & 255), lo), inv));
+    }
+  } else if (op == AA_EQUALIZE) {
+    for (int i = tid; i < 768; i += AA_LUT_THREADS) (&hist[0][0])[i] = 0;
+    __syncthreads();
+    for (int p = tid; p < P; p += AA_LUT_THREADS) {
+      atomicAdd(&hist[0][src[3 * p]], 1); atomicAdd(&hist[1][src[3 * p + 1]], 1); atomicAdd(&hist[2][src[3 * p + 2]], 1);
+    }
+    __syncthreads();
+    if (tid < 3) {                                          // PIL's LUT, as torchvision computes it (step == 0: the identity)
+      const int c = tid;
+      int last = 255;
+      while (last > 0 && hist[c][last] == 0) --last;
+      const int step = (P - hist[c][last]) / 255;
+      uint8_t* Lc = L + c * 256;
+      if (step == 0) {
+        for (int k = 0; k < 256; ++k) Lc[k] = (uint8_t)k;
+      } else {
+        int cum = 0;
+        Lc[0] = 0;
+        for (int k = 1; k < 256; ++k) { cum += hist[c][k - 1]; Lc[k] = (uint8_t)min((cum + step / 2) / step, 255); }
+      }
+    }
+  } else {
+    for (int i = tid; i < 768; i += AA_LUT_THREADS) {
+      const int v = i & 255;
+      uint8_t o;
+      if (op == AA_BRIGHTNESS) o = aa_clamp_trunc(__fmul_rn((float)v, f));
+      else if (op == AA_POSTERIZE) { const int bits = (int)f; o = bits >= 8 ? (uint8_t)v : (uint8_t)(v & (((1 << bits) - 1) << (8 - bits))); }
+      else o = (float)v >= f ? (uint8_t)(255 - v) : (uint8_t)v;      // Solarize
+      L[i] = o;
+    }
+  }
+}
+
+// One CTA per output row (n, oy), like the crop kernels, so the op is CTA-uniform; reads ping, writes pong (never in place: the
+// geometric ops and Sharpness read neighbours).
+__global__ void __launch_bounds__(128) aa_apply_kernel(const uint8_t* __restrict__ in, uint8_t* __restrict__ out, const float* __restrict__ rec,
+                                                       const uint8_t* __restrict__ lut, int slot, int slots, int ch, int cw) {
+  const int ox = blockIdx.y * blockDim.x + threadIdx.x;
+  if (ox >= cw) return;
+  const int oy = blockIdx.x % ch, n = blockIdx.x / ch;
+  const float* r = rec + ((long long)n * slots + slot) * AA_REC;
+  const int op = (int)r[0];
+  const uint8_t* img = in + (long long)n * ch * cw * 3;
+  const uint8_t* px = img + ((long long)oy * cw + ox) * 3;
+  uint8_t* o = out + ((long long)blockIdx.x * cw + ox) * 3;
+  if (op >= AA_SHEARX && op <= AA_ROTATE) {
+    // nearest source of torchvision's affine grid: (m0·xb + m1·yb + m2) + (cw − 1)/2 about the centred output coordinates
+    const float xb = (float)ox - 0.5f * (float)(cw - 1), yb = (float)oy - 0.5f * (float)(ch - 1);
+    const float sx = __fmaf_rn(r[4], xb, __fmaf_rn(r[5], yb, r[6])) + 0.5f * (float)(cw - 1);
+    const float sy = __fmaf_rn(r[7], xb, __fmaf_rn(r[8], yb, r[9])) + 0.5f * (float)(ch - 1);
+    const float fx = rintf(sx), fy = rintf(sy);
+    if (fx >= 0.f && fx <= (float)(cw - 1) && fy >= 0.f && fy <= (float)(ch - 1)) {
+      const uint8_t* q = img + ((long long)fy * cw + (int)fx) * 3;
+      o[0] = q[0]; o[1] = q[1]; o[2] = q[2];
+    } else {
+      o[0] = 0; o[1] = 0; o[2] = 0;
+    }
+  } else if (op == AA_COLOR) {
+    const float f = r[1], d = r[2];
+    const float g = aa_gray(px[0], px[1], px[2]);
+    for (int c = 0; c < 3; ++c) o[c] = aa_clamp_trunc(__fmaf_rn(g, d, __fmul_rn((float)px[c], f)));
+  } else if (op == AA_SHARPNESS) {
+    if (oy == 0 || ox == 0 || oy == ch - 1 || ox == cw - 1) { o[0] = px[0]; o[1] = px[1]; o[2] = px[2]; return; }
+    const float d = r[2];
+    const long long rs = (long long)cw * 3;
+    for (int c = 0; c < 3; ++c) {
+      const uint8_t* q = px + c;
+      const int S = q[-rs - 3] + q[-rs] + q[-rs + 3] + q[-3] + 5 * q[0] + q[3] + q[rs - 3] + q[rs] + q[rs + 3];
+      const int blur = (2 * S + 13) / 26;                   // round(S / 13): S / 13 is never within 1/26 of a half
+      const float x = (float)q[0];
+      o[c] = aa_clamp_trunc(__fmaf_rn((float)blur - x, d, x));
+    }
+  } else if (op == AA_IDENTITY) {
+    o[0] = px[0]; o[1] = px[1]; o[2] = px[2];
+  } else {
+    const uint8_t* L = lut + (long long)n * 768;
+    o[0] = L[px[0]]; o[1] = L[256 + px[1]]; o[2] = L[512 + px[2]];
+  }
+}
+
+// out = (u' − m̂)·s_c, m̂ the bilinear resample of the mean over image n's (mirrored) box with the crop kernels' taps: geometry moves
+// content, not m̂, so a fill pixel becomes −m̂·s_c (torchvision's fill 0, then Normalize).
+template <typename Tout>
+__global__ void __launch_bounds__(128) aa_normalize_kernel(const uint8_t* __restrict__ u, const float* __restrict__ mean, int mean_mode,
+                                                           float scale, const float* __restrict__ cscale, Tout* __restrict__ out,
+                                                           const int4* __restrict__ boxes, const uint8_t* __restrict__ flips, int W,
+                                                           int ch, int cw) {
+  const int ox = blockIdx.y * blockDim.x + threadIdx.x;
+  if (ox >= cw) return;
+  const int oy = blockIdx.x % ch, n = blockIdx.x / ch;
+  const long long e = ((long long)blockIdx.x * cw + ox) * 3;
+  float m[3];
+  if (mean_mode != 2) {
+    for (int c = 0; c < 3; ++c) m[c] = mean_mode == 0 ? mean[0] : mean[c];
+  } else {
+    const int4 b = boxes[n];
+    int iy0, iy1, ix0, ix1;
+    float ly, lx;
+    rrc_axis(oy, __fdiv_rn((float)b.z, (float)ch), b.z, iy0, iy1, ly);
+    rrc_axis(flips[n] ? cw - 1 - ox : ox, __fdiv_rn((float)b.w, (float)cw), b.w, ix0, ix1, lx);
+    const unsigned r0 = (unsigned)((b.x + iy0) * W + b.y) * 3u, r1 = (unsigned)((b.x + iy1) * W + b.y) * 3u;
+    const unsigned t00 = r0 + 3u * ix0, t01 = r0 + 3u * ix1, t10 = r1 + 3u * ix0, t11 = r1 + 3u * ix1;
+    const float wy0 = 1.f - ly, wx0 = 1.f - lx;
+    for (int c = 0; c < 3; ++c)
+      m[c] = wy0 * (wx0 * mean[t00 + c] + lx * mean[t01 + c]) + ly * (wx0 * mean[t10 + c] + lx * mean[t11 + c]);
+  }
+  for (int c = 0; c < 3; ++c) out[e + c] = (Tout)(((float)u[e + c] - m[c]) * (cscale ? scale * cscale[c] : scale));
+}
+
+void aa_crop_u8(const void* x, void* u, const void* boxes, const void* flips, int N, int H, int W, int ch, int cw, cudaStream_t st) {
+  if ((long long)H * W * 3 >= (1LL << 31) || (long long)N * ch >= (1LL << 31)) throw std::runtime_error("aa_crop_u8: image too large");
+  const dim3 g((unsigned)(N * ch), (unsigned)((cw + 127) / 128));
+  resized_crop_mirror_norm_kernel<uint8_t><<<g, 128, 0, st>>>((const uint8_t*)x, nullptr, 0, 1.f, nullptr, (uint8_t*)u, (const int4*)boxes,
+                                                               (const uint8_t*)flips, H, W, 3, ch, cw);
+  count_launch(); TMPI_CHECK_LAUNCH("aa_crop_u8"); ::tmpi::check_capture(st, "aa_crop_u8");
+}
+
+void aa_lut(const void* u, const void* rec, void* lut, int slot, int slots, int N, int ch, int cw, cudaStream_t st) {
+  if ((long long)ch * cw * 255 >= (1LL << 31)) throw std::runtime_error("aa_lut: image too large");
+  aa_lut_kernel<<<N, AA_LUT_THREADS, 0, st>>>((const uint8_t*)u, (const float*)rec, (uint8_t*)lut, slot, slots, ch * cw);
+  count_launch(); TMPI_CHECK_LAUNCH("aa_lut"); ::tmpi::check_capture(st, "aa_lut");
+}
+
+void aa_apply(const void* in, void* out, const void* rec, const void* lut, int slot, int slots, int N, int ch, int cw, cudaStream_t st) {
+  const dim3 g((unsigned)(N * ch), (unsigned)((cw + 127) / 128));
+  aa_apply_kernel<<<g, 128, 0, st>>>((const uint8_t*)in, (uint8_t*)out, (const float*)rec, (const uint8_t*)lut, slot, slots, ch, cw);
+  count_launch(); TMPI_CHECK_LAUNCH("aa_apply"); ::tmpi::check_capture(st, "aa_apply");
+}
+
+void aa_normalize(const void* u, const void* mean, int mean_mode, float scale, const void* cscale, void* out, int out_bf16, const void* boxes,
+                  const void* flips, int N, int W, int ch, int cw, cudaStream_t st) {
+  const dim3 g((unsigned)(N * ch), (unsigned)((cw + 127) / 128));
+  auto U = (const uint8_t*)u; auto M = (const float*)mean; auto CS = (const float*)cscale; auto B = (const int4*)boxes; auto F = (const uint8_t*)flips;
+  if (out_bf16) aa_normalize_kernel<__nv_bfloat16><<<g, 128, 0, st>>>(U, M, mean_mode, scale, CS, (__nv_bfloat16*)out, B, F, W, ch, cw);
+  else aa_normalize_kernel<float><<<g, 128, 0, st>>>(U, M, mean_mode, scale, CS, (float*)out, B, F, W, ch, cw);
+  count_launch(); TMPI_CHECK_LAUNCH("aa_normalize"); ::tmpi::check_capture(st, "aa_normalize");
+}
+
+// ============================================================================ loader: random erasing of the normalised output
+// torchvision's RandomErasing(value=0) on the loader's output slot, in place: every element of image n's box (i, j, h, w) = boxes[n]
+// (output coordinates, after the mirror; h = w = 0 erases nothing) is set to 0.  Both output dtypes store 0 as all-zero bits, so the
+// kernel writes zero words of the element's width.  Grid (N, ERASE_ROW_CTAS): CTA (n, r) zeroes rows i + r, i + r + ERASE_ROW_CTAS, ...
+// of box n, its threads striding the w·C contiguous elements of each row; no other element is read or written.
+constexpr int ERASE_ROW_CTAS = 16;
+
+template <typename T>
+__global__ void __launch_bounds__(256) erase_boxes_kernel(T* __restrict__ out, const int4* __restrict__ boxes, int ch, int cw, int C) {
+  const int n = blockIdx.x;
+  const int4 b = boxes[n];                                               // (i, j, h, w), inside the output (host-drawn)
+  const int len = b.w * C;
+  for (int y = b.x + blockIdx.y; y < b.x + b.z; y += ERASE_ROW_CTAS) {
+    T* row = out + (((long long)n * ch + y) * cw + b.y) * C;
+    for (int e = threadIdx.x; e < len; e += blockDim.x) row[e] = T(0);
+  }
+}
+
+void erase_boxes(void* out, int out_bf16, const void* boxes, int N, int ch, int cw, int C, cudaStream_t st) {
+  const dim3 g((unsigned)N, ERASE_ROW_CTAS);
+  if (out_bf16) erase_boxes_kernel<unsigned short><<<g, 256, 0, st>>>((unsigned short*)out, (const int4*)boxes, ch, cw, C);
+  else erase_boxes_kernel<unsigned int><<<g, 256, 0, st>>>((unsigned int*)out, (const int4*)boxes, ch, cw, C);
+  count_launch(); TMPI_CHECK_LAUNCH("erase_boxes"); ::tmpi::check_capture(st, "erase_boxes");
 }
 
 }  // namespace tmpi

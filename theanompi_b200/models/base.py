@@ -69,7 +69,8 @@ class ModelBase(object):
     supports_label_smoothing = True    # config['label_smoothing'] > 0 (False: no classifier head; refused at compile_iter_fns)
     supports_mixup = True          # config['mixup'] (False: no image batch before a first convolution; refused at compile_iter_fns)
     supports_drop_path = False     # config['drop_path_rate'] > 0 (True: residual blocks in self.body that read drop_row(l))
-    # True: an ImageNet model fed by ParaLoader, so config['random_resized_crop'] and config['color_jitter'] reach its loader
+    # True: an ImageNet model fed by ParaLoader, so config['random_resized_crop'], config['color_jitter'] and
+    # config['random_erasing'] reach its loader
     # (refused at construction otherwise)
     supports_resized_crop = False
     name = "Model"
@@ -138,6 +139,12 @@ class ModelBase(object):
         # colour jitter and PCA lighting of the training images (a dict, models/data/utils.py: check_color_jitter; None = off):
         # per-image colour maps drawn by the loader and applied by its crop kernel; like the crop, the training step never sees it
         self.color_jitter = self.check_color_jitter(config.get("color_jitter"))
+        # random erasing of the normalised training images (a dict, models/data/utils.py: check_random_erasing; None = off): boxes
+        # drawn by the loader and zeroed by one more launch on its copy stream; the training step never sees it
+        self.random_erasing = self.check_random_erasing(config.get("random_erasing"))
+        # TrivialAugmentWide / RandAugment on the uint8 training crop (a dict, models/data/utils.py: check_auto_augment; None = off):
+        # op records drawn by the loader and applied by its kernels on the copy stream; the training step never sees it
+        self.auto_augment = self.check_auto_augment(config.get("auto_augment"))
         self.base_lr = np.float32(self.learning_rate)
         self.current_t = self.subb_t = 0
         self.current_v = self.subb_v = 0
@@ -371,6 +378,29 @@ class ModelBase(object):
         if cfg is not None and not self.supports_resized_crop:
             raise ValueError("%s: %s is not supported; it augments the ImageNet loader of AlexNet, GoogLeNet, VGG16, ResNet50, "
                              "ResNet152 and ResNet50Torch" % (type(self).__name__, CJ_KEY))
+        return cfg
+
+    def check_auto_augment(self, cfg):
+        """The validated ``config['auto_augment']`` (models/data/utils.py: check_auto_augment; a ValueError names the key), or None.
+        A dict needs a model fed by the ImageNet loader (``supports_resized_crop``) and no ``color_jitter``."""
+        from .data.utils import AA_KEY, check_auto_augment
+        cfg = check_auto_augment(cfg)
+        if cfg is not None and not self.supports_resized_crop:
+            raise ValueError("%s: %s is not supported; it augments the ImageNet loader of AlexNet, GoogLeNet, VGG16, ResNet50, "
+                             "ResNet152 and ResNet50Torch" % (type(self).__name__, AA_KEY))
+        if cfg is not None and self.color_jitter is not None:
+            raise ValueError("%s: %s and color_jitter are two different colour recipes (torchvision's clamped uint8 ops against "
+                             "fb.resnet.torch's unclamped affine jitter); choose one" % (type(self).__name__, AA_KEY))
+        return cfg
+
+    def check_random_erasing(self, cfg):
+        """The validated ``config['random_erasing']`` (models/data/utils.py: check_random_erasing; a ValueError names the key), or
+        None.  A dict needs a model fed by the ImageNet loader (``supports_resized_crop``); every crop path composes with it."""
+        from .data.utils import RE_KEY, check_random_erasing
+        cfg = check_random_erasing(cfg)
+        if cfg is not None and not self.supports_resized_crop:
+            raise ValueError("%s: %s is not supported; it augments the ImageNet loader of AlexNet, GoogLeNet, VGG16, ResNet50, "
+                             "ResNet152 and ResNet50Torch" % (type(self).__name__, RE_KEY))
         return cfg
 
     # ------------------------------------------------------------------ stochastic depth (drop-path)

@@ -171,7 +171,10 @@ class ImageNet_data(object):
         crop/mirror on the host, return an NHWC float tensor.  With ``model.resized_crop`` a "train" batch is the random-resized
         crop of :meth:`para_load_init`'s loader, drawn from this object's generator keyed by (seed, ``model.rank``).  With
         ``model.color_jitter`` a "train" batch also gets the loader's colour maps, drawn from a generator keyed by (seed, rank, 1),
-        on the same boxes or fixed crops as without it."""
+        on the same boxes or fixed crops as without it.  With ``model.random_erasing`` a "train" batch, whichever crop made it, then
+        gets the loader's erase boxes, drawn from a generator keyed by (seed, rank, 3), set to 0.  With ``model.auto_augment`` a
+        "train" batch gets the loader's op records, drawn from a generator keyed by (seed, rank, 2), on the same boxes or fixed
+        crops."""
         import torch
         from ... import ops
         from .utils import color_jitter_records, color_jitter_rng, crop_and_mirror, draw_crops
@@ -181,6 +184,7 @@ class ImageNet_data(object):
             raw = src.numpy()
         rrc = getattr(model, "resized_crop", None)
         cj = getattr(model, "color_jitter", None) if mode == "train" else None
+        aa = getattr(model, "auto_augment", None) if mode == "train" else None
         n = raw.shape[0]
         mean, cs = torch.from_numpy(self.rawdata[4]), torch.from_numpy(1.0 / 255.0 / self.rawdata[5])
         if rrc is not None and mode == "train":
@@ -189,9 +193,9 @@ class ImageNet_data(object):
                 self._rrc_rng = resized_crop_rng(rrc, model.rank)
             out_hw = (model.input_height, model.input_width)
             boxes, flips = draw_resized_crops(n, (self.height, self.width), rrc["scale"], rrc["ratio"], self._rrc_rng)
-            if cj is None:
+            if cj is None and aa is None:
                 t = ops.reference.resized_crop_mirror_normalize(torch.from_numpy(raw), mean, cs, out_hw, boxes, flips)
-        elif cj is not None:
+        elif cj is not None or aa is not None:
             # the same RandomState draw as crop_and_mirror below, so the key changes no crop
             out_hw = (model.input_width, model.input_width)
             offs, flips = draw_crops(n, (self.height, self.width), out_hw, mode, model.rand_crop, model.batch_crop_mirror)
@@ -205,6 +209,18 @@ class ImageNet_data(object):
                 self._cj_rng = color_jitter_rng(cj, model.rank)
             records = color_jitter_records(n, cj, self._cj_rng)[0]
             t = ops.reference.color_crop_mirror_normalize(torch.from_numpy(raw), mean, cs, out_hw, boxes, flips, records)
+        if aa is not None:
+            from .utils import auto_augment_records, auto_augment_rng
+            if getattr(self, "_aa_rng", None) is None:
+                self._aa_rng = auto_augment_rng(aa, model.rank)
+            records = auto_augment_records(n, aa, self._aa_rng, out_hw)[0]
+            t = ops.reference.auto_augment_crop_normalize(torch.from_numpy(raw), mean, cs, out_hw, boxes, flips, records)
+        re_cfg = getattr(model, "random_erasing", None) if mode == "train" else None
+        if re_cfg is not None:
+            from .utils import draw_erase_boxes, random_erasing_rng
+            if getattr(self, "_re_rng", None) is None:
+                self._re_rng = random_erasing_rng(re_cfg, model.rank)
+            t = ops.reference.random_erase(t, draw_erase_boxes(n, tuple(t.shape[1:3]), re_cfg, self._re_rng))
         if model.cuda:
             t = t.pin_memory().to(model.device, non_blocking=True)
         return t
@@ -217,18 +233,20 @@ class ImageNet_data(object):
         return None
 
     def para_load_init(self, device, input_width, input_height, rand_crop, batch_crop_mirror,
-                       out_dtype=None, depth=2, mode=None, resized_crop=None, rank=0, color_jitter=None):
+                       out_dtype=None, depth=2, mode=None, resized_crop=None, rank=0, color_jitter=None, random_erasing=None,
+                       auto_augment=None):
         """``mode='thread'`` (default): loader thread + pinned ring in this process.  ``mode='process'`` (or
         ``TMPI_LOADER=process``): a separate loader process fills a page-locked shared-memory ring (see ``proc_loader.py``) —
         the reference's ``proc_load_mpi.py`` child, minus its second CUDA context.  ``resized_crop`` (a validated
-        ``config['random_resized_crop']``), ``color_jitter`` (a validated ``config['color_jitter']``) and ``rank`` go to the
-        :class:`ParaLoader`, which draws the boxes and the colour maps in this process."""
+        ``config['random_resized_crop']``), ``color_jitter`` (a validated ``config['color_jitter']``), ``random_erasing`` (a
+        validated ``config['random_erasing']``) and ``rank`` go to the :class:`ParaLoader`, which draws the boxes, the colour maps
+        and the erase boxes in this process."""
         from .loader import ParaLoader
         raw_shape = (self.file_batch_size, self.height, self.width, self.channels)
         mode = mode or os.environ.get("TMPI_LOADER", "thread")
         kw = dict(mean=self.rawdata[4], std_scale=1.0 / 255.0 / self.rawdata[5], out_dtype=out_dtype, depth=depth,
                   rand_crop=rand_crop, batch_crop_mirror=batch_crop_mirror, resized_crop=resized_crop, rank=rank,
-                  color_jitter=color_jitter)
+                  color_jitter=color_jitter, random_erasing=random_erasing, auto_augment=auto_augment)
         if mode == "process":
             from .proc_loader import ProcReader
             self.proc_reader = ProcReader(raw_shape, depth=depth, seed=self._seed)

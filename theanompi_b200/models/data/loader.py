@@ -31,29 +31,38 @@ import numpy as np
 import torch
 
 from ... import ops
-from .utils import (CJ_RECORD_FLOATS, color_jitter_records, color_jitter_rng, draw_crops, draw_resized_crops,
-                    resized_crop_rng)
+from .utils import (AA_RECORD_FLOATS, CJ_RECORD_FLOATS, auto_augment_records, auto_augment_rng, color_jitter_records, color_jitter_rng, draw_crops, draw_erase_boxes, draw_resized_crops,
+                    random_erasing_rng, resized_crop_rng)
 
 
 class LoadedBatch(object):
     """One loaded batch; ``boxes`` / ``flips``: the host copies of the random-resized-crop draw it was made with, or of the fixed
-    crops as boxes of the output's size under colour jitter (None otherwise); ``records``: the colour-jitter records (None otherwise)."""
-    __slots__ = ("x", "slot", "ready", "item", "h2d_bytes", "boxes", "flips", "records")
+    crops as boxes of the output's size under colour jitter (None otherwise); ``records``: the colour-jitter records (None otherwise);
+    ``erase``: the random-erasing boxes (i, j, h, w) in output coordinates (None otherwise); ``aa_records``: the auto_augment op
+    records, float32 [N, slots, 12] (None otherwise)."""
+    __slots__ = ("x", "slot", "ready", "item", "h2d_bytes", "boxes", "flips", "records", "erase", "aa_records")
 
-    def __init__(self, x, slot, ready, item, h2d_bytes, boxes=None, flips=None, records=None):
+    def __init__(self, x, slot, ready, item, h2d_bytes, boxes=None, flips=None, records=None, erase=None, aa_records=None):
         self.x, self.slot, self.ready, self.item, self.h2d_bytes = x, slot, ready, item, h2d_bytes
-        self.boxes, self.flips, self.records = boxes, flips, records
+        self.boxes, self.flips, self.records, self.erase, self.aa_records = boxes, flips, records, erase, aa_records
 
 
 class ParaLoader(object):
     def __init__(self, read_fn, device, raw_shape, crop_hw, mean, std_scale=1.0 / 255.0,
                  out_dtype=None, depth=2, rand_crop=True, batch_crop_mirror=False, seed=1234,
-                 threaded=True, host_buffers=None, on_close=None, resized_crop=None, rank=0, color_jitter=None):
+                 threaded=True, host_buffers=None, on_close=None, resized_crop=None, rank=0, color_jitter=None,
+                 random_erasing=None, auto_augment=None):
         """``resized_crop``: a validated ``config['random_resized_crop']`` (``utils.check_resized_crop``) or None; with it every
         "train" batch is a random-resized crop drawn per image from the generator keyed by (its seed, ``rank``), and "val" batches
         keep the centre crop.  ``color_jitter``: a validated ``config['color_jitter']`` (``utils.check_color_jitter``) or None; with
         it every "train" image gets a colour map drawn from the generator keyed by (its seed, ``rank``, 1), applied by the crop
-        kernel on the same boxes or fixed crops as without it; "val" batches are never jittered."""
+        kernel on the same boxes or fixed crops as without it; "val" batches are never jittered.  ``random_erasing``: a validated
+        ``config['random_erasing']`` (``utils.check_random_erasing``) or None; with it every "train" batch, whichever crop path made
+        it, gets erase boxes drawn from the generator keyed by (its seed, ``rank``, 3) and zeroed in the output slot by one more
+        launch on the copy stream; "val" batches are never erased.  ``auto_augment``: a validated ``config['auto_augment']``
+        (``utils.check_auto_augment``) or None; with it every "train" image gets TrivialAugmentWide / RandAugment op records drawn from
+        the generator keyed by (its seed, ``rank``, 2), applied on the uint8 crop of the same boxes or fixed crops between the crop
+        and the normalisation; "val" batches are never augmented."""
         self.read_fn = read_fn
         self.device = torch.device(device)
         self.cuda = self.device.type == "cuda"
@@ -88,7 +97,17 @@ class ParaLoader(object):
         if color_jitter is not None:
             self.cj_rng = color_jitter_rng(color_jitter, rank)
             self.host_rec = [torch.empty((N, CJ_RECORD_FLOATS), dtype=torch.float32, pin_memory=pin) for _ in range(depth)]
-        boxed = resized_crop is not None or color_jitter is not None
+        self.random_erasing = random_erasing
+        if random_erasing is not None:
+            self.re_rng = random_erasing_rng(random_erasing, rank)
+            self.host_erase = [torch.empty((N, 4), dtype=torch.int32, pin_memory=pin) for _ in range(depth)]
+        self.auto_augment = auto_augment
+        if auto_augment is not None:
+            self.aa_rng = auto_augment_rng(auto_augment, rank)
+            self.aa_slots = 1 if auto_augment["policy"] == "trivial_wide" else auto_augment["num_ops"]
+            self.host_aa = [torch.empty((N, self.aa_slots, AA_RECORD_FLOATS), dtype=torch.float32, pin_memory=pin)
+                            for _ in range(depth)]
+        boxed = resized_crop is not None or color_jitter is not None or auto_augment is not None
         if boxed:
             self.host_boxes = [torch.empty((N, 4), dtype=torch.int32, pin_memory=pin) for _ in range(depth)]
         if self.cuda:
@@ -97,6 +116,15 @@ class ParaLoader(object):
             if color_jitter is not None:
                 self.dev_rec = [torch.empty((N, CJ_RECORD_FLOATS), dtype=torch.float32, device=self.device) for _ in range(depth)]
                 self.dev_mu = [torch.empty((N, 4), dtype=torch.float32, device=self.device) for _ in range(depth)]
+            if auto_augment is not None:
+                # the uint8 ping / pong crops and the point-op LUTs: used on the copy stream one batch at a time, so one set
+                self.aa_ping = torch.empty((N,) + self.crop_hw + (3,), dtype=torch.uint8, device=self.device)
+                self.aa_pong = torch.empty_like(self.aa_ping)
+                self.aa_lut = torch.empty((N, 3, 256), dtype=torch.uint8, device=self.device)
+                self.dev_aa = [torch.empty((N, self.aa_slots, AA_RECORD_FLOATS), dtype=torch.float32, device=self.device)
+                               for _ in range(depth)]
+            if random_erasing is not None:
+                self.dev_erase = [torch.empty((N, 4), dtype=torch.int32, device=self.device) for _ in range(depth)]
             self.stage = [torch.empty(self.raw_shape, dtype=torch.uint8, device=self.device) for _ in range(depth)]
             self.dev_offs = [torch.empty((N, 2), dtype=torch.int32, device=self.device) for _ in range(depth)]
             self.dev_flip = [torch.empty((N,), dtype=torch.uint8, device=self.device) for _ in range(depth)]
@@ -132,35 +160,55 @@ class ParaLoader(object):
             # the ring slot is refilled by another process as soon as we request the next file: the DMA out of it must have
             # finished before this slot comes round again — recorded below, awaited at the top of the next _produce(s)
             pass
-        if mode == "train" and (self.resized_crop is not None or self.color_jitter is not None):
-            return self._produce_boxed(s, src, item, mode)
-        offs, flips = draw_crops(N, (H, W), self.crop_hw, mode, self.rand_crop, self.batch_crop_mirror, self.rs)
-        self.host_offs[s].numpy()[...] = offs
-        self.host_flip[s].numpy()[...] = flips
-        if self.cuda:
-            with torch.cuda.stream(self.copy_stream):
-                self.stage[s].copy_(src, non_blocking=True)
-                self.dev_offs[s].copy_(self.host_offs[s], non_blocking=True)
-                self.dev_flip[s].copy_(self.host_flip[s], non_blocking=True)
-                from ...ops import cuda_impl
-                cuda_impl.crop_mirror_normalize(self.stage[s], self.mean, self.std_scale, self.crop_hw,
-                                                self.dev_offs[s], self.dev_flip[s], self.out_dtype,
-                                                out=self.out[s])
-                ready = torch.cuda.Event()
-                ready.record(self.copy_stream)
+        aa = None
+        if mode == "train" and (self.resized_crop is not None or self.color_jitter is not None or self.auto_augment is not None):
+            boxes, flips, records, aa, nbytes = self._produce_boxed(s, src, mode)
         else:
-            x = ops.reference.crop_mirror_normalize(src, self.mean, self.std_scale, self.crop_hw,
-                                                    self.host_offs[s], self.host_flip[s], self.out_dtype)
-            self.out[s].copy_(x)
-            ready = None
-        return LoadedBatch(self.out[s], s, ready, item, self.h2d_bytes)
+            boxes = flips = records = None
+            nbytes = self.h2d_bytes
+            offs, fl = draw_crops(N, (H, W), self.crop_hw, mode, self.rand_crop, self.batch_crop_mirror, self.rs)
+            self.host_offs[s].numpy()[...] = offs
+            self.host_flip[s].numpy()[...] = fl
+            if self.cuda:
+                with torch.cuda.stream(self.copy_stream):
+                    self.stage[s].copy_(src, non_blocking=True)
+                    self.dev_offs[s].copy_(self.host_offs[s], non_blocking=True)
+                    self.dev_flip[s].copy_(self.host_flip[s], non_blocking=True)
+                    from ...ops import cuda_impl
+                    cuda_impl.crop_mirror_normalize(self.stage[s], self.mean, self.std_scale, self.crop_hw,
+                                                    self.dev_offs[s], self.dev_flip[s], self.out_dtype,
+                                                    out=self.out[s])
+            else:
+                x = ops.reference.crop_mirror_normalize(src, self.mean, self.std_scale, self.crop_hw,
+                                                        self.host_offs[s], self.host_flip[s], self.out_dtype)
+                self.out[s].copy_(x)
+        erase = None
+        if mode == "train" and self.random_erasing is not None:
+            # the erase boxes come after whichever crop path ran, from their own generator, in output coordinates
+            erase = draw_erase_boxes(N, self.crop_hw, self.random_erasing, self.re_rng)
+            self.host_erase[s].numpy()[...] = erase
+            nbytes += N * 16
+            if self.cuda:
+                with torch.cuda.stream(self.copy_stream):
+                    self.dev_erase[s].copy_(self.host_erase[s], non_blocking=True)
+                    from ...ops import cuda_impl
+                    cuda_impl.random_erase(self.out[s], self.dev_erase[s])
+            else:
+                self.out[s].copy_(ops.reference.random_erase(self.out[s], self.host_erase[s]))
+        ready = None
+        if self.cuda:
+            ready = torch.cuda.Event()
+            ready.record(self.copy_stream)
+        return LoadedBatch(self.out[s], s, ready, item, nbytes, boxes, flips, records, erase, aa)
 
-    def _produce_boxed(self, s, src, item, mode):
+    def _produce_boxed(self, s, src, mode):
         """A "train" batch with ``resized_crop`` or ``color_jitter``: boxes (the random-resized-crop draw, or the fixed crops'
         offsets with the output's size) and flips drawn on the host, the 16-byte box record copied next to the flips, and the
         96-byte colour record with them under ``color_jitter``; then on the copy stream ``resized_crop_mirror_norm``, or
         ``crop_mean`` (only when the contrast strength is > 0, since otherwise K ≡ 0) and ``color_crop_mirror_norm`` (the
-        references on the CPU)."""
+        references on the CPU).  Under ``auto_augment`` the op records (48 bytes per image and slot) travel with them and
+        ``auto_augment_crop_normalize`` runs instead: the uint8 crop, per slot a LUT launch when a point op is drawn and an apply
+        launch, then the normalisation.  Returns (boxes, flips, colour records or None, op records or None, bytes copied)."""
         N, H, W, C = self.raw_shape
         if self.resized_crop is not None:
             boxes, flips = draw_resized_crops(N, (H, W), self.resized_crop["scale"], self.resized_crop["ratio"], self.rrc_rng)
@@ -175,13 +223,23 @@ class ParaLoader(object):
             records = color_jitter_records(N, self.color_jitter, self.cj_rng)[0]
             self.host_rec[s].numpy()[...] = records
             nbytes += N * 4 * CJ_RECORD_FLOATS
+        aa = None
+        if self.auto_augment is not None:
+            aa, aa_ops, _ = auto_augment_records(N, self.auto_augment, self.aa_rng, self.crop_hw)
+            self.host_aa[s].numpy()[...] = aa
+            nbytes += aa.nbytes
         if self.cuda:
             with torch.cuda.stream(self.copy_stream):
                 self.stage[s].copy_(src, non_blocking=True)
                 self.dev_boxes[s].copy_(self.host_boxes[s], non_blocking=True)
                 self.dev_flip[s].copy_(self.host_flip[s], non_blocking=True)
                 from ...ops import cuda_impl
-                if records is None:
+                if aa is not None:
+                    self.dev_aa[s].copy_(self.host_aa[s], non_blocking=True)
+                    cuda_impl.auto_augment_crop_normalize(self.stage[s], self.mean, self.std_scale, self.crop_hw, self.dev_boxes[s],
+                                                          self.dev_flip[s], self.dev_aa[s], aa_ops, self.out_dtype, out=self.out[s],
+                                                          ping=self.aa_ping, pong=self.aa_pong, lut=self.aa_lut)
+                elif records is None:
                     cuda_impl.resized_crop_mirror_normalize(self.stage[s], self.mean, self.std_scale, self.crop_hw, self.dev_boxes[s],
                                                             self.dev_flip[s], self.out_dtype, out=self.out[s])
                 else:
@@ -191,18 +249,18 @@ class ParaLoader(object):
                         mu = cuda_impl.crop_mean(self.stage[s], self.dev_boxes[s], self.crop_hw, out=self.dev_mu[s])
                     cuda_impl.color_crop_mirror_normalize(self.stage[s], self.mean, self.std_scale, self.crop_hw, self.dev_boxes[s],
                                                           self.dev_flip[s], self.dev_rec[s], mu, self.out_dtype, out=self.out[s])
-                ready = torch.cuda.Event()
-                ready.record(self.copy_stream)
         else:
-            if records is None:
+            if aa is not None:
+                x = ops.reference.auto_augment_crop_normalize(src, self.mean, self.std_scale, self.crop_hw, self.host_boxes[s],
+                                                              self.host_flip[s], self.host_aa[s], self.out_dtype)
+            elif records is None:
                 x = ops.reference.resized_crop_mirror_normalize(src, self.mean, self.std_scale, self.crop_hw, self.host_boxes[s],
                                                                 self.host_flip[s], self.out_dtype)
             else:
                 x = ops.reference.color_crop_mirror_normalize(src, self.mean, self.std_scale, self.crop_hw, self.host_boxes[s],
                                                               self.host_flip[s], self.host_rec[s], self.out_dtype)
             self.out[s].copy_(x)
-            ready = None
-        return LoadedBatch(self.out[s], s, ready, item, nbytes, boxes, flips, records)
+        return boxes, flips, records, aa, nbytes
 
     def _run(self):
         if self.cuda:

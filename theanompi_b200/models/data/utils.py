@@ -254,6 +254,194 @@ def color_jitter_maps(factors, order, alpha):
     return M, K, 255.0 * (np.asarray(alpha, np.float64) * CJ_EIGVAL) @ CJ_EIGVEC.T
 
 
+AA_KEY = "auto_augment"
+AA_DEFAULTS = {"policy": "trivial_wide", "num_ops": 2, "magnitude": 9, "num_magnitude_bins": 31, "seed": 0}
+AA_POLICIES = ("trivial_wide", "rand")
+# torchvision's op set of TrivialAugmentWide and RandAugment, in their order; the op id is the index
+AA_OPS = ("Identity", "ShearX", "ShearY", "TranslateX", "TranslateY", "Rotate", "Brightness", "Color", "Contrast", "Sharpness",
+          "Posterize", "Solarize", "AutoContrast", "Equalize")
+AA_SIGNED = frozenset(AA_OPS[1:10])
+AA_LUT_OPS = frozenset((6, 8, 10, 11, 12, 13))                  # point ops applied through a per-image, per-channel 256-entry LUT
+AA_RECORD_FLOATS = 12                                          # op, scalar, 1 − factor, 0, inverse affine matrix (6), 0, 0: 48 bytes
+
+
+def check_auto_augment(cfg):
+    """The validated ``config['auto_augment']`` with every key filled in, or None for None; anything else is a ValueError that names
+    the key.  ``num_ops`` and ``magnitude`` belong to the "rand" policy only."""
+    if cfg is None:
+        return None
+    if not isinstance(cfg, dict):
+        raise ValueError("%s must be a dict or None, not %r" % (AA_KEY, cfg))
+    unknown = sorted(str(k) for k in cfg if k not in AA_DEFAULTS)
+    if unknown:
+        raise ValueError("%s: unknown key %r; the keys are %s" % (AA_KEY, unknown[0], ", ".join(AA_DEFAULTS)))
+    policy = cfg.get("policy", AA_DEFAULTS["policy"])
+    if policy not in AA_POLICIES:
+        raise ValueError("%s['policy'] must be one of %s, not %r" % (AA_KEY, ", ".join(AA_POLICIES), policy))
+    if policy == "trivial_wide":
+        for k in ("num_ops", "magnitude"):
+            if k in cfg:
+                raise ValueError("%s[%r] belongs to policy 'rand', not 'trivial_wide'" % (AA_KEY, k))
+    out = {"policy": policy}
+    for k in ("num_magnitude_bins", "num_ops", "magnitude", "seed"):
+        v = cfg.get(k, AA_DEFAULTS[k])
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+            raise ValueError("%s[%r] must be an int, not %r" % (AA_KEY, k, v))
+        out[k] = int(v)
+    if out["num_magnitude_bins"] < 2:
+        raise ValueError("%s['num_magnitude_bins'] must be >= 2, not %r" % (AA_KEY, out["num_magnitude_bins"]))
+    if not 1 <= out["num_ops"] <= 4:
+        raise ValueError("%s['num_ops'] must lie in [1, 4], not %r" % (AA_KEY, out["num_ops"]))
+    if not 0 <= out["magnitude"] <= out["num_magnitude_bins"] - 1:
+        raise ValueError("%s['magnitude'] must lie in [0, num_magnitude_bins - 1], not %r" % (AA_KEY, out["magnitude"]))
+    out["seed"] &= 2 ** 64 - 1
+    if policy == "trivial_wide":
+        del out["num_ops"], out["magnitude"]
+    return out
+
+
+def auto_augment_rng(cfg, rank):
+    """The policy generator of one worker, keyed by (seed, rank, 2): apart from the crop, colour and erasing generators."""
+    return np.random.default_rng([cfg["seed"], int(rank), 2])
+
+
+def auto_augment_space(policy, num_bins, out_hw):
+    """{op name: (magnitudes float64 [num_bins] or None, signed)}: torchvision's ``_AUGMENTATION_SPACE`` of ``TrivialAugmentWide``
+    ("trivial_wide") or ``RandAugment`` ("rand") for an image of ``out_hw``, computed as torchvision computes it (fp32 linspace)."""
+    import torch
+    h, w = out_hw
+    lin = lambda hi, lo=0.0: torch.linspace(lo, hi, num_bins).double().numpy()  # noqa: E731
+    if policy == "trivial_wide":
+        geo, shear, rot, col, post = (lin(32.0), lin(32.0)), lin(0.99), lin(135.0), lin(0.99), 6
+    else:
+        geo, shear, rot, col, post = (lin(150.0 / 331.0 * w), lin(150.0 / 331.0 * h)), lin(0.3), lin(30.0), lin(0.9), 4
+    bits = (8 - (torch.arange(num_bins) / ((num_bins - 1) / post))).round().int().double().numpy()
+    mags = {"Identity": None, "ShearX": shear, "ShearY": shear, "TranslateX": geo[0], "TranslateY": geo[1], "Rotate": rot,
+            "Brightness": col, "Color": col, "Contrast": col, "Sharpness": col, "Posterize": bits, "Solarize": lin(0.0, 1.0),
+            "AutoContrast": None, "Equalize": None}
+    return {k: (mags[k], k in AA_SIGNED) for k in AA_OPS}
+
+
+def inverse_affine_matrix(center, angle, translate, shear):
+    """torchvision's ``_get_inverse_affine_matrix`` (scale 1) in float64, vectorised: arrays of the centre (cx, cy), the angle and the
+    translation (tx, ty), and shear (sx, sy), both angles in degrees.  Returns float64 [n, 6]."""
+    rot, sx, sy = np.radians(angle), np.radians(shear[0]), np.radians(shear[1])
+    (cx, cy), (tx, ty) = center, translate
+    a = np.cos(rot - sy) / np.cos(sy)
+    b = -np.cos(rot - sy) * np.tan(sx) / np.cos(sy) - np.sin(rot)
+    c = np.sin(rot - sy) / np.cos(sy)
+    d = -np.sin(rot - sy) * np.tan(sx) / np.cos(sy) + np.cos(rot)
+    m = [d, -b, np.zeros_like(a), -c, a, np.zeros_like(a)]
+    m[2] = m[2] + m[0] * (-cx - tx) + m[1] * (-cy - ty)
+    m[5] = m[5] + m[3] * (-cx - tx) + m[4] * (-cy - ty)
+    m[2] = m[2] + cx
+    m[5] = m[5] + cy
+    return np.stack(m, -1)
+
+
+def auto_augment_records(n, cfg, rng, out_hw):
+    """The per-image op records of one batch: for every image and op slot (one slot for "trivial_wide", ``num_ops`` for "rand") the
+    op (uniform over the 14), the magnitude bin (uniform, or ``magnitude`` for "rand") and the sign (negative with p = ½, signed ops
+    only), drawn for the whole batch at once whatever the op.  Each record is composed in float64 as torchvision's op computes its
+    parameters and rounded once: op id; the scalar (factor 1 + m, Solarize's threshold 255·m, or Posterize's bits); 1 − factor for
+    the blends; the fp32 inverse affine matrix of ShearX / ShearY (shear degrees(atan m) about (0, 0)), TranslateX / TranslateY
+    (int(m) pixels) and Rotate (about the centre).
+
+    Returns (records float32 [n, slots, 12], op int64 [n, slots], magnitude float64 [n, slots], the signed magnitude each op uses)."""
+    h, w = out_hw
+    space = auto_augment_space(cfg["policy"], cfg["num_magnitude_bins"], out_hw)
+    slots = 1 if cfg["policy"] == "trivial_wide" else cfg["num_ops"]
+    op = rng.integers(0, len(AA_OPS), (n, slots))
+    if cfg["policy"] == "trivial_wide":
+        bins = rng.integers(0, cfg["num_magnitude_bins"], (n, slots))
+    else:
+        bins = np.full((n, slots), cfg["magnitude"])
+    neg = rng.random((n, slots)) <= 0.5
+    table = np.stack([space[k][0] if space[k][0] is not None else np.zeros(cfg["num_magnitude_bins"]) for k in AA_OPS])
+    signed = np.array([space[k][1] for k in AA_OPS])
+    mag = table[op, bins]
+    mag = np.where(signed[op] & neg, -mag, mag)
+    rec = np.zeros((n, slots, AA_RECORD_FLOATS), np.float64)
+    rec[..., 0] = op
+    factor = 1.0 + mag
+    blend = (op >= 6) & (op <= 9)
+    rec[..., 1] = np.where(blend, factor, np.where(op == 10, np.trunc(mag), np.where(op == 11, 255.0 * mag, 0.0)))
+    rec[..., 2] = np.where(blend, 1.0 - factor, 0.0)
+    deg = np.degrees(np.arctan(mag))
+    centre = (np.where(op <= 2, -0.5 * w, 0.0), np.where(op <= 2, -0.5 * h, 0.0))
+    mats = inverse_affine_matrix(centre, np.where(op == 5, -mag, 0.0),
+                                 (np.where(op == 3, np.trunc(mag), 0.0), np.where(op == 4, np.trunc(mag), 0.0)),
+                                 (np.where(op == 1, deg, 0.0), np.where(op == 2, deg, 0.0)))
+    rec[..., 4:10] = np.where(((op >= 1) & (op <= 5))[..., None], mats, 0.0)
+    return rec.astype(np.float32), op, mag
+
+
+RE_KEY = "random_erasing"
+RE_DEFAULTS = {"p": 0.5, "scale": (0.02, 0.33), "ratio": (0.3, 3.3), "seed": 0}
+RE_ATTEMPTS = 10
+
+
+def check_random_erasing(cfg):
+    """The validated ``config['random_erasing']`` with every key filled in (``p`` a float in [0, 1], ``scale`` and ``ratio`` float pairs
+    checked as :func:`check_resized_crop` checks them, an int seed), or None for None; anything else is a ValueError that names the
+    key.  There is no ``value`` key: the box is set to 0 in the normalised output, torchvision's ``RandomErasing(value=0)``."""
+    if cfg is None:
+        return None
+    if not isinstance(cfg, dict):
+        raise ValueError("%s must be a dict or None, not %r" % (RE_KEY, cfg))
+    unknown = sorted(str(k) for k in cfg if k not in RE_DEFAULTS)
+    if unknown:
+        raise ValueError("%s: unknown key %r; the keys are %s" % (RE_KEY, unknown[0], ", ".join(RE_DEFAULTS)))
+    p = cfg.get("p", RE_DEFAULTS["p"])
+    if not _real(p):
+        raise ValueError("%s['p'] must be a finite real number, not %r" % (RE_KEY, p))
+    if not 0.0 <= float(p) <= 1.0:
+        raise ValueError("%s['p'] must lie in [0, 1], not %r" % (RE_KEY, p))
+    out = {"p": float(p)}
+    for k in ("scale", "ratio"):
+        v = cfg.get(k, RE_DEFAULTS[k])
+        if not (isinstance(v, (list, tuple)) and len(v) == 2 and all(_real(e) for e in v)):
+            raise ValueError("%s[%r] must be two finite real numbers [lo, hi], not %r" % (RE_KEY, k, v))
+        lo, hi = float(v[0]), float(v[1])
+        if not (0.0 < lo <= hi and (k == "ratio" or hi <= 1.0)):
+            raise ValueError("%s[%r] must satisfy %s, not %r" % (RE_KEY, k, "0 < lo <= hi <= 1" if k == "scale" else "0 < lo <= hi", v))
+        out[k] = (lo, hi)
+    seed = cfg.get("seed", 0)
+    if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)):
+        raise ValueError("%s['seed'] must be an int, not %r" % (RE_KEY, seed))
+    out["seed"] = int(seed) & (2 ** 64 - 1)
+    return out
+
+
+def random_erasing_rng(cfg, rank):
+    """The erase-box generator of one worker, keyed by (seed, rank, 3): apart from the crop and colour generators, so turning the key
+    on or off changes neither the boxes, nor the fixed crops, nor the colour records drawn."""
+    return np.random.default_rng([cfg["seed"], int(rank), 3])
+
+
+def draw_erase_boxes(n, out_hw, cfg, rng):
+    """Per-image erase boxes (i, j, h, w) (int32 [n, 4]) in output coordinates, drawn as torchvision's ``RandomErasing``: the image
+    is erased when U < p; then up to 10 attempts of area H·W·U(scale) and ratio exp(U(log ratio)), h = round(√(area·r)),
+    w = round(√(area / r)) (round half to even), and the first attempt with h < H and w < W sits at a uniform position.  An image that
+    is not erased, or has no fitting attempt, gets (0, 0, 0, 0).  Every image draws the same count of numbers whatever p, all of the
+    batch at once."""
+    H, W = out_hw
+    lr = np.log(cfg["ratio"])
+    u = rng.random(n)
+    area = (H * W) * rng.uniform(cfg["scale"][0], cfg["scale"][1], (n, RE_ATTEMPTS))
+    r = np.exp(rng.uniform(lr[0], lr[1], (n, RE_ATTEMPTS)))
+    h = np.rint(np.sqrt(area * r)).astype(np.int64)
+    w = np.rint(np.sqrt(area / r)).astype(np.int64)
+    fits = (h < H) & (w < W)
+    first = np.argmax(fits, axis=1)
+    ok = fits[np.arange(n), first] & (u < cfg["p"])
+    h = np.where(ok, h[np.arange(n), first], 0)
+    w = np.where(ok, w[np.arange(n), first], 0)
+    i = np.where(ok, rng.integers(0, H - h + 1), 0)
+    j = np.where(ok, rng.integers(0, W - w + 1), 0)
+    return np.stack([i, j, h, w], 1).astype(np.int32)
+
+
 def crop_and_mirror(data, mode, rand_crop, flag_batch, cropsize, rs=None):
     """Host reference: ``data`` is NHWC float/uint8; returns NHWC ``cropsize²`` crops."""
     n, H, W, C = data.shape

@@ -99,7 +99,8 @@ class ResNet50(ModelBase):
             self.data.para_load_init(self.device, self.input_width, self.input_height, self.rand_crop,
                                      self.batch_crop_mirror, out_dtype=self.act_dtype,
                                      resized_crop=self.resized_crop, rank=self.rank,
-                                     color_jitter=self.color_jitter)
+                                     color_jitter=self.color_jitter, random_erasing=self.random_erasing,
+                                     auto_augment=self.auto_augment)
 
     # ---- construction: every conv is bias-free and linear; BatchNormal carries the ReLU (and the shortcut add)
     def _conv(self, inp, cout, k, stride, pad, input_shape=None):
@@ -192,4 +193,5 @@ class ResNet50Torch(TorchModelBase):
             self.data.para_load_init(self.device, self.input_width, self.input_height, self.rand_crop,
                                      self.batch_crop_mirror, out_dtype=self.act_dtype,
                                      resized_crop=self.resized_crop, rank=self.rank,
-                                     color_jitter=self.color_jitter)
+                                     color_jitter=self.color_jitter, random_erasing=self.random_erasing,
+                                     auto_augment=self.auto_augment)

@@ -61,7 +61,8 @@ class VGG16(ModelBase):
             self.data.para_load_init(self.device, self.input_width, self.input_height, self.rand_crop,
                                      self.batch_crop_mirror, out_dtype=self.act_dtype,
                                      resized_crop=self.resized_crop, rank=self.rank,
-                                     color_jitter=self.color_jitter)
+                                     color_jitter=self.color_jitter, random_erasing=self.random_erasing,
+                                     auto_augment=self.auto_augment)
 
     def build_model(self):
         v, B = self.verbose, self.batch_size

@@ -940,6 +940,107 @@ def color_crop_mirror_normalize(x, mean, std_scale, out_hw, boxes, flips, record
     return out
 
 
+def aa_crop_u8(x, out_hw, boxes, flips, out=None):
+    """auto_augment's uint8 crop (``resized_crop_mirror_norm_kernel<uint8_t>``): uint8 [N, ch, cw, 3], the bilinear resample of each
+    raw box rounded half to even, mirrored where ``flips[n]``.  See :func:`reference.aa_crop_u8`."""
+    x, boxes = _color_inputs("aa_crop_u8", x, boxes)
+    N, H, W, _ = x.shape
+    ch, cw = out_hw
+    if out is None:
+        out = torch.empty((N, ch, cw, 3), dtype=torch.uint8, device=x.device)
+    assert out.dtype == torch.uint8 and out.is_contiguous() and tuple(out.shape) == (N, ch, cw, 3)
+    flips = flips.to(torch.uint8).contiguous()
+    L().aa_crop_u8(x.data_ptr(), out.data_ptr(), boxes.data_ptr(), flips.data_ptr(), N, H, W, ch, cw, _st(x))
+    return out
+
+
+def _aa_records(records, u):
+    assert records.dtype == torch.float32 and records.is_contiguous() and records.dim() == 3 and records.shape[2] == 12
+    assert records.shape[0] == u.shape[0] and records.device == u.device and records.data_ptr() % 16 == 0
+
+
+def aa_lut(u, records, slot, out=None):
+    """The point-op LUTs of one op slot (``aa_lut_kernel``): uint8 [N, 3, 256] for the images whose op in ``slot`` is Brightness,
+    Contrast, Posterize, Solarize, AutoContrast or Equalize, computed from the uint8 crop ``u``; other images' rows are untouched."""
+    _aa_records(records, u)
+    N, ch, cw, _ = u.shape
+    if out is None:
+        out = torch.zeros((N, 3, 256), dtype=torch.uint8, device=u.device)
+    L().aa_lut(u.data_ptr(), records.data_ptr(), out.data_ptr(), int(slot), records.shape[1], N, ch, cw, _st(u))
+    return out
+
+
+def aa_apply(u, records, slot, lut, out=None):
+    """One op slot on the uint8 crop (``aa_apply_kernel``), ``u`` → ``out`` (never in place)."""
+    _aa_records(records, u)
+    N, ch, cw, _ = u.shape
+    if out is None:
+        out = torch.empty_like(u)
+    assert out.data_ptr() != u.data_ptr() and out.shape == u.shape and out.is_contiguous()
+    L().aa_apply(u.data_ptr(), out.data_ptr(), records.data_ptr(), lut.data_ptr(), int(slot), records.shape[1], N, ch, cw, _st(u))
+    return out
+
+
+def aa_normalize(u, mean, std_scale, boxes, flips, in_hw, out_dtype=None, out=None):
+    """(u' − m̂)·std_scale into bf16 / fp32 NHWC (``aa_normalize_kernel``), m̂ the resample of a per-pixel mean over each mirrored box."""
+    out_dtype = out_dtype or ADT()
+    N, ch, cw, C = u.shape
+    H, W = in_hw
+    mean = mean.float().contiguous()
+    mode = 0 if mean.numel() == 1 else (1 if mean.numel() == C else 2)
+    if mode == 2:
+        assert mean.numel() == H * W * C
+    if out is None:
+        out = torch.empty((N, ch, cw, C), dtype=out_dtype, device=u.device)
+    assert out.dtype in (BF16, torch.float32) and out.is_contiguous() and tuple(out.shape) == (N, ch, cw, C)
+    boxes = boxes.to(torch.int32).contiguous()
+    assert tuple(boxes.shape) == (N, 4) and boxes.data_ptr() % 16 == 0
+    flips = flips.to(torch.uint8).contiguous()
+    if isinstance(std_scale, torch.Tensor):
+        cs = std_scale.to(device=u.device, dtype=torch.float32).contiguous()
+        sc, cs_ptr = 1.0, cs.data_ptr()
+    else:
+        sc, cs_ptr = float(std_scale), 0
+    L().aa_normalize(u.data_ptr(), mean.data_ptr(), mode, sc, cs_ptr, out.data_ptr(), int(out.dtype == BF16), boxes.data_ptr(),
+                     flips.data_ptr(), N, W, ch, cw, _st(u))
+    return out
+
+
+def auto_augment_crop_normalize(x, mean, std_scale, out_hw, boxes, flips, records, ops=None, out_dtype=None, out=None, ping=None,
+                                pong=None, lut=None):
+    """TrivialAugmentWide / RandAugment on the crop, then normalisation: :func:`aa_crop_u8` into ``ping``; per op slot
+    :func:`aa_lut` (only when an image's op in the slot is a point op; ``ops`` = the host's int [N, slots] op ids, read from
+    ``records`` when None) and :func:`aa_apply` ping → pong, swapping; then :func:`aa_normalize`.  Launches:
+    1 + Σ over slots of (1 if a point op is drawn, + 1) + 1.  See :func:`reference.auto_augment_crop_normalize`."""
+    from ..models.data.utils import AA_LUT_OPS
+    N, H, W, _ = x.shape
+    ch, cw = out_hw
+    if ops is None:
+        ops = records[..., 0].to("cpu", torch.int64).numpy()
+    ping = aa_crop_u8(x, out_hw, boxes, flips, out=ping)
+    pong = pong if pong is not None else torch.empty_like(ping)
+    lut = lut if lut is not None else torch.empty((N, 3, 256), dtype=torch.uint8, device=x.device)
+    for slot in range(records.shape[1]):
+        if any(int(o) in AA_LUT_OPS for o in ops[:, slot]):
+            aa_lut(ping, records, slot, out=lut)
+        aa_apply(ping, records, slot, lut, out=pong)
+        ping, pong = pong, ping
+    return aa_normalize(ping, mean, std_scale, boxes, flips, (H, W), out_dtype, out=out)
+
+
+def random_erase(x, boxes):
+    """Random erasing in place (``nn_kernels.cu: erase_boxes_kernel``): every element of image n's box ``boxes[n] = (i, j, h, w)``
+    (int32 [N, 4] on the device, 16-byte aligned, inside the output; h = w = 0 erases nothing) of the bf16 or fp32 NHWC batch ``x``
+    is set to 0; nothing else is touched.  One launch.  Returns ``x``.  See :func:`reference.random_erase`."""
+    if not (x.is_cuda and x.dtype in (BF16, torch.float32) and x.dim() == 4 and x.is_contiguous()):
+        raise ValueError("random_erase takes a contiguous bf16 or fp32 NHWC batch on the device, not %s %s" % (x.dtype, tuple(x.shape)))
+    N, ch, cw, C = x.shape
+    assert boxes.dtype == torch.int32 and boxes.is_contiguous() and tuple(boxes.shape) == (N, 4)
+    assert boxes.device == x.device and boxes.data_ptr() % 16 == 0
+    L().erase_boxes(x.data_ptr(), int(x.dtype == BF16), boxes.data_ptr(), N, ch, cw, C, _st(x))
+    return x
+
+
 # --------------------------------------------------------------------------- optimizer
 def _table(arena):
     if not hasattr(arena, "_tab_cache"):

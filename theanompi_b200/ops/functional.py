@@ -584,3 +584,21 @@ def resized_crop_mirror_normalize(x, mean, std_scale, out_hw, boxes, flips, out_
         from . import cuda_impl
         return cuda_impl.resized_crop_mirror_normalize(x, mean, std_scale, out_hw, boxes, flips, out_dtype)
     return ref.resized_crop_mirror_normalize(x, mean, std_scale, out_hw, boxes, flips, out_dtype or torch.float32)
+
+
+def random_erase(x, boxes):
+    """Random erasing of a normalised NHWC batch: the native kernel in place on CUDA (``boxes`` int32 on the device), a copy from
+    :func:`reference.random_erase` on the CPU."""
+    if x.is_cuda:
+        from . import cuda_impl
+        return cuda_impl.random_erase(x, boxes)
+    return ref.random_erase(x, boxes)
+
+
+def auto_augment_crop_normalize(x, mean, std_scale, out_hw, boxes, flips, records, out_dtype=None):
+    """TrivialAugmentWide / RandAugment on the crop of a uint8 NHWC batch, then normalisation: the native kernels on CUDA,
+    :func:`reference.auto_augment_crop_normalize` on the CPU."""
+    if x.is_cuda:
+        from . import cuda_impl
+        return cuda_impl.auto_augment_crop_normalize(x, mean, std_scale, out_hw, boxes, flips, records, out_dtype=out_dtype)
+    return ref.auto_augment_crop_normalize(x, mean, std_scale, out_hw, boxes, flips, records, out_dtype or torch.float32)

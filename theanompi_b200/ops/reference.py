@@ -728,6 +728,138 @@ def color_crop_mirror_normalize(x_u8, mean, std_scale, out_hw, boxes, flips, rec
     return out.to(out_dtype)
 
 
+def aa_crop_u8(x_u8, out_hw, boxes, flips):
+    """auto_augment's uint8 crop: image i's raw box ``boxes[i] = (y0, x0, h, w)`` resampled to ``out_hw`` (``F.interpolate``, bilinear,
+    ``align_corners=False``, no antialias), rounded half to even to uint8 and mirrored where ``flips[i]``.  Returns uint8 [N, ch, cw, C]."""
+    import torch.nn.functional as F
+    N, H, W, C = x_u8.shape
+    out = torch.empty((N,) + tuple(out_hw) + (C,), dtype=torch.uint8, device=x_u8.device)
+    for i in range(N):
+        y0, x0, h, w = (int(v) for v in boxes[i])
+        if not (h > 0 and w > 0 and 0 <= y0 <= H - h and 0 <= x0 <= W - w):
+            raise ValueError("aa_crop_u8: box %r of image %d is not inside %d x %d" % ((y0, x0, h, w), i, H, W))
+        box = x_u8[i, y0:y0 + h, x0:x0 + w, :].float().permute(2, 0, 1).unsqueeze(0)
+        v = F.interpolate(box, size=tuple(out_hw), mode="bilinear", align_corners=False, antialias=False)[0].permute(1, 2, 0)
+        v = v.round().to(torch.uint8)
+        out[i] = v.flip(1) if bool(flips[i]) else v
+    return out
+
+
+def _aa_blend(img, other, f, d):
+    return img.mul(f).add_(other, alpha=d).clamp_(0, 255).to(torch.uint8)
+
+
+def _aa_gray(img):
+    r, g, b = img.unbind(0)
+    return r.mul(0.2989).add_(g, alpha=0.587).add_(b, alpha=0.114).floor_().unsqueeze(0)
+
+
+def aa_apply_op(img, rec):
+    """One op of TrivialAugmentWide / RandAugment on a uint8 CHW image (C = 3), as ``torchvision.transforms.v2.functional`` computes it
+    (nearest interpolation, fill 0), from its 12-float record (``models/data/utils.py: auto_augment_records``): op id, scalar (factor,
+    Solarize threshold or Posterize bits), 1 − factor, 0, the fp32 inverse affine matrix."""
+    import torch.nn.functional as F
+    rec = [float(v) for v in rec]
+    op, f, d = int(rec[0]), rec[1], rec[2]
+    C, h, w = img.shape
+    if op == 0:
+        return img.clone()
+    if 1 <= op <= 5:                                          # torchvision's _affine_grid and grid_sample(nearest, zeros)
+        theta = torch.tensor(rec[4:10], dtype=torch.float32).reshape(1, 2, 3)
+        base = torch.empty(1, h, w, 3, dtype=torch.float32)
+        base[..., 0].copy_(torch.linspace((1.0 - w) * 0.5, (w - 1.0) * 0.5, steps=w))
+        base[..., 1].copy_(torch.linspace((1.0 - h) * 0.5, (h - 1.0) * 0.5, steps=h).unsqueeze_(-1))
+        base[..., 2].fill_(1)
+        rescaled = theta.transpose(1, 2).div_(torch.tensor([0.5 * w, 0.5 * h], dtype=torch.float32))
+        grid = base.view(1, h * w, 3).bmm(rescaled).view(1, h, w, 2)
+        out = F.grid_sample(img.float().unsqueeze(0), grid, mode="nearest", padding_mode="zeros", align_corners=False)
+        return out[0].round_().to(torch.uint8)
+    if op == 6:
+        return img.mul(f).clamp_(0, 255).to(torch.uint8)
+    if op == 7:
+        return _aa_blend(img, _aa_gray(img), f, d)
+    if op == 8:
+        return _aa_blend(img, torch.mean(_aa_gray(img), dim=(-3, -2, -1), keepdim=True), f, d)
+    if op == 9:
+        if h <= 2 or w <= 2:
+            return img.clone()
+        a, b = 1.0 / 13.0, 5.0 / 13.0
+        kernel = torch.tensor([[a, a, a], [a, b, a], [a, a, a]], dtype=torch.float32).expand(C, 1, 3, 3)
+        out = img.to(torch.float32, copy=True)
+        blurred = F.conv2d(out.unsqueeze(0), kernel, groups=C)[0].round_()
+        view = out[..., 1:-1, 1:-1]
+        view.add_(blurred.sub_(view), alpha=d)
+        return out.clamp_(0, 255).to(torch.uint8)
+    if op == 10:
+        bits = int(f)
+        return img.clone() if bits >= 8 else img & (((1 << bits) - 1) << (8 - bits))
+    if op == 11:
+        return torch.where(img >= f, 255 - img, img)
+    if op == 12:
+        fimg = img.to(torch.float32)
+        lo = fimg.amin(dim=(-2, -1), keepdim=True)
+        hi = fimg.amax(dim=(-2, -1), keepdim=True)
+        eq = hi == lo
+        inv = hi.sub_(lo).mul_(1.0 / 255)
+        lo[eq] = 0.0
+        inv[eq] = 1.0
+        return fimg.sub_(lo).div_(inv).clamp_(0, 255).to(torch.uint8)
+    if op == 13:                                              # PIL's equalize LUT, per channel; step == 0 leaves the channel as it is
+        flat = img.flatten(start_dim=-2).to(torch.long)
+        hist = torch.zeros((C, 256), dtype=torch.int32).scatter_add_(-1, flat, torch.ones_like(flat, dtype=torch.int32))
+        cum = hist.cumsum(-1)
+        last = cum.argmax(-1, keepdim=True)
+        step = (flat.shape[-1] - hist.gather(-1, last)).div(255, rounding_mode="floor")
+        lut = (cum[:, :-1] + step // 2).div(step.clamp(min=1), rounding_mode="floor").clamp_(0, 255).to(torch.uint8)
+        lut = torch.cat([torch.zeros((C, 1), dtype=torch.uint8), lut], -1)
+        eqd = lut.gather(-1, flat).view_as(img)
+        return torch.where(step.ne(0).view(C, 1, 1), eqd, img)
+    raise ValueError("aa_apply_op: unknown op %d" % op)
+
+
+def auto_augment_crop_normalize(x_u8, mean, std_scale, out_hw, boxes, flips, records, out_dtype=torch.float32):
+    """TrivialAugmentWide / RandAugment on the (resized) crop, then normalisation: u = :func:`aa_crop_u8`; each op slot of
+    ``records[i]`` (float32 [N, slots, 12]) applied in order by :func:`aa_apply_op`; out = (u' − m̂) * std_scale with m̂ the bilinear
+    resample of a per-pixel mean over the same (mirrored) box (a [C] or scalar mean as it is).  Fill pixels become −m̂ * std_scale."""
+    import torch.nn.functional as F
+    N, H, W, C = x_u8.shape
+    if isinstance(std_scale, torch.Tensor):
+        std_scale = std_scale.to(dtype=torch.float32)
+    mean = torch.as_tensor(mean).float()
+    rec = torch.as_tensor(records).float().cpu()
+    u = aa_crop_u8(x_u8.cpu(), out_hw, boxes, flips)
+    out = torch.empty((N,) + tuple(out_hw) + (C,), dtype=torch.float32)
+    for i in range(N):
+        img = u[i].permute(2, 0, 1).contiguous()
+        for r in rec[i]:
+            img = aa_apply_op(img, r)
+        if mean.dim() == 3:
+            y0, x0, h, w = (int(v) for v in boxes[i])
+            box = mean.cpu()[y0:y0 + h, x0:x0 + w, :].permute(2, 0, 1).unsqueeze(0)
+            m = F.interpolate(box, size=tuple(out_hw), mode="bilinear", align_corners=False, antialias=False)[0].permute(1, 2, 0)
+            m = m.flip(1) if bool(flips[i]) else m
+        else:
+            m = mean.cpu()
+        out[i] = (img.permute(1, 2, 0).float() - m) * (std_scale.cpu() if isinstance(std_scale, torch.Tensor) else std_scale)
+    return out.to(device=x_u8.device, dtype=out_dtype)
+
+
+def random_erase(x, boxes):
+    """torchvision's ``RandomErasing(value=0)`` on an NHWC batch, given its boxes: a copy of ``x`` with every element of image i's box
+    ``boxes[i] = (i0, j0, h, w)`` (output coordinates, inside the image; h = w = 0 erases nothing) set to 0.
+
+    x: [N, H, W, C] float;  boxes: [N, 4] int (``models/data/utils.py: draw_erase_boxes``)
+    """
+    N, H, W, _ = x.shape
+    out = x.clone()
+    for n in range(N):
+        i, j, h, w = (int(v) for v in boxes[n])
+        if not (h >= 0 and w >= 0 and 0 <= i <= H - h and 0 <= j <= W - w):
+            raise ValueError("random_erase: box %r of image %d is not inside %d x %d" % ((i, j, h, w), n, H, W))
+        out[n, i:i + h, j:j + w, :] = 0
+    return out
+
+
 # --------------------------------------------------------------------------- batch norm (+ residual)(+ ReLU), NHWC
 def _per_sample(s, x):
     """A drop-path row (one scale per sample of x's leading axis) shaped to broadcast over x."""
