@@ -139,6 +139,10 @@ void softmax_xent_mix(const void* logits, const void* labels, const void* rec, v
 // keep_scale[l] = fp32(1 / (1 − p_l)); thresh[l] = ⌈p_l·2^24⌉ (uint32), key (seed, rank)
 void drop_path_draw(const void* thresh, const void* keep_scale, int L, int B, unsigned long long seed, int rank, const void* step, void* out,
                     cudaStream_t st);
+// cifar_augment draw (ops/cifar_augment.py owns the layout) of step counter *step, key (seed, rank): offs int32 [B, 2] (oy − pad,
+// ox − pad), flips uint8 [B], boxes int32 [B, 4] Cutout (i, j, h, w) of side L in an H × W image (16-byte aligned)
+void cifar_augment_draw(int B, int pad, int L, int H, int W, unsigned long long seed, int rank, const void* step, void* offs, void* flips,
+                        void* boxes, cudaStream_t st);
 // act: 0 none, 1 ReLU, 2 leaky ReLU (negative slope `slope`), 3 sigmoid (ACT_* in common.cuh).  accumulate = 1: db / db1 += the bias
 // gradient (no clear)
 void relu_bias_bwd(const void* dy, const void* y, void* dym, void* db, void* db1, int c_split, long long R, int C, long long ld, int act,
@@ -158,8 +162,9 @@ void im2col(const void* x, void* col, int N, int H, int W, int Ctot, int c_off, 
 void col2im(const void* dcol, void* dx, int N, int H, int W, int Ctot, int c_off, int Cg, int KH, int KW, int Ho, int Wo, int s, int p,
             long long ldcol, int f32, cudaStream_t st);
 void pad_rows(const void* src, void* dst, long long rows, int cols, long long src_ld, long long dst_ld, int f32, cudaStream_t st);
+// zero_fill = 1: offsets may put a source pixel outside the image, which then stores 0 in every channel (else the crop stays inside)
 void crop_mirror_norm(const void* x, int in_kind, const void* mean, int mean_mode, float scale, const void* cscale, void* out, int out_bf16, const void* offs,
-                      const void* flips, int N, int H, int W, int C, int ch, int cw, int Cout, cudaStream_t st);
+                      const void* flips, int N, int H, int W, int C, int ch, int cw, int Cout, int zero_fill, cudaStream_t st);
 // random-resized crop: uint8 NHWC x → bilinear resample of the normalised box boxes[n] = (y0, x0, h, w) (int32 [N, 4], 16-byte
 // aligned, inside the H × W image) to ch × cw, mirrored after the resize where flips[n]; out bf16 (out_bf16) or fp32 NHWC
 void resized_crop_mirror_norm(const void* x, const void* mean, int mean_mode, float scale, const void* cscale, void* out, int out_bf16,

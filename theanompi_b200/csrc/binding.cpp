@@ -133,8 +133,9 @@ PYBIND11_MODULE(_tmpi_native, m) {
   m.def("pad_rows", [](ptr_t src, ptr_t dst, long long rows, int cols, long long src_ld, long long dst_ld, int f32, ptr_t st) {
     pad_rows(P(src), P(dst), rows, cols, src_ld, dst_ld, f32, S(st)); });
   m.def("crop_mirror_norm", [](ptr_t x, int in_kind, ptr_t mean, int mean_mode, float scale, ptr_t cscale, ptr_t out, int out_bf16, ptr_t offs,
-                               ptr_t flips, int N, int H, int W, int C, int ch, int cw, int Cout, ptr_t st) {
-    crop_mirror_norm(P(x), in_kind, P(mean), mean_mode, scale, P(cscale), P(out), out_bf16, P(offs), P(flips), N, H, W, C, ch, cw, Cout, S(st)); });
+                               ptr_t flips, int N, int H, int W, int C, int ch, int cw, int Cout, int zero_fill, ptr_t st) {
+    crop_mirror_norm(P(x), in_kind, P(mean), mean_mode, scale, P(cscale), P(out), out_bf16, P(offs), P(flips), N, H, W, C, ch, cw, Cout, zero_fill,
+                     S(st)); });
   m.def("resized_crop_mirror_norm", [](ptr_t x, ptr_t mean, int mean_mode, float scale, ptr_t cscale, ptr_t out, int out_bf16, ptr_t boxes,
                                        ptr_t flips, int N, int H, int W, int C, int ch, int cw, ptr_t st) {
     resized_crop_mirror_norm(P(x), P(mean), mean_mode, scale, P(cscale), P(out), out_bf16, P(boxes), P(flips), N, H, W, C, ch, cw, S(st)); });
@@ -170,6 +171,9 @@ PYBIND11_MODULE(_tmpi_native, m) {
     add_scaled(P(a), P(b), P(scale), P(y), n, batch, f32, S(st)); });
   m.def("drop_path_draw", [](ptr_t thresh, ptr_t keep_scale, int L, int B, unsigned long long seed, int rank, ptr_t step, ptr_t out, ptr_t st) {
     drop_path_draw(P(thresh), P(keep_scale), L, B, seed, rank, P(step), P(out), S(st)); });
+  m.def("cifar_augment_draw", [](int B, int pad, int L, int H, int W, unsigned long long seed, int rank, ptr_t step, ptr_t offs, ptr_t flips,
+                                 ptr_t boxes, ptr_t st) {
+    cifar_augment_draw(B, pad, L, H, W, seed, rank, P(step), P(offs), P(flips), P(boxes), S(st)); });
   m.def("add4_tensors", [](ptr_t a, ptr_t b, ptr_t c, ptr_t d, ptr_t y, long long n, int f32, ptr_t st) {
     add4_tensors(P(a), P(b), P(c), P(d), P(y), n, f32, S(st)); });
   m.def("add_tensors", [](ptr_t a, ptr_t b, ptr_t y, long long n, int f32, ptr_t st) { add_tensors(P(a), P(b), P(y), n, f32, S(st)); });

@@ -759,6 +759,46 @@ void drop_path_draw(const void* thresh, const void* keep_scale, int L, int B, un
   count_launch(); TMPI_CHECK_LAUNCH("drop_path_draw"); ::tmpi::check_capture(st, "drop_path_draw");
 }
 
+// ============================================================================ CIFAR augmentation draw (cifar_augment)
+// Image n's pad-and-crop offsets, flip and Cutout box of one step (ops/cifar_augment.py owns the layout; ops/reference.py:
+// cifar_augment_draw is the same on the host).  Philox4x32-10 with key (seed_lo, seed_hi ^ rank): block 0 has counter
+// (n, kCifarAugTag, step_lo, step_hi), block 1 (n, kCifarAugTag + 1, ...).  Each value is ⌊w·k / 2^32⌋: oy, ox ∈ [0, 2·pad] from
+// block 0 words 0 and 1, flip = word 2 >> 31, Cutout centre cy ∈ [0, H) from word 3 and cx ∈ [0, W) from block 1 word 0.  The tag
+// is neither dropout's / uniform_noise's second word (at most 0x7FFFFFFF), nor the mix draw's 0xFFFFFFFF, nor in drop-path's
+// [0xC0000000, 0xC000FFFF], so no block of another stream is ever one of these.
+// offs[n] = (oy − pad, ox − pad); box[n] = (y1, x1, y2 − y1, x2 − x1) with y1 = clamp(cy − L/2, 0, H), y2 = clamp(cy + L/2, 0, H)
+// and the same for x (DeVries & Taylor's Cutout: an odd L cuts an (L − 1)-wide hole).
+constexpr uint32_t kCifarAugTag = 0xA0000000u;
+
+__global__ void cifar_augment_draw_kernel(int B, int pad, int L, int H, int W, unsigned long long seed, uint32_t rank,
+                                          const unsigned long long* __restrict__ step, int2* __restrict__ offs,
+                                          uint8_t* __restrict__ flips, int4* __restrict__ boxes) {
+  const int n = blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= B) return;
+  const unsigned long long s = *step;
+  const uint32_t s_lo = (uint32_t)s, s_hi = (uint32_t)(s >> 32), k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32) ^ rank;
+  uint32_t a[4], b[4];
+  philox4x32((uint32_t)n, kCifarAugTag, s_lo, s_hi, k0, k1, a);
+  philox4x32((uint32_t)n, kCifarAugTag + 1u, s_lo, s_hi, k0, k1, b);
+  const unsigned k = 2u * (unsigned)pad + 1u;
+  const int oy = (int)(((unsigned long long)a[0] * k) >> 32), ox = (int)(((unsigned long long)a[1] * k) >> 32);
+  const int cy = (int)(((unsigned long long)a[3] * (unsigned)H) >> 32), cx = (int)(((unsigned long long)b[0] * (unsigned)W) >> 32);
+  const int y1 = min(max(cy - L / 2, 0), H), y2 = min(max(cy + L / 2, 0), H);
+  const int x1 = min(max(cx - L / 2, 0), W), x2 = min(max(cx + L / 2, 0), W);
+  offs[n] = make_int2(oy - pad, ox - pad);
+  flips[n] = (uint8_t)(a[2] >> 31);
+  boxes[n] = make_int4(y1, x1, y2 - y1, x2 - x1);
+}
+
+void cifar_augment_draw(int B, int pad, int L, int H, int W, unsigned long long seed, int rank, const void* step, void* offs, void* flips,
+                        void* boxes, cudaStream_t st) {
+  if (B < 1 || H < 1 || W < 1 || pad < 0 || pad >= H || pad >= W || L < 0 || L > H || L > W)
+    throw std::runtime_error("cifar_augment_draw: needs B >= 1, 0 <= pad < H, W and 0 <= cutout <= H, W");
+  cifar_augment_draw_kernel<<<grid_for(B, 128), 128, 0, st>>>(B, pad, L, H, W, seed, (uint32_t)rank, (const unsigned long long*)step,
+                                                              (int2*)offs, (uint8_t*)flips, (int4*)boxes);
+  count_launch(); TMPI_CHECK_LAUNCH("cifar_augment_draw"); ::tmpi::check_capture(st, "cifar_augment_draw");
+}
+
 // One thread per element position of a pair (i, j = B − 1 − i), blockIdx.y = i: it reads both rows and writes both, so the mix is
 // in place.  kVec: N-element 16-byte vectors (the row length n = H·W·C times sizeof(T) is a multiple of 16), else one element.  The
 // grid is sized for Mixup; CutMix CTAs whose elements lie outside the box rows return before touching the batch.
@@ -1530,7 +1570,9 @@ void s2d_filter(const void* src, void* dst, int O, int KH, int KW, int C, int S,
 // math (coalesced stores; loads are contiguous runs of the source row, reversed when mirrored).
 // grid = (N * ch, ceil(cw / 128)): the output row (n, oy) comes from blockIdx.x, the pixel from blockIdx.y / threadIdx.x — no
 // per-thread divisions (the one-thread-per-pixel version with 64-bit div/mod was issue-bound: 230 instructions per pixel).
-template <typename Tin, typename Tout>
+// kZeroFill: the offsets may put (sy, sx) outside the image (the zero-padded random crop of cifar_augment); such a pixel is 0 in
+// every output channel, i.e. the mean pixel of the normalised image.  Without it the offsets must keep the crop inside the image.
+template <typename Tin, typename Tout, bool kZeroFill = false>
 __global__ void __launch_bounds__(128) crop_mirror_norm_kernel(const Tin* __restrict__ x, const float* __restrict__ mean, int mean_mode,
                                         float scale, const float* __restrict__ cscale, Tout* __restrict__ out, const int* __restrict__ offs,
                                         const uint8_t* __restrict__ flips, int N, int H, int W, int C, int ch, int cw, int Cout) {
@@ -1539,6 +1581,13 @@ __global__ void __launch_bounds__(128) crop_mirror_norm_kernel(const Tin* __rest
   const int oy = blockIdx.x % ch, n = blockIdx.x / ch;
   const int sy = offs[2 * n] + oy;
   const int sx = offs[2 * n + 1] + (flips[n] ? (cw - 1 - ox) : ox);
+  if constexpr (kZeroFill) {
+    if ((unsigned)sy >= (unsigned)H || (unsigned)sx >= (unsigned)W) {
+      Tout* z = out + ((long long)blockIdx.x * cw + ox) * Cout;
+      for (int c = 0; c < Cout; ++c) z[c] = (Tout)0.f;
+      return;
+    }
+  }
   const unsigned pix = (unsigned)(sy * W + sx) * (unsigned)C;          // inside one image (host checks H*W*C < 2^31)
   const Tin* src = x + (long long)n * H * W * C + pix;
   const float* mp = mean_mode == 2 ? mean + pix : mean;
@@ -1562,11 +1611,13 @@ __global__ void __launch_bounds__(128) crop_mirror_norm_kernel(const Tin* __rest
 }
 
 void crop_mirror_norm(const void* x, int in_kind /*0 u8, 1 bf16, 2 f32*/, const void* mean, int mean_mode, float scale, const void* cscale, void* out,
-                      int out_bf16, const void* offs, const void* flips, int N, int H, int W, int C, int ch, int cw, int Cout, cudaStream_t st) {
+                      int out_bf16, const void* offs, const void* flips, int N, int H, int W, int C, int ch, int cw, int Cout, int zero_fill,
+                      cudaStream_t st) {
   if ((long long)H * W * C >= (1LL << 31) || (long long)N * ch >= (1LL << 31)) throw std::runtime_error("crop_mirror_norm: image too large");
   const dim3 g((unsigned)(N * ch), (unsigned)((cw + 127) / 128));
   auto M = (const float*)mean; auto O = (const int*)offs; auto F = (const uint8_t*)flips;
-#define CMN(TI, TO) crop_mirror_norm_kernel<TI, TO><<<g, 128, 0, st>>>((const TI*)x, M, mean_mode, scale, (const float*)cscale, (TO*)out, O, F, N, H, W, C, ch, cw, Cout)
+#define CMN(TI, TO) (zero_fill ? crop_mirror_norm_kernel<TI, TO, true> : crop_mirror_norm_kernel<TI, TO, false>)<<<g, 128, 0, st>>>( \
+      (const TI*)x, M, mean_mode, scale, (const float*)cscale, (TO*)out, O, F, N, H, W, C, ch, cw, Cout)
   if (in_kind == 0) { if (out_bf16) CMN(uint8_t, __nv_bfloat16); else CMN(uint8_t, float); }
   else if (in_kind == 1) { if (out_bf16) CMN(__nv_bfloat16, __nv_bfloat16); else CMN(__nv_bfloat16, float); }
   else { if (out_bf16) CMN(float, __nv_bfloat16); else CMN(float, float); }

@@ -21,6 +21,7 @@ needs re-capture; costs/errors stay on the device until the recorder prints.
 """
 from __future__ import annotations
 
+import gc
 import math
 import time
 
@@ -69,6 +70,7 @@ class ModelBase(object):
     supports_label_smoothing = True    # config['label_smoothing'] > 0 (False: no classifier head; refused at compile_iter_fns)
     supports_mixup = True          # config['mixup'] (False: no image batch before a first convolution; refused at compile_iter_fns)
     supports_drop_path = False     # config['drop_path_rate'] > 0 (True: residual blocks in self.body that read drop_row(l))
+    supports_cifar_augment = False  # config['cifar_augment'] (True: a CIFAR model whose training forward reads train_augment())
     # True: an ImageNet model fed by ParaLoader, so config['random_resized_crop'], config['color_jitter'] and
     # config['random_erasing'] reach its loader
     # (refused at construction otherwise)
@@ -132,6 +134,12 @@ class ModelBase(object):
         self.drop_path_rate = config.get("drop_path_rate", 0.0)
         self.drop_path = None
         self._drop_on = False
+        # pad-and-crop, flip and Cutout of the CIFAR training batch (a dict, ops/cifar_augment.py; None = off): one draw per training
+        # step on the device, applied by the model's normalising crop.  Built by check_cifar_augment; read through train_augment only
+        # during the training forward
+        self.cifar_augment = config.get("cifar_augment")
+        self.cifar_aug = None
+        self._aug_on = False
         # random-resized crop of the training images (a dict, models/data/utils.py: check_resized_crop; None = off): per-image boxes
         # drawn by the loader and resampled by its kernel on the copy stream.  Checked here because the model's constructor builds
         # the loader; the training step never sees it
@@ -223,6 +231,8 @@ class ModelBase(object):
         # with config['mixup'] the step's draw comes first, keyed by the device step counter, so every graph replay draws anew
         # with config['drop_path_rate'] the table is drawn next (after the mix draw) from the same counter, and only this forward reads
         # it: validation and inference never drop
+        # with config['cifar_augment'] the offsets, flips and Cutout boxes are drawn last, from the same counter, and likewise only this
+        # forward reads them
         rec = None
         if self.mixer is not None:
             rec = self.mixer.draw()
@@ -230,6 +240,9 @@ class ModelBase(object):
         if self.drop_path is not None:
             self.drop_path.draw()
             self._drop_on = True
+        if self.cifar_aug is not None:
+            self.cifar_aug.draw()
+            self._aug_on = True
         try:
             if rec is None:
                 cost, err, err5 = self.loss(self.x_in, self.y_in, self.label_smoothing)
@@ -237,6 +250,7 @@ class ModelBase(object):
                 cost, err, err5 = self.loss(self.x_in, self.y_in, self.label_smoothing, mix=rec)
         finally:
             self._drop_on = False
+            self._aug_on = False
         self._dbg_capture("forward")
         cost.backward()
         return cost.detach(), err.detach()
@@ -351,6 +365,25 @@ class ModelBase(object):
             raise ValueError("%s: mixup is not supported; it mixes the image batch of AlexNet, GoogLeNet, Cifar10_model, VGG16, "
                              "ResNet50 and Wide_ResNet" % self.name)
         self.mixer = Mixer(cfg, self.rank, self.mix_hw, self.device)
+
+    # ------------------------------------------------------------------ CIFAR augmentation
+    def check_cifar_augment(self):
+        """``config['cifar_augment']`` must be None or a valid dict (ops/cifar_augment.py: check_config; a ValueError names the key),
+        and a dict needs a model that applies it (``supports_cifar_augment``); builds the step's :class:`CifarAugment`."""
+        from ..ops.cifar_augment import KEY, CifarAugment, check_config
+        self.cifar_aug = None
+        cfg = check_config(self.cifar_augment)
+        if cfg is None:
+            return
+        if not self.supports_cifar_augment:
+            raise ValueError("%s: %s is not supported; it augments the CIFAR-10 batch of Wide_ResNet inside its normalising crop"
+                             % (self.name, KEY))
+        self.cifar_aug = CifarAugment(cfg, self.rank, self.batch_size, self.device)
+
+    def train_augment(self):
+        """This training step's :class:`CifarAugment` (its offsets, flips and Cutout boxes already drawn), or None: outside the
+        training forward or without cifar_augment."""
+        return self.cifar_aug if self._aug_on else None
 
     # ------------------------------------------------------------------ random-resized crop
     def check_resized_crop(self, cfg):
@@ -500,6 +533,11 @@ class ModelBase(object):
                 cur.wait_stream(s)
                 return out
             g, inner, why = torch.cuda.CUDAGraph(), None, ""
+            # No automatic garbage collection while capturing: a collection could finalise an unreachable model (a reference
+            # cycle) whose CUDA graph, events or pinned buffers are released by calls a capturing thread must not make, which
+            # invalidates the capture.  The garbage is collected after it.
+            gc_on = gc.isenabled()
+            gc.disable()
             try:
                 with torch.cuda.stream(s), torch.cuda.graph(g, pool=self._graph_pool, stream=s, capture_error_mode="thread_local"):
                     try:
@@ -512,6 +550,9 @@ class ModelBase(object):
                 if not self._graph_auto or not isinstance(err, Exception):
                     raise err
                 why = "%s: %s" % (type(err).__name__, str(err)[:200])
+            finally:
+                if gc_on:
+                    gc.enable()
             cur.wait_stream(s)
             ex = self.exchanger
             fused = ex is not None and getattr(ex, "fused", False)
@@ -601,11 +642,12 @@ class ModelBase(object):
     def setup_train_options(self, k=1, fused_tail=None, optimizer=None):
         """Check and build the training options of the config for a step of ``k`` workers (k > 1: BSP ``sync_type='cdd'``),
         ``fused_tail`` (a fused exchange strategy's step tail, or None) and ``optimizer`` (default: the model's): grad_accum,
-        label_smoothing, mixup, drop_path_rate, lr_schedule and grad_clip.  A model refuses every option it does not support here,
-        with a ValueError that names it."""
+        label_smoothing, mixup, cifar_augment, drop_path_rate, lr_schedule and grad_clip.  A model refuses every option it does not
+        support here, with a ValueError that names it."""
         self.check_grad_accum(fused_tail)
         self.check_label_smoothing()
         self.check_mixup()
+        self.check_cifar_augment()
         self.check_drop_path()
         self.setup_lr_schedule()
         opt = self.optimizer if optimizer is None else optimizer

@@ -58,6 +58,7 @@ class WRN(nn.Module):
 
 class Wide_ResNet(ModelBase):
     supports_drop_path = True      # one drop-path block per pre-activation block
+    supports_cifar_augment = True  # pad-and-crop, flip and Cutout in the normalising crop of the training forward
     n_epochs, batch_size, file_batch_size, learning_rate = n_epochs, batch_size, file_batch_size, learning_rate
     weight_decay, momentum = 0.0, 0.9
     bias_lr_mult = 1.0             # Adam: one learning rate for every parameter
@@ -125,15 +126,34 @@ class Wide_ResNet(ModelBase):
         self.head = (bn, gap, flat, sm)
         self.output_layer = sm
 
+    def mix_input(self, rec):
+        """With cifar_augment the forward that follows mixes the augmented, normalised batch (timm's order: per-sample transforms,
+        then the batch mix); without it x_in is mixed here, before the normalisation."""
+        if self.cifar_aug is None:
+            return super().mix_input(rec)
+        self._mix_rec = rec
+
     def forward(self, x):
         from ... import ops
-        if x.is_cuda:
-            # (x − mean) / 64 → activation dtype in ONE native kernel (the loader's normalise kernel with a full-image crop)
-            if getattr(self, "_zero_off", None) is None or self._zero_off.shape[0] != x.shape[0]:
-                self._zero_off = torch.zeros((x.shape[0], 2), dtype=torch.int32, device=x.device)
-                self._zero_flip = torch.zeros((x.shape[0],), dtype=torch.uint8, device=x.device)
+        aug = self.train_augment()                               # this training step's cifar_augment draw, else None
+        rec, self._mix_rec = getattr(self, "_mix_rec", None), None
+        if x.is_cuda or aug is not None:
+            # (x − mean) / 64 → activation dtype in ONE native kernel (the loader's normalise kernel with a full-image crop, or with
+            # cifar_augment the zero-filled pad-and-crop and flip of the draw)
+            if aug is not None:
+                offs, flips = aug.offs, aug.flips
+            else:
+                if getattr(self, "_zero_off", None) is None or self._zero_off.shape[0] != x.shape[0]:
+                    self._zero_off = torch.zeros((x.shape[0], 2), dtype=torch.int32, device=x.device)
+                    self._zero_flip = torch.zeros((x.shape[0],), dtype=torch.uint8, device=x.device)
+                offs, flips = self._zero_off, self._zero_flip
             x = ops.crop_mirror_normalize(x.float() if x.dtype not in (torch.float32, torch.bfloat16, torch.uint8) else x, self._mean,
-                                          1.0 / 64.0, (x.shape[1], x.shape[2]), self._zero_off, self._zero_flip, out_dtype=self.act_dtype)
+                                          1.0 / 64.0, (x.shape[1], x.shape[2]), offs, flips, out_dtype=self.act_dtype,
+                                          zero_fill=aug is not None)
+            if aug is not None and aug.cutout:
+                x = ops.random_erase(x, aug.boxes)
+            if rec is not None:
+                x = ops.mix_batch(x, rec)
         else:
             x = ((x.float() - self._mean) / 64.0).to(self.act_dtype)
         x = self.stem.forward(x)

@@ -825,8 +825,24 @@ def drop_path_draw(dp, step, out):
     return out
 
 
+def cifar_augment_draw(cfg, rank, step, offs, flips, boxes):
+    """The cifar_augment draw of the device step counter ``step`` for worker ``rank`` (``cfg`` a validated config) into ``offs`` (int32
+    [B, 2]), ``flips`` (uint8 [B]) and ``boxes`` (int32 [B, 4]): one ``cifar_augment_draw_kernel`` launch (reference.cifar_augment_draw
+    on the CPU; ops/cifar_augment.py owns the layout)."""
+    from .cifar_augment import SIZE
+    B = offs.shape[0]
+    for t, dt, shape in ((offs, torch.int32, (B, 2)), (flips, torch.uint8, (B,)), (boxes, torch.int32, (B, 4))):
+        if not (t.is_cuda and t.dtype == dt and t.is_contiguous() and tuple(t.shape) == shape and t.device == step.device):
+            raise ValueError("cifar_augment_draw: a buffer is not a contiguous %s %s tensor on %s" % (dt, shape, step.device))
+    assert boxes.data_ptr() % 16 == 0 and offs.data_ptr() % 8 == 0
+    L().cifar_augment_draw(B, int(cfg["pad"]), int(cfg["cutout"]), SIZE, SIZE, int(cfg["seed"]) & (2 ** 64 - 1), int(rank),
+                           step.data_ptr(), offs.data_ptr(), flips.data_ptr(), boxes.data_ptr(), _st(step))
+
+
 # --------------------------------------------------------------------------- loader kernel
-def crop_mirror_normalize(x, mean, std_scale, crop_hw, offsets, flips, out_dtype=None, out=None, c_out=None):
+def crop_mirror_normalize(x, mean, std_scale, crop_hw, offsets, flips, out_dtype=None, out=None, c_out=None, zero_fill=False):
+    """``nn_kernels.cu: crop_mirror_norm_kernel``: image n normalised, cropped at ``offsets[n]`` (inside the image, or anywhere with
+    ``zero_fill``, where a pixel outside the image is 0) and mirrored where ``flips[n]``.  See :func:`reference.crop_mirror_normalize`."""
     out_dtype = out_dtype or ADT()
     x = x.contiguous()
     N, H, W, C = x.shape
@@ -849,7 +865,7 @@ def crop_mirror_normalize(x, mean, std_scale, crop_hw, offsets, flips, out_dtype
     else:
         sc, cs_ptr = float(std_scale), 0
     L().crop_mirror_norm(x.data_ptr(), kind, mean.data_ptr(), mode, sc, cs_ptr, out.data_ptr(), int(out.dtype == BF16),
-                         offsets.data_ptr(), flips.data_ptr(), N, H, W, C, ch, cw, Cout, _st(x))
+                         offsets.data_ptr(), flips.data_ptr(), N, H, W, C, ch, cw, Cout, int(bool(zero_fill)), _st(x))
     return out
 
 

@@ -539,6 +539,18 @@ def drop_path_draw(dp, out):
     return out.copy_(ref.drop_path_draw(dp.rates, _RNG["seed"], dp.rank, _RNG["step"], dp.B))
 
 
+def cifar_augment_draw(aug):
+    """This step's offsets, flips and Cutout boxes for :class:`cifar_augment.CifarAugment` ``aug`` into its buffers: on CUDA drawn by
+    the kernel from the device step counter, on the CPU by :func:`reference.cifar_augment_draw` from the host one.  Returns ``aug``."""
+    if aug.offs.is_cuda:
+        from . import cuda_impl
+        cuda_impl.cifar_augment_draw(aug.cfg, aug.rank, cuda_impl.step_counter(aug.offs.device), aug.offs, aug.flips, aug.boxes)
+        return aug
+    for buf, v in zip((aug.offs, aug.flips, aug.boxes), ref.cifar_augment_draw(aug.cfg, aug.cfg["seed"], aug.rank, _RNG["step"], aug.B)):
+        buf.copy_(v)
+    return aug
+
+
 def mix_batch(x, rec):
     """Mix the NHWC batch ``x`` in place (no autograd: it is an input) as the Mixup / CutMix record ``rec`` says; returns ``x``."""
     if x.is_cuda:
@@ -569,12 +581,14 @@ def gan_loss(scores, kind, a):
 
 
 # --------------------------------------------------------------------------- data aug
-def crop_mirror_normalize(x, mean, std_scale, crop_hw, offsets, flips, out_dtype=None):
+def crop_mirror_normalize(x, mean, std_scale, crop_hw, offsets, flips, out_dtype=None, zero_fill=False):
+    """Normalise, crop and mirror an NHWC batch: the native kernel on CUDA, :func:`reference.crop_mirror_normalize` on the CPU.
+    ``zero_fill``: offsets may put a pixel outside the image, which is then 0 (cifar_augment's zero-padded crop)."""
     if x.is_cuda:
         from . import cuda_impl
-        return cuda_impl.crop_mirror_normalize(x, mean, std_scale, crop_hw, offsets, flips, out_dtype)
+        return cuda_impl.crop_mirror_normalize(x, mean, std_scale, crop_hw, offsets, flips, out_dtype, zero_fill=zero_fill)
     return ref.crop_mirror_normalize(x, mean, std_scale, crop_hw, offsets, flips,
-                                     out_dtype or torch.float32)
+                                     out_dtype or torch.float32, zero_fill=zero_fill)
 
 
 def resized_crop_mirror_normalize(x, mean, std_scale, out_hw, boxes, flips, out_dtype=None):

@@ -426,6 +426,33 @@ def drop_path_draw(p_list, seed, rank, step, B):
     return torch.from_numpy(out.reshape(L, B))
 
 
+# --------------------------------------------------------------------------- CIFAR augmentation (cifar_augment)
+def cifar_augment_draw(cfg, seed, rank, step, B):
+    """(offs int32 [B, 2], flips uint8 [B], boxes int32 [B, 4]) of step counter value ``step`` for worker ``rank``, as the CUDA
+    ``cifar_augment_draw_kernel`` writes them (ops/cifar_augment.py owns the layout).  ``cfg`` is a validated ``config['cifar_augment']``.
+
+    Philox4x32-10, key (seed_lo, seed_hi ^ rank), counter (n, TAG, step_lo, step_hi) for block 0 and (n, TAG + 1, ...) for block 1;
+    each value ⌊w·k / 2^32⌋: oy, ox (k = 2·pad + 1) from block 0 words 0, 1; flip = word 2 >> 31; cy (k = 32) from word 3; cx from
+    block 1 word 0.  offs = (oy − pad, ox − pad); the Cutout box is DeVries & Taylor's clamp of cy ± L//2, cx ± L//2."""
+    from . import cifar_augment as ca
+    M32 = 0xFFFFFFFF
+    seed, step = int(seed) & (2 ** 64 - 1), int(step) & (2 ** 64 - 1)
+    k0, k1 = seed & M32, ((seed >> 32) ^ (int(rank) & M32)) & M32
+    n = np.arange(int(B), dtype=np.uint64)
+    lo, hi = np.full_like(n, step & M32), np.full_like(n, step >> 32)
+    a = _philox4x32((n, np.full_like(n, ca.TAG), lo, hi), k0, k1)
+    b = _philox4x32((n, np.full_like(n, ca.TAG + 1), lo, hi), k0, k1)
+    pad, L, S = cfg["pad"], cfg["cutout"], ca.SIZE
+
+    def pick(w, k):
+        return ((w * np.uint64(k)) >> np.uint64(32)).astype(np.int64)
+    oy, ox = pick(a[0], 2 * pad + 1), pick(a[1], 2 * pad + 1)
+    offs = np.stack([oy - pad, ox - pad], axis=1).astype(np.int32)
+    flips = (a[2] >> np.uint64(31)).astype(np.uint8)
+    boxes = ca.cutout_boxes(pick(a[3], S), pick(b[0], S), L)
+    return torch.from_numpy(offs), torch.from_numpy(flips), torch.from_numpy(boxes)
+
+
 # --------------------------------------------------------------------------- optimizer (flat arena)
 def clip_scale(g, offsets, sizes, max_norm):
     """Global gradient-norm clipping (``torch.nn.utils.clip_grad_norm_``) over a flat fp32 gradient laid out as a :class:`FlatArena`
@@ -648,9 +675,10 @@ def gosgd_merge(w, b, alpha_self, alpha_src):
 
 
 # --------------------------------------------------------------------------- data aug
-def crop_mirror_normalize(x_u8, mean, std_scale, crop_hw, offsets, flips, out_dtype=torch.float32):
+def crop_mirror_normalize(x_u8, mean, std_scale, crop_hw, offsets, flips, out_dtype=torch.float32, zero_fill=False):
     """``(x - mean) * std_scale`` → crop at per-image ``offsets`` → optional
     horizontal flip (ref ``data/utils.py:42-129`` + ``proc_load_mpi.py:99-104``).
+    ``zero_fill``: the crop may reach outside the image, whose pixels are then 0 (the normalised image zero-padded, then cropped).
 
     x_u8   : [N, H, W, C] uint8 or float
     mean   : [H, W, C] or [C] float
@@ -664,7 +692,13 @@ def crop_mirror_normalize(x_u8, mean, std_scale, crop_hw, offsets, flips, out_dt
     out = torch.empty((N, ch, cw, C), dtype=torch.float32, device=x.device)
     for i in range(N):
         y0, x0 = int(offsets[i, 0]), int(offsets[i, 1])
-        patch = x[i, y0:y0 + ch, x0:x0 + cw, :]
+        if zero_fill:
+            patch = torch.zeros((ch, cw, C), dtype=torch.float32, device=x.device)
+            ys, ye, xs, xe = max(0, -y0), min(ch, H - y0), max(0, -x0), min(cw, W - x0)
+            if ye > ys and xe > xs:
+                patch[ys:ye, xs:xe] = x[i, y0 + ys:y0 + ye, x0 + xs:x0 + xe, :]
+        else:
+            patch = x[i, y0:y0 + ch, x0:x0 + cw, :]
         if bool(flips[i]):
             patch = patch.flip(1)
         out[i] = patch
