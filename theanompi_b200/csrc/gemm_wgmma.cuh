@@ -607,6 +607,23 @@ gemm_wgmma(const __grid_constant__ CUtensorMap tmap_a0, const __grid_constant__ 
   constexpr int STEPS = BK / MMA_K;
   const int k_chunks = p.conv_mode == 1 ? p.c_chunks : 1;
   const int tail_steps = p.conv_mode == 1 ? (p.cCg - (p.c_chunks - 1) * BK + MMA_K - 1) / MMA_K : STEPS;
+  // global columns [nb, n_end_c) of the tile's 32-column chunk c (nb + j: column j of the chunk)
+  auto chunk_cols = [&](int nti, int n0, int c, int& nb, int& n_end_c) {
+    const int cc = 32 * c;                                     // column offset inside the tile
+    nb = n0 + cc; n_end_c = p.N;
+    if (p.conv_mode == 2) {
+      // wgrad: every ATOM-column box of the tile is one (filter tap, ATOM-channel chunk) and lands at column
+      // tap*Cg + chunk*ATOM of dW (a 32-column chunk never straddles two boxes)
+      const int box = nti * (BN >= ATOM ? BN / ATOM : 1) + cc / ATOM;
+      if (box < p.cKH * p.cKW * p.c_chunks) {
+        const int tap = box / p.c_chunks, cch = box - tap * p.c_chunks;
+        nb = tap * p.cCg + cch * ATOM + (cc % ATOM);
+        n_end_c = tap * p.cCg + min(p.cCg, cch * ATOM + ATOM);
+      } else {
+        nb = 0; n_end_c = 0;
+      }
+    }
+  };
   float acc[MT][BN / 2];
   int stage = 0; uint32_t phase = 0;
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -617,6 +634,29 @@ gemm_wgmma(const __grid_constant__ CUtensorMap tmap_a0, const __grid_constant__ 
     tile_mn(p, rem, mti, nti);
     const int m0 = mti * TM, n0 = nti * BN;
     const int kb0 = split * p.kb_per_split, kb1 = min(num_kb_total, kb0 + p.kb_per_split);
+    // per-column bias of this lane's columns of the tile, all loaded at once: at tile start, so that the k loop hides the load
+    // latency (loaded chunk by chunk in the epilogue, every 32-column chunk waited for its loads between two warp syncs).
+    // 256-row tf32 tiles keep the per-chunk loads: their accumulators leave no registers for it.
+    float bcol[BN / 8][2];
+    auto load_bias = [&]() {
+#pragma unroll
+      for (int i = 0; i < BN / 8; ++i) bcol[i][0] = bcol[i][1] = 0.f;
+      if (p.bias_mode != 1) return;
+      const float* const bias_ptr = grp ? p.bias1 : p.bias;
+#pragma unroll
+      for (int c = 0; c < BN / 32; ++c) {
+        int nb, n_end_c;
+        chunk_cols(nti, n0, c, nb, n_end_c);
+#pragma unroll
+        for (int f = 0; f < 4; ++f) {
+          const int n = nb + 8 * f + fc;
+          if (n < n_end_c) bcol[4 * c + f][0] = __ldg(bias_ptr + n);
+          if (n + 1 < n_end_c) bcol[4 * c + f][1] = __ldg(bias_ptr + n + 1);
+        }
+      }
+    };
+    constexpr bool kEarlyBias = !(E::TF32 && MT == 2);
+    if constexpr (kEarlyBias) load_bias();
     // sub-tiles in which this warpgroup owns at least one row below M (a prefix of the MT sub-tiles); a warpgroup with none
     // issues no wgmma for the tile but still hands every slot back
     int n_live = 0;
@@ -748,20 +788,8 @@ gemm_wgmma(const __grid_constant__ CUtensorMap tmap_a0, const __grid_constant__ 
       }
 #pragma unroll
       for (int c = 0; c < BN / 32; ++c) {
-        const int cc = 32 * c;                                 // column offset inside the tile
-        int nb = n0 + cc, n_end_c = p.N;
-        if (p.conv_mode == 2) {
-          // wgrad: every ATOM-column box of the tile is one (filter tap, ATOM-channel chunk) and lands at column
-          // tap*Cg + chunk*ATOM of dW (a 32-column chunk never straddles two boxes)
-          const int box = nti * (BN >= ATOM ? BN / ATOM : 1) + cc / ATOM;
-          if (box < p.cKH * p.cKW * p.c_chunks) {
-            const int tap = box / p.c_chunks, cch = box - tap * p.c_chunks;
-            nb = tap * p.cCg + cch * ATOM + (cc % ATOM);
-            n_end_c = tap * p.cCg + min(p.cCg, cch * ATOM + ATOM);
-          } else {
-            nb = 0; n_end_c = 0;
-          }
-        }
+        int nb, n_end_c;
+        chunk_cols(nti, n0, c, nb, n_end_c);
 #pragma unroll
         for (int f = 0; f < 4; ++f) {
           const int i = 4 * c + f;                             // 8-column fragment i of the tile
@@ -769,9 +797,13 @@ gemm_wgmma(const __grid_constant__ CUtensorMap tmap_a0, const __grid_constant__ 
           float v0 = acc[u][4 * i], v1 = acc[u][4 * i + 1], v2 = acc[u][4 * i + 2], v3 = acc[u][4 * i + 3];
           float b0 = bm0, b1 = bm0, b2 = bm1, b3 = bm1;
           if (p.bias_mode == 1) {
-            const int n = nb + j;
-            b0 = b2 = (n < n_end_c) ? __ldg(bias_ptr + n) : 0.f;
-            b1 = b3 = (n + 1 < n_end_c) ? __ldg(bias_ptr + n + 1) : 0.f;
+            if constexpr (kEarlyBias) {
+              b0 = b2 = bcol[i][0]; b1 = b3 = bcol[i][1];
+            } else {
+              const int n = nb + j;
+              b0 = b2 = (n < n_end_c) ? __ldg(bias_ptr + n) : 0.f;
+              b1 = b3 = (n + 1 < n_end_c) ? __ldg(bias_ptr + n + 1) : 0.f;
+            }
           }
           v0 = fmaf(v0, p.alpha, b0); v1 = fmaf(v1, p.alpha, b1); v2 = fmaf(v2, p.alpha, b2); v3 = fmaf(v3, p.alpha, b3);
           if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); v2 = fmaxf(v2, 0.f); v3 = fmaxf(v3, 0.f); }
