@@ -165,6 +165,18 @@ void pad_rows(const void* src, void* dst, long long rows, int cols, long long sr
 // zero_fill = 1: offsets may put a source pixel outside the image, which then stores 0 in every channel (else the crop stays inside)
 void crop_mirror_norm(const void* x, int in_kind, const void* mean, int mean_mode, float scale, const void* cscale, void* out, int out_bf16, const void* offs,
                       const void* flips, int N, int H, int W, int C, int ch, int cw, int Cout, int zero_fill, cudaStream_t st);
+// test-time views: kMaxViews entries (y0, x0, mirror) of the ch × cw crop inside the H × W image, passed by value
+constexpr int kMaxViews = 10;
+struct ViewTable {
+  int y0[kMaxViews], x0[kMaxViews], mirror[kMaxViews];
+};
+// the V views of the uint8 NHWC batch x, normalised as crop_mirror_norm, into the view-major out [V, N, ch, cw, C] (bf16 or fp32)
+void multi_crop_norm(const void* x, const void* mean, int mean_mode, float scale, const void* cscale, void* out, int out_bf16,
+                     const ViewTable& views, int V, int N, int H, int W, int C, int ch, int cw, cudaStream_t st);
+// view v of V: acc [B, C] fp32 = softmax(logits) (v = 0) or acc + softmax(logits); on v = V − 1 acc /= V, rowstat[b] = {−log max(p̄_y,
+// FLT_MIN), top-1 error, top-5 error} and out3 = their means over the batch
+void view_softmax_accum(const void* logits, const void* labels, void* acc, void* rowstat, void* out3, int B, int C, int v, int V, int f32,
+                        cudaStream_t st);
 // random-resized crop: uint8 NHWC x → bilinear resample of the normalised box boxes[n] = (y0, x0, h, w) (int32 [N, 4], 16-byte
 // aligned, inside the H × W image) to ch × cw, mirrored after the resize where flips[n]; out bf16 (out_bf16) or fp32 NHWC
 void resized_crop_mirror_norm(const void* x, const void* mean, int mean_mode, float scale, const void* cscale, void* out, int out_bf16,

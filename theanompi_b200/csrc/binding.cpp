@@ -136,6 +136,19 @@ PYBIND11_MODULE(_tmpi_native, m) {
                                ptr_t flips, int N, int H, int W, int C, int ch, int cw, int Cout, int zero_fill, ptr_t st) {
     crop_mirror_norm(P(x), in_kind, P(mean), mean_mode, scale, P(cscale), P(out), out_bf16, P(offs), P(flips), N, H, W, C, ch, cw, Cout, zero_fill,
                      S(st)); });
+  m.attr("MAX_VIEWS") = kMaxViews;
+  m.def("multi_crop_norm", [](ptr_t x, ptr_t mean, int mean_mode, float scale, ptr_t cscale, ptr_t out, int out_bf16,
+                              const std::vector<int>& y0, const std::vector<int>& x0, const std::vector<int>& mirror, int N, int H, int W,
+                              int C, int ch, int cw, ptr_t st) {
+    const int V = (int)y0.size();
+    if (V < 1 || V > kMaxViews || (int)x0.size() != V || (int)mirror.size() != V)
+      throw std::runtime_error("multi_crop_norm: 1 to 10 views, each with y0, x0 and mirror");
+    ViewTable t{};
+    for (int v = 0; v < V; ++v) { t.y0[v] = y0[v]; t.x0[v] = x0[v]; t.mirror[v] = mirror[v]; }
+    multi_crop_norm(P(x), P(mean), mean_mode, scale, P(cscale), P(out), out_bf16, t, V, N, H, W, C, ch, cw, S(st)); });
+  m.def("view_softmax_accum", [](ptr_t logits, ptr_t labels, ptr_t acc, ptr_t rowstat, ptr_t out3, int B, int C, int v, int V, int f32,
+                                 ptr_t st) {
+    view_softmax_accum(P(logits), P(labels), P(acc), P(rowstat), P(out3), B, C, v, V, f32, S(st)); });
   m.def("resized_crop_mirror_norm", [](ptr_t x, ptr_t mean, int mean_mode, float scale, ptr_t cscale, ptr_t out, int out_bf16, ptr_t boxes,
                                        ptr_t flips, int N, int H, int W, int C, int ch, int cw, ptr_t st) {
     resized_crop_mirror_norm(P(x), P(mean), mean_mode, scale, P(cscale), P(out), out_bf16, P(boxes), P(flips), N, H, W, C, ch, cw, S(st)); });

@@ -9,6 +9,7 @@
 #include "common.cuh"
 #include "api.h"
 #include <algorithm>
+#include <cfloat>
 #include <type_traits>
 
 namespace tmpi {
@@ -647,6 +648,79 @@ void softmax_xent(const void* logits, const void* labels, void* dlogits, void* r
   }
   count_launch(); TMPI_CHECK_LAUNCH("softmax_xent"); ::tmpi::check_capture(st, "softmax_xent");
   rowstat_mean_kernel<<<1, 256, 0, st>>>((const float*)rowstat, (float*)out3, B, weight);
+  count_launch(); TMPI_CHECK_LAUNCH("rowstat_mean"); ::tmpi::check_capture(st, "rowstat_mean");
+}
+
+// ============================================================================ multi-view validation: averaged softmax + metrics
+// One CTA per row b.  View v's max-shifted fp32 softmax p_v of the logits is stored into (v = 0) or added to (v > 0) the fp32
+// accumulator acc[b, :], each element by the thread that owns column c in every view, so the sum runs in view order.  On the last view
+// the same launch divides by V (an IEEE division), leaving p̄ = (1/V)·Σ p_v in acc, and writes rowstat[b] = {−log max(p̄_y, FLT_MIN),
+// rank ≥ 1, rank ≥ 5} with rank = #{p̄_c > p̄_y} + #{c < y : p̄_c = p̄_y}, the rank rule of softmax_xent_kernel.
+template <typename T>
+__global__ void view_softmax_accum_kernel(const T* __restrict__ logits, const long long* __restrict__ labels, float* __restrict__ acc,
+                                          float* __restrict__ rowstat, int C, int v, int V) {
+  const int b = blockIdx.x;
+  const T* row = logits + (long long)b * C;
+  float* a = acc + (long long)b * C;
+  __shared__ float red[32];
+  __shared__ float bcast;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  float mx = -INFINITY;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) mx = fmaxf(mx, to_f(row[c]));
+  mx = warp_max(mx);
+  if (lane == 0) red[warp] = mx;
+  __syncthreads();
+  if (warp == 0) { float t = lane < nw ? red[lane] : -INFINITY; t = warp_max(t); if (lane == 0) bcast = t; }
+  __syncthreads();
+  mx = bcast;
+  __syncthreads();
+  float se = 0.f;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) se += __expf(to_f(row[c]) - mx);
+  se = warp_sum(se);
+  if (lane == 0) red[warp] = se;
+  __syncthreads();
+  if (warp == 0) { float t = lane < nw ? red[lane] : 0.f; t = warp_sum(t); if (lane == 0) bcast = t; }
+  __syncthreads();
+  const float inv = 1.f / bcast;
+  const bool last = v == V - 1;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    float s = __expf(to_f(row[c]) - mx) * inv;
+    if (v > 0) s += a[c];
+    if (last) s = __fdiv_rn(s, (float)V);
+    a[c] = s;
+  }
+  if (!last) return;                                            // CTA-uniform
+  __syncthreads();                                              // p̄ of the whole row written (global writes visible to the CTA)
+  const int label = (int)labels[b];
+  const float py = a[label];
+  float gt = 0.f;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    const float p = a[c];
+    gt += (p > py || (p == py && c < label)) ? 1.f : 0.f;
+  }
+  gt = warp_sum(gt);
+  if (lane == 0) red[warp] = gt;
+  __syncthreads();
+  if (warp == 0) {
+    float t = lane < nw ? red[lane] : 0.f;
+    t = warp_sum(t);
+    if (lane == 0) {
+      rowstat[3 * b + 0] = -__logf(fmaxf(py, FLT_MIN));
+      rowstat[3 * b + 1] = t >= 1.f ? 1.f : 0.f;
+      rowstat[3 * b + 2] = t >= 5.f ? 1.f : 0.f;
+    }
+  }
+}
+
+void view_softmax_accum(const void* logits, const void* labels, void* acc, void* rowstat, void* out3, int B, int C, int v, int V, int f32,
+                        cudaStream_t st) {
+  if (!(V >= 1 && v >= 0 && v < V)) throw std::runtime_error("view_softmax_accum: needs 0 <= v < V");
+  auto LB = (const long long*)labels; auto A = (float*)acc; auto RS = (float*)rowstat;
+  if (f32) view_softmax_accum_kernel<float><<<B, 256, 0, st>>>((const float*)logits, LB, A, RS, C, v, V);
+  else view_softmax_accum_kernel<__nv_bfloat16><<<B, 256, 0, st>>>((const __nv_bfloat16*)logits, LB, A, RS, C, v, V);
+  count_launch(); TMPI_CHECK_LAUNCH("view_softmax_accum"); ::tmpi::check_capture(st, "view_softmax_accum");
+  if (v != V - 1) return;
+  rowstat_mean_kernel<<<1, 256, 0, st>>>((const float*)rowstat, (float*)out3, B, 1.f);
   count_launch(); TMPI_CHECK_LAUNCH("rowstat_mean"); ::tmpi::check_capture(st, "rowstat_mean");
 }
 
@@ -1566,6 +1640,29 @@ void s2d_filter(const void* src, void* dst, int O, int KH, int KW, int C, int S,
 }
 
 // ============================================================================ loader: normalise + crop + mirror → NHWC bf16/fp32
+// One output pixel: (src[c] − mean)·scale·cscale[c] for c < C, 0 for C ≤ c < Cout.  Shared by crop_mirror_norm_kernel and
+// multi_crop_norm_kernel, so a view of the latter is bit-equal to the former run with the view's offsets.
+template <typename Tin, typename Tout>
+__device__ __forceinline__ void norm_pixel(const Tin* __restrict__ src, const float* __restrict__ mp, int mean_mode, float scale,
+                                           const float* __restrict__ cscale, Tout* __restrict__ o, int C, int Cout) {
+  if (C == 3 && Cout == 3) {
+    const float m0 = mean_mode == 0 ? mp[0] : mp[0], m1 = mean_mode == 0 ? mp[0] : mp[1], m2 = mean_mode == 0 ? mp[0] : mp[2];
+    // per-channel 1/std on top of the scalar scale (ref proc_load_mpi.py:99: (arr - img_mean) / 255. / img_std)
+    const float s0 = cscale ? scale * cscale[0] : scale, s1 = cscale ? scale * cscale[1] : scale, s2 = cscale ? scale * cscale[2] : scale;
+    const float v0 = ((float)src[0] - m0) * s0, v1 = ((float)src[1] - m1) * s1, v2 = ((float)src[2] - m2) * s2;
+    o[0] = (Tout)v0; o[1] = (Tout)v1; o[2] = (Tout)v2;
+    return;
+  }
+  for (int c = 0; c < Cout; ++c) {
+    float v = 0.f;
+    if (c < C) {
+      const float m = mean_mode == 0 ? mp[0] : mp[c];
+      v = ((float)src[c] - m) * (cscale ? scale * cscale[c] : scale);
+    }
+    o[c] = (Tout)v;
+  }
+}
+
 // One CTA per output row (n, oy): crop offsets / flip flag are CTA-uniform, threads sweep the row's (ox, c) elements with 32-bit
 // math (coalesced stores; loads are contiguous runs of the source row, reversed when mirrored).
 // grid = (N * ch, ceil(cw / 128)): the output row (n, oy) comes from blockIdx.x, the pixel from blockIdx.y / threadIdx.x — no
@@ -1589,25 +1686,8 @@ __global__ void __launch_bounds__(128) crop_mirror_norm_kernel(const Tin* __rest
     }
   }
   const unsigned pix = (unsigned)(sy * W + sx) * (unsigned)C;          // inside one image (host checks H*W*C < 2^31)
-  const Tin* src = x + (long long)n * H * W * C + pix;
-  const float* mp = mean_mode == 2 ? mean + pix : mean;
-  Tout* o = out + ((long long)blockIdx.x * cw + ox) * Cout;
-  if (C == 3 && Cout == 3) {
-    const float m0 = mean_mode == 0 ? mp[0] : mp[0], m1 = mean_mode == 0 ? mp[0] : mp[1], m2 = mean_mode == 0 ? mp[0] : mp[2];
-    // per-channel 1/std on top of the scalar scale (ref proc_load_mpi.py:99: (arr - img_mean) / 255. / img_std)
-    const float s0 = cscale ? scale * cscale[0] : scale, s1 = cscale ? scale * cscale[1] : scale, s2 = cscale ? scale * cscale[2] : scale;
-    const float v0 = ((float)src[0] - m0) * s0, v1 = ((float)src[1] - m1) * s1, v2 = ((float)src[2] - m2) * s2;
-    o[0] = (Tout)v0; o[1] = (Tout)v1; o[2] = (Tout)v2;
-    return;
-  }
-  for (int c = 0; c < Cout; ++c) {
-    float v = 0.f;
-    if (c < C) {
-      const float m = mean_mode == 0 ? mp[0] : mp[c];
-      v = ((float)src[c] - m) * (cscale ? scale * cscale[c] : scale);
-    }
-    o[c] = (Tout)v;
-  }
+  norm_pixel(x + (long long)n * H * W * C + pix, mean_mode == 2 ? mean + pix : mean, mean_mode, scale, cscale,
+             out + ((long long)blockIdx.x * cw + ox) * Cout, C, Cout);
 }
 
 void crop_mirror_norm(const void* x, int in_kind /*0 u8, 1 bf16, 2 f32*/, const void* mean, int mean_mode, float scale, const void* cscale, void* out,
@@ -1623,6 +1703,41 @@ void crop_mirror_norm(const void* x, int in_kind /*0 u8, 1 bf16, 2 f32*/, const 
   else { if (out_bf16) CMN(float, __nv_bfloat16); else CMN(float, float); }
 #undef CMN
   count_launch(); TMPI_CHECK_LAUNCH("crop_mirror_norm"); ::tmpi::check_capture(st, "crop_mirror_norm");
+}
+
+// ============================================================================ loader: every test-time view in one launch
+// V fixed views (y0, x0, mirror) of the uint8 NHWC batch into the view-major output [V, N, ch, cw, C].  The table travels by value
+// in the kernel's parameters, so there is no per-image offset array and no copy to the device; __grid_constant__ lets the CTA-uniform
+// view index read it in place (a by-value array indexed at run time is otherwise copied to local memory by every thread, which made
+// the kernel several times slower per view than crop_mirror_norm_kernel).  The grid of crop_mirror_norm_kernel with the view in
+// blockIdx.z: output row (v·N + n)·ch + oy, no per-thread division by N; each pixel goes through norm_pixel.
+template <typename Tout>
+__global__ void __launch_bounds__(128) multi_crop_norm_kernel(const uint8_t* __restrict__ x, const float* __restrict__ mean, int mean_mode,
+                                                              float scale, const float* __restrict__ cscale, Tout* __restrict__ out,
+                                                              const __grid_constant__ ViewTable views, int N, int H, int W, int C,
+                                                              int ch, int cw) {
+  const int ox = blockIdx.y * blockDim.x + threadIdx.x;
+  if (ox >= cw) return;
+  const int oy = blockIdx.x % ch, n = blockIdx.x / ch, v = blockIdx.z;
+  const int sy = views.y0[v] + oy;
+  const int sx = views.x0[v] + (views.mirror[v] ? (cw - 1 - ox) : ox);
+  const unsigned pix = (unsigned)(sy * W + sx) * (unsigned)C;
+  norm_pixel(x + (long long)n * H * W * C + pix, mean_mode == 2 ? mean + pix : mean, mean_mode, scale, cscale,
+             out + (((long long)v * N * ch + blockIdx.x) * cw + ox) * C, C, C);
+}
+
+void multi_crop_norm(const void* x, const void* mean, int mean_mode, float scale, const void* cscale, void* out, int out_bf16,
+                     const ViewTable& views, int V, int N, int H, int W, int C, int ch, int cw, cudaStream_t st) {
+  if (V < 1 || V > kMaxViews) throw std::runtime_error("multi_crop_norm: 1 to 10 views");
+  if ((long long)H * W * C >= (1LL << 31) || (long long)V * N * ch >= (1LL << 31)) throw std::runtime_error("multi_crop_norm: image too large");
+  for (int v = 0; v < V; ++v)
+    if (views.y0[v] < 0 || views.x0[v] < 0 || views.y0[v] + ch > H || views.x0[v] + cw > W)
+      throw std::runtime_error("multi_crop_norm: a view is not inside the image");
+  const dim3 g((unsigned)(N * ch), (unsigned)((cw + 127) / 128), (unsigned)V);
+  auto X = (const uint8_t*)x; auto M = (const float*)mean; auto CS = (const float*)cscale;
+  if (out_bf16) multi_crop_norm_kernel<__nv_bfloat16><<<g, 128, 0, st>>>(X, M, mean_mode, scale, CS, (__nv_bfloat16*)out, views, N, H, W, C, ch, cw);
+  else multi_crop_norm_kernel<float><<<g, 128, 0, st>>>(X, M, mean_mode, scale, CS, (float*)out, views, N, H, W, C, ch, cw);
+  count_launch(); TMPI_CHECK_LAUNCH("multi_crop_norm"); ::tmpi::check_capture(st, "multi_crop_norm");
 }
 
 // ============================================================================ loader: random-resized crop → NHWC bf16/fp32

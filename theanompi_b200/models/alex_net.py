@@ -78,7 +78,7 @@ class AlexNet(ModelBase):
                                      self.rand_crop, self.batch_crop_mirror, out_dtype=self.act_dtype,
                                      resized_crop=self.resized_crop, rank=self.rank,
                                      color_jitter=self.color_jitter, random_erasing=self.random_erasing,
-                                     auto_augment=self.auto_augment)
+                                     auto_augment=self.auto_augment, val_crops=self.val_crops)
 
     def build_model(self):
         if self.verbose:

@@ -153,6 +153,10 @@ class ModelBase(object):
         # TrivialAugmentWide / RandAugment on the uint8 training crop (a dict, models/data/utils.py: check_auto_augment; None = off):
         # op records drawn by the loader and applied by its kernels on the copy stream; the training step never sees it
         self.auto_augment = self.check_auto_augment(config.get("auto_augment"))
+        # test-time views of every validation image (1, 2 or 10; models/data/utils.py: check_val_crops): the loader cuts them all in
+        # one launch into a view-major [V, N, ...] batch and val_fn averages the views' softmax.  Checked here because the model's
+        # constructor builds the loader; training never sees it
+        self.val_crops = self.check_val_crops(config.get("val_crops", 1))
         self.base_lr = np.float32(self.learning_rate)
         self.current_t = self.subb_t = 0
         self.current_v = self.subb_v = 0
@@ -195,6 +199,8 @@ class ModelBase(object):
         self.input_shape = tuple(input_shape)           # (B, H, W, C)
         self.shared_x = torch.zeros((fb,) + self.input_shape[1:], dtype=self.act_dtype, device=self.device)
         self.shared_y = torch.zeros((fb,), dtype=torch.int64, device=self.device)
+        # val_crops > 1: the view-major [V, fb, ...] validation batch, the loader's ring slot or the serial path's buffer
+        self.val_x = None
         self.x_in = torch.zeros((B,) + self.input_shape[1:], dtype=self.act_dtype, device=self.device)
         self.y_in = torch.zeros((B,), dtype=torch.int64, device=self.device)
         # label staging: a small ring of pinned buffers, each guarded by the event of its last H2D copy — the host runs
@@ -436,6 +442,16 @@ class ModelBase(object):
                              "ResNet152 and ResNet50Torch" % (type(self).__name__, RE_KEY))
         return cfg
 
+    def check_val_crops(self, v):
+        """The validated ``config['val_crops']`` (models/data/utils.py: check_val_crops; a ValueError names the key).  A value other
+        than 1 needs a model fed by the ImageNet loader (``supports_resized_crop``)."""
+        from .data.utils import VC_KEY, check_val_crops
+        v = check_val_crops(v)
+        if v != 1 and not self.supports_resized_crop:
+            raise ValueError("%s: %s = %d is not supported; multi-crop validation runs on the ImageNet loader of AlexNet, GoogLeNet, "
+                             "VGG16, ResNet50, ResNet152 and ResNet50Torch" % (type(self).__name__, VC_KEY, v))
+        return v
+
     # ------------------------------------------------------------------ stochastic depth (drop-path)
     def check_drop_path(self):
         """``config['drop_path_rate']`` must be a finite real p in [0, 1) (ops/drop_path.py: check_rate; a ValueError names the key),
@@ -601,7 +617,29 @@ class ModelBase(object):
             with torch.no_grad():
                 c, e, e5 = self.loss(x, y)
             return c, e, e5
-        self.val_fn = val_fn
+
+        def multi_view_val_fn(subb_ind=0):
+            # val_crops = V > 1: V forwards on the views of the sub-batch, each followed by view_softmax_accum on the main head's
+            # logits (the last one also reduces the metrics: V + 1 launches besides the forwards); the CPU runs the reference
+            B, V = self.batch_size, self.val_crops
+            y = self.shared_y[subb_ind * B:(subb_ind + 1) * B]
+            with torch.no_grad():
+                if not self.cuda:
+                    logits = []
+                    for v in range(V):
+                        self.forward(self.val_x[v, subb_ind * B:(subb_ind + 1) * B])
+                        logits.append(self.output_layer.logits)
+                    return ops.reference.multi_view_xent(logits, y, torch.float32)[:3]
+                from ..ops import cuda_impl
+                acc = None
+                for v in range(V):
+                    self.forward(self.val_x[v, subb_ind * B:(subb_ind + 1) * B])
+                    lg = self.output_layer.logits
+                    if acc is None:
+                        acc = torch.empty(tuple(lg.shape), dtype=torch.float32, device=self.device)
+                    out = cuda_impl.view_softmax_accum(lg, y, acc, v, V)
+            return out
+        self.val_fn = val_fn if self.val_crops == 1 else multi_view_val_fn
 
     def compile_inference(self):
         def inf_fn(x):
@@ -712,11 +750,20 @@ class ModelBase(object):
                 loader.request(img[idx], mode)
             loader.request(img[idx + 1] if not last else img[idx], mode)
             b = loader.get()
-            self.shared_x = b.x
+            if b.x.dim() == 5:                   # val_crops > 1: the view-major validation batch
+                self.val_x = b.x
+            else:
+                self.shared_x = b.x
             nbytes += b.h2d_bytes
         else:
             x = self.data.load_batch(img[idx], mode, self)
-            self.shared_x[:x.shape[0]].copy_(x.to(self.act_dtype), non_blocking=True)
+            if x.dim() == 5:
+                if self.val_x is None:
+                    self.val_x = torch.zeros((x.shape[0], self.file_batch_size) + self.input_shape[1:], dtype=self.act_dtype,
+                                             device=self.device)
+                self.val_x[:, :x.shape[1]].copy_(x.to(self.act_dtype), non_blocking=True)
+            else:
+                self.shared_x[:x.shape[0]].copy_(x.to(self.act_dtype), non_blocking=True)
             nbytes += x.numel() * x.element_size()
         nbytes += self._labels_to_device(labels[idx])
         self.h2d_bytes_last = nbytes

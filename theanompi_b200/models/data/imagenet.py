@@ -174,7 +174,7 @@ class ImageNet_data(object):
         on the same boxes or fixed crops as without it.  With ``model.random_erasing`` a "train" batch, whichever crop made it, then
         gets the loader's erase boxes, drawn from a generator keyed by (seed, rank, 3), set to 0.  With ``model.auto_augment`` a
         "train" batch gets the loader's op records, drawn from a generator keyed by (seed, rank, 2), on the same boxes or fixed
-        crops."""
+        crops.  With ``model.val_crops`` = V > 1 a "val" batch is the view-major [V, N, ...] of ``reference.multi_crop_normalize``."""
         import torch
         from ... import ops
         from .utils import color_jitter_records, color_jitter_rng, crop_and_mirror, draw_crops
@@ -187,6 +187,10 @@ class ImageNet_data(object):
         aa = getattr(model, "auto_augment", None) if mode == "train" else None
         n = raw.shape[0]
         mean, cs = torch.from_numpy(self.rawdata[4]), torch.from_numpy(1.0 / 255.0 / self.rawdata[5])
+        n_views = getattr(model, "val_crops", 1) if mode == "val" else 1
+        if n_views > 1:
+            t = ops.reference.multi_crop_normalize(torch.from_numpy(raw), mean, cs, (model.input_height, model.input_width), n_views)
+            return t.pin_memory().to(model.device, non_blocking=True) if model.cuda else t
         if rrc is not None and mode == "train":
             from .utils import draw_resized_crops, resized_crop_rng
             if getattr(self, "_rrc_rng", None) is None:
@@ -234,19 +238,21 @@ class ImageNet_data(object):
 
     def para_load_init(self, device, input_width, input_height, rand_crop, batch_crop_mirror,
                        out_dtype=None, depth=2, mode=None, resized_crop=None, rank=0, color_jitter=None, random_erasing=None,
-                       auto_augment=None):
+                       auto_augment=None, val_crops=1):
         """``mode='thread'`` (default): loader thread + pinned ring in this process.  ``mode='process'`` (or
         ``TMPI_LOADER=process``): a separate loader process fills a page-locked shared-memory ring (see ``proc_loader.py``) —
         the reference's ``proc_load_mpi.py`` child, minus its second CUDA context.  ``resized_crop`` (a validated
         ``config['random_resized_crop']``), ``color_jitter`` (a validated ``config['color_jitter']``), ``random_erasing`` (a
         validated ``config['random_erasing']``) and ``rank`` go to the :class:`ParaLoader`, which draws the boxes, the colour maps
-        and the erase boxes in this process."""
+        and the erase boxes in this process.  ``val_crops`` > 1 makes it cut that many views of every "val" batch, also in this
+        process."""
         from .loader import ParaLoader
         raw_shape = (self.file_batch_size, self.height, self.width, self.channels)
         mode = mode or os.environ.get("TMPI_LOADER", "thread")
         kw = dict(mean=self.rawdata[4], std_scale=1.0 / 255.0 / self.rawdata[5], out_dtype=out_dtype, depth=depth,
                   rand_crop=rand_crop, batch_crop_mirror=batch_crop_mirror, resized_crop=resized_crop, rank=rank,
-                  color_jitter=color_jitter, random_erasing=random_erasing, auto_augment=auto_augment)
+                  color_jitter=color_jitter, random_erasing=random_erasing, auto_augment=auto_augment,
+                  val_crops=val_crops)
         if mode == "process":
             from .proc_loader import ProcReader
             self.proc_reader = ProcReader(raw_shape, depth=depth, seed=self._seed)

@@ -51,7 +51,7 @@ class ParaLoader(object):
     def __init__(self, read_fn, device, raw_shape, crop_hw, mean, std_scale=1.0 / 255.0,
                  out_dtype=None, depth=2, rand_crop=True, batch_crop_mirror=False, seed=1234,
                  threaded=True, host_buffers=None, on_close=None, resized_crop=None, rank=0, color_jitter=None,
-                 random_erasing=None, auto_augment=None):
+                 random_erasing=None, auto_augment=None, val_crops=1):
         """``resized_crop``: a validated ``config['random_resized_crop']`` (``utils.check_resized_crop``) or None; with it every
         "train" batch is a random-resized crop drawn per image from the generator keyed by (its seed, ``rank``), and "val" batches
         keep the centre crop.  ``color_jitter``: a validated ``config['color_jitter']`` (``utils.check_color_jitter``) or None; with
@@ -62,7 +62,10 @@ class ParaLoader(object):
         launch on the copy stream; "val" batches are never erased.  ``auto_augment``: a validated ``config['auto_augment']``
         (``utils.check_auto_augment``) or None; with it every "train" image gets TrivialAugmentWide / RandAugment op records drawn from
         the generator keyed by (its seed, ``rank``, 2), applied on the uint8 crop of the same boxes or fixed crops between the crop
-        and the normalisation; "val" batches are never augmented."""
+        and the normalisation; "val" batches are never augmented.  ``val_crops``: 1, 2 or 10 (``utils.check_val_crops``); with
+        V > 1 every "val" batch is the view-major [V, N, ch, cw, C] of ``multi_crop_norm`` (``reference.multi_crop_views``), cut by one
+        launch from the staged uint8 batch into a ring of its own (10 × 128 × 227² × 3 × 2 B ≈ 396 MB per slot in bf16, twice that in
+        fp32, times ``depth``, allocated only when V > 1); "train" batches, their slots and draws do not change."""
         self.read_fn = read_fn
         self.device = torch.device(device)
         self.cuda = self.device.type == "cuda"
@@ -132,6 +135,12 @@ class ParaLoader(object):
             self.consumed = [None] * depth
         self.out = [torch.empty((N,) + self.crop_hw + (C,), dtype=self.out_dtype, device=self.device)
                     for _ in range(depth)]
+        # slot s of this ring is slot s of self.out for a "val" batch: the same consumed[s] event guards both
+        self.val_crops = val_crops
+        self.val_out = None
+        if val_crops > 1:
+            self.val_out = [torch.empty((val_crops, N) + self.crop_hw + (C,), dtype=self.out_dtype, device=self.device)
+                            for _ in range(depth)]
         self.h2d_bytes = int(np.prod(self.raw_shape)) + N * 9
         self._req = queue.Queue()
         self._done = queue.Queue()
@@ -161,6 +170,20 @@ class ParaLoader(object):
             # finished before this slot comes round again — recorded below, awaited at the top of the next _produce(s)
             pass
         aa = None
+        if mode == "val" and self.val_crops > 1:
+            # every view from the one staged copy; no draw, so self.rs and the training crops stay the same sequence
+            if self.cuda:
+                with torch.cuda.stream(self.copy_stream):
+                    self.stage[s].copy_(src, non_blocking=True)
+                    from ...ops import cuda_impl
+                    cuda_impl.multi_crop_normalize(self.stage[s], self.mean, self.std_scale, self.crop_hw, self.val_crops,
+                                                   self.out_dtype, out=self.val_out[s])
+                ready = torch.cuda.Event()
+                ready.record(self.copy_stream)
+            else:
+                self.val_out[s].copy_(ops.reference.multi_crop_normalize(src, self.mean, self.std_scale, self.crop_hw, self.val_crops))
+                ready = None
+            return LoadedBatch(self.val_out[s], s, ready, item, self.h2d_bytes)
         if mode == "train" and (self.resized_crop is not None or self.color_jitter is not None or self.auto_augment is not None):
             boxes, flips, records, aa, nbytes = self._produce_boxed(s, src, mode)
         else:

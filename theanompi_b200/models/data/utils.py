@@ -376,6 +376,19 @@ def auto_augment_records(n, cfg, rng, out_hw):
     return rec.astype(np.float32), op, mag
 
 
+VC_KEY = "val_crops"
+
+
+def check_val_crops(v):
+    """The validated ``config['val_crops']``: the int 1 (one centre crop, the default), 2 (the centre crop and its mirror) or 10 (the
+    four corners and the centre, each with its mirror); a bool, a float, a string or any other int is a ValueError that names the
+    key."""
+    from ...ops.reference import MULTI_CROP_VIEWS
+    if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or int(v) not in MULTI_CROP_VIEWS:
+        raise ValueError("%s must be one of the ints %s, not %r" % (VC_KEY, ", ".join(map(str, MULTI_CROP_VIEWS)), v))
+    return int(v)
+
+
 RE_KEY = "random_erasing"
 RE_DEFAULTS = {"p": 0.5, "scale": (0.02, 0.33), "ratio": (0.3, 3.3), "seed": 0}
 RE_ATTEMPTS = 10

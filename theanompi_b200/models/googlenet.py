@@ -136,7 +136,7 @@ class GoogLeNet(ModelBase):
                                      self.batch_crop_mirror, out_dtype=self.act_dtype,
                                      resized_crop=self.resized_crop, rank=self.rank,
                                      color_jitter=self.color_jitter, random_erasing=self.random_erasing,
-                                     auto_augment=self.auto_augment)
+                                     auto_augment=self.auto_augment, val_crops=self.val_crops)
 
     def build_model(self):
         v, B = self.verbose, self.batch_size

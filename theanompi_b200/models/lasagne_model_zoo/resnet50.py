@@ -100,7 +100,7 @@ class ResNet50(ModelBase):
                                      self.batch_crop_mirror, out_dtype=self.act_dtype,
                                      resized_crop=self.resized_crop, rank=self.rank,
                                      color_jitter=self.color_jitter, random_erasing=self.random_erasing,
-                                     auto_augment=self.auto_augment)
+                                     auto_augment=self.auto_augment, val_crops=self.val_crops)
 
     # ---- construction: every conv is bias-free and linear; BatchNormal carries the ReLU (and the shortcut add)
     def _conv(self, inp, cout, k, stride, pad, input_shape=None):
@@ -194,4 +194,4 @@ class ResNet50Torch(TorchModelBase):
                                      self.batch_crop_mirror, out_dtype=self.act_dtype,
                                      resized_crop=self.resized_crop, rank=self.rank,
                                      color_jitter=self.color_jitter, random_erasing=self.random_erasing,
-                                     auto_augment=self.auto_augment)
+                                     auto_augment=self.auto_augment, val_crops=self.val_crops)

@@ -101,7 +101,18 @@ class TorchModelBase(ModelBase):
                 c, e, e5 = self.loss(self.shared_x[subb_ind * B:(subb_ind + 1) * B], self.shared_y[subb_ind * B:(subb_ind + 1) * B])
             self.module.train()
             return c, e, e5
-        self.val_fn = val_fn
+
+        def multi_view_val_fn(subb_ind=0):
+            # val_crops = V > 1: the mean of softmax(logits.float()) over the V views, with the native path's clamp and rank rule
+            from ..ops.reference import view_metrics
+            B, V = self.batch_size, self.val_crops
+            self.module.eval()
+            with torch.no_grad():
+                pbar = sum(torch.softmax(self.forward(self.val_x[v, subb_ind * B:(subb_ind + 1) * B]).float(), dim=1) for v in range(V)) / V
+                c, e, e5 = view_metrics(pbar, self.shared_y[subb_ind * B:(subb_ind + 1) * B])
+            self.module.train()
+            return c, e, e5
+        self.val_fn = val_fn if self.val_crops == 1 else multi_view_val_fn
 
     def compile_iter_fns(self, sync_type="avg", aggregate="momentum", fused_tail=None):
         self.torch_opt = self.make_torch_optimizer(self.params)

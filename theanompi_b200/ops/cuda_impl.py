@@ -869,6 +869,59 @@ def crop_mirror_normalize(x, mean, std_scale, crop_hw, offsets, flips, out_dtype
     return out
 
 
+def multi_crop_normalize(x, mean, std_scale, crop_hw, n_views, out_dtype=None, out=None):
+    """Every test-time view of a uint8 NHWC batch in one launch (``nn_kernels.cu: multi_crop_norm_kernel``): view-major
+    [V, N, ch, cw, C], view v bit-equal to :func:`crop_mirror_normalize` with the view's offsets and mirror flag broadcast.  The view
+    table (:func:`reference.multi_crop_views`) goes to the kernel by value.  Same mean / ``std_scale`` forms as
+    :func:`crop_mirror_normalize`; see :func:`reference.multi_crop_normalize`."""
+    from .reference import multi_crop_views
+    out_dtype = out_dtype or ADT()
+    if x.dtype != torch.uint8 or x.dim() != 4:
+        raise ValueError("multi_crop_normalize takes a uint8 NHWC batch, not %s %s" % (x.dtype, tuple(x.shape)))
+    x = x.contiguous()
+    N, H, W, C = x.shape
+    ch, cw = crop_hw
+    views = multi_crop_views((H, W), crop_hw, n_views).tolist()
+    V = len(views)
+    mean = mean.float().contiguous()
+    mode = 0 if mean.numel() == 1 else (1 if mean.numel() == C else 2)
+    if mode == 2:
+        assert mean.numel() == H * W * C
+    if out is None:
+        out = torch.empty((V, N, ch, cw, C), dtype=out_dtype, device=x.device)
+    assert out.dtype in (BF16, F32) and out.is_contiguous() and tuple(out.shape) == (V, N, ch, cw, C) and out.device == x.device
+    if isinstance(std_scale, torch.Tensor):
+        cs = std_scale.to(device=x.device, dtype=F32).contiguous()
+        assert cs.numel() == C
+        sc, cs_ptr = 1.0, cs.data_ptr()
+    else:
+        sc, cs_ptr = float(std_scale), 0
+    L().multi_crop_norm(x.data_ptr(), mean.data_ptr(), mode, sc, cs_ptr, out.data_ptr(), int(out.dtype == BF16), [v[0] for v in views],
+                        [v[1] for v in views], [v[2] for v in views], N, H, W, C, ch, cw, _st(x))
+    return out
+
+
+def view_softmax_accum(logits, labels, acc, v, n_views, rowstat=None):
+    """View ``v`` of ``n_views`` of multi-view validation (``nn_kernels.cu: view_softmax_accum_kernel``): ``acc`` (fp32 [B, C]) takes
+    softmax(logits) (v = 0) or adds it; the last view divides by V, leaving p̄ in ``acc``, and returns the device scalars (cost, top-1
+    error, top-5 error) of :func:`reference.view_metrics` after one more ``rowstat_mean`` launch; earlier views return None.
+    ``logits``: bf16 or fp32 [B, C]."""
+    lg = logits.contiguous()
+    B, C = lg.shape
+    if lg.dtype not in (BF16, F32):
+        raise ValueError("view_softmax_accum: bf16 or fp32 logits, not %s" % lg.dtype)
+    labels = labels.contiguous()
+    assert labels.dtype == torch.int64 and tuple(labels.shape) == (B,)
+    assert acc.dtype == F32 and acc.is_contiguous() and tuple(acc.shape) == (B, C) and acc.device == lg.device
+    last = v == n_views - 1
+    if rowstat is None:
+        rowstat = torch.empty((B, 3), dtype=F32, device=lg.device)
+    out3 = torch.empty(3, dtype=F32, device=lg.device) if last else None
+    L().view_softmax_accum(lg.data_ptr(), labels.data_ptr(), acc.data_ptr(), rowstat.data_ptr(), _p(out3), B, C, int(v), int(n_views),
+                           int(_is32(lg)), _st(lg))
+    return (out3[0], out3[1], out3[2]) if last else None
+
+
 def resized_crop_mirror_normalize(x, mean, std_scale, out_hw, boxes, flips, out_dtype=None, out=None):
     """Random-resized crop of a uint8 NHWC batch (``nn_kernels.cu: resized_crop_mirror_norm_kernel``): image n's box
     ``boxes[n] = (y0, x0, h, w)`` (int32 [N, 4] on the device, inside the image) normalised, bilinearly resampled to ``out_hw`` and

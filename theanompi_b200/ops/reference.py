@@ -705,6 +705,60 @@ def crop_mirror_normalize(x_u8, mean, std_scale, crop_hw, offsets, flips, out_dt
     return out.to(out_dtype)
 
 
+MULTI_CROP_VIEWS = (1, 2, 10)
+
+
+def multi_crop_views(in_hw, crop_hw, n_views):
+    """The (y0, x0, mirror) table of the ``n_views`` test-time views of a ``crop_hw`` crop of an ``in_hw`` image, int32 [V, 3], in
+    the order of torchvision's ``ten_crop(img, size)``: top-left, top-right, bottom-left, bottom-right, centre, then the same five
+    regions of the horizontally flipped image, whose view k + 5 is (y0_k, dx − x0_k, 1) with dx = W − cw.  V = 2 is views 4 and 9 (the
+    centre crop and the centre crop of the mirrored image); V = 1 is view 4, the validation crop of :func:`crop_mirror_normalize`.
+    The centre is (dy // 2, dx // 2); torchvision's ``center_crop`` anchors at round(d / 2), which differs only when d ≡ 3 (mod 4)."""
+    H, W = in_hw
+    ch, cw = crop_hw
+    dy, dx = H - ch, W - cw
+    if dy < 0 or dx < 0:
+        raise ValueError("multi_crop_views: a %d x %d crop does not fit a %d x %d image" % (ch, cw, H, W))
+    five = [(0, 0), (0, dx), (dy, 0), (dy, dx), (dy // 2, dx // 2)]
+    ten = [(y, x, 0) for y, x in five] + [(y, dx - x, 1) for y, x in five]
+    pick = {1: [4], 2: [4, 9], 10: list(range(10))}
+    if n_views not in pick:
+        raise ValueError("multi_crop_views: n_views must be one of %s, not %r" % (MULTI_CROP_VIEWS, n_views))
+    return torch.tensor([ten[k] for k in pick[n_views]], dtype=torch.int32)
+
+
+def multi_crop_normalize(x_u8, mean, std_scale, crop_hw, n_views, out_dtype=torch.float32):
+    """The ``n_views`` test-time views (:func:`multi_crop_views`) of every image, view-major [V, N, ch, cw, C]: view v is
+    :func:`crop_mirror_normalize` with the view's offsets and mirror flag broadcast to every image."""
+    N, H, W, C = x_u8.shape
+    views = multi_crop_views((H, W), crop_hw, n_views)
+    out = []
+    for y0, x0, m in views.tolist():
+        offs = torch.tensor([[y0, x0]], dtype=torch.int32).expand(N, 2)
+        out.append(crop_mirror_normalize(x_u8, mean, std_scale, crop_hw, offs, torch.full((N,), m, dtype=torch.uint8), out_dtype))
+    return torch.stack(out)
+
+
+def view_metrics(pbar, labels):
+    """(mean −log max(p̄_y, FLT_MIN), top-1 error, top-5 error) of the averaged prediction ``pbar`` [B, C] in its own dtype, with the
+    rank rule of the native kernels: rank = #{p̄_c > p̄_y} + #{c < y : p̄_c = p̄_y}; an error when rank ≥ 1 (top-1) or ≥ 5 (top-5)."""
+    B, C = pbar.shape
+    py = pbar.gather(1, labels.view(B, 1))
+    cols = torch.arange(C, device=pbar.device).view(1, C)
+    rank = ((pbar > py) | ((pbar == py) & (cols < labels.view(B, 1)))).sum(1)
+    cost = -torch.log(py.view(B).clamp_min(float(np.finfo(np.float32).tiny))).mean()
+    return cost, (rank >= 1).to(pbar.dtype).mean(), (rank >= 5).to(pbar.dtype).mean()
+
+
+def multi_view_xent(logits_per_view, labels, dtype=torch.float64):
+    """Multi-view validation of V views' logits (a list of [B, C], or [V, B, C]): p̄ = (1/V)·Σ_v softmax(z_v), each softmax
+    computed in ``dtype``, the probabilities averaged (not the logits, as Krizhevsky et al. 2012 average the ten patches'
+    predictions).  Returns (cost, top-1 error, top-5 error, p̄) with :func:`view_metrics`."""
+    V = len(logits_per_view)
+    pbar = sum(torch.softmax(z.to(dtype), dim=1) for z in logits_per_view) / V
+    return view_metrics(pbar, labels.to(pbar.device)) + (pbar,)
+
+
 def resized_crop_mirror_normalize(x_u8, mean, std_scale, out_hw, boxes, flips, out_dtype=torch.float32):
     """Random-resized crop: ``(x - mean) * std_scale`` (each source pixel with its own mean) → image i's box
     ``boxes[i] = (y0, x0, h, w)`` → ``F.interpolate(size=out_hw, mode='bilinear', align_corners=False, antialias=False)`` → optional
