@@ -193,7 +193,9 @@ void crop_mean(const void* x, const void* boxes, void* mu, int N, int H, int W, 
 // rec = fp32 [N, slots, 12], 16-byte aligned
 void aa_crop_u8(const void* x, void* u, const void* boxes, const void* flips, int N, int H, int W, int ch, int cw, cudaStream_t st);
 void aa_lut(const void* u, const void* rec, void* lut, int slot, int slots, int N, int ch, int cw, cudaStream_t st);
-void aa_apply(const void* in, void* out, const void* rec, const void* lut, int slot, int slots, int N, int ch, int cw, cudaStream_t st);
+void aa_apply(const void* in, void* out, const void* rec, const void* lut, int slot, int slots, int N, int ch, int cw, int bilinear,
+              cudaStream_t st);
+void aa_mix(void* u, const void* chains, const void* rec, const void* weights, int width, int N, int ch, int cw, cudaStream_t st);
 void aa_normalize(const void* u, const void* mean, int mean_mode, float scale, const void* cscale, void* out, int out_bf16, const void* boxes,
                   const void* flips, int N, int W, int ch, int cw, cudaStream_t st);
 // random erasing in place: out (bf16 (out_bf16) or fp32 NHWC [N, ch, cw, C]) is set to 0 inside box n = (i, j, h, w) (int32 [N, 4],

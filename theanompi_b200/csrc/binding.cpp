@@ -162,8 +162,10 @@ PYBIND11_MODULE(_tmpi_native, m) {
     aa_crop_u8(P(x), P(u), P(boxes), P(flips), N, H, W, ch, cw, S(st)); });
   m.def("aa_lut", [](ptr_t u, ptr_t rec, ptr_t lut, int slot, int slots, int N, int ch, int cw, ptr_t st) {
     aa_lut(P(u), P(rec), P(lut), slot, slots, N, ch, cw, S(st)); });
-  m.def("aa_apply", [](ptr_t in, ptr_t out, ptr_t rec, ptr_t lut, int slot, int slots, int N, int ch, int cw, ptr_t st) {
-    aa_apply(P(in), P(out), P(rec), P(lut), slot, slots, N, ch, cw, S(st)); });
+  m.def("aa_apply", [](ptr_t in, ptr_t out, ptr_t rec, ptr_t lut, int slot, int slots, int N, int ch, int cw, int bilinear, ptr_t st) {
+    aa_apply(P(in), P(out), P(rec), P(lut), slot, slots, N, ch, cw, bilinear, S(st)); });
+  m.def("aa_mix", [](ptr_t u, ptr_t chains, ptr_t rec, ptr_t weights, int width, int N, int ch, int cw, ptr_t st) {
+    aa_mix(P(u), P(chains), P(rec), P(weights), width, N, ch, cw, S(st)); });
   m.def("aa_normalize", [](ptr_t u, ptr_t mean, int mean_mode, float scale, ptr_t cscale, ptr_t out, int out_bf16, ptr_t boxes, ptr_t flips,
                            int N, int W, int ch, int cw, ptr_t st) {
     aa_normalize(P(u), P(mean), mean_mode, scale, P(cscale), P(out), out_bf16, P(boxes), P(flips), N, W, ch, cw, S(st)); });

@@ -1910,15 +1910,16 @@ void crop_mean(const void* x, const void* boxes, void* mu, int N, int H, int W, 
   count_launch(); TMPI_CHECK_LAUNCH("crop_mean"); ::tmpi::check_capture(st, "crop_mean");
 }
 
-// ============================================================================ loader: TrivialAugmentWide / RandAugment on the uint8 crop
+// ============================================================================ loader: TrivialAugmentWide / RandAugment / AutoAugment / AugMix
 // torchvision.transforms.v2's uint8 ops, one op slot at a time, on the [N, ch, cw, 3] uint8 crop u.  rec[n] = 12 floats per slot: op id,
-// scalar (factor, Solarize threshold or Posterize bits), 1 − factor (blends), 0, the fp32 inverse affine matrix (6), 0, 0.
+// scalar (factor, Solarize threshold or Posterize bits), 1 − factor (blends), bilinear (0 / 1; the launch argument selects the path),
+// the fp32 inverse affine matrix (6), 0, 0.  AA_NONE is an AugMix chain step past the chain's depth: nothing is written.
 // aa_lut_kernel builds image n's per-channel 256-entry LUT for the point ops (Brightness, Contrast, Posterize, Solarize, AutoContrast,
 // Equalize) from the ping buffer, with the image-wide statistics they need; aa_apply_kernel maps ping → pong; aa_normalize_kernel
 // writes (u' − m̂)·s_c.  The fp32 expressions are torchvision's: a separate multiply and a fused add for the blends (ATen's vectorised
 // a + α·b), truncating casts after a clamp to [0, 255], an fma chain and a floor for the grey level.
 enum AaOp { AA_IDENTITY, AA_SHEARX, AA_SHEARY, AA_TRANSX, AA_TRANSY, AA_ROTATE, AA_BRIGHTNESS, AA_COLOR, AA_CONTRAST, AA_SHARPNESS,
-            AA_POSTERIZE, AA_SOLARIZE, AA_AUTOCONTRAST, AA_EQUALIZE };
+            AA_POSTERIZE, AA_SOLARIZE, AA_AUTOCONTRAST, AA_EQUALIZE, AA_INVERT, AA_NONE };
 constexpr int AA_REC = 12;
 constexpr int AA_LUT_THREADS = 512;
 
@@ -1934,7 +1935,8 @@ __global__ void __launch_bounds__(AA_LUT_THREADS) aa_lut_kernel(const uint8_t* _
   const int n = blockIdx.x, tid = threadIdx.x;
   const float* r = rec + ((long long)n * slots + slot) * AA_REC;
   const int op = (int)r[0];
-  if (!(op == AA_BRIGHTNESS || op == AA_CONTRAST || op == AA_POSTERIZE || op == AA_SOLARIZE || op == AA_AUTOCONTRAST || op == AA_EQUALIZE)) return;
+  if (!(op == AA_BRIGHTNESS || op == AA_CONTRAST || op == AA_POSTERIZE || op == AA_SOLARIZE || op == AA_AUTOCONTRAST || op == AA_EQUALIZE ||
+        op == AA_INVERT)) return;
   const float f = r[1], d = r[2];
   const uint8_t* src = u + (long long)n * P * 3;
   uint8_t* L = lut + (long long)n * 768;
@@ -2003,6 +2005,7 @@ __global__ void __launch_bounds__(AA_LUT_THREADS) aa_lut_kernel(const uint8_t* _
       uint8_t o;
       if (op == AA_BRIGHTNESS) o = aa_clamp_trunc(__fmul_rn((float)v, f));
       else if (op == AA_POSTERIZE) { const int bits = (int)f; o = bits >= 8 ? (uint8_t)v : (uint8_t)(v & (((1 << bits) - 1) << (8 - bits))); }
+      else if (op == AA_INVERT) o = (uint8_t)(255 - v);
       else o = (float)v >= f ? (uint8_t)(255 - v) : (uint8_t)v;      // Solarize
       L[i] = o;
     }
@@ -2010,7 +2013,11 @@ __global__ void __launch_bounds__(AA_LUT_THREADS) aa_lut_kernel(const uint8_t* _
 }
 
 // One CTA per output row (n, oy), like the crop kernels, so the op is CTA-uniform; reads ping, writes pong (never in place: the
-// geometric ops and Sharpness read neighbours).
+// geometric ops and Sharpness read neighbours).  kBilinear selects the geometric ops' resampling: nearest, or torchvision's
+// _apply_grid_transform with fill None, evaluated as ATen's CPU kernels evaluate it: the grid of _affine_grid (the rescaled matrix,
+// then bx·t0 fused into by·t1, then + t2, as the CPU bmm rounds it), grid_sample's unnormalize (g + 1)·(size/2) − ½, the four taps
+// ((nw·v + ne·v) + sw·v) + se·v with separate roundings (a tap outside the image is 0), then round half to even.
+template <bool kBilinear>
 __global__ void __launch_bounds__(128) aa_apply_kernel(const uint8_t* __restrict__ in, uint8_t* __restrict__ out, const float* __restrict__ rec,
                                                        const uint8_t* __restrict__ lut, int slot, int slots, int ch, int cw) {
   const int ox = blockIdx.y * blockDim.x + threadIdx.x;
@@ -2018,10 +2025,31 @@ __global__ void __launch_bounds__(128) aa_apply_kernel(const uint8_t* __restrict
   const int oy = blockIdx.x % ch, n = blockIdx.x / ch;
   const float* r = rec + ((long long)n * slots + slot) * AA_REC;
   const int op = (int)r[0];
+  if (op == AA_NONE) return;
   const uint8_t* img = in + (long long)n * ch * cw * 3;
   const uint8_t* px = img + ((long long)oy * cw + ox) * 3;
   uint8_t* o = out + ((long long)blockIdx.x * cw + ox) * 3;
-  if (op >= AA_SHEARX && op <= AA_ROTATE) {
+  if (kBilinear && op >= AA_SHEARX && op <= AA_ROTATE) {
+    const float bx = (float)ox - 0.5f * (float)(cw - 1), by = (float)oy - 0.5f * (float)(ch - 1);
+    const float hw = 0.5f * (float)cw, hh = 0.5f * (float)ch;
+    const float gx = __fadd_rn(__fmaf_rn(by, __fdiv_rn(r[5], hw), __fmul_rn(bx, __fdiv_rn(r[4], hw))), __fdiv_rn(r[6], hw));
+    const float gy = __fadd_rn(__fmaf_rn(by, __fdiv_rn(r[8], hh), __fmul_rn(bx, __fdiv_rn(r[7], hh))), __fdiv_rn(r[9], hh));
+    const float ix = __fsub_rn(__fmul_rn(__fadd_rn(gx, 1.f), hw), 0.5f), iy = __fsub_rn(__fmul_rn(__fadd_rn(gy, 1.f), hh), 0.5f);
+    const float xw = floorf(ix), yn = floorf(iy);
+    const float w = __fsub_rn(ix, xw), e = __fsub_rn(1.f, w), nn = __fsub_rn(iy, yn), s = __fsub_rn(1.f, nn);
+    const float wt[4] = {__fmul_rn(s, e), __fmul_rn(s, w), __fmul_rn(nn, e), __fmul_rn(nn, w)};   // nw, ne, sw, se
+    const int x0 = (int)xw, y0 = (int)yn;
+    const uint8_t* q[4];
+    for (int t = 0; t < 4; ++t) {
+      const int x = x0 + (t & 1), y = y0 + (t >> 1);
+      q[t] = (x >= 0 && x < cw && y >= 0 && y < ch) ? img + ((long long)y * cw + x) * 3 : nullptr;
+    }
+    for (int c = 0; c < 3; ++c) {
+      float v = 0.f;
+      for (int t = 0; t < 4; ++t) v = t == 0 ? __fmul_rn(q[0] ? (float)q[0][c] : 0.f, wt[0]) : __fadd_rn(v, __fmul_rn(q[t] ? (float)q[t][c] : 0.f, wt[t]));
+      o[c] = (uint8_t)(int)rintf(v);
+    }
+  } else if (op >= AA_SHEARX && op <= AA_ROTATE) {
     // nearest source of torchvision's affine grid: (m0·xb + m1·yb + m2) + (cw − 1)/2 about the centred output coordinates
     const float xb = (float)ox - 0.5f * (float)(cw - 1), yb = (float)oy - 0.5f * (float)(ch - 1);
     const float sx = __fmaf_rn(r[4], xb, __fmaf_rn(r[5], yb, r[6])) + 0.5f * (float)(cw - 1);
@@ -2099,10 +2127,43 @@ void aa_lut(const void* u, const void* rec, void* lut, int slot, int slots, int 
   count_launch(); TMPI_CHECK_LAUNCH("aa_lut"); ::tmpi::check_capture(st, "aa_lut");
 }
 
-void aa_apply(const void* in, void* out, const void* rec, const void* lut, int slot, int slots, int N, int ch, int cw, cudaStream_t st) {
+void aa_apply(const void* in, void* out, const void* rec, const void* lut, int slot, int slots, int N, int ch, int cw, int bilinear,
+              cudaStream_t st) {
   const dim3 g((unsigned)(N * ch), (unsigned)((cw + 127) / 128));
-  aa_apply_kernel<<<g, 128, 0, st>>>((const uint8_t*)in, (uint8_t*)out, (const float*)rec, (const uint8_t*)lut, slot, slots, ch, cw);
+  auto I = (const uint8_t*)in; auto O = (uint8_t*)out; auto R = (const float*)rec; auto Lt = (const uint8_t*)lut;
+  if (bilinear) aa_apply_kernel<true><<<g, 128, 0, st>>>(I, O, R, Lt, slot, slots, ch, cw);
+  else aa_apply_kernel<false><<<g, 128, 0, st>>>(I, O, R, Lt, slot, slots, ch, cw);
   count_launch(); TMPI_CHECK_LAUNCH("aa_apply"); ::tmpi::check_capture(st, "aa_apply");
+}
+
+// AugMix's mix, in place on the crop u: per element acc = m₀·u, then for each chain acc = acc + w_i·c_i (separate fp32 roundings, as
+// torchvision's mix.add_(w * aug)), then a truncating cast to uint8.  chains = [width][2][N, ch, cw, 3]: step s of chain i wrote
+// buffer s & 1, so image n's chain i ends in buffer (depth − 1) & 1, its depth read from its records (AA_NONE steps trail the chain).
+// Elementwise, so in place is safe.
+__global__ void __launch_bounds__(128) aa_mix_kernel(uint8_t* __restrict__ u, const uint8_t* __restrict__ chains, const float* __restrict__ rec,
+                                                     const float* __restrict__ weights, int width, int N, int ch, int cw) {
+  const int ox = blockIdx.y * blockDim.x + threadIdx.x;
+  if (ox >= cw) return;
+  const int n = blockIdx.x / ch;
+  const long long e = ((long long)blockIdx.x * cw + ox) * 3, img = (long long)N * ch * cw * 3;
+  const float* wn = weights + (long long)n * (1 + width);
+  float acc[3];
+  for (int c = 0; c < 3; ++c) acc[c] = __fmul_rn(wn[0], (float)u[e + c]);
+  for (int i = 0; i < width; ++i) {
+    const float* r = rec + ((long long)n * 3 * width + 3 * i) * AA_REC;
+    const int depth = 1 + ((int)r[AA_REC] != AA_NONE) + ((int)r[2 * AA_REC] != AA_NONE);
+    const uint8_t* q = chains + (2 * i + ((depth - 1) & 1)) * img + e;
+    const float wi = wn[1 + i];
+    for (int c = 0; c < 3; ++c) acc[c] = __fadd_rn(acc[c], __fmul_rn(wi, (float)q[c]));
+  }
+  for (int c = 0; c < 3; ++c) u[e + c] = (uint8_t)(int)acc[c];
+}
+
+void aa_mix(void* u, const void* chains, const void* rec, const void* weights, int width, int N, int ch, int cw, cudaStream_t st) {
+  if ((long long)N * ch * cw * 3 * 2 * width >= (1LL << 40) || (long long)N * ch >= (1LL << 31)) throw std::runtime_error("aa_mix: batch too large");
+  const dim3 g((unsigned)(N * ch), (unsigned)((cw + 127) / 128));
+  aa_mix_kernel<<<g, 128, 0, st>>>((uint8_t*)u, (const uint8_t*)chains, (const float*)rec, (const float*)weights, width, N, ch, cw);
+  count_launch(); TMPI_CHECK_LAUNCH("aa_mix"); ::tmpi::check_capture(st, "aa_mix");
 }
 
 void aa_normalize(const void* u, const void* mean, int mean_mode, float scale, const void* cscale, void* out, int out_bf16, const void* boxes,

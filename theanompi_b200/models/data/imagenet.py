@@ -173,8 +173,8 @@ class ImageNet_data(object):
         ``model.color_jitter`` a "train" batch also gets the loader's colour maps, drawn from a generator keyed by (seed, rank, 1),
         on the same boxes or fixed crops as without it.  With ``model.random_erasing`` a "train" batch, whichever crop made it, then
         gets the loader's erase boxes, drawn from a generator keyed by (seed, rank, 3), set to 0.  With ``model.auto_augment`` a
-        "train" batch gets the loader's op records, drawn from a generator keyed by (seed, rank, 2), on the same boxes or fixed
-        crops.  With ``model.val_crops`` = V > 1 a "val" batch is the view-major [V, N, ...] of ``reference.multi_crop_normalize``."""
+        "train" batch gets the loader's op records (and, for "augmix", its mixing weights), drawn from a generator keyed by (seed,
+        rank, 2), on the same boxes or fixed crops.  With ``model.val_crops`` = V > 1 a "val" batch is the view-major [V, N, ...] of ``reference.multi_crop_normalize``."""
         import torch
         from ... import ops
         from .utils import color_jitter_records, color_jitter_rng, crop_and_mirror, draw_crops
@@ -214,11 +214,16 @@ class ImageNet_data(object):
             records = color_jitter_records(n, cj, self._cj_rng)[0]
             t = ops.reference.color_crop_mirror_normalize(torch.from_numpy(raw), mean, cs, out_hw, boxes, flips, records)
         if aa is not None:
-            from .utils import auto_augment_records, auto_augment_rng
+            from .utils import augmix_records, auto_augment_records, auto_augment_rng
             if getattr(self, "_aa_rng", None) is None:
                 self._aa_rng = auto_augment_rng(aa, model.rank)
-            records = auto_augment_records(n, aa, self._aa_rng, out_hw)[0]
-            t = ops.reference.auto_augment_crop_normalize(torch.from_numpy(raw), mean, cs, out_hw, boxes, flips, records)
+            weights = None
+            if aa["policy"] == "augmix":
+                records, weights = augmix_records(n, aa, self._aa_rng, out_hw)[:2]
+            else:
+                records = auto_augment_records(n, aa, self._aa_rng, out_hw)[0]
+            t = ops.reference.auto_augment_crop_normalize(torch.from_numpy(raw), mean, cs, out_hw, boxes, flips, records,
+                                                          weights=weights)
         re_cfg = getattr(model, "random_erasing", None) if mode == "train" else None
         if re_cfg is not None:
             from .utils import draw_erase_boxes, random_erasing_rng

@@ -31,20 +31,24 @@ import numpy as np
 import torch
 
 from ... import ops
-from .utils import (AA_RECORD_FLOATS, CJ_RECORD_FLOATS, auto_augment_records, auto_augment_rng, color_jitter_records, color_jitter_rng, draw_crops, draw_erase_boxes, draw_resized_crops,
-                    random_erasing_rng, resized_crop_rng)
+from .utils import (AA_RECORD_FLOATS, CJ_RECORD_FLOATS, aa_bilinear, aa_slots, augmix_records, auto_augment_records, auto_augment_rng,
+                    color_jitter_records, color_jitter_rng, draw_crops, draw_erase_boxes, draw_resized_crops, random_erasing_rng,
+                    resized_crop_rng)
 
 
 class LoadedBatch(object):
     """One loaded batch; ``boxes`` / ``flips``: the host copies of the random-resized-crop draw it was made with, or of the fixed
     crops as boxes of the output's size under colour jitter (None otherwise); ``records``: the colour-jitter records (None otherwise);
     ``erase``: the random-erasing boxes (i, j, h, w) in output coordinates (None otherwise); ``aa_records``: the auto_augment op
-    records, float32 [N, slots, 12] (None otherwise)."""
-    __slots__ = ("x", "slot", "ready", "item", "h2d_bytes", "boxes", "flips", "records", "erase", "aa_records")
+    records, float32 [N, slots, 12] (None otherwise); ``aa_weights``: AugMix's mixing weights, float32 [N, 1 + width] (None
+    otherwise)."""
+    __slots__ = ("x", "slot", "ready", "item", "h2d_bytes", "boxes", "flips", "records", "erase", "aa_records", "aa_weights")
 
-    def __init__(self, x, slot, ready, item, h2d_bytes, boxes=None, flips=None, records=None, erase=None, aa_records=None):
+    def __init__(self, x, slot, ready, item, h2d_bytes, boxes=None, flips=None, records=None, erase=None, aa_records=None,
+                 aa_weights=None):
         self.x, self.slot, self.ready, self.item, self.h2d_bytes = x, slot, ready, item, h2d_bytes
         self.boxes, self.flips, self.records, self.erase, self.aa_records = boxes, flips, records, erase, aa_records
+        self.aa_weights = aa_weights
 
 
 class ParaLoader(object):
@@ -60,9 +64,10 @@ class ParaLoader(object):
         ``config['random_erasing']`` (``utils.check_random_erasing``) or None; with it every "train" batch, whichever crop path made
         it, gets erase boxes drawn from the generator keyed by (its seed, ``rank``, 3) and zeroed in the output slot by one more
         launch on the copy stream; "val" batches are never erased.  ``auto_augment``: a validated ``config['auto_augment']``
-        (``utils.check_auto_augment``) or None; with it every "train" image gets TrivialAugmentWide / RandAugment op records drawn from
-        the generator keyed by (its seed, ``rank``, 2), applied on the uint8 crop of the same boxes or fixed crops between the crop
-        and the normalisation; "val" batches are never augmented.  ``val_crops``: 1, 2 or 10 (``utils.check_val_crops``); with
+        (``utils.check_auto_augment``) or None; with it every "train" image gets TrivialAugmentWide / RandAugment / AutoAugment / AugMix
+        op records (and AugMix's mixing weights) drawn from the generator keyed by (its seed, ``rank``, 2), applied on the uint8 crop of
+        the same boxes or fixed crops between the crop and the normalisation; "val" batches are never augmented.  Only "augmix"
+        allocates the chains' uint8 ping-pong pairs (2 × width crops) and the weight records.  ``val_crops``: 1, 2 or 10 (``utils.check_val_crops``); with
         V > 1 every "val" batch is the view-major [V, N, ch, cw, C] of ``multi_crop_norm`` (``reference.multi_crop_views``), cut by one
         launch from the staged uint8 batch into a ring of its own (10 × 128 × 227² × 3 × 2 B ≈ 396 MB per slot in bf16, twice that in
         fp32, times ``depth``, allocated only when V > 1); "train" batches, their slots and draws do not change."""
@@ -107,9 +112,13 @@ class ParaLoader(object):
         self.auto_augment = auto_augment
         if auto_augment is not None:
             self.aa_rng = auto_augment_rng(auto_augment, rank)
-            self.aa_slots = 1 if auto_augment["policy"] == "trivial_wide" else auto_augment["num_ops"]
+            self.aa_slots = aa_slots(auto_augment)
+            self.aa_bilinear = aa_bilinear(auto_augment)
             self.host_aa = [torch.empty((N, self.aa_slots, AA_RECORD_FLOATS), dtype=torch.float32, pin_memory=pin)
                             for _ in range(depth)]
+            self.aa_width = auto_augment["mixture_width"] if auto_augment["policy"] == "augmix" else 0
+            if self.aa_width:
+                self.host_aw = [torch.empty((N, 1 + self.aa_width), dtype=torch.float32, pin_memory=pin) for _ in range(depth)]
         boxed = resized_crop is not None or color_jitter is not None or auto_augment is not None
         if boxed:
             self.host_boxes = [torch.empty((N, 4), dtype=torch.int32, pin_memory=pin) for _ in range(depth)]
@@ -126,6 +135,10 @@ class ParaLoader(object):
                 self.aa_lut = torch.empty((N, 3, 256), dtype=torch.uint8, device=self.device)
                 self.dev_aa = [torch.empty((N, self.aa_slots, AA_RECORD_FLOATS), dtype=torch.float32, device=self.device)
                                for _ in range(depth)]
+                if self.aa_width:
+                    # every chain starts from the crop in aa_ping, so the chains step through pairs of their own
+                    self.aa_chains = torch.empty((self.aa_width, 2) + tuple(self.aa_ping.shape), dtype=torch.uint8, device=self.device)
+                    self.dev_aw = [torch.empty((N, 1 + self.aa_width), dtype=torch.float32, device=self.device) for _ in range(depth)]
             if random_erasing is not None:
                 self.dev_erase = [torch.empty((N, 4), dtype=torch.int32, device=self.device) for _ in range(depth)]
             self.stage = [torch.empty(self.raw_shape, dtype=torch.uint8, device=self.device) for _ in range(depth)]
@@ -185,9 +198,9 @@ class ParaLoader(object):
                 ready = None
             return LoadedBatch(self.val_out[s], s, ready, item, self.h2d_bytes)
         if mode == "train" and (self.resized_crop is not None or self.color_jitter is not None or self.auto_augment is not None):
-            boxes, flips, records, aa, nbytes = self._produce_boxed(s, src, mode)
+            boxes, flips, records, aa, aw, nbytes = self._produce_boxed(s, src, mode)
         else:
-            boxes = flips = records = None
+            boxes = flips = records = aw = None
             nbytes = self.h2d_bytes
             offs, fl = draw_crops(N, (H, W), self.crop_hw, mode, self.rand_crop, self.batch_crop_mirror, self.rs)
             self.host_offs[s].numpy()[...] = offs
@@ -222,7 +235,7 @@ class ParaLoader(object):
         if self.cuda:
             ready = torch.cuda.Event()
             ready.record(self.copy_stream)
-        return LoadedBatch(self.out[s], s, ready, item, nbytes, boxes, flips, records, erase, aa)
+        return LoadedBatch(self.out[s], s, ready, item, nbytes, boxes, flips, records, erase, aa, aw)
 
     def _produce_boxed(self, s, src, mode):
         """A "train" batch with ``resized_crop`` or ``color_jitter``: boxes (the random-resized-crop draw, or the fixed crops'
@@ -231,7 +244,9 @@ class ParaLoader(object):
         ``crop_mean`` (only when the contrast strength is > 0, since otherwise K ≡ 0) and ``color_crop_mirror_norm`` (the
         references on the CPU).  Under ``auto_augment`` the op records (48 bytes per image and slot) travel with them and
         ``auto_augment_crop_normalize`` runs instead: the uint8 crop, per slot a LUT launch when a point op is drawn and an apply
-        launch, then the normalisation.  Returns (boxes, flips, colour records or None, op records or None, bytes copied)."""
+        launch, then the normalisation; under "augmix" the weight records (4·(1 + width) bytes per image) travel too and the chains
+        and the mix run between them.  Returns (boxes, flips, colour records or None, op records or None, AugMix weights or None,
+        bytes copied)."""
         N, H, W, C = self.raw_shape
         if self.resized_crop is not None:
             boxes, flips = draw_resized_crops(N, (H, W), self.resized_crop["scale"], self.resized_crop["ratio"], self.rrc_rng)
@@ -246,9 +261,14 @@ class ParaLoader(object):
             records = color_jitter_records(N, self.color_jitter, self.cj_rng)[0]
             self.host_rec[s].numpy()[...] = records
             nbytes += N * 4 * CJ_RECORD_FLOATS
-        aa = None
+        aa = aw = None
         if self.auto_augment is not None:
-            aa, aa_ops, _ = auto_augment_records(N, self.auto_augment, self.aa_rng, self.crop_hw)
+            if self.aa_width:
+                aa, aw, aa_ops, _ = augmix_records(N, self.auto_augment, self.aa_rng, self.crop_hw)
+                self.host_aw[s].numpy()[...] = aw
+                nbytes += aw.nbytes
+            else:
+                aa, aa_ops, _ = auto_augment_records(N, self.auto_augment, self.aa_rng, self.crop_hw)
             self.host_aa[s].numpy()[...] = aa
             nbytes += aa.nbytes
         if self.cuda:
@@ -259,9 +279,15 @@ class ParaLoader(object):
                 from ...ops import cuda_impl
                 if aa is not None:
                     self.dev_aa[s].copy_(self.host_aa[s], non_blocking=True)
+                    dw = None
+                    if aw is not None:
+                        dw = self.dev_aw[s]
+                        dw.copy_(self.host_aw[s], non_blocking=True)
                     cuda_impl.auto_augment_crop_normalize(self.stage[s], self.mean, self.std_scale, self.crop_hw, self.dev_boxes[s],
                                                           self.dev_flip[s], self.dev_aa[s], aa_ops, self.out_dtype, out=self.out[s],
-                                                          ping=self.aa_ping, pong=self.aa_pong, lut=self.aa_lut)
+                                                          ping=self.aa_ping, pong=self.aa_pong, lut=self.aa_lut,
+                                                          bilinear=self.aa_bilinear, weights=dw,
+                                                          chains=self.aa_chains if dw is not None else None)
                 elif records is None:
                     cuda_impl.resized_crop_mirror_normalize(self.stage[s], self.mean, self.std_scale, self.crop_hw, self.dev_boxes[s],
                                                             self.dev_flip[s], self.out_dtype, out=self.out[s])
@@ -275,7 +301,8 @@ class ParaLoader(object):
         else:
             if aa is not None:
                 x = ops.reference.auto_augment_crop_normalize(src, self.mean, self.std_scale, self.crop_hw, self.host_boxes[s],
-                                                              self.host_flip[s], self.host_aa[s], self.out_dtype)
+                                                              self.host_flip[s], self.host_aa[s], self.out_dtype,
+                                                              weights=self.host_aw[s] if aw is not None else None)
             elif records is None:
                 x = ops.reference.resized_crop_mirror_normalize(src, self.mean, self.std_scale, self.crop_hw, self.host_boxes[s],
                                                                 self.host_flip[s], self.out_dtype)
@@ -283,7 +310,7 @@ class ParaLoader(object):
                 x = ops.reference.color_crop_mirror_normalize(src, self.mean, self.std_scale, self.crop_hw, self.host_boxes[s],
                                                               self.host_flip[s], self.host_rec[s], self.out_dtype)
             self.out[s].copy_(x)
-        return boxes, flips, records, aa, nbytes
+        return boxes, flips, records, aa, aw, nbytes
 
     def _run(self):
         if self.cuda:

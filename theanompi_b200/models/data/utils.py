@@ -255,19 +255,61 @@ def color_jitter_maps(factors, order, alpha):
 
 
 AA_KEY = "auto_augment"
-AA_DEFAULTS = {"policy": "trivial_wide", "num_ops": 2, "magnitude": 9, "num_magnitude_bins": 31, "seed": 0}
-AA_POLICIES = ("trivial_wide", "rand")
+AA_DEFAULTS = {"policy": "trivial_wide", "num_ops": 2, "magnitude": 9, "num_magnitude_bins": 31, "seed": 0, "interpolation": None,
+               "severity": 3, "mixture_width": 3, "chain_depth": -1, "alpha": 1.0, "all_ops": True}
+AA_POLICIES = ("trivial_wide", "rand", "autoaugment", "augmix")
+# the keys that belong to some policies only; "seed" and "interpolation" belong to all four
+AA_POLICY_KEYS = {"num_ops": ("rand",), "magnitude": ("rand",), "num_magnitude_bins": ("trivial_wide", "rand"),
+                  "severity": ("augmix",), "mixture_width": ("augmix",), "chain_depth": ("augmix",), "alpha": ("augmix",),
+                  "all_ops": ("augmix",)}
+AA_INTERPOLATIONS = ("nearest", "bilinear")
+# torchvision's default interpolation of each policy
+AA_DEFAULT_INTERPOLATION = {"trivial_wide": "nearest", "rand": "nearest", "autoaugment": "nearest", "augmix": "bilinear"}
 # torchvision's op set of TrivialAugmentWide and RandAugment, in their order; the op id is the index
 AA_OPS = ("Identity", "ShearX", "ShearY", "TranslateX", "TranslateY", "Rotate", "Brightness", "Color", "Contrast", "Sharpness",
           "Posterize", "Solarize", "AutoContrast", "Equalize")
+AA_INVERT = 14                                                 # AutoAugment's Invert, 255 − v
+AA_NONE = 15                                                   # an AugMix chain step past the chain's depth: nothing is done
+AA_OP_IDS = dict({k: i for i, k in enumerate(AA_OPS)}, Invert=AA_INVERT)
 AA_SIGNED = frozenset(AA_OPS[1:10])
-AA_LUT_OPS = frozenset((6, 8, 10, 11, 12, 13))                  # point ops applied through a per-image, per-channel 256-entry LUT
-AA_RECORD_FLOATS = 12                                          # op, scalar, 1 − factor, 0, inverse affine matrix (6), 0, 0: 48 bytes
+AA_LUT_OPS = frozenset((6, 8, 10, 11, 12, 13, AA_INVERT))       # point ops applied through a per-image, per-channel 256-entry LUT
+AA_RECORD_FLOATS = 12                     # op, scalar, 1 − factor, bilinear (0 / 1), inverse affine matrix (6), 0, 0: 48 bytes
+AA_CHAIN_SLOTS = 3                                             # op slots per AugMix chain (the largest chain_depth)
+AA_BINS = 10                                                   # magnitude bins of AutoAugment and AugMix (torchvision's _PARAMETER_MAX)
+# torchvision.transforms.v2.AutoAugment's ImageNet policy: 25 sub-policies of two (op, probability, magnitude bin or None)
+AA_IMAGENET_POLICY = (
+    (("Posterize", 0.4, 8), ("Rotate", 0.6, 9)), (("Solarize", 0.6, 5), ("AutoContrast", 0.6, None)),
+    (("Equalize", 0.8, None), ("Equalize", 0.6, None)), (("Posterize", 0.6, 7), ("Posterize", 0.6, 6)),
+    (("Equalize", 0.4, None), ("Solarize", 0.2, 4)), (("Equalize", 0.4, None), ("Rotate", 0.8, 8)),
+    (("Solarize", 0.6, 3), ("Equalize", 0.6, None)), (("Posterize", 0.8, 5), ("Equalize", 1.0, None)),
+    (("Rotate", 0.2, 3), ("Solarize", 0.6, 8)), (("Equalize", 0.6, None), ("Posterize", 0.4, 6)),
+    (("Rotate", 0.8, 8), ("Color", 0.4, 0)), (("Rotate", 0.4, 9), ("Equalize", 0.6, None)),
+    (("Equalize", 0.0, None), ("Equalize", 0.8, None)), (("Invert", 0.6, None), ("Equalize", 1.0, None)),
+    (("Color", 0.6, 4), ("Contrast", 1.0, 8)), (("Rotate", 0.8, 8), ("Color", 1.0, 2)),
+    (("Color", 0.8, 8), ("Solarize", 0.8, 7)), (("Sharpness", 0.4, 7), ("Invert", 0.6, None)),
+    (("ShearX", 0.6, 5), ("Equalize", 1.0, None)), (("Color", 0.4, 0), ("Equalize", 0.6, None)),
+    (("Equalize", 0.4, None), ("Solarize", 0.2, 4)), (("Solarize", 0.6, 5), ("AutoContrast", 0.6, None)),
+    (("Invert", 0.6, None), ("Equalize", 1.0, None)), (("Color", 0.6, 4), ("Contrast", 1.0, 8)),
+    (("Equalize", 0.8, None), ("Equalize", 0.6, None)))
+# torchvision's AugMix op spaces, in their order: _PARTIAL_AUGMENTATION_SPACE (all_ops False) and _AUGMENTATION_SPACE
+AA_AUGMIX_OPS = ("ShearX", "ShearY", "TranslateX", "TranslateY", "Rotate", "Posterize", "Solarize", "AutoContrast", "Equalize",
+                 "Brightness", "Color", "Contrast", "Sharpness")
+AA_AUGMIX_PARTIAL = 9
+
+
+def _aa_int(cfg, k):
+    v = cfg.get(k, AA_DEFAULTS[k])
+    if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+        raise ValueError("%s[%r] must be an int, not %r" % (AA_KEY, k, v))
+    return int(v)
 
 
 def check_auto_augment(cfg):
-    """The validated ``config['auto_augment']`` with every key filled in, or None for None; anything else is a ValueError that names
-    the key.  ``num_ops`` and ``magnitude`` belong to the "rand" policy only."""
+    """The validated ``config['auto_augment']`` with every key of its policy filled in, or None for None; anything else is a
+    ValueError that names the key.  ``num_ops`` and ``magnitude`` belong to "rand", ``num_magnitude_bins`` to "trivial_wide" and
+    "rand", ``severity``, ``mixture_width``, ``chain_depth``, ``alpha`` and ``all_ops`` to "augmix".  ``interpolation`` ("nearest"
+    or "bilinear") is accepted by every policy; it is filled in for "autoaugment" and "augmix", and kept for "trivial_wide" and
+    "rand" only when given, so their validated dicts are what they always were (:func:`aa_bilinear` reads it)."""
     if cfg is None:
         return None
     if not isinstance(cfg, dict):
@@ -278,26 +320,54 @@ def check_auto_augment(cfg):
     policy = cfg.get("policy", AA_DEFAULTS["policy"])
     if policy not in AA_POLICIES:
         raise ValueError("%s['policy'] must be one of %s, not %r" % (AA_KEY, ", ".join(AA_POLICIES), policy))
-    if policy == "trivial_wide":
-        for k in ("num_ops", "magnitude"):
-            if k in cfg:
-                raise ValueError("%s[%r] belongs to policy 'rand', not 'trivial_wide'" % (AA_KEY, k))
+    for k, owners in AA_POLICY_KEYS.items():
+        if k in cfg and policy not in owners:
+            raise ValueError("%s[%r] belongs to policy %s, not %r" % (AA_KEY, k, " / ".join(repr(p) for p in owners), policy))
     out = {"policy": policy}
-    for k in ("num_magnitude_bins", "num_ops", "magnitude", "seed"):
-        v = cfg.get(k, AA_DEFAULTS[k])
-        if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
-            raise ValueError("%s[%r] must be an int, not %r" % (AA_KEY, k, v))
-        out[k] = int(v)
-    if out["num_magnitude_bins"] < 2:
-        raise ValueError("%s['num_magnitude_bins'] must be >= 2, not %r" % (AA_KEY, out["num_magnitude_bins"]))
-    if not 1 <= out["num_ops"] <= 4:
-        raise ValueError("%s['num_ops'] must lie in [1, 4], not %r" % (AA_KEY, out["num_ops"]))
-    if not 0 <= out["magnitude"] <= out["num_magnitude_bins"] - 1:
-        raise ValueError("%s['magnitude'] must lie in [0, num_magnitude_bins - 1], not %r" % (AA_KEY, out["magnitude"]))
-    out["seed"] &= 2 ** 64 - 1
-    if policy == "trivial_wide":
-        del out["num_ops"], out["magnitude"]
+    if policy in ("trivial_wide", "rand"):
+        for k in ("num_magnitude_bins", "num_ops", "magnitude", "seed"):
+            out[k] = _aa_int(cfg, k)
+        if out["num_magnitude_bins"] < 2:
+            raise ValueError("%s['num_magnitude_bins'] must be >= 2, not %r" % (AA_KEY, out["num_magnitude_bins"]))
+        if not 1 <= out["num_ops"] <= 4:
+            raise ValueError("%s['num_ops'] must lie in [1, 4], not %r" % (AA_KEY, out["num_ops"]))
+        if not 0 <= out["magnitude"] <= out["num_magnitude_bins"] - 1:
+            raise ValueError("%s['magnitude'] must lie in [0, num_magnitude_bins - 1], not %r" % (AA_KEY, out["magnitude"]))
+        if policy == "trivial_wide":
+            del out["num_ops"], out["magnitude"]
+    elif policy == "augmix":
+        for k, lo, hi in (("severity", 1, 10), ("mixture_width", 1, 4), ("chain_depth", -1, 3)):
+            out[k] = _aa_int(cfg, k)
+            if not lo <= out[k] <= hi or (k == "chain_depth" and out[k] == 0):
+                raise ValueError("%s[%r] must lie in [%d, %d]%s, not %r" % (AA_KEY, k, lo, hi, " and not be 0" if k == "chain_depth"
+                                                                            else "", cfg.get(k)))
+        alpha = cfg.get("alpha", AA_DEFAULTS["alpha"])
+        if not _real(alpha) or not 0.0 < float(alpha) <= 16.0:
+            raise ValueError("%s['alpha'] must be a finite real number in (0, 16], not %r" % (AA_KEY, alpha))
+        out["alpha"] = float(alpha)
+        all_ops = cfg.get("all_ops", AA_DEFAULTS["all_ops"])
+        if not isinstance(all_ops, (bool, np.bool_)):
+            raise ValueError("%s['all_ops'] must be a bool, not %r" % (AA_KEY, all_ops))
+        out["all_ops"] = bool(all_ops)
+    if policy in ("autoaugment", "augmix") or "interpolation" in cfg:
+        interp = cfg.get("interpolation", AA_DEFAULT_INTERPOLATION[policy])
+        if interp not in AA_INTERPOLATIONS:
+            raise ValueError("%s['interpolation'] must be one of %s, not %r" % (AA_KEY, ", ".join(AA_INTERPOLATIONS), interp))
+        out["interpolation"] = interp
+    out["seed"] = _aa_int(cfg, "seed") & (2 ** 64 - 1)
     return out
+
+
+def aa_bilinear(cfg):
+    """Whether a validated ``auto_augment`` config resamples its geometric ops bilinearly (torchvision's default per policy)."""
+    return cfg.get("interpolation", AA_DEFAULT_INTERPOLATION[cfg["policy"]]) == "bilinear"
+
+
+def aa_slots(cfg):
+    """Op slots per image of a validated ``auto_augment`` config: 1 ("trivial_wide"), ``num_ops`` ("rand"), 2 ("autoaugment") or
+    3 per chain ("augmix")."""
+    return {"trivial_wide": 1, "autoaugment": 2}.get(cfg["policy"]) or (
+        cfg["num_ops"] if cfg["policy"] == "rand" else AA_CHAIN_SLOTS * cfg["mixture_width"])
 
 
 def auto_augment_rng(cfg, rank):
@@ -305,21 +375,26 @@ def auto_augment_rng(cfg, rank):
     return np.random.default_rng([cfg["seed"], int(rank), 2])
 
 
-def auto_augment_space(policy, num_bins, out_hw):
+def auto_augment_space(policy, num_bins, out_hw, all_ops=True):
     """{op name: (magnitudes float64 [num_bins] or None, signed)}: torchvision's ``_AUGMENTATION_SPACE`` of ``TrivialAugmentWide``
-    ("trivial_wide") or ``RandAugment`` ("rand") for an image of ``out_hw``, computed as torchvision computes it (fp32 linspace)."""
+    ("trivial_wide"), ``RandAugment`` ("rand"), ``AutoAugment`` ("autoaugment": RandAugment's without Identity, with Invert) or
+    ``AugMix`` ("augmix"; its ``_PARTIAL_AUGMENTATION_SPACE`` when not ``all_ops``) for an image of ``out_hw``, in torchvision's
+    order, computed as torchvision computes it (fp32 linspace)."""
     import torch
     h, w = out_hw
     lin = lambda hi, lo=0.0: torch.linspace(lo, hi, num_bins).double().numpy()  # noqa: E731
+    bits = lambda top, post: (top - (torch.arange(num_bins) / ((num_bins - 1) / post))).round().int().double().numpy()  # noqa: E731
     if policy == "trivial_wide":
-        geo, shear, rot, col, post = (lin(32.0), lin(32.0)), lin(0.99), lin(135.0), lin(0.99), 6
+        geo, shear, rot, col, post = (lin(32.0), lin(32.0)), lin(0.99), lin(135.0), lin(0.99), bits(8, 6)
+    elif policy == "augmix":
+        geo, shear, rot, col, post = (lin(w / 3.0), lin(h / 3.0)), lin(0.3), lin(30.0), lin(0.9), bits(4, 4)
     else:
-        geo, shear, rot, col, post = (lin(150.0 / 331.0 * w), lin(150.0 / 331.0 * h)), lin(0.3), lin(30.0), lin(0.9), 4
-    bits = (8 - (torch.arange(num_bins) / ((num_bins - 1) / post))).round().int().double().numpy()
+        geo, shear, rot, col, post = (lin(150.0 / 331.0 * w), lin(150.0 / 331.0 * h)), lin(0.3), lin(30.0), lin(0.9), bits(8, 4)
     mags = {"Identity": None, "ShearX": shear, "ShearY": shear, "TranslateX": geo[0], "TranslateY": geo[1], "Rotate": rot,
-            "Brightness": col, "Color": col, "Contrast": col, "Sharpness": col, "Posterize": bits, "Solarize": lin(0.0, 1.0),
-            "AutoContrast": None, "Equalize": None}
-    return {k: (mags[k], k in AA_SIGNED) for k in AA_OPS}
+            "Brightness": col, "Color": col, "Contrast": col, "Sharpness": col, "Posterize": post, "Solarize": lin(0.0, 1.0),
+            "AutoContrast": None, "Equalize": None, "Invert": None}
+    names = {"autoaugment": AA_OPS[1:] + ("Invert",), "augmix": AA_AUGMIX_OPS if all_ops else AA_AUGMIX_OPS[:AA_AUGMIX_PARTIAL]}
+    return {k: (mags[k], k in AA_SIGNED) for k in names.get(policy, AA_OPS)}
 
 
 def inverse_affine_matrix(center, angle, translate, shear):
@@ -347,8 +422,27 @@ def auto_augment_records(n, cfg, rng, out_hw):
     the blends; the fp32 inverse affine matrix of ShearX / ShearY (shear degrees(atan m) about (0, 0)), TranslateX / TranslateY
     (int(m) pixels) and Rotate (about the centre).
 
+    "autoaugment" draws a sub-policy of :data:`AA_IMAGENET_POLICY` per image (uniform over the 25); each of its two ops applies iff
+    U ≤ p (torchvision's ``torch.rand(()) <= probability``) and is an Identity record otherwise; signed ops are negated with p = ½.
+    "augmix" is :func:`augmix_records`, whose weights this function drops.  Geometric records of a bilinear config carry 1 in
+    field 3.
+
     Returns (records float32 [n, slots, 12], op int64 [n, slots], magnitude float64 [n, slots], the signed magnitude each op uses)."""
-    h, w = out_hw
+    if cfg["policy"] == "augmix":
+        rec, _, op, mag = augmix_records(n, cfg, rng, out_hw)
+        return rec, op, mag
+    if cfg["policy"] == "autoaugment":
+        space = auto_augment_space("autoaugment", AA_BINS, out_hw)
+        names = [[AA_OP_IDS[o] for o, _, _ in sub] for sub in AA_IMAGENET_POLICY]
+        prob = np.array([[p for _, p, _ in sub] for sub in AA_IMAGENET_POLICY])
+        mags = np.array([[space[o][0][b] if b is not None else 0.0 for o, _, b in sub] for sub in AA_IMAGENET_POLICY])
+        signed = np.array([[space[o][1] for o, _, _ in sub] for sub in AA_IMAGENET_POLICY])
+        sub = rng.integers(0, len(AA_IMAGENET_POLICY), n)
+        applies = rng.random((n, 2)) <= prob[sub]
+        neg = rng.random((n, 2)) <= 0.5
+        op = np.where(applies, np.array(names)[sub], 0)
+        mag = np.where(applies, np.where(signed[sub] & neg, -mags[sub], mags[sub]), 0.0)
+        return aa_compose_records(op, mag, out_hw, aa_bilinear(cfg)), op, mag
     space = auto_augment_space(cfg["policy"], cfg["num_magnitude_bins"], out_hw)
     slots = 1 if cfg["policy"] == "trivial_wide" else cfg["num_ops"]
     op = rng.integers(0, len(AA_OPS), (n, slots))
@@ -361,7 +455,44 @@ def auto_augment_records(n, cfg, rng, out_hw):
     signed = np.array([space[k][1] for k in AA_OPS])
     mag = table[op, bins]
     mag = np.where(signed[op] & neg, -mag, mag)
-    rec = np.zeros((n, slots, AA_RECORD_FLOATS), np.float64)
+    return aa_compose_records(op, mag, out_hw, aa_bilinear(cfg)), op, mag
+
+
+def augmix_records(n, cfg, rng, out_hw):
+    """The AugMix draw of one batch ("augmix" configs), all at once: per image m = Dirichlet(α, α) and d = Dirichlet(α·1_width);
+    per chain a depth (``chain_depth``, or uniform over {1, 2, 3} for −1); per chain step an op uniform over the space
+    (:func:`auto_augment_space`, 13 or 9 ops), a magnitude bin uniform over [0, severity) and a sign (negative with p = ½, signed ops
+    only).  Chain i's steps are slots 3i … 3i + 2; a step past its chain's depth is :data:`AA_NONE`.  The weights are computed in fp32
+    as torchvision's ``AugMix.forward`` computes them: m₀ = fl32(m₀) and w_i = fl32(d_i)·fl32(m₁).
+
+    Returns (records float32 [n, 3·width, 12], weights float32 [n, 1 + width] = (m₀, w_0 … w_{width−1}), op int64 [n, 3·width],
+    magnitude float64 [n, 3·width])."""
+    width, alpha = cfg["mixture_width"], cfg["alpha"]
+    space = auto_augment_space("augmix", AA_BINS, out_hw, cfg["all_ops"])
+    names = list(space)
+    m = rng.dirichlet([alpha, alpha], n).astype(np.float32)
+    d = rng.dirichlet([alpha] * width, n).astype(np.float32)
+    if cfg["chain_depth"] > 0:
+        depth = np.full((n, width), cfg["chain_depth"])
+    else:
+        depth = rng.integers(1, AA_CHAIN_SLOTS + 1, (n, width))
+    k = rng.integers(0, len(names), (n, width, AA_CHAIN_SLOTS))
+    bins = rng.integers(0, cfg["severity"], (n, width, AA_CHAIN_SLOTS))
+    neg = rng.random((n, width, AA_CHAIN_SLOTS)) <= 0.5
+    table = np.stack([space[o][0] if space[o][0] is not None else np.zeros(AA_BINS) for o in names])
+    signed = np.array([space[o][1] for o in names])
+    live = np.arange(AA_CHAIN_SLOTS) < depth[..., None]
+    op = np.where(live, np.array([AA_OP_IDS[o] for o in names])[k], AA_NONE).reshape(n, -1)
+    mag = np.where(live, np.where(signed[k] & neg, -table[k, bins], table[k, bins]), 0.0).reshape(n, -1)
+    weights = np.concatenate([m[:, :1], d * m[:, 1:]], 1)
+    return aa_compose_records(op, mag, out_hw, aa_bilinear(cfg)), weights, op, mag
+
+
+def aa_compose_records(op, mag, out_hw, bilinear=False):
+    """The float32 [..., 12] records of op ids ``op`` at signed magnitudes ``mag`` (see :func:`auto_augment_records`), composed in
+    float64 and rounded once; field 3 is 1 for a geometric op when ``bilinear``."""
+    h, w = out_hw
+    rec = np.zeros(op.shape + (AA_RECORD_FLOATS,), np.float64)
     rec[..., 0] = op
     factor = 1.0 + mag
     blend = (op >= 6) & (op <= 9)
@@ -372,8 +503,10 @@ def auto_augment_records(n, cfg, rng, out_hw):
     mats = inverse_affine_matrix(centre, np.where(op == 5, -mag, 0.0),
                                  (np.where(op == 3, np.trunc(mag), 0.0), np.where(op == 4, np.trunc(mag), 0.0)),
                                  (np.where(op == 1, deg, 0.0), np.where(op == 2, deg, 0.0)))
-    rec[..., 4:10] = np.where(((op >= 1) & (op <= 5))[..., None], mats, 0.0)
-    return rec.astype(np.float32), op, mag
+    geo = (op >= 1) & (op <= 5)
+    rec[..., 3] = np.where(geo & bool(bilinear), 1.0, 0.0)
+    rec[..., 4:10] = np.where(geo[..., None], mats, 0.0)
+    return rec.astype(np.float32)
 
 
 VC_KEY = "val_crops"

@@ -1039,15 +1039,31 @@ def aa_lut(u, records, slot, out=None):
     return out
 
 
-def aa_apply(u, records, slot, lut, out=None):
-    """One op slot on the uint8 crop (``aa_apply_kernel``), ``u`` → ``out`` (never in place)."""
+def aa_apply(u, records, slot, lut, out=None, bilinear=False):
+    """One op slot on the uint8 crop (``aa_apply_kernel``), ``u`` → ``out`` (never in place); ``bilinear`` resamples the geometric ops
+    bilinearly (``aa_apply_kernel<true>``).  An image whose op in ``slot`` is AA_NONE leaves its part of ``out`` untouched."""
     _aa_records(records, u)
     N, ch, cw, _ = u.shape
     if out is None:
         out = torch.empty_like(u)
     assert out.data_ptr() != u.data_ptr() and out.shape == u.shape and out.is_contiguous()
-    L().aa_apply(u.data_ptr(), out.data_ptr(), records.data_ptr(), lut.data_ptr(), int(slot), records.shape[1], N, ch, cw, _st(u))
+    L().aa_apply(u.data_ptr(), out.data_ptr(), records.data_ptr(), lut.data_ptr(), int(slot), records.shape[1], N, ch, cw, int(bool(bilinear)),
+                 _st(u))
     return out
+
+
+def aa_mix(u, chains, records, weights):
+    """AugMix's mix in place on the uint8 crop ``u`` (``aa_mix_kernel``): u = trunc(m₀·u + Σ w_i·chain_i) in fp32, chain i read from
+    ``chains[i, (depth − 1) & 1]`` with its depth from ``records`` (AA_NONE steps).  ``chains``: uint8 [width, 2, N, ch, cw, 3];
+    ``records``: [N, 3·width, 12]; ``weights``: fp32 [N, 1 + width] on the device.  One launch.  See :func:`reference.augmix_mix`."""
+    _aa_records(records, u)
+    N, ch, cw, _ = u.shape
+    width = records.shape[1] // 3
+    assert records.shape[1] == 3 * width and tuple(chains.shape) == (width, 2) + tuple(u.shape) and chains.dtype == torch.uint8
+    assert chains.is_contiguous() and u.is_contiguous() and chains.device == u.device
+    assert weights.dtype == torch.float32 and weights.is_contiguous() and tuple(weights.shape) == (N, 1 + width) and weights.device == u.device
+    L().aa_mix(u.data_ptr(), chains.data_ptr(), records.data_ptr(), weights.data_ptr(), width, N, ch, cw, _st(u))
+    return u
 
 
 def aa_normalize(u, mean, std_scale, boxes, flips, in_hw, out_dtype=None, out=None):
@@ -1076,23 +1092,47 @@ def aa_normalize(u, mean, std_scale, boxes, flips, in_hw, out_dtype=None, out=No
 
 
 def auto_augment_crop_normalize(x, mean, std_scale, out_hw, boxes, flips, records, ops=None, out_dtype=None, out=None, ping=None,
-                                pong=None, lut=None):
-    """TrivialAugmentWide / RandAugment on the crop, then normalisation: :func:`aa_crop_u8` into ``ping``; per op slot
+                                pong=None, lut=None, bilinear=None, weights=None, chains=None):
+    """TrivialAugmentWide / RandAugment / AutoAugment on the crop, then normalisation: :func:`aa_crop_u8` into ``ping``; per op slot
     :func:`aa_lut` (only when an image's op in the slot is a point op; ``ops`` = the host's int [N, slots] op ids, read from
-    ``records`` when None) and :func:`aa_apply` ping → pong, swapping; then :func:`aa_normalize`.  Launches:
-    1 + Σ over slots of (1 if a point op is drawn, + 1) + 1.  See :func:`reference.auto_augment_crop_normalize`."""
-    from ..models.data.utils import AA_LUT_OPS
+    ``records`` when None) and :func:`aa_apply` ping → pong, swapping; then :func:`aa_normalize`.  ``bilinear``: the geometric ops'
+    interpolation (read from ``records`` when None).  Launches: 1 + Σ over slots of (1 if a point op is drawn, + 1) + 1.
+
+    AugMix, with ``weights`` (fp32 [N, 1 + width] on the device): the slots are ``width`` chains of 3, and ``ping`` (the crop u)
+    survives them.  Step s of chain i maps u (s = 0) or ``chains[i, (s − 1) & 1]`` to ``chains[i, s & 1]`` (``chains``: uint8
+    [width, 2, N, ch, cw, 3]); a step that no image of the batch reaches is not launched, and an image whose chain has ended
+    (AA_NONE) returns at once, so a short chain costs no copy.  :func:`aa_mix` then mixes in place into ``ping``.  Launches:
+    1 + Σ over slots of (1 if a point op is drawn, + 1 if any image's op is not AA_NONE) + 1 (mix) + 1.
+    See :func:`reference.auto_augment_crop_normalize`."""
+    from ..models.data.utils import AA_LUT_OPS, AA_NONE
     N, H, W, _ = x.shape
     ch, cw = out_hw
     if ops is None:
         ops = records[..., 0].to("cpu", torch.int64).numpy()
+    if bilinear is None:
+        bilinear = bool((records[..., 3] != 0).any())
     ping = aa_crop_u8(x, out_hw, boxes, flips, out=ping)
-    pong = pong if pong is not None else torch.empty_like(ping)
     lut = lut if lut is not None else torch.empty((N, 3, 256), dtype=torch.uint8, device=x.device)
+    if weights is not None:
+        width = records.shape[1] // 3
+        if chains is None:
+            chains = torch.empty((width, 2) + tuple(ping.shape), dtype=torch.uint8, device=x.device)
+        for slot in range(records.shape[1]):
+            i, s = divmod(slot, 3)
+            live = [int(o) for o in ops[:, slot] if int(o) != AA_NONE]
+            if not live:
+                continue
+            src = ping if s == 0 else chains[i, (s - 1) & 1]
+            if any(o in AA_LUT_OPS for o in live):
+                aa_lut(src, records, slot, out=lut)
+            aa_apply(src, records, slot, lut, out=chains[i, s & 1], bilinear=bilinear)
+        aa_mix(ping, chains, records, weights)
+        return aa_normalize(ping, mean, std_scale, boxes, flips, (H, W), out_dtype, out=out)
+    pong = pong if pong is not None else torch.empty_like(ping)
     for slot in range(records.shape[1]):
         if any(int(o) in AA_LUT_OPS for o in ops[:, slot]):
             aa_lut(ping, records, slot, out=lut)
-        aa_apply(ping, records, slot, lut, out=pong)
+        aa_apply(ping, records, slot, lut, out=pong, bilinear=bilinear)
         ping, pong = pong, ping
     return aa_normalize(ping, mean, std_scale, boxes, flips, (H, W), out_dtype, out=out)
 

@@ -609,10 +609,12 @@ def random_erase(x, boxes):
     return ref.random_erase(x, boxes)
 
 
-def auto_augment_crop_normalize(x, mean, std_scale, out_hw, boxes, flips, records, out_dtype=None):
-    """TrivialAugmentWide / RandAugment on the crop of a uint8 NHWC batch, then normalisation: the native kernels on CUDA,
-    :func:`reference.auto_augment_crop_normalize` on the CPU."""
+def auto_augment_crop_normalize(x, mean, std_scale, out_hw, boxes, flips, records, out_dtype=None, weights=None):
+    """TrivialAugmentWide / RandAugment / AutoAugment, or AugMix with ``weights``, on the crop of a uint8 NHWC batch, then
+    normalisation: the native kernels on CUDA, :func:`reference.auto_augment_crop_normalize` on the CPU."""
     if x.is_cuda:
         from . import cuda_impl
-        return cuda_impl.auto_augment_crop_normalize(x, mean, std_scale, out_hw, boxes, flips, records, out_dtype=out_dtype)
-    return ref.auto_augment_crop_normalize(x, mean, std_scale, out_hw, boxes, flips, records, out_dtype or torch.float32)
+        return cuda_impl.auto_augment_crop_normalize(x, mean, std_scale, out_hw, boxes, flips, records, out_dtype=out_dtype,
+                                                     weights=weights)
+    return ref.auto_augment_crop_normalize(x, mean, std_scale, out_hw, boxes, flips, records, out_dtype or torch.float32,
+                                           weights=weights)

@@ -843,16 +843,24 @@ def _aa_gray(img):
 
 
 def aa_apply_op(img, rec):
-    """One op of TrivialAugmentWide / RandAugment on a uint8 CHW image (C = 3), as ``torchvision.transforms.v2.functional`` computes it
-    (nearest interpolation, fill 0), from its 12-float record (``models/data/utils.py: auto_augment_records``): op id, scalar (factor,
-    Solarize threshold or Posterize bits), 1 − factor, 0, the fp32 inverse affine matrix."""
+    """One op of TrivialAugmentWide / RandAugment / AutoAugment / AugMix on a uint8 CHW image (C = 3), as
+    ``torchvision.transforms.v2.functional`` computes it (fill 0), from its 12-float record (``models/data/utils.py:
+    auto_augment_records``): op id, scalar (factor, Solarize threshold or Posterize bits), 1 − factor, the interpolation of a
+    geometric op (0 nearest, 1 bilinear), the fp32 inverse affine matrix.  Invert (op 14) is 255 − v; op 15 (an AugMix step past its
+    chain's depth) returns the image as it is.
+
+    The bilinear geometry is torchvision's ``_apply_grid_transform`` with fill None: ``grid_sample(mode="bilinear",
+    padding_mode="zeros", align_corners=False)`` of the fp32 image (a tap outside the image contributes 0), ``round_()`` (half to
+    even) and a cast to uint8."""
     import torch.nn.functional as F
     rec = [float(v) for v in rec]
     op, f, d = int(rec[0]), rec[1], rec[2]
     C, h, w = img.shape
-    if op == 0:
+    if op == 0 or op == 15:
         return img.clone()
-    if 1 <= op <= 5:                                          # torchvision's _affine_grid and grid_sample(nearest, zeros)
+    if op == 14:
+        return 255 - img
+    if 1 <= op <= 5:                                          # torchvision's _affine_grid and grid_sample(nearest / bilinear, zeros)
         theta = torch.tensor(rec[4:10], dtype=torch.float32).reshape(1, 2, 3)
         base = torch.empty(1, h, w, 3, dtype=torch.float32)
         base[..., 0].copy_(torch.linspace((1.0 - w) * 0.5, (w - 1.0) * 0.5, steps=w))
@@ -860,7 +868,8 @@ def aa_apply_op(img, rec):
         base[..., 2].fill_(1)
         rescaled = theta.transpose(1, 2).div_(torch.tensor([0.5 * w, 0.5 * h], dtype=torch.float32))
         grid = base.view(1, h * w, 3).bmm(rescaled).view(1, h, w, 2)
-        out = F.grid_sample(img.float().unsqueeze(0), grid, mode="nearest", padding_mode="zeros", align_corners=False)
+        mode = "bilinear" if rec[3] != 0.0 else "nearest"
+        out = F.grid_sample(img.float().unsqueeze(0), grid, mode=mode, padding_mode="zeros", align_corners=False)
         return out[0].round_().to(torch.uint8)
     if op == 6:
         return img.mul(f).clamp_(0, 255).to(torch.uint8)
@@ -905,10 +914,23 @@ def aa_apply_op(img, rec):
     raise ValueError("aa_apply_op: unknown op %d" % op)
 
 
-def auto_augment_crop_normalize(x_u8, mean, std_scale, out_hw, boxes, flips, records, out_dtype=torch.float32):
-    """TrivialAugmentWide / RandAugment on the (resized) crop, then normalisation: u = :func:`aa_crop_u8`; each op slot of
-    ``records[i]`` (float32 [N, slots, 12]) applied in order by :func:`aa_apply_op`; out = (u' − m̂) * std_scale with m̂ the bilinear
-    resample of a per-pixel mean over the same (mirrored) box (a [C] or scalar mean as it is).  Fill pixels become −m̂ * std_scale."""
+def augmix_mix(u, chains, weights):
+    """AugMix's mix of one image, as torchvision's ``AugMix.forward`` computes it in fp32: mix = m₀·u, then mix.add_(w_i·chain_i)
+    for each chain in order (a separate multiply and add each), then ``.to(uint8)``, which truncates.  ``u`` and ``chains[i]``: uint8
+    tensors of one shape; ``weights``: (m₀, w_0, …) as fp32."""
+    wt = torch.as_tensor(weights).float().cpu()
+    mix = wt[0] * u
+    for i, c in enumerate(chains):
+        mix.add_(wt[1 + i] * c)
+    return mix.to(torch.uint8)
+
+
+def auto_augment_crop_normalize(x_u8, mean, std_scale, out_hw, boxes, flips, records, out_dtype=torch.float32, weights=None):
+    """TrivialAugmentWide / RandAugment / AutoAugment on the (resized) crop, then normalisation: u = :func:`aa_crop_u8`; each op
+    slot of ``records[i]`` (float32 [N, slots, 12]) applied in order by :func:`aa_apply_op`; out = (u' − m̂) * std_scale with m̂ the
+    bilinear resample of a per-pixel mean over the same (mirrored) box (a [C] or scalar mean as it is).  Fill pixels become
+    −m̂ * std_scale.  With ``weights`` (AugMix's float32 [N, 1 + width]) the slots are ``width`` chains of 3 that each start from u,
+    and u' is :func:`augmix_mix` of u and the chains."""
     import torch.nn.functional as F
     N, H, W, C = x_u8.shape
     if isinstance(std_scale, torch.Tensor):
@@ -919,8 +941,17 @@ def auto_augment_crop_normalize(x_u8, mean, std_scale, out_hw, boxes, flips, rec
     out = torch.empty((N,) + tuple(out_hw) + (C,), dtype=torch.float32)
     for i in range(N):
         img = u[i].permute(2, 0, 1).contiguous()
-        for r in rec[i]:
-            img = aa_apply_op(img, r)
+        if weights is None:
+            for r in rec[i]:
+                img = aa_apply_op(img, r)
+        else:
+            chains = []
+            for chain in rec[i].view(-1, 3, rec.shape[-1]):
+                aug = img
+                for r in chain:
+                    aug = aa_apply_op(aug, r)
+                chains.append(aug)
+            img = augmix_mix(img, chains, weights[i])
         if mean.dim() == 3:
             y0, x0, h, w = (int(v) for v in boxes[i])
             box = mean.cpu()[y0:y0 + h, x0:x0 + w, :].permute(2, 0, 1).unsqueeze(0)
