@@ -348,6 +348,30 @@ void easgd_elastic(void* w, void* h, void* center, float alpha, long long n, int
 void ticket_acquire(const CommCtx& c, int owner, void* local_state, cudaStream_t st);
 void ticket_release(const CommCtx& c, int owner, void* local_state, cudaStream_t st);
 void copy_flat(void* dst, void* dst_h, const void* src, long long n, int max_blocks, const void* gate, cudaStream_t st);
+// Model EMA (utils/opt.py: ModelEma).  state: uint64 {u, n_averaged, mode} in device memory.  ema_advance (one thread): u += 1; when
+// u % every == 0 the mode is EMA_COPY (n_averaged = 1) if n_averaged == 0 or u <= warmup, else EMA_AVERAGE (n_averaged += 1);
+// otherwise EMA_SKIP.  ema_update: per the mode, nothing, E ← W, or E ← fp32(d)·E + fp32(1 − d)·W (each product and the sum rounded
+// once) over the n arena elements and every segment (dst = the E part, src = a batch-norm statistics tensor).  ema_swap: W ↔ E,
+// H ← bf16-RN(new W) when H is not null, and dst ↔ src of every segment.
+enum EmaMode : int { EMA_SKIP = 0, EMA_COPY = 1, EMA_AVERAGE = 2 };
+struct EmaSegment {
+  float* dst;
+  float* src;
+  long long n;
+};
+struct EmaArgs {
+  void* W;
+  void* E;
+  void* H;                               // ema_swap: bf16 shadow of W, or null
+  long long n;                           // arena elements (a multiple of kArenaBlock)
+  const void* segs;                      // EmaSegment[n_segs] in device memory
+  int n_segs;
+  const void* state;                     // ema_update: the state words
+  float decay, one_minus_decay;
+};
+void ema_advance(void* state, long long every, long long warmup, cudaStream_t st);
+void ema_update(const EmaArgs& a, cudaStream_t st);
+void ema_swap(const EmaArgs& a, cudaStream_t st);
 // device-side gossip (GOSGD): state = 64 uint32 of local device memory, [0] holds the push-sum weight (float)
 void gosgd_push(const CommCtx& c, void* state, int dest, long long w_off, long long snap_off, long long n, int max_blocks, cudaStream_t st);
 void gosgd_poll_merge(const CommCtx& c, void* state, long long w_off, long long h_off, long long snap_off, long long n, int max_blocks,

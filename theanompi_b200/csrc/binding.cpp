@@ -243,6 +243,12 @@ PYBIND11_MODULE(_tmpi_native, m) {
     py::arg("w"), py::arg("h"), py::arg("center"), py::arg("alpha"), py::arg("n"), py::arg("max_blocks"), py::arg("st"), py::arg("lockfree") = 0);
   m.def("copy_flat", [](ptr_t dst, ptr_t dst_h, ptr_t src, long long n, int max_blocks, ptr_t st) {
     copy_flat(P(dst), P(dst_h), P(src), n, max_blocks, nullptr, S(st)); });
+  m.attr("EMA_MODES") = py::dict(py::arg("skip") = (int)EMA_SKIP, py::arg("copy") = (int)EMA_COPY, py::arg("average") = (int)EMA_AVERAGE);
+  m.def("ema_advance", [](ptr_t state, long long every, long long warmup, ptr_t st) { ema_advance(P(state), every, warmup, S(st)); });
+  m.def("ema_update", [](ptr_t W, ptr_t E, long long n, ptr_t segs, int n_segs, ptr_t state, float decay, float one_minus_decay, ptr_t st) {
+    ema_update(EmaArgs{P(W), P(E), nullptr, n, P(segs), n_segs, P(state), decay, one_minus_decay}, S(st)); });
+  m.def("ema_swap", [](ptr_t W, ptr_t E, ptr_t H, long long n, ptr_t segs, int n_segs, ptr_t st) {
+    ema_swap(EmaArgs{P(W), P(E), P(H), n, P(segs), n_segs, nullptr, 0.f, 0.f}, S(st)); });
   m.def("gosgd_merge", [](ptr_t w, ptr_t h, ptr_t b, float a_self, float a_src, long long n, int max_blocks, ptr_t st) {
     gosgd_merge(P(w), P(h), P(b), a_self, a_src, n, max_blocks, S(st)); });
   m.def("cast_flat", [](ptr_t src, ptr_t dst, long long n, int kind, ptr_t st) { cast_flat(P(src), P(dst), n, kind, S(st)); });

@@ -1039,6 +1039,143 @@ void copy_flat(void* dst, void* dst_h, const void* src, long long n, int max_blo
   count_launch(); TMPI_CHECK_LAUNCH("copy_flat"); ::tmpi::check_capture(st, "copy_flat");
 }
 
+// ============================================================================ model EMA (utils/opt.py: ModelEma)
+// state: uint64 {u, n_averaged, mode}.  ema_advance_kernel counts one more optimizer update and writes what ema_update_kernel does
+// after it: nothing, E ← W, or E ← d·E + (1 − d)·W.  every, warmup, d and 1 − d are launch arguments, fixed when a step is captured;
+// the counters live in device memory, so a captured CUDA graph keeps counting.
+__global__ void ema_advance_kernel(unsigned long long* __restrict__ state, long long every, long long warmup) {
+  const unsigned long long u = state[0] + 1ull;
+  unsigned long long n = state[1], mode = EMA_SKIP;
+  if (u % (unsigned long long)every == 0ull) {
+    if (n == 0ull || u <= (unsigned long long)warmup) {
+      n = 1ull; mode = EMA_COPY;
+    } else {
+      n += 1ull; mode = EMA_AVERAGE;
+    }
+  }
+  state[0] = u; state[1] = n; state[2] = mode;
+}
+
+// fp32(d)·e + fp32(1 − d)·w with each product and the sum rounded once: mul.rn / add.rn are never contracted into an FMA, and without
+// .ftz they keep subnormals (the build's --use_fast_math would flush them in __fmul_rn), so the result is bit-equal to torch's fp32
+// expression d * e + (1 - d) * w on the CPU.
+__device__ __forceinline__ float ema_avg(float e, float w, float d, float omd) {
+  float a, b, r;
+  asm("mul.rn.f32 %0, %1, %2;" : "=f"(a) : "f"(d), "f"(e));
+  asm("mul.rn.f32 %0, %1, %2;" : "=f"(b) : "f"(omd), "f"(w));
+  asm("add.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+
+constexpr int kEmaUnroll = 4;            // arena blocks in flight per CTA iteration
+constexpr int kEmaSegCtas = 16;          // CTAs that walk the statistics segments
+
+// CTAs [0, arena_ctas) walk the arena blocks of W / E with float4 loads and stores, the others the statistics segments {E part, the
+// layer's tensor}.  A skip step returns before it touches memory; a copy step does not read E.
+__global__ void __launch_bounds__(kThreads) ema_update_kernel(const float* __restrict__ W, float* __restrict__ E, long long nblk,
+                                                              int arena_ctas, const EmaSegment* __restrict__ segs, int n_segs,
+                                                              const unsigned long long* __restrict__ state, float d, float omd) {
+  const unsigned long long mode = state[2];
+  if (mode == EMA_SKIP) return;
+  const bool copy = mode == EMA_COPY;
+  if ((int)blockIdx.x >= arena_ctas) {
+    for (int s = (int)blockIdx.x - arena_ctas; s < n_segs; s += (int)gridDim.x - arena_ctas) {
+      const EmaSegment g = segs[s];
+      for (long long i = threadIdx.x; i < g.n; i += kThreads) g.dst[i] = copy ? g.src[i] : ema_avg(g.dst[i], g.src[i], d, omd);
+    }
+    return;
+  }
+  for (long long b0 = blockIdx.x; b0 < nblk; b0 += (long long)arena_ctas * kEmaUnroll) {
+    float4 w[kEmaUnroll], e[kEmaUnroll];
+#pragma unroll
+    for (int u = 0; u < kEmaUnroll; ++u) {
+      const long long b = b0 + (long long)u * arena_ctas;
+      if (b >= nblk) continue;
+      const long long i = b * kArenaBlock + threadIdx.x * 4;
+      w[u] = *reinterpret_cast<const float4*>(W + i);
+      if (!copy) e[u] = *reinterpret_cast<const float4*>(E + i);
+    }
+#pragma unroll
+    for (int u = 0; u < kEmaUnroll; ++u) {
+      const long long b = b0 + (long long)u * arena_ctas;
+      if (b >= nblk) continue;
+      const long long i = b * kArenaBlock + threadIdx.x * 4;
+      const float4 o = copy ? w[u]
+                            : make_float4(ema_avg(e[u].x, w[u].x, d, omd), ema_avg(e[u].y, w[u].y, d, omd),
+                                          ema_avg(e[u].z, w[u].z, d, omd), ema_avg(e[u].w, w[u].w, d, omd));
+      *reinterpret_cast<float4*>(E + i) = o;
+    }
+  }
+}
+
+// W ↔ E, H ← bf16-RN(new W) when there is a shadow, and every segment's two parts exchanged: applying it twice is the identity.
+__global__ void __launch_bounds__(kThreads) ema_swap_kernel(float* __restrict__ W, float* __restrict__ E, __nv_bfloat16* __restrict__ H,
+                                                            long long nblk, int arena_ctas, const EmaSegment* __restrict__ segs,
+                                                            int n_segs) {
+  if ((int)blockIdx.x >= arena_ctas) {
+    for (int s = (int)blockIdx.x - arena_ctas; s < n_segs; s += (int)gridDim.x - arena_ctas) {
+      const EmaSegment g = segs[s];
+      for (long long i = threadIdx.x; i < g.n; i += kThreads) {
+        const float a = g.dst[i];
+        g.dst[i] = g.src[i];
+        g.src[i] = a;
+      }
+    }
+    return;
+  }
+  for (long long b0 = blockIdx.x; b0 < nblk; b0 += (long long)arena_ctas * kEmaUnroll) {
+    float4 w[kEmaUnroll], e[kEmaUnroll];
+#pragma unroll
+    for (int u = 0; u < kEmaUnroll; ++u) {
+      const long long b = b0 + (long long)u * arena_ctas;
+      if (b >= nblk) continue;
+      const long long i = b * kArenaBlock + threadIdx.x * 4;
+      w[u] = *reinterpret_cast<const float4*>(W + i);
+      e[u] = *reinterpret_cast<const float4*>(E + i);
+    }
+#pragma unroll
+    for (int u = 0; u < kEmaUnroll; ++u) {
+      const long long b = b0 + (long long)u * arena_ctas;
+      if (b >= nblk) continue;
+      const long long i = b * kArenaBlock + threadIdx.x * 4;
+      *reinterpret_cast<float4*>(W + i) = e[u];
+      *reinterpret_cast<float4*>(E + i) = w[u];
+      if (H) *reinterpret_cast<uint2*>(H + i) = pack_bf16x4(e[u]);
+    }
+  }
+}
+
+static void ema_grid(const EmaArgs& a, const char* name, long long& nb, int& arena_ctas, int& grid) {
+  if (a.n <= 0 || a.n % kArenaBlock) throw std::runtime_error(std::string(name) + ": the arena size must be a positive multiple of the block");
+  if (!a.W || !a.E || (a.n_segs > 0 && !a.segs) || a.n_segs < 0) throw std::runtime_error(std::string(name) + ": missing buffers");
+  nb = a.n / kArenaBlock;
+  arena_ctas = (int)std::min<long long>((nb + kEmaUnroll - 1) / kEmaUnroll, (long long)sm_count() * 8);
+  grid = arena_ctas + std::min(a.n_segs, kEmaSegCtas);
+}
+
+void ema_advance(void* state, long long every, long long warmup, cudaStream_t st) {
+  if (!state || every < 1 || warmup < 0) throw std::runtime_error("ema_advance: needs the state words, every >= 1 and warmup >= 0");
+  ema_advance_kernel<<<1, 1, 0, st>>>((unsigned long long*)state, every, warmup);
+  count_launch(); TMPI_CHECK_LAUNCH("ema_advance"); ::tmpi::check_capture(st, "ema_advance");
+}
+
+void ema_update(const EmaArgs& a, cudaStream_t st) {
+  if (!a.state) throw std::runtime_error("ema_update: needs the state words");
+  long long nb; int arena_ctas, grid;
+  ema_grid(a, "ema_update", nb, arena_ctas, grid);
+  ema_update_kernel<<<grid, kThreads, 0, st>>>((const float*)a.W, (float*)a.E, nb, arena_ctas, (const EmaSegment*)a.segs, a.n_segs,
+                                               (const unsigned long long*)a.state, a.decay, a.one_minus_decay);
+  count_launch(); TMPI_CHECK_LAUNCH("ema_update"); ::tmpi::check_capture(st, "ema_update");
+}
+
+void ema_swap(const EmaArgs& a, cudaStream_t st) {
+  long long nb; int arena_ctas, grid;
+  ema_grid(a, "ema_swap", nb, arena_ctas, grid);
+  ema_swap_kernel<<<grid, kThreads, 0, st>>>((float*)a.W, (float*)a.E, (__nv_bfloat16*)a.H, nb, arena_ctas, (const EmaSegment*)a.segs,
+                                             a.n_segs);
+  count_launch(); TMPI_CHECK_LAUNCH("ema_swap"); ::tmpi::check_capture(st, "ema_swap");
+}
+
 // ============================================================================ GOSGD:  w ← (a_self·w + a_src·b) / (a_self + a_src)
 // Host-driven form (CPU-mirrored semantics, tests): coefficients passed by value, `b` = local mailbox or a peer's snapshot.
 template <int U>

@@ -21,6 +21,7 @@ needs re-capture; costs/errors stay on the device until the recorder prints.
 """
 from __future__ import annotations
 
+import contextlib
 import gc
 import math
 import time
@@ -31,7 +32,7 @@ import torch
 from .. import ops
 from ..parallel.arena import FlatArena
 from ..utils import nvtx
-from ..utils.opt import FlatSGD, LrSchedule, SharedScalar, pre_model_iter_fn
+from ..utils.opt import FlatSGD, LrSchedule, ModelEma, SharedScalar, pre_model_iter_fn
 from .layers2 import BatchNormal, Crop, Dropout, count_params
 
 
@@ -71,6 +72,7 @@ class ModelBase(object):
     supports_mixup = True          # config['mixup'] (False: no image batch before a first convolution; refused at compile_iter_fns)
     supports_drop_path = False     # config['drop_path_rate'] > 0 (True: residual blocks in self.body that read drop_row(l))
     supports_cifar_augment = False  # config['cifar_augment'] (True: a CIFAR model whose training forward reads train_augment())
+    supports_model_ema = True      # config['model_ema'] (False: no single arena updated by the step tail; refused at compile_iter_fns)
     # True: an ImageNet model fed by ParaLoader, so config['random_resized_crop'], config['color_jitter'] and
     # config['random_erasing'] reach its loader
     # (refused at construction otherwise)
@@ -122,6 +124,10 @@ class ModelBase(object):
         # update's step writes lr; built by setup_lr_schedule at compile_iter_fns
         self.lr_schedule = config.get("lr_schedule")
         self.lr_sched = None
+        # exponential moving average of the weights and batch-norm statistics (a dict, utils/opt.py: ModelEma; None = off): two launches
+        # after every update's step tail average W into E; ema_weights() validates, infers and saves with E.  Built by check_model_ema
+        self.model_ema = config.get("model_ema")
+        self.ema = None
         # label smoothing ε of the training loss (cross-entropy against (1 − ε)·onehot + ε / C; 0 = plain NLL); validation stays
         # plain NLL.  Checked by check_label_smoothing at compile_iter_fns
         self.label_smoothing = config.get("label_smoothing", 0.0)
@@ -291,6 +297,8 @@ class ModelBase(object):
         if kind in ("step", "last") and self._tail is not None:
             with torch.no_grad():
                 self._tail()
+                if self.ema is not None:
+                    self.ema.update()
             self._dbg_capture("step tail")
         self._after_step()
         return out
@@ -674,14 +682,24 @@ class ModelBase(object):
         if k > 1 and fused_tail is None:
             _ = self.arena.R                      # allocate the receive region
         pre_model_iter_fn(self, k, aggregate=aggregate, fused_tail=fused_tail)
+        if self.ema is not None and k > 1:
+            # BSP 'cdd' over a split strategy: W is the same on every rank once post() has run, so the average follows it there
+            post = self.descent_vel
+
+            def descent_vel():
+                post()
+                with torch.no_grad():
+                    self.ema.update()
+            self.descent_vel = descent_vel
+            self.compiled_train_fn_list = [self.get_vel, descent_vel]
         if self.verbose:
             print("Compile time: %.3f s" % (time.time() - start))
 
     def setup_train_options(self, k=1, fused_tail=None, optimizer=None):
         """Check and build the training options of the config for a step of ``k`` workers (k > 1: BSP ``sync_type='cdd'``),
         ``fused_tail`` (a fused exchange strategy's step tail, or None) and ``optimizer`` (default: the model's): grad_accum,
-        label_smoothing, mixup, cifar_augment, drop_path_rate, lr_schedule and grad_clip.  A model refuses every option it does not
-        support here, with a ValueError that names it."""
+        label_smoothing, mixup, cifar_augment, drop_path_rate, lr_schedule, grad_clip and model_ema.  A model refuses every option it
+        does not support here, with a ValueError that names it."""
         self.check_grad_accum(fused_tail)
         self.check_label_smoothing()
         self.check_mixup()
@@ -694,6 +712,43 @@ class ModelBase(object):
                              "strategies (fused*, oneshot*, twoshot*, nvls*, fused_rs) update bucket slices as they are reduced. "
                              "Use a split strategy: ar, nccl32, nccl16, asa32, asa16 or p2p32" % opt)
         self.check_grad_clip(k, fused_tail, opt)
+        self.check_model_ema(k, fused_tail)
+
+    def check_model_ema(self, k=1, fused_tail=None):
+        """``config['model_ema']`` must be None or a valid dict (utils/opt.py: ModelEma.check_config; a ValueError names the key).  A
+        dict needs a model whose step tail updates one arena (``supports_model_ema``), on one worker or on BSP ``sync_type='cdd'`` over a
+        split strategy (``k`` = the number of workers, no ``fused_tail``): elsewhere the weights change after the step, in the exchange
+        (BSP 'avg', EASGD, ASGD, GOSGD), or non-owners' fp32 masters are stale (the fused strategies).  Builds :class:`ModelEma`, whose
+        average starts from the weights and statistics as they are now."""
+        self.ema = None
+        if self.model_ema is None:
+            return
+        key = ModelEma.KEY
+        cfg = ModelEma.check_config(self.model_ema)
+        supported = ("%s runs on AlexNet, GoogLeNet, Cifar10_model, VGG16, ResNet50, ResNet152 and Wide_ResNet, on one worker or on BSP "
+                     "sync_type='cdd' over a split strategy (ar, nccl32, nccl16, asa32, asa16, p2p32)" % key)
+        if not self.supports_model_ema:
+            raise ValueError("%s: %s is not supported; %s" % (self.name, key, supported))
+        if self.size > 1 and fused_tail is not None:
+            raise ValueError("%s: %s does not combine with a fused exchange strategy on %d workers, whose non-owners' fp32 master weights "
+                             "are stale; %s" % (self.name, key, self.size, supported))
+        if self.size > 1 and k != self.size:
+            raise ValueError("%s: %s needs the same updated weights on every worker after the step; with BSP sync_type='avg', EASGD, "
+                             "ASGD or GOSGD on %d workers they change in the exchange; %s" % (self.name, key, self.size, supported))
+        self.ema = ModelEma(self.arena, self._bn_layers, cfg)
+
+    @contextlib.contextmanager
+    def ema_weights(self):
+        """Inside the block the model's weights W, their bf16 shadow and its batch-norm running statistics are the moving average E
+        (``config['model_ema']``), so that ``val_iter``, ``inf_fn`` and ``save_weights`` run on the averaged model; on exit all three
+        are restored bit for bit.  One ``ema_swap`` launch each way."""
+        if self.ema is None:
+            raise RuntimeError("%s: ema_weights() needs config['model_ema'] and compile_iter_fns()" % self.name)
+        self.ema.swap()
+        try:
+            yield
+        finally:
+            self.ema.swap()
 
     def check_grad_clip(self, k=1, fused_tail=None, optimizer=None):
         """Refuse ``grad_clip`` where the native step cannot clip by the global norm: with ``optimizer`` (default: the model's)
@@ -873,6 +928,8 @@ class ModelBase(object):
             sd["grad_clip"] = self.clip_opt.state_dict()
         if self.lr_sched is not None:                   # the update index of the lr schedule
             sd["lr_schedule"] = self.lr_sched.state_dict()
+        if self.ema is not None:                        # the moving average and its counters
+            sd["model_ema"] = self.ema.state_dict()
         return sd
 
     def load_extra_state(self, sd):
@@ -885,6 +942,8 @@ class ModelBase(object):
             self.clip_opt.load_state_dict(sd["grad_clip"])
         if "lr_schedule" in sd and self.lr_sched is not None:
             self.lr_sched.load_state_dict(sd["lr_schedule"])
+        if "model_ema" in sd and self.ema is not None:
+            self.ema.load_state_dict(sd["model_ema"])
 
     def cleanup(self):
         if getattr(self.data, "para_load", False) and hasattr(self.data, "para_load_close"):

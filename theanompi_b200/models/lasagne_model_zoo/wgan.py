@@ -235,6 +235,7 @@ class NativeWGAN(ModelBase):
     ``opt_c.skipped`` / ``opt_g.skipped`` count it.  The reference's CIFAR-10 LSGAN uses plain RMSProp without rescaling, so there
     ``grad_clip`` is simply available."""
     supports_grad_accum = False    # its critic / generator steps keep their own gaccum accumulation
+    supports_model_ema = False     # two arenas, critic and generator
     supports_lr_schedule = False   # two arenas and critic / generator step ratios: the reference's per-epoch decay
     supports_label_smoothing = False   # no classifier head
     supports_mixup = False             # no classifier head

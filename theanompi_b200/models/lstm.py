@@ -111,6 +111,7 @@ class LSTM(ModelBase):
     unpadded batch; validation is always eager."""
     supports_mixup = False         # token input: nothing to mix
     supports_grad_accum = False    # one graph per sequence-length bucket, each with its own update
+    supports_model_ema = False     # one graph per sequence-length bucket
     n_epochs = max_epochs
     batch_size = file_batch_size = batch_size
     learning_rate = 1.0

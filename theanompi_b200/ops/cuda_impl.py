@@ -21,6 +21,7 @@ from __future__ import annotations
 
 import os
 
+import numpy as np
 import torch
 
 from . import accum, native, precision
@@ -1232,6 +1233,37 @@ def lr_schedule_step(arena, sched, counter):
     lib.lr_schedule(lib.LR_POLICIES[sched.decay], int(sched.warmup_steps), int(sched.total_steps), float(sched.warmup_start),
                     float(sched.peak), float(sched.final_lr), float(sched.power), float(sched.gamma), [int(m) for m in sched.milestones],
                     counter.data_ptr(), arena.hyper.data_ptr(), _st(arena.hyper))
+
+
+def _ema_check(arena, e, table):
+    assert e.dtype == torch.float32 and e.is_contiguous() and e.numel() == arena.numel and e.device == arena.W.device, (e.dtype, e.shape)
+    assert table.dtype == torch.int64 and table.dim() == 2 and table.shape[1] == 3 and table.device == arena.W.device, (table.dtype,
+                                                                                                                         table.shape)
+
+
+def ema_advance(state, every, warmup):
+    """One single-thread launch of ``csrc/comm_kernels.cu: ema_advance_kernel``: ``state`` (int64 [3] on the device: u, n_averaged,
+    mode) counts one more optimizer update and takes the mode of :func:`ema_update` (``reference.ema_advance``).  Reads only device
+    memory, so it can be captured in a CUDA graph."""
+    assert state.dtype == torch.int64 and state.numel() == 3 and state.is_cuda and state.is_contiguous(), (state.dtype, state.shape)
+    L().ema_advance(state.data_ptr(), int(every), int(warmup), _st(state))
+
+
+def ema_update(arena, e, state, table, decay, one_minus_decay):
+    """One launch of ``csrc/comm_kernels.cu: ema_update_kernel``: per the mode in ``state[2]`` (skip, copy or average), nothing,
+    E ← W or E ← fp32(d)·E + fp32(1 − d)·W over the arena's W region into ``e`` (fp32 [arena.numel]) and over the segments of
+    ``table`` (int64 [n, 3]: E part address, statistics tensor address, n elements).  Reads only device memory."""
+    _ema_check(arena, e, table)
+    assert state.dtype == torch.int64 and state.numel() == 3 and state.device == arena.W.device, (state.dtype, state.shape)
+    L().ema_update(arena.W.data_ptr(), e.data_ptr(), int(arena.numel), table.data_ptr(), int(table.shape[0]), state.data_ptr(),
+                   float(np.float32(decay)), float(np.float32(one_minus_decay)), _st(arena.W))
+
+
+def ema_swap(arena, e, table):
+    """One launch of ``csrc/comm_kernels.cu: ema_swap_kernel``: W ↔ ``e``, the bf16 shadow ← bf16-RN(new W), and the two parts of
+    every segment of ``table`` exchanged.  Twice is the identity."""
+    _ema_check(arena, e, table)
+    L().ema_swap(arena.W.data_ptr(), e.data_ptr(), _p(arena.H), int(arena.numel), table.data_ptr(), int(table.shape[0]), _st(arena.W))
 
 
 def sgd_flat(arena, g, lr, mu, nesterov, inv_k, lo, hi, only_local=False, only_exchanged=False, clip=None):

@@ -674,6 +674,48 @@ def gosgd_merge(w, b, alpha_self, alpha_src):
     return w
 
 
+EMA_SKIP, EMA_COPY, EMA_AVERAGE = 0, 1, 2
+
+
+def ema_advance(u, n_averaged, every, warmup):
+    """Model EMA bookkeeping after one more optimizer update: returns (u + 1, n_averaged', mode).  Update u + 1 averages iff it is a
+    multiple of ``every``; it copies (mode EMA_COPY, n_averaged becomes 1) when nothing has been averaged yet or u + 1 <= ``warmup``,
+    else it averages (EMA_AVERAGE, n_averaged + 1).  Otherwise EMA_SKIP."""
+    u += 1
+    if u % every:
+        return u, n_averaged, EMA_SKIP
+    if n_averaged == 0 or u <= warmup:
+        return u, 1, EMA_COPY
+    return u, n_averaged + 1, EMA_AVERAGE
+
+
+def ema_update(pairs, mode, decay, one_minus_decay):
+    """One model-EMA step over ``pairs`` of fp32 tensors (e, w), e updated in place: nothing (EMA_SKIP), e = w (EMA_COPY), or
+    e = fp32(d)·e + fp32(1 − d)·w (EMA_AVERAGE) with both products and the sum each rounded once to fp32, which is what torch's
+    fp32 expression ``d * e + (1 - d) * w`` gives (``torch.optim.swa_utils.AveragedModel`` with that ``avg_fn``).
+    ``one_minus_decay``: 1 − d evaluated in float64, then rounded to fp32."""
+    if mode == EMA_SKIP:
+        return
+    d = torch.tensor(float(np.float32(decay)), dtype=torch.float32)
+    omd = torch.tensor(float(np.float32(one_minus_decay)), dtype=torch.float32)
+    for e, w in pairs:
+        if mode == EMA_COPY:
+            e.copy_(w)
+        else:
+            e.copy_(torch.add(torch.mul(e, d.to(e.device)), torch.mul(w, omd.to(w.device))))
+
+
+def ema_swap(pairs, w_half=None):
+    """Exchange the contents of every pair (a, b) of equal-sized fp32 tensors; ``w_half`` (the bf16 shadow of the first pair's
+    first tensor, or None) then takes bf16-RN of that tensor's new value.  Applying it twice restores every tensor."""
+    for a, b in pairs:
+        t = a.clone()
+        a.copy_(b)
+        b.copy_(t)
+    if w_half is not None:
+        w_half.copy_(pairs[0][0])
+
+
 # --------------------------------------------------------------------------- data aug
 def crop_mirror_normalize(x_u8, mean, std_scale, crop_hw, offsets, flips, out_dtype=torch.float32, zero_fill=False):
     """``(x - mean) * std_scale`` → crop at per-image ``offsets`` → optional

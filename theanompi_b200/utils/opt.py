@@ -168,6 +168,135 @@ class LrSchedule(object):
         self.u.fill_(int(sd["u"]))
 
 
+class ModelEma(object):
+    """Exponential moving average of the model (``config['model_ema']``, a dict): torchvision's ``ExponentialMovingAverage``, i.e.
+    ``torch.optim.swa_utils.AveragedModel`` with ``avg_fn = d·e + (1 − d)·w`` and ``use_buffers=True``.  E holds an fp32 copy of the
+    arena's W region and of the running mean and variance of every batch-norm layer, taken when the model is compiled.
+
+    Keys: ``decay`` d in [0, 1] (0.9999), ``every`` >= 1 (1; torchvision's ``--model-ema-steps``), ``warmup`` >= 0 (0).  After
+    optimizer update u = 1, 2, ... the average moves iff u is a multiple of ``every``: it copies E ← W when nothing has been averaged
+    yet or u <= ``warmup``, else E ← fp32(d)·E + fp32(1 − d)·W (``reference.ema_update``).
+
+    On CUDA :meth:`update` is two launches after the step's update (``cuda_impl.ema_advance``, ``cuda_impl.ema_update``) that read
+    only device memory: the counters {u, n_averaged} and the step's mode live in :attr:`state`, so a captured CUDA graph keeps
+    counting.  The batch-norm statistics are reached through a device table of {dst, src, n} segments, built at the first
+    :meth:`update` or :meth:`swap` and rebuilt when a layer's statistics tensors have been replaced (``BatchNormal.forward`` moves
+    them to the device lazily, ``load_extra_state`` replaces them).  :meth:`swap` exchanges the model's weights and statistics with
+    E in one pass, the bf16 shadow following W."""
+
+    KEY = "model_ema"
+    KEYS = ("decay", "every", "warmup")
+
+    def __init__(self, arena, bn_layers, cfg):
+        """``bn_layers``: a callable returning the model's batch-norm layers; ``cfg``: a dict that :meth:`check_config` accepts."""
+        cfg = self.check_config(cfg)
+        self.decay, self.every, self.warmup = cfg["decay"], cfg["every"], cfg["warmup"]
+        self.one_minus_decay = float(np.float32(1.0 - self.decay))          # 1 − d in float64, rounded once to fp32
+        self.arena, self.bn_layers = arena, bn_layers
+        dev = arena.W.device
+        stats = self._stats()
+        self.sizes = [int(s.numel()) for s in stats]
+        with torch.no_grad():
+            self.E = arena.W.detach().clone()
+            self.E_bn = (torch.cat([s.detach().reshape(-1).to(dev, torch.float32) for s in stats]) if stats
+                         else torch.zeros(0, dtype=torch.float32, device=dev))
+        self.state = torch.zeros(3, dtype=torch.int64, device=dev)          # u, n_averaged, mode of the last update
+        self._table, self._src = None, None
+
+    @classmethod
+    def check_config(cls, cfg):
+        """The validated dict {decay, every, warmup}; anything else is a ValueError that names ``model_ema``."""
+        k = cls.KEY
+        if not isinstance(cfg, dict):
+            raise ValueError("%s must be a dict or None, not %r" % (k, cfg))
+        unknown = sorted(set(cfg) - set(cls.KEYS))
+        if unknown:
+            raise ValueError("%s: unknown key %r; the keys are %s" % (k, unknown[0], ", ".join(cls.KEYS)))
+        d = cfg.get("decay", 0.9999)
+        if isinstance(d, bool) or not isinstance(d, (int, float, np.integer, np.floating)) or not np.isfinite(d) or not 0.0 <= d <= 1.0:
+            raise ValueError("%s['decay'] must be a real number in [0, 1], not %r" % (k, d))
+        out = {"decay": float(d)}
+        for key, default, lo in (("every", 1, 1), ("warmup", 0, 0)):
+            v = cfg.get(key, default)
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < lo:
+                raise ValueError("%s[%r] must be an int >= %d, not %r" % (k, key, lo, v))
+            out[key] = int(v)
+        return out
+
+    def _stats(self):
+        return [t for l in self.bn_layers() for t in (l.running_mean, l.running_var)]
+
+    def _pairs(self):
+        """(E part, model tensor) for W and every statistics tensor (the CPU path)."""
+        out, o = [(self.E, self.arena.W)], 0
+        for s, n in zip(self._stats(), self.sizes):
+            out.append((self.E_bn[o:o + n], s))
+            o += n
+        return out
+
+    def _ensure_table(self):
+        """The device segment table of the statistics ({E_bn + offset, statistics tensor, n} per tensor, int64 [n, 3]), built again in
+        place when a layer holds other tensors than the ones it points at, first moving statistics still on the host to the device
+        (as the layer's first forward would)."""
+        dev = self.arena.W.device
+        for l in self.bn_layers():
+            if l.running_mean.device != dev:
+                l.running_mean = l.running_mean.to(dev)
+                l.running_var = l.running_var.to(dev)
+        stats = self._stats()
+        if self._src is not None and all(a is b for a, b in zip(self._src, stats)):
+            return
+        rows, o = [], 0
+        for s, n in zip(stats, self.sizes):
+            assert s.dtype == torch.float32 and s.is_contiguous() and s.numel() == n, (s.dtype, tuple(s.shape), n)
+            rows.append((self.E_bn.data_ptr() + 4 * o, s.data_ptr(), n))
+            o += n
+        host = torch.tensor(rows, dtype=torch.int64).view(-1, 3)
+        if self._table is None:
+            self._table = torch.zeros_like(host, device=dev)
+        self._table.copy_(host)
+        self._src = stats
+
+    def update(self):
+        """The averaging step after an optimizer update (on CUDA two launches, inside a captured step)."""
+        if self.arena.W.is_cuda:
+            from ..ops import cuda_impl
+            self._ensure_table()
+            cuda_impl.ema_advance(self.state, self.every, self.warmup)
+            cuda_impl.ema_update(self.arena, self.E, self.state, self._table, self.decay, self.one_minus_decay)
+            return
+        u, n, mode = ref.ema_advance(int(self.state[0]), int(self.state[1]), self.every, self.warmup)
+        self.state.copy_(torch.tensor([u, n, mode]))
+        ref.ema_update(self._pairs(), mode, self.decay, self.one_minus_decay)
+
+    def swap(self):
+        """Exchange the model's W and batch-norm statistics with E (the bf16 shadow takes bf16-RN of the new W); twice is the
+        identity."""
+        a = self.arena
+        if a.W.is_cuda:
+            from ..ops import cuda_impl
+            self._ensure_table()
+            cuda_impl.ema_swap(a, self.E, self._table)
+            return
+        ref.ema_swap([(a.W, self.E)] + [(s, e) for e, s in self._pairs()[1:]], w_half=a.H)
+
+    @property
+    def n_averaged(self):
+        return int(self.state[1])
+
+    def state_dict(self):
+        return {"E": self.E.detach().cpu().clone(), "bn": self.E_bn.detach().cpu().clone(), "u": int(self.state[0]),
+                "n_averaged": int(self.state[1])}
+
+    def load_state_dict(self, sd):
+        if tuple(sd["E"].shape) != tuple(self.E.shape) or tuple(sd["bn"].shape) != tuple(self.E_bn.shape):
+            raise ValueError("model_ema: the checkpoint's average does not match this model's arena and batch-norm layers")
+        with torch.no_grad():
+            self.E.copy_(sd["E"].to(self.E.device))
+            self.E_bn.copy_(sd["bn"].to(self.E_bn.device))
+        self.state.copy_(torch.tensor([int(sd["u"]), int(sd["n_averaged"]), 0]))
+
+
 def _fc_fusable(p, block):
     """Can ``p``'s weight gradient be consumed by the SGD epilogue of its wgrad GEMM?  It must come from ONE fp32 GEMM straight
     into ``gbuf`` (native FC / Softmax weights, ``rs_ok``), not be accumulated over several passes, and its shape must take the

@@ -20,6 +20,7 @@ H100-native differences:
 """
 from __future__ import annotations
 
+import contextlib
 import os
 import pickle
 import time
@@ -42,6 +43,10 @@ class Recorder(object):
         self.info_dict = {"train_info": [], "val_info": [], "epoch_time": [], "all_time": [], "lr": []}
         self.train_info = {"cost": [], "error": []}
         self.val_info = {"cost": [], "error": [], "error_top5": []}
+        # the second validation channel: the same validation on the moving average of the model (config['model_ema']), logged as
+        # info_dict['val_info_ema'] once a pass has recorded into it (ema_channel)
+        self.val_info_ema = {"cost": [], "error": [], "error_top5": []}
+        self._ema = False
         self.all_time = {m: [] for m in self.MODES}
         self._pending = {m: [] for m in self.MODES}     # (start_event, end_event)
         self.epoch_time = None
@@ -106,9 +111,19 @@ class Recorder(object):
         self.train_info["error"].append(error)
 
     def val_error(self, count, cost, error, error_top5):
-        self.val_info["cost"].append(cost)
-        self.val_info["error"].append(error)
-        self.val_info["error_top5"].append(error_top5)
+        info = self.val_info_ema if self._ema else self.val_info
+        info["cost"].append(cost)
+        info["error"].append(error)
+        info["error_top5"].append(error_top5)
+
+    @contextlib.contextmanager
+    def ema_channel(self):
+        """Inside the block :meth:`val_error` records into the EMA channel (``val_info_ema``)."""
+        self._ema = True
+        try:
+            yield
+        finally:
+            self._ema = False
 
     def _max_over_ranks(self, vals):
         comm = self.comm
@@ -148,27 +163,34 @@ class Recorder(object):
             self.all_time[m][:] = []
 
     def gather_val_info(self):
-        for k in ("cost", "error", "error_top5"):
-            local = [_tofloat(v) for v in self.val_info[k]]
-            if self.comm is not None and getattr(self.comm, "size", 1) > 1:
-                parts = self.comm.allgather(local)
-                local = [x for p in parts for x in p]
-            self.val_info[k] = local
+        """Gather both validation channels over the ranks; the EMA channel only when this epoch recorded into it (on every rank)."""
+        for info in (self.val_info, self.val_info_ema):
+            if info is self.val_info_ema and not info["cost"]:
+                continue
+            for k in ("cost", "error", "error_top5"):
+                local = [_tofloat(v) for v in info[k]]
+                if self.comm is not None and getattr(self.comm, "size", 1) > 1:
+                    parts = self.comm.allgather(local)
+                    local = [x for p in parts for x in p]
+                info[k] = local
 
     def print_val_info(self, count, comment=None):
-        n = max(1, len(self.val_info["cost"]))
-        cost = sum(_tofloat(v) for v in self.val_info["cost"]) / n
-        error = sum(_tofloat(v) for v in self.val_info["error"]) / n
-        error_top5 = sum(_tofloat(v) for v in self.val_info["error_top5"]) / n
-        self.info_dict["val_info"].append([count, cost, error, error_top5])
-        if self.verbose:
-            if comment is not None:
-                print(comment)
-            print("\nvalidation cost:%.4f" % cost)
-            print("validation error:%.4f" % error)
-            print("validation top_5_error:%.4f" % error_top5)
-        for k in self.val_info:
-            self.val_info[k][:] = []
+        for key, info, label in (("val_info", self.val_info, "validation"), ("val_info_ema", self.val_info_ema, "EMA validation")):
+            if info is self.val_info_ema and not info["cost"]:
+                continue
+            n = max(1, len(info["cost"]))
+            cost = sum(_tofloat(v) for v in info["cost"]) / n
+            error = sum(_tofloat(v) for v in info["error"]) / n
+            error_top5 = sum(_tofloat(v) for v in info["error_top5"]) / n
+            self.info_dict.setdefault(key, []).append([count, cost, error, error_top5])
+            if self.verbose:
+                if comment is not None and info is self.val_info:
+                    print(comment)
+                print("\n%s cost:%.4f" % (label, cost))
+                print("%s error:%.4f" % (label, error))
+                print("%s top_5_error:%.4f" % (label, error_top5))
+            for k in info:
+                info[k][:] = []
 
     def get_latest_val_info(self):
         return self.info_dict["val_info"][-1] if self.info_dict["val_info"] else None
@@ -185,11 +207,14 @@ class Recorder(object):
             d = pickle.load(f)
         for k in ("train_info", "val_info", "epoch_time", "all_time", "lr"):
             self.info_dict[k].extend(d.get(k, []))
+        if "val_info_ema" in d:
+            self.info_dict.setdefault("val_info_ema", []).extend(d["val_info_ema"])
 
     def cut(self, load_epoch):
         """Truncate curves to ``load_epoch`` entries when resuming (ref ``:212-224``)."""
-        for k in ("train_info", "val_info", "epoch_time", "all_time", "lr"):
-            self.info_dict[k] = self.info_dict[k][0:load_epoch]
+        for k in ("train_info", "val_info", "val_info_ema", "epoch_time", "all_time", "lr"):
+            if k in self.info_dict:
+                self.info_dict[k] = self.info_dict[k][0:load_epoch]
 
     # ------------------------------------------------------------------ plotting (matplotlib optional)
     def plot_init(self, name, fig_specs=None, save=False):

@@ -97,6 +97,23 @@ class BSP_Worker(MPI_GPU_Process):
         if self.verbose:
             print("learning rate %f will be used for epoch %d" % (model.shared_lr.get_value(), epoch))
 
+    def _validate(self, model, recorder, n_val, count):
+        """One pass over the first ``n_val`` validation files (the early-'stop' protocol sets ``self.stop``)."""
+        batch_j = 0
+        while batch_j < n_val:
+            for subb_i in range(model.n_subb):
+                out = model.val_iter(count, recorder)
+                if out == "stop":
+                    self.stop = True
+                    break
+                elif out is not None:
+                    batch_j = out
+                else:
+                    batch_j += 1
+            if self.stop:
+                break
+        model.reset_iter("val")
+
     def BSP_run(self, model, snapshot_freq=5, snapshot_path="./snapshots/", max_batches=None):
         from .utils.helper_funcs import save_model
         self.comm.Barrier()
@@ -125,21 +142,12 @@ class BSP_Worker(MPI_GPU_Process):
             model.reset_iter("train")
 
             self.comm.Barrier()
-            batch_j = 0
             n_val = model.data.n_batch_val if max_batches is None else min(max_batches, model.data.n_batch_val)
-            while batch_j < n_val:
-                for subb_i in range(model.n_subb):
-                    out = model.val_iter(batch_i * self.size, recorder)
-                    if out == "stop":
-                        self.stop = True
-                        break
-                    elif out is not None:
-                        batch_j = out
-                    else:
-                        batch_j += 1
-                if self.stop:
-                    break
-            model.reset_iter("val")
+            self._validate(model, recorder, n_val, batch_i * self.size)
+            if getattr(model, "ema", None) is not None and not self.stop:
+                # config['model_ema']: the same validation files again on the averaged weights, into the recorder's EMA channel
+                with model.ema_weights(), recorder.ema_channel():
+                    self._validate(model, recorder, n_val, batch_i * self.size)
             recorder.gather_val_info()
             recorder.print_val_info(batch_i * self.size)
             model.current_info = recorder.get_latest_val_info()
