@@ -50,7 +50,6 @@ struct ReduceArgs {
 
 // ---- gemm_wgmma.cu
 void gemm_set_debug(int flags);
-void gemm_set_bulk(int mask);      // epilogue through the bulk copy engine: bit0 stores, bit1 split-K adds, bit2 reduce-scatter adds; -1 = env
 // Reduce-scatter fused into the wgrad GEMM epilogue: register the peer views of the gradient region and the tensors whose
 // fp32 GEMM output (C pointer inside [c_lo, c_hi)) must be red.add-ed into the OWNER rank's G instead of stored locally.
 // Ownership = the two-shot exchange kernel's partition of the bucket [blo, blo + world * per) in 1024-element blocks.

@@ -47,7 +47,6 @@ PYBIND11_MODULE(_tmpi_native, m) {
 
   // ---------------------------------------------------------------- GEMM
   m.def("gemm_set_debug", &gemm_set_debug);
-  m.def("gemm_set_bulk", &gemm_set_bulk);
   m.def("gemm_rs_add_range", [](ptr_t c_lo, ptr_t c_hi, long long blo, long long per) { gemm_rs_add_range(P(c_lo), P(c_hi), blo, per); });
   m.def("gemm_rs_clear", &gemm_rs_clear);
   m.def("gemm_plan_splits", &gemm_plan_splits);

@@ -9,7 +9,6 @@ std::atomic<unsigned long long> g_launch_count{0};
 namespace wgmma {
 
 int g_dbg = 0;
-int g_bulk = -1;
 
 // Split-K factor for a persistent grid of `sms` CTAs walking equal-length tiles round-robin: minimise
 // waves x (k-blocks per slice + per-tile overhead).  A plain ceil(sms / tiles) overshoots the machine by a few tiles
@@ -37,8 +36,7 @@ static int choose_splits(int tiles, int num_kb, int sms) {
 // and the per-k-block barrier traffic between two sub-tiles, so it is taken as costing 1.7x a 128-row tile; it wins unless
 // halving the tile count wastes most of a wave.
 static bool use_tall_tiles(long long M, int nt, int eligible, int sms) {
-  static const bool enabled = [] { const char* e = getenv("TMPI_GEMM_TALL"); return !(e && e[0] == '0'); }();
-  if (!enabled || !eligible || M < 2 * BM) return false;
+  if (!eligible || M < 2 * BM) return false;
   const long long t1 = ((M + BM - 1) / BM) * nt, t2 = ((M + 2 * BM - 1) / (2 * BM)) * nt;
   const long long w1 = (t1 + sms - 1) / sms, w2 = (t2 + sms - 1) / sms;
   return w2 * 17 <= w1 * 10;
@@ -84,7 +82,6 @@ static ConvTile choose_conv_tile(int kind, long long M, int N, int groups, int n
 }  // namespace wgmma
 
 void gemm_set_debug(int flags) { wgmma::g_dbg = flags; }
-void gemm_set_bulk(int mask) { wgmma::g_bulk = mask; }
 
 // ---- reduce-scatter epilogue registry (see api.h)
 namespace wgmma {
@@ -260,7 +257,7 @@ static CUtensorMap make_im2col_map(const void* x, int N, int H, int W, int Ctot,
   int lower[2] = {-P, -P};
   int upper[2] = {P - (KW - 1), P - (KH - 1)};
   cuuint32_t estr[4] = {1u, (cuuint32_t)S, (cuuint32_t)S, 1u};
-  CUresult r = get_encode_im2col()(&m, esz == 4 ? f32_map_type() : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<char*>(base),
+  CUresult r = get_encode_im2col()(&m, map_type(esz), 4, const_cast<char*>(base),
                                    dims, strides, lower, upper, (cuuint32_t)(128 / esz), (cuuint32_t)pixels, estr,
                                    CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -286,7 +283,7 @@ static CUtensorMap make_weight_map(const void* w, int O, int taps, int Cg, int b
   cuuint64_t strides[2] = {(cuuint64_t)Cg * esz, (cuuint64_t)taps * Cg * esz};
   cuuint32_t box[3] = {(cuuint32_t)box_c, 1u, (cuuint32_t)box_o};
   cuuint32_t estr[3] = {1u, 1u, 1u};
-  CUresult r = get_encode()(&m, esz == 4 ? f32_map_type() : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(w), dims, strides,
+  CUresult r = get_encode()(&m, map_type(esz), 3, const_cast<void*>(w), dims, strides,
                             box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) throw std::runtime_error("tmpi_native: cuTensorMapEncodeTiled(3D weights) failed, code " + std::to_string((int)r));

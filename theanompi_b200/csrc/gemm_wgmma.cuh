@@ -97,15 +97,12 @@ struct Params {
   int group_m;          // tile raster: m-tiles per band (0 = plain m-fastest order); see tile_mn()
   int dbg;              // bottleneck probe (scripts/gemm_probe.py): 1 = skip A loads, 2 = skip B loads, 4 = skip the MMAs
   // reduce-scatter fused into the epilogue (fp32 wgrad outputs living in the symmetric gradient arena): element e of the G
-  // region is owned by rank ((e >> 10) - rs_blo) / rs_per; every 16-byte vector is red.add-ed into the OWNER's G over NVLink
-  // (rs_g[q] = rank q's G region as mapped here) instead of being stored locally.  rs_world == 0: off.
+  // region is owned by rank ((e >> 10) - rs_blo) / rs_per; every row segment of dW is added into the OWNER's G over NVLink
+  // (rs_g[q] = rank q's G region as mapped here) by the bulk copy engine instead of being stored locally.  rs_world == 0: off.
   int rs_world = 0, rs_rank = 0;
   unsigned rs_blo = 0, rs_per = 1;
   long long rs_e0 = 0;  // element index of C[0, 0] inside the G region
   float* rs_g[kMaxRanks] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-  // epilogue through the bulk copy engine (cp.async.bulk / cp.reduce.async.bulk, one 64–128 byte row segment per lane):
-  // bit 0 plain stores, bit 1 split-K reductions, bit 2 reduce-scatter reductions over NVLink (TMPI_GEMM_BULK, see launch())
-  int bulk = 0;
   // momentum-SGD epilogue (gemm_wgmma<SgdEpilogue<T>, ...> only): C is not written; the accumulator at (m, n) is the gradient of weight element
   // m * ldw + n, updated in place together with its momentum and bf16 shadow, exactly as sgd_flat would update it
   struct Sgd {
@@ -192,11 +189,8 @@ __device__ __forceinline__ void tma_load_im2col(uint32_t dst, const CUtensorMap*
       "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};"
       ::"r"(dst), "l"(map), "r"(bar), "r"(c), "r"(w), "r"(h), "r"(n), "h"((uint16_t)off_w), "h"((uint16_t)off_h) : "memory");
 }
-// Bulk (TMA engine) epilogue ops: one contiguous row segment shared → global per call; the reduce form adds fp32 into global
-// (or peer-mapped) memory as ONE packet per segment instead of 16-byte vector atomics.
-__device__ __forceinline__ void bulk_store(void* gdst, uint32_t ssrc, uint32_t bytes) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(ssrc), "r"(bytes) : "memory");
-}
+// Bulk (TMA engine) epilogue ops: one contiguous row segment of fp32 in shared memory added into global (or peer-mapped)
+// memory as ONE packet per call instead of 16-byte vector atomics.
 __device__ __forceinline__ void bulk_reduce_add_f32(void* gdst, uint32_t ssrc, uint32_t bytes) {
   asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [%0], [%1], %2;" ::"l"(gdst), "r"(ssrc), "r"(bytes) : "memory");
 }
@@ -817,27 +811,18 @@ gemm_wgmma(const __grid_constant__ CUtensorMap tmap_a0, const __grid_constant__ 
         }
         __syncwarp();
         // Fast path: chunk fully in range and 16-byte aligned → coalesced 16 B row-segment stores (plain, or vector
-        // reductions red.global.add.v4.f32 for split-K / the fused reduce-scatter).
+        // reductions red.global.add.v4.f32 for split-K); the fused reduce-scatter goes through the bulk copy engine.
         const bool staged = (nb + 32 <= n_end_c) && ld_ok && (((reinterpret_cast<uintptr_t>(Cg_ptr) + (long long)nb * esz) % 16) == 0);
         if (staged) {
-          const int bulk_kind = p.rs_world > 0 ? 4 : (p.atomic_out ? 2 : 1);
-          if (p.bulk & bulk_kind) {
-            // one row segment (32 columns) per lane through the bulk copy engine: the staging row is the source;
-            // generic-proxy writes are fenced into the async proxy first
+          if (p.rs_world > 0) {
+            // one row segment (32 columns) per lane, reduced into its owner's G as ONE bulk packet: the staging row is the
+            // source; generic-proxy writes are fenced into the async proxy first
             fence_proxy_async();
             const long long gm = (long long)mbase + lane;
             if (lane < 16 && gm < p.M) {
-              const uint32_t ssrc = smem_u32(wstage + (size_t)lane * pitch);
-              const uint32_t nbytes = (uint32_t)(32 * esz);
-              if (p.rs_world > 0) {
-                bool local;
-                float* d = rs_addr(p, p.rs_e0 + gm * p.ldc + nb, local);
-                bulk_reduce_add_f32(d, ssrc, nbytes);
-              } else if (p.atomic_out) {
-                bulk_reduce_add_f32(Cg_ptr + ((long long)gm * p.ldc + nb) * esz, ssrc, nbytes);
-              } else {
-                bulk_store(Cg_ptr + ((long long)gm * p.ldc + nb) * esz, ssrc, nbytes);
-              }
+              bool local;
+              float* d = rs_addr(p, p.rs_e0 + gm * p.ldc + nb, local);
+              bulk_reduce_add_f32(d, smem_u32(wstage + (size_t)lane * pitch), (uint32_t)(32 * esz));
             }
             bulk_commit();
             bulk_wait_read();                                  // staging row may be overwritten by the next chunk
@@ -849,19 +834,7 @@ gemm_wgmma(const __grid_constant__ CUtensorMap tmap_a0, const __grid_constant__ 
               if (gm < p.M) {
                 const uint4 val = *reinterpret_cast<const uint4*>(wstage + (size_t)rr * pitch + (size_t)lv * 16);
                 uint8_t* gp = gbase + gm * p.ldc * esz;
-                if (p.rs_world > 0) {
-                  // fused reduce-scatter: this 16-byte vector of dW goes to the rank that owns it in the exchange
-                  bool local;
-                  float* d = rs_addr(p, p.rs_e0 + gm * p.ldc + nb + lv * 4, local);
-                  if (local) {
-                    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(d), "f"(__uint_as_float(val.x)),
-                                 "f"(__uint_as_float(val.y)), "f"(__uint_as_float(val.z)), "f"(__uint_as_float(val.w)) : "memory");
-                  } else {
-                    // ONE 16-byte vector reduction per NVLink packet
-                    asm volatile("red.relaxed.sys.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(d), "f"(__uint_as_float(val.x)),
-                                 "f"(__uint_as_float(val.y)), "f"(__uint_as_float(val.z)), "f"(__uint_as_float(val.w)) : "memory");
-                  }
-                } else if (p.atomic_out) {
+                if (p.atomic_out) {
                   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(gp), "f"(__uint_as_float(val.x)),
                                "f"(__uint_as_float(val.y)), "f"(__uint_as_float(val.z)), "f"(__uint_as_float(val.w)) : "memory");
                 } else {
@@ -892,7 +865,7 @@ gemm_wgmma(const __grid_constant__ CUtensorMap tmap_a0, const __grid_constant__ 
       }
     }
   }
-  if (p.bulk) bulk_wait_all();                                 // bulk stores / reductions have landed before the kernel retires
+  if (p.rs_world > 0) bulk_wait_all();                         // bulk reductions have landed before the kernel retires
 }
 
 
@@ -915,11 +888,10 @@ static PFN_encodeTiled get_encode() {
   return fn;
 }
 
-// fp32 operands of the tf32 path are described to the TMA unit as TFLOAT32 (the tensor core alone would truncate the low 13
-// mantissa bits, a biased error that does not average out over K).  TMPI_TF32_TMA_ROUND=0 falls back to raw fp32 bits.
-static CUtensorMapDataType f32_map_type() {
-  static const bool rnd = [] { const char* e = getenv("TMPI_TF32_TMA_ROUND"); return !(e && e[0] == '0'); }();
-  return rnd ? CU_TENSOR_MAP_DATA_TYPE_TFLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+// Element type of a tensor map: fp32 operands of the tf32 path are described to the TMA unit as TFLOAT32, which rounds them
+// (the tensor core alone would truncate the low 13 mantissa bits, a biased error that does not average out over K).
+static CUtensorMapDataType map_type(int esz) {
+  return esz == 4 ? CU_TENSOR_MAP_DATA_TYPE_TFLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
 }
 
 // 2-D tensor map (bf16 or fp32 elements): dims {inner, outer}, row pitch in bytes, box {128 bytes, box_outer}, 128B swizzle,
@@ -941,7 +913,7 @@ static CUtensorMap make_tmap(const void* ptr, uint64_t inner, uint64_t outer, ui
   cuuint64_t strides[1] = {pitch_bytes};
   cuuint32_t box[2] = {(cuuint32_t)(128 / esz), box_outer};
   cuuint32_t estr[2] = {1u, 1u};
-  CUresult r = get_encode()(&m, esz == 4 ? f32_map_type() : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+  CUresult r = get_encode()(&m, map_type(esz), 2, const_cast<void*>(ptr), dims, strides, box, estr,
                             CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) throw std::runtime_error("tmpi_native: cuTensorMapEncodeTiled failed, code " + std::to_string((int)r));
@@ -951,11 +923,6 @@ static CUtensorMap make_tmap(const void* ptr, uint64_t inner, uint64_t outer, ui
 }
 
 extern int g_dbg;                  // gemm_set_debug()
-extern int g_bulk;                 // gemm_set_bulk(): -1 = TMPI_GEMM_BULK env (default 4: reduce-scatter reductions only)
-static int bulk_default() {
-  static const int v = [] { const char* e = getenv("TMPI_GEMM_BULK"); return e ? atoi(e) : 4; }();
-  return v;
-}
 
 template <typename OP, int BN, int MT>
 static void launch(const CUtensorMap& ta, const CUtensorMap& tb, Params& p, int splits, cudaStream_t st,
@@ -963,7 +930,6 @@ static void launch(const CUtensorMap& ta, const CUtensorMap& tb, Params& p, int 
   using T = typename Operand<OP>::Type;
   using C = Cfg<T, BN, MT>;
   p.dbg = g_dbg;
-  p.bulk = g_bulk < 0 ? bulk_default() : g_bulk;
   if (!ta1) { p.groups = 1; p.C1 = nullptr; p.bias1 = nullptr; }
   static bool attr_set = false;
   if (!attr_set) {

@@ -19,8 +19,6 @@ Everything raises if the extension is missing — there is no eager fallback on 
 """
 from __future__ import annotations
 
-import os
-
 import numpy as np
 import torch
 
@@ -146,7 +144,7 @@ def linear_bias_act(x, w, b, relu=True):
     xa, lda = _rows8(x2)
     wa, ldb = _rows8(_bf(w))
     bias = b.float() if b is not None and b.dtype != torch.float32 else b
-    if (FC_SPLITK and B_ <= 128 and I >= 1024 and O % 8 == 0) or _act(relu) > 1:
+    if (B_ <= 128 and I >= 1024 and O % 8 == 0) or _act(relu) > 1:
         # small-batch FC forward is a weight stream: one m-tile, so the parallelism comes from n-tiles x split-K (fp32
         # reductions into a scratch tile), followed by a tiny bias + ReLU (+ bf16 cast) pass; fp32 output is finished in
         # place.  (The fused-epilogue kernel needs 32-wide tiles to fill the machine and then re-reads the activations 128
@@ -291,16 +289,11 @@ def _w2d(w, K, Kp):
     return wp
 
 
-GROUP2_FUSED = os.environ.get("TMPI_GROUP2_FUSED", "1") != "0"   # both groups of a 2-group conv per launch
-FC_SPLITK = os.environ.get("TMPI_FC_SPLITK", "1") != "0"      # small-batch FC forward: n-tiles x split-K + finishing pass
-CONV_MODE = os.environ.get("TMPI_CONV", "implicit")      # implicit: TMA-im2col implicit GEMM; explicit: im2col matrix + GEMM
-
-
 def _implicit_ok(x, w, c_off, Cg, Ot, o_off):
     """TMA im2col needs 16-byte aligned channel slices; C = 3 (first layer) stays on the explicit path."""
     Ct = x.shape[3]
     al = _al(x)
-    return (CONV_MODE == "implicit" and Cg % al == 0 and c_off % al == 0 and Ct % al == 0 and Ot % al == 0 and o_off % al == 0
+    return (Cg % al == 0 and c_off % al == 0 and Ct % al == 0 and Ot % al == 0 and o_off % al == 0
             and w.shape[0] % al == 0 and w.is_contiguous() and w.data_ptr() % 16 == 0)
 
 
@@ -327,7 +320,7 @@ def _conv_fwd_group(x, w, b, y, o_off, c_off, Cg, s, p, relu):
 def _s2d_geom(H, W, C, KH, KW, stride, pad):
     """Geometry of the space-to-depth rewrite of a strided few-channel conv, or None when it does not apply.  The zero padding
     of the original convolution is folded into the space-to-depth image (the kernel reads x[S*i + dy - pad, ...])."""
-    if not (CONV_MODE == "implicit" and C < 8 and C % 4 != 0 and stride > 1):
+    if not (C < 8 and C % 4 != 0 and stride > 1):
         return None
     S = stride
     Hp, Wp = H + 2 * pad, W + 2 * pad
@@ -428,7 +421,7 @@ def conv2d_group2_bias_act(x, w0, b0, w1, b1, stride, pad, relu, return_cols=Fal
     y = torch.empty((N, Ho, Wo, 2 * Og), dtype=x.dtype, device=x.device)
     wb0, wb1 = _bf(w0), _bf(w1)
     es, f32 = x.element_size(), int(_is32(x))
-    if GROUP2_FUSED and _implicit_ok(x, wb0, 0, Cg, 2 * Og, 0) and _implicit_ok(x, wb1, Cg, Cg, 2 * Og, Og) and (b0 is None) == (b1 is None):
+    if _implicit_ok(x, wb0, 0, Cg, 2 * Og, 0) and _implicit_ok(x, wb1, Cg, Cg, 2 * Og, Og) and (b0 is None) == (b1 is None):
         # both groups in ONE persistent launch: their tiles fill the SMs together instead of two under-filled waves
         L().conv_fprop2(x.data_ptr(), wb0.data_ptr(), wb1.data_ptr(), y.data_ptr(), y.data_ptr() + Og * es, _p(b0), _p(b1), N, H, W, C, 0,
                         int(Cg), int(Cg), KH, KW, Ho, Wo, int(stride), int(pad), Og, 2 * Og, int(bool(relu)), 0, f32, _st(x))
@@ -532,7 +525,7 @@ def conv2d_group2_bias_act_bwd(x, w0, w1, y, dy, stride, pad, relu, need_dx, out
     wb0, wb1 = _bf(w0), _bf(w1)
     Ot = 2 * Og
     no_cols = not cols or (cols[0] is None and cols[1] is None)
-    if (GROUP2_FUSED and no_cols and _implicit_ok(x, wb0, 0, Cg, Ot, 0) and _implicit_ok(x, wb1, Cg, Cg, Ot, Og)
+    if (no_cols and _implicit_ok(x, wb0, 0, Cg, Ot, 0) and _implicit_ok(x, wb1, Cg, Cg, Ot, Og)
             and (not need_dx or stride == 1)):
         # ---- both groups per launch: one mask/bias pass over the full width, one wgrad launch, one dgrad launch
         N, H, W, Ct = x.shape

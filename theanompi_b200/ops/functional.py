@@ -25,8 +25,6 @@ import os
 from . import accum
 from . import reference as ref
 
-CACHE_COL = os.environ.get("TMPI_CACHE_COL", "1") != "0"
-
 
 def _impl(x):
     if x.is_cuda:
@@ -128,8 +126,6 @@ class _ConvFn(torch.autograd.Function):
             # keep the im2col matrix of the forward for wgrad (memory is cheap on an 80 GB part; recomputing
             # it cost ~13 % of the AlexNet step)
             y, ctx.cols = impl.conv2d_bias_act(x, wc, b, stride, pad, groups, relu, return_cols=True)
-            if not CACHE_COL:
-                ctx.cols = None
         ctx.w, ctx.b = w, b
         ctx.cfg = (stride, pad, groups, relu)
         ctx.pool = pool
@@ -201,8 +197,6 @@ class _ConvG2Fn(torch.autograd.Function):
             ctx.cols = None
         else:
             y, ctx.cols = impl.conv2d_group2_bias_act(x, ws[0], b0, ws[1], b1, stride, pad, relu, return_cols=True)
-            if not CACHE_COL:
-                ctx.cols = None
         ctx.p = (w0, b0, w1, b1)
         ctx.cfg = (stride, pad, relu)
         ctx.pool = pool
