@@ -371,6 +371,27 @@ struct EmaArgs {
 void ema_advance(void* state, long long every, long long warmup, cudaStream_t st);
 void ema_update(const EmaArgs& a, cudaStream_t st);
 void ema_swap(const EmaArgs& a, cudaStream_t st);
+// Sharpness-aware minimization (utils/opt.py: Sam), over the n_blocks arena blocks.  sam_norm, two launches: per-block Σg² (SAM) or
+// Σ(w·g)² (adaptive, ASAM) over the real elements into partial ([n_blocks] fp32), then one CTA sums them in fp64 in a fixed order and
+// writes the ClipRecord *rec: n = ‖g‖ or ‖|w|⊙g‖ rounded to fp32, s = fp32(1 / (n + 1e-12)) · rho, finite.  sam_perturb, one launch:
+// P ← W; if finite, W ← W + e on the real elements with e = g·s or ((w·w)·g)·s, H ← bf16(W).  sam_restore, one launch: W ← P,
+// H ← bf16(P).  H may be null (no bf16 shadow).
+struct SamArgs {
+  void* W;
+  const void* G;
+  void* P;
+  void* H;
+  const void* block_tensor;
+  const void* tensor_span;
+  long long n_blocks;
+  float rho;
+  int adaptive;
+  void* partial;
+  void* rec;
+};
+void sam_norm(const SamArgs& a, cudaStream_t st);
+void sam_perturb(const SamArgs& a, cudaStream_t st);
+void sam_restore(const SamArgs& a, cudaStream_t st);
 // device-side gossip (GOSGD): state = 64 uint32 of local device memory, [0] holds the push-sum weight (float)
 void gosgd_push(const CommCtx& c, void* state, int dest, long long w_off, long long snap_off, long long n, int max_blocks, cudaStream_t st);
 void gosgd_poll_merge(const CommCtx& c, void* state, long long w_off, long long h_off, long long snap_off, long long n, int max_blocks,

@@ -248,6 +248,14 @@ PYBIND11_MODULE(_tmpi_native, m) {
     ema_update(EmaArgs{P(W), P(E), nullptr, n, P(segs), n_segs, P(state), decay, one_minus_decay}, S(st)); });
   m.def("ema_swap", [](ptr_t W, ptr_t E, ptr_t H, long long n, ptr_t segs, int n_segs, ptr_t st) {
     ema_swap(EmaArgs{P(W), P(E), P(H), n, P(segs), n_segs, nullptr, 0.f, 0.f}, S(st)); });
+  m.def("sam_norm", [](ptr_t W, ptr_t G, ptr_t block_tensor, ptr_t tensor_span, long long n_blocks, float rho, int adaptive, ptr_t partial,
+                       ptr_t rec, ptr_t st) {
+    sam_norm(SamArgs{P(W), P(G), nullptr, nullptr, P(block_tensor), P(tensor_span), n_blocks, rho, adaptive, P(partial), P(rec)}, S(st)); });
+  m.def("sam_perturb", [](ptr_t W, ptr_t G, ptr_t Pw, ptr_t H, ptr_t block_tensor, ptr_t tensor_span, long long n_blocks, int adaptive,
+                          ptr_t rec, ptr_t st) {
+    sam_perturb(SamArgs{P(W), P(G), P(Pw), P(H), P(block_tensor), P(tensor_span), n_blocks, 0.f, adaptive, nullptr, P(rec)}, S(st)); });
+  m.def("sam_restore", [](ptr_t W, ptr_t Pw, ptr_t H, long long n_blocks, ptr_t st) {
+    sam_restore(SamArgs{P(W), nullptr, P(Pw), P(H), nullptr, nullptr, n_blocks, 0.f, 0, nullptr, nullptr}, S(st)); });
   m.def("gosgd_merge", [](ptr_t w, ptr_t h, ptr_t b, float a_self, float a_src, long long n, int max_blocks, ptr_t st) {
     gosgd_merge(P(w), P(h), P(b), a_self, a_src, n, max_blocks, S(st)); });
   m.def("cast_flat", [](ptr_t src, ptr_t dst, long long n, int kind, ptr_t st) { cast_flat(P(src), P(dst), n, kind, S(st)); });

@@ -1176,6 +1176,150 @@ void ema_swap(const EmaArgs& a, cudaStream_t st) {
   count_launch(); TMPI_CHECK_LAUNCH("ema_swap"); ::tmpi::check_capture(st, "ema_swap");
 }
 
+// ============================================================================ sharpness-aware minimization (utils/opt.py: Sam)
+// The products and sums below use mul.rn / add.rn / rcp.rn without .ftz (the build's --use_fast_math would flush subnormals in
+// __fmul_rn and friends) and are never contracted into an FMA, so each is rounded once, as torch's fp32 CPU expressions are.
+__device__ __forceinline__ float mul_rn(float a, float b) { float r; asm("mul.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b)); return r; }
+__device__ __forceinline__ float add_rn(float a, float b) { float r; asm("add.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b)); return r; }
+
+// ASAM's pass 1: partial[b] = Σ(w·g)² over the real elements of block b, w·g rounded once; the reduction of lars_partial_kernel (no
+// atomics, the result does not depend on the grid).  SAM's Σg² is lars_partial_kernel<false>.
+__global__ void __launch_bounds__(kThreads) sam_partial_wg_kernel(const float* __restrict__ W, const float* __restrict__ G,
+                                                                  const int* __restrict__ block_tensor,
+                                                                  const long long* __restrict__ tensor_span, float* __restrict__ partial,
+                                                                  long long n_blocks) {
+  __shared__ float red[kThreads / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (long long b = blockIdx.x; b < n_blocks; b += gridDim.x) {
+    const long long i = b * kArenaBlock + threadIdx.x * 4;
+    const int t = block_tensor[b];
+    const long long end = tensor_span[2 * t] + tensor_span[2 * t + 1];
+    const float4 w = *reinterpret_cast<const float4*>(W + i), g = *reinterpret_cast<const float4*>(G + i);
+    float4 p = make_float4(mul_rn(w.x, g.x), mul_rn(w.y, g.y), mul_rn(w.z, g.z), mul_rn(w.w, g.w));
+    if (i + 4 > end) {                                   // the tensor's last block: zero the padding past its end
+      if (i + 0 >= end) p.x = 0.f;
+      if (i + 1 >= end) p.y = 0.f;
+      if (i + 2 >= end) p.z = 0.f;
+      if (i + 3 >= end) p.w = 0.f;
+    }
+    float s = warp_sum(p.x * p.x + p.y * p.y + p.z * p.z + p.w * p.w);
+    if (lane == 0) red[warp] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      s = red[0];
+#pragma unroll
+      for (int k = 1; k < kThreads / 32; ++k) s += red[k];
+      partial[b] = s;
+    }
+    __syncthreads();                                     // red[] is reused by the next block
+  }
+}
+
+// Pass 2: one CTA sums the n_blocks partials in fp64 in a fixed order (as clip_finalize_kernel) and writes the record:
+// n = fp32(sqrt(Σ)), s = fp32(1 / fp32(n + 1e-12)) · fp32(rho), which is how torch evaluates rho / (grad_norm + 1e-12) on an fp32
+// tensor (Tensor.__rtruediv__ is reciprocal() * other), and finite = n is neither NaN nor Inf.
+__global__ void __launch_bounds__(kThreads) sam_finalize_kernel(const float* __restrict__ partial, long long n_blocks, float rho,
+                                                                ClipRecord* __restrict__ rec) {
+  __shared__ double red[kThreads / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  double s = 0.0;
+  for (long long k = threadIdx.x; k < n_blocks; k += kThreads) s += (double)partial[k];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) red[warp] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    s = red[0];
+    for (int k = 1; k < kThreads / 32; ++k) s += red[k];
+    const float n = (float)sqrt(s);
+    const bool finite = isfinite(n);
+    float r;
+    asm("rcp.rn.f32 %0, %1;" : "=f"(r) : "f"(add_rn(n, 1e-12f)));
+    ClipRecord out;
+    out.norm = n;
+    out.scale = finite ? mul_rn(r, rho) : 0.f;
+    out.finite = finite ? 1 : 0;
+    out.pad = 0;
+    *rec = out;
+  }
+}
+
+// The ascent step, one pass: P ← W, then on the real elements W ← W + e with e = g·s (SAM) or ((w·w)·g)·s (ASAM), and H ← bf16-RN(W)
+// when there is a shadow.  A non-finite record only copies W into P.  Reads W and G, writes P, W and H: 18 B per element.
+template <bool kAdaptive>
+__global__ void __launch_bounds__(kThreads) sam_perturb_kernel(float* __restrict__ W, const float* __restrict__ G, float* __restrict__ P,
+                                                               __nv_bfloat16* __restrict__ H, const int* __restrict__ block_tensor,
+                                                               const long long* __restrict__ tensor_span, long long n_blocks,
+                                                               const ClipRecord* __restrict__ rec) {
+  const float s = rec->scale;
+  const bool finite = rec->finite != 0;
+  for (long long b = blockIdx.x; b < n_blocks; b += gridDim.x) {
+    const long long i = b * kArenaBlock + threadIdx.x * 4;
+    const float4 w = *reinterpret_cast<const float4*>(W + i);
+    *reinterpret_cast<float4*>(P + i) = w;
+    if (!finite) continue;
+    const int t = block_tensor[b];
+    const long long end = tensor_span[2 * t] + tensor_span[2 * t + 1];
+    const float4 g = *reinterpret_cast<const float4*>(G + i);
+    float o[4] = {w.x, w.y, w.z, w.w};
+    const float wv[4] = {w.x, w.y, w.z, w.w}, gv[4] = {g.x, g.y, g.z, g.w};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      if (i + k >= end) continue;                        // padding past the tensor's end stays as it is
+      const float d = kAdaptive ? mul_rn(mul_rn(wv[k], wv[k]), gv[k]) : gv[k];
+      o[k] = add_rn(wv[k], mul_rn(d, s));
+    }
+    const float4 nw = make_float4(o[0], o[1], o[2], o[3]);
+    *reinterpret_cast<float4*>(W + i) = nw;
+    if (H) *reinterpret_cast<uint2*>(H + i) = pack_bf16x4(nw);
+  }
+}
+
+// The restore: W ← P, H ← bf16-RN(P).  Reads P, writes W and H: 10 B per element.
+__global__ void __launch_bounds__(kThreads) sam_restore_kernel(float* __restrict__ W, const float* __restrict__ P, __nv_bfloat16* __restrict__ H,
+                                                               long long n_blocks) {
+  for (long long b = blockIdx.x; b < n_blocks; b += gridDim.x) {
+    const long long i = b * kArenaBlock + threadIdx.x * 4;
+    const float4 p = *reinterpret_cast<const float4*>(P + i);
+    *reinterpret_cast<float4*>(W + i) = p;
+    if (H) *reinterpret_cast<uint2*>(H + i) = pack_bf16x4(p);
+  }
+}
+
+static int sam_grid(const SamArgs& a, const char* name, bool ok) {
+  if (a.n_blocks <= 0) throw std::runtime_error(std::string(name) + ": empty arena");
+  if (!a.W || !ok) throw std::runtime_error(std::string(name) + ": missing buffers");
+  return (int)std::min<long long>(a.n_blocks, (long long)sm_count() * 8);
+}
+
+void sam_norm(const SamArgs& a, cudaStream_t st) {
+  const int grid = sam_grid(a, "sam_norm", a.G && a.partial && a.rec && a.block_tensor && a.tensor_span);
+  if (!(a.rho > 0.f) || !std::isfinite(a.rho)) throw std::runtime_error("sam_norm: rho must be finite and positive");
+  if (a.adaptive)
+    sam_partial_wg_kernel<<<grid, kThreads, 0, st>>>((const float*)a.W, (const float*)a.G, (const int*)a.block_tensor,
+                                                     (const long long*)a.tensor_span, (float*)a.partial, a.n_blocks);
+  else
+    lars_partial_kernel<false><<<grid, kThreads, 0, st>>>(nullptr, (const float*)a.G, (const int*)a.block_tensor,
+                                                          (const long long*)a.tensor_span, (float*)a.partial, 0, a.n_blocks);
+  TMPI_CHECK_LAUNCH("sam_partial");
+  sam_finalize_kernel<<<1, kThreads, 0, st>>>((const float*)a.partial, a.n_blocks, a.rho, (ClipRecord*)a.rec);
+  count_launch(2); TMPI_CHECK_LAUNCH("sam_finalize"); ::tmpi::check_capture(st, "sam_norm");
+}
+
+void sam_perturb(const SamArgs& a, cudaStream_t st) {
+  const int grid = sam_grid(a, "sam_perturb", a.G && a.P && a.rec && a.block_tensor && a.tensor_span);
+  auto k = a.adaptive ? sam_perturb_kernel<true> : sam_perturb_kernel<false>;
+  k<<<grid, kThreads, 0, st>>>((float*)a.W, (const float*)a.G, (float*)a.P, (__nv_bfloat16*)a.H, (const int*)a.block_tensor,
+                               (const long long*)a.tensor_span, a.n_blocks, (const ClipRecord*)a.rec);
+  count_launch(); TMPI_CHECK_LAUNCH("sam_perturb"); ::tmpi::check_capture(st, "sam_perturb");
+}
+
+void sam_restore(const SamArgs& a, cudaStream_t st) {
+  const int grid = sam_grid(a, "sam_restore", a.P != nullptr);
+  sam_restore_kernel<<<grid, kThreads, 0, st>>>((float*)a.W, (const float*)a.P, (__nv_bfloat16*)a.H, a.n_blocks);
+  count_launch(); TMPI_CHECK_LAUNCH("sam_restore"); ::tmpi::check_capture(st, "sam_restore");
+}
+
 // ============================================================================ GOSGD:  w ← (a_self·w + a_src·b) / (a_self + a_src)
 // Host-driven form (CPU-mirrored semantics, tests): coefficients passed by value, `b` = local mailbox or a peer's snapshot.
 template <int U>

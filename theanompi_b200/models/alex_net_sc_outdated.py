@@ -10,6 +10,7 @@ class AlexNet_sc(AlexNet):
     graph_safe = False            # the in-graph Crop layer draws offsets / mirrors from the host RNG every step
     supports_mixup = False        # the outdated in-step Subtract / Crop variant of AlexNet
     supports_model_ema = False    # the outdated variant: the average is offered on the loader-fed AlexNet
+    supports_sam = False          # its in-graph Crop draws new crops at every forward: a second forward would see another crop
     supports_resized_crop = False  # its crop is the in-graph Crop layer, not the loader's
     def __init__(self, config):
         config = dict(config)

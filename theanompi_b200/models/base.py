@@ -32,7 +32,7 @@ import torch
 from .. import ops
 from ..parallel.arena import FlatArena
 from ..utils import nvtx
-from ..utils.opt import FlatSGD, LrSchedule, ModelEma, SharedScalar, pre_model_iter_fn
+from ..utils.opt import FlatSGD, LrSchedule, ModelEma, Sam, SharedScalar, pre_model_iter_fn
 from .layers2 import BatchNormal, Crop, Dropout, count_params
 
 
@@ -73,6 +73,8 @@ class ModelBase(object):
     supports_drop_path = False     # config['drop_path_rate'] > 0 (True: residual blocks in self.body that read drop_row(l))
     supports_cifar_augment = False  # config['cifar_augment'] (True: a CIFAR model whose training forward reads train_augment())
     supports_model_ema = True      # config['model_ema'] (False: no single arena updated by the step tail; refused at compile_iter_fns)
+    # config['sam'] (False: the step cannot run its training forward twice on the same draws; refused at compile_iter_fns)
+    supports_sam = True
     # True: an ImageNet model fed by ParaLoader, so config['random_resized_crop'], config['color_jitter'] and
     # config['random_erasing'] reach its loader
     # (refused at construction otherwise)
@@ -128,6 +130,11 @@ class ModelBase(object):
         # after every update's step tail average W into E; ema_weights() validates, infers and saves with E.  Built by check_model_ema
         self.model_ema = config.get("model_ema")
         self.ema = None
+        # sharpness-aware minimization (a dict, utils/opt.py: Sam; None = off): after the step's forward and backward the weights move
+        # to the ascent point, a second forward and backward there on the same batch and draws gives the gradient the optimizer steps
+        # on, and the weights are restored before it.  Built by check_sam
+        self.sam = config.get("sam")
+        self.sam_opt = None
         # label smoothing ε of the training loss (cross-entropy against (1 − ε)·onehot + ε / C; 0 = plain NLL); validation stays
         # plain NLL.  Checked by check_label_smoothing at compile_iter_fns
         self.label_smoothing = config.get("label_smoothing", 0.0)
@@ -245,16 +252,34 @@ class ModelBase(object):
         # it: validation and inference never drop
         # with config['cifar_augment'] the offsets, flips and Cutout boxes are drawn last, from the same counter, and likewise only this
         # forward reads them
+        # with config['sam'] the second pass at the ascent point reuses every draw: the step counter only advances in _after_step
         rec = None
         if self.mixer is not None:
             rec = self.mixer.draw()
             self.mix_input(rec)
         if self.drop_path is not None:
             self.drop_path.draw()
-            self._drop_on = True
         if self.cifar_aug is not None:
             self.cifar_aug.draw()
-            self._aug_on = True
+        out = self._train_pass(rec)
+        if self.sam_opt is not None:
+            with torch.no_grad():
+                self.sam_opt.perturb()
+            if rec is not None:
+                self.repeat_mix(rec)
+            with self.bn_stats_frozen():
+                self._train_pass(rec)
+            with torch.no_grad():
+                self.sam_opt.restore()
+            self._dbg_capture("sam")
+        return out
+
+    def _train_pass(self, rec):
+        """Forward and backward of the training step on x_in with the draws of this step already made: the drop-path table and the
+        cifar_augment draw are read by the forward, ``rec`` (the Mixup / CutMix record, or None) gives the mixed target, and the
+        batch is mixed at the mix point as :meth:`mix_input` left it.  The gradient is stored in the arena's G region."""
+        self._drop_on = self.drop_path is not None
+        self._aug_on = self.cifar_aug is not None
         try:
             if rec is None:
                 cost, err, err5 = self.loss(self.x_in, self.y_in, self.label_smoothing)
@@ -366,6 +391,10 @@ class ModelBase(object):
         """Mix this step's batch at the mix point as the record ``rec`` says: x_in, in place.  x_in is refilled from shared_x every
         step; shared_x itself (the loader's buffer, sliced into sub-batches and read by validation) is never mixed."""
         ops.mix_batch(self.x_in, rec)
+
+    def repeat_mix(self, rec):
+        """Before a second training forward of the same step (``config['sam']``): mix the mix point again as :meth:`mix_input` did with
+        ``rec``.  x_in still holds the mixed batch, so by default there is nothing to do."""
 
     def check_mixup(self):
         """``config['mixup']`` must be None or a valid dict (ops/mixup.py: check_config; a ValueError names the offending key), and a
@@ -698,7 +727,7 @@ class ModelBase(object):
     def setup_train_options(self, k=1, fused_tail=None, optimizer=None):
         """Check and build the training options of the config for a step of ``k`` workers (k > 1: BSP ``sync_type='cdd'``),
         ``fused_tail`` (a fused exchange strategy's step tail, or None) and ``optimizer`` (default: the model's): grad_accum,
-        label_smoothing, mixup, cifar_augment, drop_path_rate, lr_schedule, grad_clip and model_ema.  A model refuses every option it
+        label_smoothing, mixup, cifar_augment, drop_path_rate, lr_schedule, grad_clip, model_ema and sam.  A model refuses every option it
         does not support here, with a ValueError that names it."""
         self.check_grad_accum(fused_tail)
         self.check_label_smoothing()
@@ -713,6 +742,49 @@ class ModelBase(object):
                              "Use a split strategy: ar, nccl32, nccl16, asa32, asa16 or p2p32" % opt)
         self.check_grad_clip(k, fused_tail, opt)
         self.check_model_ema(k, fused_tail)
+        self.check_sam(fused_tail)
+
+    def check_sam(self, fused_tail=None):
+        """``config['sam']`` must be None or a valid dict (utils/opt.py: Sam.check_config; a ValueError names the key).  A dict needs a
+        model that can run its training forward twice on the same draws (``supports_sam``), ``grad_accum`` = 1 (the ascent step needs
+        the whole window's gradient) and no ``fused_tail`` (a fused exchange strategy's bucket launches would fire during the first
+        backward).  Each worker perturbs by its own gradient (m-sharpness, m = its batch): one worker, BSP 'avg' or 'cdd' over a split
+        strategy, EASGD, ASGD and GOSGD.  Builds :class:`Sam`."""
+        self.sam_opt = None
+        if self.sam is None:
+            return
+        key = Sam.KEY
+        cfg = Sam.check_config(self.sam)
+        supported = ("%s runs on AlexNet, GoogLeNet, VGG16, ResNet50, ResNet152 and Wide_ResNet with grad_accum = 1: on one worker, BSP "
+                     "sync_type='avg' or 'cdd' over a split strategy (ar, nccl32, nccl16, asa32, asa16, p2p32), EASGD, ASGD or GOSGD" % key)
+        if not self.supports_sam:
+            raise ValueError("%s: %s is not supported; %s" % (self.name, key, supported))
+        if self.grad_accum > 1:
+            raise ValueError("%s: %s does not combine with grad_accum = %d: the ascent step needs the gradient of the whole window; %s"
+                             % (self.name, key, self.grad_accum, supported))
+        if fused_tail is not None:
+            raise ValueError("%s: %s does not combine with a fused exchange strategy, whose bucket launches would fire during the first "
+                             "backward; %s" % (self.name, key, supported))
+        self.sam_opt = Sam(self.arena, cfg)
+
+    @property
+    def sam_norm(self):
+        """n = ‖g‖ (ASAM: ‖|w|⊙g‖) of the last training step's first gradient (``config['sam']``; a device scalar, NaN or Inf when the
+        weights were not moved), or None without the key."""
+        return None if self.sam_opt is None else self.sam_opt.norm
+
+    @contextlib.contextmanager
+    def bn_stats_frozen(self):
+        """Inside the block this model's batch-norm layers still normalise with batch statistics in training mode, but do not update
+        their running mean and variance (SAM's second pass)."""
+        layers = self._bn_layers()
+        for l in layers:
+            l.update_stats = False
+        try:
+            yield
+        finally:
+            for l in layers:
+                l.update_stats = True
 
     def check_model_ema(self, k=1, fused_tail=None):
         """``config['model_ema']`` must be None or a valid dict (utils/opt.py: ModelEma.check_config; a ValueError names the key).  A

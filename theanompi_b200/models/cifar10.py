@@ -28,6 +28,7 @@ monitor_grad = False
 
 class Cifar10_model(ModelBase):
     graph_safe = False            # the in-graph Crop layer draws offsets / mirrors from the host RNG every step
+    supports_sam = False          # that Crop draws at every forward: a second forward of the step would see another crop
     n_epochs, momentum, weight_decay = n_epochs, momentum, weight_decay
     batch_size, file_batch_size, learning_rate = batch_size, file_batch_size, learning_rate
     lr_policy, lr_step = lr_policy, lr_step

@@ -133,6 +133,11 @@ class Wide_ResNet(ModelBase):
             return super().mix_input(rec)
         self._mix_rec = rec
 
+    def repeat_mix(self, rec):
+        """With cifar_augment the forward consumed the record: hand it over again for the second forward of the step."""
+        if self.cifar_aug is not None:
+            self._mix_rec = rec
+
     def forward(self, x):
         from ... import ops
         aug = self.train_augment()                               # this training step's cifar_augment draw, else None

@@ -236,6 +236,7 @@ class NativeWGAN(ModelBase):
     ``grad_clip`` is simply available."""
     supports_grad_accum = False    # its critic / generator steps keep their own gaccum accumulation
     supports_model_ema = False     # two arenas, critic and generator
+    supports_sam = False           # two arenas and an adversarial step, not one loss to flatten
     supports_lr_schedule = False   # two arenas and critic / generator step ratios: the reference's per-epoch decay
     supports_label_smoothing = False   # no classifier head
     supports_mixup = False             # no classifier head

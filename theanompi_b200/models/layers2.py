@@ -436,6 +436,7 @@ class BatchNormal(Layer):
         self.running_var = torch.ones(C)
         self.eps, self.momentum, self.relu = eps, momentum, relu
         self.training = True
+        self.update_stats = True       # False: training mode without a running-statistics update (ModelBase.bn_stats_frozen)
         BatchNormal.layers.append(self)
         self.output_shape = self.input_shape
         self.name = "BatchNorm"
@@ -448,8 +449,9 @@ class BatchNormal(Layer):
         if self.running_mean.device != x.device:
             self.running_mean = self.running_mean.to(x.device)
             self.running_var = self.running_var.to(x.device)
-        return ops.batch_norm(x, self.gamma.val, self.beta.val, self.running_mean, self.running_var, self.training,
-                              self.momentum, self.eps, self.relu, residual, drop=drop)
+        keep = self.update_stats or not self.training
+        return ops.batch_norm(x, self.gamma.val, self.beta.val, self.running_mean if keep else None, self.running_var if keep else None,
+                              self.training, self.momentum, self.eps, self.relu, residual, drop=drop)
 
     @staticmethod
     def SetTrainOn():

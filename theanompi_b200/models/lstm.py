@@ -112,6 +112,7 @@ class LSTM(ModelBase):
     supports_mixup = False         # token input: nothing to mix
     supports_grad_accum = False    # one graph per sequence-length bucket, each with its own update
     supports_model_ema = False     # one graph per sequence-length bucket
+    supports_sam = False           # its step has its own forward and backward per bucket
     n_epochs = max_epochs
     batch_size = file_batch_size = batch_size
     learning_rate = 1.0

@@ -43,6 +43,7 @@ class TorchModelBase(ModelBase):
     autocast = True
     supports_grad_accum = False    # torch autograd writes .grad: the native accumulate mode does not reach it
     supports_model_ema = False     # the library yardsticks: torch's own AveragedModel is their EMA
+    supports_sam = False           # the library yardsticks train with torch's plain optimizers
     supports_lr_schedule = False   # the library yardsticks keep the per-epoch lr policies
     supports_mixup = False         # the library yardsticks train on the plain batch
     supports_grad_clip = False     # torch.optim or the flat SGD without a clipping pass: refused rather than trained unclipped

@@ -1259,6 +1259,39 @@ def ema_swap(arena, e, table):
     L().ema_swap(arena.W.data_ptr(), e.data_ptr(), _p(arena.H), int(arena.numel), table.data_ptr(), int(table.shape[0]), _st(arena.W))
 
 
+def _sam_check(arena, p, rec):
+    assert p.dtype == torch.float32 and p.is_contiguous() and p.numel() == arena.numel and p.device == arena.W.device, (p.dtype, p.shape)
+    if rec is not None:
+        assert rec.dtype == torch.float32 and rec.is_contiguous() and rec.numel() == 4 and rec.device == arena.W.device, (rec.dtype,
+                                                                                                                         rec.shape)
+
+
+def sam_norm(arena, rho, adaptive, partial, rec):
+    """The ascent-step norm of sharpness-aware minimization (two launches, ``csrc/comm_kernels.cu: lars_partial_kernel<false>`` or
+    ``sam_partial_wg_kernel``, then ``sam_finalize_kernel``): n = ‖g‖ (``adaptive``: ‖|w|⊙g‖) over the real elements of the arena's G
+    and W, accumulated in fp64 in a fixed order, into ``rec`` (4 x fp32, ``csrc/api.h: ClipRecord``) with s = fp32(1 / (n + 1e-12))·ρ
+    and the int32 flag "n is finite" (``reference.sam_norm`` / ``sam_scale``).  ``partial`` [n_blocks] receives the per-block sums."""
+    _sam_check(arena, arena.W, rec)
+    assert partial.dtype == torch.float32 and partial.is_contiguous() and tuple(partial.shape) == (arena.n_blocks,), tuple(partial.shape)
+    L().sam_norm(arena.W.data_ptr(), arena.G.data_ptr(), arena.block_tensor.data_ptr(), arena.tensor_span.data_ptr(),
+                 int(arena.n_blocks), float(np.float32(rho)), int(bool(adaptive)), partial.data_ptr(), rec.data_ptr(), _st(arena.W))
+
+
+def sam_perturb(arena, p, rec, adaptive):
+    """The ascent step (one launch of ``csrc/comm_kernels.cu: sam_perturb_kernel``): ``p`` ← W, then, when the record ``rec`` of
+    :func:`sam_norm` is finite, W ← W + e on the real elements (e = g·s, ``adaptive``: ((w·w)·g)·s, each product and the sum rounded
+    once) and the bf16 shadow ← bf16-RN(W) (``reference.sam_perturb``)."""
+    _sam_check(arena, p, rec)
+    L().sam_perturb(arena.W.data_ptr(), arena.G.data_ptr(), p.data_ptr(), _p(arena.H), arena.block_tensor.data_ptr(),
+                    arena.tensor_span.data_ptr(), int(arena.n_blocks), int(bool(adaptive)), rec.data_ptr(), _st(arena.W))
+
+
+def sam_restore(arena, p):
+    """W ← ``p`` and the bf16 shadow ← bf16-RN(``p``) (one launch of ``csrc/comm_kernels.cu: sam_restore_kernel``)."""
+    _sam_check(arena, p, None)
+    L().sam_restore(arena.W.data_ptr(), p.data_ptr(), _p(arena.H), int(arena.n_blocks), _st(arena.W))
+
+
 def sgd_flat(arena, g, lr, mu, nesterov, inv_k, lo, hi, only_local=False, only_exchanged=False, clip=None):
     """Fused momentum-SGD over arena elements [lo, hi): ``flat_update``'s SGD rule.  ``lr`` is not used: the kernel reads
     ``arena.hyper[0]`` on the device (so a captured CUDA graph follows lr changes)."""

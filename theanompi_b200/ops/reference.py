@@ -716,6 +716,50 @@ def ema_swap(pairs, w_half=None):
         w_half.copy_(pairs[0][0])
 
 
+def sam_norm(w, g, offsets, sizes, adaptive=False):
+    """The ascent-step norm of sharpness-aware minimization over a flat fp32 arena (tensor ``i`` is ``[offsets[i], offsets[i] +
+    sizes[i])``, the padding ignored): n = ‖g‖₂, or with ``adaptive`` (ASAM) ‖|w|⊙g‖₂ with each w·g rounded once to fp32; the squares
+    are summed in fp64 and n is rounded once to fp32.  Returns n as an np.float32."""
+    sq = 0.0
+    for o, s in zip(offsets, sizes):
+        v = (w[o:o + s] * g[o:o + s] if adaptive else g[o:o + s]).double()
+        sq += float(torch.dot(v, v))
+    return np.float32(math.sqrt(sq))
+
+
+def sam_scale(n, rho):
+    """(s, finite) for the norm ``n`` (an fp32 value): s = rho / (n + 1e-12) as torch evaluates it on an fp32 tensor,
+    fp32(1 / fp32(n + 1e-12)) · fp32(rho) (``Tensor.__rtruediv__`` is ``reciprocal() * other``); finite is False, and s = 0, when n is
+    NaN or Inf."""
+    n = torch.tensor(float(n), dtype=torch.float32)
+    if not bool(torch.isfinite(n)):
+        return 0.0, False
+    return float(rho / (n + 1e-12)), True
+
+
+def sam_perturb(w, g, p, s, finite, offsets, sizes, adaptive=False, w_half=None):
+    """The ascent step of SAM over a flat fp32 arena laid out as in :func:`sam_norm`: ``p`` ← w; when ``finite``, w ← w + e on the real
+    elements with e = g·s (``adaptive``: ((w·w)·g)·s), each product and the sum rounded once to fp32 (torch's ``p.add_(e_w)`` of the
+    SAM wrapper), and ``w_half`` (the bf16 shadow, or None) ← bf16(w).  A non-finite norm leaves w as it is."""
+    p.copy_(w)
+    if not finite:
+        return
+    st = torch.tensor(float(s), dtype=torch.float32)
+    for o, n in zip(offsets, sizes):
+        wv, gv = w[o:o + n], g[o:o + n]
+        e = (wv * wv * gv if adaptive else gv) * st
+        wv.add_(e)
+    if w_half is not None:
+        w_half.copy_(w)
+
+
+def sam_restore(w, p, w_half=None):
+    """The end of a SAM step: w ← ``p`` and ``w_half`` (the bf16 shadow, or None) ← bf16(p)."""
+    w.copy_(p)
+    if w_half is not None:
+        w_half.copy_(p)
+
+
 # --------------------------------------------------------------------------- data aug
 def crop_mirror_normalize(x_u8, mean, std_scale, crop_hw, offsets, flips, out_dtype=torch.float32, zero_fill=False):
     """``(x - mean) * std_scale`` → crop at per-image ``offsets`` → optional

@@ -297,6 +297,78 @@ class ModelEma(object):
         self.state.copy_(torch.tensor([int(sd["u"]), int(sd["n_averaged"]), 0]))
 
 
+class Sam(object):
+    """Sharpness-aware minimization (``config['sam']``, a dict; Foret et al., 2021) and its adaptive variant ASAM (Kwon et al., 2021),
+    with the semantics of the standard PyTorch SAM wrapper (davda54/sam, the version that keeps ``old_p``).  After the step's first
+    forward and backward at w, :meth:`perturb` computes n = ‖g‖₂ (ASAM: ‖|w|⊙g‖₂) over the real elements of every arena tensor and
+    s = ρ / (n + 1e-12), saves w into P and moves the weights to w + e, e = g·s (ASAM: w²·g·s); the model then runs the second forward
+    and backward there, and :meth:`restore` puts w back before the optimizer steps on the second gradient.
+
+    Keys: ``rho`` ρ > 0 (0.05; ASAM's papers use about 0.5 to 2), ``adaptive`` (False).
+
+    On CUDA :meth:`perturb` is three launches and :meth:`restore` one (``cuda_impl.sam_norm``, ``sam_perturb``, ``sam_restore``), all
+    reading only device memory: they run inside the captured step.  The record {n, s, finite} (``csrc/api.h: ClipRecord``) stays on the
+    device.  When n is NaN or Inf the weights are not moved, so the second pass runs at w; the wrapper would write NaN into every
+    weight instead.  P costs 4 bytes per arena element and exists only with the key."""
+
+    KEY = "sam"
+    KEYS = ("rho", "adaptive")
+
+    def __init__(self, arena, cfg):
+        cfg = self.check_config(cfg)
+        self.rho, self.adaptive = cfg["rho"], cfg["adaptive"]
+        self.arena = arena
+        dev = arena.W.device
+        self.P = torch.zeros_like(arena.W)
+        self.rec = torch.zeros(4, dtype=torch.float32, device=dev)          # csrc/api.h: ClipRecord {n, s, finite, pad}
+        self._partial = torch.zeros(arena.n_blocks, dtype=torch.float32, device=dev) if arena.W.is_cuda else None
+
+    @classmethod
+    def check_config(cls, cfg):
+        """The validated dict {rho, adaptive}; anything else is a ValueError that names ``sam``."""
+        k = cls.KEY
+        if not isinstance(cfg, dict):
+            raise ValueError("%s must be a dict or None, not %r" % (k, cfg))
+        unknown = sorted(set(cfg) - set(cls.KEYS))
+        if unknown:
+            raise ValueError("%s: unknown key %r; the keys are %s" % (k, unknown[0], ", ".join(cls.KEYS)))
+        rho = cfg.get("rho", 0.05)
+        if isinstance(rho, bool) or not isinstance(rho, (int, float, np.integer, np.floating)) or not np.isfinite(rho) or not rho > 0:
+            raise ValueError("%s['rho'] must be a finite real number > 0, not %r" % (k, rho))
+        adaptive = cfg.get("adaptive", False)
+        if not isinstance(adaptive, (bool, np.bool_)):
+            raise ValueError("%s['adaptive'] must be a bool, not %r" % (k, adaptive))
+        return {"rho": float(rho), "adaptive": bool(adaptive)}
+
+    @property
+    def norm(self):
+        """n of the last :meth:`perturb` (a device scalar): NaN or Inf when the weights were not moved."""
+        return self.rec[0]
+
+    def perturb(self):
+        """P ← W, then W ← W + e and the bf16 shadow ← bf16(W), from the gradient of the first pass in the arena's G region."""
+        a = self.arena
+        if a.W.is_cuda:
+            from ..ops import cuda_impl
+            cuda_impl.sam_norm(a, self.rho, self.adaptive, self._partial, self.rec)
+            cuda_impl.sam_perturb(a, self.P, self.rec, self.adaptive)
+            return
+        n = ref.sam_norm(a.W, a.G, a.offsets, a.sizes, self.adaptive)
+        s, finite = ref.sam_scale(n, self.rho)
+        self.rec[0], self.rec[1] = float(n), s
+        self.rec[2:3].view(torch.int32).fill_(int(finite))
+        ref.sam_perturb(a.W, a.G, self.P, s, finite, a.offsets, a.sizes, self.adaptive, w_half=a.H)
+
+    def restore(self):
+        """W ← P and the bf16 shadow ← bf16(P): the weights before :meth:`perturb`, bit for bit."""
+        a = self.arena
+        if a.W.is_cuda:
+            from ..ops import cuda_impl
+            cuda_impl.sam_restore(a, self.P)
+            return
+        ref.sam_restore(a.W, self.P, w_half=a.H)
+
+
 def _fc_fusable(p, block):
     """Can ``p``'s weight gradient be consumed by the SGD epilogue of its wgrad GEMM?  It must come from ONE fp32 GEMM straight
     into ``gbuf`` (native FC / Softmax weights, ``rs_ok``), not be accumulated over several passes, and its shape must take the
@@ -436,7 +508,8 @@ class FlatSGD(FlatOptimizer):
     (``cuda_impl.gemm_sgd``): their fp32 gradient is never written, and ``step(lr, 1)`` updates only the rest of the arena.  With
     gradient clipping (:meth:`FlatOptimizer.set_grad_clip`) nothing is armed: an epilogue would update its weight before the
     global norm exists.  Nor with gradient accumulation (``model.grad_accum`` > 1): the epilogue would update the weight on every
-    micro-step.  The clipping factor is folded into inv_k."""
+    micro-step.  Nor with sharpness-aware minimization (``model.sam_opt``): the first backward of the step would update the weight
+    before the ascent step.  The clipping factor is folded into inv_k."""
 
     rule = "sgd"
 
@@ -456,7 +529,7 @@ class FlatSGD(FlatOptimizer):
             p.sgd_epilogue = None
         self.armed, self.rest = [], None
         if (not enable or not a.W.is_cuda or getattr(model, "monitor_grad", False) or self.max_norm is not None
-                or getattr(model, "grad_accum", 1) > 1):
+                or getattr(model, "grad_accum", 1) > 1 or getattr(model, "sam_opt", None) is not None):
             return
         dt = getattr(model, "act_dtype", None)
         block = 16 // torch.empty((), dtype=dt).element_size() if dt is not None else 8
