@@ -134,6 +134,11 @@ void mix_batch(void* x, const void* rec, int B, int H, int W, int C, int f32, cu
 // else y_j
 void softmax_xent_mix(const void* logits, const void* labels, const void* rec, void* dlogits, void* rowstat, void* out3, int B, int C,
                       float weight, float grad_weight, float label_smoothing, int f32, cudaStream_t st);
+// knowledge distillation: out3 = {mean L, top-1 error, top-5 error} with L = (1 − α)·CE_q(z) + α·T²·KL(softmax(t/T) ‖ softmax(z/T)) per row,
+// dlogits = [(1 − α)·(softmax(z) − q) + α·T·(softmax(z/T) − softmax(t/T))] · grad_weight / B; q is the target of softmax_xent
+// (label_smoothing ε) or, with a mix record rec (nullptr: none), of softmax_xent_mix.  teacher: the teacher's logits, in the same dtype
+void softmax_xent_kd(const void* logits, const void* teacher, const void* labels, const void* rec, void* dlogits, void* rowstat, void* out3,
+                     int B, int C, float grad_weight, float label_smoothing, float alpha, float temperature, int f32, cudaStream_t st);
 // drop-path table (ops/drop_path.py owns the layout): out[l·B + n] = 0 when block l drops sample n at step counter *step, else
 // keep_scale[l] = fp32(1 / (1 − p_l)); thresh[l] = ⌈p_l·2^24⌉ (uint32), key (seed, rank)
 void drop_path_draw(const void* thresh, const void* keep_scale, int L, int B, unsigned long long seed, int rank, const void* step, void* out,

@@ -110,6 +110,10 @@ PYBIND11_MODULE(_tmpi_native, m) {
   m.def("softmax_xent_mix", [](ptr_t logits, ptr_t labels, ptr_t rec, ptr_t dlogits, ptr_t rowstat, ptr_t out3, int B, int C, float weight,
                                float grad_weight, float label_smoothing, int f32, ptr_t st) {
     softmax_xent_mix(P(logits), P(labels), P(rec), P(dlogits), P(rowstat), P(out3), B, C, weight, grad_weight, label_smoothing, f32, S(st)); });
+  m.def("softmax_xent_kd", [](ptr_t logits, ptr_t teacher, ptr_t labels, ptr_t rec, ptr_t dlogits, ptr_t rowstat, ptr_t out3, int B, int C,
+                              float grad_weight, float label_smoothing, float alpha, float temperature, int f32, ptr_t st) {
+    softmax_xent_kd(P(logits), P(teacher), P(labels), P(rec), P(dlogits), P(rowstat), P(out3), B, C, grad_weight, label_smoothing, alpha,
+                    temperature, f32, S(st)); });
   m.def("maxpool_relu_bias_bwd", [](ptr_t dyp, ptr_t arg, ptr_t y, ptr_t dym, ptr_t db0, ptr_t db1, int c_split, int N, int H, int W, int C,
                                     int Ho, int Wo, int k, int s, int p, int accumulate, ptr_t st) {
     maxpool_relu_bias_bwd(P(dyp), P(arg), P(y), P(dym), P(db0), P(db1), c_split, N, H, W, C, Ho, Wo, k, s, p, accumulate, S(st)); });

@@ -1017,6 +1017,94 @@ void softmax_xent_mix(const void* logits, const void* labels, const void* rec, v
   count_launch(); TMPI_CHECK_LAUNCH("rowstat_mean"); ::tmpi::check_capture(st, "rowstat_mean");
 }
 
+// Knowledge distillation: the student's logits z against the hard target q (one-hot, smoothed, or the mixed target of rec when kMix)
+// and the teacher's logits t of the same batch at temperature T.  One CTA per row, three passes over it as softmax_xent_kernel:
+//   1. m = max z, m_t = max t (max z/T = m/T since T > 0);
+//   2. se = Σ e^(z−m), sT = Σ e^((z−m)/T), st = Σ e_t with e_t = e^((t−m_t)/T), sd = Σ e_t·((t−m_t) − (z−m)), sz = Σ (z−m), the rank;
+//   3. dlogits = scale·[(1 − α)·(p − q) + α·T·(softmax(z/T) − softmax(t/T))].
+// KL(softmax(t/T) ‖ softmax(z/T)) = sd / (T·st) − log st + log sT in closed form, so
+//   rowstat[3b] = (1 − α)·(log se − on·(λ·(z_i − m) + (1 − λ)·(z_j − m)) − off·sz) + α·T²·KL,
+// and err1 / err5 rank the student's logit of the label with the larger weight (y_i when λ ≥ ½, else y_j).
+template <typename T, bool kMix>
+__global__ void __launch_bounds__(256) softmax_xent_kd_kernel(const T* __restrict__ logits, const T* __restrict__ teacher,
+                                                              const long long* __restrict__ labels, const MixRecord* __restrict__ rec,
+                                                              T* __restrict__ dlogits, float* __restrict__ rowstat, int C, float scale,
+                                                              float on, float off, float alpha, float temp) {
+  const int b = blockIdx.x;
+  const T* row = logits + (long long)b * C;
+  const T* trow = teacher + (long long)b * C;
+  const int yi = (int)labels[b];
+  const int yj = kMix ? (int)labels[gridDim.x - 1 - b] : yi;
+  const float lam = (kMix && rec->mode != MIX_NONE) ? rec->lam : 1.f, oml = 1.f - lam;
+  const int label = lam >= 0.5f ? yi : yj;                      // the errors' label
+  __shared__ float red[6][32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  float mx = -INFINITY, mt = -INFINITY;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) { mx = fmaxf(mx, to_f(row[c])); mt = fmaxf(mt, to_f(trow[c])); }
+  mx = warp_max(mx); mt = warp_max(mt);
+  if (lane == 0) { red[0][warp] = mx; red[1][warp] = mt; }
+  __syncthreads();
+  mx = red[0][0]; mt = red[1][0];
+  for (int w = 1; w < nw; ++w) { mx = fmaxf(mx, red[0][w]); mt = fmaxf(mt, red[1][w]); }
+  __syncthreads();
+  const float invT = 1.f / temp;
+  const float lab = to_f(row[label]);
+  float se = 0.f, sT = 0.f, st = 0.f, sd = 0.f, sz = 0.f, gt = 0.f;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    const float zc = to_f(row[c]), v = zc - mx, u = to_f(trow[c]) - mt;
+    const float et = __expf(u * invT);
+    se += __expf(v);
+    sT += __expf(v * invT);
+    st += et;
+    sd += et * (u - v);
+    sz += v;
+    gt += (zc > lab || (zc == lab && c < label)) ? 1.f : 0.f;     // rank of the errors' label's logit
+  }
+  se = warp_sum(se); sT = warp_sum(sT); st = warp_sum(st); sd = warp_sum(sd); sz = warp_sum(sz); gt = warp_sum(gt);
+  if (lane == 0) { red[0][warp] = se; red[1][warp] = sT; red[2][warp] = st; red[3][warp] = sd; red[4][warp] = sz; red[5][warp] = gt; }
+  __syncthreads();
+  se = red[0][0]; sT = red[1][0]; st = red[2][0]; sd = red[3][0]; sz = red[4][0]; gt = red[5][0];
+  for (int w = 1; w < nw; ++w) { se += red[0][w]; sT += red[1][w]; st += red[2][w]; sd += red[3][w]; sz += red[4][w]; gt += red[5][w]; }
+  const float hw = 1.f - alpha, sw = alpha * temp;              // weights of (p − q) and of (softmax(z/T) − softmax(t/T))
+  const float inv = 1.f / se, invsT = 1.f / sT, invst = 1.f / st;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    const float v = to_f(row[c]) - mx;
+    float pq = __expf(v) * inv - off;
+    if (c == yi) pq -= on * lam;
+    if (kMix && c == yj) pq -= on * oml;
+    const float kd = __expf(v * invT) * invsT - __expf((to_f(trow[c]) - mt) * invT) * invst;
+    dlogits[(long long)b * C + c] = from_f<T>((hw * pq + sw * kd) * scale);
+  }
+  if (threadIdx.x == 0) {
+    const float hard = __logf(se) - on * (lam * (to_f(row[yi]) - mx) + oml * (to_f(row[yj]) - mx)) - off * sz;
+    const float kl = sd * invT * invst - __logf(st) + __logf(sT);
+    rowstat[3 * b + 0] = hw * hard + sw * temp * kl;
+    rowstat[3 * b + 1] = gt >= 1.f ? 1.f : 0.f;
+    rowstat[3 * b + 2] = gt >= 5.f ? 1.f : 0.f;
+  }
+}
+
+void softmax_xent_kd(const void* logits, const void* teacher, const void* labels, const void* rec, void* dlogits, void* rowstat, void* out3,
+                     int B, int C, float grad_weight, float label_smoothing, float alpha, float temperature, int f32, cudaStream_t st) {
+  if (!(label_smoothing >= 0.f && label_smoothing <= 1.f)) throw std::runtime_error("softmax_xent_kd: label_smoothing must be in [0, 1]");
+  if (!(alpha > 0.f && alpha <= 1.f)) throw std::runtime_error("softmax_xent_kd: alpha must be in (0, 1]");
+  if (!(temperature > 0.f && temperature <= 3.4e38f)) throw std::runtime_error("softmax_xent_kd: temperature must be finite and > 0");
+  auto LB = (const long long*)labels; auto RS = (float*)rowstat; auto R = (const MixRecord*)rec;
+  const float scale = grad_weight / (float)B;
+  const float on = 1.f - label_smoothing, off = label_smoothing / (float)C;
+  if (f32) {
+    auto k = rec ? softmax_xent_kd_kernel<float, true> : softmax_xent_kd_kernel<float, false>;
+    k<<<B, 256, 0, st>>>((const float*)logits, (const float*)teacher, LB, R, (float*)dlogits, RS, C, scale, on, off, alpha, temperature);
+  } else {
+    auto k = rec ? softmax_xent_kd_kernel<__nv_bfloat16, true> : softmax_xent_kd_kernel<__nv_bfloat16, false>;
+    k<<<B, 256, 0, st>>>((const __nv_bfloat16*)logits, (const __nv_bfloat16*)teacher, LB, R, (__nv_bfloat16*)dlogits, RS, C, scale, on,
+                         off, alpha, temperature);
+  }
+  count_launch(); TMPI_CHECK_LAUNCH("softmax_xent_kd"); ::tmpi::check_capture(st, "softmax_xent_kd");
+  rowstat_mean_kernel<<<1, 256, 0, st>>>((const float*)rowstat, (float*)out3, B, 1.f);
+  count_launch(); TMPI_CHECK_LAUNCH("rowstat_mean"); ::tmpi::check_capture(st, "rowstat_mean");
+}
+
 // ============================================================================ activation mask + bias gradient
 // dym = act'(y) * dy (contiguous [R, C]; ReLU: dy * (y > 0));  db[c] += sum_r dym[r, c]   (db pre-zeroed by the launcher, unless it
 // accumulates a gradient over several micro-batches)

@@ -40,6 +40,7 @@ seed_weight_on_pid = False
 
 class AlexNet(ModelBase):
     supports_resized_crop = True
+    supports_distill = True
     n_epochs, momentum, weight_decay = n_epochs, momentum, weight_decay
     batch_size, file_batch_size, learning_rate = batch_size, file_batch_size, learning_rate
     lr_policy, lr_step = lr_policy, lr_step

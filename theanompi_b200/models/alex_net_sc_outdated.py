@@ -12,6 +12,7 @@ class AlexNet_sc(AlexNet):
     supports_model_ema = False    # the outdated variant: the average is offered on the loader-fed AlexNet
     supports_sam = False          # its in-graph Crop draws new crops at every forward: a second forward would see another crop
     supports_resized_crop = False  # its crop is the in-graph Crop layer, not the loader's
+    supports_distill = False       # its in-graph Crop: the teacher would see the uncropped batch
     def __init__(self, config):
         config = dict(config)
         config["no_paraload"] = True

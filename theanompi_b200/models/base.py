@@ -75,6 +75,8 @@ class ModelBase(object):
     supports_model_ema = True      # config['model_ema'] (False: no single arena updated by the step tail; refused at compile_iter_fns)
     # config['sam'] (False: the step cannot run its training forward twice on the same draws; refused at compile_iter_fns)
     supports_sam = True
+    # config['distill'] (True: a native ImageNet classifier whose teacher can be one of the five in ops/distill.py; refused otherwise)
+    supports_distill = False
     # True: an ImageNet model fed by ParaLoader, so config['random_resized_crop'], config['color_jitter'] and
     # config['random_erasing'] reach its loader
     # (refused at construction otherwise)
@@ -135,6 +137,10 @@ class ModelBase(object):
         # on, and the weights are restored before it.  Built by check_sam
         self.sam = config.get("sam")
         self.sam_opt = None
+        # knowledge distillation from a frozen teacher (a dict, ops/distill.py; None = off): every training step the teacher's eval forward
+        # on x_in, after the draws and the mix, gives the loss its soft target.  Built by check_distill
+        self.distill = config.get("distill")
+        self.distiller = None
         # label smoothing ε of the training loss (cross-entropy against (1 − ε)·onehot + ε / C; 0 = plain NLL); validation stays
         # plain NLL.  Checked by check_label_smoothing at compile_iter_fns
         self.label_smoothing = config.get("label_smoothing", 0.0)
@@ -236,13 +242,14 @@ class ModelBase(object):
         """Return logits-layer output; must leave ``self.output_layer`` evaluated."""
         raise NotImplementedError
 
-    def loss(self, x, y, label_smoothing=0.0, mix=None):
+    def loss(self, x, y, label_smoothing=0.0, mix=None, kd=None):
         """(cost, top-1 error, top-5 error); the cost is the mean NLL, or with ``label_smoothing`` ε > 0 the cross-entropy against
         (1 − ε)·onehot + ε / C.  ``mix``: the step's Mixup / CutMix record; the cost is then the cross-entropy against its mixed
-        target and the errors count against the label with the larger weight."""
+        target and the errors count against the label with the larger weight.  ``kd``: the step's distillation target
+        (ops/distill.py: KdTarget); the cost is then (1 − α)·that cross-entropy + α·T²·KL(teacher ‖ student) at temperature T."""
         self.forward(x)
         sm = self.output_layer
-        return sm.negative_log_likelihood(y, label_smoothing, mix), sm.errors(y), sm.errors_top_x(y)
+        return sm.negative_log_likelihood(y, label_smoothing, mix, kd), sm.errors(y), sm.errors_top_x(y)
 
     # ------------------------------------------------------------------ step functions
     def _fwd_bwd_eager(self):
@@ -253,6 +260,7 @@ class ModelBase(object):
         # with config['cifar_augment'] the offsets, flips and Cutout boxes are drawn last, from the same counter, and likewise only this
         # forward reads them
         # with config['sam'] the second pass at the ascent point reuses every draw: the step counter only advances in _after_step
+        # with config['distill'] the teacher's forward runs last, on the mixed batch, once per step: SAM's second pass reuses its logits
         rec = None
         if self.mixer is not None:
             rec = self.mixer.draw()
@@ -261,30 +269,36 @@ class ModelBase(object):
             self.drop_path.draw()
         if self.cifar_aug is not None:
             self.cifar_aug.draw()
-        out = self._train_pass(rec)
+        kd = {}
+        if self.distiller is not None:
+            kd["kd"] = self.distiller.target(self.x_in)
+            self._dbg_capture("teacher forward")
+        out = self._train_pass(rec, **kd)
         if self.sam_opt is not None:
             with torch.no_grad():
                 self.sam_opt.perturb()
             if rec is not None:
                 self.repeat_mix(rec)
             with self.bn_stats_frozen():
-                self._train_pass(rec)
+                self._train_pass(rec, **kd)
             with torch.no_grad():
                 self.sam_opt.restore()
             self._dbg_capture("sam")
         return out
 
-    def _train_pass(self, rec):
+    def _train_pass(self, rec, kd=None):
         """Forward and backward of the training step on x_in with the draws of this step already made: the drop-path table and the
         cifar_augment draw are read by the forward, ``rec`` (the Mixup / CutMix record, or None) gives the mixed target, and the
-        batch is mixed at the mix point as :meth:`mix_input` left it.  The gradient is stored in the arena's G region."""
+        batch is mixed at the mix point as :meth:`mix_input` left it.  ``kd`` (config['distill']: the teacher's target of this step,
+        or None) makes the loss the distillation loss.  The gradient is stored in the arena's G region."""
         self._drop_on = self.drop_path is not None
         self._aug_on = self.cifar_aug is not None
+        kw = {} if kd is None else {"kd": kd}
         try:
             if rec is None:
-                cost, err, err5 = self.loss(self.x_in, self.y_in, self.label_smoothing)
+                cost, err, err5 = self.loss(self.x_in, self.y_in, self.label_smoothing, **kw)
             else:
-                cost, err, err5 = self.loss(self.x_in, self.y_in, self.label_smoothing, mix=rec)
+                cost, err, err5 = self.loss(self.x_in, self.y_in, self.label_smoothing, mix=rec, **kw)
         finally:
             self._drop_on = False
             self._aug_on = False
@@ -727,8 +741,8 @@ class ModelBase(object):
     def setup_train_options(self, k=1, fused_tail=None, optimizer=None):
         """Check and build the training options of the config for a step of ``k`` workers (k > 1: BSP ``sync_type='cdd'``),
         ``fused_tail`` (a fused exchange strategy's step tail, or None) and ``optimizer`` (default: the model's): grad_accum,
-        label_smoothing, mixup, cifar_augment, drop_path_rate, lr_schedule, grad_clip, model_ema and sam.  A model refuses every option it
-        does not support here, with a ValueError that names it."""
+        label_smoothing, mixup, cifar_augment, drop_path_rate, lr_schedule, grad_clip, model_ema, sam and distill.  A model refuses every
+        option it does not support here, with a ValueError that names it."""
         self.check_grad_accum(fused_tail)
         self.check_label_smoothing()
         self.check_mixup()
@@ -743,6 +757,23 @@ class ModelBase(object):
         self.check_grad_clip(k, fused_tail, opt)
         self.check_model_ema(k, fused_tail)
         self.check_sam(fused_tail)
+        self.check_distill()
+
+    def check_distill(self):
+        """``config['distill']`` must be None or a valid dict (ops/distill.py: check_config; a ValueError names the key), on a model that
+        supports it (``supports_distill``).  Builds the teacher (:class:`ops.distill.Distill`) from its class and checkpoint, after this
+        model is finalised: a teacher class, input or class count that does not fit, or a checkpoint that is missing or does not match the
+        teacher's layout, is a ValueError that names the key.  The key changes only the loss of the training step, so every optimizer,
+        training option and exchange strategy runs with it."""
+        self.distiller = None
+        if self.distill is None:
+            return
+        from ..ops.distill import KEY, Distill, check_config
+        cfg = check_config(self.distill)
+        if not self.supports_distill:
+            raise ValueError("%s: %s is not supported; the students and teachers are the native ImageNet classifiers AlexNet, GoogLeNet, "
+                             "VGG16, ResNet50 and ResNet152" % (self.name, KEY))
+        self.distiller = Distill(self, cfg)
 
     def check_sam(self, fused_tail=None):
         """``config['sam']`` must be None or a valid dict (utils/opt.py: Sam.check_config; a ValueError names the key).  A dict needs a

@@ -105,6 +105,7 @@ class Aux_tower(Layer):
 
 class GoogLeNet(ModelBase):
     supports_resized_crop = True
+    supports_distill = True
     n_epochs, momentum, weight_decay = n_epochs, momentum, weight_decay
     batch_size, file_batch_size, learning_rate = batch_size, file_batch_size, learning_rate
     lr_policy = lr_policy
@@ -181,10 +182,11 @@ class GoogLeNet(ModelBase):
         self._taps = taps
         return x
 
-    def loss(self, x, y, label_smoothing=0.0, mix=None):
+    def loss(self, x, y, label_smoothing=0.0, mix=None, kd=None):
+        # config['distill'] (kd): only the main head distils; the auxiliary towers keep their hard loss
         self.forward(x)
         sm = self.output_layer
-        cost = sm.negative_log_likelihood(y, label_smoothing, mix)
+        cost = sm.negative_log_likelihood(y, label_smoothing, mix, kd)
         if Dropout.layers and Dropout.layers[0].flag_on:          # aux towers only contribute while training
             self.aux1.forward(self._taps[id(self._tap1)])
             self.aux2.forward(self._taps[id(self._tap2)])

@@ -68,6 +68,7 @@ class ResNet50Net(nn.Module):
 class ResNet50(ModelBase):
     supports_drop_path = True      # one drop-path block per bottleneck
     supports_resized_crop = True
+    supports_distill = True
     n_epochs, momentum, weight_decay = n_epochs, momentum, weight_decay
     batch_size, file_batch_size, learning_rate = batch_size, file_batch_size, learning_rate
     lr_policy, lr_step = lr_policy, lr_step

@@ -594,14 +594,18 @@ class Softmax(Layer):
         self._cache = None
         return self.logits
 
-    def _eval(self, y, label_smoothing=None, mix=None):
-        """(y, ε, mix, loss, err1, err5) of one launch on this forward's logits, cached per (y, ε, mix record); ``label_smoothing``
-        None takes the cached launch whatever its ε and mix (the errors of a training step are those of its loss launch), else
-        ε = 0 and no mix."""
+    def _eval(self, y, label_smoothing=None, mix=None, kd=None):
+        """(y, ε, mix, kd, loss, err1, err5) of one launch on this forward's logits, cached per (y, ε, mix record, kd);
+        ``label_smoothing`` None takes the cached launch whatever its ε, mix and kd (the errors of a training step are those of its
+        loss launch), else ε = 0, no mix and no distillation."""
         c = self._cache
-        if c is None or c[0] is not y or (label_smoothing is not None and (c[1] != label_smoothing or c[2] is not mix)):
+        if c is None or c[0] is not y or (label_smoothing is not None and (c[1] != label_smoothing or c[2] is not mix or c[3] is not kd)):
             eps = label_smoothing or 0.0
-            self._cache = (y, eps, mix) + tuple(ops.softmax_xent(self.logits, y, eps, mix))
+            if kd is None:
+                out = ops.softmax_xent(self.logits, y, eps, mix)
+            else:
+                out = ops.softmax_xent_kd(self.logits, y, kd.logits, kd.alpha, kd.temperature, eps, mix)
+            self._cache = (y, eps, mix, kd) + tuple(out)
         return self._cache
 
     @property
@@ -612,20 +616,21 @@ class Softmax(Layer):
     def y_pred(self):
         return self.logits.argmax(1)
 
-    def negative_log_likelihood(self, y, label_smoothing=0.0, mix=None):
+    def negative_log_likelihood(self, y, label_smoothing=0.0, mix=None, kd=None):
         """Mean NLL of ``y``; ``label_smoothing`` ε > 0 gives the cross-entropy against (1 − ε)·onehot + ε / C instead, and a Mixup /
-        CutMix record ``mix`` the cross-entropy against its mixed target (ops/mixup.py)."""
-        return self._eval(y, label_smoothing, mix)[3]
+        CutMix record ``mix`` the cross-entropy against its mixed target (ops/mixup.py).  ``kd`` (ops/distill.py: a teacher's logits
+        with α and T) makes it the distillation loss (1 − α)·CE + α·T²·KL of ops.softmax_xent_kd."""
+        return self._eval(y, label_smoothing, mix, kd)[4]
 
     def errors(self, y):
-        return self._eval(y)[4]
+        return self._eval(y)[5]
 
     def errors_top_x(self, y, num_top=5):
         if num_top != 5:
             lg = self.logits.float()
             topk = lg.topk(num_top, dim=1).indices
             return 1.0 - (topk == y[:, None]).any(1).float().mean()
-        return self._eval(y)[5]
+        return self._eval(y)[6]
 
 
 # =========================================================================== graph helpers

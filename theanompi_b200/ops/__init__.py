@@ -9,10 +9,10 @@ from . import accum, cifar_augment, drop_path, mixup, native, reference
 from .functional import (add, advance_rng_step, batch_norm, compute_weight, conv2d_bias_act,
                          conv2d_group2_bias_act, crop_mirror_normalize, dropout, fork2,
                          linear_bias_act, lrn, mix_batch, mix_draw, pool2d, random_erase, resized_crop_mirror_normalize,
-                         rng_state, seed_dropout, softmax_xent)
+                         rng_state, seed_dropout, softmax_xent, softmax_xent_kd)
 
 __all__ = [
     "accum", "cifar_augment", "drop_path", "mixup", "native", "reference", "conv2d_bias_act", "conv2d_group2_bias_act", "linear_bias_act",
-    "pool2d", "lrn", "dropout", "softmax_xent", "crop_mirror_normalize", "resized_crop_mirror_normalize", "compute_weight",
+    "pool2d", "lrn", "dropout", "softmax_xent", "softmax_xent_kd", "crop_mirror_normalize", "resized_crop_mirror_normalize", "compute_weight",
     "seed_dropout", "advance_rng_step", "rng_state", "batch_norm", "add", "fork2", "mix_draw", "mix_batch", "random_erase",
 ]

@@ -684,6 +684,30 @@ def softmax_xent(logits, labels, weight=1.0, grad_scale=1.0, label_smoothing=0.0
     return out3[0], out3[1], out3[2], dl
 
 
+def softmax_xent_kd(logits, labels, teacher, alpha, temperature, grad_scale=1.0, label_smoothing=0.0, mix=None):
+    """Knowledge distillation against the teacher's logits ``teacher`` (same shape and dtype as ``logits``): (mean L, top-1 error,
+    top-5 error, dlogits) with L = (1 − α)·CE_q(z) + α·T²·KL(softmax(t/T) ‖ softmax(z/T)) per row, q the target of :func:`softmax_xent`
+    (``label_smoothing`` ε, ``mix``), and dlogits = [(1 − α)·(p − q) + α·T·(softmax(z/T) − softmax(t/T))] / B times ``grad_scale``,
+    scaled in fp32 inside the kernel.  One ``softmax_xent_kd`` launch and one ``rowstat_mean`` (reference.softmax_xent_kd)."""
+    lg = _bf(logits).contiguous()
+    t = _bf(teacher).contiguous()
+    B_, C = lg.shape
+    if t.shape != lg.shape or t.dtype != lg.dtype:
+        raise ValueError("softmax_xent_kd: the teacher's logits %s %s do not match the student's %s %s"
+                         % (tuple(t.shape), t.dtype, tuple(lg.shape), lg.dtype))
+    labels = labels.contiguous()
+    assert labels.dtype == torch.int64
+    dl = torch.empty_like(lg)
+    rowstat = torch.empty((B_, 3), dtype=torch.float32, device=lg.device)
+    out3 = torch.empty(3, dtype=torch.float32, device=lg.device)
+    if mix is not None:
+        _check_record(mix, lg.device)
+    L().softmax_xent_kd(lg.data_ptr(), t.data_ptr(), labels.data_ptr(), 0 if mix is None else mix.data_ptr(), dl.data_ptr(),
+                        rowstat.data_ptr(), out3.data_ptr(), B_, C, float(grad_scale), float(label_smoothing), float(alpha),
+                        float(temperature), int(_is32(lg)), _st(lg))
+    return out3[0], out3[1], out3[2], dl
+
+
 def _check_record(rec, device):
     from .mixup import RECORD_BYTES
     if not (rec.is_cuda and rec.device == device and rec.dtype == torch.uint8 and rec.is_contiguous() and rec.numel() % RECORD_BYTES == 0

@@ -512,6 +512,30 @@ def softmax_xent(logits, labels, label_smoothing=0.0, mix=None):
     return _SoftmaxXentFn.apply(logits, labels, float(label_smoothing), mix)
 
 
+class _SoftmaxXentKdFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, logits, labels, teacher, alpha, temperature, label_smoothing, mix):
+        # the teacher's logits carry no gradient; under gradient accumulation dlogits carries 1/n, as in _SoftmaxXentFn
+        loss, err1, err5, dlogits = _impl(logits).softmax_xent_kd(logits, labels, teacher, alpha, temperature,
+                                                                  grad_scale=accum.grad_scale(), label_smoothing=label_smoothing, mix=mix)
+        ctx.save_for_backward(dlogits)
+        ctx.in_dtype = logits.dtype
+        ctx.mark_non_differentiable(err1, err5)
+        return loss, err1, err5
+
+    @staticmethod
+    def backward(ctx, gl, g1, g5):
+        (dlogits,) = ctx.saved_tensors
+        return (dlogits * gl.to(dlogits.dtype)).to(ctx.in_dtype), None, None, None, None, None, None
+
+
+def softmax_xent_kd(logits, labels, teacher, alpha, temperature, label_smoothing=0.0, mix=None):
+    """Returns (mean L, top-1 error, top-5 error) of knowledge distillation, fused on CUDA: L = (1 − α)·CE_q(z) +
+    α·T²·KL(softmax(t/T) ‖ softmax(z/T)) per row, with ``teacher`` the teacher's logits t of the same batch (no gradient) and q the
+    target :func:`softmax_xent` takes with ``label_smoothing`` and ``mix``.  The errors are the student's."""
+    return _SoftmaxXentKdFn.apply(logits, labels, teacher.detach(), float(alpha), float(temperature), float(label_smoothing), mix)
+
+
 def mix_draw(cfg, rank, hw, out):
     """This step's Mixup / CutMix record (``cfg`` a validated ``config['mixup']``, ``hw`` the image size at the mix point) into
     ``out``, a uint8 tensor of ops/mixup.py's 64 bytes: on CUDA drawn by the kernel from the device step counter, on the CPU by

@@ -231,6 +231,33 @@ def softmax_xent_mix(logits, labels, mix, grad_scale=1.0, weight=1.0, label_smoo
     return loss * weight, err1, err5, dlogits
 
 
+def softmax_xent_kd(logits, labels, teacher, alpha, temperature, grad_scale=1.0, label_smoothing=0.0, mix=None):
+    """Knowledge distillation (Hinton et al. 2015) of the student's logits z against the teacher's logits t of the same batch: per row
+    L = (1 − α)·CE_q(z) + α·T²·KL(softmax(t/T) ‖ softmax(z/T)), q the target of :func:`softmax_xent` (``label_smoothing`` ε; with
+    ``mix`` that of :func:`softmax_xent_mix`), the teacher's distribution never smoothed.  Returns (mean L, top-1 error, top-5 error,
+    dlogits) with dlogits = [(1 − α)·(p − q) + α·T·(softmax(z/T) − softmax(t/T))] / B times ``grad_scale``; the errors are the student's,
+    ranked as :func:`softmax_xent_mix` ranks them.  Computed in fp64 when the logits are fp64, else in fp32."""
+    dt = torch.float64 if logits.dtype == torch.float64 else torch.float32
+    z, t = logits.to(dt), teacher.to(dt)
+    B, C = z.shape
+    lam = 1.0 if mix is None else mix_lambda(mix)
+    eps, a, T = float(label_smoothing), float(alpha), float(temperature)
+
+    def soft(y):
+        return (1.0 - eps) * F.one_hot(y, C).to(dt) + eps / C
+    q = soft(labels) if lam == 1.0 else lam * soft(labels) + (1.0 - lam) * soft(labels.flip(0))
+    lsm = F.log_softmax(z, dim=1)
+    ls_s, ls_t = F.log_softmax(z / T, dim=1), F.log_softmax(t / T, dim=1)
+    p_t = ls_t.exp()
+    rows = (1.0 - a) * -(q * lsm).sum(1) + a * T * T * (p_t * (ls_t - ls_s)).sum(1)
+    ye = labels if lam >= 0.5 else labels.flip(0)
+    err1 = (z.argmax(1) != ye).to(dt).mean()
+    topk = z.topk(min(5, C), dim=1).indices
+    err5 = 1.0 - (topk == ye[:, None]).any(1).to(dt).mean()
+    dlogits = ((1.0 - a) * (lsm.exp() - q) + a * T * (ls_s.exp() - p_t)) / B * grad_scale
+    return rows.mean(), err1, err5, dlogits
+
+
 # --------------------------------------------------------------------------- GAN losses / noise
 def gan_loss(scores, kind, a):
     """Loss over the critic's scores and d loss / d scores.
