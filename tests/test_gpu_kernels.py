@@ -466,47 +466,3 @@ def test_inception_node_matches_composition(dtype):
             assert rel_err(bs[i].grad, br[i].grad) < 2 * tol, i
     finally:
         precision.set_precision(old)
-
-
-@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32])
-def test_rnn_ops_match_reference(dtype):
-    """Embedding gather/scatter, the masked LSTM sequence node (GEMMs on the wgmma kernel + fused cell kernels) and masked
-    mean pooling against the plain-torch fp32 implementation of the same recurrence (the CPU path of ops/rnn.py)."""
-    from theanompi_b200.ops import precision, rnn
-    old = precision.precision()
-    precision.set_precision("tf32" if dtype == torch.float32 else "bf16")
-    try:
-        torch.manual_seed(23)
-        T, B, H, V = 12, 16, 64, 100
-        ids = torch.randint(0, V, (T, B), device=DEV)
-        mask = (torch.rand(T, B, device=DEV) > 0.25).float(); mask[0] = 1
-        Wemb = (torch.randn(V, H, device=DEV) * 0.5).requires_grad_(True)
-        U = (torch.randn(4 * H, H, device=DEV) * 0.2).requires_grad_(True)
-        gx0 = torch.randn(T, B, 4 * H, device=DEV)
-        # GPU (native)
-        e = rnn.embedding(ids, Wemb)
-        gx = (gx0.to(dtype) + torch.cat([e, e, e, e], -1).to(dtype)).detach().requires_grad_(True)
-        h = rnn.lstm_sequence(gx, U, mask)
-        p = rnn.masked_mean(h, mask)
-        w = torch.linspace(-1, 1, H, device=DEV)
-        (p.float() * w).sum().backward()
-        # CPU reference (fp32)
-        Wc, Uc = Wemb.detach().cpu().requires_grad_(True), U.detach().cpu().requires_grad_(True)
-        ec = rnn.embedding(ids.cpu(), Wc)
-        gxc = gx.detach().float().cpu().requires_grad_(True)
-        hc = rnn.lstm_sequence(gxc, Uc, mask.cpu())
-        pc = rnn.masked_mean(hc, mask.cpu())
-        (pc * w.cpu()).sum().backward()
-        tol = 3e-2 if dtype == torch.bfloat16 else 2e-3
-        assert rel_err(e.cpu(), ec) < tol
-        assert rel_err(h.cpu(), hc) < tol and rel_err(p.cpu(), pc) < tol
-        assert rel_err(gx.grad.cpu(), gxc.grad) < 2 * tol
-        assert rel_err(U.grad.cpu(), Uc.grad) < 2 * tol
-        # embedding scatter: gradient of sum(e * r)
-        r = torch.randn(T, B, H, device=DEV)
-        Wemb.grad = None
-        (rnn.embedding(ids, Wemb).float() * r).sum().backward()
-        want = torch.zeros(V, H).index_add_(0, ids.cpu().reshape(-1), r.cpu().reshape(-1, H))
-        assert rel_err(Wemb.grad.cpu(), want) < tol
-    finally:
-        precision.set_precision(old)

@@ -82,6 +82,58 @@ __global__ void embedding_bwd_kernel(const long long* __restrict__ ids, const T*
   for (int d = threadIdx.x; d < D; d += blockDim.x) atomicAdd(dst + d, ldf(dout + row * D + d));
 }
 
+// Deterministic mode: dW[v, :] = ((dout[r0] + dout[r1]) + dout[r2]) + ... over the rows r0 < r1 < ... with ids[r] = v, in
+// ascending row order and without atomics.  CTA k owns the ids [k·EMB_DET_IDS, (k + 1)·EMB_DET_IDS): it walks all rows in chunks
+// of EMB_DET_CHUNK, compacts the chunk's rows that hit its ids into an ordered list (block-wide scan) and then each thread adds
+// its columns of those rows in list order.  A thread keeps the running sum of the current id in a register and writes it back
+// when the id changes, so the padding id's long run costs one fp32 add per row.
+constexpr int EMB_DET_IDS = 64, EMB_DET_THREADS = 256, EMB_DET_PER_THREAD = 4, EMB_DET_CHUNK = EMB_DET_THREADS * EMB_DET_PER_THREAD;
+template <typename T>
+__global__ void __launch_bounds__(EMB_DET_THREADS) embedding_bwd_det_kernel(const long long* __restrict__ ids, const T* __restrict__ dout,
+                                                                            float* __restrict__ dW, int n, int D, long long V) {
+  __shared__ int hit_row[EMB_DET_CHUNK], hit_id[EMB_DET_CHUNK], warp_tot[EMB_DET_THREADS / 32];
+  const long long v0 = (long long)blockIdx.x * EMB_DET_IDS;
+  const int nv = (int)min((long long)EMB_DET_IDS, V - v0);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int base = 0; base < n; base += EMB_DET_CHUNK) {
+    int loc[EMB_DET_PER_THREAD], cnt = 0;
+#pragma unroll
+    for (int j = 0; j < EMB_DET_PER_THREAD; ++j) {
+      const int r = base + threadIdx.x * EMB_DET_PER_THREAD + j;
+      const long long v = r < n ? ids[r] - v0 : -1;
+      loc[j] = (v >= 0 && v < nv) ? (int)v : -1;
+      cnt += loc[j] >= 0;
+    }
+    int incl = cnt;                                   // block-wide exclusive scan of the per-thread hit counts
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const int x = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += x; }
+    if (lane == 31) warp_tot[warp] = incl;
+    __syncthreads();
+    int pos = incl - cnt, total = 0;
+    for (int w = 0; w < EMB_DET_THREADS / 32; ++w) { if (w < warp) pos += warp_tot[w]; total += warp_tot[w]; }
+#pragma unroll
+    for (int j = 0; j < EMB_DET_PER_THREAD; ++j)
+      if (loc[j] >= 0) { hit_row[pos] = base + threadIdx.x * EMB_DET_PER_THREAD + j; hit_id[pos] = loc[j]; ++pos; }
+    __syncthreads();
+    for (int d = threadIdx.x; d < D; d += EMB_DET_THREADS) {
+      int cur = -1;
+      float acc = 0.f;
+      for (int k = 0; k < total; ++k) {
+        const int v = hit_id[k];
+        const float x = ldf(dout + (long long)hit_row[k] * D + d);
+        if (v != cur) {
+          if (cur >= 0) dW[(v0 + cur) * D + d] = acc;
+          cur = v;
+          acc = dW[(v0 + v) * D + d];
+        }
+        acc += x;
+      }
+      if (cur >= 0) dW[(v0 + cur) * D + d] = acc;
+    }
+    __syncthreads();                                  // hit_row / hit_id / warp_tot are rewritten by the next chunk
+  }
+}
+
 // pooled[b, :] = sum_t h[t, b, :] * mask[t, b] / max(1, sum_t mask[t, b])     (h: [T, B, H])
 template <typename T>
 __global__ void masked_mean_fwd_kernel(const T* __restrict__ h, const float* __restrict__ mask, T* __restrict__ out, int Tn, int B, int H) {
@@ -138,6 +190,16 @@ void embedding_fwd(const void* ids, const void* W, void* out, long long n, int D
 void embedding_bwd(const void* ids, const void* dout, void* dW, long long n, int D, long long V, int f32, cudaStream_t st) {
   check_cuda(cudaMemsetAsync(dW, 0, (size_t)V * D * 4, st), "embedding_bwd memset");
   if (n <= 0) return;
+  if (deterministic_mode()) {                       // fixed ascending-row order per id, no float atomics
+    if (n > 0x7fffffffLL) throw std::runtime_error("embedding_bwd: too many rows for the deterministic mode");
+    const unsigned g = (unsigned)((V + EMB_DET_IDS - 1) / EMB_DET_IDS);
+    TMPI_RNN_DISPATCH(
+        (embedding_bwd_det_kernel<float><<<g, EMB_DET_THREADS, 0, st>>>((const long long*)ids, (const float*)dout, (float*)dW, (int)n, D, V)),
+        (embedding_bwd_det_kernel<__nv_bfloat16><<<g, EMB_DET_THREADS, 0, st>>>((const long long*)ids, (const __nv_bfloat16*)dout, (float*)dW,
+                                                                                (int)n, D, V)));
+    count_launch(); TMPI_CHECK_LAUNCH("embedding_bwd"); ::tmpi::check_capture(st, "embedding_bwd");
+    return;
+  }
   TMPI_RNN_DISPATCH((embedding_bwd_kernel<float><<<(unsigned)n, 128, 0, st>>>((const long long*)ids, (const float*)dout, (float*)dW, n, D)),
                     (embedding_bwd_kernel<__nv_bfloat16><<<(unsigned)n, 128, 0, st>>>((const long long*)ids, (const __nv_bfloat16*)dout, (float*)dW, n, D)));
   count_launch(); TMPI_CHECK_LAUNCH("embedding_bwd"); ::tmpi::check_capture(st, "embedding_bwd");
